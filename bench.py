@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the sonar front end (BASELINE.json metric: sonar frames/sec, CFAR + ICP).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--frames F] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--frames F] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload (BASELINE config 4, the configuration the metric is quoted on): a synthetic bag replay --
 F = 4096 polar sonar frames (512 beams x 512 range bins, uint8) per step and per GPU, rendered from a
@@ -16,9 +16,11 @@ iterations, window of 3 previous frames).  One step = one batch through sfe_fron
   cpu_baseline  the CPU oracle (oracle/: reference cfar.cpp compiled unmodified + restated cloud/ICP
           code) on a bounded sample of the same frames, one thread
   --impl reference   the reference arm: that CPU path on all host cores (rank 0 only under torchrun)
+  --dump-outputs DIR  rank 0 writes what the timed path left on the device after its last step (per-frame results and
+          keyframe clouds) as DIR/<name>.npy; the inputs are seeded, so two builds can be compared output for output
 
   config3_icp   BASELINE config 3 (2 000 x 20 000-point scan matches, 20 iterations and the shipped checkers) on
-          rank 0: pairs/s over 8 waves of 148 problems, ms per wave
+          rank 0: pairs/s over 8 waves of one problem per SM (132 on an H100 SXM), ms per wave
   config5   BASELINE config 5: a FIXED backlog of 80 000 such pairs held by rank 0, sharded over the N ranks
           (strong scaling): pair batches leave rank 0 by grouped NCCL send/recv (sonar_slam_b200/dist.py), are
           solved while the next batch arrives, and the 48-byte results come back by NCCL gather; pairs/s with and
@@ -65,28 +67,9 @@ def parse():
     ap.add_argument("--pairs", type=int, default=80000, help="config 5: size of the scan-match backlog (0: skip)")
     ap.add_argument("--pair-steps", type=int, default=2, help="config 5: timed steps (after one warm-up step)")
     ap.add_argument("--pair-chunks", type=int, default=8, help="config 5: pieces per shard in the pipelined scatter")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's results of its last step as DIR/<name>.npy (float32/float64)")
     return ap.parse_args()
-
-
-NCU_SUMMARY = os.path.join("profiles", "r02_ncu_full_summaries.json")
-NCU_KEY = "prof_cfar_u8gate4"
-
-
-def ncu_traffic_per_frame():
-    """(dram read+write bytes per frame, source) of the pipeline's CFAR kernel.  ncu cannot run inside a timed
-    bench (it replays kernels), so this is STATIC: read from this round's committed `ncu --set full` capture of the
-    same kernel on a 4096-frame launch (tools/prof_cfar.py 4096 u8 bits); (None, reason) if that file is absent."""
-    try:
-        with open(os.path.join(REPO, NCU_SUMMARY)) as f:
-            d = json.load(f)[NCU_KEY]
-
-        def gb(v):
-            x, unit = v.split()
-            return float(x) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[unit]
-        return (gb(d["dram__bytes_read.sum"]) + gb(d["dram__bytes_write.sum"])) / 4096.0, \
-            f"static: {NCU_SUMMARY}[{NCU_KEY}] (ncu --set full of the same kernel, 4096-frame launch)"
-    except Exception as e:  # noqa: BLE001
-        return None, f"no committed ncu capture ({type(e).__name__})"
 
 
 def measured_peak():
@@ -94,7 +77,47 @@ def measured_peak():
         with open(os.path.join(REPO, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3), not measured"
+
+
+def gpu_info(idx):
+    """Name and power limit of the card the numbers were measured on (read only)."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(idx), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(idx), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout
+        info["power_limit_w"] = float(out.strip())
+    except Exception:  # noqa: BLE001
+        pass
+    return info
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, ctx, r, n, seed=0):
+    """Write what sfe_frontend_run_dev left on the device (`r` = FrontEnd.results_dev()) for its `n` frames as
+    out_dir/<name>.npy: per-frame T, iterations, inliers, status, cloud_count and the keyframe clouds, concatenated
+    (cloud_points [M,2] float32; cloud_frames / cloud_offsets say which frame each slice belongs to).  Integers are
+    written as float64 (exact).  When all clouds would take the total past DUMP_BYTES, those of a fixed, seeded
+    subset of frames are written."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"T": ctx.to_host(r["T"], (n, 3, 3), np.float32)}
+    for k in ("iterations", "inliers", "status"):
+        out[k] = ctx.to_host(r[k], (n,), np.int32).astype(np.float64)
+    count = ctx.to_host(r["cloud_count"], (n,), np.int32)
+    out["cloud_count"] = count.astype(np.float64)
+    budget = DUMP_BYTES - sum(a.nbytes for a in out.values()) - 8
+    order = np.random.default_rng(seed).permutation(n)
+    frames = np.sort(order[np.cumsum(count[order].astype(np.int64) * 8 + 16) <= budget])
+    xy = ctx.to_host(r["cloud_xy"], (n, r["cloud_stride"], 2), np.float32)
+    out["cloud_frames"] = frames.astype(np.float64)
+    out["cloud_offsets"] = np.concatenate([[0], np.cumsum(count[frames])]).astype(np.float64)
+    out["cloud_points"] = np.concatenate([xy[i, :count[i]] for i in frames] or [np.zeros((0, 2), np.float32)])
+    for k, v in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    return sorted(out)
 
 
 class ClockSampler:
@@ -173,8 +196,8 @@ def parse_cpulist(text):
 def bind_near_gpu(pci_domain, pci_bus, pci_device, sysfs="/sys/bus/pci/devices"):
     """Multi-rank runs: restrict this rank's threads to the CPUs next to its GPU (sysfs local_cpulist of the PCI
     device) BEFORE it allocates pinned host memory, so the pinned frames are first-touched on the GPU's own NUMA
-    node.  Eight ranks pulling 53 GB/s each through whichever socket the scheduler happened to start them on is what
-    made the N = 8 `e2e` swing between 1.31 and 1.59 M frames/s.  Returns a description for the bench line; never
+    node: eight ranks pulling host frames through whichever socket the scheduler happened to start them on make the
+    `e2e` leg swing from run to run.  Returns a description for the bench line; never
     raises (a box without the sysfs entry keeps the scheduler's placement)."""
     try:
         path = os.path.join(sysfs, f"{pci_domain:04x}:{pci_bus:02x}:{pci_device:02x}.0", "local_cpulist")
@@ -366,7 +389,7 @@ def run_ours(args):
 
     # ---- synthetic bag replay for this rank (frames stay resident in HBM; > L2 by far: F*256 KiB).  Every rank replays
     #      the SAME seeded bag: the stages' cost follows the scene (detections, cloud sizes), and with one scene per
-    #      rank the max over ranks measured the unluckiest scene (+7 % at N = 8), not the parallel overhead
+    #      rank the max over ranks would measure the unluckiest scene, not the parallel overhead
     d = synth.make_trajectory_frames(F, seed=0, device=f"cuda:{local}")
     frames_dev, poses = d["frames"], d["poses_odom"]
     fx = FeatureExtraction()
@@ -408,6 +431,7 @@ def run_ours(args):
     barrier()
     dev_ms = max_over_ranks(e0.elapsed_time(e1))
     launches = ctx.launches - l0
+    dumped = dump_outputs(args.dump_outputs, ctx, fe.results_dev(), F) if args.dump_outputs and rank == 0 else None
 
     # ---- end-to-end leg: host buffers in, results out, through one C-ABI call per step
     for _ in range(W):
@@ -459,7 +483,7 @@ def run_ours(args):
                     torch.cuda.synchronize()
                     ts.append(a.elapsed_time(b))
                 ms = float(np.median(ts))
-                cfg3[name] = {"pairs_per_s": P3 / (ms * 1e-3), "ms_per_wave_of_148": ms / 8, "ms": ms,
+                cfg3[name] = {"pairs_per_s": P3 / (ms * 1e-3), "ms_per_wave": ms / 8, "ms": ms,
                               "mean_iterations": float(r3["iterations"].float().mean().item()),
                               "converged": int((r3["status"] == 0).sum().item())}
             del s3, t3, g3
@@ -516,11 +540,11 @@ def run_ours(args):
         cfar_ms, cfar_calls = stage["cfar"]
         cfar_bytes = F * R * B * (1 + 1 / 8)            # uint8 image in, bit plane out, per launch
         achieved = cfar_bytes / (cfar_ms / max(1, cfar_calls) * 1e-3) / 1e9
-        traffic_pf, traffic_src = ncu_traffic_per_frame()
         line = {
             "metric": METRIC, "value": world * F * K / (dev_ms * 1e-3), "unit": "frames/s", "n_gpus": world,
             "steps": K, "warmup": W, "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "f32", "data": "synthetic",
+            "vs_baseline": None, "dtype": "f32", "data": "synthetic", "gpu": gpu_info(local),
+            "dumped_outputs": dumped,
             "config": {"workload": "config4-pipeline: synthetic bag replay, CFAR(SOCA 40/10, Pfa 0.1, gate 65) -> "
                                    "cloud -> voxel 0.5 m -> outlier(1.0 m, 5) -> keyframe cloud (x, -z) -> ICP 20 "
                                    "iterations vs 3-frame submap",
@@ -536,9 +560,7 @@ def run_ours(args):
                     "h2d_bytes_per_step": F * R * B + F * 4 * 9 * 4, "d2h_bytes_per_step": F * (36 + 16)},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "cfar_u8_gate4_kernel<SOCA, bits>", "achieved": achieved,
-                         "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (traffic_pf * F) if traffic_pf else None, "traffic_source": traffic_src,
-                         "peak_source": peak_src, "algorithmic_bytes_per_launch": cfar_bytes,
+                         "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src, "algorithmic_bytes_per_launch": cfar_bytes,
                          "kernel_ms_per_launch": cfar_ms / max(1, cfar_calls),
                          "timing": "CUDA events on the launch stream around the kernel, separate pass after the "
                                    "timed steps (the timed `value` loop carries no stage events)"},
@@ -562,7 +584,7 @@ def run_ours(args):
             by = F * R * B * 5
             ach = by / (float(np.median(ts)) * 1e-3) / 1e9
             line["roofline_config2_cfar_f32"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
-                                                 "frac": ach / peak, "frac_of_8TBps_nominal": ach / 8000.0,
+                                                 "frac": ach / peak,
                                                  "ms_median_of_10": float(np.median(ts)), "frames": F,
                                                  "algorithmic_bytes_per_launch": by,
                                                  "note": "outside the timed pipeline steps; includes the flag memset and "

@@ -1,4 +1,4 @@
-/* libsonarfe -- B200 (sm_100a) sonar front end: CFAR detector, polar->Cartesian
+/* libsonarfe -- H100 (sm_90a) sonar front end: CFAR detector, polar->Cartesian
  * feature cloud, cloud filters, ICP scan matcher.
  *
  * C ABI that replaces the two pybind11 modules of jake3991/sonar-SLAM's
@@ -182,8 +182,8 @@ typedef struct {
                              bit 1: accumulate the sums over points (reference mean, pair means, cross-covariance) in
                                     float64, order-independent.  DEFAULT (bit clear): every such sum is a SEQUENTIAL
                                     float32 sum in point order, the accumulation order of the CPU oracle
-                                    (oracle/icp_ref.c) -- results are bit-identical to it.  The float64 mode is a few
-                                    per cent faster and closer to exact arithmetic, but differs from the float32 chain by
+                                    (oracle/icp_ref.c) -- results are bit-identical to it.  The float64 mode is
+                                    closer to exact arithmetic, but differs from the float32 chain by
                                     up to ~2e-3 m on ill-conditioned scans (tests/test_icp_parity_gpu.py). */
   int minimizer;          /* errorMinimizer: 0 PointToPointErrorMinimizer (shipped, icp.yaml:20)
                              1 PointToPlaneErrorMinimizer force2D (the alternative the YAML keeps commented out,

@@ -1,6 +1,6 @@
 """ctypes binding of libsonarfe.so (the C ABI declared in include/sonarfe.h).
 
-Fails loudly: a missing shared object or a machine without a B200 raises -- there
+Fails loudly: a missing shared object or a machine without an H100 (sm_90) raises -- there
 is no CPU path behind these functions.
 """
 import ctypes

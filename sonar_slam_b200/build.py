@@ -1,9 +1,9 @@
-"""Build libsonarfe.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libsonarfe.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m sonar_slam_b200.build [--force] [--verbose]
 
 The shared object lands next to this file (sonar_slam_b200/libsonarfe.so); it is
-git-ignored but travels to the GPU box with the gpurun snapshot.
+git-ignored.  A rebuild happens whenever the sources, the header or the flags change.
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, "libsonarfe.so")
 STAMP = os.path.join(HERE, "build", "stamp.txt")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
@@ -63,7 +63,7 @@ def build(force=False, verbose=False):
     if verbose:
         print("\n".join(log))
     # hidden visibility + explicit SFE_API exports keep the ABI to what include/sonarfe.h declares
-    subprocess.run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"],
+    subprocess.run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"],
                    check=True)
     with open(STAMP, "w") as f:
         f.write(fp)

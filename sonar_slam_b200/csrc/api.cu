@@ -97,8 +97,8 @@ int sfe_ctx_create(int device, void *cuda_stream, int own_stream, sfe_ctx **out)
   SFE_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   SFE_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("sfe_ctx_create: device %d is sm_%d%d; this library is built for sm_100a (B200) only", device,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("sfe_ctx_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
               prop.major, prop.minor);
     return SFE_ERR_UNSUPPORTED;
   }

@@ -1,4 +1,4 @@
-// CFAR detector kernels (sm_100a).
+// CFAR detector kernels (sm_90a).
 //
 // Replaces bruce_slam/src/bruce_slam/cpp/cfar.cpp:10-192 (ca/soca/goca/os and the
 // "2" variants) for batches of polar sonar frames laid out [frame][range][beam].
@@ -43,7 +43,7 @@ namespace sfe {
 
 constexpr int CF_W = 128;     // beams per strip / consumer threads per CTA
 constexpr int CF_CH = 16;     // range bins per TMA box
-constexpr int CF_NSTAGE = 4;     // input ring depth (stages of CF_CH rows); 2 is 20 % slower, 8 no faster (B200)
+constexpr int CF_NSTAGE = 4;     // input ring depth (stages of CF_CH rows)
 constexpr int CF_NSTAGE_U8 = 4;  // same for the uint8 kernel
 constexpr int CF_RING = 32;   // two 32-deep register rings per thread (cells, window sums)
 constexpr int CF_T = 20;      // train_hs of the streaming path
@@ -505,17 +505,17 @@ __global__ void __launch_bounds__(CF_W, 5)
 //   * after the block each warp compacts its parked (lane, row) pairs into a queue and decides them 32 at a time
 //     against the table M[S] (atomicOr into a zero-initialised bit tile / byte stores into a mask tile): the
 //     cost follows the NUMBER of candidates, not how they are spread over rows and lanes.
-// 15 instructions per row of 4 cells; measured 288 M warp instructions per 4096 replay frames against 537 M for the
-// table kernel (ncu, profiles/).  All-integer, exact: identical to the table
+// 15 instructions per row of 4 cells, about half the warp instructions of the table kernel per frame.  All-integer,
+// exact: identical to the table
 // kernel by construction (the gate test is a necessary condition; the decision is the same table compare).
 // A strip is 512 beams (128 threads x 4); 16-row chunks arrive by TMA as two [16 x 256] boxes per stage.  Block b
 // consumes chunk b (newest cell rn = 16 b + i) and decides cell r = rn - 25, so every block touches ONE tile.
 // The four warps of a CTA only share the tiles: no CTA barrier in the loop (see cfar_block16_g).
 constexpr int CG_BEAMS = 4;
 constexpr int CG_W = CF_W * CG_BEAMS;  // beams per strip
-// Ring depth / occupancy, measured on the replay frames (ms per 4096 frames, bit-plane output): 4 stages with 3
-// CTAs per SM (155 registers) 0.463; 2 stages with 3 CTAs 0.476; 2 stages with 4 CTAs per SM (128 registers,
-// 55 KB of shared memory each) 0.439 -- the kernel is latency-bound, a fourth CTA buys more than a deeper ring.
+// Ring depth / occupancy: 2 stages with 4 CTAs per SM (128 registers, 55 KB of shared memory each) -- the kernel is
+// latency-bound, so a fourth CTA per SM buys more than a deeper ring (chosen on replay frames; not re-measured on
+// H100).
 #ifndef SFE_CG_NS
 #define SFE_CG_NS 2    // input ring depth (stages of 16 rows x 512 beams)
 #endif

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libsonarfe (sm_100a only).
+// Shared device/host helpers for libsonarfe (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -45,7 +45,7 @@ struct sfe_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool owns_stream = false;
-  int sm_count = 148;
+  int sm_count = 0;
   int max_smem_optin = 0;
   sfe::Buffer scratch[8];   // per-subsystem scratch (see SCR_* below)
   sfe::Buffer stage_in[2];  // device staging for the *_host entry points

@@ -1,4 +1,4 @@
-// Polar -> Cartesian feature cloud (sm_100a).
+// Polar -> Cartesian feature cloud (sm_90a).
 //
 // Replaces the numeric body of FeatureExtraction.callback between the CFAR detector and the
 // point-cloud filters, bruce_slam/src/bruce_slam/feature_extraction.py:231-238:

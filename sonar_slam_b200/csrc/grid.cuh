@@ -486,8 +486,7 @@ __device__ __forceinline__ NNResult nn_query_seeded(const GridView &g, float qx,
 // IEEE operation in the oracle's order, so the normals are bit-identical to the oracle's.
 // The running best-knn list is the caller's: bd[j * stride], bi[j * stride], j < knn.  The scan matcher hands out
 // shared memory that is idle while the normals are computed (stride = CTA size, one column per thread): a list in
-// local memory spills past the little L1 that a CTA's shared-memory carve-out leaves (config 3: 1.15 -> 0.79 ms per
-// wave for the normals), so local arrays (stride 1) are only the fallback for CTAs without that room.
+// local memory spills past the little L1 that a CTA's shared-memory carve-out leaves, so local arrays (stride 1) are only the fallback for CTAs without that room.
 constexpr int GRID_KNN_MAX = 16;
 __device__ inline float2 grid_surface_normal(const GridView &g, int p, int knn, float *bd, uint16_t *bi, int stride) {
   const float2 q = g.pts[p];

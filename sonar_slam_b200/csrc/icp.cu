@@ -1,4 +1,4 @@
-// ICP scan matcher and nearest-neighbour matcher (sm_100a).
+// ICP scan matcher and nearest-neighbour matcher (sm_90a).
 //
 // Replaces bruce_slam.pcl.ICP.compute and bruce_slam.pcl.match
 // (bruce_slam/src/bruce_slam/cpp/pcl.cpp:161-174,185-212), i.e. libpointmatcher's
@@ -66,7 +66,7 @@ struct IcpBatch {
   int slot_by_smid;   // workspace slot = %smid (one CTA per SM, one CTA per problem) instead of blockIdx.x
 };
 
-constexpr int ICP_SM_SLOTS = 256;  // >= %nsmid on every sm_100 part
+constexpr int ICP_SM_SLOTS = 256;  // >= %nsmid on every sm_90 part
 __device__ __forceinline__ unsigned icp_smid() {
   unsigned r;
   asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
@@ -430,7 +430,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
   const int smooth = min(prm.smooth_length, ICP_HIST - 1);
   // Default: every sum over points is a sequential float32 sum in point order, as in oracle/icp_ref.c -- results
   // are bit-identical to the oracle.  flags bit 1: float32 terms accumulated in float64 (order-independent,
-  // ~1e-4 closer to exact arithmetic, a few per cent faster; deviates from the oracle by up to ~2e-3 m on
+  // ~1e-4 closer to exact arithmetic; deviates from the oracle by up to ~2e-3 m on
   // ill-conditioned scans because the float32-sequential sums themselves are that noisy).
   const bool seq = (prm.flags & 2) == 0;
 
@@ -634,7 +634,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       // while the distance to the old match is below it, the old match is the unique nearest neighbour -- the
       // answer an exhaustive search would give, ties impossible -- and costs one distance instead of a search.
       // Used for the small problems of the front end (window submaps thinned to 0.5 m: runner-ups are decimetres
-      // away and a certificate lasts several iterations; ICP stage 2.53 -> 2.36 ms per 4096 frames).
+      // away and a certificate lasts several iterations).
       float Tp[9];
 #pragma unroll
       for (int i = 0; i < 9; ++i) Tp[i] = sh.Tprev[i];
@@ -742,7 +742,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
         int exact;
         const int seed = prev[i];
         // (no certificates here: a 20 000-point target puts the runner-up a centimetre from the match, so a
-        // certificate rarely outlives an iteration -- measured 2.32 -> 2.59 ms per wave with them)
+        // certificate rarely outlives an iteration, and checking it costs more than it saves)
         const float2 ts = sorted[seed != 0xffff ? seed : 0];
         if (seed != 0xffff && dist2_rn(q.x - ts.x, q.y - ts.y) <= stop_a) {
           r = nn_query_seeded(g, q.x, q.y, max_d2, seed);  // last iteration's match is still close: settle it now
@@ -1238,8 +1238,8 @@ int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const
   b.prm = *prm;
   {
     // One-pass exact path (per-lane searches with certified matches, no pruning passes) for problems of up to
-    // 5 source points per thread: measured on the config-4 replay (sources of ~360 points, 128-thread CTAs), ICP
-    // stage per 4096 frames 2.54 ms with a limit of 2 points per thread, 2.23 with 3, 1.82 with 5.
+    // 5 source points per thread (chosen on the config-4 replay, sources of ~360 points in 128-thread CTAs: a lower
+    // limit sends more problems down the slower pruned path; not re-measured on H100).
     static const int mult = [] {  // development switch: SFE_ICP_SMALL_MULT
       const char *e = getenv("SFE_ICP_SMALL_MULT");
       return e ? atoi(e) : 5;
@@ -1268,7 +1268,7 @@ int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const
     return SFE_ERR_UNSUPPORTED;
   }
   // CTA size follows the source size (one NN query per thread and iteration is the sweet spot)
-  // (measured on the config-4 replay: 256 threads beat 128 and 512 for ~360-point sources)
+  // (chosen on the config-4 replay for ~360-point sources; not re-measured on H100)
   const int threads = force_threads > 0 ? force_threads : (b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS));
   SFE_REQUIRE(threads == 128 || threads == 256 || threads == 512, "icp: CTA size must be 128, 256 or 512 (got %d)", threads);
   // instantiation: (threads, register budget).  512-thread CTAs whose shared memory allows only one per SM get the

@@ -33,17 +33,16 @@ int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const
             int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
             int class_ns = 0, int class_nt = 0, int force_threads = 0);
 
-// Size class of the first ICP launch (fe_match).  Measured on the config-4 replay (filtered clouds: median 326,
-// max 639 points; window submaps <= 1808 raw points): one launch sized for the capacities (1024 / 3072, 4 CTAs per
-// SM) 2.40 ms per 4096 frames with 256 threads, 2.59 ms with 128; this class with 128 threads (6 CTAs per SM) 2.11 ms;
-// a class that leaves 14 % of the frames to the second launch (512 points) 3.11 ms -- the tail of a nearly empty
-// launch costs a full problem latency.
+// Size class of the first ICP launch (fe_match), chosen on the config-4 replay (filtered clouds: median 326,
+// max 639 points; window submaps <= 1808 raw points; not re-measured on H100): this class with 128 threads (6 CTAs
+// per SM) beat one launch sized for the capacities (1024 / 3072, 4 CTAs per SM), and a smaller class that leaves
+// frames to the second launch loses -- the tail of a nearly empty launch costs a full problem latency.
 constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 1536, FE_ICP_SMALL_THREADS = 128;
 // Size classes of the cloud filters (cloud.cu: two launches by cloud size).  Config-4 replay: 3-5 k raw Cartesian
 // points per frame, ~580 after the voxel filter, ~400 after the outlier filter, window submaps <= 1.8 k raw points.
-// Measured (ms per 4096 frames): outlier filter 0.145 -> 0.113 and submap down-sampling 0.241 -> 0.215 with a
-// small-cloud class; the per-frame down-sampling is best left as one launch (0.79; 0.90 / 0.87 with a class
-// boundary at 4608 / 5632 points: too many frames land in the second, poorly filled launch).
+// The outlier filter and the submap down-sampling gain from a small-cloud class; the per-frame down-sampling is best
+// left as one launch (with a class boundary at 4608 or 5632 points too many frames land in the second, poorly
+// filled launch).  Chosen on the replay; not re-measured on H100.
 constexpr int FE_DS_SPLIT = 0, FE_RO_SPLIT = 1024, FE_SUBMAP_SPLIT = 2048;
 
 // T_ab = pose_a^-1 * pose_b as float32 3x3 (gtsam Pose2::between, then matrix().astype(float32)).

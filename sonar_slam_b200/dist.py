@@ -208,7 +208,7 @@ def run_pair_backlog(P, ns, nt, prm, src_all=None, tgt_all=None, guess_all=None,
         return local
     compute = torch.cuda.current_stream() if cuda else None
     # the pieces are solved on two alternating streams: a piece is one launch of one CTA per problem, and its last,
-    # partly filled wave of CTAs would otherwise idle most SMs once per piece (8 pieces: ~10 ms of a 145 ms shard).
+    # partly filled wave of CTAs would otherwise idle most SMs once per piece.
     # (the side streams are created once per device and reused: libsonarfe contexts are cached per stream)
     comm, solve = _side_streams(torch.cuda.current_device()) if cuda else (None, [None, None])
     if cuda:
@@ -241,9 +241,8 @@ def run_pair_backlog(P, ns, nt, prm, src_all=None, tgt_all=None, guess_all=None,
     else:
         # The whole shard is received into its final place (memory is not the constraint: 176 KB per pair), every
         # piece as its own grouped recv posted up front on the communication stream: the sender never waits for a
-        # buffer to free up -- a send kernel parked on the sender's SMs until the receiver's solver drains costs
-        # the sender a tenth of its throughput (measured: 703 ms instead of 599 ms per 80 k pairs at N = 2) --
-        # and the solver starts on piece c as soon as piece c is there.
+        # buffer to free up -- a send kernel parked on the sender's SMs until the receiver's solver drains slows
+        # the sender down -- and the solver starts on piece c as soon as piece c is there.
         n_loc = e - s
         sb = torch.empty((n_loc, ns, 2), dtype=torch.float32, device=device)
         tb = torch.empty((n_loc, nt, 2), dtype=torch.float32, device=device)

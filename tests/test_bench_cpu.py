@@ -105,3 +105,49 @@ def test_rank_binding_near_its_gpu(tmp_path):
             assert r["bound"] and r["cpus"] == 1 and os.sched_getaffinity(0) == {one}
     finally:
         os.sched_setaffinity(0, before)
+
+
+def test_dump_outputs_writes_float_arrays_within_the_budget(tmp_path, monkeypatch):
+    """--dump-outputs: every array is float32 / float64 and integers survive exactly; when all clouds would pass the
+    byte budget, those of a fixed, seeded subset of frames are written, the same subset on every run."""
+    import os
+    import numpy as np
+    import bench
+    rng = np.random.default_rng(3)
+    n, stride = 64, 100
+    dev = {"T": rng.random((n, 3, 3), dtype=np.float32), "iterations": rng.integers(0, 40, n, dtype=np.int32),
+           "inliers": rng.integers(0, 500, n, dtype=np.int32), "status": rng.integers(0, 8, n, dtype=np.int32),
+           "cloud_count": rng.integers(0, stride, n, dtype=np.int32),
+           "cloud_xy": rng.random((n, stride, 2), dtype=np.float32)}
+    names = list(dev)
+
+    class FakeCtx:
+        def to_host(self, p, shape, dtype):
+            a = dev[names[p]]
+            assert a.dtype == dtype
+            return a.reshape(shape).copy()
+
+    r = dict({k: i for i, k in enumerate(names)}, cloud_stride=stride)
+
+    def load(d):
+        return {f[:-4]: np.load(d / f) for f in sorted(os.listdir(d))}
+
+    bench.dump_outputs(str(tmp_path / "all"), FakeCtx(), r, n)
+    a = load(tmp_path / "all")
+    assert all(v.dtype in (np.float32, np.float64) for v in a.values())
+    assert np.array_equal(a["status"], dev["status"]) and np.array_equal(a["T"], dev["T"])
+    assert np.array_equal(a["cloud_frames"], np.arange(n))
+    want = np.concatenate([dev["cloud_xy"][i, :dev["cloud_count"][i]] for i in range(n)])
+    assert np.array_equal(a["cloud_points"], want)
+
+    monkeypatch.setattr(bench, "DUMP_BYTES", 20000)
+    for tag in ("s1", "s2"):
+        bench.dump_outputs(str(tmp_path / tag), FakeCtx(), r, n)
+    s1, s2 = load(tmp_path / "s1"), load(tmp_path / "s2")
+    assert sum(v.nbytes for v in s1.values()) <= 20000
+    assert all(np.array_equal(s1[k], s2[k]) for k in s1)
+    fr = s1["cloud_frames"].astype(int)
+    assert 0 < len(fr) < n and np.all(np.diff(fr) > 0)
+    off = s1["cloud_offsets"].astype(int)
+    for j, i in enumerate(fr):
+        assert np.array_equal(s1["cloud_points"][off[j]:off[j + 1]], dev["cloud_xy"][i, :dev["cloud_count"][i]])

@@ -1,4 +1,4 @@
-"""B200: global-initialisation cost (include/sonarfe.h sfe_costmap_*; reference slam.py:461-570, 683-701) against
+"""GPU: global-initialisation cost (include/sonarfe.h sfe_costmap_*; reference slam.py:461-570, 683-701) against
 the reference-generated fixture and the CPU oracle, through the C ABI."""
 import os
 

@@ -11,8 +11,7 @@ what an unpinned stage can offer):
     the worst of 200 scans, 1e-5 m on the median one.
 
 200 BASELINE-config-3 pairs (2 000 x 20 000 points, identity guess) x {fixed 20 iterations, shipped checkers} and
-200 pipeline-sized problems (~350 x ~1 100 points, odometry-like guesses).  The deviation histograms are printed and
-written to gpurun_out/icp_parity_sweep.json (copied to profiles/ by the round's evidence pass)."""
+200 pipeline-sized problems (~350 x ~1 100 points, odometry-like guesses).  The deviation histograms are printed."""
 import json
 import os
 
@@ -125,25 +124,16 @@ def _sweep(name, pairs, guesses, kw, fixed_iters):
     return rep
 
 
-@pytest.fixture(scope="module")
-def sweep_log():
-    log = {}
-    yield log
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/icp_parity_sweep.json", "w") as f:
-        json.dump(log, f, indent=1)
-
-
 @pytest.mark.parametrize("mode", ["fixed20", "checkers"])
-def test_config3_sweep(gpu_ctx, mode, sweep_log):
+def test_config3_sweep(gpu_ctx, mode):
     kw = dict(smooth_length=0, max_iterations=20) if mode == "fixed20" else {}
     pairs = [synth.make_icp_pair(s)[:2] for s in range(N_SWEEP)]
     guesses = [np.eye(3)] * len(pairs)
-    sweep_log["config3_" + mode] = _sweep("config3_" + mode, pairs, guesses, kw, 20 if mode == "fixed20" else 0)
+    _sweep("config3_" + mode, pairs, guesses, kw, 20 if mode == "fixed20" else 0)
 
 
 @pytest.mark.parametrize("mode", ["fixed20", "checkers"])
-def test_pipeline_sized_sweep(gpu_ctx, mode, sweep_log):
+def test_pipeline_sized_sweep(gpu_ctx, mode):
     kw = dict(smooth_length=0, max_iterations=20) if mode == "fixed20" else {}
     rng = np.random.default_rng(77)
     pairs, guesses = [], []
@@ -153,4 +143,4 @@ def test_pipeline_sized_sweep(gpu_ctx, mode, sweep_log):
         pairs.append((src, tgt))
         # odometry-like guess: the ground truth disturbed by the odometry noise of a step
         guesses.append(Tgt @ synth.se2(*rng.normal(0, [0.1, 0.1, 0.01])))
-    sweep_log["pipeline_" + mode] = _sweep("pipeline_" + mode, pairs, guesses, kw, 20 if mode == "fixed20" else 0)
+    _sweep("pipeline_" + mode, pairs, guesses, kw, 20 if mode == "fixed20" else 0)

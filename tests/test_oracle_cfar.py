@@ -1,11 +1,12 @@
 """CPU-only: pin the CFAR oracle (oracle/cfar_ref.c) against the reference.
 
- * against oracle/_ref/libcfar_ref.so = the UNMODIFIED reference cfar.cpp compiled from
-   /root/reference (present in the dev container and, as a prebuilt file, on the GPU box);
+ * against tests/golden/cfar_reference.json, digests of the output of the UNMODIFIED reference cfar.cpp
+   (oracle/_ref/libcfar_ref.so) on the inputs below (tools/make_golden.py --only-cfar-reference);
  * against tests/golden/cfar_masks.npz, produced by running the reference's own CFAR class
    (tools/make_golden.py).
 """
 import hashlib
+import json
 
 import numpy as np
 import pytest
@@ -26,17 +27,36 @@ def _inputs():
     yield "negative_and_big", (rng.normal(0, 1e6, (80, 17))).astype(np.float32), 6, 1, 11
 
 
-@pytest.mark.skipif(not orc.have_reference(), reason="oracle/_ref not built (needs /root/reference once)")
-@pytest.mark.parametrize("alg", ALGS)
-def test_port_equals_unmodified_reference(alg):
+def cases(alg):
     for name, img, T, G, k in _inputs():
         for tau in (TAU[alg], 0.37):
-            m0, t0 = orc.cfar_reference(alg, img, T, G, k, tau, want_thr=True)
-            m1, t1 = orc.cfar(alg, img, T, G, k, tau, want_thr=True)
-            assert np.array_equal(m0, m1), (name, alg)
-            assert np.array_equal(t0.view(np.uint32), t1.view(np.uint32)), (name, alg)  # bit-exact thresholds
-            m2, _ = orc.cfar_reference(alg, img, T, G, k, tau, want_thr=False)
-            assert np.array_equal(m0, m2)
+            yield name, img, T, G, k, tau
+
+
+def digests(masks, thrs):
+    """Detection count of every case, one sha256 over all masks and one over all threshold images."""
+    h = [hashlib.sha256(), hashlib.sha256()]
+    for m, t in zip(masks, thrs):
+        h[0].update(np.ascontiguousarray(m).tobytes())
+        h[1].update(np.ascontiguousarray(t).tobytes())
+    return {"mask_counts": [int(m.sum()) for m in masks], "mask_sha256": h[0].hexdigest(),
+            "thr_sha256": h[1].hexdigest()}
+
+
+@pytest.mark.parametrize("alg", ALGS)
+def test_port_equals_unmodified_reference(alg, golden_dir):
+    with open(f"{golden_dir}/cfar_reference.json") as f:
+        want = json.load(f)[alg]
+    masks, thrs, masks_no_thr = [], [], []
+    for name, img, T, G, k, tau in cases(alg):
+        m, t = orc.cfar(alg, img, T, G, k, tau, want_thr=True)
+        masks.append(m), thrs.append(t)
+        masks_no_thr.append(orc.cfar(alg, img, T, G, k, tau, want_thr=False)[0])
+    got = digests(masks, thrs)
+    assert got["mask_counts"] == want["mask_counts"]
+    assert got["mask_sha256"] == want["mask_sha256"]
+    assert got["thr_sha256"] == want["thr_sha256"]  # bit-exact thresholds
+    assert digests(masks_no_thr, thrs)["mask_sha256"] == want["mask_sha256"]
 
 
 @pytest.mark.parametrize("alg", ALGS)

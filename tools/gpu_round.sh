@@ -21,7 +21,7 @@ for s in $steps; do
     stage_sweep) for v in 0 4800 5056; do echo "SFE_FE_DS_SPLIT=$v"; SFE_FE_DS_SPLIT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
     icp_sweep) for v in 2 3 5; do echo "SFE_ICP_SMALL_MULT=$v"; SFE_ICP_SMALL_MULT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
     margin_sweep) for v in 2 4 6 10 16 32; do echo "SFE_ICP_MARGIN_MULT=$v"; SFE_ICP_MARGIN_MULT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
-    icp_variants) for so in sonar_slam_b200/libsonarfe.so scratch/lib_*.so; do echo "== $so"; SFE_LIB_PATH=$PWD/$so timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 5 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3), round(d['config3_icp']['fixed20']['ms_per_wave_of_148'],3))"; done ;;
+    icp_variants) for so in sonar_slam_b200/libsonarfe.so scratch/lib_*.so; do echo "== $so"; SFE_LIB_PATH=$PWD/$so timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 5 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3), round(d['config3_icp']['fixed20']['ms_per_wave'],3))"; done ;;
     cfar_variants) for so in scratch/lib_*.so; do echo "== $so"; SFE_LIB_PATH=$PWD/$so timeout 300 python tools/bench_cfar.py 4096 replay 2>&1 | grep -E "u8_SOCA_bits|u8_SOCA_mask " | cut -c1-120; done ;;
     bench_ref) timeout 900 python bench.py --impl reference --steps 3 --warmup 1 > gpurun_out/${tag}_bench_ref.json 2> gpurun_out/${tag}_bench_ref.err; cat gpurun_out/${tag}_bench_ref.json ;;
     ncu_list) timeout 900 ncu --metrics gpu__time_duration.sum --clock-control none -k regex:"cfar|cart_|downsample|outlier|assemble|icp_|fill_off|match_|flip_|feat" -c 400 --csv \

@@ -1,5 +1,5 @@
 """Where the point-to-plane mode spends its time: ms per launch by iteration count, both minimisers, for the
-config-3 size (148 problems, one wave) and the front end's size (4096 problems of ~360 x ~1000 points)."""
+config-3 size (one problem per SM: one wave) and the front end's size (4096 problems of ~360 x ~1000 points)."""
 import numpy as np, torch
 from sonar_slam_b200 import _lib, ops, synth
 
@@ -25,7 +25,8 @@ small, gsm = [], []
 for s in range(64):
     a, b, T = synth.make_icp_pair(5000 + s, n_source=int(rng.integers(300, 420)), n_target=int(rng.integers(900, 1100)))
     small.append((a, b)); gsm.append(T @ synth.se2(*rng.normal(0, [0.1, 0.1, 0.01])))
-for name, pairs, P, ns, nt, g in (("2k/20k x148", big, 148, 2000, 20000, None), ("360/1000 x4096", small, 4096, 640, 1100, gsm)):
+SMS = torch.cuda.get_device_properties(0).multi_processor_count
+for name, pairs, P, ns, nt, g in ((f"2k/20k x{SMS}", big, SMS, 2000, 20000, None), ("360/1000 x4096", small, 4096, 640, 1100, gsm)):
     a = pack(pairs, P)
     gs = torch.eye(3, device="cuda").repeat(P, 1, 1).contiguous() if g is None else \
         torch.from_numpy(np.stack([g[i % len(g)] for i in range(P)]).astype(np.float32)).cuda()

@@ -1,6 +1,6 @@
 import numpy as np, torch
 from sonar_slam_b200 import _lib, ops, synth
-P = 148
+P = torch.cuda.get_device_properties(0).multi_processor_count  # one wave: one problem per SM
 pairs = [synth.make_icp_pair(s)[:2] for s in range(4)]
 def pack(ns=None, nt=None):
     src = np.concatenate([pairs[i % 4][0][:ns] for i in range(P)]); tgt = np.concatenate([pairs[i % 4][1][:nt] for i in range(P)])

@@ -1,6 +1,6 @@
 """Per-kernel totals of an `ncu --metrics gpu__time_duration.sum --csv` launch list:
 
-    python tools/launch_summary.py gpurun_out/launches.csv profiles/r01_launch_list_summary.csv [first_id [last_id]]
+    python tools/launch_summary.py launches.csv launch_summary.csv [first_id [last_id]]
 
 Only launches with first_id <= ID <= last_id are counted (e.g. the steps with frames resident in HBM, leaving out
 the chunked host-buffer runs that follow in the same bench.py process)."""

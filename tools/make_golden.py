@@ -27,6 +27,9 @@ Fixtures written:
                                     (:325-387) run unmodified, with bruce_slam.pcl.{downsample,match}
                                     served by the CPU oracle and ICP.compute returning preset
                                     transforms (the natives themselves are covered elsewhere)
+  tests/golden/cfar_reference.json  per-algorithm mask / threshold-image digests and detection counts of the
+                                    unmodified cfar.cpp (oracle/_ref) on the inputs of
+                                    tests/test_oracle_cfar.py (--only-cfar-reference)
   tests/golden/globalinit.npz       SLAM.get_matching_cost_subroutine1 (slam.py:461-570) run
                                     unmodified on a synthetic source/target pair: the dilated
                                     target grid (packed) and the cost of 96 candidate poses.
@@ -350,9 +353,36 @@ def fov_fixture():
     print("fov_select:", len(target_points), "targets ->", int(ns["sel"].sum()), "kept; written to", out)
 
 
+def cfar_reference_fixture():
+    """tests/golden/cfar_reference.json: the unmodified reference cfar.cpp (oracle/_ref/libcfar_ref.so, built by
+    oracle/Makefile) on the seeded inputs of tests/test_oracle_cfar.py, both entry points (with and without the
+    threshold image).  Per algorithm: the detection count of every case and one sha256 over the bytes of all its
+    masks, one over all its threshold images (cases in the order of tests/test_oracle_cfar.py:cases)."""
+    from oracle import oracle as orc
+    sys.path.insert(0, os.path.join(REPO, "tests"))
+    import test_oracle_cfar as t
+    assert orc.have_reference(), "oracle/_ref/libcfar_ref.so is not built"
+    g = {}
+    for alg in t.ALGS:
+        masks, thrs = [], []
+        for name, img, T, G, k, tau in t.cases(alg):
+            m, thr = orc.cfar_reference(alg, img, T, G, k, tau, want_thr=True)
+            m2, _ = orc.cfar_reference(alg, img, T, G, k, tau, want_thr=False)
+            assert np.array_equal(m, m2), (name, alg, tau)
+            masks.append(m), thrs.append(thr)
+        g[alg] = t.digests(masks, thrs)
+    out = os.path.join(REPO, "tests", "golden", "cfar_reference.json")
+    with open(out, "w") as f:
+        json.dump(g, f, indent=1)
+    print("cfar_reference:", {a: len(v["mask_counts"]) for a, v in g.items()}, "cases written to", out)
+
+
 if __name__ == "__main__":
     if "--only-fov" in sys.argv:
         fov_fixture()
+    elif "--only-cfar-reference" in sys.argv:
+        cfar_reference_fixture()
     else:
         main()
         fov_fixture()
+        cfar_reference_fixture()

@@ -4,7 +4,7 @@
 
 ncu's CSV export of the source page is per SASS instruction; this joins it with nvdisasm's line table of the same
 cubin (the build must be the profiled one) and prints, per source line, the share of warp-stall samples and of
-executed warp instructions, and the mean number of active threads -- the table profiles/*.txt quote."""
+executed warp instructions, and the mean number of active threads."""
 import csv
 import os
 import re

@@ -1,10 +1,9 @@
-"""Condense `ncu --set full` reports into the JSON kept under profiles/ (run where ncu is installed):
+"""Condense `ncu --set full` reports into one JSON file (run where ncu is installed):
 
-    python tools/ncu_summary.py profiles/r02_ncu_full_summaries.json name=path.ncu-rep[@kernel-substring] [...]
+    python tools/ncu_summary.py summaries.json name=path.ncu-rep[@kernel-substring] [...]
 
 One entry per report (its first kernel): launch shape, duration, DRAM bytes, issue utilisation, divergence and the
-warp-stall reasons per issued instruction -- the numbers DESIGN.md / profiles/README.md quote and bench.py's
-roofline.traffic reads."""
+warp-stall reasons per issued instruction."""
 import csv
 import json
 import subprocess

@@ -2,7 +2,7 @@
 import sys
 import numpy as np, torch
 from sonar_slam_b200 import _lib, ops, synth
-P = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+P = int(sys.argv[1]) if len(sys.argv) > 1 else torch.cuda.get_device_properties(0).multi_processor_count
 pairs = [synth.make_icp_pair(s)[:2] for s in range(4)]
 src = np.concatenate([pairs[i % 4][0] for i in range(P)]); tgt = np.concatenate([pairs[i % 4][1] for i in range(P)])
 so = np.zeros(P + 1, np.int32); so[1:] = np.cumsum([len(pairs[i % 4][0]) for i in range(P)])

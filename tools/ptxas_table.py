@@ -2,7 +2,7 @@
 (sonar_slam_b200/build/ptxas.log, written by sonar_slam_b200/build.py): registers, spills, stack, static shared
 memory, barriers.  No GPU needed.
 
-    python tools/ptxas_table.py [> profiles/r02_ptxas_resources.txt]
+    python tools/ptxas_table.py
 """
 import os
 import re
@@ -59,8 +59,8 @@ def main():
             cur["smem"] = int(s.group(1)) if s else 0
             cur = None
     names = [short(n) for n in demangle([r["name"] for r in rows])]
-    print("# ptxas -v of the build that produced sonar_slam_b200/libsonarfe.so (nvcc -gencode arch=compute_100a,"
-          "code=sm_100a -O3 -lineinfo); static shared memory only -- dynamic shared memory is chosen at launch")
+    print("# ptxas -v of the build that produced sonar_slam_b200/libsonarfe.so (nvcc -gencode arch=compute_90a,"
+          "code=sm_90a -O3 -lineinfo); static shared memory only -- dynamic shared memory is chosen at launch")
     print(f"# {len(rows)} entry functions, {sum(1 for r in rows if r['spill_st'] or r['spill_ld'])} with register spills")
     print(f"{'kernel':<78} {'regs':>4} {'spill st/ld B':>13} {'stack B':>7} {'smem B':>7} {'bar':>3}")
     for r, n in sorted(zip(rows, names), key=lambda t: t[1]):
