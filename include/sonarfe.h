@@ -224,6 +224,47 @@ SFE_API int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *sr
 SFE_API int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host,
                          int nt, const float *guess_host, int n_guesses, float *T_host, int32_t *iters_host,
                          int32_t *inliers_host, int32_t *status_host);
+/* Host-buffer flavour of sfe_icp_dev: packed clouds with CSR offsets (src_off [n_src_clouds + 1], tgt_off
+ * [n_tgt_clouds + 1]) and per-problem src_id / tgt_id, all in host memory, so that the guesses of many loop-closure
+ * candidates (each its own cloud pair) go out in one launch.  ns_max / nt_max are taken from the offsets. */
+SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host,
+                               const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
+                               const int32_t *tgt_off_host, int n_tgt_clouds, const int32_t *src_id_host,
+                               const int32_t *tgt_id_host, int n_problems, const float *guess_host, float *T_host,
+                               int32_t *iters_host, int32_t *inliers_host, int32_t *status_host);
+
+/* ------------------------------------------------------------------ robust covariance of ICP samples (row N1)
+ * SLAM.compute_icp_with_cov, slam.py:365-371: MinCovDet(store_precision=False, support_fraction=0.8).fit(samples),
+ * batched over n_problems candidates.  The algorithm is scikit-learn 1.9's (sklearn/covariance/_robust_covariance.py:
+ * fast_mcd for n_samples <= 500, then MinCovDet.correct_covariance and reweight_covariance); releases before the
+ * _consistency_factor correction reweight differently and are not what this computes.  See csrc/mcd.cu.
+ *   samples      double [P][32][3], rows 0 .. n[p]-1 used (x, y, theta)
+ *   n            int32 [P]; n > 32 is SFE_ERR_UNSUPPORTED (host flavour) or status SFE_MCD_UNSUPPORTED (device)
+ *   subsets      int8 [P][30][32]: the 30 random trial supports, first h = int(0.8 n) entries used -- what
+ *                np.random.permutation(n)[:h] gives for each of sklearn's 30 trials, in order
+ *   c_support_host  double [33], ALWAYS host memory: entry n = _consistency_factor(3, int(0.8 n) / n)
+ *   c_reweight   _consistency_factor(3, 0.975);  chi2_cut = chi2(3).isf(0.025)  (computed by the caller with scipy)
+ *   flags        SFE_MCD_FLOAT32: the samples are float32 values and numpy's float32 arithmetic applies where
+ *                sklearn keeps that dtype (the location mean, X - location); compute_icp_with_cov's samples are float32
+ * Outputs per problem: location [3] and covariance [3][3] as MinCovDet leaves location_ / covariance_ (NaN unless
+ * status is SFE_MCD_OK), raw_support / support as bit masks (bit i = sample i), status SFE_MCD_*. */
+enum { SFE_MCD_TRIALS = 30, SFE_MCD_MAX_SAMPLES = 32, SFE_MCD_FLOAT32 = 1 };
+enum {
+  SFE_MCD_OK = 0,
+  SFE_MCD_TOO_FEW = 1,     /* n < 5: "Too few samples for covariance computation" (slam.py:361-363) */
+  SFE_MCD_ZERO_COV = 2,    /* correct_covariance's ValueError: "Failed to calculate covariance" (slam.py:365-371) */
+  SFE_MCD_UNSUPPORTED = 3, /* n > 32 */
+  SFE_MCD_BAD_SUBSET = 4   /* a trial support does not name h distinct rows below n */
+};
+SFE_API int sfe_mincovdet_dev(sfe_ctx *ctx, const double *samples_dev, const int32_t *n_dev, const int8_t *subsets_dev,
+                              int n_problems, const double *c_support_host, double c_reweight, double chi2_cut,
+                              int flags, double *location_dev, double *covariance_dev, uint32_t *raw_support_dev,
+                              uint32_t *support_dev, int32_t *status_dev);
+SFE_API int sfe_mincovdet_host(sfe_ctx *ctx, const double *samples_host, const int32_t *n_host,
+                               const int8_t *subsets_host, int n_problems, const double *c_support_host,
+                               double c_reweight, double chi2_cut, int flags, double *location_host,
+                               double *covariance_host, uint32_t *raw_support_host, uint32_t *support_host,
+                               int32_t *status_host);
 
 /* ------------------------------------------------------------------ batched per-keyframe front end
  * One call for a backlog of frames: FeatureExtraction.callback (feature_extraction.py:196-252)

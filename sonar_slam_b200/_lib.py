@@ -106,6 +106,12 @@ _EXTRA_SIGNATURES = {
     "sfe_fov_select_host": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
     "sfe_icp_host": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                      c_void_p, c_void_p],
+    "sfe_icp_batch_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                           c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_mincovdet_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
+                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_mincovdet_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
+                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
 }
 
 

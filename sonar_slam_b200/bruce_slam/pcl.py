@@ -201,5 +201,49 @@ class ICP(object):
                 raise RuntimeError(m)
         return dict(messages=msgs, T=T, iterations=iters, inliers=inl, status=st)
 
+    def compute_pairs(self, sources, targets, guesses):
+        """Many cloud pairs, each with its own guesses, in ONE launch (sfe_icp_batch_host): pair k aligns sources[k]
+        to targets[k] from every 3x3 in guesses[k].  Returns a list with compute_batch's dict for every pair."""
+        if self.params is None:
+            raise RuntimeError("You must setup a matcher before running ICP")
+        srcs = [_points(s, "source", cols=(2,)) for s in sources]
+        tgts = [_points(t, "target", cols=(2,)) for t in targets]
+        gs = [np.asarray(g, dtype=np.float32).reshape(-1, 3, 3) for g in guesses]
+        if not (len(srcs) == len(tgts) == len(gs)):
+            raise ValueError("sources, targets and guesses must have one entry per pair")
+        counts = np.array([len(g) for g in gs], np.int64)
+        n = int(counts.sum())
+        if n == 0:
+            return [dict(messages=[], T=np.empty((0, 3, 3), np.float32), iterations=np.zeros(0, np.int32),
+                         inliers=np.zeros(0, np.int32), status=np.zeros(0, np.int32)) for _ in gs]
+
+        def packed(clouds):
+            off = np.zeros(len(clouds) + 1, np.int32)
+            off[1:] = np.cumsum([len(c) for c in clouds])
+            return np.ascontiguousarray(np.concatenate(clouds + [np.zeros((0, 2), np.float32)]), np.float32), off
+
+        src, soff = packed(srcs)
+        tgt, toff = packed(tgts)
+        ids = np.ascontiguousarray(np.repeat(np.arange(len(gs), dtype=np.int32), counts))
+        g = np.ascontiguousarray(np.concatenate(gs))
+        T = np.empty((n, 3, 3), np.float32)
+        iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
+        ctx = _lib.default_context()
+        import ctypes
+        _lib.check(ctx.lib.sfe_icp_batch_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), _lib.ptr(soff),
+                                              len(srcs), _lib.ptr(tgt), _lib.ptr(toff), len(tgts), _lib.ptr(ids),
+                                              _lib.ptr(ids), n, _lib.ptr(g), _lib.ptr(T), _lib.ptr(iters),
+                                              _lib.ptr(inl), _lib.ptr(st)), "ICP.compute_pairs")
+        msgs = [ctx.lib.sfe_icp_status_message(int(s)).decode() for s in st]
+        for s, m in zip(st, msgs):
+            if int(s) in (5, 6):  # as in compute_batch: not ConvergenceErrors, they propagate as exceptions
+                raise RuntimeError(m)
+        out, a = [], 0
+        for c in counts:
+            b = a + int(c)
+            out.append(dict(messages=msgs[a:b], T=T[a:b], iterations=iters[a:b], inliers=inl[a:b], status=st[a:b]))
+            a = b
+        return out
+
     def getCovariance(self):
         raise NotImplementedError("ICP.getCovariance is never called by the reference's Python and is not provided")

@@ -110,6 +110,76 @@ class SLAM(object):
             cov = default_cov
         return "success", m, cov, sample_transforms
 
+    def compute_icp_with_cov_batch(self, problems):
+        """compute_icp_with_cov for many loop-closure candidates: `problems` is an iterable of (source_points,
+        target_points, guesses); returns the list of (message, Pose2, cov, sample_transforms) that one
+        compute_icp_with_cov call per candidate would return.  Every candidate's guesses go to the GPU in one ICP
+        launch and every MinCovDet fit in one more (sonar_slam_b200/mcd.py).
+
+        The fits' random trial supports are drawn here from numpy's global generator, 30 permutations per candidate
+        that reaches the fit, in candidate order -- the draws MinCovDet(random_state=None) makes -- so under the same
+        np.random seed this returns what the sequence of compute_icp_with_cov calls returns.  A batch of one is the
+        device path for a single candidate."""
+        from .. import mcd
+        sources, targets, guesses = [], [], []
+        for source_points, target_points, gs in problems:
+            gs = list(gs)
+            if len(gs) > mcd.MAX_SAMPLES:
+                raise ValueError(f"compute_icp_with_cov_batch: at most {mcd.MAX_SAMPLES} guesses per candidate")
+            sources.append(np.array(source_points, np.float32))
+            targets.append(np.array(target_points, np.float32))
+            guesses.append([g.matrix() for g in gs])
+        if not sources:
+            return []
+        results = self.icp.compute_pairs(sources, targets, guesses)
+        samples = []
+        for res in results:   # slam.py:349-360, per candidate
+            sample_transforms = []
+            for message, T in zip(res["messages"], res["T"]):
+                if message == "success":
+                    x, y = T[:2, 2]
+                    sample_transforms.append((x, y, np.arctan2(T[1, 0], T[0, 0])))
+            samples.append(np.array(sample_transforms))
+        out = [("Too few samples for covariance computation", None, None, None)] * len(samples)
+        # MinCovDet.fit validates its input (finite values) before it draws; such a fit raises ValueError
+        fit = []
+        for i, s in enumerate(samples):
+            if len(s) < mcd.MIN_SAMPLES:
+                continue
+            if not np.isfinite(s).all():
+                out[i] = ("Failed to calculate covariance", None, None, None)
+                continue
+            fit.append(i)
+        if not fit:
+            return out
+        subsets = np.stack([mcd.draw_trial_supports(len(samples[i])) for i in fit])
+        X, n = mcd.pack([samples[i] for i in fit])
+        f32 = np.array([samples[i].dtype == np.float32 for i in fit])
+        loc, covs = np.empty((len(fit), 3)), np.empty((len(fit), 3, 3))
+        status = np.empty(len(fit), np.int32)
+        for flag in (True, False):   # one call per sample dtype (float32 for the shipped ICP)
+            sel = np.flatnonzero(f32 == flag)
+            if len(sel):
+                r = mcd.mincovdet_host(X[sel], n[sel], subsets[sel], float32=flag)
+                loc[sel], covs[sel], status[sel] = r["location"], r["covariance"], r["status"]
+        # slam.py:372-385: unrotate into the local frame, keep the default covariance when it is bigger
+        default_cov = np.diag(self.icp_odom_sigmas) ** 2
+        ok = np.flatnonzero(status == mcd.OK)
+        ms = [Pose2(*loc[k]) for k in ok]
+        for m, k in zip(ms, ok):
+            cov = covs[k]
+            R = m.matrix()[:2, :2]
+            cov[:2, :] = R.T.dot(cov[:2, :])
+            cov[:, :2] = cov[:, :2].dot(R)
+        small = np.linalg.det(covs[ok]) < np.linalg.det(default_cov) if len(ok) else np.zeros(0, bool)
+        for m, k, s in zip(ms, ok, small):
+            out[fit[k]] = ("success", m, default_cov if s else covs[k], samples[fit[k]])
+        for k in np.flatnonzero(status != mcd.OK):
+            if status[k] != mcd.ZERO_COV:
+                raise RuntimeError(f"sfe_mincovdet: status {int(status[k])} for candidate {fit[k]}")
+            out[fit[k]] = ("Failed to calculate covariance", None, None, None)
+        return out
+
     # ---- slam.py:389-424
     def get_overlap(self, source_points, target_points, source_pose=None, target_pose=None, return_indices=False):
         if source_pose:

@@ -2,7 +2,9 @@
 // Declarations and reference citations: include/sonarfe.h.
 #include <cudaTypedefs.h>
 
+#include <algorithm>
 #include <mutex>
+#include <vector>
 
 #include "common.cuh"
 
@@ -374,47 +376,78 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
 int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host, int nt,
                  const float *guess_host, int n_guesses, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                  int32_t *status_host) {
-  SFE_REQUIRE(ctx && prm, "sfe_icp_host: null context or parameters");
   SFE_REQUIRE(ns >= 0 && nt >= 0 && n_guesses >= 0, "sfe_icp_host: negative size");
   if (n_guesses == 0) return SFE_OK;
-  SFE_REQUIRE(guess_host && T_host && iters_host && inliers_host && status_host, "sfe_icp_host: null pointer");
-  SFE_REQUIRE((src_host || ns == 0) && (tgt_host || nt == 0), "sfe_icp_host: null cloud pointer");
+  // one source / target pair: every guess is a problem on clouds 0 / 0
+  const int32_t src_off[2] = {0, ns}, tgt_off[2] = {0, nt};
+  std::vector<int32_t> zero((size_t)n_guesses, 0);
+  return sfe_icp_batch_host(ctx, prm, src_host, src_off, 1, tgt_host, tgt_off, 1, zero.data(), zero.data(), n_guesses,
+                            guess_host, T_host, iters_host, inliers_host, status_host);
+}
+
+int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host, const int32_t *src_off_host,
+                       int n_src_clouds, const float *tgt_pts_host, const int32_t *tgt_off_host, int n_tgt_clouds,
+                       const int32_t *src_id_host, const int32_t *tgt_id_host, int n_problems, const float *guess_host,
+                       float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
+  SFE_REQUIRE(ctx && prm, "sfe_icp_batch_host: null context or parameters");
+  SFE_REQUIRE(n_src_clouds >= 1 && n_tgt_clouds >= 1 && n_problems >= 0, "sfe_icp_batch_host: bad sizes");
+  if (n_problems == 0) return SFE_OK;
+  SFE_REQUIRE(src_off_host && tgt_off_host && src_id_host && tgt_id_host && guess_host && T_host && iters_host &&
+                  inliers_host && status_host,
+              "sfe_icp_batch_host: null pointer");
+  int ns_max = 0, nt_max = 0;
+  for (int c = 0; c < n_src_clouds; ++c) {
+    SFE_REQUIRE(src_off_host[c + 1] >= src_off_host[c], "sfe_icp_batch_host: source offsets decrease at %d", c);
+    ns_max = std::max(ns_max, src_off_host[c + 1] - src_off_host[c]);
+  }
+  for (int c = 0; c < n_tgt_clouds; ++c) {
+    SFE_REQUIRE(tgt_off_host[c + 1] >= tgt_off_host[c], "sfe_icp_batch_host: target offsets decrease at %d", c);
+    nt_max = std::max(nt_max, tgt_off_host[c + 1] - tgt_off_host[c]);
+  }
+  SFE_REQUIRE(src_off_host[0] == 0 && tgt_off_host[0] == 0, "sfe_icp_batch_host: offsets must start at 0");
+  const int ns = src_off_host[n_src_clouds], nt = tgt_off_host[n_tgt_clouds];
+  SFE_REQUIRE((src_pts_host || ns == 0) && (tgt_pts_host || nt == 0), "sfe_icp_batch_host: null cloud pointer");
+  for (int p = 0; p < n_problems; ++p)
+    SFE_REQUIRE(src_id_host[p] >= 0 && src_id_host[p] < n_src_clouds && tgt_id_host[p] >= 0 &&
+                    tgt_id_host[p] < n_tgt_clouds,
+                "sfe_icp_batch_host: problem %d names cloud %d / %d", p, src_id_host[p], tgt_id_host[p]);
   SFE_CUDA(cudaSetDevice(ctx->device));
+  const size_t P = (size_t)n_problems;
   Carver cv;
   for (int pass = 0; pass < 2; ++pass) {
     cv.off = 0;
     float *d_src = (float *)cv.take(sizeof(float) * 2 * (size_t)(ns > 0 ? ns : 1));
     float *d_tgt = (float *)cv.take(sizeof(float) * 2 * (size_t)(nt > 0 ? nt : 1));
-    int32_t *d_off = (int32_t *)cv.take(4 * sizeof(int32_t));
-    int32_t *d_zero = (int32_t *)cv.take(sizeof(int32_t) * (size_t)n_guesses);
-    float *d_guess = (float *)cv.take(sizeof(float) * 9 * (size_t)n_guesses);
-    float *d_T = (float *)cv.take(sizeof(float) * 9 * (size_t)n_guesses);
-    int32_t *d_res = (int32_t *)cv.take(sizeof(int32_t) * 3 * (size_t)n_guesses);
+    int32_t *d_soff = (int32_t *)cv.take(sizeof(int32_t) * (size_t)(n_src_clouds + 1));
+    int32_t *d_toff = (int32_t *)cv.take(sizeof(int32_t) * (size_t)(n_tgt_clouds + 1));
+    int32_t *d_ids = (int32_t *)cv.take(sizeof(int32_t) * 2 * P);
+    float *d_guess = (float *)cv.take(sizeof(float) * 9 * P);
+    float *d_T = (float *)cv.take(sizeof(float) * 9 * P);
+    int32_t *d_res = (int32_t *)cv.take(sizeof(int32_t) * 3 * P);
     if (pass == 0) {
       int rc = ensure(ctx, ctx->stage_in[1], cv.off);
       if (rc != SFE_OK) return rc;
       cv.base = (char *)ctx->stage_in[1].ptr;
       continue;
     }
-    const int32_t off[4] = {0, ns, 0, nt};
     if (ns > 0)
-      SFE_CUDA(cudaMemcpyAsync(d_src, src_host, sizeof(float) * 2 * (size_t)ns, cudaMemcpyHostToDevice, ctx->stream));
+      SFE_CUDA(cudaMemcpyAsync(d_src, src_pts_host, sizeof(float) * 2 * (size_t)ns, cudaMemcpyHostToDevice, ctx->stream));
     if (nt > 0)
-      SFE_CUDA(cudaMemcpyAsync(d_tgt, tgt_host, sizeof(float) * 2 * (size_t)nt, cudaMemcpyHostToDevice, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
-    SFE_CUDA(cudaMemsetAsync(d_zero, 0, sizeof(int32_t) * (size_t)n_guesses, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * (size_t)n_guesses, cudaMemcpyHostToDevice,
+      SFE_CUDA(cudaMemcpyAsync(d_tgt, tgt_pts_host, sizeof(float) * 2 * (size_t)nt, cudaMemcpyHostToDevice, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_soff, src_off_host, sizeof(int32_t) * (size_t)(n_src_clouds + 1), cudaMemcpyHostToDevice,
                              ctx->stream));
-    int rc = icp_run(ctx, prm, d_src, d_off, nullptr, d_tgt, d_off + 2, nullptr, 0, d_zero, d_zero, n_guesses, ns, nt,
-                     d_guess, d_T, d_res, d_res + n_guesses, d_res + 2 * n_guesses);
+    SFE_CUDA(cudaMemcpyAsync(d_toff, tgt_off_host, sizeof(int32_t) * (size_t)(n_tgt_clouds + 1), cudaMemcpyHostToDevice,
+                             ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_ids, src_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_ids + P, tgt_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
+    int rc = icp_run(ctx, prm, d_src, d_soff, nullptr, d_tgt, d_toff, nullptr, 0, d_ids, d_ids + P, n_problems, ns_max,
+                     nt_max, d_guess, d_T, d_res, d_res + P, d_res + 2 * P);
     if (rc != SFE_OK) return rc;
-    SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * (size_t)n_guesses, cudaMemcpyDeviceToHost, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * (size_t)n_guesses, cudaMemcpyDeviceToHost,
-                             ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(inliers_host, d_res + n_guesses, sizeof(int32_t) * (size_t)n_guesses,
-                             cudaMemcpyDeviceToHost, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(status_host, d_res + 2 * n_guesses, sizeof(int32_t) * (size_t)n_guesses,
-                             cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(inliers_host, d_res + P, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(status_host, d_res + 2 * P, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   return SFE_OK;

@@ -133,3 +133,31 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
                                    _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, int(ns_max), int(nt_max), _dp(guess),
                                    _dp(T), _dp(iters), _dp(inl), _dp(st)), "sfe_icp_dev")
     return dict(T=T, iterations=iters, inliers=inl, status=st)
+
+
+def mincovdet(samples, n, subsets, float32=False, ctx=None):
+    """Batched MinCovDet(support_fraction=0.8) fits (include/sonarfe.h: sfe_mincovdet_dev; sonar_slam_b200/mcd.py).
+
+    samples: float64 [P,32,3] cuda, n: int32 [P] cuda, subsets: int8 [P,30,32] cuda (mcd.draw_trial_supports).
+    Returns dict(location=f64[P,3], covariance=f64[P,3,3], raw_support=i32[P], support=i32[P] (bit masks), status=i32[P]).
+    """
+    from . import mcd
+    for name, t, dt in (("samples", samples, torch.float64), ("n", n, torch.int32), ("subsets", subsets, torch.int8)):
+        if not t.is_cuda or t.dtype != dt:
+            raise _lib.SonarFEError(f"ops.mincovdet: {name} must be a CUDA {dt} tensor")
+    samples, n, subsets = samples.contiguous(), n.contiguous(), subsets.contiguous()
+    P = n.numel()
+    if samples.numel() != P * mcd.MAX_SAMPLES * 3 or subsets.numel() != P * mcd.TRIALS * mcd.MAX_SAMPLES:
+        raise ValueError("ops.mincovdet: samples must be [P,32,3] and subsets [P,30,32]")
+    ctx = ctx or context(samples.device)
+    c, c_rw, cut = mcd.constants()
+    dev = samples.device
+    loc = torch.empty((P, 3), dtype=torch.float64, device=dev)
+    cov = torch.empty((P, 3, 3), dtype=torch.float64, device=dev)
+    raw = torch.empty((P,), dtype=torch.int32, device=dev)
+    sup = torch.empty_like(raw)
+    st = torch.empty_like(raw)
+    _lib.check(ctx.lib.sfe_mincovdet_dev(ctx.handle, _dp(samples), _dp(n), _dp(subsets), P, _lib.ptr(c), c_rw, cut,
+                                         mcd.FLOAT32 if float32 else 0, _dp(loc), _dp(cov), _dp(raw), _dp(sup), _dp(st)),
+               "sfe_mincovdet_dev")
+    return dict(location=loc, covariance=cov, raw_support=raw, support=sup, status=st)
