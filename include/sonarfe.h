@@ -382,6 +382,68 @@ SFE_API int sfe_fov_select_host(sfe_ctx *ctx, const float *pts_host, int n, cons
                                 const double *range_bound_host, const double *bearing_bound_host, int n_frames,
                                 uint8_t *sel_host);
 
+/* ------------------------------------------------------------------ compressed pings (row N4)
+ * feature_extraction.py:210-213 (compressed_images: True): cv2.cvtColor(cv2.imdecode(buf, IMREAD_COLOR), BGR2GRAY),
+ * i.e. libjpeg-turbo's default decompression (JDCT_ISLOW, fancy upsampling) followed by OpenCV's fixed-point
+ * BGR -> gray.  The decoder reproduces that uint8 frame bit for bit for the streams it accepts:
+ *   baseline / extended sequential Huffman (SOF0, SOF1), 8-bit samples, one interleaved scan;
+ *   1 component, or 3 components that libjpeg-turbo takes as YCbCr (JFIF marker, ids 1/2/3, Adobe transform 1);
+ *   sampling 4:4:4, 4:2:2 (luma 2x1), 4:2:0 (luma 2x2); any restart interval; 8- and 16-bit DQT tables;
+ *   tables that differ from frame to frame; APPn / COM segments are skipped.
+ * Everything else gets a per-stream status (sfe_jpeg_status_message names the reason); PNG stays on the host path.
+ * Streams are packed: stream i = bytes[offsets[i] .. offsets[i+1]), offsets int64 [n + 1].  See csrc/jpeg.cu. */
+enum {
+  SFE_JPEG_OK = 0,
+  SFE_JPEG_NOT_JPEG = 1,     /* no SOI marker (PNG, random bytes ...) */
+  SFE_JPEG_TRUNCATED = 2,    /* the headers end before the start of scan */
+  SFE_JPEG_PROGRESSIVE = 3,
+  SFE_JPEG_LOSSLESS = 4,
+  SFE_JPEG_ARITHMETIC = 5,
+  SFE_JPEG_PRECISION = 6,    /* sample precision other than 8 (12-bit) */
+  SFE_JPEG_SAMPLING = 7,     /* 4:1:1, 4:4:0 and other factors */
+  SFE_JPEG_COLORSPACE = 8,   /* CMYK / YCCK, 2 components, RGB (Adobe transform 0, R/G/B ids) */
+  SFE_JPEG_ORIENTATION = 9,  /* EXIF orientation other than 1: imdecode would rotate the image */
+  SFE_JPEG_SIZE = 10,        /* decoders only: frame size differs from the call's R x B */
+  SFE_JPEG_CORRUPT = 11,     /* decoders only: invalid Huffman code, run past coefficient 63, data ending before the
+                                last MCU of a segment (libjpeg-turbo pads such data with zeros and warns), missing or
+                                out-of-sequence RSTn.  Data after a segment's last MCU is skipped, as libjpeg-turbo
+                                skips it */
+  SFE_JPEG_BAD_HEADER = 12   /* malformed tables, multi-scan or partial scans, hierarchical mode */
+};
+/* sampling codes of sfe_jpeg_inspect_host */
+enum { SFE_JPEG_GRAY = 0, SFE_JPEG_444 = 1, SFE_JPEG_422 = 2, SFE_JPEG_420 = 3, SFE_JPEG_INFO = 6 };
+SFE_API const char *sfe_jpeg_status_message(int status);
+/* Headers only, no context, no GPU.  info int32 [n][SFE_JPEG_INFO]: status, height, width, components, sampling code
+ * (-1 unless status is SFE_JPEG_OK), restart interval (MCUs; 0 = none). */
+SFE_API int sfe_jpeg_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, int32_t *info);
+/* Decode n streams into uint8 [n][R][B] frames (host memory / device memory of the context's GPU).  Headers are
+ * parsed on the host; the entropy-coded bytes go in chunk by chunk on a copy stream, overlapped with decoding, and
+ * device scratch is bounded by the chunk.  status_host int32 [n]: SFE_JPEG_*; a frame whose status is not
+ * SFE_JPEG_OK is written as zeros.  Both return when the frames and statuses are there. */
+SFE_API int sfe_jpeg_decode_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
+                                 uint8_t *out_host, int32_t *status_host);
+SFE_API int sfe_jpeg_decode_to_dev(sfe_ctx *ctx, const uint8_t *bytes_host, const int64_t *offsets_host, int n, int R,
+                                   int B, uint8_t *out_dev, int32_t *status_host);
+/* Diagnostic: the dequantised coefficient blocks the IDCT consumes, int32 [n][cap_blocks][64] in natural order, blocks
+ * in decode (MCU) order, zeros after a frame's last block and for frames whose status is not SFE_JPEG_OK.
+ * SFE_ERR_CAPACITY when a frame has more than cap_blocks blocks. */
+/* Optional per-stage device timing of the decoders (CUDA events on the context's stream around the kernels of every
+ * chunk).  get_timing synchronises, adds the intervals recorded since the last call to running totals and returns them:
+ * stage_ms[SFE_JPEG_STAGES], stage_calls[SFE_JPEG_STAGES] (may be NULL). */
+enum { SFE_JPEG_T_UNSTUFF = 0, SFE_JPEG_T_ENTROPY = 1, SFE_JPEG_T_PIXELS = 2 /* IDCT + colour */, SFE_JPEG_STAGES = 3 };
+SFE_API int sfe_jpeg_set_timing(sfe_ctx *ctx, int enable);
+SFE_API int sfe_jpeg_get_timing(sfe_ctx *ctx, double *stage_ms, int64_t *stage_calls);
+SFE_API int sfe_jpeg_coefficients_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
+                                       int cap_blocks, int32_t *coef_host, int32_t *status_host);
+/* sfe_frontend_run_host with compressed pings: the copy of raw frames is replaced by the copy of the streams' bytes
+ * and the decode into the front end's frame buffer.  Carry, chunking and results are those of sfe_frontend_run_host.
+ * A stream that is rejected (checked for all n before any work) or fails to decode makes the call return
+ * SFE_ERR_ARG naming the first such frame, before any front-end stage runs on its chunk. */
+SFE_API int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                       const double *poses_host, int n_frames, int chunk_frames, float *T_host,
+                                       int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                                       int32_t *npoints_host);
+
 #ifdef __cplusplus
 }
 #endif

@@ -59,6 +59,8 @@ def load():
         lib.sfe_frontend_params_default.restype = None
         lib.sfe_frontend_destroy.argtypes = [c_void_p]
         lib.sfe_frontend_destroy.restype = None
+        lib.sfe_jpeg_status_message.argtypes = [c_int]
+        lib.sfe_jpeg_status_message.restype = ctypes.c_char_p
         _lib = lib
         return lib
 
@@ -112,6 +114,14 @@ _EXTRA_SIGNATURES = {
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_mincovdet_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_jpeg_inspect_host": [c_void_p, c_void_p, c_int, c_void_p],
+    "sfe_jpeg_decode_host": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sfe_jpeg_decode_to_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sfe_jpeg_coefficients_host": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sfe_jpeg_set_timing": [c_void_p, c_int],
+    "sfe_jpeg_get_timing": [c_void_p, c_void_p, c_void_p],
+    "sfe_frontend_run_jpeg_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                   c_void_p, c_void_p],
 }
 
 

@@ -127,6 +127,7 @@ void sfe_ctx_destroy(sfe_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
+  if (ctx->jpeg_free) ctx->jpeg_free(ctx->jpeg);
   for (auto &b : ctx->scratch)
     if (b.ptr) cudaFree(b.ptr);
   for (auto &b : ctx->stage_in)

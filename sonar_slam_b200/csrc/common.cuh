@@ -59,6 +59,8 @@ struct sfe_ctx {
   const void *cfar_lut_buf = nullptr;            // ... and the buffer it was uploaded to (null = none)
   struct OccEntry { size_t smem; int threads, per_sm, variant; } icp_occ[8] = {};
   int icp_occ_next = 0;
+  void *jpeg = nullptr;                 // JPEG decoder state (jpeg.cu), created on first use
+  void (*jpeg_free)(void *) = nullptr;
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)

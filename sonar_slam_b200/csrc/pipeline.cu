@@ -13,6 +13,7 @@
 // Device layout: every per-frame cloud lives at a fixed stride (`cap_points` rows) with a count
 // array, so all stages run without packing or host round trips; the host flavour overlaps the
 // host->device copy of frame chunk k+1 with the kernels of chunk k on two streams.
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -32,6 +33,15 @@ int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const
             const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out, int *iters,
             int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
             int class_ns = 0, int class_nt = 0, int force_threads = 0);
+// compressed pings (jpeg.cu)
+struct JpegBatch;
+struct JpegState;
+int jpeg_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, JpegBatch **out);
+void jpeg_batch_free(JpegBatch *b);
+int jpeg_batch_status(const JpegBatch *b, int i);
+int jpeg_begin(sfe_ctx *ctx, const JpegBatch &bt, int chunk, JpegState **js);
+int jpeg_decode_frames(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int f0, int nf, uint8_t *out_dev);
+const int32_t *jpeg_status_dev(const JpegState *js);
 
 // Size class of the first ICP launch (fe_match), chosen on the config-4 replay (filtered clouds: median 326,
 // max 639 points; window submaps <= 1808 raw points; not re-measured on H100): this class with 128 threads (6 CTAs
@@ -563,6 +573,87 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
     if (rc != SFE_OK) return rc;
   }
   int rc = fe_update_carry(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(inliers_host, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(status_host, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  if (npoints_host) {
+    const int32_t *cnt;
+    fe_cloud(fe, &cnt);
+    SFE_CUDA(cudaMemcpyAsync(npoints_host, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SFE_OK;
+}
+
+// The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
+// fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
+// so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
+static int fe_run_jpeg(sfe_frontend *fe, JpegBatch *bt, const double *poses_host, int n_frames, int chunk_frames) {
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  for (int i = 0; i < n_frames; ++i)
+    if (jpeg_batch_status(bt, i) != SFE_JPEG_OK) {
+      set_error("sfe_frontend_run_jpeg_host: frame %d: %s", i, sfe_jpeg_status_message(jpeg_batch_status(bt, i)));
+      return SFE_ERR_ARG;
+    }
+  JpegState *js;
+  int rc = jpeg_begin(ctx, *bt, chunk_frames, &js);
+  if (rc != SFE_OK) return rc;
+  rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
+  if (rc != SFE_OK) return rc;
+  int32_t *st_host = static_cast<int32_t *>(ctx->pinned);
+  rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  auto decode = [&](int f0, int k) -> int {
+    const int n = std::min(chunk_frames, n_frames - f0);
+    int r = jpeg_decode_frames(ctx, js, *bt, f0, n, fe->frames + (size_t)f0 * fbytes);
+    if (r != SFE_OK) return r;
+    SFE_CUDA(cudaMemcpyAsync(st_host + f0, jpeg_status_dev(js) + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost,
+                             ctx->stream));
+    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
+    return SFE_OK;
+  };
+  rc = decode(0, 0);
+  int k = 0;
+  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
+    const int n = std::min(chunk_frames, n_frames - f0);
+    if (f0 + chunk_frames < n_frames) rc = decode(f0 + chunk_frames, k + 1);
+    if (rc != SFE_OK) break;
+    SFE_CUDA(cudaEventSynchronize(fe->ev_copy[k & 1]));
+    for (int i = f0; i < f0 + n; ++i)
+      if (st_host[i] != SFE_JPEG_OK) {
+        SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+        set_error("sfe_frontend_run_jpeg_host: frame %d: %s", i, sfe_jpeg_status_message(st_host[i]));
+        return SFE_ERR_ARG;
+      }
+    rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
+    if (rc == SFE_OK) rc = fe_match(fe, f0, n);
+  }
+  return rc;
+}
+
+int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
+                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
+                               int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
+  SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
+              "sfe_frontend_run_jpeg_host: null argument");
+  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_jpeg_host: %d frames exceed max_frames %d",
+              n_frames, fe->max_frames);
+  for (int i = 0; i < n_frames; ++i)
+    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0,
+                "sfe_frontend_run_jpeg_host: offsets must be non-decreasing");
+  if (n_frames == 0) return SFE_OK;
+  sfe_ctx *ctx = fe->ctx;
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  if (chunk_frames <= 0) chunk_frames = 256;
+  JpegBatch *bt;
+  int rc = jpeg_batch_parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
+  if (rc == SFE_OK) rc = fe_run_jpeg(fe, bt, poses_host, n_frames, chunk_frames);
+  jpeg_batch_free(bt);
+  if (rc != SFE_OK) return rc;
+  rc = fe_update_carry(fe, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));

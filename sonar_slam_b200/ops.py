@@ -6,6 +6,7 @@ on the torch current stream of the tensor's device and return torch tensors.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -161,3 +162,19 @@ def mincovdet(samples, n, subsets, float32=False, ctx=None):
                                          mcd.FLOAT32 if float32 else 0, _dp(loc), _dp(cov), _dp(raw), _dp(sup), _dp(st)),
                "sfe_mincovdet_dev")
     return dict(location=loc, covariance=cov, raw_support=raw, support=sup, status=st)
+
+
+def decode_jpeg(streams, R, B, device=None, ctx=None):
+    """Decode compressed pings into a uint8 [n, R, B] tensor on the device (include/sonarfe.h: sfe_jpeg_decode_to_dev;
+    sonar_slam_b200/jpeg.py).  streams: a sequence of bytes objects, or (bytes, offsets) from jpeg.pack.
+    Returns (frames, status int32 [n] numpy): a frame whose status is not jpeg.OK is zeros.  The call returns once the
+    frames are written (the statuses are read back)."""
+    from . import jpeg
+    buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
+    n = len(off) - 1
+    ctx = ctx or context(device)
+    out = torch.empty((n, int(R), int(B)), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    st = np.empty(n, np.int32)
+    _lib.check(ctx.lib.sfe_jpeg_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
+                                              _lib.ptr(st)), "sfe_jpeg_decode_to_dev")
+    return out, st

@@ -377,8 +377,45 @@ def cfar_reference_fixture():
     print("cfar_reference:", {a: len(v["mask_counts"]) for a, v in g.items()}, "cases written to", out)
 
 
+def jpeg_fixture():
+    """tests/golden/jpeg_streams.npz: encoded pings over the decoder's option grid with the SHA-256 of the gray image
+    cv2.imdecode(IMREAD_COLOR) + BGR2GRAY gives, and the cv2 / libjpeg-turbo versions that produced them.  Needs only
+    cv2 (no reference tree)."""
+    import hashlib
+    import cv2
+    from oracle import jpeg_ref
+    streams, names, digests, shapes = [], [], [], []
+    grid = [((512, 512), "synth", 80, "gray", 0, 0), ((511, 509), "synth", 50, "420", 1, 17),
+            ((96, 80), "noise", 50, "422", 0, 3), ((511, 509), "checker", 5, "444", 1, 0),
+            ((17, 33), "checker", 1, "420", 0, 1), ((17, 33), "noise", 100, "444", 0, 0),
+            ((7, 9), "synth", 25, "422", 1, 1), ((1, 1), "full", 75, "420", 0, 0), ((8, 8), "zero", 10, "gray", 1, 3),
+            ((16, 16), "checker", 90, "gray", 0, 17)]
+    for q in (1, 5, 10, 25, 50, 75, 80, 90, 95, 100):
+        for samp in jpeg_ref.SAMPLINGS:
+            grid.append(((64, 48), "synth" if q % 2 else "checker", q, samp, q % 3 == 0, (0, 1, 3, 17)[q % 4]))
+    for (h, w), content, q, samp, opt, ri in grid:
+        img = jpeg_ref.contents(h, w, seed=h)[content]
+        b = jpeg_ref.encode(img, q, samp, opt, ri)
+        gray = jpeg_ref.cv2_gray(b)
+        streams.append(np.frombuffer(b, np.uint8))
+        names.append(f"{h}x{w}_{content}_q{q}_{samp}_opt{int(bool(opt))}_ri{ri}")
+        digests.append(hashlib.sha256(np.ascontiguousarray(gray).tobytes()).hexdigest())
+        shapes.append((h, w))
+    off = np.zeros(len(streams) + 1, np.int64)
+    off[1:] = np.cumsum([len(s) for s in streams])
+    out = os.path.join(REPO, "tests", "golden", "jpeg_streams.npz")
+    info = cv2.getBuildInformation()
+    jpeg_line = [l.strip() for l in info.splitlines() if l.strip().startswith("JPEG:")]
+    np.savez_compressed(out, bytes=np.concatenate(streams), offsets=off, names=np.array(names),
+                        sha256=np.array(digests), shapes=np.array(shapes, np.int32),
+                        cv2_version=np.array(cv2.__version__), libjpeg=np.array(jpeg_line[0] if jpeg_line else ""))
+    print("jpeg_streams:", len(streams), "streams,", int(off[-1]), "bytes written to", out)
+
+
 if __name__ == "__main__":
-    if "--only-fov" in sys.argv:
+    if "--only-jpeg" in sys.argv:
+        jpeg_fixture()
+    elif "--only-fov" in sys.argv:
         fov_fixture()
     elif "--only-cfar-reference" in sys.argv:
         cfar_reference_fixture()
@@ -386,3 +423,4 @@ if __name__ == "__main__":
         main()
         fov_fixture()
         cfar_reference_fixture()
+        jpeg_fixture()
