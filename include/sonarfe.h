@@ -444,6 +444,50 @@ SFE_API int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, c
                                        int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
                                        int32_t *npoints_host);
 
+/* PNG pings: the same cv2.imdecode(IMREAD_COLOR) + BGR2GRAY frame, bit for bit, for the streams a ping encoder
+ * writes: IHDR with bit depth 8, colour type 0 (gray) or 2 (truecolour), no interlace; any number of IDAT chunks;
+ * stored, fixed and dynamic deflate blocks with any window; the five row filters.  Ancillary chunks are ignored as
+ * libpng ignores them.  Gray samples are the image; truecolour goes through OpenCV 4.x's BGR2GRAY.  Everything else
+ * gets a per-stream status.  Inflated data past the last row is skipped (libpng warns "Too much image data") but must
+ * still be valid deflate with a matching Adler-32.  Streams are packed as for JPEG.  See csrc/png.cu. */
+enum {
+  SFE_PNG_OK = 0,
+  SFE_PNG_NOT_PNG = 1,      /* no PNG signature (JPEG, random bytes ...) */
+  SFE_PNG_TRUNCATED = 2,    /* the chunk list ends before IEND */
+  SFE_PNG_BAD_HEADER = 3,   /* malformed IHDR (or its CRC), no IDAT, IDATs not consecutive, unknown critical chunk,
+                               PLTE after IDAT, width or height 0 or above libpng's 1000000 limit */
+  SFE_PNG_DEPTH = 4,        /* bit depth other than 8 */
+  SFE_PNG_COLORTYPE = 5,    /* palette, gray + alpha, RGBA */
+  SFE_PNG_INTERLACED = 6,   /* Adam7 */
+  SFE_PNG_ORIENTATION = 7,  /* eXIf orientation other than 1: imdecode would rotate the image */
+  SFE_PNG_ANIMATED = 8,     /* acTL chunk (APNG) */
+  SFE_PNG_SIZE = 9,         /* decoders only: frame size differs from the call's R x B */
+  SFE_PNG_CORRUPT = 10      /* decoders only: IDAT CRC, zlib header, invalid deflate (reserved block type, stored
+                               LEN / NLEN, bad code lengths, invalid symbol, distance beyond the output or the
+                               declared window), Adler-32, filter byte above 4, too little image data */
+};
+enum { SFE_PNG_INFO = 5 };
+SFE_API const char *sfe_png_status_message(int status);
+/* Chunk list only, no context, no GPU.  info int32 [n][SFE_PNG_INFO]: status, height, width, colour type, number of
+ * IDAT chunks (geometry as far as the IHDR could be read, else 0). */
+SFE_API int sfe_png_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, int32_t *info);
+/* As sfe_jpeg_decode_host / _to_dev: uint8 [n][R][B] frames, status_host int32 [n] SFE_PNG_*; a frame whose status is
+ * not SFE_PNG_OK is written as zeros. */
+SFE_API int sfe_png_decode_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
+                                uint8_t *out_host, int32_t *status_host);
+SFE_API int sfe_png_decode_to_dev(sfe_ctx *ctx, const uint8_t *bytes_host, const int64_t *offsets_host, int n, int R,
+                                  int B, uint8_t *out_dev, int32_t *status_host);
+/* Per-stage device timing, as sfe_jpeg_set_timing / _get_timing. */
+enum { SFE_PNG_T_CHECK = 0 /* IDAT CRC + gather */, SFE_PNG_T_INFLATE = 1, SFE_PNG_T_UNFILTER = 2 /* + gray, Adler */,
+       SFE_PNG_STAGES = 3 };
+SFE_API int sfe_png_set_timing(sfe_ctx *ctx, int enable);
+SFE_API int sfe_png_get_timing(sfe_ctx *ctx, double *stage_ms, int64_t *stage_calls);
+/* sfe_frontend_run_jpeg_host with PNG streams. */
+SFE_API int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                      const double *poses_host, int n_frames, int chunk_frames, float *T_host,
+                                      int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                                      int32_t *npoints_host);
+
 #ifdef __cplusplus
 }
 #endif

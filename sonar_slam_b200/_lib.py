@@ -61,6 +61,8 @@ def load():
         lib.sfe_frontend_destroy.restype = None
         lib.sfe_jpeg_status_message.argtypes = [c_int]
         lib.sfe_jpeg_status_message.restype = ctypes.c_char_p
+        lib.sfe_png_status_message.argtypes = [c_int]
+        lib.sfe_png_status_message.restype = ctypes.c_char_p
         _lib = lib
         return lib
 
@@ -122,6 +124,13 @@ _EXTRA_SIGNATURES = {
     "sfe_jpeg_get_timing": [c_void_p, c_void_p, c_void_p],
     "sfe_frontend_run_jpeg_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p],
+    "sfe_png_inspect_host": [c_void_p, c_void_p, c_int, c_void_p],
+    "sfe_png_decode_host": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sfe_png_decode_to_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sfe_png_set_timing": [c_void_p, c_int],
+    "sfe_png_get_timing": [c_void_p, c_void_p, c_void_p],
+    "sfe_frontend_run_png_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p],
 }
 
 

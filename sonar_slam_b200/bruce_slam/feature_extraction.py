@@ -64,8 +64,8 @@ class FeatureExtraction(object):
         self.maxRange = None
 
         self.compressed_images = True
-        # opt-in: decode compressed pings that sonar_slam_b200.jpeg accepts on the GPU (same uint8 image bit for bit);
-        # other streams (PNG, progressive JPEG, ...) keep the cv2 path
+        # opt-in: decode compressed pings that sonar_slam_b200.jpeg or sonar_slam_b200.png accepts on the GPU (same
+        # uint8 image bit for bit); other streams (progressive JPEG, palette PNG, ...) keep the cv2 path
         self.decode_on_device = False
         self.rov_id = ""
 
@@ -149,7 +149,7 @@ class FeatureExtraction(object):
         """The polar uint8 image of a ping.  Compressed pings (`compressed_images: True`, a sensor_msgs/CompressedImage
         whose `.data` holds the PNG/JPEG bytes) are decoded on the host exactly like the reference does
         (feature_extraction.py:210-213: cv2.imdecode as BGR, then BGR -> gray) -- or, with `decode_on_device`, on the GPU
-        when sonar_slam_b200.jpeg accepts the stream (the same image); anything else is taken as the decoded
+        when sonar_slam_b200.jpeg or .png accepts the stream (the same image); anything else is taken as the decoded
         [num_ranges, num_beams] array (the reference's ros_numpy.image_to_numpy branch, :217)."""
         img = getattr(sonar_msg, "image", None)
         if img is None:
@@ -157,11 +157,12 @@ class FeatureExtraction(object):
         data = getattr(img, "data", None)
         if self.compressed_images and isinstance(data, (bytes, bytearray, memoryview)):
             if self.decode_on_device:
-                from .. import jpeg
-                info = jpeg.inspect([data])[0]
-                if info[0] == jpeg.OK:
-                    out, st = jpeg.decode_host([data], info[1], info[2])
-                    if st[0] == jpeg.OK:
+                from .. import jpeg, png
+                codec = png if bytes(data[:8]) == png.SIGNATURE else jpeg
+                info = codec.inspect([data])[0]
+                if info[0] == codec.OK:
+                    out, st = codec.decode_host([data], info[1], info[2])
+                    if st[0] == codec.OK:
                         return out[0]
                 # rejected, or data the device calls corrupt (e.g. truncated: libjpeg-turbo pads it and warns):
                 # the reference's own decoder decides, as it does without decode_on_device

@@ -128,6 +128,7 @@ void sfe_ctx_destroy(sfe_ctx *ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->jpeg_free) ctx->jpeg_free(ctx->jpeg);
+  if (ctx->png_free) ctx->png_free(ctx->png);
   for (auto &b : ctx->scratch)
     if (b.ptr) cudaFree(b.ptr);
   for (auto &b : ctx->stage_in)

@@ -61,6 +61,8 @@ struct sfe_ctx {
   int icp_occ_next = 0;
   void *jpeg = nullptr;                 // JPEG decoder state (jpeg.cu), created on first use
   void (*jpeg_free)(void *) = nullptr;
+  void *png = nullptr;                  // PNG decoder state (png.cu), created on first use
+  void (*png_free)(void *) = nullptr;
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
@@ -80,6 +82,34 @@ enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC =
 
 int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes);  // (re)allocate if too small
 int ensure_pinned(sfe_ctx *ctx, size_t bytes);
+
+// ---------------------------------------------------------------- compressed pings (jpeg.cu, png.cu)
+// Orientation (tag 0x0112 of IFD0) of a TIFF structure, as carried by JPEG's APP1 "Exif" segment and PNG's eXIf
+// chunk; 1 when absent or unreadable.
+inline int tiff_orientation(const uint8_t *t, int64_t tl) {
+  if (tl < 8) return 1;
+  const bool le = t[0] == 'I' && t[1] == 'I', be = t[0] == 'M' && t[1] == 'M';
+  if (!le && !be) return 1;
+  auto u16 = [&](int64_t o) { return le ? (t[o] | t[o + 1] << 8) : (t[o] << 8 | t[o + 1]); };
+  auto u32 = [&](int64_t o) { return ((uint32_t)u16(le ? o + 2 : o) << 16) | (uint32_t)u16(le ? o : o + 2); };
+  const int64_t ifd = u32(4);
+  if (ifd + 2 > tl) return 1;
+  const int cnt = u16(ifd);
+  for (int k = 0; k < cnt; ++k) {
+    const int64_t e = ifd + 2 + 12 * (int64_t)k;
+    if (e + 12 > tl) break;
+    if (u16(e) == 0x0112) return u16(e + 8);
+  }
+  return 1;
+}
+
+#ifdef __CUDACC__
+// OpenCV 4.x cvtColor BGR2GRAY, 8-bit: fixed point with 15 fractional bits (the weights sum to 2^15, so three equal
+// channels give the value back)
+__host__ __device__ __forceinline__ uint8_t bgr2gray(int b, int g, int r) {
+  return (uint8_t)((3735 * b + 19235 * g + 9798 * r + (1 << 14)) >> 15);
+}
+#endif
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda needed)
 int encode_tensor_map_3d(CUtensorMap *map, CUtensorMapDataType dt, size_t elem_bytes, const void *base,

@@ -73,21 +73,7 @@ __constant__ uint8_t c_natural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32
 // EXIF orientation (tag 0x0112 of IFD0) of an APP1 "Exif" segment; 1 when absent or unreadable
 static int exif_orientation(const uint8_t *s, int64_t sl) {
   if (sl < 14 || memcmp(s, "Exif\0\0", 6) != 0) return 1;
-  const uint8_t *t = s + 6;
-  const int64_t tl = sl - 6;
-  const bool le = t[0] == 'I' && t[1] == 'I', be = t[0] == 'M' && t[1] == 'M';
-  if (!le && !be) return 1;
-  auto u16 = [&](int64_t o) { return le ? (t[o] | t[o + 1] << 8) : (t[o] << 8 | t[o + 1]); };
-  auto u32 = [&](int64_t o) { return ((uint32_t)u16(le ? o + 2 : o) << 16) | (uint32_t)u16(le ? o : o + 2); };
-  const int64_t ifd = u32(4);
-  if (ifd + 2 > tl) return 1;
-  const int cnt = u16(ifd);
-  for (int k = 0; k < cnt; ++k) {
-    const int64_t e = ifd + 2 + 12 * (int64_t)k;
-    if (e + 12 > tl) break;
-    if (u16(e) == 0x0112) return u16(e + 8);
-  }
-  return 1;
+  return tiff_orientation(s + 6, sl - 6);
 }
 
 // Headers up to the start of the (single) scan.  Mirrors libjpeg-turbo's marker reader where it decides what is
@@ -871,9 +857,7 @@ __global__ void __launch_bounds__(256) jpeg_color_kernel(const JDesc *__restrict
     const int r = clamp255(Y + ((91881 * cr + 32768) >> 16));
     const int g = clamp255(Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16));
     const int b = clamp255(Y + ((116130 * cb + 32768) >> 16));
-    // OpenCV 4.x cvtColor BGR2GRAY, 8-bit: fixed point with 15 fractional bits (the weights sum to 2^15, so three
-    // equal channels give the value back)
-    o[i] = (uint8_t)((3735 * b + 19235 * g + 9798 * r + (1 << 14)) >> 15);
+    o[i] = bgr2gray(b, g, r);
   }
 }
 

@@ -42,6 +42,47 @@ int jpeg_batch_status(const JpegBatch *b, int i);
 int jpeg_begin(sfe_ctx *ctx, const JpegBatch &bt, int chunk, JpegState **js);
 int jpeg_decode_frames(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int f0, int nf, uint8_t *out_dev);
 const int32_t *jpeg_status_dev(const JpegState *js);
+// (png.cu)
+struct PngBatch;
+struct PngState;
+int png_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, PngBatch **out);
+void png_batch_free(PngBatch *b);
+int png_batch_status(const PngBatch *b, int i);
+int png_begin(sfe_ctx *ctx, const PngBatch &bt, int chunk, PngState **ps);
+int png_decode_frames(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int f0, int nf, uint8_t *out_dev);
+const int32_t *png_status_dev(const PngState *ps);
+
+// The decoders the compressed front-end entry points are written over.
+struct JpegFormat {
+  using Batch = JpegBatch;
+  using State = JpegState;
+  static int parse(const uint8_t *b, const int64_t *o, int n, int R, int B, Batch **out) {
+    return jpeg_batch_parse(b, o, n, R, B, out);
+  }
+  static void free(Batch *b) { jpeg_batch_free(b); }
+  static int status(const Batch *b, int i) { return jpeg_batch_status(b, i); }
+  static const char *message(int st) { return sfe_jpeg_status_message(st); }
+  static int begin(sfe_ctx *c, const Batch &b, int chunk, State **s) { return jpeg_begin(c, b, chunk, s); }
+  static int decode(sfe_ctx *c, State *s, const Batch &b, int f0, int nf, uint8_t *o) {
+    return jpeg_decode_frames(c, s, b, f0, nf, o);
+  }
+  static const int32_t *status_dev(const State *s) { return jpeg_status_dev(s); }
+};
+struct PngFormat {
+  using Batch = PngBatch;
+  using State = PngState;
+  static int parse(const uint8_t *b, const int64_t *o, int n, int R, int B, Batch **out) {
+    return png_batch_parse(b, o, n, R, B, out);
+  }
+  static void free(Batch *b) { png_batch_free(b); }
+  static int status(const Batch *b, int i) { return png_batch_status(b, i); }
+  static const char *message(int st) { return sfe_png_status_message(st); }
+  static int begin(sfe_ctx *c, const Batch &b, int chunk, State **s) { return png_begin(c, b, chunk, s); }
+  static int decode(sfe_ctx *c, State *s, const Batch &b, int f0, int nf, uint8_t *o) {
+    return png_decode_frames(c, s, b, f0, nf, o);
+  }
+  static const int32_t *status_dev(const State *s) { return png_status_dev(s); }
+};
 
 // Size class of the first ICP launch (fe_match), chosen on the config-4 replay (filtered clouds: median 326,
 // max 639 points; window submaps <= 1808 raw points; not re-measured on H100): this class with 128 threads (6 CTAs
@@ -587,19 +628,24 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
   return SFE_OK;
 }
 
+}  // extern "C"
+
 // The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
 // fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
 // so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
-static int fe_run_jpeg(sfe_frontend *fe, JpegBatch *bt, const double *poses_host, int n_frames, int chunk_frames) {
+// Fmt::status is 0 for a frame the decoder takes (SFE_JPEG_OK, SFE_PNG_OK).
+template <class Fmt>
+static int fe_run_compressed(sfe_frontend *fe, typename Fmt::Batch *bt, const double *poses_host, int n_frames,
+                             int chunk_frames, const char *what) {
   sfe_ctx *ctx = fe->ctx;
   const size_t fbytes = (size_t)fe->p.R * fe->p.B;
   for (int i = 0; i < n_frames; ++i)
-    if (jpeg_batch_status(bt, i) != SFE_JPEG_OK) {
-      set_error("sfe_frontend_run_jpeg_host: frame %d: %s", i, sfe_jpeg_status_message(jpeg_batch_status(bt, i)));
+    if (Fmt::status(bt, i) != 0) {
+      set_error("%s: frame %d: %s", what, i, Fmt::message(Fmt::status(bt, i)));
       return SFE_ERR_ARG;
     }
-  JpegState *js;
-  int rc = jpeg_begin(ctx, *bt, chunk_frames, &js);
+  typename Fmt::State *js;
+  int rc = Fmt::begin(ctx, *bt, chunk_frames, &js);
   if (rc != SFE_OK) return rc;
   rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
   if (rc != SFE_OK) return rc;
@@ -608,9 +654,9 @@ static int fe_run_jpeg(sfe_frontend *fe, JpegBatch *bt, const double *poses_host
   if (rc != SFE_OK) return rc;
   auto decode = [&](int f0, int k) -> int {
     const int n = std::min(chunk_frames, n_frames - f0);
-    int r = jpeg_decode_frames(ctx, js, *bt, f0, n, fe->frames + (size_t)f0 * fbytes);
+    int r = Fmt::decode(ctx, js, *bt, f0, n, fe->frames + (size_t)f0 * fbytes);
     if (r != SFE_OK) return r;
-    SFE_CUDA(cudaMemcpyAsync(st_host + f0, jpeg_status_dev(js) + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost,
+    SFE_CUDA(cudaMemcpyAsync(st_host + f0, Fmt::status_dev(js) + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost,
                              ctx->stream));
     SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
     return SFE_OK;
@@ -623,9 +669,9 @@ static int fe_run_jpeg(sfe_frontend *fe, JpegBatch *bt, const double *poses_host
     if (rc != SFE_OK) break;
     SFE_CUDA(cudaEventSynchronize(fe->ev_copy[k & 1]));
     for (int i = f0; i < f0 + n; ++i)
-      if (st_host[i] != SFE_JPEG_OK) {
+      if (st_host[i] != 0) {
         SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-        set_error("sfe_frontend_run_jpeg_host: frame %d: %s", i, sfe_jpeg_status_message(st_host[i]));
+        set_error("%s: frame %d: %s", what, i, Fmt::message(st_host[i]));
         return SFE_ERR_ARG;
       }
     rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
@@ -634,24 +680,25 @@ static int fe_run_jpeg(sfe_frontend *fe, JpegBatch *bt, const double *poses_host
   return rc;
 }
 
-int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
-                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
-                               int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
+template <class Fmt>
+static int fe_run_compressed_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                  const double *poses_host, int n_frames, int chunk_frames, float *T_host,
+                                  int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                                  int32_t *npoints_host, const char *what) {
   SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
-              "sfe_frontend_run_jpeg_host: null argument");
-  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_jpeg_host: %d frames exceed max_frames %d",
-              n_frames, fe->max_frames);
+              "%s: null argument", what);
+  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
+              fe->max_frames);
   for (int i = 0; i < n_frames; ++i)
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0,
-                "sfe_frontend_run_jpeg_host: offsets must be non-decreasing");
+    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "%s: offsets must be non-decreasing", what);
   if (n_frames == 0) return SFE_OK;
   sfe_ctx *ctx = fe->ctx;
   SFE_CUDA(cudaSetDevice(ctx->device));
   if (chunk_frames <= 0) chunk_frames = 256;
-  JpegBatch *bt;
-  int rc = jpeg_batch_parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
-  if (rc == SFE_OK) rc = fe_run_jpeg(fe, bt, poses_host, n_frames, chunk_frames);
-  jpeg_batch_free(bt);
+  typename Fmt::Batch *bt;
+  int rc = Fmt::parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
+  if (rc == SFE_OK) rc = fe_run_compressed<Fmt>(fe, bt, poses_host, n_frames, chunk_frames, what);
+  Fmt::free(bt);
   if (rc != SFE_OK) return rc;
   rc = fe_update_carry(fe, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
@@ -666,6 +713,22 @@ int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int
   }
   SFE_CUDA(cudaStreamSynchronize(ctx->stream));
   return SFE_OK;
+}
+
+extern "C" {
+
+int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
+                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
+                               int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
+  return fe_run_compressed_host<JpegFormat>(fe, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                                            inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
+}
+
+int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
+                              int n_frames, int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
+                              int32_t *status_host, int32_t *npoints_host) {
+  return fe_run_compressed_host<PngFormat>(fe, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                                           inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
 }
 
 }  // extern "C"

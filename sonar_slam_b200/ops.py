@@ -178,3 +178,16 @@ def decode_jpeg(streams, R, B, device=None, ctx=None):
     _lib.check(ctx.lib.sfe_jpeg_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
                                               _lib.ptr(st)), "sfe_jpeg_decode_to_dev")
     return out, st
+
+
+def decode_png(streams, R, B, device=None, ctx=None):
+    """decode_jpeg for PNG streams (include/sonarfe.h: sfe_png_decode_to_dev; sonar_slam_b200/png.py)."""
+    from . import jpeg
+    buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
+    n = len(off) - 1
+    ctx = ctx or context(device)
+    out = torch.empty((n, int(R), int(B)), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    st = np.empty(n, np.int32)
+    _lib.check(ctx.lib.sfe_png_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
+                                             _lib.ptr(st)), "sfe_png_decode_to_dev")
+    return out, st

@@ -59,6 +59,19 @@ class FrontEnd:
                                                        _lib.ptr(o["npoints"])), "sfe_frontend_run_jpeg_host")
         return o
 
+    def run_png_host(self, streams, poses, chunk_frames=256, out=None):
+        """run_jpeg_host for PNG streams (sfe_frontend_run_png_host)."""
+        from . import jpeg
+        buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
+        poses = np.ascontiguousarray(poses, np.float64)
+        n = len(off) - 1
+        o = out or self.alloc_results(n)
+        _lib.check(self.lib.sfe_frontend_run_png_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
+                                                      int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                                                      _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
+                                                      _lib.ptr(o["npoints"])), "sfe_frontend_run_png_host")
+        return o
+
     @staticmethod
     def alloc_results(n):
         return dict(T=np.empty((n, 3, 3), np.float32), iterations=np.empty(n, np.int32),

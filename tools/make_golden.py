@@ -412,8 +412,65 @@ def jpeg_fixture():
     print("jpeg_streams:", len(streams), "streams,", int(off[-1]), "bytes written to", out)
 
 
+def png_streams():
+    """(name, PNG bytes) of the PNG fixture: the writer's option grid on small images, the deflate edge cases, and a
+    few cv2-written pings."""
+    import cv2
+    from oracle import jpeg_ref, png_ref
+    out = []
+    strategies = list(png_ref.STRATEGIES)
+    for k, (h, w) in enumerate([(1, 1), (1, 17), (13, 1), (7, 9), (16, 16), (17, 33), (31, 29), (64, 48)]):
+        for j, content in enumerate(("synth", "noise", "checker", "zero", "full")):
+            img = jpeg_ref.contents(h, w, seed=k)[content]
+            i = k * 5 + j
+            rgb = i % 3 == 2
+            filters = [(y + i) % 5 for y in range(h)] if i % 2 else (i // 2) % 5
+            level = (0, 1, 6, 9)[i % 4]
+            strategy = strategies[i % len(strategies)]
+            idat = (None, 1, -7)[i % 3]
+            b = png_ref.write(png_ref.rgb_of(img) if rgb else img, filters, level, strategy, 9 if i % 5 == 0 else 15,
+                              idat)
+            out.append((f"{h}x{w}_{content}_{'rgb' if rgb else 'gray'}_f{i % 5}{'mix' if i % 2 else ''}_l{level}_"
+                        f"{strategy}_idat{idat}", b))
+    for name, (h, w, b) in png_ref.edge_streams().items():
+        out.append((name, b))
+    for seed in range(3):
+        img = jpeg_ref.contents(96, 80, seed=seed)["synth"]
+        out.append((f"96x80_cv2_seed{seed}", cv2.imencode(".png", img)[1].tobytes()))
+    out.append(("96x80_cv2_rgb", cv2.imencode(".png", png_ref.rgb_of(jpeg_ref.contents(96, 80)["synth"]))[1].tobytes()))
+    return out
+
+
+def png_fixture():
+    """tests/golden/png_streams.npz: PNG streams over the decoder's option grid with the SHA-256 of the gray image
+    cv2.imdecode(IMREAD_COLOR) + BGR2GRAY gives, and the OpenCV / libpng / zlib versions that produced them.  Needs only
+    cv2 (no reference tree)."""
+    import hashlib
+    import cv2
+    from oracle import png_ref
+    streams, names, digests, shapes = [], [], [], []
+    for name, b in png_streams():
+        gray = png_ref.cv2_gray(b)
+        streams.append(np.frombuffer(b, np.uint8))
+        names.append(name)
+        digests.append(hashlib.sha256(np.ascontiguousarray(gray).tobytes()).hexdigest())
+        shapes.append(gray.shape)
+    off = np.zeros(len(streams) + 1, np.int64)
+    off[1:] = np.cumsum([len(s) for s in streams])
+    out = os.path.join(REPO, "tests", "golden", "png_streams.npz")
+    info = cv2.getBuildInformation()
+    lines = {k: next((l.strip() for l in info.splitlines() if l.strip().startswith(k + ":")), "") for k in ("PNG", "ZLib")}
+    np.savez_compressed(out, bytes=np.concatenate(streams), offsets=off, names=np.array(names),
+                        sha256=np.array(digests), shapes=np.array(shapes, np.int32),
+                        cv2_version=np.array(cv2.__version__), libpng=np.array(lines["PNG"]),
+                        zlib=np.array(lines["ZLib"]))
+    print("png_streams:", len(streams), "streams,", int(off[-1]), "bytes written to", out)
+
+
 if __name__ == "__main__":
-    if "--only-jpeg" in sys.argv:
+    if "--only-png" in sys.argv:
+        png_fixture()
+    elif "--only-jpeg" in sys.argv:
         jpeg_fixture()
     elif "--only-fov" in sys.argv:
         fov_fixture()
@@ -424,3 +481,4 @@ if __name__ == "__main__":
         fov_fixture()
         cfar_reference_fixture()
         jpeg_fixture()
+        png_fixture()
