@@ -127,6 +127,19 @@ SFE_API int sfe_cart_points_dev(sfe_ctx *ctx, const sfe_maps *maps, const uint8_
 SFE_API int sfe_cart_points_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *mask_host, int n_frames,
                                  int capacity, int32_t *ij_host, float *xy_host, int32_t *count_host);
 
+/* ------------------------------------------------------------------ feature image
+ * feature_extraction.py:226-228: cv2.applyColorMap(cv2.remap(img, map_x, map_y, INTER_LINEAR), COLORMAP_JET), the
+ * bgr8 image the reference publishes on its feature-image topic, for n_frames uint8 polar frames [n][R][B] of the maps'
+ * geometry.  Output: uint8 [n][rows][cols][3], B, G, R = lut_bgr[v] where v is cv2.remap's 8-bit value (fixed-point
+ * bilinear on 1/32-px coordinates, constant-0 border; NaN, infinite or |map * 32| >= 1e9 coordinates give 0), bit for
+ * bit.  lut_bgr_host: uint8 [256][3] in HOST memory (COLORMAP_JET: sonar_slam_b200.feature_image.JET).
+ * Device flavour: asynchronous on the context's stream.  Host flavour: copies the frames in and the images out in
+ * chunks overlapped with the kernel and returns when the images are in out_host. */
+SFE_API int sfe_feature_image_dev(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *frames_dev, int n_frames,
+                                  const uint8_t *lut_bgr_host, uint8_t *out_dev);
+SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *frames_host, int n_frames,
+                                   const uint8_t *lut_bgr_host, uint8_t *out_host);
+
 /* ------------------------------------------------------------------ point-cloud filters
  * Clouds are packed: pts [total][dim] float32 (dim = 2: x,y; remove_outlier also takes 3: x,y,z),
  * off [n_clouds + 1] int32 offsets (cloud c = rows off[c] .. off[c+1]-1), n_max = largest cloud.
@@ -322,6 +335,16 @@ SFE_API int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, co
  * exactly as if the batches had been one call -- a replay can be fed in pieces of any size without a cold window at
  * every seam.  enable = 0 (the default) drops the carried frames: every call starts cold (frame 0 SFE_ICP_SKIPPED). */
 SFE_API int sfe_frontend_set_carry(sfe_frontend *fe, int enable);
+/* Feature images from the front end.  With dst != NULL, every later run call on this handle also writes frame i's
+ * feature image (as sfe_feature_image_dev, table lut_bgr_host, copied by this call) to dst + i * rows * cols * 3.
+ * sfe_frontend_run_dev needs dst in device memory (dst_is_host = 0; asynchronous like the rest of the call);
+ * sfe_frontend_run_host / _run_jpeg_host / _run_png_host need it in host memory (dst_is_host != 0): each chunk is
+ * rendered as soon as its frames are on the device, into a double-buffered device staging area (chunk_frames images,
+ * allocated on first use) that is copied out while later chunks compute, and the call returns after the last image has
+ * landed.  Pinned host memory lets the copies run asynchronously.  dst = NULL (the default) turns it off.  The numeric
+ * results are the same with and without images. */
+SFE_API int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_host, uint8_t *dst,
+                                            int dst_is_host);
 /* Optional per-stage device timing (CUDA events on the launch stream around every stage's kernels).
  * get_timing synchronises, adds the intervals recorded since the last call to running totals and
  * returns the totals: stage_ms[SFE_FE_STAGES], stage_calls[SFE_FE_STAGES] (may be NULL). */

@@ -131,6 +131,9 @@ _EXTRA_SIGNATURES = {
     "sfe_png_get_timing": [c_void_p, c_void_p, c_void_p],
     "sfe_frontend_run_png_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p],
+    "sfe_feature_image_dev": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
+    "sfe_feature_image_host": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
+    "sfe_frontend_set_feature_images": [c_void_p, c_void_p, c_void_p, c_int],
 }
 
 

@@ -12,7 +12,10 @@ field, and the sign convention of the hand-off -- (p0, p1) -> [p0, 0, p1] -> (x,
               OculusPing  -> gamma-corrected float32   utils/conversions.py:229-235
     pointcloud2_to_xyz_array(msg, remove_nans=True)    ros_numpy.point_cloud2 (slam_ros.py:169)
     feature_msg(ping, points) / keyframe_points(msg)   feature_extraction.py:181-190 / slam_ros.py:169-170
+    numpy_to_image(arr, encoding)                      ros_numpy.image (feature_extraction.py:228)
 """
+import sys
+
 import numpy as np
 
 
@@ -128,3 +131,47 @@ def keyframe_points(feature_message):
     """SLAMNode.SLAM_callback (slam_ros.py:169-170): the keyframe's 2-D cloud is (x, -z) of the message."""
     points = pointcloud2_to_xyz_array(feature_message)
     return np.c_[points[:, 0], -1 * points[:, 2]]
+
+
+class Image(object):
+    """sensor_msgs/Image (same attribute names, `data` = the message's byte string)."""
+    _type = "sensor_msgs/Image"
+    __slots__ = ("header", "height", "width", "encoding", "is_bigendian", "step", "data")
+
+    def __init__(self, encoding=""):
+        self.header = Header()
+        self.height, self.width, self.encoding, self.is_bigendian, self.step, self.data = 0, 0, encoding, False, 0, b""
+
+
+# ros_numpy.image.name_to_dtypes: encoding -> (element type, channels)
+IMAGE_ENCODINGS = {
+    "rgb8": (np.uint8, 3), "rgba8": (np.uint8, 4), "rgb16": (np.uint16, 3), "rgba16": (np.uint16, 4),
+    "bgr8": (np.uint8, 3), "bgra8": (np.uint8, 4), "bgr16": (np.uint16, 3), "bgra16": (np.uint16, 4),
+    "mono8": (np.uint8, 1), "mono16": (np.uint16, 1),
+    "8UC1": (np.uint8, 1), "8UC2": (np.uint8, 2), "8UC3": (np.uint8, 3), "8UC4": (np.uint8, 4),
+    "16UC1": (np.uint16, 1), "16UC3": (np.uint16, 3), "32FC1": (np.float32, 1), "32FC3": (np.float32, 3),
+}
+
+
+def numpy_to_image(arr, encoding):
+    """ros_numpy.image.numpy_to_image: a sensor_msgs/Image holding `arr` ([height, width] or [height, width,
+    channels]) with `encoding`; data is the C-contiguous bytes, step the row stride."""
+    if encoding not in IMAGE_ENCODINGS:
+        raise TypeError("Unrecognized encoding {}".format(encoding))
+    im = Image(encoding=encoding)
+    dtype_class, exp_channels = IMAGE_ENCODINGS[encoding]
+    if arr.ndim == 2:
+        im.height, im.width, channels = arr.shape + (1,)
+    elif arr.ndim == 3:
+        im.height, im.width, channels = arr.shape
+    else:
+        raise TypeError("Array must be two or three dimensional")
+    if exp_channels != channels:
+        raise TypeError("Array has {} channels, {} requires {}".format(channels, encoding, exp_channels))
+    if dtype_class != arr.dtype.type:
+        raise TypeError("Array is {}, {} requires {}".format(arr.dtype.type, encoding, dtype_class))
+    contig = np.ascontiguousarray(arr)
+    im.data = contig.tobytes()
+    im.step = contig.strides[0]
+    im.is_bigendian = arr.dtype.byteorder == ">" or (arr.dtype.byteorder == "=" and sys.byteorder == "big")
+    return im

@@ -14,7 +14,8 @@ gives the same single NaN point the reference publishes (feature_extraction.py:2
 The polar->Cartesian maps stay host-side numpy/scipy exactly as in the reference
 (generate_map_xy, :134-173, re-run only when the geometry changes); everything per ping runs on the
 GPU: CFAR with the amplitude gate fused (:223-224), the remap/nonzero/metres step (:231-238),
-pcl.downsample and pcl.remove_outlier (:241-249).
+pcl.downsample and pcl.remove_outlier (:241-249).  With `render_feature_img` the feature image the reference publishes
+(:226-228) is rendered on the GPU too.
 """
 import numpy as np
 from scipy.interpolate import interp1d
@@ -49,6 +50,10 @@ class FeatureExtraction(object):
         self.skip = 5
 
         self.feature_img = None
+        # opt-in: also render the bgr8 feature image the reference publishes (:226-228) into `feature_img`, and its
+        # sensor_msgs/Image mirror into `feature_img_msg`, on the GPU (sonar_slam_b200.feature_image)
+        self.render_feature_img = False
+        self.feature_img_msg = None
 
         # polar -> Cartesian remapping state (:59-70)
         self.res = None
@@ -197,8 +202,13 @@ class FeatureExtraction(object):
         _lib.check(ctx.lib.sfe_cfar_host(ctx.handle, _lib.ptr(img), 0, 1, R, B, _ALG[self.alg], int(train_hs),
                                          int(guard_hs), int(rank), float(tau), 1, float(self.threshold),
                                          _lib.ptr(mask), None), "FeatureExtraction: cfar")
-        # remap + nonzero + metres (:231-238)
         maps = self.device_maps(ctx, B)
+        if self.render_feature_img:  # cv2.remap(img) + applyColorMap(JET), published as bgr8 (:226-228)
+            from .. import feature_image
+            from . import conversions
+            self.feature_img = feature_image.render_host(maps, img, ctx=ctx)[0]
+            self.feature_img_msg = conversions.numpy_to_image(self.feature_img, "bgr8")
+        # remap + nonzero + metres (:231-238)
         cap = self.rows * self.cols
         ij = np.empty((cap, 2), np.int32)
         xy = np.empty((cap, 2), np.float32)

@@ -136,6 +136,12 @@ void sfe_ctx_destroy(sfe_ctx *ctx) {
   for (auto &b : ctx->stage_out)
     if (b.ptr) cudaFree(b.ptr);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
+  if (ctx->copy_stream) {
+    cudaStreamSynchronize(ctx->copy_stream);
+    cudaStreamDestroy(ctx->copy_stream);
+  }
+  for (auto ev : ctx->copy_ev)
+    if (ev) cudaEventDestroy(ev);
   if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }

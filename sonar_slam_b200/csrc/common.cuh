@@ -63,6 +63,8 @@ struct sfe_ctx {
   void (*jpeg_free)(void *) = nullptr;
   void *png = nullptr;                  // PNG decoder state (png.cu), created on first use
   void (*png_free)(void *) = nullptr;
+  cudaStream_t copy_stream = nullptr;   // host flavours that overlap copies with kernels (featx.cu), created on first use
+  cudaEvent_t copy_ev[4] = {};
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)

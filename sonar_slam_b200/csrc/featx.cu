@@ -19,6 +19,7 @@
 // and converted to metres with the reference's float64 expressions.
 //
 // One CTA handles FPB frames per pass over the table so the table is read once per FPB frames.
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -57,8 +58,10 @@ struct __align__(8) MapEntry {
   int16_t ix, iy;   // top-left tap (saturated like cv::saturate_cast<short>)
   uint8_t fx, fy;   // 1/32-pixel fractions
   uint8_t flags;    // bit 0: the pixel can reach weight 512 with in-image taps
+                    // bit 1: the map coordinate is NaN, infinite or |map * 32| >= 1e9: cv2.remap gives 0 there
   uint8_t pad;
 };
+constexpr uint8_t MAP_FIRES = 1, MAP_DEAD = 2;
 
 constexpr int FX_THREADS = 1024;
 constexpr int FXS_THREADS = 512;  // detection-driven variant
@@ -355,6 +358,95 @@ __global__ void __launch_bounds__(FX_THREADS)
   }
 }
 
+// ---------------------------------------------------------------------------- feature image
+// feature_extraction.py:226-227: cv2.remap(img, map_x, map_y, INTER_LINEAR) of the uint8 polar frame, then
+// cv2.applyColorMap(., COLORMAP_JET) -- here the caller's 256-entry BGR table.  The remap is cart_pixel_fires' fixed-point
+// rule on the full 8-bit frame: v = (32 * sum w_k img[tap_k] + 2^14) >> 15, taps outside the frame contribute 0, and a
+// MAP_DEAD entry gives 0, as cv2 does for such coordinates.
+//
+// A CTA owns FI_TILE consecutive Cartesian pixels of FI_FPB frames: it loads their table entries once, into registers,
+// and uses them for every frame.  Lanes take consecutive pixels, so a warp's tap gathers fall in a few polar rows (read
+// through the read-only path).  Each frame's tile is assembled in shared memory and written with coalesced 16-B
+// evict-first stores, three per thread: the images are written once and should not push the table and the frames out
+// of L2.
+constexpr int FI_THREADS = 256, FI_PPT = 16, FI_TILE = FI_THREADS * FI_PPT, FI_FPB = 8;
+struct FeatureLut {
+  uint8_t bgr[256 * 3];
+};
+
+__device__ __forceinline__ uint32_t remap_u8(uint2 e, const uint8_t *__restrict__ img, int R, int B) {
+  if ((e.y >> 16) & MAP_DEAD) return 0;
+  const int ix = (int16_t)(e.x & 0xffffu), iy = (int16_t)(e.x >> 16);
+  const int fx = e.y & 0xff, fy = (e.y >> 8) & 0xff;
+  const bool x0 = (unsigned)ix < (unsigned)B, x1 = (unsigned)(ix + 1) < (unsigned)B;
+  const bool y0 = (unsigned)iy < (unsigned)R, y1 = (unsigned)(iy + 1) < (unsigned)R;
+  const int v00 = (x0 && y0) ? __ldg(img + iy * B + ix) : 0, v01 = (x1 && y0) ? __ldg(img + iy * B + ix + 1) : 0;
+  const int v10 = (x0 && y1) ? __ldg(img + (iy + 1) * B + ix) : 0, v11 = (x1 && y1) ? __ldg(img + (iy + 1) * B + ix + 1) : 0;
+  const int sum = (32 - fx) * (32 - fy) * v00 + fx * (32 - fy) * v01 + (32 - fx) * fy * v10 + fx * fy * v11;
+  return (uint32_t)((32 * sum + (1 << 14)) >> 15);
+}
+
+__global__ void __launch_bounds__(FI_THREADS)
+    feature_image_kernel(const uint2 *__restrict__ tab, int npix, int R, int B, const uint8_t *__restrict__ frames,
+                         int F, int n_tiles, const FeatureLut lut, uint8_t *__restrict__ out) {
+  __shared__ uint32_t slut[256];  // B | G << 8 | R << 16
+  __shared__ __align__(16) uint8_t simg[FI_TILE * 3];
+  const int tid = threadIdx.x;
+  const int p0 = (blockIdx.x % n_tiles) * FI_TILE, f0 = (blockIdx.x / n_tiles) * FI_FPB;
+  const int np = min(FI_TILE, npix - p0), nf = min(FI_FPB, F - f0);
+  for (int i = tid; i < 256; i += FI_THREADS)
+    slut[i] = lut.bgr[3 * i] | (uint32_t)lut.bgr[3 * i + 1] << 8 | (uint32_t)lut.bgr[3 * i + 2] << 16;
+  uint2 e[FI_PPT];
+#pragma unroll
+  for (int k = 0; k < FI_PPT; ++k) {
+    const int p = k * FI_THREADS + tid;
+    e[k] = p < np ? __ldg(tab + p0 + p) : make_uint2(0u, (uint32_t)MAP_DEAD << 16);
+  }
+  __syncthreads();
+  const size_t img_bytes = (size_t)npix * 3;
+  for (int j = 0; j < nf; ++j) {
+    const uint8_t *img = frames + (size_t)(f0 + j) * R * B;
+#pragma unroll
+    for (int k = 0; k < FI_PPT; ++k) {
+      const int p = k * FI_THREADS + tid;
+      const uint32_t c = slut[remap_u8(e[k], img, R, B)];
+      simg[3 * p] = (uint8_t)c, simg[3 * p + 1] = (uint8_t)(c >> 8), simg[3 * p + 2] = (uint8_t)(c >> 16);
+    }
+    __syncthreads();
+    uint8_t *dst = out + (size_t)(f0 + j) * img_bytes + (size_t)p0 * 3;
+    if (np == FI_TILE && ((uintptr_t)dst & 15) == 0) {
+      const uint4 *s = reinterpret_cast<const uint4 *>(simg);
+      uint4 *d = reinterpret_cast<uint4 *>(dst);
+#pragma unroll
+      for (int q = 0; q < 3; ++q) __stcs(d + q * FI_THREADS + tid, s[q * FI_THREADS + tid]);
+    } else {  // the last tile of a frame, or a frame base that is not 16-B aligned (rows * cols * 3 % 16 != 0)
+      for (int b = tid; b < np * 3; b += FI_THREADS) dst[b] = simg[b];
+    }
+    __syncthreads();
+  }
+}
+
+int feature_image_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames, int F, const uint8_t *lut_bgr,
+                      uint8_t *out, const char *what) {
+  SFE_REQUIRE(ctx && m, "%s: null context or maps", what);
+  SFE_REQUIRE(ctx->device == m->device, "%s: maps were created on device %d, context is on %d", what, m->device,
+              ctx->device);
+  SFE_REQUIRE(F >= 0, "%s: negative frame count", what);
+  if (F == 0) return SFE_OK;
+  SFE_REQUIRE(frames && lut_bgr && out, "%s: null frames, table or output pointer", what);
+  SFE_REQUIRE((long long)m->R * m->B < (1ll << 31), "%s: a %d x %d polar frame is too large", what, m->R, m->B);
+  const int npix = m->rows * m->cols, n_tiles = (npix + FI_TILE - 1) / FI_TILE;
+  const long long grid = (long long)n_tiles * (((long long)F + FI_FPB - 1) / FI_FPB);
+  SFE_REQUIRE(grid <= 0x7fffffffll, "%s: %d frames of %d x %d are too many for one call", what, F, m->rows, m->cols);
+  FeatureLut lut;
+  memcpy(lut.bgr, lut_bgr, sizeof(lut.bgr));
+  feature_image_kernel<<<(unsigned)grid, FI_THREADS, 0, ctx->stream>>>((const uint2 *)m->table, npix, m->R, m->B,
+                                                                        frames, F, n_tiles, lut, out);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return SFE_OK;
+}
+
 static bool ctx_force_gather(const sfe_ctx *) {
   const char *e = getenv("SFE_CART_DENSE");  // development switch: force the dense kernel
   return e && e[0] == '1';
@@ -436,7 +528,9 @@ static void build_map_table(const float *map_x_host, const float *map_y_host, in
       const int reach = (x0 && y0 ? (32 - fx) * (32 - fy) : 0) + (x1 && y0 ? fx * (32 - fy) : 0) +
                         (x0 && y1 ? (32 - fx) * fy : 0) + (x1 && y1 ? fx * fy : 0);
       e.ix = (int16_t)ix, e.iy = (int16_t)iy, e.fx = (uint8_t)fx, e.fy = (uint8_t)fy;
-      e.flags = reach >= 512 ? 1 : 0;
+      e.flags = reach >= 512 ? MAP_FIRES : 0;
+    } else {
+      e.flags = MAP_DEAD;
     }
     tab[p] = e;
   }
@@ -616,6 +710,77 @@ int sfe_cart_points_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *mask
       return SFE_ERR_CAPACITY;
     }
   return SFE_OK;
+}
+
+int sfe_feature_image_dev(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *frames_dev, int n_frames,
+                          const uint8_t *lut_bgr_host, uint8_t *out_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_feature_image_dev: null context");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  return feature_image_run(ctx, maps, frames_dev, n_frames, lut_bgr_host, out_dev, "sfe_feature_image_dev");
+}
+
+// Chunks of FI_HOST_CHUNK frames: the copies in and out run on the context's copy stream, in the order
+// in(0) in(1) out(0) in(2) out(1) ..., so the kernel of chunk k overlaps the copy-out of chunk k-1 and the copy-in of
+// chunk k+1.  Staging is double-buffered both ways.
+constexpr int FI_HOST_CHUNK = 16;
+
+static int feature_image_host(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames_host, int n,
+                              const uint8_t *lut_bgr, uint8_t *out_host) {
+  const char *what = "sfe_feature_image_host";
+  const size_t fbytes = (size_t)m->R * m->B, ibytes = (size_t)m->rows * m->cols * 3;
+  const int chunk = n < FI_HOST_CHUNK ? n : FI_HOST_CHUNK;
+  int rc;
+  for (int b = 0; b < 2; ++b) {
+    if ((rc = ensure(ctx, ctx->stage_in[b], chunk * fbytes)) != SFE_OK) return rc;
+    if ((rc = ensure(ctx, ctx->stage_out[b], chunk * ibytes)) != SFE_OK) return rc;
+  }
+  if (!ctx->copy_stream) SFE_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+  for (auto &ev : ctx->copy_ev)
+    if (!ev) SFE_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  cudaEvent_t *in_done = ctx->copy_ev, *kernel_done = ctx->copy_ev + 2;
+  // the staging buffers are allocated (and may be still in use) in the launch stream's order
+  SFE_CUDA(cudaEventRecord(kernel_done[1], ctx->stream));
+  SFE_CUDA(cudaStreamWaitEvent(ctx->copy_stream, kernel_done[1], 0));
+  const int n_chunks = (n + chunk - 1) / chunk;
+  auto copy_in = [&](int k) -> int {
+    const int f0 = k * chunk, nf = std::min(chunk, n - f0);
+    if (k >= 2) SFE_CUDA(cudaStreamWaitEvent(ctx->copy_stream, kernel_done[k & 1], 0));  // kernel k-2 read the buffer
+    SFE_CUDA(cudaMemcpyAsync(ctx->stage_in[k & 1].ptr, frames_host + f0 * fbytes, nf * fbytes, cudaMemcpyHostToDevice,
+                             ctx->copy_stream));
+    SFE_CUDA(cudaEventRecord(in_done[k & 1], ctx->copy_stream));
+    return SFE_OK;
+  };
+  if ((rc = copy_in(0)) != SFE_OK) return rc;
+  for (int k = 0; k < n_chunks; ++k) {
+    const int f0 = k * chunk, nf = std::min(chunk, n - f0);
+    if (k + 1 < n_chunks && (rc = copy_in(k + 1)) != SFE_OK) return rc;
+    // the copy-out of chunk k-2 (enqueued on the copy stream before in_done[k]) has drained this output buffer
+    SFE_CUDA(cudaStreamWaitEvent(ctx->stream, in_done[k & 1], 0));
+    rc = feature_image_run(ctx, m, (const uint8_t *)ctx->stage_in[k & 1].ptr, nf, lut_bgr,
+                           (uint8_t *)ctx->stage_out[k & 1].ptr, what);
+    if (rc != SFE_OK) return rc;
+    SFE_CUDA(cudaEventRecord(kernel_done[k & 1], ctx->stream));
+    SFE_CUDA(cudaStreamWaitEvent(ctx->copy_stream, kernel_done[k & 1], 0));
+    SFE_CUDA(cudaMemcpyAsync(out_host + f0 * ibytes, ctx->stage_out[k & 1].ptr, nf * ibytes, cudaMemcpyDeviceToHost,
+                             ctx->copy_stream));
+  }
+  return SFE_OK;
+}
+
+int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *frames_host, int n_frames,
+                           const uint8_t *lut_bgr_host, uint8_t *out_host) {
+  SFE_REQUIRE(ctx && maps, "sfe_feature_image_host: null context or maps");
+  SFE_REQUIRE(ctx->device == maps->device, "sfe_feature_image_host: maps were created on device %d, context is on %d",
+              maps->device, ctx->device);
+  SFE_REQUIRE(n_frames >= 0, "sfe_feature_image_host: negative frame count");
+  if (n_frames == 0) return SFE_OK;
+  SFE_REQUIRE(frames_host && lut_bgr_host && out_host, "sfe_feature_image_host: null frames, table or output pointer");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  const int rc = feature_image_host(ctx, maps, frames_host, n_frames, lut_bgr_host, out_host);
+  // copies already enqueued finish before the call returns, also on an error
+  if (ctx->copy_stream) SFE_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+  return rc;
 }
 
 }  // extern "C"

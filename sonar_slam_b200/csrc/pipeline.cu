@@ -23,6 +23,8 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
              double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
 int cart_points_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
                     int32_t *ij, float *xy, int32_t *count);
+int feature_image_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames, int F, const uint8_t *lut_bgr,
+                      uint8_t *out, const char *what);
 int downsample_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
                    float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split = 0);
 int remove_outlier_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
@@ -197,6 +199,14 @@ struct sfe_frontend {
   double *carry_poses;   // host [window][3]
   cudaStream_t copy_stream;
   cudaEvent_t ev_copy[2], ev_done;
+  // feature images (sfe_frontend_set_feature_images)
+  uint8_t img_lut[256 * 3];
+  uint8_t *img_dst;      // null: off
+  int img_dst_host;
+  uint8_t *img_stage[2];  // host flavours: [img_stage_frames][rows][cols][3] each
+  int img_stage_frames;
+  cudaStream_t img_stream;  // copies the images out, next to the frame copies of copy_stream
+  cudaEvent_t ev_img_ready[2], ev_img_copied[2];
   // optional per-stage timing (CUDA events on the launch stream)
   int timing;
   std::vector<cudaEvent_t> *tev;    // pool
@@ -337,6 +347,15 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   for (auto &ev : fe->ev_copy)
     if (ev) cudaEventDestroy(ev);
   if (fe->ev_done) cudaEventDestroy(fe->ev_done);
+  if (fe->img_stream) {
+    cudaStreamSynchronize(fe->img_stream);
+    cudaStreamDestroy(fe->img_stream);
+  }
+  for (int k = 0; k < 2; ++k) {
+    if (fe->img_stage[k]) cudaFree(fe->img_stage[k]);
+    if (fe->ev_img_ready[k]) cudaEventDestroy(fe->ev_img_ready[k]);
+    if (fe->ev_img_copied[k]) cudaEventDestroy(fe->ev_img_copied[k]);
+  }
   if (fe->tev) {
     for (auto e : *fe->tev) cudaEventDestroy(e);
     delete fe->tev;
@@ -344,6 +363,59 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   delete fe->tstage;
   delete fe;
 }
+
+// Feature images of the host flavours.  fe_images_begin checks the destination and sizes the staging buffers;
+// fe_render_chunk renders frames [f0, f0 + n) of fe->frames (on the device by now) into staging buffer k & 1 and copies
+// them out on img_stream; the render of chunk k waits for the copy-out of chunk k - 2, which used the same buffer.
+static int fe_images_begin(sfe_frontend *fe, int n_frames, int chunk_frames, const char *what) {
+  if (!fe->img_dst) return SFE_OK;
+  SFE_REQUIRE(fe->img_dst_host, "%s: feature images are set to go to device memory; this flavour writes them to host "
+              "memory (sfe_frontend_set_feature_images with dst_is_host != 0)", what);
+  const int want = std::min(chunk_frames, n_frames);
+  if (fe->img_stage_frames >= want) return SFE_OK;
+  const size_t ib = (size_t)fe->maps->rows * fe->maps->cols * 3;
+  if (!fe->img_stream) {
+    SFE_CUDA(cudaStreamCreateWithFlags(&fe->img_stream, cudaStreamNonBlocking));
+    for (int k = 0; k < 2; ++k) {
+      SFE_CUDA(cudaEventCreateWithFlags(&fe->ev_img_ready[k], cudaEventDisableTiming));
+      SFE_CUDA(cudaEventCreateWithFlags(&fe->ev_img_copied[k], cudaEventDisableTiming));
+    }
+  }
+  SFE_CUDA(cudaStreamSynchronize(fe->ctx->stream));
+  SFE_CUDA(cudaStreamSynchronize(fe->img_stream));
+  fe->img_stage_frames = 0;
+  for (int k = 0; k < 2; ++k) {
+    if (fe->img_stage[k]) SFE_CUDA(cudaFree(fe->img_stage[k]));
+    fe->img_stage[k] = nullptr;
+  }
+  for (int k = 0; k < 2; ++k) SFE_CUDA(cudaMalloc((void **)&fe->img_stage[k], (size_t)want * ib));
+  fe->img_stage_frames = want;
+  return SFE_OK;
+}
+
+static int fe_render_chunk(sfe_frontend *fe, int f0, int n, int k, const char *what) {
+  if (!fe->img_dst) return SFE_OK;
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B, ib = (size_t)fe->maps->rows * fe->maps->cols * 3;
+  uint8_t *stage = fe->img_stage[k & 1];
+  SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_img_copied[k & 1], 0));
+  int rc = feature_image_run(ctx, fe->maps, fe->frames + (size_t)f0 * fbytes, n, fe->img_lut, stage, what);
+  if (rc != SFE_OK) return rc;
+  SFE_CUDA(cudaEventRecord(fe->ev_img_ready[k & 1], ctx->stream));
+  SFE_CUDA(cudaStreamWaitEvent(fe->img_stream, fe->ev_img_ready[k & 1], 0));
+  SFE_CUDA(cudaMemcpyAsync(fe->img_dst + (size_t)f0 * ib, stage, (size_t)n * ib, cudaMemcpyDeviceToHost,
+                           fe->img_stream));
+  SFE_CUDA(cudaEventRecord(fe->ev_img_copied[k & 1], fe->img_stream));
+  return SFE_OK;
+}
+
+// A host flavour returns only after the image copies it enqueued have landed, on every path.
+struct ImagesDrained {
+  const sfe_frontend *fe;
+  ~ImagesDrained() {
+    if (fe->img_dst && fe->img_stream) cudaStreamSynchronize(fe->img_stream);
+  }
+};
 
 // window transforms + guesses from the odometry poses (host, double), uploaded as float32.  With carried frames the
 // pose sequence is (carried poses ++ this batch's poses): frame i of the batch is virtual frame v = carry_n + i, its
@@ -526,6 +598,15 @@ int sfe_frontend_set_carry(sfe_frontend *fe, int enable) {
   return SFE_OK;
 }
 
+int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_host, uint8_t *dst, int dst_is_host) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_feature_images: null handle");
+  SFE_REQUIRE(dst == nullptr || lut_bgr_host != nullptr, "sfe_frontend_set_feature_images: null colour table");
+  if (dst) memcpy(fe->img_lut, lut_bgr_host, sizeof(fe->img_lut));
+  fe->img_dst = dst;
+  fe->img_dst_host = dst_is_host != 0;
+  return SFE_OK;
+}
+
 int sfe_frontend_set_timing(sfe_frontend *fe, int enable) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_timing: null handle");
   fe->timing = enable != 0;
@@ -559,10 +640,16 @@ int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const doub
   SFE_REQUIRE(fe && frames_dev && poses_host, "sfe_frontend_run_dev: null argument");
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_dev: %d frames exceed max_frames %d",
               n_frames, fe->max_frames);
+  SFE_REQUIRE(!fe->img_dst || !fe->img_dst_host, "sfe_frontend_run_dev: feature images are set to go to host memory; "
+              "this flavour writes them to device memory (sfe_frontend_set_feature_images with dst_is_host = 0)");
   if (n_frames == 0) return SFE_OK;
   SFE_CUDA(cudaSetDevice(fe->ctx->device));
   int rc = fe_upload_poses(fe, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
+  if (fe->img_dst) {
+    rc = feature_image_run(fe->ctx, fe->maps, frames_dev, n_frames, fe->img_lut, fe->img_dst, "sfe_frontend_run_dev");
+    if (rc != SFE_OK) return rc;
+  }
   rc = fe_features(fe, frames_dev, 0, n_frames);
   if (rc != SFE_OK) return rc;
   rc = fe_match(fe, 0, n_frames);
@@ -598,7 +685,10 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
   SFE_CUDA(cudaSetDevice(ctx->device));
   const size_t fbytes = (size_t)fe->p.R * fe->p.B;
   if (chunk_frames <= 0) chunk_frames = 256;
-  int rc0 = fe_upload_poses(fe, poses_host, n_frames);
+  int rc0 = fe_images_begin(fe, n_frames, chunk_frames, "sfe_frontend_run_host");
+  if (rc0 != SFE_OK) return rc0;
+  ImagesDrained drained{fe};
+  rc0 = fe_upload_poses(fe, poses_host, n_frames);
   if (rc0 != SFE_OK) return rc0;
   // frame chunks stream in on the copy stream; the feature stages of chunk k run while chunk k+1 copies
   int k = 0;
@@ -608,7 +698,9 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
                              cudaMemcpyHostToDevice, fe->copy_stream));
     SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
     SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
-    int rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
+    int rc = fe_render_chunk(fe, f0, n, k, "sfe_frontend_run_host");
+    if (rc != SFE_OK) return rc;
+    rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
     if (rc != SFE_OK) return rc;
     rc = fe_match(fe, f0, n);  // its window only reaches back into chunks already processed
     if (rc != SFE_OK) return rc;
@@ -674,7 +766,8 @@ static int fe_run_compressed(sfe_frontend *fe, typename Fmt::Batch *bt, const do
         set_error("%s: frame %d: %s", what, i, Fmt::message(st_host[i]));
         return SFE_ERR_ARG;
       }
-    rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
+    rc = fe_render_chunk(fe, f0, n, k, what);
+    if (rc == SFE_OK) rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
     if (rc == SFE_OK) rc = fe_match(fe, f0, n);
   }
   return rc;
@@ -695,8 +788,11 @@ static int fe_run_compressed_host(sfe_frontend *fe, const uint8_t *bytes, const 
   sfe_ctx *ctx = fe->ctx;
   SFE_CUDA(cudaSetDevice(ctx->device));
   if (chunk_frames <= 0) chunk_frames = 256;
+  int rc = fe_images_begin(fe, n_frames, chunk_frames, what);
+  if (rc != SFE_OK) return rc;
+  ImagesDrained drained{fe};
   typename Fmt::Batch *bt;
-  int rc = Fmt::parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
+  rc = Fmt::parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
   if (rc == SFE_OK) rc = fe_run_compressed<Fmt>(fe, bt, poses_host, n_frames, chunk_frames, what);
   Fmt::free(bt);
   if (rc != SFE_OK) return rc;

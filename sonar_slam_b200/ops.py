@@ -191,3 +191,25 @@ def decode_png(streams, R, B, device=None, ctx=None):
     _lib.check(ctx.lib.sfe_png_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
                                              _lib.ptr(st)), "sfe_png_decode_to_dev")
     return out, st
+
+
+def feature_image(frames, maps, lut=None, ctx=None):
+    """Feature images (feature_extraction.py:226-228: cv2.remap + applyColorMap(JET)) of polar frames on the device
+    (include/sonarfe.h: sfe_feature_image_dev; sonar_slam_b200/feature_image.py).  frames: uint8 [n, R, B] (or [R, B])
+    cuda tensor of the maps' geometry; lut: uint8 [256, 3] BGR table (default feature_image.JET).
+    Returns a uint8 [n, rows, cols, 3] bgr8 cuda tensor."""
+    from . import feature_image as fimg
+    if not frames.is_cuda or frames.dtype != torch.uint8:
+        raise _lib.SonarFEError("ops.feature_image: frames must be a CUDA uint8 tensor")
+    if frames.dim() == 2:
+        frames = frames.unsqueeze(0)
+    if frames.dim() != 3 or tuple(frames.shape[1:]) != (maps.R, maps.B):
+        raise ValueError(f"ops.feature_image: frames must be [n, {maps.R}, {maps.B}] for these maps, "
+                         f"got {tuple(frames.shape)}")
+    frames = frames.contiguous()
+    lut = fimg.lut_array(fimg.JET if lut is None else lut)
+    ctx = ctx or context(frames.device)
+    out = torch.empty((frames.shape[0], maps.rows, maps.cols, 3), dtype=torch.uint8, device=frames.device)
+    _lib.check(ctx.lib.sfe_feature_image_dev(ctx.handle, maps.handle, _dp(frames), frames.shape[0], _lib.ptr(lut),
+                                             _dp(out)), "sfe_feature_image_dev")
+    return out

@@ -5,6 +5,7 @@ in host memory (`run_host`, the end-to-end path: frames are copied in chunks ove
 kernels) or already on the device (`run_dev`).  See csrc/pipeline.cu for what is computed and how
 it maps onto the reference's FeatureExtraction.callback / SLAM.add_sequential_scan_matching.
 """
+import contextlib
 import ctypes
 
 import numpy as np
@@ -31,45 +32,80 @@ class FrontEnd:
                                                 ctypes.byref(h)), "sfe_frontend_create")
         self.handle = h
 
-    def run_host(self, frames, poses, chunk_frames=256, out=None):
+    @contextlib.contextmanager
+    def _images(self, images, n, on_device, lut):
+        """Feature images of the frames of one run call (sfe_frontend_set_feature_images), off again afterwards.
+        images: uint8 [n, rows, cols, 3] C-contiguous -- a numpy array for the host flavours, a CUDA tensor on the
+        context's device for run_dev; lut: uint8 [256, 3] BGR table (default feature_image.JET)."""
+        if images is None:
+            yield
+            return
+        from . import feature_image
+        shape = (n, self.maps.rows, self.maps.cols, 3)
+        if on_device:
+            import torch
+            if not (isinstance(images, torch.Tensor) and images.is_cuda and images.dtype == torch.uint8
+                    and tuple(images.shape) == shape and images.is_contiguous()):
+                raise ValueError(f"FrontEnd.run_dev: images must be a contiguous CUDA uint8 tensor {list(shape)}")
+            dst = images.data_ptr()
+        else:
+            if not (isinstance(images, np.ndarray) and images.dtype == np.uint8 and images.shape == shape
+                    and images.flags["C_CONTIGUOUS"] and images.flags["WRITEABLE"]):
+                raise ValueError(f"FrontEnd: images must be a writeable C-contiguous uint8 numpy array {list(shape)}")
+            dst = images.ctypes.data
+        lut = feature_image.lut_array(feature_image.JET if lut is None else lut)
+        _lib.check(self.lib.sfe_frontend_set_feature_images(self.handle, _lib.ptr(lut), ctypes.c_void_p(dst),
+                                                            0 if on_device else 1), "sfe_frontend_set_feature_images")
+        try:
+            yield
+        finally:
+            self.lib.sfe_frontend_set_feature_images(self.handle, None, None, 0)
+
+    def run_host(self, frames, poses, chunk_frames=256, out=None, images=None, image_lut=None):
         """frames: uint8 [n,R,B] numpy (pinned memory gives full copy bandwidth); poses: float64 [n,3].
-        Returns dict(T [n,3,3] f32, iterations, inliers, status, npoints)."""
+        Returns dict(T [n,3,3] f32, iterations, inliers, status, npoints).  images: an optional uint8
+        [n, rows, cols, 3] numpy array that receives every frame's feature image (feature_image.py; colour table
+        image_lut, default JET); the results are the same with and without it."""
         frames = np.ascontiguousarray(frames, np.uint8)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(frames)
         o = out or self.alloc_results(n)
-        _lib.check(self.lib.sfe_frontend_run_host(self.handle, _lib.ptr(frames), _lib.ptr(poses), n,
-                                                  int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                  _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                  _lib.ptr(o["npoints"])), "sfe_frontend_run_host")
+        with self._images(images, n, False, image_lut):
+            _lib.check(self.lib.sfe_frontend_run_host(self.handle, _lib.ptr(frames), _lib.ptr(poses), n,
+                                                      int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                                                      _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
+                                                      _lib.ptr(o["npoints"])), "sfe_frontend_run_host")
         return o
 
-    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None):
+    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None):
         """run_host on compressed pings: streams is a sequence of JPEG bytes objects (or (bytes, offsets) from
         jpeg.pack); the compressed bytes are copied and decoded on the device instead of copying raw frames
-        (sfe_frontend_run_jpeg_host).  A stream that is rejected or fails to decode raises, naming the frame."""
+        (sfe_frontend_run_jpeg_host).  A stream that is rejected or fails to decode raises, naming the frame.
+        images / image_lut: as run_host."""
         from . import jpeg
         buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
         o = out or self.alloc_results(n)
-        _lib.check(self.lib.sfe_frontend_run_jpeg_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
-                                                       int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                       _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                       _lib.ptr(o["npoints"])), "sfe_frontend_run_jpeg_host")
+        with self._images(images, n, False, image_lut):
+            _lib.check(self.lib.sfe_frontend_run_jpeg_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
+                                                           int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                                                           _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
+                                                           _lib.ptr(o["npoints"])), "sfe_frontend_run_jpeg_host")
         return o
 
-    def run_png_host(self, streams, poses, chunk_frames=256, out=None):
+    def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None):
         """run_jpeg_host for PNG streams (sfe_frontend_run_png_host)."""
         from . import jpeg
         buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
         o = out or self.alloc_results(n)
-        _lib.check(self.lib.sfe_frontend_run_png_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
-                                                      int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                      _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                      _lib.ptr(o["npoints"])), "sfe_frontend_run_png_host")
+        with self._images(images, n, False, image_lut):
+            _lib.check(self.lib.sfe_frontend_run_png_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
+                                                          int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                                                          _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
+                                                          _lib.ptr(o["npoints"])), "sfe_frontend_run_png_host")
         return o
 
     @staticmethod
@@ -77,11 +113,13 @@ class FrontEnd:
         return dict(T=np.empty((n, 3, 3), np.float32), iterations=np.empty(n, np.int32),
                     inliers=np.empty(n, np.int32), status=np.empty(n, np.int32), npoints=np.empty(n, np.int32))
 
-    def run_dev(self, frames_ptr, poses, n):
-        """frames_ptr: device address of uint8 [n,R,B]; poses: float64 [n,3] numpy (host).  Asynchronous."""
+    def run_dev(self, frames_ptr, poses, n, images=None, image_lut=None):
+        """frames_ptr: device address of uint8 [n,R,B]; poses: float64 [n,3] numpy (host).  Asynchronous.
+        images: an optional uint8 [n, rows, cols, 3] CUDA tensor that receives every frame's feature image."""
         poses = np.ascontiguousarray(poses, np.float64)
-        _lib.check(self.lib.sfe_frontend_run_dev(self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(poses),
-                                                 int(n)), "sfe_frontend_run_dev")
+        with self._images(images, int(n), True, image_lut):
+            _lib.check(self.lib.sfe_frontend_run_dev(self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(poses),
+                                                         int(n)), "sfe_frontend_run_dev")
 
     def results_dev(self):
         """Device addresses of the last run's results: dict(T, iterations, inliers, status, cloud_xy,

@@ -30,6 +30,8 @@ Fixtures written:
   tests/golden/cfar_reference.json  per-algorithm mask / threshold-image digests and detection counts of the
                                     unmodified cfar.cpp (oracle/_ref) on the inputs of
                                     tests/test_oracle_cfar.py (--only-cfar-reference)
+  tests/golden/feature_img.npz      the feature image FeatureExtraction.callback publishes (feature_extraction.py:
+                                    226-228) for the config-1 ping, both bearing tables (--only-feature-img)
   tests/golden/globalinit.npz       SLAM.get_matching_cost_subroutine1 (slam.py:461-570) run
                                     unmodified on a synthetic source/target pair: the dilated
                                     target grid (packed) and the cost of 96 candidate poses.
@@ -467,8 +469,52 @@ def png_fixture():
     print("png_streams:", len(streams), "streams,", int(off[-1]), "bytes written to", out)
 
 
+def feature_img_fixture():
+    """tests/golden/feature_img.npz: the reference's own FeatureExtraction.callback on the config-1 ping for both
+    bearing tables, with ros_numpy.image.numpy_to_image patched to capture the bgr8 image it publishes (:226-228).
+    Stored: its SHA-256, shape and a sample, the digests of the maps it was made from, and the versions that wrote it."""
+    import cv2
+    from sonar_slam_b200 import synth
+    _install_reference()
+    fe_mod = importlib.import_module("bruce_slam.feature_extraction")
+    img = synth.make_frame(seed=1)
+    res = {}
+    for tag, bearings in [("uniform", synth.bearings_uniform(512)), ("oculus", synth.bearings_oculus(512))]:
+        fe = fe_mod.FeatureExtraction()
+        fe.Ntc, fe.Ngc, fe.Pfa, fe.rank, fe.alg = 40, 10, 0.1, 10, "SOCA"
+        fe.threshold, fe.resolution, fe.skip = 65, 0.5, 1
+        fe.outlier_filter_radius, fe.outlier_filter_min_points = 1.0, 5
+        fe.compressed_images = False
+        fe.feature_img_pub = mock.MagicMock()
+        fe.feature_pub = mock.MagicMock()
+        fe.configure()
+        captured = []
+
+        def to_image(arr, encoding):
+            captured.append((np.array(arr), encoding))
+            return mock.MagicMock()
+        msg = types.SimpleNamespace(ping_id=0, ping=img, range_resolution=30.0 / 512, num_ranges=512,
+                                    bearings=list(bearings), header=mock.MagicMock())
+        with mock.patch.object(fe_mod.ros_numpy.image, "image_to_numpy", lambda x: x), \
+                mock.patch.object(fe_mod.ros_numpy.image, "numpy_to_image", to_image):
+            fe.callback(msg)
+        (vis, encoding), = captured
+        assert encoding == "bgr8" and vis.dtype == np.uint8 and vis.shape == (fe.rows, fe.cols, 3), vis.shape
+        res[tag + "_shape"] = np.array(vis.shape, np.int64)
+        res[tag + "_sha256"] = np.array(_digest(vis))
+        res[tag + "_sample"] = vis[::17, ::23].copy()
+        res[tag + "_map_x_sha256"] = np.array(_digest(fe.map_x))
+        res[tag + "_map_y_sha256"] = np.array(_digest(fe.map_y))
+        print(tag, "feature image", vis.shape, _digest(vis)[:16])
+    out = os.path.join(REPO, "tests", "golden", "feature_img.npz")
+    np.savez_compressed(out, cv2_version=np.array(cv2.__version__), numpy_version=np.array(np.__version__), **res)
+    print("feature_img written to", out)
+
+
 if __name__ == "__main__":
-    if "--only-png" in sys.argv:
+    if "--only-feature-img" in sys.argv:
+        feature_img_fixture()
+    elif "--only-png" in sys.argv:
         png_fixture()
     elif "--only-jpeg" in sys.argv:
         jpeg_fixture()
@@ -482,3 +528,4 @@ if __name__ == "__main__":
         cfar_reference_fixture()
         jpeg_fixture()
         png_fixture()
+        feature_img_fixture()
