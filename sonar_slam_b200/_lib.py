@@ -101,6 +101,7 @@ _EXTRA_SIGNATURES = {
     "sfe_frontend_create": [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(c_void_p)],
     "sfe_frontend_set_timing": [c_void_p, c_int],
     "sfe_frontend_set_carry": [c_void_p, c_int],
+    "sfe_frontend_set_overlap": [c_void_p, c_int],
     "sfe_frontend_get_timing": [c_void_p, c_void_p, c_void_p],
     "sfe_frontend_run_dev": [c_void_p, c_void_p, c_void_p, c_int],
     "sfe_frontend_results_dev": [c_void_p] + [ctypes.POINTER(c_void_p)] * 6 + [ctypes.POINTER(ctypes.c_int32)],

@@ -19,14 +19,16 @@ void set_error(const char *fmt, ...) {
   va_end(ap);
 }
 
-int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes) {
+int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes) { return ensure(ctx, b, bytes, ctx->stream); }
+
+int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes, cudaStream_t stream) {
   if (bytes <= b.cap) return SFE_OK;
   // grow-only; the old block may still be in use by enqueued work -> stream-ordered free
-  if (b.ptr) SFE_CUDA(cudaFreeAsync(b.ptr, ctx->stream));
+  if (b.ptr) SFE_CUDA(cudaFreeAsync(b.ptr, stream));
   if (b.ptr == ctx->cfar_lut_buf) ctx->cfar_lut_buf = nullptr;  // the cached table went with the block
   b.ptr = nullptr, b.cap = 0;
   size_t want = bytes + bytes / 4 + 256;
-  SFE_CUDA(cudaMallocAsync(&b.ptr, want, ctx->stream));
+  SFE_CUDA(cudaMallocAsync(&b.ptr, want, stream));
   b.cap = want;
   return SFE_OK;
 }
@@ -73,8 +75,8 @@ int encode_tensor_map_3d(CUtensorMap *map, CUtensorMapDataType dt, size_t es, co
   return SFE_OK;
 }
 
-int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int alg, int T, int G, int k,
-             double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
+int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
+             int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
 
 }  // namespace sfe
 
@@ -119,6 +121,13 @@ int sfe_ctx_create(int device, void *cuda_stream, int own_stream, sfe_ctx **out)
     }
     ctx->owns_stream = true;
   }
+  if (cudaMalloc((void **)&ctx->work, SFE_WORK_COUNTERS * sizeof(int)) != cudaSuccess) {
+    set_error("sfe_ctx_create: cudaMalloc of the work counters failed");
+    (void)cudaGetLastError();
+    if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
+    delete ctx;
+    return SFE_ERR_CUDA;
+  }
   *out = ctx;
   return SFE_OK;
 }
@@ -136,6 +145,7 @@ void sfe_ctx_destroy(sfe_ctx *ctx) {
   for (auto &b : ctx->stage_out)
     if (b.ptr) cudaFree(b.ptr);
   if (ctx->pinned) cudaFreeHost(ctx->pinned);
+  if (ctx->work) cudaFree(ctx->work);
   if (ctx->copy_stream) {
     cudaStreamSynchronize(ctx->copy_stream);
     cudaStreamDestroy(ctx->copy_stream);
@@ -168,7 +178,7 @@ int sfe_cfar_dev(sfe_ctx *ctx, const void *img_dev, int dtype, int n_frames, int
                  float *thr_dev, uint32_t *bits_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_cfar_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return cfar_run(ctx, img_dev, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable, gate_threshold,
+  return cfar_run(ctx, ctx->stream, img_dev, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable, gate_threshold,
                   mask_dev, thr_dev, bits_dev, 0);
 }
 
@@ -188,7 +198,7 @@ int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, i
   if ((rc = ensure(ctx, ctx->stage_out[0], cells)) != SFE_OK) return rc;
   if (thr_host && (rc = ensure(ctx, ctx->stage_out[1], cells * sizeof(float))) != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(ctx->stage_in[0].ptr, img_host, cells * es, cudaMemcpyHostToDevice, ctx->stream));
-  rc = cfar_run(ctx, ctx->stage_in[0].ptr, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable,
+  rc = cfar_run(ctx, ctx->stream, ctx->stage_in[0].ptr, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable,
                 gate_threshold, (uint8_t *)ctx->stage_out[0].ptr, thr_host ? (float *)ctx->stage_out[1].ptr : nullptr,
                 nullptr, 0);
   if (rc != SFE_OK) return rc;
@@ -204,15 +214,16 @@ int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, i
 
 // ============================================================================ clouds / match / ICP
 namespace sfe {
-int downsample_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
-                   float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split = 0);
-int remove_outlier_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
-                       double radius, int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count,
-                       int n_split = 0);
-int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const int *src_off, const int *src_cnt,
-            const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points, const int *src_id,
-            const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out, int *iters,
-            int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
+int downsample_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
+                   int dim, int n_max, float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count,
+                   int n_split = 0, int slot = SCR_CLOUD);
+int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
+                       int dim, int n_max, double radius, int min_points, float *out_pts, int32_t *out_idx,
+                       int32_t *out_count, int n_split = 0);
+int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off,
+            const int *src_cnt, const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points,
+            const int *src_id, const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out,
+            int *iters, int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
             int class_ns = 0, int class_nt = 0, int force_threads = 0);
 int match_run(sfe_ctx *ctx, const float *ref_pts, const int *ref_off, const float *in_pts, const int *in_off, int P,
               int nt_max, float max_dist, int32_t *ids, float *dists);
@@ -235,7 +246,7 @@ int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_de
                        float resolution, float *out_pts_dev, int32_t *out_idx_dev, int32_t *out_count_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_downsample_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return downsample_run(ctx, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, resolution, out_pts_dev, out_idx_dev,
+  return downsample_run(ctx, ctx->stream, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, resolution, out_pts_dev, out_idx_dev,
                         out_count_dev);
 }
 
@@ -244,7 +255,7 @@ int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *of
                            int32_t *out_count_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_remove_outlier_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return remove_outlier_run(ctx, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, radius, min_points, out_pts_dev,
+  return remove_outlier_run(ctx, ctx->stream, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, radius, min_points, out_pts_dev,
                             out_idx_dev, out_count_dev);
 }
 
@@ -275,8 +286,8 @@ static int cloud_filter_host(sfe_ctx *ctx, int which, const float *pts_host, int
     const int32_t off[2] = {0, n};
     SFE_CUDA(cudaMemcpyAsync(d_pts, pts_host, sizeof(float) * (size_t)n * dim, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
-    int rc = which == 0 ? downsample_run(ctx, d_pts, d_off, nullptr, 1, dim, n, resolution, d_out, d_idx, d_cnt)
-                        : remove_outlier_run(ctx, d_pts, d_off, nullptr, 1, dim, n, radius, min_points, d_out, d_idx,
+    int rc = which == 0 ? downsample_run(ctx, ctx->stream, d_pts, d_off, nullptr, 1, dim, n, resolution, d_out, d_idx, d_cnt)
+                        : remove_outlier_run(ctx, ctx->stream, d_pts, d_off, nullptr, 1, dim, n, radius, min_points, d_out, d_idx,
                                              d_cnt);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(n_out, d_cnt, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -377,7 +388,7 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
                 int32_t *iters_dev, int32_t *inliers_dev, int32_t *status_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_icp_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return icp_run(ctx, prm, src_pts_dev, src_off_dev, nullptr, tgt_pts_dev, tgt_off_dev, nullptr, 0, src_id_dev,
+  return icp_run(ctx, ctx->stream, prm, src_pts_dev, src_off_dev, nullptr, tgt_pts_dev, tgt_off_dev, nullptr, 0, src_id_dev,
                  tgt_id_dev, n_problems, ns_max, nt_max, guess_dev, T_dev, iters_dev, inliers_dev, status_dev);
 }
 
@@ -449,7 +460,7 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
     SFE_CUDA(cudaMemcpyAsync(d_ids, src_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_ids + P, tgt_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
-    int rc = icp_run(ctx, prm, d_src, d_soff, nullptr, d_tgt, d_toff, nullptr, 0, d_ids, d_ids + P, n_problems, ns_max,
+    int rc = icp_run(ctx, ctx->stream, prm, d_src, d_soff, nullptr, d_tgt, d_toff, nullptr, 0, d_ids, d_ids + P, n_problems, ns_max,
                      nt_max, d_guess, d_T, d_res, d_res + P, d_res + 2 * P);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));

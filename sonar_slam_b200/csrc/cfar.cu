@@ -865,38 +865,38 @@ static float gate_as_float(double t) {
 }
 
 template <typename InT, int ALG, bool WITH_THR, bool MASK, bool BITS>
-static int launch_ring(sfe_ctx *ctx, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
+static int launch_ring(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
   cfar_ring_tma_kernel<InT, ALG, WITH_THR, MASK, BITS>
-      <<<p.F * p.strips, CF_W, 0, ctx->stream>>>(in_map, out_map, p);
+      <<<p.F * p.strips, CF_W, 0, st>>>(in_map, out_map, p);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
 }
 
 template <typename InT, int ALG>
-static int launch_ring_out(sfe_ctx *ctx, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
+static int launch_ring_out(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
   const bool m = p.mask != nullptr, b = p.bits != nullptr;
   if (p.thr != nullptr) {  // the "2" variants
-    if (m && b) return launch_ring<InT, ALG, true, true, true>(ctx, in_map, out_map, p);
-    if (m) return launch_ring<InT, ALG, true, true, false>(ctx, in_map, out_map, p);
-    if (b) return launch_ring<InT, ALG, true, false, true>(ctx, in_map, out_map, p);
-    return launch_ring<InT, ALG, true, false, false>(ctx, in_map, out_map, p);
+    if (m && b) return launch_ring<InT, ALG, true, true, true>(ctx, st, in_map, out_map, p);
+    if (m) return launch_ring<InT, ALG, true, true, false>(ctx, st, in_map, out_map, p);
+    if (b) return launch_ring<InT, ALG, true, false, true>(ctx, st, in_map, out_map, p);
+    return launch_ring<InT, ALG, true, false, false>(ctx, st, in_map, out_map, p);
   }
-  if (m && b) return launch_ring<InT, ALG, false, true, true>(ctx, in_map, out_map, p);
-  if (m) return launch_ring<InT, ALG, false, true, false>(ctx, in_map, out_map, p);
-  if (b) return launch_ring<InT, ALG, false, false, true>(ctx, in_map, out_map, p);
+  if (m && b) return launch_ring<InT, ALG, false, true, true>(ctx, st, in_map, out_map, p);
+  if (m) return launch_ring<InT, ALG, false, true, false>(ctx, st, in_map, out_map, p);
+  if (b) return launch_ring<InT, ALG, false, false, true>(ctx, st, in_map, out_map, p);
   return SFE_OK;  // nothing to write
 }
 
 template <typename InT>
-static int launch_ring_alg(sfe_ctx *ctx, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
+static int launch_ring_alg(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
   switch (p.alg) {
     case SFE_CFAR_CA:
-      return launch_ring_out<InT, SFE_CFAR_CA>(ctx, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_CA>(ctx, st, in_map, out_map, p);
     case SFE_CFAR_SOCA:
-      return launch_ring_out<InT, SFE_CFAR_SOCA>(ctx, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_SOCA>(ctx, st, in_map, out_map, p);
     default:
-      return launch_ring_out<InT, SFE_CFAR_GOCA>(ctx, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_GOCA>(ctx, st, in_map, out_map, p);
   }
 }
 
@@ -924,13 +924,13 @@ static void build_u8_lut(const CfarParams &p, std::vector<uint16_t> &lut) {
 }
 
 template <int ALG>
-static int launch_u8_lut(sfe_ctx *ctx, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p,
+static int launch_u8_lut(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p,
                          const uint16_t *lut, int lut_n) {
   const bool m = p.mask != nullptr, b = p.bits != nullptr;
   const int grid = p.F * p.strips, thr = CF_W;
-  if (m && b) cfar_u8_lut_kernel<ALG, true, true><<<grid, thr, 0, ctx->stream>>>(in_map, out_map, p, lut, lut_n);
-  else if (m) cfar_u8_lut_kernel<ALG, true, false><<<grid, thr, 0, ctx->stream>>>(in_map, out_map, p, lut, lut_n);
-  else if (b) cfar_u8_lut_kernel<ALG, false, true><<<grid, thr, 0, ctx->stream>>>(in_map, out_map, p, lut, lut_n);
+  if (m && b) cfar_u8_lut_kernel<ALG, true, true><<<grid, thr, 0, st>>>(in_map, out_map, p, lut, lut_n);
+  else if (m) cfar_u8_lut_kernel<ALG, true, false><<<grid, thr, 0, st>>>(in_map, out_map, p, lut, lut_n);
+  else if (b) cfar_u8_lut_kernel<ALG, false, true><<<grid, thr, 0, st>>>(in_map, out_map, p, lut, lut_n);
   else return SFE_OK;
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
@@ -938,7 +938,7 @@ static int launch_u8_lut(sfe_ctx *ctx, const CUtensorMap &in_map, const CUtensor
 }
 
 template <int ALG>
-static int launch_u8_gate4(sfe_ctx *ctx, const CUtensorMap &in_map, const CfarParams &p, const uint16_t *lut, int lut_n,
+static int launch_u8_gate4(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CfarParams &p, const uint16_t *lut, int lut_n,
                            uint32_t gate_add) {
   const bool m = p.mask != nullptr, b = p.bits != nullptr;
   const int grid = p.F * p.strips;
@@ -947,7 +947,7 @@ static int launch_u8_gate4(sfe_ctx *ctx, const CUtensorMap &in_map, const CfarPa
   do {                                                                                                              \
     SFE_CUDA(cudaFuncSetAttribute(cfar_u8_gate4_kernel<ALG, M_, B_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
                                   (int)smem));                                                                      \
-    cfar_u8_gate4_kernel<ALG, M_, B_><<<grid, CF_W, smem, ctx->stream>>>(in_map, p, lut, lut_n, gate_add);          \
+    cfar_u8_gate4_kernel<ALG, M_, B_><<<grid, CF_W, smem, st>>>(in_map, p, lut, lut_n, gate_add);          \
   } while (0)
   if (m && b) SFE_GO(true, true);
   else if (m) SFE_GO(true, false);
@@ -959,7 +959,7 @@ static int launch_u8_gate4(sfe_ctx *ctx, const CUtensorMap &in_map, const CfarPa
 }
 
 template <typename InT>
-static int launch_exact(sfe_ctx *ctx, const InT *img, const CfarParams &p, const uint8_t *only_flagged) {
+static int launch_exact(sfe_ctx *ctx, cudaStream_t st, const InT *img, const CfarParams &p, const uint8_t *only_flagged) {
   size_t smem = 0;
   if (p.alg == SFE_CFAR_OS) {
     smem = (size_t)2 * p.T * CF_W * sizeof(float);
@@ -971,13 +971,13 @@ static int launch_exact(sfe_ctx *ctx, const InT *img, const CfarParams &p, const
       SFE_CUDA(cudaFuncSetAttribute(cfar_exact_kernel<InT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
   }
-  cfar_exact_kernel<InT><<<p.F * p.strips, CF_W, smem, ctx->stream>>>(img, p, only_flagged);
+  cfar_exact_kernel<InT><<<p.F * p.strips, CF_W, smem, st>>>(img, p, only_flagged);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
 }
 
-int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int alg, int T, int G, int k,
+int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G, int k,
              double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact) {
   SFE_REQUIRE(ctx != nullptr, "cfar: null context");
   SFE_REQUIRE(img != nullptr || F == 0, "cfar: null image pointer");
@@ -1012,7 +1012,7 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
   if (mask != nullptr) fast = fast && ((uintptr_t)mask % 16 == 0) && (B % 16 == 0);
   fast = fast && isfinite(c) && fabs(c) > 1e-20 && fabs(c) < 1e20;
 
-  if (thr != nullptr) SFE_CUDA(cudaMemsetAsync(thr, 0, (size_t)F * R * B * sizeof(float), ctx->stream));
+  if (thr != nullptr) SFE_CUDA(cudaMemsetAsync(thr, 0, (size_t)F * R * B * sizeof(float), st));
 
   if (fast) {
     CUtensorMap in_map, out_map;
@@ -1026,13 +1026,13 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
       out_map = in_map;  // unused
     }
     if (dtype == SFE_F32) {
-      rc = ensure(ctx, ctx->scratch[SCR_CFAR_FLAGS], (size_t)F * p.strips);
+      rc = ensure(ctx, ctx->scratch[SCR_CFAR_FLAGS], (size_t)F * p.strips, st);
       if (rc != SFE_OK) return rc;
       p.flags = (uint8_t *)ctx->scratch[SCR_CFAR_FLAGS].ptr;
-      SFE_CUDA(cudaMemsetAsync(p.flags, 0, (size_t)F * p.strips, ctx->stream));
-      rc = launch_ring_alg<float>(ctx, in_map, out_map, p);
+      SFE_CUDA(cudaMemsetAsync(p.flags, 0, (size_t)F * p.strips, st));
+      rc = launch_ring_alg<float>(ctx, st, in_map, out_map, p);
       if (rc != SFE_OK) return rc;
-      return launch_exact<float>(ctx, (const float *)img, p, p.flags);  // re-does flagged strips only
+      return launch_exact<float>(ctx, st, (const float *)img, p, p.flags);  // re-does flagged strips only
     }
     if (thr == nullptr && isfinite(tau)) {
       // integer kernels with the threshold table (re-uploaded only when the parameters change; the cache key lives
@@ -1043,13 +1043,13 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
       int g_min = 256;
       for (uint16_t v : lut_host) g_min = v < g_min ? v : g_min;
       lut_host.resize((lut_host.size() + 7) / 8 * 8, 256);  // pad for the kernels' 16-byte copies
-      rc = ensure(ctx, ctx->scratch[SCR_CFAR_LUT], 65536);  // [0, 32 KiB): this table, [32 KiB, 64 KiB): the OS table
+      rc = ensure(ctx, ctx->scratch[SCR_CFAR_LUT], 65536, st);  // [0, 32 KiB): this table, [32 KiB, 64 KiB): the OS table
       if (rc != SFE_OK) return rc;
       const double k6[6] = {(double)alg, tau, (double)p.gate_on, p.gate_d, (double)lut_host.size(), 1.0};
       if (memcmp(k6, ctx->cfar_lut_key, sizeof(k6)) != 0 || ctx->cfar_lut_buf != ctx->scratch[SCR_CFAR_LUT].ptr) {
         SFE_CUDA(cudaMemcpyAsync(ctx->scratch[SCR_CFAR_LUT].ptr, lut_host.data(), lut_host.size() * sizeof(uint16_t),
-                                 cudaMemcpyHostToDevice, ctx->stream));
-        SFE_CUDA(cudaStreamSynchronize(ctx->stream));  // lut_host is a local
+                                 cudaMemcpyHostToDevice, st));
+        SFE_CUDA(cudaStreamSynchronize(st));  // lut_host is a local
         memcpy(ctx->cfar_lut_key, k6, sizeof(k6));
         ctx->cfar_lut_buf = ctx->scratch[SCR_CFAR_LUT].ptr;
       }
@@ -1066,18 +1066,18 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
         q.strips = (B + CG_W - 1) / CG_W;
         const uint32_t gate_add = 0x01010101u * (uint32_t)(128 - g_min);
         switch (alg) {
-          case SFE_CFAR_CA: return launch_u8_gate4<SFE_CFAR_CA>(ctx, in4, q, lut, n, gate_add);
-          case SFE_CFAR_SOCA: return launch_u8_gate4<SFE_CFAR_SOCA>(ctx, in4, q, lut, n, gate_add);
-          default: return launch_u8_gate4<SFE_CFAR_GOCA>(ctx, in4, q, lut, n, gate_add);
+          case SFE_CFAR_CA: return launch_u8_gate4<SFE_CFAR_CA>(ctx, st, in4, q, lut, n, gate_add);
+          case SFE_CFAR_SOCA: return launch_u8_gate4<SFE_CFAR_SOCA>(ctx, st, in4, q, lut, n, gate_add);
+          default: return launch_u8_gate4<SFE_CFAR_GOCA>(ctx, st, in4, q, lut, n, gate_add);
         }
       }
       switch (alg) {
-        case SFE_CFAR_CA: return launch_u8_lut<SFE_CFAR_CA>(ctx, in_map, out_map, p, lut, n);
-        case SFE_CFAR_SOCA: return launch_u8_lut<SFE_CFAR_SOCA>(ctx, in_map, out_map, p, lut, n);
-        default: return launch_u8_lut<SFE_CFAR_GOCA>(ctx, in_map, out_map, p, lut, n);
+        case SFE_CFAR_CA: return launch_u8_lut<SFE_CFAR_CA>(ctx, st, in_map, out_map, p, lut, n);
+        case SFE_CFAR_SOCA: return launch_u8_lut<SFE_CFAR_SOCA>(ctx, st, in_map, out_map, p, lut, n);
+        default: return launch_u8_lut<SFE_CFAR_GOCA>(ctx, st, in_map, out_map, p, lut, n);
       }
     }
-    return launch_ring_alg<uint8_t>(ctx, in_map, out_map, p);
+    return launch_ring_alg<uint8_t>(ctx, st, in_map, out_map, p);
   }
   if (dtype == SFE_U8 && alg == SFE_CFAR_OS && !force_exact && T >= 1 && T <= 127 && R > 2 * (T + G) && isfinite(tau)) {
     // sliding-histogram OS-CFAR; 256-entry pass table M[v] = smallest cell value with x > tau*v (and the gate)
@@ -1089,18 +1089,18 @@ int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int 
       const int m = (d != d) ? 256 : (d < 0 ? 0 : (d >= 255.0 ? 256 : (int)floor(d) + 1));
       lut[v] = (uint16_t)(m > g ? m : g);
     }
-    int rc = ensure(ctx, ctx->scratch[SCR_CFAR_LUT], 65536);
+    int rc = ensure(ctx, ctx->scratch[SCR_CFAR_LUT], 65536, st);
     if (rc != SFE_OK) return rc;
     uint16_t *lut_dev = (uint16_t *)((char *)ctx->scratch[SCR_CFAR_LUT].ptr + 32768);  // second half: OS table
-    SFE_CUDA(cudaMemcpyAsync(lut_dev, lut.data(), 512, cudaMemcpyHostToDevice, ctx->stream));
-    SFE_CUDA(cudaStreamSynchronize(ctx->stream));  // `lut` is a local
-    cfar_os_hist_kernel<<<F * p.strips, CF_W, 0, ctx->stream>>>((const uint8_t *)img, p, lut_dev);
+    SFE_CUDA(cudaMemcpyAsync(lut_dev, lut.data(), 512, cudaMemcpyHostToDevice, st));
+    SFE_CUDA(cudaStreamSynchronize(st));  // `lut` is a local
+    cfar_os_hist_kernel<<<F * p.strips, CF_W, 0, st>>>((const uint8_t *)img, p, lut_dev);
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;
     return SFE_OK;
   }
-  if (dtype == SFE_F32) return launch_exact<float>(ctx, (const float *)img, p, nullptr);
-  return launch_exact<uint8_t>(ctx, (const uint8_t *)img, p, nullptr);
+  if (dtype == SFE_F32) return launch_exact<float>(ctx, st, (const float *)img, p, nullptr);
+  return launch_exact<uint8_t>(ctx, st, (const uint8_t *)img, p, nullptr);
 }
 
 }  // namespace sfe

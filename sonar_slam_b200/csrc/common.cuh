@@ -65,6 +65,7 @@ struct sfe_ctx {
   void (*png_free)(void *) = nullptr;
   cudaStream_t copy_stream = nullptr;   // host flavours that overlap copies with kernels (featx.cu), created on first use
   cudaEvent_t copy_ev[4] = {};
+  int *work = nullptr;  // device [SFE_WORK_COUNTERS]: work counters of the persistent kernels (sfe::next_work_item)
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
@@ -80,9 +81,15 @@ struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
 };
 
 namespace sfe {
-enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5 };
+enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_SUBMAP = 6 };
+// Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
+// different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
+enum { WORK_CART = 0, WORK_ICP = 1, SFE_WORK_COUNTERS = 2 };
 
-int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes);  // (re)allocate if too small
+// (re)allocate if too small, stream-ordered on `stream` (default: ctx->stream).  A buffer must only grow on a stream
+// that is ordered after every earlier user of the block and before every later one: the stream that uses it.
+int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes);
+int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes, cudaStream_t stream);
 int ensure_pinned(sfe_ctx *ctx, size_t bytes);
 
 // ---------------------------------------------------------------- compressed pings (jpeg.cu, png.cu)
@@ -180,6 +187,16 @@ __device__ __forceinline__ void tma_wait_all() {
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+// Persistent CTAs: CTA c starts with work item c; every later item is the next one no CTA has taken yet (`counter`
+// zero at launch), so CTAs that drew short items take more and a launch ends in a short tail instead of waiting for
+// the CTAs whose static share (c, c + gridDim.x, ...) happened to be the longest.  All threads of the CTA call it;
+// `bcast` is a CTA-shared int.
+__device__ __forceinline__ int next_work_item(int *counter, int *bcast) {
+  __syncthreads();  // every thread has read the previous item
+  if (threadIdx.x == 0) *bcast = (int)gridDim.x + atomicAdd(counter, 1);
+  __syncthreads();
+  return *bcast;
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -119,9 +119,9 @@ __global__ void __launch_bounds__(FXS_THREADS)
                         const int32_t *__restrict__ inv_idx, int npix, int cols, int rows, int R, int B, int wpr,
                         const uint8_t *__restrict__ mask, const uint32_t *__restrict__ bits, int F, int cap,
                         const float *__restrict__ metres, int32_t *__restrict__ ij, float *__restrict__ xy,
-                        int32_t *__restrict__ count) {
+                        int32_t *__restrict__ count, int *__restrict__ next) {
   extern __shared__ uint32_t fxs_smem[];
-  __shared__ int scan_s[36];
+  __shared__ int scan_s[36], next_s;
   const float inv_cols = 1.0f / (float)cols;
   const int words = R * wpr, cwords = (npix + 31) / 32;
   uint32_t *sb = fxs_smem;           // polar bit plane
@@ -129,7 +129,7 @@ __global__ void __launch_bounds__(FXS_THREADS)
   uint32_t *doff = fxs_smem + words + cwords;  // [(words + 1) / 2]: rank of the first set bit of every pair of polar words
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = FXS_THREADS / 32;
 
-  for (int f = blockIdx.x; f < F; f += gridDim.x) {
+  for (int f = blockIdx.x; f < F; f = next_work_item(next, &next_s)) {
     __syncthreads();
     if (bits != nullptr) {
       const uint32_t *src = bits + (size_t)f * words;
@@ -453,7 +453,7 @@ static bool ctx_force_gather(const sfe_ctx *) {
 }
 
 template <int FPB>
-static int launch_cart(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
+static int launch_cart(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
                        int32_t *ij, float *xy, int32_t *count) {
   const int wpr = (m->B + 31) / 32;
   const size_t smem = (size_t)FPB * m->R * wpr * sizeof(uint32_t);
@@ -461,7 +461,7 @@ static int launch_cart(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, con
   if (smem > 40 * 1024)
     SFE_CUDA(cudaFuncSetAttribute(cart_points_kernel<FPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = (F + FPB - 1) / FPB;
-  cart_points_kernel<FPB><<<grid, FX_THREADS, smem, ctx->stream>>>(
+  cart_points_kernel<FPB><<<grid, FX_THREADS, smem, st>>>(
       (const MapEntry *)m->table, m->rows * m->cols, m->cols, m->rows, m->R, m->B, wpr, mask, bits, F, cap, m->width,
       m->height, ij, xy, count);
   SFE_CUDA(cudaGetLastError());
@@ -469,7 +469,7 @@ static int launch_cart(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, con
   return SFE_OK;
 }
 
-int cart_points_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
+int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
                     int32_t *ij, float *xy, int32_t *count) {
   SFE_REQUIRE(ctx && m, "cart_points: null context or maps");
   SFE_REQUIRE(ctx->device == m->device, "cart_points: maps were created on device %d, context is on %d", m->device,
@@ -490,9 +490,10 @@ int cart_points_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const 
       SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cart_scatter_kernel, FXS_THREADS, smem));
       int grid = ctx->sm_count * (per_sm < 1 ? 1 : per_sm);
       if (grid > F) grid = F;
-      cart_scatter_kernel<<<grid, FXS_THREADS, smem, ctx->stream>>>(
+      SFE_CUDA(cudaMemsetAsync(ctx->work + WORK_CART, 0, sizeof(int), st));
+      cart_scatter_kernel<<<grid, FXS_THREADS, smem, st>>>(
           (const MapEntry *)m->table, m->inv_off, m->inv_idx, npix, m->cols, m->rows, m->R, m->B, wpr, mask, bits, F,
-          cap, m->metres, ij, xy, count);
+          cap, m->metres, ij, xy, count, ctx->work + WORK_CART);
       SFE_CUDA(cudaGetLastError());
       ctx->launches++;
       return SFE_OK;
@@ -500,9 +501,9 @@ int cart_points_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const 
   }
   // dense variant: several frames per CTA amortise the table read once there are enough frames
   int rc = SFE_ERR_UNSUPPORTED;
-  if (F >= 4 * ctx->sm_count) rc = launch_cart<4>(ctx, m, mask, bits, F, cap, ij, xy, count);
-  if (rc == SFE_ERR_UNSUPPORTED && F >= 2 * ctx->sm_count) rc = launch_cart<2>(ctx, m, mask, bits, F, cap, ij, xy, count);
-  if (rc == SFE_ERR_UNSUPPORTED) rc = launch_cart<1>(ctx, m, mask, bits, F, cap, ij, xy, count);
+  if (F >= 4 * ctx->sm_count) rc = launch_cart<4>(ctx, st, m, mask, bits, F, cap, ij, xy, count);
+  if (rc == SFE_ERR_UNSUPPORTED && F >= 2 * ctx->sm_count) rc = launch_cart<2>(ctx, st, m, mask, bits, F, cap, ij, xy, count);
+  if (rc == SFE_ERR_UNSUPPORTED) rc = launch_cart<1>(ctx, st, m, mask, bits, F, cap, ij, xy, count);
   if (rc == SFE_ERR_UNSUPPORTED)
     set_error("cart_points: a %d x %d polar bit plane does not fit in shared memory", m->R, m->B);
   return rc;
@@ -676,7 +677,7 @@ int sfe_cart_points_dev(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *mask_
                         int n_frames, int capacity, int32_t *ij_dev, float *xy_dev, int32_t *count_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_cart_points_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return cart_points_run(ctx, maps, mask_dev, bits_dev, n_frames, capacity, ij_dev, xy_dev, count_dev);
+  return cart_points_run(ctx, ctx->stream, maps, mask_dev, bits_dev, n_frames, capacity, ij_dev, xy_dev, count_dev);
 }
 
 int sfe_cart_points_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *mask_host, int n_frames, int capacity,
@@ -693,7 +694,7 @@ int sfe_cart_points_host(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *mask
   if ((rc = ensure(ctx, ctx->stage_out[1], slots * sizeof(float) + 16)) != SFE_OK) return rc;
   if ((rc = ensure(ctx, ctx->stage_out[2], (size_t)n_frames * sizeof(int32_t))) != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(ctx->stage_in[0].ptr, mask_host, cells, cudaMemcpyHostToDevice, ctx->stream));
-  rc = cart_points_run(ctx, maps, (const uint8_t *)ctx->stage_in[0].ptr, nullptr, n_frames, capacity,
+  rc = cart_points_run(ctx, ctx->stream, maps, (const uint8_t *)ctx->stage_in[0].ptr, nullptr, n_frames, capacity,
                        (int32_t *)ctx->stage_out[0].ptr, (float *)ctx->stage_out[1].ptr,
                        (int32_t *)ctx->stage_out[2].ptr);
   if (rc != SFE_OK) return rc;

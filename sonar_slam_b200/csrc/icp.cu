@@ -64,6 +64,7 @@ struct IcpBatch {
   float margin_mult;  // certificate size in units of the point's last step (one-pass path)
   int small_mult;     // problems with ns <= small_mult * blockDim.x (and nt <= 4096) take the one-pass exact path
   int slot_by_smid;   // workspace slot = %smid (one CTA per SM, one CTA per problem) instead of blockIdx.x
+  int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
 };
 
 constexpr int ICP_SM_SLOTS = 256;  // >= %nsmid on every sm_90 part
@@ -434,7 +435,12 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
   // ill-conditioned scans because the float32-sequential sums themselves are that noisy).
   const bool seq = (prm.flags & 2) == 0;
 
-  for (int p = blockIdx.x; p < b.P; p += gridDim.x) {
+  // Persistent CTAs take problems from a work counter: problems differ in length (cloud sizes, early exits), and with
+  // a static share the batch ends when the CTAs that drew the most work finish -- at the front end's 4096 problems
+  // over 6 x 132 CTAs, 136 CTAs run a sixth problem while the other 656 are done.  Problem p's results do not depend
+  // on the CTA that solves it.  The index is broadcast through sh.status, which thread 0 rewrites only after the
+  // next problem's first barrier (the shared-memory layout is sized to the byte, so no field is added for it).
+  for (int p = blockIdx.x; p < b.P; p = b.next ? next_work_item(b.next, &sh.status) : p + (int)gridDim.x) {
     const int si = b.src_id ? b.src_id[p] : p, ti = b.tgt_id ? b.tgt_id[p] : p;
     const float *src = b.src_pts + 2 * (size_t)b.src_off[si];
     const int ns = b.src_cnt ? b.src_cnt[si] : b.src_off[si + 1] - b.src_off[si];
@@ -1206,7 +1212,7 @@ static int pick_max_cells(int nt_max) {
   return c;
 }
 
-int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const int *src_off, const int *src_cnt,
+int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off, const int *src_cnt,
             const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points, const int *src_id,
             const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out, int *iters,
             int *inliers, int *status, const int *raw_cnt, int raw_cap, int class_mode, int class_ns, int class_nt,
@@ -1312,12 +1318,16 @@ int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const
   if (per_sm == 1 && P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = P;  // one CTA per problem
   const size_t orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
   const size_t nrm_bytes = plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0;
-  int rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes);
+  int rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes, st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
   b.nrm_ws = plane ? (float2 *)((char *)ctx->scratch[SCR_ICP].ptr + orig_bytes) : nullptr;
+  if (!b.slot_by_smid && grid < P) {  // persistent CTAs
+    b.next = ctx->work + WORK_ICP;
+    SFE_CUDA(cudaMemsetAsync(b.next, 0, sizeof(int), st));
+  }
   void *args[] = {(void *)&b};
-  SFE_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(threads), args, smem, ctx->stream));
+  SFE_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(threads), args, smem, st));
   ctx->launches++;
   return SFE_OK;
 }

@@ -19,21 +19,22 @@
 #include "common.cuh"
 
 namespace sfe {
-int cfar_run(sfe_ctx *ctx, const void *img, int dtype, int F, int R, int B, int alg, int T, int G, int k,
-             double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
-int cart_points_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
-                    int32_t *ij, float *xy, int32_t *count);
+int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
+             int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
+int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F,
+                    int cap, int32_t *ij, float *xy, int32_t *count);
 int feature_image_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames, int F, const uint8_t *lut_bgr,
                       uint8_t *out, const char *what);
-int downsample_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
-                   float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split = 0);
-int remove_outlier_run(sfe_ctx *ctx, const float *pts, const int *off, const int *cnt, int n_clouds, int dim, int n_max,
-                       double radius, int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count,
-                       int n_split = 0);
-int icp_run(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts, const int *src_off, const int *src_cnt,
-            const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points, const int *src_id,
-            const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out, int *iters,
-            int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
+int downsample_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
+                   int dim, int n_max, float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count,
+                   int n_split = 0, int slot = SCR_CLOUD);
+int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
+                       int dim, int n_max, double radius, int min_points, float *out_pts, int32_t *out_idx,
+                       int32_t *out_count, int n_split = 0);
+int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off,
+            const int *src_cnt, const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points,
+            const int *src_id, const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out,
+            int *iters, int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
             int class_ns = 0, int class_nt = 0, int force_threads = 0);
 // compressed pings (jpeg.cu)
 struct JpegBatch;
@@ -97,6 +98,9 @@ constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 1536, FE_ICP_SMALL_THRE
 // left as one launch (with a class boundary at 4608 or 5632 points too many frames land in the second, poorly
 // filled launch).  Chosen on the replay; not re-measured on H100.
 constexpr int FE_DS_SPLIT = 0, FE_RO_SPLIT = 1024, FE_SUBMAP_SPLIT = 2048;
+// Default schedule of sfe_frontend_run_dev (sfe_frontend_set_overlap): serial.  On an H100 (700 W) the overlapped
+// schedule measured slower at every sub-batch size tried on the config-4 replay (DESIGN.md section 4).
+constexpr int FE_OVERLAP_FRAMES = 0;
 
 // T_ab = pose_a^-1 * pose_b as float32 3x3 (gtsam Pose2::between, then matrix().astype(float32)).
 // Evaluated on the host in double (libm), so the float32 matrices the kernels see are the ones a
@@ -199,6 +203,11 @@ struct sfe_frontend {
   double *carry_poses;   // host [window][3]
   cudaStream_t copy_stream;
   cudaEvent_t ev_copy[2], ev_done;
+  // overlapped run_dev (sfe_frontend_set_overlap): sub-batch size (0: serial on ctx->stream), the two streams and the
+  // events that fork them from ctx->stream, hand each sub-batch from features to match, and join them back
+  int overlap;
+  cudaStream_t feat_stream, match_stream;
+  cudaEvent_t ev_fork, ev_feat, ev_join;
   // feature images (sfe_frontend_set_feature_images)
   uint8_t img_lut[256 * 3];
   uint8_t *img_dst;      // null: off
@@ -230,6 +239,23 @@ static void fe_toc(sfe_frontend *fe) {
   if (!fe->timing) return;
   cudaEventRecord((*fe->tev)[fe->tused + 1], fe->ctx->stream);
   fe->tused += 2;
+}
+
+// The streams of the overlapped schedule.  The match side (submap + ICP) is the longer chain, so its CTAs go first
+// when both sides have work ready; SFE_FE_OVERLAP_PRIO=features|equal (development switch, read when a front end is
+// created) gives the feature side the higher priority or neither.
+static cudaError_t fe_create_overlap_streams(sfe_frontend *fe) {
+  int least = 0, greatest = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
+  const char *sw = getenv("SFE_FE_OVERLAP_PRIO");
+  int p_feat = least, p_match = greatest;
+  if (sw && strcmp(sw, "features") == 0) p_feat = greatest, p_match = least;
+  if (sw && strcmp(sw, "equal") == 0) p_feat = p_match = least;
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&fe->feat_stream, cudaStreamNonBlocking, p_feat);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&fe->match_stream, cudaStreamNonBlocking, p_match);
+  for (cudaEvent_t *ev : {&fe->ev_fork, &fe->ev_feat, &fe->ev_join})
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+  return e;
 }
 
 extern "C" {
@@ -316,6 +342,7 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_copy[0], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_copy[1], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_done, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = fe_create_overlap_streams(fe);
   if (e != cudaSuccess) {
     sfe::set_error("sfe_frontend_create: %s", cudaGetErrorString(e));
     sfe_frontend_destroy(fe);
@@ -325,6 +352,7 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
   fill_offsets_kernel<<<(max_frames + 256) / 256, 256, 0, ctx->stream>>>(fe->off_tgt, max_frames, (int)tcap);
   SFE_CUDA(cudaGetLastError());
   ctx->launches += 2;
+  fe->overlap = FE_OVERLAP_FRAMES;
   *out = fe;
   return SFE_OK;
 }
@@ -347,6 +375,13 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   for (auto &ev : fe->ev_copy)
     if (ev) cudaEventDestroy(ev);
   if (fe->ev_done) cudaEventDestroy(fe->ev_done);
+  for (cudaStream_t st : {fe->feat_stream, fe->match_stream})
+    if (st) {
+      cudaStreamSynchronize(st);
+      cudaStreamDestroy(st);
+    }
+  for (cudaEvent_t ev : {fe->ev_fork, fe->ev_feat, fe->ev_join})
+    if (ev) cudaEventDestroy(ev);
   if (fe->img_stream) {
     cudaStreamSynchronize(fe->img_stream);
     cudaStreamDestroy(fe->img_stream);
@@ -451,18 +486,18 @@ static const float *fe_cloud(const sfe_frontend *fe, const int32_t **cnt);
 
 // stages 1-3 on frames [f0, f0+n): CFAR (bit plane) -> Cartesian points -> downsample -> outlier removal.
 // Final per-frame clouds end in xy_a / cnt_c (or wherever the last enabled filter wrote; see cloud()).
-static int fe_features(sfe_frontend *fe, const uint8_t *frames_dev, int f0, int n) {
+static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_dev, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
   const sfe_frontend_params &p = fe->p;
   const size_t cap = p.cap_points, wpr = (p.B + 31) / 32;
   uint32_t *bits = fe->bits + (size_t)f0 * p.R * wpr;
   fe_tic(fe, SFE_FE_CFAR);
-  int rc = cfar_run(ctx, frames_dev, SFE_U8, n, p.R, p.B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank, p.tau,
+  int rc = cfar_run(ctx, st, frames_dev, SFE_U8, n, p.R, p.B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank, p.tau,
                     p.gate_enable, p.gate_threshold, nullptr, nullptr, bits, 0);
   fe_toc(fe);
   if (rc != SFE_OK) return rc;
   fe_tic(fe, SFE_FE_CART);
-  rc = cart_points_run(ctx, fe->maps, nullptr, bits, n, (int)cap, fe->ij + (size_t)f0 * cap * 2,
+  rc = cart_points_run(ctx, st, fe->maps, nullptr, bits, n, (int)cap, fe->ij + (size_t)f0 * cap * 2,
                        fe->xy_a + (size_t)f0 * cap * 2, fe->cnt_a + f0);
   fe_toc(fe);
   if (rc != SFE_OK) return rc;
@@ -475,7 +510,7 @@ static int fe_features(sfe_frontend *fe, const uint8_t *frames_dev, int f0, int 
       const char *e = getenv("SFE_FE_DS_SPLIT");
       return e ? atoi(e) : FE_DS_SPLIT;
     }();
-    rc = downsample_run(ctx, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.resolution, fe->xy_b, fe->idx,
+    rc = downsample_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.resolution, fe->xy_b, fe->idx,
                         fe->cnt_b + f0, ds_split);
     fe_toc(fe);
     if (rc != SFE_OK) return rc;
@@ -484,7 +519,7 @@ static int fe_features(sfe_frontend *fe, const uint8_t *frames_dev, int f0, int 
   if (p.outlier_min_points > 1) {
     float *dst = (cur == fe->xy_a) ? fe->xy_b : fe->xy_a;
     fe_tic(fe, SFE_FE_OUTLIER);
-    rc = remove_outlier_run(ctx, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.outlier_radius,
+    rc = remove_outlier_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.outlier_radius,
                             p.outlier_min_points, dst, fe->idx, fe->cnt_c + f0, FE_RO_SPLIT);
     fe_toc(fe);
     if (rc != SFE_OK) return rc;
@@ -493,7 +528,7 @@ static int fe_features(sfe_frontend *fe, const uint8_t *frames_dev, int f0, int 
     const int32_t *cnt;
     float *cloud = const_cast<float *>(fe_cloud(fe, &cnt));
     fe_tic(fe, SFE_FE_OUTLIER);
-    flip_lateral_kernel<<<n, 128, 0, ctx->stream>>>(cloud + 2 * (size_t)f0 * cap, cnt + f0, (int)cap, n);
+    flip_lateral_kernel<<<n, 128, 0, st>>>(cloud + 2 * (size_t)f0 * cap, cnt + f0, (int)cap, n);
     fe_toc(fe);
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;
@@ -517,23 +552,23 @@ static const float *fe_cloud(const sfe_frontend *fe, const int32_t **cnt) {
 }
 
 // stage 4-5 on frames [f0, f0+n): targets from the window of previous frames (which may precede f0), then ICP
-static int fe_match(sfe_frontend *fe, int f0, int n) {
+static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
   const sfe_frontend_params &p = fe->p;
   const int cap = p.cap_points, tcap = p.window * cap;
   const int32_t *cnt;
   const float *cloud = fe_cloud(fe, &cnt);
   fe_tic(fe, SFE_FE_SUBMAP);
-  assemble_targets_kernel<<<n, 256, 0, ctx->stream>>>(cloud, cnt, cap, fe->rel, f0, f0 + n, p.window, fe->tgt_a,
-                                                      fe->tcnt_a, tcap, fe->guess, fe->carry_xy, fe->carry_cnt,
-                                                      fe->carry_n);
+  assemble_targets_kernel<<<n, 256, 0, st>>>(cloud, cnt, cap, fe->rel, f0, f0 + n, p.window, fe->tgt_a, fe->tcnt_a,
+                                             tcap, fe->guess, fe->carry_xy, fe->carry_cnt, fe->carry_n);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   const float *tgt = fe->tgt_a;
   const int32_t *tcnt = fe->tcnt_a;
   if (p.submap_resolution > 0.f) {
-    int rc = downsample_run(ctx, fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, n, 2, tcap, p.submap_resolution,
-                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT);
+    // (its own sort workspace: in the overlapped schedule it runs next to the frame down-sampling)
+    int rc = downsample_run(ctx, st, fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, n, 2, tcap, p.submap_resolution,
+                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_SUBMAP);
     if (rc != SFE_OK) return rc;
     tgt = fe->tgt_b, tcnt = fe->tcnt_b;
   }
@@ -548,12 +583,12 @@ static int fe_match(sfe_frontend *fe, int f0, int n) {
   // class_mode 1 leaves oversize problems untouched for the second launch; when the capacities are not larger than
   // the small class there is no second launch and this one must report them itself (SFE_ICP_TOO_LARGE)
   const bool two = ns_small < p.cap_source || nt_small < p.cap_target;
-  int rc = icp_run(ctx, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
+  int rc = icp_run(ctx, st, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
                    nullptr, nullptr, n, ns_small, nt_small, fe->guess + 9 * (size_t)f0, fe->T + 9 * (size_t)f0,
                    fe->iters + f0, fe->inliers + f0, fe->status + f0, fe->cnt_a + f0, cap, two ? 1 : 0, 0, 0,
                    FE_ICP_SMALL_THREADS);
   if (rc == SFE_OK && two)
-    rc = icp_run(ctx, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
+    rc = icp_run(ctx, st, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
                  nullptr, nullptr, n, p.cap_source, p.cap_target, fe->guess + 9 * (size_t)f0,
                  fe->T + 9 * (size_t)f0, fe->iters + f0, fe->inliers + f0, fe->status + f0, fe->cnt_a + f0, cap, 2,
                  ns_small, nt_small);
@@ -564,7 +599,7 @@ static int fe_match(sfe_frontend *fe, int f0, int n) {
 // After a batch: the carried window becomes the last `window` frames of (carried ++ batch), stream-ordered after
 // the batch's matching (which still reads the old carried clouds).  Slots move towards the front, in ascending
 // order, so no frame is overwritten before it has been moved.
-static int fe_update_carry(sfe_frontend *fe, const double *poses, int n) {
+static int fe_update_carry(sfe_frontend *fe, cudaStream_t st, const double *poses, int n) {
   if (!fe->carry_on) return SFE_OK;
   const int W = fe->p.window, C = fe->carry_n, total = C + n, keep = total < W ? total : W;
   const size_t cap = fe->p.cap_points, cbytes = cap * 2 * sizeof(float);
@@ -575,15 +610,15 @@ static int fe_update_carry(sfe_frontend *fe, const double *poses, int n) {
     if (v < C) {
       if (v != j) {
         SFE_CUDA(cudaMemcpyAsync(fe->carry_xy + (size_t)j * cap * 2, fe->carry_xy + (size_t)v * cap * 2, cbytes,
-                                 cudaMemcpyDeviceToDevice, fe->ctx->stream));
-        SFE_CUDA(cudaMemcpyAsync(fe->carry_cnt + j, fe->carry_cnt + v, 4, cudaMemcpyDeviceToDevice, fe->ctx->stream));
+                                 cudaMemcpyDeviceToDevice, st));
+        SFE_CUDA(cudaMemcpyAsync(fe->carry_cnt + j, fe->carry_cnt + v, 4, cudaMemcpyDeviceToDevice, st));
         memcpy(fe->carry_poses + 3 * (size_t)j, fe->carry_poses + 3 * (size_t)v, 3 * sizeof(double));
       }
     } else {
       const size_t b = (size_t)(v - C);
       SFE_CUDA(cudaMemcpyAsync(fe->carry_xy + (size_t)j * cap * 2, cloud + b * cap * 2, cbytes, cudaMemcpyDeviceToDevice,
-                               fe->ctx->stream));
-      SFE_CUDA(cudaMemcpyAsync(fe->carry_cnt + j, cnt + b, 4, cudaMemcpyDeviceToDevice, fe->ctx->stream));
+                               st));
+      SFE_CUDA(cudaMemcpyAsync(fe->carry_cnt + j, cnt + b, 4, cudaMemcpyDeviceToDevice, st));
       memcpy(fe->carry_poses + 3 * (size_t)j, poses + 3 * b, 3 * sizeof(double));
     }
   }
@@ -604,6 +639,13 @@ int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_hos
   if (dst) memcpy(fe->img_lut, lut_bgr_host, sizeof(fe->img_lut));
   fe->img_dst = dst;
   fe->img_dst_host = dst_is_host != 0;
+  return SFE_OK;
+}
+
+int sfe_frontend_set_overlap(sfe_frontend *fe, int sub_batch_frames) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_overlap: null handle");
+  SFE_REQUIRE(sub_batch_frames >= 0, "sfe_frontend_set_overlap: negative sub-batch size %d", sub_batch_frames);
+  fe->overlap = sub_batch_frames;
   return SFE_OK;
 }
 
@@ -636,6 +678,42 @@ int sfe_frontend_get_timing(sfe_frontend *fe, double *stage_ms, int64_t *stage_c
   return SFE_OK;
 }
 
+}  // extern "C"
+
+// `after` waits for what has been enqueued on `before` so far
+static int fe_order(cudaStream_t before, cudaEvent_t ev, cudaStream_t after) {
+  SFE_CUDA(cudaEventRecord(ev, before));
+  SFE_CUDA(cudaStreamWaitEvent(after, ev, 0));
+  return SFE_OK;
+}
+
+// The overlapped schedule of run_dev (DESIGN.md section 4): the batch in sub-batches of fe->overlap frames, the
+// feature stages of every sub-batch on feat_stream, submap + ICP of sub-batch k on match_stream once the features of
+// sub-batch k are done -- its window reaches back only into sub-batches <= k.  So the HBM-bound CFAR of sub-batch k+1
+// runs next to the latency-bound ICP of sub-batch k, and each stage's tail is filled by the other side's CTAs.  Both
+// streams fork from ctx->stream (after the pose upload and anything the caller enqueued there) and join back into it,
+// so ctx->stream orders later work -- the next call included -- after the whole batch.
+static int fe_run_overlapped(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  const int S = fe->overlap;
+  int rc = fe_order(ctx->stream, fe->ev_fork, fe->feat_stream);
+  if (rc == SFE_OK) rc = fe_order(ctx->stream, fe->ev_fork, fe->match_stream);
+  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += S) {
+    const int n = std::min(S, n_frames - f0);
+    rc = fe_features(fe, fe->feat_stream, frames_dev + (size_t)f0 * fbytes, f0, n);
+    if (rc == SFE_OK) rc = fe_order(fe->feat_stream, fe->ev_feat, fe->match_stream);
+    if (rc == SFE_OK) rc = fe_match(fe, fe->match_stream, f0, n);
+  }
+  if (rc == SFE_OK) rc = fe_update_carry(fe, fe->match_stream, poses_host, n_frames);
+  // join on every path, so that whatever did get enqueued is ordered before later work on ctx->stream
+  const int rj = fe_order(fe->feat_stream, fe->ev_join, ctx->stream);
+  const int rm = fe_order(fe->match_stream, fe->ev_join, ctx->stream);
+  return rc != SFE_OK ? rc : (rj != SFE_OK ? rj : rm);
+}
+
+extern "C" {
+
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
   SFE_REQUIRE(fe && frames_dev && poses_host, "sfe_frontend_run_dev: null argument");
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_dev: %d frames exceed max_frames %d",
@@ -650,11 +728,13 @@ int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const doub
     rc = feature_image_run(fe->ctx, fe->maps, frames_dev, n_frames, fe->img_lut, fe->img_dst, "sfe_frontend_run_dev");
     if (rc != SFE_OK) return rc;
   }
-  rc = fe_features(fe, frames_dev, 0, n_frames);
+  // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
+  if (fe->overlap > 0 && !fe->timing) return fe_run_overlapped(fe, frames_dev, poses_host, n_frames);
+  rc = fe_features(fe, fe->ctx->stream, frames_dev, 0, n_frames);
   if (rc != SFE_OK) return rc;
-  rc = fe_match(fe, 0, n_frames);
+  rc = fe_match(fe, fe->ctx->stream, 0, n_frames);
   if (rc != SFE_OK) return rc;
-  return fe_update_carry(fe, poses_host, n_frames);
+  return fe_update_carry(fe, fe->ctx->stream, poses_host, n_frames);
 }
 
 int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, const int32_t **iters, const int32_t **inliers,
@@ -700,12 +780,12 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
     SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
     int rc = fe_render_chunk(fe, f0, n, k, "sfe_frontend_run_host");
     if (rc != SFE_OK) return rc;
-    rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
+    rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
     if (rc != SFE_OK) return rc;
-    rc = fe_match(fe, f0, n);  // its window only reaches back into chunks already processed
+    rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
     if (rc != SFE_OK) return rc;
   }
-  int rc = fe_update_carry(fe, poses_host, n_frames);
+  int rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
@@ -767,8 +847,8 @@ static int fe_run_compressed(sfe_frontend *fe, typename Fmt::Batch *bt, const do
         return SFE_ERR_ARG;
       }
     rc = fe_render_chunk(fe, f0, n, k, what);
-    if (rc == SFE_OK) rc = fe_features(fe, fe->frames + (size_t)f0 * fbytes, f0, n);
-    if (rc == SFE_OK) rc = fe_match(fe, f0, n);
+    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
+    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
   }
   return rc;
 }
@@ -796,7 +876,7 @@ static int fe_run_compressed_host(sfe_frontend *fe, const uint8_t *bytes, const 
   if (rc == SFE_OK) rc = fe_run_compressed<Fmt>(fe, bt, poses_host, n_frames, chunk_frames, what);
   Fmt::free(bt);
   if (rc != SFE_OK) return rc;
-  rc = fe_update_carry(fe, poses_host, n_frames);
+  rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));

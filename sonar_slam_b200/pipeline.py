@@ -138,6 +138,12 @@ class FrontEnd:
         as the window of the next call's first frames (sfe_frontend_set_carry).  False: every call starts cold."""
         _lib.check(self.lib.sfe_frontend_set_carry(self.handle, 1 if enable else 0), "sfe_frontend_set_carry")
 
+    def set_overlap(self, sub_batch_frames):
+        """Schedule of run_dev (sfe_frontend_set_overlap): > 0 overlaps the feature stages of one sub-batch of that
+        many frames with the scan matching of the previous one on two streams; 0 (the default) runs every stage over
+        the whole batch one after another.  The results are the same either way."""
+        _lib.check(self.lib.sfe_frontend_set_overlap(self.handle, int(sub_batch_frames)), "sfe_frontend_set_overlap")
+
     STAGES = ("cfar", "cart_points", "downsample", "remove_outlier", "submap", "icp")
 
     def set_timing(self, enable=True):
