@@ -67,6 +67,39 @@ struct IcpBatch {
   int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
 };
 
+// Per-phase cycle counts (development build, -DSFE_ICP_PHASE_CLOCKS; tools/build_icp_variants.sh, tools/icp_phases.py):
+// thread 0 of every CTA reads clock64() at the phase boundaries below and adds its totals to a global array when the
+// CTA exits.  Phases: 0 set-up (mean, grid, coarse map) per problem; per iteration 1 search + re-search list, 2
+// trimmed-quantile select, 3 keep count, 4 means sums, 5 covariance sums, 6 fit + end barrier.  Thread 0 belongs to
+// warp 0, which runs the sums and the fit, so the counts follow the CTA's critical path.  Off: no code at all.
+#ifdef SFE_ICP_PHASE_CLOCKS
+constexpr int ICP_PHASES = 7;
+__device__ unsigned long long icp_phase_cycles[ICP_PHASES], icp_phase_count[ICP_PHASES];
+static int icp_phase_per_sm[3];  // CTAs per SM of the last 128 / 256 / 512-thread launch
+#define ICP_PH_DECL long long ph_t = 0, ph_acc[ICP_PHASES] = {}, ph_cnt[ICP_PHASES] = {};
+#define ICP_PH_START() (threadIdx.x == 0 ? (void)(ph_t = clock64()) : (void)0)
+#define ICP_PH_MARK(k)                           \
+  do {                                           \
+    if (threadIdx.x == 0) {                      \
+      const long long t_ = clock64();            \
+      ph_acc[k] += t_ - ph_t, ph_cnt[k] += 1;    \
+      ph_t = t_;                                 \
+    }                                            \
+  } while (0)
+#define ICP_PH_FLUSH()                                                                              \
+  do {                                                                                              \
+    if (threadIdx.x == 0)                                                                           \
+      _Pragma("unroll") for (int k_ = 0; k_ < ICP_PHASES; ++k_)                                     \
+        atomicAdd(&icp_phase_cycles[k_], (unsigned long long)ph_acc[k_]),                          \
+            atomicAdd(&icp_phase_count[k_], (unsigned long long)ph_cnt[k_]);                       \
+  } while (0)
+#else
+#define ICP_PH_DECL
+#define ICP_PH_START() ((void)0)
+#define ICP_PH_MARK(k) ((void)0)
+#define ICP_PH_FLUSH() ((void)0)
+#endif
+
 constexpr int ICP_SM_SLOTS = 256;  // >= %nsmid on every sm_90 part
 __device__ __forceinline__ unsigned icp_smid() {
   unsigned r;
@@ -159,17 +192,19 @@ struct IcpShared {  // small fixed-size part of the shared state
   float mean[2];
   float bbox[4];
   int iterate, status, count, inliers;
-  int sel_bin, sel_k;
   uint32_t sel_val;  // radix select: the element found alone in its bin
+  int todo_n;        // one-pass path: length of the re-search list
   int hist[3][256];  // radix-select histograms, used in rotation (block_select_kth)
   int scan[36];
   int tot[2][16];
-  double red[2 * 5 * 16];  // <= 16 warps per CTA
-  float wred[4 * 16];      // per-warp partials of the bounding-box / maximum reductions
+  float wred[4 * 16];  // per-warp partials of the bounding-box / maximum reductions
   float hq_w[ICP_HIST], hq_z[ICP_HIST], ht_x[ICP_HIST], ht_y[ICP_HIST];
   int hn;
-  float seq[4];               // results of the sequential sums
-  __align__(16) float seq_buf[2 * 4 * 36];  // staging of seq_sum4_warp
+  float seq[2];  // reference mean (sequential sums)
+  union {        // a launch runs one accumulation mode (flags bit 1)
+    double red[2 * 5 * 16];                   // float64 mode: block_sum, <= 16 warps per CTA
+    __align__(16) float seq_buf[2 * 4 * 36];  // sequential mode: staging of seq_sum4_warp
+  };
   int cnx, cny;               // coarse occupancy grid (ICP_COARSE x ICP_COARSE fine cells per coarse cell)
   uint32_t coarse[ICP_COARSE_WORDS];
 };
@@ -410,12 +445,13 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
   off = (off + 15) & ~size_t(15);
   // PLANE only: 640 floats for seq_sum9_warp.  dist[] is dead between the weights (3c) and the next iteration's
   // search, which rewrites all of it: launches with room for 640 source points (the front end's small class is
-  // exactly that, and sized to six CTAs per SM to the byte; 2 000 x 20 000 points leave nothing to spare at all)
-  // park the scratch there, smaller ones get their own 2.5 KB.
+  // exactly that; 2 000 x 20 000 points leave nothing to spare at all) park the scratch there, smaller ones get
+  // their own 2.5 KB.
   float *pl_scratch = b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
   (void)pl_scratch;
 
   const int tid = threadIdx.x, nthr = blockDim.x;
+  ICP_PH_DECL
   int red_phase = 0, tot_phase = 0, sel_pass = 0;  // rotation counters of the one-barrier reductions (CTA-uniform)
   for (int h = threadIdx.x; h < 3 * 256; h += blockDim.x) (&sh.hist[0][0])[h] = 0;
   // Problems that allow one CTA per SM (config 3: ~200 KB of shared memory) are launched one CTA per problem, not
@@ -436,10 +472,9 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
   const bool seq = (prm.flags & 2) == 0;
 
   // Persistent CTAs take problems from a work counter: problems differ in length (cloud sizes, early exits), and with
-  // a static share the batch ends when the CTAs that drew the most work finish -- at the front end's 4096 problems
-  // over 6 x 132 CTAs, 136 CTAs run a sixth problem while the other 656 are done.  Problem p's results do not depend
+  // a static share the batch ends when the CTAs that drew the most work finish.  Problem p's results do not depend
   // on the CTA that solves it.  The index is broadcast through sh.status, which thread 0 rewrites only after the
-  // next problem's first barrier (the shared-memory layout is sized to the byte, so no field is added for it).
+  // next problem's first barrier.
   for (int p = blockIdx.x; p < b.P; p = b.next ? next_work_item(b.next, &sh.status) : p + (int)gridDim.x) {
     const int si = b.src_id ? b.src_id[p] : p, ti = b.tgt_id ? b.tgt_id[p] : p;
     const float *src = b.src_pts + 2 * (size_t)b.src_off[si];
@@ -469,6 +504,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       continue;
     }
 
+    ICP_PH_START();
     // ---- 1. mean of the reference, bounding box of the centred reference
     {
       float mx, my;
@@ -573,7 +609,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       sh.ht_x[0] = 0.f, sh.ht_y[0] = 0.f;
       sh.hn = 1;
       sh.iterate = 1;
-      sh.sel_val = 0;  // (also the one-pass path's list counter, see 3a)
+      sh.todo_n = 0;
     }
     __syncthreads();
     for (int i = tid; i < ns; i += nthr) {
@@ -615,6 +651,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       __syncthreads();
     }
 
+    ICP_PH_MARK(0);
     // ---- 3. iterations
     while (true) {
       float Ti[9];
@@ -631,7 +668,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       //           from above: call it U.  An unsettled point whose search proves "farther than U" has weight
       //           0 and needs no exact distance.  Results are identical to an exhaustive search (same
       //           quantile element, same kept pairs); the far outliers of a scan stop costing O(area).
-      int n_fin = 0;
+      int n_fin = 0, total_fin = -1;
       const bool small = ns <= b.small_mult * nthr && nt <= 4096;  // few, cheap searches: one exact pass, no pruning
       // Certified matches.  A search that scans at least the 3x3 block also yields a lower bound L on the distance
       // from the point to every target point OTHER than its match (grid.cuh: nn_query_certified).  The point then
@@ -663,9 +700,9 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
         if constexpr (THREADS <= 256) {
           // Two halves, so that the lanes of a warp stay on one code path.  First every point tests its certificate
           // (one distance; points without a seed search at once: that is the first iteration, all lanes together);
-          // the points whose certificate failed are only LISTED -- in match[], which is rewritten below anyway, with
-          // the counter in sel_val (zeroed by the single-thread step of the previous iteration).  Then the list is
-          // searched densely.  In one loop the re-search ran with 2.4 of 32 lanes active and took 25 % of this
+          // the points whose certificate failed are only LISTED -- in match[], which the weights (3c) rewrite from
+          // prev[], with the counter in todo_n (zeroed by the single-thread step of the previous iteration).  Then the
+          // list is searched densely.  In one loop the re-search ran with 2.4 of 32 lanes active and took 25 % of this
           // kernel's warp instructions on the front end's problems (tools/ncu_call_sites.py).
           uint16_t *todo = match;
           for (int base = 0; base < ns; base += nthr) {
@@ -694,13 +731,13 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
             if (m) {  // one shared-memory atomic per warp
               const int lane = tid & 31, lead = __ffs(m) - 1;
               int at = 0;
-              if (lane == lead) at = (int)atomicAdd(&sh.sel_val, (uint32_t)__popc(m));
+              if (lane == lead) at = atomicAdd(&sh.todo_n, __popc(m));
               at = __shfl_sync(0xffffffffu, at, lead);
               if (later) todo[at + __popc(m & ((1u << lane) - 1u))] = (uint16_t)i;
             }
           }
           __syncthreads();
-          const int n_todo = (int)sh.sel_val;
+          const int n_todo = sh.todo_n;
           for (int k = tid; k < n_todo; k += nthr) {
             const int i = todo[k];
             const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
@@ -713,8 +750,8 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
             prev[i] = r.pos >= 0 ? (uint16_t)r.pos : (uint16_t)0xffff;
             n_fin += r.pos >= 0;
           }
-          __syncthreads();
-          for (int i = tid; i < ns; i += nthr) match[i] = prev[i];
+          // the matches are prev[] now (3c reads them there); this barrier also publishes prev[] and dist[]
+          total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);
         } else {
           // (512-thread CTAs rarely see a problem this small: the single loop is kept there, and with it the code of the
           //  config-3 instantiation)
@@ -814,7 +851,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
         n_fin += verdict;
         dist[i] = verdict ? max_d2 : INFINITY;  // upper bound of a finite point without candidate
       }
-      const int total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);  // (its barrier also publishes dist[] / qstate[])
+      if (total_fin < 0) total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);  // (its barrier also publishes dist[] / qstate[])
       // pass C: settle what still matters
       if (!small) {
         float stop_d2 = INFINITY;
@@ -862,9 +899,10 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
             }
           }
         }
+        __syncthreads();
       }
-      __syncthreads();
 
+      ICP_PH_MARK(1);
       // 3b. trimmed-distance limit = element floor(float(n)*ratio) of the ascending finite distances
       float limit = INFINITY;
       if (prm.trim_ratio >= 0.f) {
@@ -893,61 +931,85 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
         }
       }
 
-      // 3c. kept pairs: count and sums for the means
-      int n_keep;
+      ICP_PH_MARK(2);
+      // 3c. kept pairs.  The candidate match of point i is prev[i] on the one-pass path (its re-search list took
+      // match[] meanwhile) and match[i] after the pruning passes; match[i] becomes the candidate or 0xffff (dropped).
+      const uint16_t *cand = small ? prev : match;
+      auto kept = [&](int i) -> int {
+        const int m = cand[i];
+        bool keep = m != 0xffff;
+        if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
+        if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
+        return keep ? m : 0xffff;
+      };
+      // Sequential mode: the sums are warp 0's alone, so warp 0 also forms the fit and, on the one-pass path, the
+      // weights, with warp-level synchronisation only; the other warps go straight to the barrier that ends the
+      // iteration.  (The pruned path's 2 000-point sources keep the weights parallel: measured slower on warp 0.)
+      // Float64 mode: every thread takes part in the block_sum reductions.
+      int n_keep = 0;
       float mrx = 0.f, mry = 0.f, mfx = 0.f, mfy = 0.f;
-      if (seq) {
-        int cnt = 0;
-        for (int i = tid; i < ns; i += nthr) {
-          bool keep = match[i] != 0xffff;
-          if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
-          if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
-          if (!keep) match[i] = 0xffff;
-          cnt += keep;
-        }
-        n_keep = block_total(cnt, &sh.tot[0][0], tot_phase);  // (its barrier publishes match[])
-      } else {
-        double s5[5] = {0, 0, 0, 0, 0}, t5[5];
-        for (int i = tid; i < ns; i += nthr) {
-          bool keep = match[i] != 0xffff;
-          if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
-          if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
-          if (!keep) {
-            match[i] = 0xffff;
-            continue;
-          }
-          const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-          const float2 r = sorted[match[i]];
-          s5[0] += 1.0, s5[1] += (double)q.x, s5[2] += (double)q.y, s5[3] += (double)r.x, s5[4] += (double)r.y;
-        }
-        block_sum<5>(s5, sh.red, red_phase, t5);
-        n_keep = (int)t5[0];
-        mrx = (float)t5[1], mry = (float)t5[2], mfx = (float)t5[3], mfy = (float)t5[4];
-      }
-      if (n_keep == 0) {
-        if (tid == 0) sh.status = ICP_NO_POINT;
-        __syncthreads();
-        break;
-      }
       double t4[4] = {0, 0, 0, 0};
       float pl[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};  // PLANE: A00 A01 A02 A11 A12 A22, sum F (q-r).n (thread 0)
-      if constexpr (PLANE) {
-        // 3c'/3d'. point-to-plane normal equations over the kept pairs (oracle/icp_ref.c, minimizer 1):
-        //   c = q.x n.y - q.y n.x,  F = (c, n.x, n.y),  A = sum F F^T,  b = -sum F ((q - r).n)
-        auto terms = [&](int i, float (&v)[9]) {
-          const int m = match[i];
-          const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-          const float2 r = sorted[m];
-          const float2 n = nrm[m];
-          const float cr = __fsub_rn(__fmul_rn(q.x, n.y), __fmul_rn(q.y, n.x));
-          const float dp = __fadd_rn(__fmul_rn(__fsub_rn(q.x, r.x), n.x), __fmul_rn(__fsub_rn(q.y, r.y), n.y));
-          v[0] = __fmul_rn(cr, cr), v[1] = __fmul_rn(cr, n.x), v[2] = __fmul_rn(cr, n.y), v[3] = __fmul_rn(n.x, n.x);
-          v[4] = __fmul_rn(n.x, n.y), v[5] = __fmul_rn(n.y, n.y), v[6] = __fmul_rn(cr, dp), v[7] = __fmul_rn(n.x, dp);
-          v[8] = __fmul_rn(n.y, dp);
-        };
-        if (seq) {
-          if (tid < 32) {  // nine sequential sums in one pass; dropped pairs add +0
-            const float sum = seq_sum9_warp(ns, pl_scratch, match, nrm, [&](int i, int m, float2 n, float (&v)[9]) {
+      if (seq && !small) {  // big problems (long serial sums): every thread forms the weights of its points
+        int cnt = 0;
+        for (int i = tid; i < ns; i += nthr) {
+          const int m = kept(i);
+          match[i] = (uint16_t)m;
+          cnt += m != 0xffff;
+        }
+        n_keep = block_total(cnt, &sh.tot[0][0], tot_phase);  // (its barrier publishes match[])
+      }
+      ICP_PH_MARK(3);
+      if (!seq || tid < 32) {
+        if (!seq) {
+          double s5[5] = {0, 0, 0, 0, 0}, t5[5];
+          for (int i = tid; i < ns; i += nthr) {
+            const int m = kept(i);
+            match[i] = (uint16_t)m;
+            if (m == 0xffff) continue;
+            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
+            const float2 r = sorted[m];
+            s5[0] += 1.0, s5[1] += (double)q.x, s5[2] += (double)q.y, s5[3] += (double)r.x, s5[4] += (double)r.y;
+          }
+          block_sum<5>(s5, sh.red, red_phase, t5);
+          n_keep = (int)t5[0];
+          mrx = (float)t5[1], mry = (float)t5[2], mfx = (float)t5[3], mfy = (float)t5[4];
+        } else if (PLANE) {
+          if (small) {
+            int cnt = 0;
+            for (int i = tid; i < ns; i += 32) {
+              const int m = kept(i);
+              match[i] = (uint16_t)m;
+              cnt += m != 0xffff;
+            }
+            n_keep = __reduce_add_sync(0xffffffffu, cnt);
+            __syncwarp();  // (seq_sum9_warp's lanes read other lanes' match[] entries)
+          }
+        } else {
+          // the four sums (step x, step y, matched reference x, y); dropped pairs add +0
+          int cnt = 0;
+          const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
+            const int m = small ? kept(i) : match[i];
+            if (small) match[i] = (uint16_t)m;
+            if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
+            ++cnt;
+            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
+            const float2 r = sorted[m];
+            return make_float4(q.x, q.y, r.x, r.y);
+          });
+          if (small) n_keep = __reduce_add_sync(0xffffffffu, cnt);
+          mrx = __shfl_sync(0xffffffffu, sum, 0), mry = __shfl_sync(0xffffffffu, sum, 1);
+          mfx = __shfl_sync(0xffffffffu, sum, 2), mfy = __shfl_sync(0xffffffffu, sum, 3);
+          __syncwarp();  // (seq_buf and match[] are read again by other lanes below)
+        }
+        ICP_PH_MARK(4);
+        if (n_keep == 0) {
+          if (tid == 0) sh.status = ICP_NO_POINT;
+        } else {
+          if constexpr (PLANE) {
+            // 3c'/3d'. point-to-plane normal equations over the kept pairs (oracle/icp_ref.c, minimizer 1):
+            //   c = q.x n.y - q.y n.x,  F = (c, n.x, n.y),  A = sum F F^T,  b = -sum F ((q - r).n)
+            auto terms = [&](int i, int m, float2 n, float (&v)[9]) {
               const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
               const float2 r = sorted[m];
               const float cr = __fsub_rn(__fmul_rn(q.x, n.y), __fmul_rn(q.y, n.x));
@@ -955,158 +1017,141 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
               v[0] = __fmul_rn(cr, cr), v[1] = __fmul_rn(cr, n.x), v[2] = __fmul_rn(cr, n.y), v[3] = __fmul_rn(n.x, n.x);
               v[4] = __fmul_rn(n.x, n.y), v[5] = __fmul_rn(n.y, n.y), v[6] = __fmul_rn(cr, dp), v[7] = __fmul_rn(n.x, dp);
               v[8] = __fmul_rn(n.y, dp);
-            });
-            __syncwarp();
-            if (tid < 9) sh.seq_buf[tid] = sum;
-          }
-          __syncthreads();
+            };
+            if (seq) {  // nine sequential sums in one pass; dropped pairs add +0
+              const float sum = seq_sum9_warp(ns, pl_scratch, match, nrm, terms);
 #pragma unroll
-          for (int k = 0; k < 9; ++k) pl[k] = sh.seq_buf[k];
-          __syncthreads();  // seq_buf is scratch again next iteration
-        } else {
-          double s5[5] = {0, 0, 0, 0, 0}, s4[4] = {0, 0, 0, 0}, o5[5], o4[4];
-          for (int i = tid; i < ns; i += nthr) {
-            if (match[i] == 0xffff) continue;
-            float v[9];
-            terms(i, v);
+              for (int k = 0; k < 9; ++k) pl[k] = __shfl_sync(0xffffffffu, sum, k);
+            } else {
+              double s5[5] = {0, 0, 0, 0, 0}, s4[4] = {0, 0, 0, 0}, o5[5], o4[4];
+              for (int i = tid; i < ns; i += nthr) {
+                const int m = match[i];
+                if (m == 0xffff) continue;
+                float v[9];
+                terms(i, m, nrm[m], v);
 #pragma unroll
-            for (int k = 0; k < 5; ++k) s5[k] += (double)v[k];
+                for (int k = 0; k < 5; ++k) s5[k] += (double)v[k];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) s4[k] += (double)v[5 + k];
-          }
-          block_sum<5>(s5, sh.red, red_phase, o5);
-          block_sum<4>(s4, sh.red, red_phase, o4);
+                for (int k = 0; k < 4; ++k) s4[k] += (double)v[5 + k];
+              }
+              block_sum<5>(s5, sh.red, red_phase, o5);
+              block_sum<4>(s4, sh.red, red_phase, o4);
 #pragma unroll
-          for (int k = 0; k < 5; ++k) pl[k] = (float)o5[k];
+              for (int k = 0; k < 5; ++k) pl[k] = (float)o5[k];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) pl[5 + k] = (float)o4[k];
-        }
-      } else {
-        if (seq) {
-          // warp 0 forms the four sums (step x, step y, matched reference x, y); dropped pairs add +0
-          if (tid < 32) {
-            const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
-              const int m = match[i];
-              if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
-              const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-              const float2 r = sorted[m];
-              return make_float4(q.x, q.y, r.x, r.y);
-            });
-            if (tid < 4) sh.seq[tid] = sum;
-          }
-          __syncthreads();
-          mrx = sh.seq[0], mry = sh.seq[1], mfx = sh.seq[2], mfy = sh.seq[3];
-          __syncthreads();  // sh.seq is rewritten below
-        }
-        const float winv = __fdiv_rn(1.0f, (float)n_keep);
-        mrx = __fmul_rn(mrx, winv), mry = __fmul_rn(mry, winv);
-        mfx = __fmul_rn(mfx, winv), mfy = __fmul_rn(mfy, winv);
-
-        // 3d. cross-covariance of the centred pairs
-        if (seq) {
-          if (tid < 32) {  // m00 = qx*px, m01 = qx*py, m10 = qy*px, m11 = qy*py
-            const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
-              const int m = match[i];
-              if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
-              const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-              const float2 r = sorted[m];
-              const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
-              const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
-              return make_float4(__fmul_rn(qx, px), __fmul_rn(qx, py), __fmul_rn(qy, px), __fmul_rn(qy, py));
-            });
-            if (tid < 4) sh.seq[tid] = sum;
-          }
-          __syncthreads();
-          t4[0] = (double)sh.seq[0], t4[1] = (double)sh.seq[1], t4[2] = (double)sh.seq[2], t4[3] = (double)sh.seq[3];
-        } else {
-          double s4[4] = {0, 0, 0, 0};
-          for (int i = tid; i < ns; i += nthr) {
-            if (match[i] == 0xffff) continue;
-            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-            const float2 r = sorted[match[i]];
-            const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
-            const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
-            s4[0] += (double)__fmul_rn(qx, px), s4[1] += (double)__fmul_rn(qx, py);
-            s4[2] += (double)__fmul_rn(qy, px), s4[3] += (double)__fmul_rn(qy, py);
-          }
-          block_sum<4>(s4, sh.red, red_phase, t4);
-        }
-      }
-
-      // 3e. rigid fit, T_iter update, checkers (one thread)
-      if (tid == 0) {
-        float c = 1.f, s = 0.f, tx, ty;
-        if constexpr (PLANE) {
-          // A x = b by Cholesky (A.llt()); an unknown whose pivot is not positive stays 0
-          const float a00 = pl[0], a01 = pl[1], a02 = pl[2], a11 = pl[3], a12 = pl[4], a22 = pl[5];
-          const float b0 = -pl[6], b1 = -pl[7], b2 = -pl[8];
-          float l00 = 0.f, l10 = 0.f, l20 = 0.f, l11 = 0.f, l21 = 0.f, l22 = 0.f;
-          const bool p0 = a00 > 0.f;
-          if (p0) l00 = __fsqrt_rn(a00), l10 = __fdiv_rn(a01, l00), l20 = __fdiv_rn(a02, l00);
-          const float d1 = __fsub_rn(a11, __fmul_rn(l10, l10));
-          const bool p1 = d1 > 0.f;
-          if (p1) l11 = __fsqrt_rn(d1), l21 = __fdiv_rn(__fsub_rn(a12, __fmul_rn(l20, l10)), l11);
-          const float d2 = __fsub_rn(__fsub_rn(a22, __fmul_rn(l20, l20)), __fmul_rn(l21, l21));
-          const bool p2 = d2 > 0.f;
-          if (p2) l22 = __fsqrt_rn(d2);
-          const float y0 = p0 ? __fdiv_rn(b0, l00) : 0.f;
-          const float y1 = p1 ? __fdiv_rn(__fsub_rn(b1, __fmul_rn(l10, y0)), l11) : 0.f;
-          const float y2 = p2 ? __fdiv_rn(__fsub_rn(__fsub_rn(b2, __fmul_rn(l20, y0)), __fmul_rn(l21, y1)), l22) : 0.f;
-          const float x2 = p2 ? __fdiv_rn(y2, l22) : 0.f;
-          const float x1 = p1 ? __fdiv_rn(__fsub_rn(y1, __fmul_rn(l21, x2)), l11) : 0.f;
-          const float x0 = p0 ? __fdiv_rn(__fsub_rn(__fsub_rn(y0, __fmul_rn(l10, x1)), __fmul_rn(l20, x2)), l00) : 0.f;
-          c = (float)cos((double)x0), s = (float)sin((double)x0);  // Rotation2D(x0)
-          tx = x1, ty = x2;
-        } else {
-          const float m00 = (float)t4[0], m01 = (float)t4[1], m10 = (float)t4[2], m11 = (float)t4[3];
-          const float a = __fadd_rn(m00, m11), bq = __fsub_rn(m10, m01);
-          const float h = sqrtf(__fadd_rn(__fmul_rn(a, a), __fmul_rn(bq, bq)));
-          if (h > 0.f) c = __fdiv_rn(a, h), s = __fdiv_rn(bq, h);
-          tx = __fsub_rn(mfx, __fadd_rn(__fmul_rn(c, mrx), __fmul_rn(-s, mry)));
-          ty = __fsub_rn(mfy, __fadd_rn(__fmul_rn(s, mrx), __fmul_rn(c, mry)));
-        }
-        const float dT[9] = {c, -s, tx, s, c, ty, 0.f, 0.f, 1.f};
-        float Tn[9];
-        mat3_mul_rn(dT, Ti, Tn);
-#pragma unroll
-        for (int i = 0; i < 9; ++i) sh.Tprev[i] = Ti[i], sh.Ti[i] = Tn[i];
-        sh.sel_val = 0;  // the next iteration's list counter (the select that also uses it is done)
-        sh.inliers = n_keep;
-        const int count = ++sh.count;
-        bool counter_stop = false;
-        if (count >= prm.max_iterations) sh.iterate = 0, counter_stop = true;
-        if (!counter_stop && smooth > 0) {
-          int hn = sh.hn;
-          if (hn == ICP_HIST) {
-            for (int i = 0; i + 1 < ICP_HIST; ++i)
-              sh.hq_w[i] = sh.hq_w[i + 1], sh.hq_z[i] = sh.hq_z[i + 1], sh.ht_x[i] = sh.ht_x[i + 1],
-              sh.ht_y[i] = sh.ht_y[i + 1];
-            hn = ICP_HIST - 1;
-          }
-          rot_to_quat(Tn, sh.hq_w[hn], sh.hq_z[hn]);
-          sh.ht_x[hn] = Tn[2], sh.ht_y[hn] = Tn[5];
-          ++hn;
-          sh.hn = hn;
-          float vr = 0.f, vt = 0.f;
-          if (hn > smooth) {
-            for (int i = hn - 1; i >= hn - smooth; --i) {
-              const float dw = __fadd_rn(__fmul_rn(sh.hq_w[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_z[i], sh.hq_z[i - 1]));
-              const float dz = __fsub_rn(__fmul_rn(sh.hq_z[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_w[i], sh.hq_z[i - 1]));
-              vr = __fadd_rn(vr, fabsf(__fmul_rn(2.0f, atan2f(fabsf(dz), fabsf(dw)))));
-              const float ex = __fsub_rn(sh.ht_x[i], sh.ht_x[i - 1]), ey = __fsub_rn(sh.ht_y[i], sh.ht_y[i - 1]);
-              vt = __fadd_rn(vt, fabsf(sqrtf(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)))));
+              for (int k = 0; k < 4; ++k) pl[5 + k] = (float)o4[k];
             }
-            vr = __fdiv_rn(vr, (float)smooth);
-            vt = __fdiv_rn(vt, (float)smooth);
-            if (vr < prm.min_diff_rot && vt < prm.min_diff_trans) sh.iterate = 0;
+          } else {
+            const float winv = __fdiv_rn(1.0f, (float)n_keep);
+            mrx = __fmul_rn(mrx, winv), mry = __fmul_rn(mry, winv);
+            mfx = __fmul_rn(mfx, winv), mfy = __fmul_rn(mfy, winv);
+
+            // 3d. cross-covariance of the centred pairs
+            if (seq) {  // m00 = qx*px, m01 = qx*py, m10 = qy*px, m11 = qy*py
+              const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
+                const int m = match[i];
+                if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
+                const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
+                const float2 r = sorted[m];
+                const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
+                const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
+                return make_float4(__fmul_rn(qx, px), __fmul_rn(qx, py), __fmul_rn(qy, px), __fmul_rn(qy, py));
+              });
+#pragma unroll
+              for (int k = 0; k < 4; ++k) t4[k] = (double)__shfl_sync(0xffffffffu, sum, k);
+            } else {
+              double s4[4] = {0, 0, 0, 0};
+              for (int i = tid; i < ns; i += nthr) {
+                if (match[i] == 0xffff) continue;
+                const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
+                const float2 r = sorted[match[i]];
+                const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
+                const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
+                s4[0] += (double)__fmul_rn(qx, px), s4[1] += (double)__fmul_rn(qx, py);
+                s4[2] += (double)__fmul_rn(qy, px), s4[3] += (double)__fmul_rn(qy, py);
+              }
+              block_sum<4>(s4, sh.red, red_phase, t4);
+            }
           }
-          if (vr != vr)
-            sh.status = ICP_NAN_ROT;
-          else if (vt != vt)
-            sh.status = ICP_NAN_TRANS;
+
+          ICP_PH_MARK(5);
+          // 3e. rigid fit, T_iter update, checkers (one thread)
+          if (tid == 0) {
+            float c = 1.f, s = 0.f, tx, ty;
+            if constexpr (PLANE) {
+              // A x = b by Cholesky (A.llt()); an unknown whose pivot is not positive stays 0
+              const float a00 = pl[0], a01 = pl[1], a02 = pl[2], a11 = pl[3], a12 = pl[4], a22 = pl[5];
+              const float b0 = -pl[6], b1 = -pl[7], b2 = -pl[8];
+              float l00 = 0.f, l10 = 0.f, l20 = 0.f, l11 = 0.f, l21 = 0.f, l22 = 0.f;
+              const bool p0 = a00 > 0.f;
+              if (p0) l00 = __fsqrt_rn(a00), l10 = __fdiv_rn(a01, l00), l20 = __fdiv_rn(a02, l00);
+              const float d1 = __fsub_rn(a11, __fmul_rn(l10, l10));
+              const bool p1 = d1 > 0.f;
+              if (p1) l11 = __fsqrt_rn(d1), l21 = __fdiv_rn(__fsub_rn(a12, __fmul_rn(l20, l10)), l11);
+              const float d2 = __fsub_rn(__fsub_rn(a22, __fmul_rn(l20, l20)), __fmul_rn(l21, l21));
+              const bool p2 = d2 > 0.f;
+              if (p2) l22 = __fsqrt_rn(d2);
+              const float y0 = p0 ? __fdiv_rn(b0, l00) : 0.f;
+              const float y1 = p1 ? __fdiv_rn(__fsub_rn(b1, __fmul_rn(l10, y0)), l11) : 0.f;
+              const float y2 = p2 ? __fdiv_rn(__fsub_rn(__fsub_rn(b2, __fmul_rn(l20, y0)), __fmul_rn(l21, y1)), l22) : 0.f;
+              const float x2 = p2 ? __fdiv_rn(y2, l22) : 0.f;
+              const float x1 = p1 ? __fdiv_rn(__fsub_rn(y1, __fmul_rn(l21, x2)), l11) : 0.f;
+              const float x0 = p0 ? __fdiv_rn(__fsub_rn(__fsub_rn(y0, __fmul_rn(l10, x1)), __fmul_rn(l20, x2)), l00) : 0.f;
+              c = (float)cos((double)x0), s = (float)sin((double)x0);  // Rotation2D(x0)
+              tx = x1, ty = x2;
+            } else {
+              const float m00 = (float)t4[0], m01 = (float)t4[1], m10 = (float)t4[2], m11 = (float)t4[3];
+              const float a = __fadd_rn(m00, m11), bq = __fsub_rn(m10, m01);
+              const float h = sqrtf(__fadd_rn(__fmul_rn(a, a), __fmul_rn(bq, bq)));
+              if (h > 0.f) c = __fdiv_rn(a, h), s = __fdiv_rn(bq, h);
+              tx = __fsub_rn(mfx, __fadd_rn(__fmul_rn(c, mrx), __fmul_rn(-s, mry)));
+              ty = __fsub_rn(mfy, __fadd_rn(__fmul_rn(s, mrx), __fmul_rn(c, mry)));
+            }
+            const float dT[9] = {c, -s, tx, s, c, ty, 0.f, 0.f, 1.f};
+            float Tn[9];
+            mat3_mul_rn(dT, Ti, Tn);
+#pragma unroll
+            for (int i = 0; i < 9; ++i) sh.Tprev[i] = Ti[i], sh.Ti[i] = Tn[i];
+            sh.todo_n = 0;  // the next iteration's list counter (read before this iteration's n_fin total)
+            sh.inliers = n_keep;
+            const int count = ++sh.count;
+            bool counter_stop = false;
+            if (count >= prm.max_iterations) sh.iterate = 0, counter_stop = true;
+            if (!counter_stop && smooth > 0) {
+              int hn = sh.hn;
+              if (hn == ICP_HIST) {
+                for (int i = 0; i + 1 < ICP_HIST; ++i)
+                  sh.hq_w[i] = sh.hq_w[i + 1], sh.hq_z[i] = sh.hq_z[i + 1], sh.ht_x[i] = sh.ht_x[i + 1],
+                  sh.ht_y[i] = sh.ht_y[i + 1];
+                hn = ICP_HIST - 1;
+              }
+              rot_to_quat(Tn, sh.hq_w[hn], sh.hq_z[hn]);
+              sh.ht_x[hn] = Tn[2], sh.ht_y[hn] = Tn[5];
+              ++hn;
+              sh.hn = hn;
+              float vr = 0.f, vt = 0.f;
+              if (hn > smooth) {
+                for (int i = hn - 1; i >= hn - smooth; --i) {
+                  const float dw = __fadd_rn(__fmul_rn(sh.hq_w[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_z[i], sh.hq_z[i - 1]));
+                  const float dz = __fsub_rn(__fmul_rn(sh.hq_z[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_w[i], sh.hq_z[i - 1]));
+                  vr = __fadd_rn(vr, fabsf(__fmul_rn(2.0f, atan2f(fabsf(dz), fabsf(dw)))));
+                  const float ex = __fsub_rn(sh.ht_x[i], sh.ht_x[i - 1]), ey = __fsub_rn(sh.ht_y[i], sh.ht_y[i - 1]);
+                  vt = __fadd_rn(vt, fabsf(sqrtf(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)))));
+                }
+                vr = __fdiv_rn(vr, (float)smooth);
+                vt = __fdiv_rn(vt, (float)smooth);
+                if (vr < prm.min_diff_rot && vt < prm.min_diff_trans) sh.iterate = 0;
+              }
+              if (vr != vr)
+                sh.status = ICP_NAN_ROT;
+              else if (vt != vt)
+                sh.status = ICP_NAN_TRANS;
+            }
+          }
         }
       }
       __syncthreads();
+      ICP_PH_MARK(6);
       if (sh.status != ICP_OK || !sh.iterate) break;
     }
 
@@ -1130,6 +1175,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
       b.status[p] = sh.status;
     }
   }
+  ICP_PH_FLUSH();
 }
 
 // pcl.match: nearest reference point (within max_dist) of every query point; one CTA per (ref, query) pair
@@ -1239,7 +1285,7 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
   b.T_out = T_out, b.iters = iters, b.inliers = inliers, b.status = status;
   b.P = P, b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
   b.max_cells = pick_max_cells(b.nt_max);
-  b.use_order = b.ns_max > 1024;  // (the front end's 640-point class is sized to 6 CTAs per SM to the byte)
+  b.use_order = b.ns_max > 1024;
   b.cell_scale = 1.0f;
   b.prm = *prm;
   {
@@ -1281,11 +1327,11 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
   // full 128 registers.
   const int variant = threads == 128 ? 0 : (threads == 256 ? 1 : (smem > 110 * 1024 ? 3 : 2));
   const bool plane = prm->minimizer == 1;
-  const void *fn = plane ? (variant == 0   ? (const void *)icp_kernel<128, 6, true>
+  const void *fn = plane ? (variant == 0   ? (const void *)icp_kernel<128, 7, true>
                             : variant == 1 ? (const void *)icp_kernel<256, 4, true>
                             : variant == 2 ? (const void *)icp_kernel<512, 2, true>
                                            : (const void *)icp_kernel<512, 1, true>)
-                         : (variant == 0   ? (const void *)icp_kernel<128, 6, false>
+                         : (variant == 0   ? (const void *)icp_kernel<128, 7, false>
                             : variant == 1 ? (const void *)icp_kernel<256, 4, false>
                             : variant == 2 ? (const void *)icp_kernel<512, 2, false>
                                            : (const void *)icp_kernel<512, 1, false>);
@@ -1312,6 +1358,9 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
     ctx->icp_occ_next = (ctx->icp_occ_next + 1) % 8;
   }
   const int per_sm = c_per_sm;
+#ifdef SFE_ICP_PHASE_CLOCKS
+  icp_phase_per_sm[threads == 128 ? 0 : threads == 256 ? 1 : 2] = per_sm;
+#endif
   int grid = ctx->sm_count * per_sm;
   if (grid > P) grid = P;
   int slots = grid;
@@ -1365,3 +1414,21 @@ int match_run(sfe_ctx *ctx, const float *ref_pts, const int *ref_off, const floa
 }
 
 }  // namespace sfe
+
+#ifdef SFE_ICP_PHASE_CLOCKS
+// Development build only (not declared in include/sonarfe.h): out[0..6] cycles per phase, out[7..13] phase counts,
+// out[14..16] CTAs per SM of the last 128 / 256 / 512-thread launch.  reset != 0 clears the totals afterwards.
+extern "C" __attribute__((visibility("default"))) int sfe_icp_phase_clocks(unsigned long long *out, int reset) {
+  using namespace sfe;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (cudaMemcpyFromSymbol(out, icp_phase_cycles, sizeof(icp_phase_cycles)) != cudaSuccess) return -1;
+  if (cudaMemcpyFromSymbol(out + ICP_PHASES, icp_phase_count, sizeof(icp_phase_count)) != cudaSuccess) return -1;
+  for (int k = 0; k < 3; ++k) out[2 * ICP_PHASES + k] = (unsigned long long)icp_phase_per_sm[k];
+  if (reset) {
+    const unsigned long long z[ICP_PHASES] = {};
+    if (cudaMemcpyToSymbol(icp_phase_cycles, z, sizeof z) != cudaSuccess) return -1;
+    if (cudaMemcpyToSymbol(icp_phase_count, z, sizeof z) != cudaSuccess) return -1;
+  }
+  return 0;
+}
+#endif

@@ -87,11 +87,15 @@ struct PngFormat {
   static const int32_t *status_dev(const State *s) { return png_status_dev(s); }
 };
 
-// Size class of the first ICP launch (fe_match), chosen on the config-4 replay (filtered clouds: median 326,
-// max 639 points; window submaps <= 1808 raw points; not re-measured on H100): this class with 128 threads (6 CTAs
-// per SM) beat one launch sized for the capacities (1024 / 3072, 4 CTAs per SM), and a smaller class that leaves
-// frames to the second launch loses -- the tail of a nearly empty launch costs a full problem latency.
-constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 1536, FE_ICP_SMALL_THREADS = 128;
+// Size class of the first ICP launch (fe_match), from the problem sizes of bench.py's 4096-frame bag
+// (tools/icp_sizes.py): sources after the filters mean 359, max 639 points; window submaps after the 0.5 m thinning
+// (the ICP target) mean 406, max 779.  The class takes every frame of that bag: a second launch that holds only a
+// few frames costs a full problem latency at its tail.  The source cap has no margin over the bag's largest source
+// (639): above 5 points per thread (640 for 128 threads, icp.cu: small_mult) a problem leaves the one-pass path, so a
+// larger cap would only admit problems that take the slower pruned path.  At 640 / 896 points a 128-thread CTA needs 29 KB of shared
+// memory and the 128-thread instantiation is held to 72 registers, so an H100 SM holds 7 problems (6 at the former
+// 640 / 1536 class with 80 registers).
+constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 896, FE_ICP_SMALL_THREADS = 128;
 // Size classes of the cloud filters (cloud.cu: two launches by cloud size).  Config-4 replay: 3-5 k raw Cartesian
 // points per frame, ~580 after the voxel filter, ~400 after the outlier filter, window submaps <= 1.8 k raw points.
 // The outlier filter and the submap down-sampling gain from a small-cloud class; the per-frame down-sampling is best
@@ -576,7 +580,7 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   fe_tic(fe, SFE_FE_ICP);
   // Two launches by problem size: a sonar frame's filtered cloud is a few hundred points, far below the
   // capacities the buffers are sized for, and the ICP kernel's occupancy is set by its shared-memory footprint.
-  // The first launch is sized for the common case (6 CTAs per SM instead of 4) and leaves bigger problems
+  // The first launch is sized for the common case (7 CTAs per SM instead of 4) and leaves bigger problems
   // untouched; the second, sized for the capacities, only takes those.
   const int ns_small = p.cap_source < FE_ICP_SMALL_SRC ? p.cap_source : FE_ICP_SMALL_SRC;
   const int nt_small = p.cap_target < FE_ICP_SMALL_TGT ? p.cap_target : FE_ICP_SMALL_TGT;

@@ -12,4 +12,5 @@ build() { tag=$1; shift
 }
 rm -f scratch/lib_*.so
 build pipe128 -DSFE_SEQ_PIPE_MIN=128
+build phases -DSFE_ICP_PHASE_CLOCKS  # per-phase cycle counts of icp_kernel (tools/icp_phases.py)
 ls -la scratch/*.so
