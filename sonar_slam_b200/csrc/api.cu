@@ -136,8 +136,8 @@ void sfe_ctx_destroy(sfe_ctx *ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  if (ctx->jpeg_free) ctx->jpeg_free(ctx->jpeg);
-  if (ctx->png_free) ctx->png_free(ctx->png);
+  sfe::destroy(ctx->jpeg);
+  sfe::destroy(ctx->png);
   for (auto &b : ctx->scratch)
     if (b.ptr) cudaFree(b.ptr);
   for (auto &b : ctx->stage_in)

@@ -39,6 +39,11 @@ struct Buffer {  // grow-only device scratch
   size_t cap = 0;
 };
 
+struct JpegState;  // jpeg.cu
+struct PngState;   // png.cu
+void destroy(JpegState *s);
+void destroy(PngState *s);
+
 }  // namespace sfe
 
 struct sfe_ctx {
@@ -59,10 +64,8 @@ struct sfe_ctx {
   const void *cfar_lut_buf = nullptr;            // ... and the buffer it was uploaded to (null = none)
   struct OccEntry { size_t smem; int threads, per_sm, variant; } icp_occ[8] = {};
   int icp_occ_next = 0;
-  void *jpeg = nullptr;                 // JPEG decoder state (jpeg.cu), created on first use
-  void (*jpeg_free)(void *) = nullptr;
-  void *png = nullptr;                  // PNG decoder state (png.cu), created on first use
-  void (*png_free)(void *) = nullptr;
+  sfe::JpegState *jpeg = nullptr;       // JPEG decoder state, created on first use
+  sfe::PngState *png = nullptr;         // PNG decoder state, created on first use
   cudaStream_t copy_stream = nullptr;   // host flavours that overlap copies with kernels (featx.cu), created on first use
   cudaEvent_t copy_ev[4] = {};
   int *work = nullptr;  // device [SFE_WORK_COUNTERS]: work counters of the persistent kernels (sfe::next_work_item)

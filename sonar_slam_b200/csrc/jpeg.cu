@@ -36,7 +36,7 @@
 #include <unordered_map>
 #include <vector>
 
-#include "common.cuh"
+#include "stream_decode.cuh"
 
 namespace sfe {
 
@@ -882,77 +882,6 @@ static void derive_table(const JHuffSpec &s, HT &t) {
   t.maxcode[17] = -1;
 }
 
-struct JpegBatch {
-  const uint8_t *bytes = nullptr;
-  const int64_t *offsets = nullptr;
-  int n = 0, R = 0, B = 0;
-  std::vector<JHeader> hdr;
-};
-
-struct JpegState {
-  cudaStream_t copy = nullptr;
-  cudaEvent_t ev_copied[2] = {}, ev_used[2] = {}, ev_ready = nullptr;
-  uint8_t *pin[2] = {};
-  size_t pin_cap[2] = {};
-  Buffer dev_in[2], scr, coef, status, out;
-  int turn = 0;
-  // optional per-stage device timing (CUDA events on the context's stream), sfe_jpeg_set_timing / _get_timing
-  bool timing = false;
-  std::vector<cudaEvent_t> tev;   // pool; pair [2k, 2k+1] brackets interval k
-  std::vector<int> tstage;        // stage of interval k
-  size_t tused = 0;
-  double stage_ms[SFE_JPEG_STAGES] = {};
-  int64_t stage_calls[SFE_JPEG_STAGES] = {};
-};
-
-static void jt_tic(JpegState *js, cudaStream_t st, int stage) {
-  if (!js->timing) return;
-  while (js->tev.size() < js->tused + 2) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    js->tev.push_back(e);
-  }
-  cudaEventRecord(js->tev[js->tused], st);
-  js->tstage.push_back(stage);
-}
-static void jt_toc(JpegState *js, cudaStream_t st) {
-  if (!js->timing) return;
-  cudaEventRecord(js->tev[js->tused + 1], st);
-  js->tused += 2;
-}
-
-static void jpeg_state_free(void *p) {
-  JpegState *s = static_cast<JpegState *>(p);
-  if (!s) return;
-  if (s->copy) cudaStreamSynchronize(s->copy), cudaStreamDestroy(s->copy);
-  for (int k = 0; k < 2; ++k) {
-    if (s->ev_copied[k]) cudaEventDestroy(s->ev_copied[k]);
-    if (s->ev_used[k]) cudaEventDestroy(s->ev_used[k]);
-    if (s->pin[k]) cudaFreeHost(s->pin[k]);
-    if (s->dev_in[k].ptr) cudaFree(s->dev_in[k].ptr);
-  }
-  if (s->ev_ready) cudaEventDestroy(s->ev_ready);
-  for (cudaEvent_t e : s->tev) cudaEventDestroy(e);
-  for (Buffer *b : {&s->scr, &s->coef, &s->status, &s->out})
-    if (b->ptr) cudaFree(b->ptr);
-  delete s;
-}
-
-static int jpeg_state(sfe_ctx *ctx, JpegState **out) {
-  if (!ctx->jpeg) {
-    JpegState *s = new JpegState();
-    ctx->jpeg = s, ctx->jpeg_free = jpeg_state_free;
-    SFE_CUDA(cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      SFE_CUDA(cudaEventCreateWithFlags(&s->ev_copied[k], cudaEventDisableTiming));
-      SFE_CUDA(cudaEventCreateWithFlags(&s->ev_used[k], cudaEventDisableTiming));
-    }
-    SFE_CUDA(cudaEventCreateWithFlags(&s->ev_ready, cudaEventDisableTiming));
-  }
-  *out = static_cast<JpegState *>(ctx->jpeg);
-  return SFE_OK;
-}
-
 // descriptor of frame h (everything but the buffer offsets)
 static void describe(const JHeader &h, JDesc &d) {
   memset(&d, 0, sizeof(d));
@@ -984,7 +913,7 @@ struct ChunkPlan {
   size_t off_huff = 0, off_quant = 0, off_bytes = 0, total = 0;
 };
 
-static void plan_chunk(const JpegBatch &bt, int f0, int nf, ChunkPlan &p) {
+static void plan_chunk(const StreamBatch<JHeader> &bt, int f0, int nf, ChunkPlan &p) {
   p = ChunkPlan();
   p.desc.resize(nf);
   std::unordered_map<std::string, int> hmap, qmap;
@@ -1047,23 +976,37 @@ static void plan_chunk(const JpegBatch &bt, int f0, int nf, ChunkPlan &p) {
   p.total = p.off_bytes + p.ecs_bytes + 16;
 }
 
-int jpeg_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, JpegBatch **out) {
-  JpegBatch *b = new JpegBatch();
-  b->bytes = bytes, b->offsets = offsets, b->n = n, b->R = R, b->B = B;
-  b->hdr.resize(n);
-  for (int i = 0; i < n; ++i) {
-    parse_header(bytes + offsets[i], offsets[i + 1] - offsets[i], b->hdr[i]);
-    if (b->hdr[i].status == SFE_JPEG_OK && (b->hdr[i].H != R || b->hdr[i].W != B)) b->hdr[i].status = SFE_JPEG_SIZE;
-  }
-  *out = b;
-  return SFE_OK;
-}
-void jpeg_batch_free(JpegBatch *b) { delete b; }
-int jpeg_batch_status(const JpegBatch *b, int i) { return b->hdr[i].status; }
+enum { JPEG_CHUNK = 256 };
 
-// Size every buffer for the largest chunk of [0, n) in pieces of `chunk` frames (before any work of this call is
-// enqueued: the buffers are not reallocated while the copy stream may use them).
-static int jpeg_reserve(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int chunk, size_t out_bytes) {
+struct JpegState final : StreamDecoder {
+  StreamBatch<JHeader> bt;
+  Buffer scr, coef;
+  // sfe_jpeg_coefficients_host: with cap_blocks > 0 every chunk also writes its dequantised coefficients
+  // (int32 [nf][cap_blocks][64], in ctx->stage_out[0]) and copies them to coef_host
+  int cap_blocks = 0;
+  int32_t *coef_host = nullptr;
+
+  ~JpegState() override {
+    for (Buffer *b : {&scr, &coef})
+      if (b->ptr) cudaFree(b->ptr);
+  }
+  int chunk_frames(const sfe_ctx *) const override { return cap_blocks > 0 ? 16 : JPEG_CHUNK; }
+  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B) override {
+    bt.parse(bytes, offsets, n, R, B, parse_header, SFE_JPEG_SIZE);
+  }
+  int frame_status(int i) const override { return bt.hdr[i].status; }
+  const char *message(int status) const override { return sfe_jpeg_status_message(status); }
+  int reserve(sfe_ctx *ctx, int chunk, size_t out_bytes) override;
+  int decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) override;
+};
+
+StreamDecoder *jpeg_decoder(sfe_ctx *ctx) {
+  if (!ctx->jpeg) ctx->jpeg = new JpegState();
+  return ctx->jpeg;
+}
+void destroy(JpegState *s) { delete s; }
+
+int JpegState::reserve(sfe_ctx *ctx, int chunk, size_t out_bytes) {
   size_t in_max = 0, scr_max = 0, coef_max = 0;
   ChunkPlan p;
   for (int f0 = 0; f0 < bt.n; f0 += chunk) {
@@ -1072,37 +1015,18 @@ static int jpeg_reserve(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int ch
     scr_max = std::max(scr_max, (size_t)p.scr_bytes);
     coef_max = std::max(coef_max, (size_t)p.coef_blocks * 128);
   }
-  SFE_CUDA(cudaStreamSynchronize(js->copy));
-  for (int k = 0; k < 2; ++k) {
-    int rc = ensure(ctx, js->dev_in[k], in_max);
-    if (rc != SFE_OK) return rc;
-    if (js->pin_cap[k] < in_max) {
-      if (js->pin[k]) SFE_CUDA(cudaFreeHost(js->pin[k]));
-      js->pin[k] = nullptr, js->pin_cap[k] = 0;
-      SFE_CUDA(cudaMallocHost((void **)&js->pin[k], in_max + in_max / 4));
-      js->pin_cap[k] = in_max + in_max / 4;
-    }
-  }
-  int rc = ensure(ctx, js->scr, scr_max + 16);
-  if (rc == SFE_OK) rc = ensure(ctx, js->coef, coef_max + 16);
-  if (rc == SFE_OK) rc = ensure(ctx, js->status, 4 * (size_t)bt.n + 16);
-  if (rc == SFE_OK && out_bytes) rc = ensure(ctx, js->out, out_bytes);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaEventRecord(js->ev_ready, ctx->stream));
-  SFE_CUDA(cudaStreamWaitEvent(js->copy, js->ev_ready, 0));
-  return SFE_OK;
+  int rc = ensure(ctx, scr, scr_max + 16);
+  if (rc == SFE_OK) rc = ensure(ctx, coef, coef_max + 16);
+  if (rc == SFE_OK && cap_blocks > 0) rc = ensure(ctx, ctx->stage_out[0], (size_t)chunk * cap_blocks * 64 * 4);
+  return rc == SFE_OK ? reserve_common(ctx, bt.n, in_max, out_bytes) : rc;
 }
 
-// Decode frames [f0, f0 + nf) of the batch into out_dev (uint8 [nf][R][B]); per-frame status into the state's
-// device status array at [f0, f0 + nf).  Asynchronous on ctx->stream; the bytes go in on the copy stream.
-// cap_blocks > 0: also the dequantised coefficients into coef_dev (int32 [nf][cap_blocks][64]).
-static int jpeg_decode_chunk(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int f0, int nf, uint8_t *out_dev,
-                             int cap_blocks = 0, int32_t *coef_dev = nullptr) {
+int JpegState::decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) {
   ChunkPlan p;
   plan_chunk(bt, f0, nf, p);
-  const int turn = js->turn ^= 1;
-  SFE_CUDA(cudaEventSynchronize(js->ev_copied[turn]));  // the pinned block is free again
-  uint8_t *pin = js->pin[turn];
+  uint8_t *pin, *dev;
+  int rc = stager.acquire(&pin);
+  if (rc != SFE_OK) return rc;
   memcpy(pin, p.desc.data(), sizeof(JDesc) * nf);
   memcpy(pin + p.off_huff, p.huff.data(), sizeof(HT) * p.huff.size());
   memcpy(pin + p.off_quant, p.quant.data(), 2 * p.quant.size());
@@ -1112,97 +1036,40 @@ static int jpeg_decode_chunk(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, i
     const JHeader &h = bt.hdr[f0 + i];
     memcpy(pin + p.off_bytes + d.src, bt.bytes + bt.offsets[f0 + i] + h.ecs, d.src_len);
   }
-  uint8_t *dev = static_cast<uint8_t *>(js->dev_in[turn].ptr);
-  SFE_CUDA(cudaStreamWaitEvent(js->copy, js->ev_used[turn], 0));  // kernels of two chunks ago are done with it
-  SFE_CUDA(cudaMemcpyAsync(dev, pin, p.off_bytes + p.ecs_bytes, cudaMemcpyHostToDevice, js->copy));
-  SFE_CUDA(cudaEventRecord(js->ev_copied[turn], js->copy));
-  SFE_CUDA(cudaStreamWaitEvent(ctx->stream, js->ev_copied[turn], 0));
+  rc = stager.upload(ctx, p.off_bytes + p.ecs_bytes, &dev);
+  if (rc != SFE_OK) return rc;
   const JDesc *desc = reinterpret_cast<const JDesc *>(dev);
   const HT *huff = reinterpret_cast<const HT *>(dev + p.off_huff);
   const uint16_t *quant = reinterpret_cast<const uint16_t *>(dev + p.off_quant);
-  uint8_t *scr = static_cast<uint8_t *>(js->scr.ptr);
-  int16_t *coef = static_cast<int16_t *>(js->coef.ptr);
-  int32_t *st = static_cast<int32_t *>(js->status.ptr) + f0;
+  uint8_t *s = static_cast<uint8_t *>(scr.ptr);
+  int16_t *c = static_cast<int16_t *>(coef.ptr);
+  int32_t *st = static_cast<int32_t *>(status.ptr) + f0;
   const int64_t fstride = (int64_t)bt.R * bt.B;
-  jt_tic(js, ctx->stream, SFE_JPEG_T_UNSTUFF);
-  jpeg_unstuff_kernel<<<nf, JT, 0, ctx->stream>>>(desc, dev + p.off_bytes, scr, st);
-  jt_toc(js, ctx->stream);
-  jt_tic(js, ctx->stream, SFE_JPEG_T_ENTROPY);
-  jpeg_entropy_kernel<<<nf, JT, 0, ctx->stream>>>(desc, huff, scr, coef, st);
-  jt_toc(js, ctx->stream);
+  timer.tic(ctx->stream, SFE_JPEG_T_UNSTUFF);
+  jpeg_unstuff_kernel<<<nf, JT, 0, ctx->stream>>>(desc, dev + p.off_bytes, s, st);
+  timer.toc(ctx->stream);
+  timer.tic(ctx->stream, SFE_JPEG_T_ENTROPY);
+  jpeg_entropy_kernel<<<nf, JT, 0, ctx->stream>>>(desc, huff, s, c, st);
+  timer.toc(ctx->stream);
   int maxblk = 1;
   for (const JDesc &d : p.desc) maxblk = std::max(maxblk, d.nblocks);
-  jt_tic(js, ctx->stream, SFE_JPEG_T_PIXELS);
-  jpeg_idct_kernel<<<dim3((maxblk + 15) / 16, nf), 128, 0, ctx->stream>>>(desc, quant, scr, coef, st, out_dev, fstride);
+  timer.tic(ctx->stream, SFE_JPEG_T_PIXELS);
+  jpeg_idct_kernel<<<dim3((maxblk + 15) / 16, nf), 128, 0, ctx->stream>>>(desc, quant, s, c, st, out_dev, fstride);
   const int per = (int)std::min<int64_t>((fstride + 1023) / 1024, 64);
-  jpeg_color_kernel<<<dim3(per, nf), 256, 0, ctx->stream>>>(desc, scr, st, out_dev, fstride, bt.R, bt.B);
-  jt_toc(js, ctx->stream);
+  jpeg_color_kernel<<<dim3(per, nf), 256, 0, ctx->stream>>>(desc, s, st, out_dev, fstride, bt.R, bt.B);
+  timer.toc(ctx->stream);
   ctx->launches += 4;
+  int32_t *coef_dev = static_cast<int32_t *>(ctx->stage_out[0].ptr);
   if (cap_blocks > 0) {
     jpeg_dequant_kernel<<<dim3((int)(((int64_t)cap_blocks * 64 + 255) / 256), nf), 256, 0, ctx->stream>>>(
-        desc, quant, scr, coef, st, cap_blocks, coef_dev);
+        desc, quant, s, c, st, cap_blocks, coef_dev);
     ctx->launches++;
   }
   SFE_CUDA(cudaGetLastError());
-  SFE_CUDA(cudaEventRecord(js->ev_used[turn], ctx->stream));
-  return SFE_OK;
-}
-
-int jpeg_begin(sfe_ctx *ctx, const JpegBatch &bt, int chunk, JpegState **js) {
-  int rc = jpeg_state(ctx, js);
-  if (rc != SFE_OK) return rc;
-  return jpeg_reserve(ctx, *js, bt, chunk, 0);
-}
-int jpeg_decode_frames(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int f0, int nf, uint8_t *out_dev) {
-  return jpeg_decode_chunk(ctx, js, bt, f0, nf, out_dev);
-}
-const int32_t *jpeg_status_dev(const JpegState *js) { return static_cast<const int32_t *>(js->status.ptr); }
-
-enum { JPEG_CHUNK = 256 };
-
-// the shared body of the decode entries: out_dev (device, [n][R][B]) or out_host
-static int jpeg_decode_all(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
-                           uint8_t *out_dev, uint8_t *out_host, int cap_blocks, int32_t *coef_host,
-                           int32_t *status_host, const char *what) {
-  SFE_REQUIRE(ctx && bytes && offsets && status_host && (out_dev || out_host || coef_host), "%s: null argument", what);
-  SFE_REQUIRE(n >= 0 && R > 0 && B > 0, "%s: bad shape n=%d R=%d B=%d", what, n, R, B);
-  for (int i = 0; i < n; ++i)
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "%s: offsets must be non-decreasing", what);
-  if (n == 0) return SFE_OK;
-  SFE_CUDA(cudaSetDevice(ctx->device));
-  JpegBatch *bt;
-  jpeg_batch_parse(bytes, offsets, n, R, B, &bt);
-  JpegState *js;
-  int rc = jpeg_state(ctx, &js);
-  const size_t fb = (size_t)R * B;
-  const int chunk = cap_blocks > 0 ? 16 : JPEG_CHUNK;
-  const bool via_out = !out_dev;
-  if (rc == SFE_OK) rc = jpeg_reserve(ctx, js, *bt, chunk, via_out ? fb * chunk : 0);
-  int32_t *coef_dev = nullptr;
-  if (rc == SFE_OK && cap_blocks > 0) {
-    const size_t cb = (size_t)chunk * cap_blocks * 64 * 4;
-    rc = ensure(ctx, ctx->stage_out[0], cb);
-    coef_dev = static_cast<int32_t *>(ctx->stage_out[0].ptr);
-  }
-  for (int f0 = 0; rc == SFE_OK && f0 < n; f0 += chunk) {
-    const int nf = std::min(chunk, n - f0);
-    uint8_t *o = via_out ? static_cast<uint8_t *>(js->out.ptr) : out_dev + fb * f0;
-    rc = jpeg_decode_chunk(ctx, js, *bt, f0, nf, o, cap_blocks, coef_dev);
-    if (rc != SFE_OK) break;
-    if (out_host) {
-      cudaError_t e = cudaMemcpyAsync(out_host + fb * f0, o, fb * nf, cudaMemcpyDeviceToHost, ctx->stream);
-      if (e != cudaSuccess) rc = SFE_ERR_CUDA, set_error("%s: %s", what, cudaGetErrorString(e));
-    }
-    if (rc == SFE_OK && coef_host) {
-      cudaError_t e = cudaMemcpyAsync(coef_host + (size_t)f0 * cap_blocks * 64, coef_dev,
-                                      (size_t)nf * cap_blocks * 64 * 4, cudaMemcpyDeviceToHost, ctx->stream);
-      if (e != cudaSuccess) rc = SFE_ERR_CUDA, set_error("%s: %s", what, cudaGetErrorString(e));
-    }
-  }
-  jpeg_batch_free(bt);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaMemcpyAsync(status_host, js->status.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+  rc = stager.done(ctx);
+  if (rc != SFE_OK || !coef_host) return rc;
+  SFE_CUDA(cudaMemcpyAsync(coef_host + (size_t)f0 * cap_blocks * 64, coef_dev, (size_t)nf * cap_blocks * 64 * 4,
+                           cudaMemcpyDeviceToHost, ctx->stream));
   return SFE_OK;
 }
 
@@ -1234,8 +1101,8 @@ const char *sfe_jpeg_status_message(int status) {
 int sfe_jpeg_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, int32_t *info) {
   SFE_REQUIRE(bytes && offsets && info, "sfe_jpeg_inspect_host: null argument");
   SFE_REQUIRE(n >= 0, "sfe_jpeg_inspect_host: negative count");
+  SFE_REQUIRE(offsets_ok(offsets, n), "sfe_jpeg_inspect_host: offsets must be non-decreasing");
   for (int i = 0; i < n; ++i) {
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "sfe_jpeg_inspect_host: offsets must be non-decreasing");
     JHeader h;
     parse_header(bytes + offsets[i], offsets[i + 1] - offsets[i], h);
     int32_t *o = info + (size_t)SFE_JPEG_INFO * i;
@@ -1247,24 +1114,21 @@ int sfe_jpeg_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, i
 int sfe_jpeg_decode_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
                          uint8_t *out_host, int32_t *status_host) {
   SFE_REQUIRE(out_host, "sfe_jpeg_decode_host: null output");
-  return jpeg_decode_all(ctx, bytes, offsets, n, R, B, nullptr, out_host, 0, nullptr, status_host,
-                         "sfe_jpeg_decode_host");
+  return decode_all(ctx, jpeg_decoder, bytes, offsets, n, R, B, nullptr, out_host, status_host, "sfe_jpeg_decode_host");
 }
 
 int sfe_jpeg_decode_to_dev(sfe_ctx *ctx, const uint8_t *bytes_host, const int64_t *offsets_host, int n, int R, int B,
                            uint8_t *out_dev, int32_t *status_host) {
   SFE_REQUIRE(out_dev, "sfe_jpeg_decode_to_dev: null output");
-  return jpeg_decode_all(ctx, bytes_host, offsets_host, n, R, B, out_dev, nullptr, 0, nullptr, status_host,
-                         "sfe_jpeg_decode_to_dev");
+  return decode_all(ctx, jpeg_decoder, bytes_host, offsets_host, n, R, B, out_dev, nullptr, status_host,
+                    "sfe_jpeg_decode_to_dev");
 }
 
 int sfe_jpeg_coefficients_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
                                int cap_blocks, int32_t *coef_host, int32_t *status_host) {
   SFE_REQUIRE(coef_host && cap_blocks > 0, "sfe_jpeg_coefficients_host: null output or cap_blocks <= 0");
   SFE_REQUIRE(ctx && bytes && offsets && status_host && n >= 0, "sfe_jpeg_coefficients_host: null argument");
-  for (int i = 0; i < n; ++i)
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0,
-                "sfe_jpeg_coefficients_host: offsets must be non-decreasing");
+  SFE_REQUIRE(offsets_ok(offsets, n), "sfe_jpeg_coefficients_host: offsets must be non-decreasing");
   for (int i = 0; i < n; ++i) {
     JHeader h;
     parse_header(bytes + offsets[i], offsets[i + 1] - offsets[i], h);
@@ -1276,44 +1140,25 @@ int sfe_jpeg_coefficients_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t
       return SFE_ERR_CAPACITY;
     }
   }
-  return jpeg_decode_all(ctx, bytes, offsets, n, R, B, nullptr, nullptr, cap_blocks, coef_host, status_host,
-                         "sfe_jpeg_coefficients_host");
+  JpegState *js = static_cast<JpegState *>(jpeg_decoder(ctx));
+  js->cap_blocks = cap_blocks, js->coef_host = coef_host;
+  const int rc = decode_all(ctx, jpeg_decoder, bytes, offsets, n, R, B, nullptr, nullptr, status_host,
+                            "sfe_jpeg_coefficients_host");
+  js->cap_blocks = 0, js->coef_host = nullptr;
+  return rc;
 }
 
 int sfe_jpeg_set_timing(sfe_ctx *ctx, int enable) {
   SFE_REQUIRE(ctx != nullptr, "sfe_jpeg_set_timing: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  JpegState *js;
-  int rc = jpeg_state(ctx, &js);
-  if (rc != SFE_OK) return rc;
-  js->timing = enable != 0;
-  js->tused = 0;
-  js->tstage.clear();
-  for (int i = 0; i < SFE_JPEG_STAGES; ++i) js->stage_ms[i] = 0.0, js->stage_calls[i] = 0;
+  jpeg_decoder(ctx)->timer.reset(enable != 0);
   return SFE_OK;
 }
 
 int sfe_jpeg_get_timing(sfe_ctx *ctx, double *stage_ms, int64_t *stage_calls) {
   SFE_REQUIRE(ctx && stage_ms, "sfe_jpeg_get_timing: null argument");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  JpegState *js;
-  int rc = jpeg_state(ctx, &js);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (size_t k = 0; k < js->tstage.size(); ++k) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, js->tev[2 * k], js->tev[2 * k + 1]) == cudaSuccess) {
-      js->stage_ms[js->tstage[k]] += ms;
-      js->stage_calls[js->tstage[k]]++;
-    }
-  }
-  js->tused = 0;
-  js->tstage.clear();
-  for (int i = 0; i < SFE_JPEG_STAGES; ++i) {
-    stage_ms[i] = js->stage_ms[i];
-    if (stage_calls) stage_calls[i] = js->stage_calls[i];
-  }
-  return SFE_OK;
+  return jpeg_decoder(ctx)->timer.collect(ctx->stream, SFE_JPEG_STAGES, stage_ms, stage_calls);
 }
 
 }  // extern "C"

@@ -16,7 +16,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "stream_decode.cuh"
 
 namespace sfe {
 int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
@@ -36,57 +36,6 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
             const int *src_id, const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out,
             int *iters, int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
             int class_ns = 0, int class_nt = 0, int force_threads = 0);
-// compressed pings (jpeg.cu)
-struct JpegBatch;
-struct JpegState;
-int jpeg_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, JpegBatch **out);
-void jpeg_batch_free(JpegBatch *b);
-int jpeg_batch_status(const JpegBatch *b, int i);
-int jpeg_begin(sfe_ctx *ctx, const JpegBatch &bt, int chunk, JpegState **js);
-int jpeg_decode_frames(sfe_ctx *ctx, JpegState *js, const JpegBatch &bt, int f0, int nf, uint8_t *out_dev);
-const int32_t *jpeg_status_dev(const JpegState *js);
-// (png.cu)
-struct PngBatch;
-struct PngState;
-int png_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, PngBatch **out);
-void png_batch_free(PngBatch *b);
-int png_batch_status(const PngBatch *b, int i);
-int png_begin(sfe_ctx *ctx, const PngBatch &bt, int chunk, PngState **ps);
-int png_decode_frames(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int f0, int nf, uint8_t *out_dev);
-const int32_t *png_status_dev(const PngState *ps);
-
-// The decoders the compressed front-end entry points are written over.
-struct JpegFormat {
-  using Batch = JpegBatch;
-  using State = JpegState;
-  static int parse(const uint8_t *b, const int64_t *o, int n, int R, int B, Batch **out) {
-    return jpeg_batch_parse(b, o, n, R, B, out);
-  }
-  static void free(Batch *b) { jpeg_batch_free(b); }
-  static int status(const Batch *b, int i) { return jpeg_batch_status(b, i); }
-  static const char *message(int st) { return sfe_jpeg_status_message(st); }
-  static int begin(sfe_ctx *c, const Batch &b, int chunk, State **s) { return jpeg_begin(c, b, chunk, s); }
-  static int decode(sfe_ctx *c, State *s, const Batch &b, int f0, int nf, uint8_t *o) {
-    return jpeg_decode_frames(c, s, b, f0, nf, o);
-  }
-  static const int32_t *status_dev(const State *s) { return jpeg_status_dev(s); }
-};
-struct PngFormat {
-  using Batch = PngBatch;
-  using State = PngState;
-  static int parse(const uint8_t *b, const int64_t *o, int n, int R, int B, Batch **out) {
-    return png_batch_parse(b, o, n, R, B, out);
-  }
-  static void free(Batch *b) { png_batch_free(b); }
-  static int status(const Batch *b, int i) { return png_batch_status(b, i); }
-  static const char *message(int st) { return sfe_png_status_message(st); }
-  static int begin(sfe_ctx *c, const Batch &b, int chunk, State **s) { return png_begin(c, b, chunk, s); }
-  static int decode(sfe_ctx *c, State *s, const Batch &b, int f0, int nf, uint8_t *o) {
-    return png_decode_frames(c, s, b, f0, nf, o);
-  }
-  static const int32_t *status_dev(const State *s) { return png_status_dev(s); }
-};
-
 // Size class of the first ICP launch (fe_match), from the problem sizes of bench.py's 4096-frame bag
 // (tools/icp_sizes.py): sources after the filters mean 359, max 639 points; window submaps after the 0.5 m thinning
 // (the ICP target) mean 406, max 779.  The class takes every frame of that bag: a second launch that holds only a
@@ -180,70 +129,48 @@ __global__ void __launch_bounds__(256)
 using namespace sfe;
 
 struct sfe_frontend {
-  sfe_ctx *ctx;
-  const sfe_maps *maps;
-  sfe_frontend_params p;
-  int max_frames;
+  sfe_ctx *ctx = nullptr;
+  const sfe_maps *maps = nullptr;
+  sfe_frontend_params p = {};
+  int max_frames = 0;
   // device buffers (sized for max_frames)
-  uint8_t *frames;      // [max_frames][R][B]      (host flavour only)
-  uint32_t *bits;       // [max_frames][R][wpr]
-  int32_t *ij;          // [max_frames][cap][2]
-  float *xy_a, *xy_b;   // [max_frames][cap][2] ping-pong
-  int32_t *idx;         // [max_frames][cap]
-  int32_t *cnt_a, *cnt_b, *cnt_c;
-  int32_t *off_pts, *off_tgt;
-  float *tgt_a, *tgt_b; // [max_frames][window*cap][2]
-  int32_t *tgt_idx, *tcnt_a, *tcnt_b;
-  float *rel;           // [max_frames][window+1][9] relative transforms (window slots, then the guess)
-  float *rel_host[2];   // pinned staging of the same, double-buffered (no stream sync per call)
-  cudaEvent_t ev_rel[2];
-  int rel_turn;
-  float *guess, *T;
-  int32_t *iters, *inliers, *status;
+  uint8_t *frames = nullptr;      // [max_frames][R][B]      (host flavour only)
+  uint32_t *bits = nullptr;       // [max_frames][R][wpr]
+  int32_t *ij = nullptr;          // [max_frames][cap][2]
+  float *xy_a = nullptr, *xy_b = nullptr;  // [max_frames][cap][2] ping-pong
+  int32_t *idx = nullptr;         // [max_frames][cap]
+  int32_t *cnt_a = nullptr, *cnt_b = nullptr, *cnt_c = nullptr;
+  int32_t *off_pts = nullptr, *off_tgt = nullptr;
+  float *tgt_a = nullptr, *tgt_b = nullptr;  // [max_frames][window*cap][2]
+  int32_t *tgt_idx = nullptr, *tcnt_a = nullptr, *tcnt_b = nullptr;
+  float *rel = nullptr;           // [max_frames][window+1][9] relative transforms (window slots, then the guess)
+  float *rel_host[2] = {};        // pinned staging of the same, double-buffered (no stream sync per call)
+  cudaEvent_t ev_rel[2] = {};
+  int rel_turn = 0;
+  float *guess = nullptr, *T = nullptr;
+  int32_t *iters = nullptr, *inliers = nullptr, *status = nullptr;
   // continuation across calls: the last `window` clouds (+ host poses) of the previous call
-  int carry_on, carry_n;
-  float *carry_xy;       // [window][cap][2]
-  int32_t *carry_cnt;    // [window]
-  double *carry_poses;   // host [window][3]
-  cudaStream_t copy_stream;
-  cudaEvent_t ev_copy[2], ev_done;
+  int carry_on = 0, carry_n = 0;
+  float *carry_xy = nullptr;       // [window][cap][2]
+  int32_t *carry_cnt = nullptr;    // [window]
+  double *carry_poses = nullptr;   // host [window][3]
+  cudaStream_t copy_stream = nullptr;
+  cudaEvent_t ev_copy[2] = {}, ev_done = nullptr;
   // overlapped run_dev (sfe_frontend_set_overlap): sub-batch size (0: serial on ctx->stream), the two streams and the
   // events that fork them from ctx->stream, hand each sub-batch from features to match, and join them back
-  int overlap;
-  cudaStream_t feat_stream, match_stream;
-  cudaEvent_t ev_fork, ev_feat, ev_join;
+  int overlap = 0;
+  cudaStream_t feat_stream = nullptr, match_stream = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_feat = nullptr, ev_join = nullptr;
   // feature images (sfe_frontend_set_feature_images)
-  uint8_t img_lut[256 * 3];
-  uint8_t *img_dst;      // null: off
-  int img_dst_host;
-  uint8_t *img_stage[2];  // host flavours: [img_stage_frames][rows][cols][3] each
-  int img_stage_frames;
-  cudaStream_t img_stream;  // copies the images out, next to the frame copies of copy_stream
-  cudaEvent_t ev_img_ready[2], ev_img_copied[2];
-  // optional per-stage timing (CUDA events on the launch stream)
-  int timing;
-  std::vector<cudaEvent_t> *tev;    // pool
-  std::vector<int> *tstage;         // stage id of interval [2k, 2k+1]
-  size_t tused;
-  double stage_ms[SFE_FE_STAGES];
-  long long stage_launches[SFE_FE_STAGES];
+  uint8_t img_lut[256 * 3] = {};
+  uint8_t *img_dst = nullptr;      // null: off
+  int img_dst_host = 0;
+  uint8_t *img_stage[2] = {};      // host flavours: [img_stage_frames][rows][cols][3] each
+  int img_stage_frames = 0;
+  cudaStream_t img_stream = nullptr;  // copies the images out, next to the frame copies of copy_stream
+  cudaEvent_t ev_img_ready[2] = {}, ev_img_copied[2] = {};
+  StageTimer timer;  // optional per-stage timing, on ctx->stream (the serial schedule)
 };
-
-static void fe_tic(sfe_frontend *fe, int stage) {
-  if (!fe->timing) return;
-  while (fe->tev->size() < fe->tused + 2) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    fe->tev->push_back(e);
-  }
-  cudaEventRecord((*fe->tev)[fe->tused], fe->ctx->stream);
-  fe->tstage->push_back(stage);
-}
-static void fe_toc(sfe_frontend *fe) {
-  if (!fe->timing) return;
-  cudaEventRecord((*fe->tev)[fe->tused + 1], fe->ctx->stream);
-  fe->tused += 2;
-}
 
 // The streams of the overlapped schedule.  The match side (submap + ICP) is the longer chain, so its CTAs go first
 // when both sides have work ready; SFE_FE_OVERLAP_PRIO=features|equal (development switch, read when a front end is
@@ -304,10 +231,7 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
               "sfe_frontend_create: cap_source / cap_target must be in [1, 65535]");
   SFE_CUDA(cudaSetDevice(ctx->device));
   sfe_frontend *fe = new sfe_frontend();
-  memset(fe, 0, sizeof(*fe));
   fe->ctx = ctx, fe->maps = maps, fe->p = *params, fe->max_frames = max_frames;
-  fe->tev = new std::vector<cudaEvent_t>();
-  fe->tstage = new std::vector<int>();
   const size_t F = max_frames, cap = params->cap_points, tcap = (size_t)params->window * cap;
   const size_t wpr = (params->B + 31) / 32;
   FE_ALLOC(fe->frames, F * params->R * params->B);
@@ -395,11 +319,6 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
     if (fe->ev_img_ready[k]) cudaEventDestroy(fe->ev_img_ready[k]);
     if (fe->ev_img_copied[k]) cudaEventDestroy(fe->ev_img_copied[k]);
   }
-  if (fe->tev) {
-    for (auto e : *fe->tev) cudaEventDestroy(e);
-    delete fe->tev;
-  }
-  delete fe->tstage;
   delete fe;
 }
 
@@ -495,45 +414,45 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_
   const sfe_frontend_params &p = fe->p;
   const size_t cap = p.cap_points, wpr = (p.B + 31) / 32;
   uint32_t *bits = fe->bits + (size_t)f0 * p.R * wpr;
-  fe_tic(fe, SFE_FE_CFAR);
+  fe->timer.tic(st, SFE_FE_CFAR);
   int rc = cfar_run(ctx, st, frames_dev, SFE_U8, n, p.R, p.B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank, p.tau,
                     p.gate_enable, p.gate_threshold, nullptr, nullptr, bits, 0);
-  fe_toc(fe);
+  fe->timer.toc(st);
   if (rc != SFE_OK) return rc;
-  fe_tic(fe, SFE_FE_CART);
+  fe->timer.tic(st, SFE_FE_CART);
   rc = cart_points_run(ctx, st, fe->maps, nullptr, bits, n, (int)cap, fe->ij + (size_t)f0 * cap * 2,
                        fe->xy_a + (size_t)f0 * cap * 2, fe->cnt_a + f0);
-  fe_toc(fe);
+  fe->timer.toc(st);
   if (rc != SFE_OK) return rc;
   // feature_extraction.py:241-249
   const float *cur = fe->xy_a;
   const int32_t *cur_cnt = fe->cnt_a;
   if (p.resolution > 0.f) {
-    fe_tic(fe, SFE_FE_DOWNSAMPLE);
+    fe->timer.tic(st, SFE_FE_DOWNSAMPLE);
     static const int ds_split = [] {  // development switch: SFE_FE_DS_SPLIT=<points> (0: one launch)
       const char *e = getenv("SFE_FE_DS_SPLIT");
       return e ? atoi(e) : FE_DS_SPLIT;
     }();
     rc = downsample_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.resolution, fe->xy_b, fe->idx,
                         fe->cnt_b + f0, ds_split);
-    fe_toc(fe);
+    fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
     cur = fe->xy_b, cur_cnt = fe->cnt_b;
   }
   if (p.outlier_min_points > 1) {
     float *dst = (cur == fe->xy_a) ? fe->xy_b : fe->xy_a;
-    fe_tic(fe, SFE_FE_OUTLIER);
+    fe->timer.tic(st, SFE_FE_OUTLIER);
     rc = remove_outlier_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.outlier_radius,
                             p.outlier_min_points, dst, fe->idx, fe->cnt_c + f0, FE_RO_SPLIT);
-    fe_toc(fe);
+    fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
   }
   if (p.flip_lateral) {
     const int32_t *cnt;
     float *cloud = const_cast<float *>(fe_cloud(fe, &cnt));
-    fe_tic(fe, SFE_FE_OUTLIER);
+    fe->timer.tic(st, SFE_FE_OUTLIER);
     flip_lateral_kernel<<<n, 128, 0, st>>>(cloud + 2 * (size_t)f0 * cap, cnt + f0, (int)cap, n);
-    fe_toc(fe);
+    fe->timer.toc(st);
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;
   }
@@ -562,7 +481,7 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const int cap = p.cap_points, tcap = p.window * cap;
   const int32_t *cnt;
   const float *cloud = fe_cloud(fe, &cnt);
-  fe_tic(fe, SFE_FE_SUBMAP);
+  fe->timer.tic(st, SFE_FE_SUBMAP);
   assemble_targets_kernel<<<n, 256, 0, st>>>(cloud, cnt, cap, fe->rel, f0, f0 + n, p.window, fe->tgt_a, fe->tcnt_a,
                                              tcap, fe->guess, fe->carry_xy, fe->carry_cnt, fe->carry_n);
   SFE_CUDA(cudaGetLastError());
@@ -576,8 +495,8 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
     if (rc != SFE_OK) return rc;
     tgt = fe->tgt_b, tcnt = fe->tcnt_b;
   }
-  fe_toc(fe);
-  fe_tic(fe, SFE_FE_ICP);
+  fe->timer.toc(st);
+  fe->timer.tic(st, SFE_FE_ICP);
   // Two launches by problem size: a sonar frame's filtered cloud is a few hundred points, far below the
   // capacities the buffers are sized for, and the ICP kernel's occupancy is set by its shared-memory footprint.
   // The first launch is sized for the common case (7 CTAs per SM instead of 4) and leaves bigger problems
@@ -596,7 +515,7 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
                  nullptr, nullptr, n, p.cap_source, p.cap_target, fe->guess + 9 * (size_t)f0,
                  fe->T + 9 * (size_t)f0, fe->iters + f0, fe->inliers + f0, fe->status + f0, fe->cnt_a + f0, cap, 2,
                  ns_small, nt_small);
-  fe_toc(fe);
+  fe->timer.toc(st);
   return rc;
 }
 
@@ -655,31 +574,14 @@ int sfe_frontend_set_overlap(sfe_frontend *fe, int sub_batch_frames) {
 
 int sfe_frontend_set_timing(sfe_frontend *fe, int enable) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_timing: null handle");
-  fe->timing = enable != 0;
-  fe->tused = 0;
-  fe->tstage->clear();
-  for (int i = 0; i < SFE_FE_STAGES; ++i) fe->stage_ms[i] = 0.0, fe->stage_launches[i] = 0;
+  fe->timer.reset(enable != 0);
   return SFE_OK;
 }
 
 int sfe_frontend_get_timing(sfe_frontend *fe, double *stage_ms, int64_t *stage_calls) {
   SFE_REQUIRE(fe && stage_ms, "sfe_frontend_get_timing: null argument");
   SFE_CUDA(cudaSetDevice(fe->ctx->device));
-  SFE_CUDA(cudaStreamSynchronize(fe->ctx->stream));
-  for (size_t k = 0; k + 1 < fe->tused + 1 && 2 * k + 1 < fe->tused + 1 && k < fe->tstage->size(); ++k) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, (*fe->tev)[2 * k], (*fe->tev)[2 * k + 1]) == cudaSuccess) {
-      fe->stage_ms[(*fe->tstage)[k]] += ms;
-      fe->stage_launches[(*fe->tstage)[k]]++;
-    }
-  }
-  fe->tused = 0;
-  fe->tstage->clear();
-  for (int i = 0; i < SFE_FE_STAGES; ++i) {
-    stage_ms[i] = fe->stage_ms[i];
-    if (stage_calls) stage_calls[i] = fe->stage_launches[i];
-  }
-  return SFE_OK;
+  return fe->timer.collect(fe->ctx->stream, SFE_FE_STAGES, stage_ms, stage_calls);
 }
 
 }  // extern "C"
@@ -716,6 +618,93 @@ static int fe_run_overlapped(sfe_frontend *fe, const uint8_t *frames_dev, const 
   return rc != SFE_OK ? rc : (rj != SFE_OK ? rj : rm);
 }
 
+// The start of a host flavour after its argument checks, for n_frames > 0: the device, the default chunk size and the
+// feature-image staging.
+static int fe_host_begin(sfe_frontend *fe, int n_frames, int &chunk_frames, const char *what) {
+  SFE_CUDA(cudaSetDevice(fe->ctx->device));
+  if (chunk_frames <= 0) chunk_frames = 256;
+  return fe_images_begin(fe, n_frames, chunk_frames, what);
+}
+
+// The end of a host flavour: the carried window moves on, the results go to the host and the call waits for them.
+static int fe_host_finish(sfe_frontend *fe, const double *poses_host, int n_frames, float *T_host, int32_t *iters_host,
+                          int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
+  sfe_ctx *ctx = fe->ctx;
+  int rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(inliers_host, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(status_host, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  if (npoints_host) {
+    const int32_t *cnt;
+    fe_cloud(fe, &cnt);
+    SFE_CUDA(cudaMemcpyAsync(npoints_host, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SFE_OK;
+}
+
+// The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
+// fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
+// so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
+static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sfe_ctx *), const uint8_t *bytes,
+                                  const int64_t *offsets, const double *poses_host, int n_frames, int chunk_frames,
+                                  float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                                  int32_t *npoints_host, const char *what) {
+  SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
+              "%s: null argument", what);
+  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
+              fe->max_frames);
+  SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
+  if (n_frames == 0) return SFE_OK;
+  int rc = fe_host_begin(fe, n_frames, chunk_frames, what);
+  if (rc != SFE_OK) return rc;
+  ImagesDrained drained{fe};
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  StreamDecoder *dec = decoder(ctx);
+  dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B);
+  for (int i = 0; i < n_frames; ++i)
+    if (dec->frame_status(i) != 0) {
+      set_error("%s: frame %d: %s", what, i, dec->message(dec->frame_status(i)));
+      return SFE_ERR_ARG;
+    }
+  rc = dec->reserve(ctx, chunk_frames, 0);
+  if (rc == SFE_OK) rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
+  if (rc == SFE_OK) rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  int32_t *st_host = static_cast<int32_t *>(ctx->pinned);
+  const int32_t *st_dev = static_cast<const int32_t *>(dec->status.ptr);
+  auto decode = [&](int f0, int k) -> int {
+    const int n = std::min(chunk_frames, n_frames - f0);
+    int r = dec->decode_chunk(ctx, f0, n, fe->frames + (size_t)f0 * fbytes);
+    if (r != SFE_OK) return r;
+    SFE_CUDA(cudaMemcpyAsync(st_host + f0, st_dev + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
+    return SFE_OK;
+  };
+  rc = decode(0, 0);
+  int k = 0;
+  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
+    const int n = std::min(chunk_frames, n_frames - f0);
+    if (f0 + chunk_frames < n_frames) rc = decode(f0 + chunk_frames, k + 1);
+    if (rc != SFE_OK) break;
+    SFE_CUDA(cudaEventSynchronize(fe->ev_copy[k & 1]));
+    for (int i = f0; i < f0 + n; ++i)
+      if (st_host[i] != 0) {
+        SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+        set_error("%s: frame %d: %s", what, i, dec->message(st_host[i]));
+        return SFE_ERR_ARG;
+      }
+    rc = fe_render_chunk(fe, f0, n, k, what);
+    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
+    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
+  }
+  if (rc != SFE_OK) return rc;
+  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
+}
+
 extern "C" {
 
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
@@ -733,7 +722,7 @@ int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const doub
     if (rc != SFE_OK) return rc;
   }
   // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
-  if (fe->overlap > 0 && !fe->timing) return fe_run_overlapped(fe, frames_dev, poses_host, n_frames);
+  if (fe->overlap > 0 && !fe->timer.on) return fe_run_overlapped(fe, frames_dev, poses_host, n_frames);
   rc = fe_features(fe, fe->ctx->stream, frames_dev, 0, n_frames);
   if (rc != SFE_OK) return rc;
   rc = fe_match(fe, fe->ctx->stream, 0, n_frames);
@@ -765,150 +754,43 @@ int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const do
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_host: %d frames exceed max_frames %d",
               n_frames, fe->max_frames);
   if (n_frames == 0) return SFE_OK;
-  sfe_ctx *ctx = fe->ctx;
-  SFE_CUDA(cudaSetDevice(ctx->device));
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
-  if (chunk_frames <= 0) chunk_frames = 256;
-  int rc0 = fe_images_begin(fe, n_frames, chunk_frames, "sfe_frontend_run_host");
-  if (rc0 != SFE_OK) return rc0;
+  int rc = fe_host_begin(fe, n_frames, chunk_frames, "sfe_frontend_run_host");
+  if (rc != SFE_OK) return rc;
   ImagesDrained drained{fe};
-  rc0 = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc0 != SFE_OK) return rc0;
+  rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
   // frame chunks stream in on the copy stream; the feature stages of chunk k run while chunk k+1 copies
   int k = 0;
   for (int f0 = 0; f0 < n_frames; f0 += chunk_frames, ++k) {
-    const int n = (n_frames - f0) < chunk_frames ? (n_frames - f0) : chunk_frames;
+    const int n = std::min(chunk_frames, n_frames - f0);
     SFE_CUDA(cudaMemcpyAsync(fe->frames + (size_t)f0 * fbytes, frames_host + (size_t)f0 * fbytes, (size_t)n * fbytes,
                              cudaMemcpyHostToDevice, fe->copy_stream));
     SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
     SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
-    int rc = fe_render_chunk(fe, f0, n, k, "sfe_frontend_run_host");
+    rc = fe_render_chunk(fe, f0, n, k, "sfe_frontend_run_host");
     if (rc != SFE_OK) return rc;
     rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
     if (rc != SFE_OK) return rc;
     rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
     if (rc != SFE_OK) return rc;
   }
-  int rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(inliers_host, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(status_host, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  if (npoints_host) {
-    const int32_t *cnt;
-    fe_cloud(fe, &cnt);
-    SFE_CUDA(cudaMemcpyAsync(npoints_host, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SFE_OK;
+  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
 }
-
-}  // extern "C"
-
-// The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
-// fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
-// so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
-// Fmt::status is 0 for a frame the decoder takes (SFE_JPEG_OK, SFE_PNG_OK).
-template <class Fmt>
-static int fe_run_compressed(sfe_frontend *fe, typename Fmt::Batch *bt, const double *poses_host, int n_frames,
-                             int chunk_frames, const char *what) {
-  sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
-  for (int i = 0; i < n_frames; ++i)
-    if (Fmt::status(bt, i) != 0) {
-      set_error("%s: frame %d: %s", what, i, Fmt::message(Fmt::status(bt, i)));
-      return SFE_ERR_ARG;
-    }
-  typename Fmt::State *js;
-  int rc = Fmt::begin(ctx, *bt, chunk_frames, &js);
-  if (rc != SFE_OK) return rc;
-  rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
-  if (rc != SFE_OK) return rc;
-  int32_t *st_host = static_cast<int32_t *>(ctx->pinned);
-  rc = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  auto decode = [&](int f0, int k) -> int {
-    const int n = std::min(chunk_frames, n_frames - f0);
-    int r = Fmt::decode(ctx, js, *bt, f0, n, fe->frames + (size_t)f0 * fbytes);
-    if (r != SFE_OK) return r;
-    SFE_CUDA(cudaMemcpyAsync(st_host + f0, Fmt::status_dev(js) + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost,
-                             ctx->stream));
-    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
-    return SFE_OK;
-  };
-  rc = decode(0, 0);
-  int k = 0;
-  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
-    const int n = std::min(chunk_frames, n_frames - f0);
-    if (f0 + chunk_frames < n_frames) rc = decode(f0 + chunk_frames, k + 1);
-    if (rc != SFE_OK) break;
-    SFE_CUDA(cudaEventSynchronize(fe->ev_copy[k & 1]));
-    for (int i = f0; i < f0 + n; ++i)
-      if (st_host[i] != 0) {
-        SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-        set_error("%s: frame %d: %s", what, i, Fmt::message(st_host[i]));
-        return SFE_ERR_ARG;
-      }
-    rc = fe_render_chunk(fe, f0, n, k, what);
-    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
-    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
-  }
-  return rc;
-}
-
-template <class Fmt>
-static int fe_run_compressed_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
-                                  const double *poses_host, int n_frames, int chunk_frames, float *T_host,
-                                  int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
-                                  int32_t *npoints_host, const char *what) {
-  SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
-              "%s: null argument", what);
-  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
-              fe->max_frames);
-  for (int i = 0; i < n_frames; ++i)
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "%s: offsets must be non-decreasing", what);
-  if (n_frames == 0) return SFE_OK;
-  sfe_ctx *ctx = fe->ctx;
-  SFE_CUDA(cudaSetDevice(ctx->device));
-  if (chunk_frames <= 0) chunk_frames = 256;
-  int rc = fe_images_begin(fe, n_frames, chunk_frames, what);
-  if (rc != SFE_OK) return rc;
-  ImagesDrained drained{fe};
-  typename Fmt::Batch *bt;
-  rc = Fmt::parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, &bt);
-  if (rc == SFE_OK) rc = fe_run_compressed<Fmt>(fe, bt, poses_host, n_frames, chunk_frames, what);
-  Fmt::free(bt);
-  if (rc != SFE_OK) return rc;
-  rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(inliers_host, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(status_host, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  if (npoints_host) {
-    const int32_t *cnt;
-    fe_cloud(fe, &cnt);
-    SFE_CUDA(cudaMemcpyAsync(npoints_host, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SFE_OK;
-}
-
-extern "C" {
 
 int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                                int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
                                int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host<JpegFormat>(fe, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                                            inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
+  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                                inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
 }
 
 int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                               int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host<PngFormat>(fe, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                                           inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
+  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                                inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
 }
 
 }  // extern "C"

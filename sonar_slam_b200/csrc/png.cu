@@ -31,7 +31,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "stream_decode.cuh"
 
 namespace sfe {
 
@@ -629,62 +629,6 @@ __global__ void __launch_bounds__(32 * PNG_WARPS) png_unfilter_kernel(const PDes
 }
 
 // ------------------------------------------------------------------ host: batches of streams
-struct PngBatch {
-  const uint8_t *bytes = nullptr;
-  const int64_t *offsets = nullptr;
-  int n = 0, R = 0, B = 0;
-  std::vector<PHeader> hdr;
-};
-
-struct PngState {
-  cudaStream_t copy = nullptr;
-  cudaEvent_t ev_copied[2] = {}, ev_used[2] = {}, ev_ready = nullptr;
-  uint8_t *pin[2] = {};
-  size_t pin_cap[2] = {};
-  Buffer dev_in[2], scr, status, out;
-  int turn = 0;
-  X2N x2n;
-  bool timing = false;            // sfe_png_set_timing / _get_timing
-  std::vector<cudaEvent_t> tev;   // pool; pair [2k, 2k+1] brackets interval k
-  std::vector<int> tstage;
-  size_t tused = 0;
-  double stage_ms[SFE_PNG_STAGES] = {};
-  int64_t stage_calls[SFE_PNG_STAGES] = {};
-};
-
-static void pt_tic(PngState *ps, cudaStream_t st, int stage) {
-  if (!ps->timing) return;
-  while (ps->tev.size() < ps->tused + 2) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    ps->tev.push_back(e);
-  }
-  cudaEventRecord(ps->tev[ps->tused], st);
-  ps->tstage.push_back(stage);
-}
-static void pt_toc(PngState *ps, cudaStream_t st) {
-  if (!ps->timing) return;
-  cudaEventRecord(ps->tev[ps->tused + 1], st);
-  ps->tused += 2;
-}
-
-static void png_state_free(void *p) {
-  PngState *s = static_cast<PngState *>(p);
-  if (!s) return;
-  if (s->copy) cudaStreamSynchronize(s->copy), cudaStreamDestroy(s->copy);
-  for (int k = 0; k < 2; ++k) {
-    if (s->ev_copied[k]) cudaEventDestroy(s->ev_copied[k]);
-    if (s->ev_used[k]) cudaEventDestroy(s->ev_used[k]);
-    if (s->pin[k]) cudaFreeHost(s->pin[k]);
-    if (s->dev_in[k].ptr) cudaFree(s->dev_in[k].ptr);
-  }
-  if (s->ev_ready) cudaEventDestroy(s->ev_ready);
-  for (cudaEvent_t e : s->tev) cudaEventDestroy(e);
-  for (Buffer *b : {&s->scr, &s->status, &s->out})
-    if (b->ptr) cudaFree(b->ptr);
-  delete s;
-}
-
 static uint32_t multmodp_host(uint32_t a, uint32_t b) {
   uint32_t m = 1u << 31, p = 0;
   for (;;) {
@@ -698,23 +642,6 @@ static uint32_t multmodp_host(uint32_t a, uint32_t b) {
   return p;
 }
 
-static int png_state(sfe_ctx *ctx, PngState **out) {
-  if (!ctx->png) {
-    PngState *s = new PngState();
-    ctx->png = s, ctx->png_free = png_state_free;
-    s->x2n.t[0] = 1u << 30;  // x^1
-    for (int k = 1; k < 32; ++k) s->x2n.t[k] = multmodp_host(s->x2n.t[k - 1], s->x2n.t[k - 1]);
-    SFE_CUDA(cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      SFE_CUDA(cudaEventCreateWithFlags(&s->ev_copied[k], cudaEventDisableTiming));
-      SFE_CUDA(cudaEventCreateWithFlags(&s->ev_used[k], cudaEventDisableTiming));
-    }
-    SFE_CUDA(cudaEventCreateWithFlags(&s->ev_ready, cudaEventDisableTiming));
-  }
-  *out = static_cast<PngState *>(ctx->png);
-  return SFE_OK;
-}
-
 // the device-side bytes of a chunk of frames [f0, f0 + nf): descriptors, IDAT table, IDAT spans
 struct PngPlan {
   std::vector<PDesc> desc;
@@ -724,7 +651,7 @@ struct PngPlan {
   size_t off_idat = 0, off_bytes = 0, total = 0;
 };
 
-static void plan_png_chunk(const PngBatch &bt, int f0, int nf, PngPlan &p) {
+static void plan_png_chunk(const StreamBatch<PHeader> &bt, int f0, int nf, PngPlan &p) {
   p = PngPlan();
   p.desc.resize(nf);
   p.src.assign(nf, 0);
@@ -755,21 +682,37 @@ static void plan_png_chunk(const PngBatch &bt, int f0, int nf, PngPlan &p) {
   p.total = p.off_bytes + p.span_bytes + 16;
 }
 
-int png_batch_parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, PngBatch **out) {
-  PngBatch *b = new PngBatch();
-  b->bytes = bytes, b->offsets = offsets, b->n = n, b->R = R, b->B = B;
-  b->hdr.resize(n);
-  for (int i = 0; i < n; ++i) {
-    parse_png(bytes + offsets[i], offsets[i + 1] - offsets[i], b->hdr[i]);
-    if (b->hdr[i].status == SFE_PNG_OK && (b->hdr[i].H != R || b->hdr[i].W != B)) b->hdr[i].status = SFE_PNG_SIZE;
-  }
-  *out = b;
-  return SFE_OK;
-}
-void png_batch_free(PngBatch *b) { delete b; }
-int png_batch_status(const PngBatch *b, int i) { return b->hdr[i].status; }
+struct PngState final : StreamDecoder {
+  StreamBatch<PHeader> bt;
+  Buffer scr;
+  X2N x2n;
 
-static int png_reserve(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int chunk, size_t out_bytes) {
+  PngState() {
+    x2n.t[0] = 1u << 30;  // x^1
+    for (int k = 1; k < 32; ++k) x2n.t[k] = multmodp_host(x2n.t[k - 1], x2n.t[k - 1]);
+  }
+  ~PngState() override {
+    if (scr.ptr) cudaFree(scr.ptr);
+  }
+  // Inflate is serial within a frame and latency-bound: a chunk of 32 frames (warps) per SM keeps every scheduler
+  // busy.  A 512 x 512 ping takes about 0.5 MB of scratch, so a chunk of ~4k frames takes about 2 GB.
+  int chunk_frames(const sfe_ctx *ctx) const override { return std::max(256, ctx->sm_count * 32); }
+  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B) override {
+    bt.parse(bytes, offsets, n, R, B, parse_png, SFE_PNG_SIZE);
+  }
+  int frame_status(int i) const override { return bt.hdr[i].status; }
+  const char *message(int status) const override { return sfe_png_status_message(status); }
+  int reserve(sfe_ctx *ctx, int chunk, size_t out_bytes) override;
+  int decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) override;
+};
+
+StreamDecoder *png_decoder(sfe_ctx *ctx) {
+  if (!ctx->png) ctx->png = new PngState();
+  return ctx->png;
+}
+void destroy(PngState *s) { delete s; }
+
+int PngState::reserve(sfe_ctx *ctx, int chunk, size_t out_bytes) {
   size_t in_max = 0, scr_max = 0;
   PngPlan p;
   for (int f0 = 0; f0 < bt.n; f0 += chunk) {
@@ -777,34 +720,16 @@ static int png_reserve(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int chunk
     in_max = std::max(in_max, p.total);
     scr_max = std::max(scr_max, (size_t)p.scr_bytes);
   }
-  SFE_CUDA(cudaStreamSynchronize(ps->copy));
-  for (int k = 0; k < 2; ++k) {
-    int rc = ensure(ctx, ps->dev_in[k], in_max);
-    if (rc != SFE_OK) return rc;
-    if (ps->pin_cap[k] < in_max) {
-      if (ps->pin[k]) SFE_CUDA(cudaFreeHost(ps->pin[k]));
-      ps->pin[k] = nullptr, ps->pin_cap[k] = 0;
-      SFE_CUDA(cudaMallocHost((void **)&ps->pin[k], in_max + in_max / 4));
-      ps->pin_cap[k] = in_max + in_max / 4;
-    }
-  }
-  int rc = ensure(ctx, ps->scr, scr_max + 16);
-  if (rc == SFE_OK) rc = ensure(ctx, ps->status, 4 * (size_t)bt.n + 16);
-  if (rc == SFE_OK && out_bytes) rc = ensure(ctx, ps->out, out_bytes);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaEventRecord(ps->ev_ready, ctx->stream));
-  SFE_CUDA(cudaStreamWaitEvent(ps->copy, ps->ev_ready, 0));
-  return SFE_OK;
+  const int rc = ensure(ctx, scr, scr_max + 16);
+  return rc == SFE_OK ? reserve_common(ctx, bt.n, in_max, out_bytes) : rc;
 }
 
-// Decode frames [f0, f0 + nf) into out_dev (uint8 [nf][R][B]); per-frame status into the state's device status
-// array at [f0, f0 + nf).  Asynchronous on ctx->stream; the bytes go in on the copy stream.
-static int png_decode_chunk(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int f0, int nf, uint8_t *out_dev) {
+int PngState::decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) {
   PngPlan p;
   plan_png_chunk(bt, f0, nf, p);
-  const int turn = ps->turn ^= 1;
-  SFE_CUDA(cudaEventSynchronize(ps->ev_copied[turn]));  // the pinned block is free again
-  uint8_t *pin = ps->pin[turn];
+  uint8_t *pin, *dev;
+  int rc = stager.acquire(&pin);
+  if (rc != SFE_OK) return rc;
   memcpy(pin, p.desc.data(), sizeof(PDesc) * nf);
   memcpy(pin + p.off_idat, p.idat.data(), sizeof(PIdat) * p.idat.size());
   for (int i = 0; i < nf; ++i) {
@@ -812,76 +737,25 @@ static int png_decode_chunk(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int 
     const PHeader &h = bt.hdr[f0 + i];
     memcpy(pin + p.off_bytes + p.src[i], bt.bytes + bt.offsets[f0 + i] + h.span0, h.span1 - h.span0);
   }
-  uint8_t *dev = static_cast<uint8_t *>(ps->dev_in[turn].ptr);
-  SFE_CUDA(cudaStreamWaitEvent(ps->copy, ps->ev_used[turn], 0));  // kernels of two chunks ago are done with it
-  SFE_CUDA(cudaMemcpyAsync(dev, pin, p.off_bytes + p.span_bytes, cudaMemcpyHostToDevice, ps->copy));
-  SFE_CUDA(cudaEventRecord(ps->ev_copied[turn], ps->copy));
-  SFE_CUDA(cudaStreamWaitEvent(ctx->stream, ps->ev_copied[turn], 0));
+  rc = stager.upload(ctx, p.off_bytes + p.span_bytes, &dev);
+  if (rc != SFE_OK) return rc;
   const PDesc *desc = reinterpret_cast<const PDesc *>(dev);
   const PIdat *idat = reinterpret_cast<const PIdat *>(dev + p.off_idat);
-  uint8_t *scr = static_cast<uint8_t *>(ps->scr.ptr);
-  int32_t *st = static_cast<int32_t *>(ps->status.ptr) + f0;
+  uint8_t *s = static_cast<uint8_t *>(scr.ptr);
+  int32_t *st = static_cast<int32_t *>(status.ptr) + f0;
   const int wblocks = (nf + PNG_WARPS - 1) / PNG_WARPS;
-  pt_tic(ps, ctx->stream, SFE_PNG_T_CHECK);
-  png_check_kernel<<<nf, PNG_CHECK_T, 0, ctx->stream>>>(desc, idat, dev + p.off_bytes, scr, st, ps->x2n);
-  pt_toc(ps, ctx->stream);
-  pt_tic(ps, ctx->stream, SFE_PNG_T_INFLATE);
-  png_inflate_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, scr, st);
-  pt_toc(ps, ctx->stream);
-  pt_tic(ps, ctx->stream, SFE_PNG_T_UNFILTER);
-  png_unfilter_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, scr, st, out_dev,
-                                                                   (int64_t)bt.R * bt.B);
-  pt_toc(ps, ctx->stream);
+  timer.tic(ctx->stream, SFE_PNG_T_CHECK);
+  png_check_kernel<<<nf, PNG_CHECK_T, 0, ctx->stream>>>(desc, idat, dev + p.off_bytes, s, st, x2n);
+  timer.toc(ctx->stream);
+  timer.tic(ctx->stream, SFE_PNG_T_INFLATE);
+  png_inflate_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, s, st);
+  timer.toc(ctx->stream);
+  timer.tic(ctx->stream, SFE_PNG_T_UNFILTER);
+  png_unfilter_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, s, st, out_dev, (int64_t)bt.R * bt.B);
+  timer.toc(ctx->stream);
   ctx->launches += 3;
   SFE_CUDA(cudaGetLastError());
-  SFE_CUDA(cudaEventRecord(ps->ev_used[turn], ctx->stream));
-  return SFE_OK;
-}
-
-int png_begin(sfe_ctx *ctx, const PngBatch &bt, int chunk, PngState **ps) {
-  int rc = png_state(ctx, ps);
-  if (rc != SFE_OK) return rc;
-  return png_reserve(ctx, *ps, bt, chunk, 0);
-}
-int png_decode_frames(sfe_ctx *ctx, PngState *ps, const PngBatch &bt, int f0, int nf, uint8_t *out_dev) {
-  return png_decode_chunk(ctx, ps, bt, f0, nf, out_dev);
-}
-const int32_t *png_status_dev(const PngState *ps) { return static_cast<const int32_t *>(ps->status.ptr); }
-
-
-static int png_decode_all(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
-                          uint8_t *out_dev, uint8_t *out_host, int32_t *status_host, const char *what) {
-  SFE_REQUIRE(ctx && bytes && offsets && status_host && (out_dev || out_host), "%s: null argument", what);
-  SFE_REQUIRE(n >= 0 && R > 0 && B > 0, "%s: bad shape n=%d R=%d B=%d", what, n, R, B);
-  for (int i = 0; i < n; ++i)
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "%s: offsets must be non-decreasing", what);
-  if (n == 0) return SFE_OK;
-  SFE_CUDA(cudaSetDevice(ctx->device));
-  PngBatch *bt;
-  png_batch_parse(bytes, offsets, n, R, B, &bt);
-  PngState *ps;
-  int rc = png_state(ctx, &ps);
-  const size_t fb = (size_t)R * B;
-  // Inflate is serial within a frame and latency-bound: a chunk of 32 frames (warps) per SM keeps every scheduler
-  // busy.  A 512 x 512 ping takes about 0.5 MB of scratch, so a chunk of ~4k frames takes about 2 GB.
-  const int chunk = std::max(256, ctx->sm_count * 32);
-  const bool via_out = !out_dev;
-  if (rc == SFE_OK) rc = png_reserve(ctx, ps, *bt, chunk, via_out ? fb * chunk : 0);
-  for (int f0 = 0; rc == SFE_OK && f0 < n; f0 += chunk) {
-    const int nf = std::min(chunk, n - f0);
-    uint8_t *o = via_out ? static_cast<uint8_t *>(ps->out.ptr) : out_dev + fb * f0;
-    rc = png_decode_chunk(ctx, ps, *bt, f0, nf, o);
-    if (rc != SFE_OK) break;
-    if (out_host) {
-      cudaError_t e = cudaMemcpyAsync(out_host + fb * f0, o, fb * nf, cudaMemcpyDeviceToHost, ctx->stream);
-      if (e != cudaSuccess) rc = SFE_ERR_CUDA, set_error("%s: %s", what, cudaGetErrorString(e));
-    }
-  }
-  png_batch_free(bt);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaMemcpyAsync(status_host, ps->status.ptr, 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SFE_OK;
+  return stager.done(ctx);
 }
 
 }  // namespace sfe
@@ -910,8 +784,8 @@ const char *sfe_png_status_message(int status) {
 int sfe_png_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, int32_t *info) {
   SFE_REQUIRE(bytes && offsets && info, "sfe_png_inspect_host: null argument");
   SFE_REQUIRE(n >= 0, "sfe_png_inspect_host: negative count");
+  SFE_REQUIRE(offsets_ok(offsets, n), "sfe_png_inspect_host: offsets must be non-decreasing");
   for (int i = 0; i < n; ++i) {
-    SFE_REQUIRE(offsets[i + 1] >= offsets[i] && offsets[i] >= 0, "sfe_png_inspect_host: offsets must be non-decreasing");
     PHeader h;
     parse_png(bytes + offsets[i], offsets[i + 1] - offsets[i], h);
     int32_t *o = info + (size_t)SFE_PNG_INFO * i;
@@ -923,50 +797,27 @@ int sfe_png_inspect_host(const uint8_t *bytes, const int64_t *offsets, int n, in
 int sfe_png_decode_host(sfe_ctx *ctx, const uint8_t *bytes, const int64_t *offsets, int n, int R, int B,
                         uint8_t *out_host, int32_t *status_host) {
   SFE_REQUIRE(out_host, "sfe_png_decode_host: null output");
-  return png_decode_all(ctx, bytes, offsets, n, R, B, nullptr, out_host, status_host, "sfe_png_decode_host");
+  return decode_all(ctx, png_decoder, bytes, offsets, n, R, B, nullptr, out_host, status_host, "sfe_png_decode_host");
 }
 
 int sfe_png_decode_to_dev(sfe_ctx *ctx, const uint8_t *bytes_host, const int64_t *offsets_host, int n, int R, int B,
                           uint8_t *out_dev, int32_t *status_host) {
   SFE_REQUIRE(out_dev, "sfe_png_decode_to_dev: null output");
-  return png_decode_all(ctx, bytes_host, offsets_host, n, R, B, out_dev, nullptr, status_host,
-                        "sfe_png_decode_to_dev");
+  return decode_all(ctx, png_decoder, bytes_host, offsets_host, n, R, B, out_dev, nullptr, status_host,
+                    "sfe_png_decode_to_dev");
 }
 
 int sfe_png_set_timing(sfe_ctx *ctx, int enable) {
   SFE_REQUIRE(ctx != nullptr, "sfe_png_set_timing: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  PngState *ps;
-  int rc = png_state(ctx, &ps);
-  if (rc != SFE_OK) return rc;
-  ps->timing = enable != 0;
-  ps->tused = 0;
-  ps->tstage.clear();
-  for (int i = 0; i < SFE_PNG_STAGES; ++i) ps->stage_ms[i] = 0.0, ps->stage_calls[i] = 0;
+  png_decoder(ctx)->timer.reset(enable != 0);
   return SFE_OK;
 }
 
 int sfe_png_get_timing(sfe_ctx *ctx, double *stage_ms, int64_t *stage_calls) {
   SFE_REQUIRE(ctx && stage_ms, "sfe_png_get_timing: null argument");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  PngState *ps;
-  int rc = png_state(ctx, &ps);
-  if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-  for (size_t k = 0; k < ps->tstage.size(); ++k) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, ps->tev[2 * k], ps->tev[2 * k + 1]) == cudaSuccess) {
-      ps->stage_ms[ps->tstage[k]] += ms;
-      ps->stage_calls[ps->tstage[k]]++;
-    }
-  }
-  ps->tused = 0;
-  ps->tstage.clear();
-  for (int i = 0; i < SFE_PNG_STAGES; ++i) {
-    stage_ms[i] = ps->stage_ms[i];
-    if (stage_calls) stage_calls[i] = ps->stage_calls[i];
-  }
-  return SFE_OK;
+  return png_decoder(ctx)->timer.collect(ctx->stream, SFE_PNG_STAGES, stage_ms, stage_calls);
 }
 
 }  // extern "C"

@@ -7,21 +7,13 @@ status naming the reason and stay on the host path.  Headers are parsed on the h
 """
 import numpy as np
 
-from . import _lib
+from . import _lib, _streams
+from ._streams import pack  # noqa: F401  (jpeg.pack: the packing of every codec)
 
 (OK, NOT_JPEG, TRUNCATED, PROGRESSIVE, LOSSLESS, ARITHMETIC, PRECISION, SAMPLING, COLORSPACE, ORIENTATION, SIZE,
  CORRUPT, BAD_HEADER) = range(13)                         # SFE_JPEG_* status
 GRAY, S444, S422, S420 = range(4)                        # sampling codes
 INFO_FIELDS = ("status", "height", "width", "components", "sampling", "restart_interval")
-
-
-def pack(streams):
-    """Sequence of byte strings -> (uint8 bytes [total], int64 offsets [n + 1])."""
-    streams = [bytes(s) for s in streams]
-    off = np.zeros(len(streams) + 1, np.int64)
-    off[1:] = np.cumsum([len(s) for s in streams])
-    buf = np.frombuffer(b"".join(streams), np.uint8) if off[-1] else np.zeros(1, np.uint8)
-    return np.ascontiguousarray(buf), off
 
 
 def status_message(status):
@@ -30,31 +22,19 @@ def status_message(status):
 
 def inspect(streams):
     """Headers only (no GPU): int32 [n, 6] rows (status, height, width, components, sampling, restart interval)."""
-    buf, off = streams if isinstance(streams, tuple) else pack(streams)
-    n = len(off) - 1
-    info = np.zeros((n, len(INFO_FIELDS)), np.int32)
-    _lib.check(_lib.load().sfe_jpeg_inspect_host(_lib.ptr(buf), _lib.ptr(off), n, _lib.ptr(info)),
-               "sfe_jpeg_inspect_host")
-    return info
+    return _streams.inspect("sfe_jpeg_", streams, INFO_FIELDS)
 
 
 def decode_host(streams, R, B, ctx=None):
     """Decode into host memory: (uint8 [n, R, B], status int32 [n]); a frame whose status is not OK is zeros."""
-    ctx = ctx or _lib.default_context()
-    buf, off = streams if isinstance(streams, tuple) else pack(streams)
-    n = len(off) - 1
-    out = np.zeros((n, int(R), int(B)), np.uint8)
-    st = np.zeros(n, np.int32)
-    _lib.check(ctx.lib.sfe_jpeg_decode_host(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B),
-                                            _lib.ptr(out), _lib.ptr(st)), "sfe_jpeg_decode_host")
-    return out, st
+    return _streams.decode_host("sfe_jpeg_", streams, R, B, ctx)
 
 
 def coefficients_host(streams, R, B, ctx=None):
     """Diagnostic: the dequantised coefficient blocks the device IDCT consumes, int32 [n, cap_blocks, 64] (natural
     order, blocks in decode order), and the status array."""
     ctx = ctx or _lib.default_context()
-    buf, off = streams if isinstance(streams, tuple) else pack(streams)
+    buf, off = _streams.packed(streams)
     n = len(off) - 1
     info = inspect((buf, off))
     cap = 1
@@ -75,14 +55,9 @@ STAGES = ("unstuff", "entropy", "idct_color")
 
 def set_timing(enable=True, ctx=None):
     """Per-stage device timing of the decoders on this context (CUDA events around every chunk's kernels)."""
-    ctx = ctx or _lib.default_context()
-    _lib.check(ctx.lib.sfe_jpeg_set_timing(ctx.handle, 1 if enable else 0), "sfe_jpeg_set_timing")
+    _streams.set_timing("sfe_jpeg_", enable, ctx)
 
 
 def get_timing(ctx=None):
     """dict stage -> (total ms, number of timed intervals) since set_timing(True)."""
-    ctx = ctx or _lib.default_context()
-    ms = np.zeros(len(STAGES), np.float64)
-    calls = np.zeros(len(STAGES), np.int64)
-    _lib.check(ctx.lib.sfe_jpeg_get_timing(ctx.handle, _lib.ptr(ms), _lib.ptr(calls)), "sfe_jpeg_get_timing")
-    return {k: (float(ms[i]), int(calls[i])) for i, k in enumerate(STAGES)}
+    return _streams.get_timing("sfe_jpeg_", STAGES, ctx)

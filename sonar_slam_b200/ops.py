@@ -9,7 +9,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, _streams
 
 ALG = {"CA": 0, "SOCA": 1, "GOCA": 2, "OS": 3}
 _ctx_cache = {}
@@ -169,27 +169,22 @@ def decode_jpeg(streams, R, B, device=None, ctx=None):
     sonar_slam_b200/jpeg.py).  streams: a sequence of bytes objects, or (bytes, offsets) from jpeg.pack.
     Returns (frames, status int32 [n] numpy): a frame whose status is not jpeg.OK is zeros.  The call returns once the
     frames are written (the statuses are read back)."""
-    from . import jpeg
-    buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
-    n = len(off) - 1
-    ctx = ctx or context(device)
-    out = torch.empty((n, int(R), int(B)), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
-    st = np.empty(n, np.int32)
-    _lib.check(ctx.lib.sfe_jpeg_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
-                                              _lib.ptr(st)), "sfe_jpeg_decode_to_dev")
-    return out, st
+    return _decode_to_dev("sfe_jpeg_decode_to_dev", streams, R, B, device, ctx)
 
 
 def decode_png(streams, R, B, device=None, ctx=None):
     """decode_jpeg for PNG streams (include/sonarfe.h: sfe_png_decode_to_dev; sonar_slam_b200/png.py)."""
-    from . import jpeg
-    buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
+    return _decode_to_dev("sfe_png_decode_to_dev", streams, R, B, device, ctx)
+
+
+def _decode_to_dev(name, streams, R, B, device, ctx):
+    buf, off = _streams.packed(streams)
     n = len(off) - 1
     ctx = ctx or context(device)
     out = torch.empty((n, int(R), int(B)), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
     st = np.empty(n, np.int32)
-    _lib.check(ctx.lib.sfe_png_decode_to_dev(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
-                                             _lib.ptr(st)), "sfe_png_decode_to_dev")
+    _lib.check(getattr(ctx.lib, name)(ctx.handle, _lib.ptr(buf), _lib.ptr(off), n, int(R), int(B), _dp(out),
+                                      _lib.ptr(st)), name)
     return out, st
 
 

@@ -10,7 +10,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib
+from . import _lib, _streams
 
 
 class FrontEnd:
@@ -82,30 +82,22 @@ class FrontEnd:
         jpeg.pack); the compressed bytes are copied and decoded on the device instead of copying raw frames
         (sfe_frontend_run_jpeg_host).  A stream that is rejected or fails to decode raises, naming the frame.
         images / image_lut: as run_host."""
-        from . import jpeg
-        buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
-        poses = np.ascontiguousarray(poses, np.float64)
-        n = len(off) - 1
-        o = out or self.alloc_results(n)
-        with self._images(images, n, False, image_lut):
-            _lib.check(self.lib.sfe_frontend_run_jpeg_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
-                                                           int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                           _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                           _lib.ptr(o["npoints"])), "sfe_frontend_run_jpeg_host")
-        return o
+        return self._run_compressed("sfe_frontend_run_jpeg_host", streams, poses, chunk_frames, out, images, image_lut)
 
     def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None):
         """run_jpeg_host for PNG streams (sfe_frontend_run_png_host)."""
-        from . import jpeg
-        buf, off = streams if isinstance(streams, tuple) else jpeg.pack(streams)
+        return self._run_compressed("sfe_frontend_run_png_host", streams, poses, chunk_frames, out, images, image_lut)
+
+    def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut):
+        buf, off = _streams.packed(streams)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
         o = out or self.alloc_results(n)
         with self._images(images, n, False, image_lut):
-            _lib.check(self.lib.sfe_frontend_run_png_host(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
-                                                          int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                          _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                          _lib.ptr(o["npoints"])), "sfe_frontend_run_png_host")
+            _lib.check(getattr(self.lib, name)(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
+                                               int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                                               _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])),
+                       name)
         return o
 
     @staticmethod
@@ -151,10 +143,7 @@ class FrontEnd:
 
     def get_timing(self):
         """dict stage -> (total ms, number of timed intervals) since set_timing(True)."""
-        ms = np.zeros(len(self.STAGES), np.float64)
-        calls = np.zeros(len(self.STAGES), np.int64)
-        _lib.check(self.lib.sfe_frontend_get_timing(self.handle, _lib.ptr(ms), _lib.ptr(calls)), "sfe_frontend_get_timing")
-        return {k: (float(ms[i]), int(calls[i])) for i, k in enumerate(self.STAGES)}
+        return _streams.read_timing(self.lib.sfe_frontend_get_timing, self.handle, self.STAGES)
 
     def close(self):
         if getattr(self, "handle", None):
