@@ -6,7 +6,7 @@
 #include <mutex>
 #include <vector>
 
-#include "common.cuh"
+#include "stages.cuh"
 
 namespace sfe {
 
@@ -74,9 +74,6 @@ int encode_tensor_map_3d(CUtensorMap *map, CUtensorMapDataType dt, size_t es, co
   }
   return SFE_OK;
 }
-
-int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
-             int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
 
 }  // namespace sfe
 
@@ -178,8 +175,8 @@ int sfe_cfar_dev(sfe_ctx *ctx, const void *img_dev, int dtype, int n_frames, int
                  float *thr_dev, uint32_t *bits_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_cfar_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return cfar_run(ctx, ctx->stream, img_dev, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable, gate_threshold,
-                  mask_dev, thr_dev, bits_dev, 0);
+  return cfar_run(ctx, ctx->stream, img_dev, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable,
+                  gate_threshold, mask_dev, thr_dev, bits_dev);
 }
 
 int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, int R, int B, int alg, int train_hs,
@@ -200,7 +197,7 @@ int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, i
   SFE_CUDA(cudaMemcpyAsync(ctx->stage_in[0].ptr, img_host, cells * es, cudaMemcpyHostToDevice, ctx->stream));
   rc = cfar_run(ctx, ctx->stream, ctx->stage_in[0].ptr, dtype, n_frames, R, B, alg, train_hs, guard_hs, k, tau, gate_enable,
                 gate_threshold, (uint8_t *)ctx->stage_out[0].ptr, thr_host ? (float *)ctx->stage_out[1].ptr : nullptr,
-                nullptr, 0);
+                nullptr);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(mask_host, ctx->stage_out[0].ptr, cells, cudaMemcpyDeviceToHost, ctx->stream));
   if (thr_host)
@@ -214,20 +211,6 @@ int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, i
 
 // ============================================================================ clouds / match / ICP
 namespace sfe {
-int downsample_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
-                   int dim, int n_max, float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count,
-                   int n_split = 0, int slot = SCR_CLOUD);
-int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
-                       int dim, int n_max, double radius, int min_points, float *out_pts, int32_t *out_idx,
-                       int32_t *out_count, int n_split = 0);
-int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off,
-            const int *src_cnt, const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points,
-            const int *src_id, const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out,
-            int *iters, int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
-            int class_ns = 0, int class_nt = 0, int force_threads = 0);
-int match_run(sfe_ctx *ctx, const float *ref_pts, const int *ref_off, const float *in_pts, const int *in_off, int P,
-              int nt_max, float max_dist, int32_t *ids, float *dists);
-
 // carve `n` sub-buffers out of one grow-only scratch block (256 B aligned each)
 struct Carver {
   char *base = nullptr;
@@ -246,8 +229,8 @@ int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_de
                        float resolution, float *out_pts_dev, int32_t *out_idx_dev, int32_t *out_count_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_downsample_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return downsample_run(ctx, ctx->stream, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, resolution, out_pts_dev, out_idx_dev,
-                        out_count_dev);
+  return downsample_run(ctx, ctx->stream, {pts_dev, off_dev, nullptr, n_max}, n_clouds, dim, resolution, out_pts_dev,
+                        out_idx_dev, out_count_dev, 0, SCR_CLOUD);
 }
 
 int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
@@ -255,8 +238,8 @@ int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *of
                            int32_t *out_count_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_remove_outlier_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return remove_outlier_run(ctx, ctx->stream, pts_dev, off_dev, nullptr, n_clouds, dim, n_max, radius, min_points, out_pts_dev,
-                            out_idx_dev, out_count_dev);
+  return remove_outlier_run(ctx, ctx->stream, {pts_dev, off_dev, nullptr, n_max}, n_clouds, dim, radius, min_points,
+                            out_pts_dev, out_idx_dev, out_count_dev, 0);
 }
 
 static int cloud_filter_host(sfe_ctx *ctx, int which, const float *pts_host, int n, int dim, float resolution,
@@ -286,9 +269,9 @@ static int cloud_filter_host(sfe_ctx *ctx, int which, const float *pts_host, int
     const int32_t off[2] = {0, n};
     SFE_CUDA(cudaMemcpyAsync(d_pts, pts_host, sizeof(float) * (size_t)n * dim, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
-    int rc = which == 0 ? downsample_run(ctx, ctx->stream, d_pts, d_off, nullptr, 1, dim, n, resolution, d_out, d_idx, d_cnt)
-                        : remove_outlier_run(ctx, ctx->stream, d_pts, d_off, nullptr, 1, dim, n, radius, min_points, d_out, d_idx,
-                                             d_cnt);
+    const PackedClouds in{d_pts, d_off, nullptr, n};
+    int rc = which == 0 ? downsample_run(ctx, ctx->stream, in, 1, dim, resolution, d_out, d_idx, d_cnt, 0, SCR_CLOUD)
+                        : remove_outlier_run(ctx, ctx->stream, in, 1, dim, radius, min_points, d_out, d_idx, d_cnt, 0);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(n_out, d_cnt, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(out_pts_host, d_out, sizeof(float) * (size_t)n * dim, cudaMemcpyDeviceToHost,
@@ -314,8 +297,8 @@ int sfe_match_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off
                   float *dists_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_match_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return match_run(ctx, ref_pts_dev, ref_off_dev, in_pts_dev, in_off_dev, n_pairs, n_ref_max, max_dist, ids_dev,
-                   dists_dev);
+  return match_run(ctx, ctx->stream, {ref_pts_dev, ref_off_dev, nullptr, n_ref_max},
+                   {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, max_dist, ids_dev, dists_dev);
 }
 
 int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, float max_dist,
@@ -344,7 +327,8 @@ int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *
       SFE_CUDA(cudaMemcpyAsync(d_ref, ref_host, sizeof(float) * 2 * (size_t)n_ref, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_in, in_host, sizeof(float) * 2 * (size_t)n_in, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
-    int rc = match_run(ctx, d_ref, d_off, d_in, d_off + 2, 1, n_ref, max_dist, d_ids, d_d);
+    int rc = match_run(ctx, ctx->stream, {d_ref, d_off, nullptr, n_ref}, {d_in, d_off + 2, nullptr, n_in}, 1, max_dist,
+                       d_ids, d_d);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(ids_host, d_ids, sizeof(int32_t) * (size_t)n_in, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(dists_host, d_d, sizeof(float) * (size_t)n_in, cudaMemcpyDeviceToHost, ctx->stream));
@@ -388,8 +372,9 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
                 int32_t *iters_dev, int32_t *inliers_dev, int32_t *status_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_icp_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return icp_run(ctx, ctx->stream, prm, src_pts_dev, src_off_dev, nullptr, tgt_pts_dev, tgt_off_dev, nullptr, 0, src_id_dev,
-                 tgt_id_dev, n_problems, ns_max, nt_max, guess_dev, T_dev, iters_dev, inliers_dev, status_dev);
+  return icp_run(ctx, ctx->stream, prm,
+                 {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
+                  tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, 0, 0);
 }
 
 int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host, int nt,
@@ -460,8 +445,9 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
     SFE_CUDA(cudaMemcpyAsync(d_ids, src_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_ids + P, tgt_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
-    int rc = icp_run(ctx, ctx->stream, prm, d_src, d_soff, nullptr, d_tgt, d_toff, nullptr, 0, d_ids, d_ids + P, n_problems, ns_max,
-                     nt_max, d_guess, d_T, d_res, d_res + P, d_res + 2 * P);
+    int rc = icp_run(ctx, ctx->stream, prm,
+                     {{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
+                      d_guess, d_T, d_res, d_res + P, d_res + 2 * P}, 0, 0);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));

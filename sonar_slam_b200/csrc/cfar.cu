@@ -37,7 +37,7 @@
 //      arbitrary float32 images.  It is a device path, not a CPU fallback.
 #include <vector>
 
-#include "common.cuh"
+#include "stages.cuh"
 
 namespace sfe {
 
@@ -977,8 +977,10 @@ static int launch_exact(sfe_ctx *ctx, cudaStream_t st, const InT *img, const Cfa
   return SFE_OK;
 }
 
-int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G, int k,
-             double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact) {
+}  // namespace sfe
+
+int sfe::cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
+                  int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits) {
   SFE_REQUIRE(ctx != nullptr, "cfar: null context");
   SFE_REQUIRE(img != nullptr || F == 0, "cfar: null image pointer");
   SFE_REQUIRE(dtype == SFE_U8 || dtype == SFE_F32, "cfar: dtype must be SFE_U8 or SFE_F32 (got %d)", dtype);
@@ -1007,7 +1009,7 @@ int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, i
 
   // the streaming path's preconditions (shape of the register rings; TMA alignment rules; a slope
   // whose two-float split is accurate)
-  bool fast = !force_exact && T == CF_T && G == CF_G && alg != SFE_CFAR_OS && R > 2 * CF_HALF;
+  bool fast = T == CF_T && G == CF_G && alg != SFE_CFAR_OS && R > 2 * CF_HALF;
   fast = fast && ((uintptr_t)img % 16 == 0) && ((size_t)B * es % 16 == 0);
   if (mask != nullptr) fast = fast && ((uintptr_t)mask % 16 == 0) && (B % 16 == 0);
   fast = fast && isfinite(c) && fabs(c) > 1e-20 && fabs(c) < 1e20;
@@ -1079,7 +1081,7 @@ int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, i
     }
     return launch_ring_alg<uint8_t>(ctx, st, in_map, out_map, p);
   }
-  if (dtype == SFE_U8 && alg == SFE_CFAR_OS && !force_exact && T >= 1 && T <= 127 && R > 2 * (T + G) && isfinite(tau)) {
+  if (dtype == SFE_U8 && alg == SFE_CFAR_OS && T >= 1 && T <= 127 && R > 2 * (T + G) && isfinite(tau)) {
     // sliding-histogram OS-CFAR; 256-entry pass table M[v] = smallest cell value with x > tau*v (and the gate)
     std::vector<uint16_t> lut(256);
     int g = 0;
@@ -1102,5 +1104,3 @@ int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, i
   if (dtype == SFE_F32) return launch_exact<float>(ctx, st, (const float *)img, p, nullptr);
   return launch_exact<uint8_t>(ctx, st, (const uint8_t *)img, p, nullptr);
 }
-
-}  // namespace sfe

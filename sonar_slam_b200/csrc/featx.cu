@@ -22,7 +22,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "common.cuh"
+#include "stages.cuh"
 
 namespace sfe {
 
@@ -426,27 +426,6 @@ __global__ void __launch_bounds__(FI_THREADS)
   }
 }
 
-int feature_image_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames, int F, const uint8_t *lut_bgr,
-                      uint8_t *out, const char *what) {
-  SFE_REQUIRE(ctx && m, "%s: null context or maps", what);
-  SFE_REQUIRE(ctx->device == m->device, "%s: maps were created on device %d, context is on %d", what, m->device,
-              ctx->device);
-  SFE_REQUIRE(F >= 0, "%s: negative frame count", what);
-  if (F == 0) return SFE_OK;
-  SFE_REQUIRE(frames && lut_bgr && out, "%s: null frames, table or output pointer", what);
-  SFE_REQUIRE((long long)m->R * m->B < (1ll << 31), "%s: a %d x %d polar frame is too large", what, m->R, m->B);
-  const int npix = m->rows * m->cols, n_tiles = (npix + FI_TILE - 1) / FI_TILE;
-  const long long grid = (long long)n_tiles * (((long long)F + FI_FPB - 1) / FI_FPB);
-  SFE_REQUIRE(grid <= 0x7fffffffll, "%s: %d frames of %d x %d are too many for one call", what, F, m->rows, m->cols);
-  FeatureLut lut;
-  memcpy(lut.bgr, lut_bgr, sizeof(lut.bgr));
-  feature_image_kernel<<<(unsigned)grid, FI_THREADS, 0, ctx->stream>>>((const uint2 *)m->table, npix, m->R, m->B,
-                                                                        frames, F, n_tiles, lut, out);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return SFE_OK;
-}
-
 static bool ctx_force_gather(const sfe_ctx *) {
   const char *e = getenv("SFE_CART_DENSE");  // development switch: force the dense kernel
   return e && e[0] == '1';
@@ -469,8 +448,31 @@ static int launch_cart(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const u
   return SFE_OK;
 }
 
-int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
-                    int32_t *ij, float *xy, int32_t *count) {
+}  // namespace sfe
+
+int sfe::feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *frames, int F,
+                           const uint8_t *lut_bgr, uint8_t *out, const char *what) {
+  SFE_REQUIRE(ctx && m, "%s: null context or maps", what);
+  SFE_REQUIRE(ctx->device == m->device, "%s: maps were created on device %d, context is on %d", what, m->device,
+              ctx->device);
+  SFE_REQUIRE(F >= 0, "%s: negative frame count", what);
+  if (F == 0) return SFE_OK;
+  SFE_REQUIRE(frames && lut_bgr && out, "%s: null frames, table or output pointer", what);
+  SFE_REQUIRE((long long)m->R * m->B < (1ll << 31), "%s: a %d x %d polar frame is too large", what, m->R, m->B);
+  const int npix = m->rows * m->cols, n_tiles = (npix + FI_TILE - 1) / FI_TILE;
+  const long long grid = (long long)n_tiles * (((long long)F + FI_FPB - 1) / FI_FPB);
+  SFE_REQUIRE(grid <= 0x7fffffffll, "%s: %d frames of %d x %d are too many for one call", what, F, m->rows, m->cols);
+  FeatureLut lut;
+  memcpy(lut.bgr, lut_bgr, sizeof(lut.bgr));
+  feature_image_kernel<<<(unsigned)grid, FI_THREADS, 0, st>>>((const uint2 *)m->table, npix, m->R, m->B, frames, F,
+                                                               n_tiles, lut, out);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return SFE_OK;
+}
+
+int sfe::cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits,
+                         int F, int cap, int32_t *ij, float *xy, int32_t *count) {
   SFE_REQUIRE(ctx && m, "cart_points: null context or maps");
   SFE_REQUIRE(ctx->device == m->device, "cart_points: maps were created on device %d, context is on %d", m->device,
               ctx->device);
@@ -508,6 +510,8 @@ int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint
     set_error("cart_points: a %d x %d polar bit plane does not fit in shared memory", m->R, m->B);
   return rc;
 }
+
+namespace sfe {
 
 // ---------------------------------------------------------------------------- host side: per-geometry tables
 // cv2.remap's fixed-point sampling position of every Cartesian pixel (see cart_pixel_fires)
@@ -717,7 +721,8 @@ int sfe_feature_image_dev(sfe_ctx *ctx, const sfe_maps *maps, const uint8_t *fra
                           const uint8_t *lut_bgr_host, uint8_t *out_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_feature_image_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return feature_image_run(ctx, maps, frames_dev, n_frames, lut_bgr_host, out_dev, "sfe_feature_image_dev");
+  return feature_image_run(ctx, ctx->stream, maps, frames_dev, n_frames, lut_bgr_host, out_dev,
+                           "sfe_feature_image_dev");
 }
 
 // Chunks of FI_HOST_CHUNK frames: the copies in and out run on the context's copy stream, in the order
@@ -757,7 +762,7 @@ static int feature_image_host(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *fr
     if (k + 1 < n_chunks && (rc = copy_in(k + 1)) != SFE_OK) return rc;
     // the copy-out of chunk k-2 (enqueued on the copy stream before in_done[k]) has drained this output buffer
     SFE_CUDA(cudaStreamWaitEvent(ctx->stream, in_done[k & 1], 0));
-    rc = feature_image_run(ctx, m, (const uint8_t *)ctx->stage_in[k & 1].ptr, nf, lut_bgr,
+    rc = feature_image_run(ctx, ctx->stream, m, (const uint8_t *)ctx->stage_in[k & 1].ptr, nf, lut_bgr,
                            (uint8_t *)ctx->stage_out[k & 1].ptr, what);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaEventRecord(kernel_done[k & 1], ctx->stream));

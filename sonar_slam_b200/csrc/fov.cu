@@ -33,13 +33,13 @@ __global__ void __launch_bounds__(256)
   sel[i] = keep ? 1 : 0;
 }
 
-int fov_select_run(sfe_ctx *ctx, const float *pts, int n, const float *invT, const double *rb, const double *bb, int K,
-                   uint8_t *sel) {
+static int fov_select_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, int n, const float *invT, const double *rb,
+                          const double *bb, int K, uint8_t *sel) {
   SFE_REQUIRE(ctx, "fov_select: null context");
   SFE_REQUIRE(n >= 0 && K >= 0, "fov_select: negative sizes");
   if (n == 0) return SFE_OK;
   SFE_REQUIRE(pts && sel && (K == 0 || (invT && rb && bb)), "fov_select: null pointer");
-  fov_select_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(pts, n, invT, rb, bb, K, sel);
+  fov_select_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, invT, rb, bb, K, sel);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
@@ -55,7 +55,7 @@ int sfe_fov_select_dev(sfe_ctx *ctx, const float *pts_dev, int n, const float *i
                        const double *bearing_bound_dev, int n_frames, uint8_t *sel_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_fov_select_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return fov_select_run(ctx, pts_dev, n, inv_T_dev, range_bound_dev, bearing_bound_dev, n_frames, sel_dev);
+  return fov_select_run(ctx, ctx->stream, pts_dev, n, inv_T_dev, range_bound_dev, bearing_bound_dev, n_frames, sel_dev);
 }
 
 int sfe_fov_select_host(sfe_ctx *ctx, const float *pts_host, int n, const float *inv_T_host, const double *range_bound_host,
@@ -80,7 +80,8 @@ int sfe_fov_select_host(sfe_ctx *ctx, const float *pts_host, int n, const float 
     SFE_CUDA(cudaMemcpyAsync(bb, bearing_bound_host, sizeof(double) * n_frames, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(invT, inv_T_host, sizeof(float) * 6 * n_frames, cudaMemcpyHostToDevice, ctx->stream));
   }
-  rc = fov_select_run(ctx, (const float *)ctx->stage_in[0].ptr, n, invT, rb, bb, n_frames, (uint8_t *)ctx->stage_out[0].ptr);
+  rc = fov_select_run(ctx, ctx->stream, (const float *)ctx->stage_in[0].ptr, n, invT, rb, bb, n_frames,
+                      (uint8_t *)ctx->stage_out[0].ptr);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(sel_host, ctx->stage_out[0].ptr, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaStreamSynchronize(ctx->stream));

@@ -108,15 +108,14 @@ __global__ void __launch_bounds__(GI_THREADS) costmap_score_kernel(const sfe_cos
   if (tid < CPB && blockIdx.x * CPB + tid < n_cand) cost[blockIdx.x * CPB + tid] = -acc[tid];
 }
 
-int score_launch(sfe_ctx *ctx, const sfe_costmap *cm, const float *src, int n_src, const float *tf, int K,
-                 int32_t *cost) {
+int score_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_costmap *cm, const float *src, int n_src, const float *tf,
+                 int K, int32_t *cost) {
   // few candidates: spread each over more warps so that the launch still fills the machine
   const int sm = ctx->sm_count;
   int W = 1;
   while (W < 8 && (long long)K * W < 8LL * 4 * sm) W *= 2;
-#define SFE_GI(W_)                                                                                         \
-  costmap_score_kernel<W_><<<(K + (8 / W_) - 1) / (8 / W_), GI_THREADS, 0, ctx->stream>>>(*cm, src, n_src, tf, K, \
-                                                                                          cost)
+#define SFE_GI(W_) \
+  costmap_score_kernel<W_><<<(K + (8 / W_) - 1) / (8 / W_), GI_THREADS, 0, st>>>(*cm, src, n_src, tf, K, cost)
   if (W == 1) SFE_GI(1); else if (W == 2) SFE_GI(2); else if (W == 4) SFE_GI(4); else SFE_GI(8);
 #undef SFE_GI
   ctx->launches++;
@@ -230,7 +229,7 @@ int sfe_costmap_score_dev(sfe_ctx *ctx, const sfe_costmap *cm, const float *sour
   if (n_candidates == 0) return SFE_OK;
   SFE_REQUIRE((source_xy_dev || n_source == 0) && transforms_dev && cost_dev, "sfe_costmap_score_dev: null pointer");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return score_launch(ctx, cm, source_xy_dev, n_source, transforms_dev, n_candidates, cost_dev);
+  return score_launch(ctx, ctx->stream, cm, source_xy_dev, n_source, transforms_dev, n_candidates, cost_dev);
 }
 
 int sfe_costmap_score_host(sfe_ctx *ctx, const sfe_costmap *cm_c, const float *transforms_host, int n_candidates,
@@ -250,7 +249,7 @@ int sfe_costmap_score_host(sfe_ctx *ctx, const sfe_costmap *cm_c, const float *t
     float *h_tf = (float *)ctx->pinned;
     int32_t *h_cost = (int32_t *)((char *)ctx->pinned + tf_bytes);
     memcpy(h_tf, transforms_host, sizeof(float) * 6 * (size_t)n_candidates);
-    rc = score_launch(ctx, cm, cm->src, cm->n_src, h_tf, n_candidates, h_cost);
+    rc = score_launch(ctx, ctx->stream, cm, cm->src, cm->n_src, h_tf, n_candidates, h_cost);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaStreamSynchronize(ctx->stream));
     memcpy(cost_host, h_cost, sizeof(int32_t) * (size_t)n_candidates);
@@ -267,7 +266,7 @@ int sfe_costmap_score_host(sfe_ctx *ctx, const sfe_costmap *cm_c, const float *t
   }
   SFE_CUDA(cudaMemcpyAsync(cm->tf, transforms_host, sizeof(float) * 6 * (size_t)n_candidates, cudaMemcpyHostToDevice,
                            ctx->stream));
-  int rc = score_launch(ctx, cm, cm->src, cm->n_src, cm->tf, n_candidates, cm->cost);
+  int rc = score_launch(ctx, ctx->stream, cm, cm->src, cm->n_src, cm->tf, n_candidates, cm->cost);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(cost_host, cm->cost, sizeof(int32_t) * (size_t)n_candidates, cudaMemcpyDeviceToHost,
                            ctx->stream));

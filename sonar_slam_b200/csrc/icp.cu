@@ -17,9 +17,11 @@
 //   order: deterministic)  ->  closed-form 2-D rotation and translation, T_iter update and the
 //   Counter / Differential checkers on one thread.
 // CTAs are persistent over the problem list (batch of keyframe pairs / of initial guesses).
+#include <algorithm>
 #include <mutex>
 
 #include "grid.cuh"
+#include "stages.cuh"
 
 namespace sfe {
 
@@ -1258,32 +1260,9 @@ static int pick_max_cells(int nt_max) {
   return c;
 }
 
-int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off, const int *src_cnt,
-            const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points, const int *src_id,
-            const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out, int *iters,
-            int *inliers, int *status, const int *raw_cnt, int raw_cap, int class_mode, int class_ns, int class_nt,
-            int force_threads) {
-  SFE_REQUIRE(ctx && prm, "icp: null context or parameters");
-  SFE_REQUIRE(P >= 0 && ns_max >= 0 && nt_max >= 0, "icp: negative sizes");
-  if (P == 0) return SFE_OK;
-  SFE_REQUIRE(src_pts && src_off && tgt_pts && tgt_off && guess && T_out && iters && inliers && status,
-              "icp: null pointer");
-  SFE_REQUIRE(nt_max <= 65535 && ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d, %d)",
-              ns_max, nt_max);
-  SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
-  SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "icp: unknown error minimizer %d", prm->minimizer);
-  SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
-              "icp: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", prm->normals_knn, GRID_KNN_MAX);
-  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
-              ICP_HIST - 1);
-  IcpBatch b{};
-  b.src_pts = src_pts, b.src_off = src_off, b.tgt_pts = tgt_pts, b.tgt_off = tgt_off;
-  b.src_cnt = src_cnt, b.tgt_cnt = tgt_cnt, b.min_points = min_points;
-  b.raw_cnt = raw_cnt, b.raw_cap = raw_cap;
-  b.class_mode = class_mode, b.class_ns = class_ns, b.class_nt = class_nt;
-  b.src_id = src_id, b.tgt_id = tgt_id, b.guess = guess;
-  b.T_out = T_out, b.iters = iters, b.inliers = inliers, b.status = status;
-  b.P = P, b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
+// One launch over the batch, laid out for problems of up to ns_max x nt_max points; b.class_mode is its size class.
+static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max) {
+  b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
   b.max_cells = pick_max_cells(b.nt_max);
   b.use_order = b.ns_max > 1024;
   b.cell_scale = 1.0f;
@@ -1321,8 +1300,7 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
   }
   // CTA size follows the source size (one NN query per thread and iteration is the sweet spot)
   // (chosen on the config-4 replay for ~360-point sources; not re-measured on H100)
-  const int threads = force_threads > 0 ? force_threads : (b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS));
-  SFE_REQUIRE(threads == 128 || threads == 256 || threads == 512, "icp: CTA size must be 128, 256 or 512 (got %d)", threads);
+  const int threads = b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS);
   // instantiation: (threads, register budget).  512-thread CTAs whose shared memory allows only one per SM get the
   // full 128 registers.
   const int variant = threads == 128 ? 0 : (threads == 256 ? 1 : (smem > 110 * 1024 ? 3 : 2));
@@ -1362,16 +1340,16 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
   icp_phase_per_sm[threads == 128 ? 0 : threads == 256 ? 1 : 2] = per_sm;
 #endif
   int grid = ctx->sm_count * per_sm;
-  if (grid > P) grid = P;
+  if (grid > b.P) grid = b.P;
   int slots = grid;
-  if (per_sm == 1 && P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = P;  // one CTA per problem
+  if (per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
   const size_t orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
   const size_t nrm_bytes = plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0;
   int rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes, st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
   b.nrm_ws = plane ? (float2 *)((char *)ctx->scratch[SCR_ICP].ptr + orig_bytes) : nullptr;
-  if (!b.slot_by_smid && grid < P) {  // persistent CTAs
+  if (!b.slot_by_smid && grid < b.P) {  // persistent CTAs
     b.next = ctx->work + WORK_ICP;
     SFE_CUDA(cudaMemsetAsync(b.next, 0, sizeof(int), st));
   }
@@ -1381,15 +1359,57 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
   return SFE_OK;
 }
 
-int match_run(sfe_ctx *ctx, const float *ref_pts, const int *ref_off, const float *in_pts, const int *in_off, int P,
-              int nt_max, float max_dist, int32_t *ids, float *dists) {
+}  // namespace sfe
+
+// Size classes (IcpBatch::class_mode): a small class (both sizes positive, clamped to the capacities src.n_max x
+// tgt.n_max) that is smaller on either axis gets a first launch laid out for it, whose smaller shared-memory footprint
+// fits more CTAs per SM; a second launch, laid out for the capacities, takes the problems that did not fit.
+// Otherwise one launch takes every problem and reports oversize ones itself (SFE_ICP_TOO_LARGE).
+int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
+                 int small_nt) {
+  const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
+  SFE_REQUIRE(ctx && prm, "icp: null context or parameters");
+  SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp: negative sizes");
+  if (pb.P == 0) return SFE_OK;
+  SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
+                  pb.status,
+              "icp: null pointer");
+  SFE_REQUIRE(nt_max <= 65535 && ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d, %d)",
+              ns_max, nt_max);
+  SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
+  SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "icp: unknown error minimizer %d", prm->minimizer);
+  SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
+              "icp: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", prm->normals_knn, GRID_KNN_MAX);
+  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
+              ICP_HIST - 1);
+  IcpBatch b{};
+  b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
+  b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;
+  b.raw_cnt = pb.raw_cnt, b.raw_cap = pb.raw_cap;
+  b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
+  b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
+  b.P = pb.P;
+  const int ns_small = std::min(small_ns, ns_max), nt_small = std::min(small_nt, nt_max);
+  if (small_ns <= 0 || small_nt <= 0 || (ns_small == ns_max && nt_small == nt_max))
+    return icp_launch(ctx, st, prm, b, ns_max, nt_max);
+  b.class_mode = 1;
+  int rc = icp_launch(ctx, st, prm, b, ns_small, nt_small);
+  if (rc != SFE_OK) return rc;
+  b.class_mode = 2, b.class_ns = ns_small, b.class_nt = nt_small;
+  return icp_launch(ctx, st, prm, b, ns_max, nt_max);
+}
+
+int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P,
+                   float max_dist, int32_t *ids, float *dists) {
+  const int nt_max = ref.n_max;
   SFE_REQUIRE(ctx, "match: null context");
   SFE_REQUIRE(P >= 0 && nt_max >= 0, "match: negative sizes");
   if (P == 0) return SFE_OK;
-  SFE_REQUIRE(ref_pts && ref_off && in_pts && in_off && ids && dists, "match: null pointer");
+  SFE_REQUIRE(ref.pts && ref.off && in.pts && in.off && ids && dists, "match: null pointer");
+  SFE_REQUIRE(!ref.cnt && !in.cnt, "match: per-cloud counts are not supported");
   SFE_REQUIRE(nt_max <= 65535, "match: reference clouds of more than 65535 points are not supported (got %d)", nt_max);
   MatchBatch b{};
-  b.ref_pts = ref_pts, b.ref_off = ref_off, b.in_pts = in_pts, b.in_off = in_off;
+  b.ref_pts = ref.pts, b.ref_off = ref.off, b.in_pts = in.pts, b.in_off = in.off;
   b.P = P, b.nt_max = nt_max > 0 ? nt_max : 1, b.max_cells = pick_max_cells(b.nt_max), b.max_dist = max_dist;
   b.ids = ids, b.dists = dists;
   const size_t smem = sizeof(float2) * (size_t)b.nt_max + sizeof(uint32_t) * (size_t)((b.max_cells + 2) / 2 + 1) + 16;
@@ -1404,16 +1424,14 @@ int match_run(sfe_ctx *ctx, const float *ref_pts, const int *ref_off, const floa
   if (per_sm < 1) per_sm = 1;
   int grid = ctx->sm_count * per_sm;
   if (grid > P) grid = P;
-  int rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t));
+  int rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
-  match_kernel<<<grid, ICP_THREADS, smem, ctx->stream>>>(b);
+  match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
 }
-
-}  // namespace sfe
 
 #ifdef SFE_ICP_PHASE_CLOCKS
 // Development build only (not declared in include/sonarfe.h): out[0..6] cycles per phase, out[7..13] phase counts,

@@ -382,9 +382,10 @@ __global__ void __launch_bounds__(MCD_WARPS * 32, 1)
 
 }  // namespace
 
-int mincovdet_run(sfe_ctx *ctx, const double *samples, const int32_t *n, const int8_t *subsets, int P,
-                  const double *c_support_host, double c_reweight, double chi2_cut, int flags, double *location,
-                  double *covariance, uint32_t *raw_support, uint32_t *support, int32_t *status) {
+static int mincovdet_run(sfe_ctx *ctx, cudaStream_t st, const double *samples, const int32_t *n, const int8_t *subsets,
+                         int P, const double *c_support_host, double c_reweight, double chi2_cut, int flags,
+                         double *location, double *covariance, uint32_t *raw_support, uint32_t *support,
+                         int32_t *status) {
   SFE_REQUIRE(P >= 0, "sfe_mincovdet: negative problem count");
   SFE_REQUIRE((flags & ~SFE_MCD_FLOAT32) == 0, "sfe_mincovdet: unknown flags 0x%x", flags);
   if (P == 0) return SFE_OK;
@@ -395,8 +396,8 @@ int mincovdet_run(sfe_ctx *ctx, const double *samples, const int32_t *n, const i
   k.c_reweight = c_reweight;
   k.chi2_cut = chi2_cut;
   k.f32 = (flags & SFE_MCD_FLOAT32) ? 1 : 0;
-  mincovdet_kernel<<<P, MCD_WARPS * 32, 0, ctx->stream>>>(samples, n, subsets, k, location, covariance, raw_support,
-                                                           support, status);
+  mincovdet_kernel<<<P, MCD_WARPS * 32, 0, st>>>(samples, n, subsets, k, location, covariance, raw_support, support,
+                                                  status);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
@@ -414,8 +415,8 @@ int sfe_mincovdet_dev(sfe_ctx *ctx, const double *samples_dev, const int32_t *n_
                       int32_t *status_dev) {
   SFE_REQUIRE(ctx != nullptr, "sfe_mincovdet_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
-  return mincovdet_run(ctx, samples_dev, n_dev, subsets_dev, n_problems, c_support_host, c_reweight, chi2_cut, flags,
-                       location_dev, covariance_dev, raw_support_dev, support_dev, status_dev);
+  return mincovdet_run(ctx, ctx->stream, samples_dev, n_dev, subsets_dev, n_problems, c_support_host, c_reweight,
+                       chi2_cut, flags, location_dev, covariance_dev, raw_support_dev, support_dev, status_dev);
 }
 
 int sfe_mincovdet_host(sfe_ctx *ctx, const double *samples_host, const int32_t *n_host, const int8_t *subsets_host,
@@ -451,8 +452,8 @@ int sfe_mincovdet_host(sfe_ctx *ctx, const double *samples_host, const int32_t *
   SFE_CUDA(cudaMemcpyAsync(d_x, samples_host, b_x, cudaMemcpyHostToDevice, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(d_n, n_host, b_n, cudaMemcpyHostToDevice, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(d_s, subsets_host, b_s, cudaMemcpyHostToDevice, ctx->stream));
-  rc = mincovdet_run(ctx, d_x, d_n, d_s, n_problems, c_support_host, c_reweight, chi2_cut, flags, d_loc, d_cov, d_raw,
-                     d_sup, d_st);
+  rc = mincovdet_run(ctx, ctx->stream, d_x, d_n, d_s, n_problems, c_support_host, c_reweight, chi2_cut, flags, d_loc,
+                     d_cov, d_raw, d_sup, d_st);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(location_host, d_loc, b_loc, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(covariance_host, d_cov, b_cov, cudaMemcpyDeviceToHost, ctx->stream));

@@ -16,27 +16,11 @@
 #include <algorithm>
 #include <vector>
 
+#include "stages.cuh"
 #include "stream_decode.cuh"
 
 namespace sfe {
-int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
-             int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits, int force_exact);
-int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F,
-                    int cap, int32_t *ij, float *xy, int32_t *count);
-int feature_image_run(sfe_ctx *ctx, const sfe_maps *m, const uint8_t *frames, int F, const uint8_t *lut_bgr,
-                      uint8_t *out, const char *what);
-int downsample_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
-                   int dim, int n_max, float resolution, float *out_pts, int32_t *out_idx, int32_t *out_count,
-                   int n_split = 0, int slot = SCR_CLOUD);
-int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const float *pts, const int *off, const int *cnt, int n_clouds,
-                       int dim, int n_max, double radius, int min_points, float *out_pts, int32_t *out_idx,
-                       int32_t *out_count, int n_split = 0);
-int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const float *src_pts, const int *src_off,
-            const int *src_cnt, const float *tgt_pts, const int *tgt_off, const int *tgt_cnt, int min_points,
-            const int *src_id, const int *tgt_id, int P, int ns_max, int nt_max, const float *guess, float *T_out,
-            int *iters, int *inliers, int *status, const int *raw_cnt = nullptr, int raw_cap = 0, int class_mode = 0,
-            int class_ns = 0, int class_nt = 0, int force_threads = 0);
-// Size class of the first ICP launch (fe_match), from the problem sizes of bench.py's 4096-frame bag
+// Small ICP size class of the front end (icp_run), from the problem sizes of bench.py's 4096-frame bag
 // (tools/icp_sizes.py): sources after the filters mean 359, max 639 points; window submaps after the 0.5 m thinning
 // (the ICP target) mean 406, max 779.  The class takes every frame of that bag: a second launch that holds only a
 // few frames costs a full problem latency at its tail.  The source cap has no margin over the bag's largest source
@@ -44,7 +28,9 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const floa
 // larger cap would only admit problems that take the slower pruned path.  At 640 / 896 points a 128-thread CTA needs 29 KB of shared
 // memory and the 128-thread instantiation is held to 72 registers, so an H100 SM holds 7 problems (6 at the former
 // 640 / 1536 class with 80 registers).
-constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 896, FE_ICP_SMALL_THREADS = 128;
+constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 896;
+// (the class is sized for 128-thread CTAs, which icp_run's CTA-size rule gives sources of up to 640 points)
+static_assert(FE_ICP_SMALL_SRC <= 640, "the small ICP class must stay within icp_run's 128-thread CTAs");
 // Size classes of the cloud filters (cloud.cu: two launches by cloud size).  Config-4 replay: 3-5 k raw Cartesian
 // points per frame, ~580 after the voxel filter, ~400 after the outlier filter, window submaps <= 1.8 k raw points.
 // The outlier filter and the submap down-sampling gain from a small-cloud class; the per-frame down-sampling is best
@@ -357,7 +343,7 @@ static int fe_render_chunk(sfe_frontend *fe, int f0, int n, int k, const char *w
   const size_t fbytes = (size_t)fe->p.R * fe->p.B, ib = (size_t)fe->maps->rows * fe->maps->cols * 3;
   uint8_t *stage = fe->img_stage[k & 1];
   SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_img_copied[k & 1], 0));
-  int rc = feature_image_run(ctx, fe->maps, fe->frames + (size_t)f0 * fbytes, n, fe->img_lut, stage, what);
+  int rc = feature_image_run(ctx, ctx->stream, fe->maps, fe->frames + (size_t)f0 * fbytes, n, fe->img_lut, stage, what);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaEventRecord(fe->ev_img_ready[k & 1], ctx->stream));
   SFE_CUDA(cudaStreamWaitEvent(fe->img_stream, fe->ev_img_ready[k & 1], 0));
@@ -416,7 +402,7 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_
   uint32_t *bits = fe->bits + (size_t)f0 * p.R * wpr;
   fe->timer.tic(st, SFE_FE_CFAR);
   int rc = cfar_run(ctx, st, frames_dev, SFE_U8, n, p.R, p.B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank, p.tau,
-                    p.gate_enable, p.gate_threshold, nullptr, nullptr, bits, 0);
+                    p.gate_enable, p.gate_threshold, nullptr, nullptr, bits);
   fe->timer.toc(st);
   if (rc != SFE_OK) return rc;
   fe->timer.tic(st, SFE_FE_CART);
@@ -433,8 +419,8 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_
       const char *e = getenv("SFE_FE_DS_SPLIT");
       return e ? atoi(e) : FE_DS_SPLIT;
     }();
-    rc = downsample_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.resolution, fe->xy_b, fe->idx,
-                        fe->cnt_b + f0, ds_split);
+    rc = downsample_run(ctx, st, {cur, fe->off_pts + f0, cur_cnt + f0, (int)cap}, n, 2, p.resolution, fe->xy_b, fe->idx,
+                        fe->cnt_b + f0, ds_split, SCR_CLOUD);
     fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
     cur = fe->xy_b, cur_cnt = fe->cnt_b;
@@ -442,7 +428,7 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_
   if (p.outlier_min_points > 1) {
     float *dst = (cur == fe->xy_a) ? fe->xy_b : fe->xy_a;
     fe->timer.tic(st, SFE_FE_OUTLIER);
-    rc = remove_outlier_run(ctx, st, cur, fe->off_pts + f0, cur_cnt + f0, n, 2, (int)cap, p.outlier_radius,
+    rc = remove_outlier_run(ctx, st, {cur, fe->off_pts + f0, cur_cnt + f0, (int)cap}, n, 2, p.outlier_radius,
                             p.outlier_min_points, dst, fe->idx, fe->cnt_c + f0, FE_RO_SPLIT);
     fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
@@ -490,31 +476,21 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const int32_t *tcnt = fe->tcnt_a;
   if (p.submap_resolution > 0.f) {
     // (its own sort workspace: in the overlapped schedule it runs next to the frame down-sampling)
-    int rc = downsample_run(ctx, st, fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, n, 2, tcap, p.submap_resolution,
+    int rc = downsample_run(ctx, st, {fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, tcap}, n, 2, p.submap_resolution,
                             fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_SUBMAP);
     if (rc != SFE_OK) return rc;
     tgt = fe->tgt_b, tcnt = fe->tcnt_b;
   }
   fe->timer.toc(st);
   fe->timer.tic(st, SFE_FE_ICP);
-  // Two launches by problem size: a sonar frame's filtered cloud is a few hundred points, far below the
-  // capacities the buffers are sized for, and the ICP kernel's occupancy is set by its shared-memory footprint.
-  // The first launch is sized for the common case (7 CTAs per SM instead of 4) and leaves bigger problems
-  // untouched; the second, sized for the capacities, only takes those.
-  const int ns_small = p.cap_source < FE_ICP_SMALL_SRC ? p.cap_source : FE_ICP_SMALL_SRC;
-  const int nt_small = p.cap_target < FE_ICP_SMALL_TGT ? p.cap_target : FE_ICP_SMALL_TGT;
-  // class_mode 1 leaves oversize problems untouched for the second launch; when the capacities are not larger than
-  // the small class there is no second launch and this one must report them itself (SFE_ICP_TOO_LARGE)
-  const bool two = ns_small < p.cap_source || nt_small < p.cap_target;
-  int rc = icp_run(ctx, st, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
-                   nullptr, nullptr, n, ns_small, nt_small, fe->guess + 9 * (size_t)f0, fe->T + 9 * (size_t)f0,
-                   fe->iters + f0, fe->inliers + f0, fe->status + f0, fe->cnt_a + f0, cap, two ? 1 : 0, 0, 0,
-                   FE_ICP_SMALL_THREADS);
-  if (rc == SFE_OK && two)
-    rc = icp_run(ctx, st, &p.icp, cloud, fe->off_pts + f0, cnt + f0, tgt, fe->off_tgt + f0, tcnt + f0, p.min_points,
-                 nullptr, nullptr, n, p.cap_source, p.cap_target, fe->guess + 9 * (size_t)f0,
-                 fe->T + 9 * (size_t)f0, fe->iters + f0, fe->inliers + f0, fe->status + f0, fe->cnt_a + f0, cap, 2,
-                 ns_small, nt_small);
+  IcpProblems pb{};
+  pb.src = {cloud, fe->off_pts + f0, cnt + f0, p.cap_source};
+  pb.tgt = {tgt, fe->off_tgt + f0, tcnt + f0, p.cap_target};
+  pb.P = n, pb.min_points = p.min_points;
+  pb.raw_cnt = fe->cnt_a + f0, pb.raw_cap = cap;  // the source's Cartesian points before the filters
+  pb.guess = fe->guess + 9 * (size_t)f0, pb.T_out = fe->T + 9 * (size_t)f0;
+  pb.iters = fe->iters + f0, pb.inliers = fe->inliers + f0, pb.status = fe->status + f0;
+  const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_SMALL_SRC, FE_ICP_SMALL_TGT);
   fe->timer.toc(st);
   return rc;
 }
@@ -718,7 +694,8 @@ int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const doub
   int rc = fe_upload_poses(fe, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   if (fe->img_dst) {
-    rc = feature_image_run(fe->ctx, fe->maps, frames_dev, n_frames, fe->img_lut, fe->img_dst, "sfe_frontend_run_dev");
+    rc = feature_image_run(fe->ctx, fe->ctx->stream, fe->maps, frames_dev, n_frames, fe->img_lut, fe->img_dst,
+                           "sfe_frontend_run_dev");
     if (rc != SFE_OK) return rc;
   }
   // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule

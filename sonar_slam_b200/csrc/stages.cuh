@@ -1,0 +1,51 @@
+// Stage launchers shared by the C entry points and the batched front end (pipeline.cu).  Each one checks its
+// arguments, then enqueues all of its work -- launches, memsets, scratch growth -- on `st` and nowhere else, so a
+// caller may run stages on streams of its own.  Returns an SFE_* code.
+#pragma once
+#include "common.cuh"
+
+namespace sfe {
+
+// A batch of 2-D point clouds packed row-wise: cloud c starts at row off[c] of pts.  Its point count is cnt[c] or,
+// with cnt null, off[c + 1] - off[c].  n_max bounds every count and sizes the launches.
+struct PackedClouds {
+  const float *pts;
+  const int *off;
+  const int *cnt;
+  int n_max;
+};
+
+// P scan-matching problems: problem p moves source src_id[p] onto target tgt_id[p] (null ids: cloud p) from
+// guess[p].  Problems whose source or target has fewer than min_points points are skipped; with raw_cnt, a source
+// whose raw cloud had more than raw_cap points is reported too large.
+struct IcpProblems {
+  PackedClouds src, tgt;
+  const int *src_id, *tgt_id;
+  int P;
+  const float *guess;  // [P][9] row-major 3x3
+  float *T_out;        // [P][9]
+  int *iters, *inliers, *status;
+  int min_points;
+  const int *raw_cnt;
+  int raw_cap;
+};
+
+int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
+             int k, double tau, int gate_on, double gate, uint8_t *mask, float *thr, uint32_t *bits);
+int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F,
+                    int cap, int32_t *ij, float *xy, int32_t *count);
+int feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *frames, int F,
+                      const uint8_t *lut_bgr, uint8_t *out, const char *what);  // what: the caller, for errors
+// n_split > 0: two launches by cloud size (cloud.cu), 0: one launch
+int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
+                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot);
+int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
+                       int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split);
+// problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu), (0, 0): one launch
+int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
+            int small_nt);
+// nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used
+int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
+              int32_t *ids, float *dists);
+
+}  // namespace sfe
