@@ -151,6 +151,12 @@ SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uin
  *                       quadtree on the cloud's bounding square, one medoid per leaf, leaves in
  *                       depth-first order.  The two-argument overload (points + descriptors,
  *                       pcl.cpp:143) is served by gathering descriptors with out_idx.
+ *                       Any cloud size is accepted: clouds that fit one CTA's shared memory
+ *                       (57 084 points on an H100) run one CTA each; larger ones (whole maps)
+ *                       run in the same call on a grid-wide path (radix sort of path keys,
+ *                       medoid sums one thread per member), with the same results.  Its
+ *                       workspace holds 48 bytes for each of n_clouds * n_max slots (at most
+ *                       2^31 - 1).  Trees stop at 15 levels (16 km at a 0.5 m resolution).
  * sfe_remove_outlier_*  bruce_slam.pcl.remove_outlier (pcl.cpp:54-74): PCL RadiusOutlierRemoval:
  *                       keep a point iff at least min_points OTHER points lie within `radius`;
  *                       input order is preserved.

@@ -84,7 +84,8 @@ struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
 };
 
 namespace sfe {
-enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_SUBMAP = 6 };
+enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_SUBMAP = 6,
+       SCR_DS_GRID = 7 };
 // Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
 // different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
 enum { WORK_CART = 0, WORK_ICP = 1, SFE_WORK_COUNTERS = 2 };

@@ -12,6 +12,7 @@ every test / bench input is generated here:
                           reads (feature_extraction.py:142-146,201,217)
   make_walls / make_icp_pair
                           2-D wall scene, (source, target, ground truth) scan pairs
+  make_map_cloud          whole-map cloud: walls re-observed from keyframes along a trajectory
   make_trajectory_frames  frames seen from a moving vehicle (pipeline replay)
 """
 from dataclasses import dataclass
@@ -74,6 +75,30 @@ def sample_walls(rng, walls, n, sigma):
     t = rng.uniform(0.0, 1.0, size=n)
     pts = walls[which, :2] + (walls[which, 2:] - walls[which, :2]) * t[:, None]
     return pts + rng.normal(0.0, sigma, size=pts.shape)
+
+
+def make_map_cloud(n_points, seed=0, points_per_keyframe=360, sensor_range=30.0, sigma=0.05):
+    """Whole-map cloud, what SLAM.get_points concatenates: wall segments re-observed from keyframes along a vehicle
+    trajectory, `points_per_keyframe` wall points within `sensor_range` of every keyframe.  The scene grows with the
+    run (about one 8-40 m wall per 12 000 points, ~250 points per 0.5 m cell on the walls).
+    Returns (points float32 [n_points, 2] in world coordinates, keyframe index int32 [n_points],
+    keyframe poses float64 [n_keyframes, 3] as x, y, theta)."""
+    rng = np.random.default_rng(seed)
+    n_segments = max(8, n_points // 12000)
+    extent = 18.0 * np.sqrt(n_segments)
+    walls = make_walls(rng, n_segments=n_segments, extent=extent)
+    n_kf = -(-n_points // points_per_keyframe)
+    s = np.linspace(0.0, 2 * np.pi, n_kf, endpoint=False)  # a closed loop through the scene, ridden once
+    poses = np.c_[extent * (0.5 + 0.3 * np.cos(s)), extent * (0.5 + 0.3 * np.sin(2 * s)), s]
+    pts, kf = [], []
+    for k in range(n_kf):
+        got = np.zeros((0, 2))
+        while len(got) < points_per_keyframe:
+            c = sample_walls(rng, walls, 8 * points_per_keyframe, sigma)
+            got = np.r_[got, c[np.hypot(c[:, 0] - poses[k, 0], c[:, 1] - poses[k, 1]) < sensor_range]]
+        pts.append(got[:points_per_keyframe])
+        kf.append(np.full(points_per_keyframe, k, np.int32))
+    return np.concatenate(pts)[:n_points].astype(np.float32), np.concatenate(kf)[:n_points], poses
 
 
 def grid_thin(points, cell):
