@@ -369,6 +369,34 @@ SFE_API int sfe_frontend_get_timing(sfe_frontend *fe, double *stage_ms, int64_t 
 SFE_API int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const double *poses_host,
                                   int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
                                   int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host);
+/* Several sonar geometries in one front end: a bag whose range setting changes (num_ranges, range_resolution, beam
+ * count) is fed as one sequence, and the first frames after a change are matched against the keyframes before it, as
+ * the reference's window of metric keyframe clouds does (slam.py:632-633).
+ *
+ * sfe_frontend_add_geometry registers `maps` as a further geometry and returns its id; the creation maps are geometry
+ * 0.  The geometry must fit the frame slots the front end was created with (maps->R <= params.R, maps->B <= params.B);
+ * nothing is reallocated.  The front end keeps `maps` referenced (it does not own it).  At most
+ * SFE_FE_MAX_GEOMETRIES geometries, the creation maps included.
+ *
+ * The *_geometry run flavours take one geometry id per frame (geometry, int32 [n_frames], HOST memory), checked before
+ * any device work; otherwise they are the flavours above, carry and schedule included.  The feature stages (CFAR,
+ * Cartesian points) run once per maximal run of consecutive frames of one geometry; everything after the Cartesian
+ * points runs over the whole batch (or chunk) as before.
+ *   _run_dev_geometry:  frame i of geometry g occupies the first R_g * B_g bytes of its slot, frames_dev + i * R * B,
+ *                       row-major [R_g][B_g].
+ *   _run_host_geometry: frames packed as the compressed flavours pack streams: frame i = bytes[offsets[i] ..
+ *                       offsets[i + 1]), exactly R_g * B_g bytes (offsets int64 [n_frames + 1]).
+ *   _run_jpeg_host_geometry / _run_png_host_geometry: every stream must decode to its own geometry's R_g x B_g.
+ * Feature images (sfe_frontend_set_feature_images) need every frame of a call in one geometry; they then have that
+ * geometry's rows x cols.  A call whose frames have more than one geometry is rejected while images are set. */
+enum { SFE_FE_MAX_GEOMETRIES = 8 };
+SFE_API int sfe_frontend_add_geometry(sfe_frontend *fe, const sfe_maps *maps, int *geometry_id);
+SFE_API int sfe_frontend_run_dev_geometry(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t *geometry,
+                                          const double *poses_host, int n_frames);
+SFE_API int sfe_frontend_run_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                           const int32_t *geometry, const double *poses_host, int n_frames,
+                                           int chunk_frames, float *T_host, int32_t *iters_host,
+                                           int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host);
 
 /* ------------------------------------------------------------------ global-initialisation cost (next row N2)
  * SLAM.get_matching_cost_subroutine1 (slam.py:461-570), the function scipy.shgo minimises in
@@ -524,6 +552,15 @@ SFE_API int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, co
                                       const double *poses_host, int n_frames, int chunk_frames, float *T_host,
                                       int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
                                       int32_t *npoints_host);
+/* The compressed flavours with one geometry id per frame (sfe_frontend_add_geometry). */
+SFE_API int sfe_frontend_run_jpeg_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                                const int32_t *geometry, const double *poses_host, int n_frames,
+                                                int chunk_frames, float *T_host, int32_t *iters_host,
+                                                int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host);
+SFE_API int sfe_frontend_run_png_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                               const int32_t *geometry, const double *poses_host, int n_frames,
+                                               int chunk_frames, float *T_host, int32_t *iters_host,
+                                               int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host);
 
 #ifdef __cplusplus
 }

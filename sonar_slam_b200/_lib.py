@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SFE_LIB_PATH") or os.path.join(_HERE, "libsonarfe.so")  # (override: kernel experiments)
 
 c_int, c_double, c_void_p, c_float = ctypes.c_int, ctypes.c_double, ctypes.c_void_p, ctypes.c_float
+MAX_GEOMETRIES = 8  # SFE_FE_MAX_GEOMETRIES: sonar geometries per front end, the creation maps included
 
 _lib = None
 _lock = threading.Lock()
@@ -135,6 +136,14 @@ _EXTRA_SIGNATURES = {
     "sfe_feature_image_dev": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "sfe_feature_image_host": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "sfe_frontend_set_feature_images": [c_void_p, c_void_p, c_void_p, c_int],
+    "sfe_frontend_add_geometry": [c_void_p, c_void_p, ctypes.POINTER(c_int)],
+    "sfe_frontend_run_dev_geometry": [c_void_p, c_void_p, c_void_p, c_void_p, c_int],
+    "sfe_frontend_run_host_geometry": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_frontend_run_jpeg_host_geometry": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_frontend_run_png_host_geometry": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p],
 }
 
 
@@ -220,7 +229,8 @@ def default_context(device=0):
 
 
 class Maps:
-    """Device-resident polar->Cartesian sampling table for one sonar geometry (sfe_maps)."""
+    """Device-resident polar->Cartesian sampling table for one sonar geometry (sfe_maps); a FrontEnd may hold several
+    (FrontEnd.add_geometry)."""
 
     def __init__(self, ctx, map_x, map_y, R, B, width, height):
         map_x = np.ascontiguousarray(map_x, np.float32)

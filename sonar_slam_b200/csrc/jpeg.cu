@@ -957,7 +957,7 @@ static void plan_chunk(const StreamBatch<JHeader> &bt, int f0, int nf, ChunkPlan
       const int sd = use_table(0, h.td[c]), sa = use_table(1, h.ta[c]);
       for (int j = 0; j < nb; ++j, ++b) d.bcomp[b] = (int8_t)c, d.bdc[b] = (int8_t)sd, d.bac[b] = (int8_t)sa;
     }
-    if (h.H != bt.R || h.W != bt.B) {
+    if (h.H != bt.R_of(f0 + i) || h.W != bt.B_of(f0 + i)) {
       d.status = SFE_JPEG_SIZE;
       continue;
     }
@@ -991,8 +991,8 @@ struct JpegState final : StreamDecoder {
       if (b->ptr) cudaFree(b->ptr);
   }
   int chunk_frames(const sfe_ctx *) const override { return cap_blocks > 0 ? 16 : JPEG_CHUNK; }
-  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B) override {
-    bt.parse(bytes, offsets, n, R, B, parse_header, SFE_JPEG_SIZE);
+  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, const int32_t *shape) override {
+    bt.parse(bytes, offsets, n, R, B, shape, parse_header, SFE_JPEG_SIZE);
   }
   int frame_status(int i) const override { return bt.hdr[i].status; }
   const char *message(int status) const override { return sfe_jpeg_status_message(status); }
@@ -1044,7 +1044,8 @@ int JpegState::decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) {
   uint8_t *s = static_cast<uint8_t *>(scr.ptr);
   int16_t *c = static_cast<int16_t *>(coef.ptr);
   int32_t *st = static_cast<int32_t *>(status.ptr) + f0;
-  const int64_t fstride = (int64_t)bt.R * bt.B;
+  const int R = bt.R_of(f0), B = bt.B_of(f0);
+  const int64_t fstride = (int64_t)R * B;
   timer.tic(ctx->stream, SFE_JPEG_T_UNSTUFF);
   jpeg_unstuff_kernel<<<nf, JT, 0, ctx->stream>>>(desc, dev + p.off_bytes, s, st);
   timer.toc(ctx->stream);
@@ -1056,7 +1057,7 @@ int JpegState::decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) {
   timer.tic(ctx->stream, SFE_JPEG_T_PIXELS);
   jpeg_idct_kernel<<<dim3((maxblk + 15) / 16, nf), 128, 0, ctx->stream>>>(desc, quant, s, c, st, out_dev, fstride);
   const int per = (int)std::min<int64_t>((fstride + 1023) / 1024, 64);
-  jpeg_color_kernel<<<dim3(per, nf), 256, 0, ctx->stream>>>(desc, s, st, out_dev, fstride, bt.R, bt.B);
+  jpeg_color_kernel<<<dim3(per, nf), 256, 0, ctx->stream>>>(desc, s, st, out_dev, fstride, R, B);
   timer.toc(ctx->stream);
   ctx->launches += 4;
   int32_t *coef_dev = static_cast<int32_t *>(ctx->stage_out[0].ptr);

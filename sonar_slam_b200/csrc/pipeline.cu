@@ -14,6 +14,7 @@
 // array, so all stages run without packing or host round trips; the host flavour overlaps the
 // host->device copy of frame chunk k+1 with the kernels of chunk k on two streams.
 #include <algorithm>
+#include <functional>
 #include <vector>
 
 #include "stages.cuh"
@@ -110,6 +111,16 @@ __global__ void __launch_bounds__(256)
   if (threadIdx.x == 0) tgt_count[i] = base;
 }
 
+// A maximal run of consecutive frames of one geometry within a call: frames [f0, f0 + n) of geometry g.  Its polar
+// frames lie at `frames`, packed at the geometry's natural stride R_g * B_g, and its bit planes likewise from the
+// bit-plane slot of frame f0 on, so a run never needs more than its own n slots and the CFAR and Cartesian-point
+// launchers serve it as they serve a batch of the creation geometry.  A call without per-frame geometry is one run of
+// geometry 0, whose natural stride is the slot's.
+struct GeoRun {
+  int f0, n, g;
+  const uint8_t *frames;
+};
+
 }  // namespace sfe
 
 using namespace sfe;
@@ -119,6 +130,12 @@ struct sfe_frontend {
   const sfe_maps *maps = nullptr;
   sfe_frontend_params p = {};
   int max_frames = 0;
+  // geometries (sfe_frontend_add_geometry; geo[0] = maps), the runs of the current call, and for the compressed
+  // flavours each frame's expected R x B
+  const sfe_maps *geo[SFE_FE_MAX_GEOMETRIES] = {};
+  int n_geo = 1;
+  std::vector<GeoRun> runs;
+  std::vector<int32_t> frame_shape;
   // device buffers (sized for max_frames)
   uint8_t *frames = nullptr;      // [max_frames][R][B]      (host flavour only)
   uint32_t *bits = nullptr;       // [max_frames][R][wpr]
@@ -151,8 +168,8 @@ struct sfe_frontend {
   uint8_t img_lut[256 * 3] = {};
   uint8_t *img_dst = nullptr;      // null: off
   int img_dst_host = 0;
-  uint8_t *img_stage[2] = {};      // host flavours: [img_stage_frames][rows][cols][3] each
-  int img_stage_frames = 0;
+  uint8_t *img_stage[2] = {};      // host flavours: a chunk's images [frames][rows][cols][3] each
+  size_t img_stage_bytes = 0;
   cudaStream_t img_stream = nullptr;  // copies the images out, next to the frame copies of copy_stream
   cudaEvent_t ev_img_ready[2] = {}, ev_img_copied[2] = {};
   StageTimer timer;  // optional per-stage timing, on ctx->stream (the serial schedule)
@@ -218,6 +235,7 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
   SFE_CUDA(cudaSetDevice(ctx->device));
   sfe_frontend *fe = new sfe_frontend();
   fe->ctx = ctx, fe->maps = maps, fe->p = *params, fe->max_frames = max_frames;
+  fe->geo[0] = maps;
   const size_t F = max_frames, cap = params->cap_points, tcap = (size_t)params->window * cap;
   const size_t wpr = (params->B + 31) / 32;
   FE_ALLOC(fe->frames, F * params->R * params->B);
@@ -308,16 +326,16 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   delete fe;
 }
 
-// Feature images of the host flavours.  fe_images_begin checks the destination and sizes the staging buffers;
-// fe_render_chunk renders frames [f0, f0 + n) of fe->frames (on the device by now) into staging buffer k & 1 and copies
-// them out on img_stream; the render of chunk k waits for the copy-out of chunk k - 2, which used the same buffer.
-static int fe_images_begin(sfe_frontend *fe, int n_frames, int chunk_frames, const char *what) {
+// Feature images of the host flavours, of geometry m (a call with images has one).  fe_images_begin checks the
+// destination and sizes the staging buffers; fe_render_chunk renders frames [f0, f0 + n) (on the device by now, at
+// `frames`) into staging buffer k & 1 and copies them out on img_stream; the render of chunk k waits for the copy-out of
+// chunk k - 2, which used the same buffer.
+static int fe_images_begin(sfe_frontend *fe, const sfe_maps *m, int n_frames, int chunk_frames, const char *what) {
   if (!fe->img_dst) return SFE_OK;
   SFE_REQUIRE(fe->img_dst_host, "%s: feature images are set to go to device memory; this flavour writes them to host "
               "memory (sfe_frontend_set_feature_images with dst_is_host != 0)", what);
-  const int want = std::min(chunk_frames, n_frames);
-  if (fe->img_stage_frames >= want) return SFE_OK;
-  const size_t ib = (size_t)fe->maps->rows * fe->maps->cols * 3;
+  const size_t ib = (size_t)m->rows * m->cols * 3, want = (size_t)std::min(chunk_frames, n_frames) * ib;
+  if (fe->img_stage_bytes >= want) return SFE_OK;
   if (!fe->img_stream) {
     SFE_CUDA(cudaStreamCreateWithFlags(&fe->img_stream, cudaStreamNonBlocking));
     for (int k = 0; k < 2; ++k) {
@@ -327,23 +345,24 @@ static int fe_images_begin(sfe_frontend *fe, int n_frames, int chunk_frames, con
   }
   SFE_CUDA(cudaStreamSynchronize(fe->ctx->stream));
   SFE_CUDA(cudaStreamSynchronize(fe->img_stream));
-  fe->img_stage_frames = 0;
+  fe->img_stage_bytes = 0;
   for (int k = 0; k < 2; ++k) {
     if (fe->img_stage[k]) SFE_CUDA(cudaFree(fe->img_stage[k]));
     fe->img_stage[k] = nullptr;
   }
-  for (int k = 0; k < 2; ++k) SFE_CUDA(cudaMalloc((void **)&fe->img_stage[k], (size_t)want * ib));
-  fe->img_stage_frames = want;
+  for (int k = 0; k < 2; ++k) SFE_CUDA(cudaMalloc((void **)&fe->img_stage[k], want));
+  fe->img_stage_bytes = want;
   return SFE_OK;
 }
 
-static int fe_render_chunk(sfe_frontend *fe, int f0, int n, int k, const char *what) {
+static int fe_render_chunk(sfe_frontend *fe, const sfe_maps *m, const uint8_t *frames, int f0, int n, int k,
+                           const char *what) {
   if (!fe->img_dst) return SFE_OK;
   sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B, ib = (size_t)fe->maps->rows * fe->maps->cols * 3;
+  const size_t ib = (size_t)m->rows * m->cols * 3;
   uint8_t *stage = fe->img_stage[k & 1];
   SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_img_copied[k & 1], 0));
-  int rc = feature_image_run(ctx, ctx->stream, fe->maps, fe->frames + (size_t)f0 * fbytes, n, fe->img_lut, stage, what);
+  int rc = feature_image_run(ctx, ctx->stream, m, frames, n, fe->img_lut, stage, what);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaEventRecord(fe->ev_img_ready[k & 1], ctx->stream));
   SFE_CUDA(cudaStreamWaitEvent(fe->img_stream, fe->ev_img_ready[k & 1], 0));
@@ -391,24 +410,78 @@ static int fe_upload_poses(sfe_frontend *fe, const double *poses, int n) {
   return SFE_OK;
 }
 
+// The runs of a call's frames (geometry: one id per frame, or null: every frame geometry 0), after checking every id;
+// each run's `frames` is set by the caller.  Nothing touches the device.
+static int fe_geometry_runs(sfe_frontend *fe, const int32_t *geometry, int n, const char *what) {
+  fe->runs.clear();
+  for (int i = 0; i < n; ++i) {
+    const int g = geometry ? geometry[i] : 0;
+    SFE_REQUIRE(g >= 0 && g < fe->n_geo, "%s: frame %d has geometry id %d; this front end has geometries 0 .. %d "
+                "(sfe_frontend_add_geometry)", what, i, g, fe->n_geo - 1);
+    if (!fe->runs.empty() && fe->runs.back().g == g)
+      fe->runs.back().n++;
+    else
+      fe->runs.push_back({i, 1, g, nullptr});
+  }
+  SFE_REQUIRE(!fe->img_dst || fe->runs.size() <= 1, "%s: feature images are set, but the frames of this call have "
+              "more than one geometry (%d runs), whose images differ in size; run each geometry's frames in calls of "
+              "their own or turn the images off", what, (int)fe->runs.size());
+  return SFE_OK;
+}
+
+static size_t fe_geo_bytes(const sfe_frontend *fe, int g) { return (size_t)fe->geo[g]->R * fe->geo[g]->B; }
+
+// polar frame i of run r
+static const uint8_t *fe_run_frame(const sfe_frontend *fe, const GeoRun &r, int i) {
+  return r.frames + (size_t)(i - r.f0) * fe_geo_bytes(fe, r.g);
+}
+
+// the place of frame i of run r in the front end's frame buffer (where the host flavours copy or decode it)
+static uint8_t *fe_slot_frame(const sfe_frontend *fe, const GeoRun &r, int i) {
+  return fe->frames + (size_t)r.f0 * fe->p.R * fe->p.B + (size_t)(i - r.f0) * fe_geo_bytes(fe, r.g);
+}
+
+// fn(run, a, m) for the frames [a, a + m) of every run inside frames [f0, f0 + n), in frame order
+static int fe_for_pieces(const sfe_frontend *fe, int f0, int n,
+                         const std::function<int(const GeoRun &, int, int)> &fn) {
+  auto r = std::partition_point(fe->runs.begin(), fe->runs.end(), [&](const GeoRun &q) { return q.f0 + q.n <= f0; });
+  for (; r != fe->runs.end() && r->f0 < f0 + n; ++r) {
+    const int a = std::max(r->f0, f0), b = std::min(r->f0 + r->n, f0 + n);
+    const int rc = fn(*r, a, b - a);
+    if (rc != SFE_OK) return rc;
+  }
+  return SFE_OK;
+}
+
 static const float *fe_cloud(const sfe_frontend *fe, const int32_t **cnt);
 
-// stages 1-3 on frames [f0, f0+n): CFAR (bit plane) -> Cartesian points -> downsample -> outlier removal.
-// Final per-frame clouds end in xy_a / cnt_c (or wherever the last enabled filter wrote; see cloud()).
-static int fe_features(sfe_frontend *fe, cudaStream_t st, const uint8_t *frames_dev, int f0, int n) {
+// stages 1-2 on frames [f0, f0+n) of run r: CFAR (bit plane) -> Cartesian points, with the run's geometry
+static int fe_polar(sfe_frontend *fe, cudaStream_t st, const GeoRun &r, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
   const sfe_frontend_params &p = fe->p;
-  const size_t cap = p.cap_points, wpr = (p.B + 31) / 32;
-  uint32_t *bits = fe->bits + (size_t)f0 * p.R * wpr;
+  const sfe_maps *m = fe->geo[r.g];
+  const size_t cap = p.cap_points, wpr = (m->B + 31) / 32;
+  uint32_t *bits = fe->bits + (size_t)r.f0 * p.R * ((p.B + 31) / 32) + (size_t)(f0 - r.f0) * m->R * wpr;
   fe->timer.tic(st, SFE_FE_CFAR);
-  int rc = cfar_run(ctx, st, frames_dev, SFE_U8, n, p.R, p.B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank, p.tau,
-                    p.gate_enable, p.gate_threshold, nullptr, nullptr, bits);
+  int rc = cfar_run(ctx, st, fe_run_frame(fe, r, f0), SFE_U8, n, m->R, m->B, p.cfar_alg, p.train_hs, p.guard_hs, p.rank,
+                    p.tau, p.gate_enable, p.gate_threshold, nullptr, nullptr, bits);
   fe->timer.toc(st);
   if (rc != SFE_OK) return rc;
   fe->timer.tic(st, SFE_FE_CART);
-  rc = cart_points_run(ctx, st, fe->maps, nullptr, bits, n, (int)cap, fe->ij + (size_t)f0 * cap * 2,
+  rc = cart_points_run(ctx, st, m, nullptr, bits, n, (int)cap, fe->ij + (size_t)f0 * cap * 2,
                        fe->xy_a + (size_t)f0 * cap * 2, fe->cnt_a + f0);
   fe->timer.toc(st);
+  return rc;
+}
+
+// stages 1-3 on frames [f0, f0+n): CFAR (bit plane) -> Cartesian points once per run of one geometry, then
+// downsample -> outlier removal over all n frames.
+// Final per-frame clouds end in xy_a / cnt_c (or wherever the last enabled filter wrote; see cloud()).
+static int fe_features(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
+  sfe_ctx *ctx = fe->ctx;
+  const sfe_frontend_params &p = fe->p;
+  const size_t cap = p.cap_points;
+  int rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) { return fe_polar(fe, st, r, a, m); });
   if (rc != SFE_OK) return rc;
   // feature_extraction.py:241-249
   const float *cur = fe->xy_a;
@@ -532,6 +605,20 @@ int sfe_frontend_set_carry(sfe_frontend *fe, int enable) {
   return SFE_OK;
 }
 
+int sfe_frontend_add_geometry(sfe_frontend *fe, const sfe_maps *maps, int *geometry_id) {
+  SFE_REQUIRE(fe && maps && geometry_id, "sfe_frontend_add_geometry: null argument");
+  SFE_REQUIRE(fe->n_geo < SFE_FE_MAX_GEOMETRIES, "sfe_frontend_add_geometry: the front end already has %d geometries, "
+              "the most it takes (SFE_FE_MAX_GEOMETRIES)", fe->n_geo);
+  SFE_REQUIRE(maps->R <= fe->p.R && maps->B <= fe->p.B, "sfe_frontend_add_geometry: polar shape %dx%d does not fit "
+              "the front end's %dx%d frame slots (create it with the largest R and B the geometries need)", maps->R,
+              maps->B, fe->p.R, fe->p.B);
+  SFE_REQUIRE(maps->device == fe->ctx->device, "sfe_frontend_add_geometry: the maps live on device %d, the front end "
+              "on device %d", maps->device, fe->ctx->device);
+  fe->geo[fe->n_geo] = maps;
+  *geometry_id = fe->n_geo++;
+  return SFE_OK;
+}
+
 int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_host, uint8_t *dst, int dst_is_host) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_feature_images: null handle");
   SFE_REQUIRE(dst == nullptr || lut_bgr_host != nullptr, "sfe_frontend_set_feature_images: null colour table");
@@ -574,16 +661,16 @@ static int fe_order(cudaStream_t before, cudaEvent_t ev, cudaStream_t after) {
 // sub-batch k are done -- its window reaches back only into sub-batches <= k.  So the HBM-bound CFAR of sub-batch k+1
 // runs next to the latency-bound ICP of sub-batch k, and each stage's tail is filled by the other side's CTAs.  Both
 // streams fork from ctx->stream (after the pose upload and anything the caller enqueued there) and join back into it,
-// so ctx->stream orders later work -- the next call included -- after the whole batch.
-static int fe_run_overlapped(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
+// so ctx->stream orders later work -- the next call included -- after the whole batch.  With several geometries a
+// sub-batch runs CFAR and the Cartesian points once per run inside it, the rest once.
+static int fe_run_overlapped(sfe_frontend *fe, const double *poses_host, int n_frames) {
   sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
   const int S = fe->overlap;
   int rc = fe_order(ctx->stream, fe->ev_fork, fe->feat_stream);
   if (rc == SFE_OK) rc = fe_order(ctx->stream, fe->ev_fork, fe->match_stream);
   for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += S) {
     const int n = std::min(S, n_frames - f0);
-    rc = fe_features(fe, fe->feat_stream, frames_dev + (size_t)f0 * fbytes, f0, n);
+    rc = fe_features(fe, fe->feat_stream, f0, n);
     if (rc == SFE_OK) rc = fe_order(fe->feat_stream, fe->ev_feat, fe->match_stream);
     if (rc == SFE_OK) rc = fe_match(fe, fe->match_stream, f0, n);
   }
@@ -594,12 +681,20 @@ static int fe_run_overlapped(sfe_frontend *fe, const uint8_t *frames_dev, const 
   return rc != SFE_OK ? rc : (rj != SFE_OK ? rj : rm);
 }
 
-// The start of a host flavour after its argument checks, for n_frames > 0: the device, the default chunk size and the
-// feature-image staging.
+// The start of a host flavour after its argument checks, for n_frames > 0: the device, the default chunk size, the
+// feature-image staging (of the call's one geometry) and every run's place in fe->frames.
 static int fe_host_begin(sfe_frontend *fe, int n_frames, int &chunk_frames, const char *what) {
   SFE_CUDA(cudaSetDevice(fe->ctx->device));
   if (chunk_frames <= 0) chunk_frames = 256;
-  return fe_images_begin(fe, n_frames, chunk_frames, what);
+  for (GeoRun &r : fe->runs) r.frames = fe->frames + (size_t)r.f0 * fe->p.R * fe->p.B;
+  return fe_images_begin(fe, fe->geo[fe->runs[0].g], n_frames, chunk_frames, what);
+}
+
+// feature images of chunk [f0, f0 + n) of a host flavour (the call has one run when images are on)
+static int fe_render_host_chunk(sfe_frontend *fe, int f0, int n, int k, const char *what) {
+  if (!fe->img_dst) return SFE_OK;
+  const GeoRun &r = fe->runs[0];
+  return fe_render_chunk(fe, fe->geo[r.g], fe_run_frame(fe, r, f0), f0, n, k, what);
 }
 
 // The end of a host flavour: the carried window moves on, the results go to the host and the call waits for them.
@@ -624,28 +719,42 @@ static int fe_host_finish(sfe_frontend *fe, const double *poses_host, int n_fram
 // The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
 // fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
 // so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
+// geometry: one id per frame, or null (every frame geometry 0, R x B).
 static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sfe_ctx *), const uint8_t *bytes,
-                                  const int64_t *offsets, const double *poses_host, int n_frames, int chunk_frames,
-                                  float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
-                                  int32_t *npoints_host, const char *what) {
+                                  const int64_t *offsets, const int32_t *geometry, const double *poses_host,
+                                  int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
+                                  int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host,
+                                  const char *what) {
   SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
               "%s: null argument", what);
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
               fe->max_frames);
   SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
-  if (n_frames == 0) return SFE_OK;
-  int rc = fe_host_begin(fe, n_frames, chunk_frames, what);
+  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  if (rc != SFE_OK || n_frames == 0) return rc;
+  const int32_t *shape = nullptr;  // each frame's R x B, checked by the decoder
+  if (geometry) {
+    fe->frame_shape.resize(2 * (size_t)n_frames);
+    for (int i = 0; i < n_frames; ++i)
+      fe->frame_shape[2 * i] = fe->geo[geometry[i]]->R, fe->frame_shape[2 * i + 1] = fe->geo[geometry[i]]->B;
+    shape = fe->frame_shape.data();
+  }
+  rc = fe_host_begin(fe, n_frames, chunk_frames, what);
   if (rc != SFE_OK) return rc;
   ImagesDrained drained{fe};
   sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
   StreamDecoder *dec = decoder(ctx);
-  dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B);
+  dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, shape);
+  auto reject = [&](int i, int status) {
+    if (geometry)
+      set_error("%s: frame %d (geometry %d, %d x %d): %s", what, i, geometry[i], shape[2 * i], shape[2 * i + 1],
+                dec->message(status));
+    else
+      set_error("%s: frame %d: %s", what, i, dec->message(status));
+    return SFE_ERR_ARG;
+  };
   for (int i = 0; i < n_frames; ++i)
-    if (dec->frame_status(i) != 0) {
-      set_error("%s: frame %d: %s", what, i, dec->message(dec->frame_status(i)));
-      return SFE_ERR_ARG;
-    }
+    if (dec->frame_status(i) != 0) return reject(i, dec->frame_status(i));
   rc = dec->reserve(ctx, chunk_frames, 0);
   if (rc == SFE_OK) rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
   if (rc == SFE_OK) rc = fe_upload_poses(fe, poses_host, n_frames);
@@ -654,7 +763,11 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
   const int32_t *st_dev = static_cast<const int32_t *>(dec->status.ptr);
   auto decode = [&](int f0, int k) -> int {
     const int n = std::min(chunk_frames, n_frames - f0);
-    int r = dec->decode_chunk(ctx, f0, n, fe->frames + (size_t)f0 * fbytes);
+    // a decode_chunk takes frames of one shape: a chunk that crosses a geometry change decodes run by run, each part
+    // into its place in its run (every part is a subset of the chunk, which reserve() sized the decoder for)
+    int r = fe_for_pieces(fe, f0, n, [&](const GeoRun &run, int a, int m) {
+      return dec->decode_chunk(ctx, a, m, fe_slot_frame(fe, run, a));
+    });
     if (r != SFE_OK) return r;
     SFE_CUDA(cudaMemcpyAsync(st_host + f0, st_dev + f0, 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
@@ -670,12 +783,104 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
     for (int i = f0; i < f0 + n; ++i)
       if (st_host[i] != 0) {
         SFE_CUDA(cudaStreamSynchronize(ctx->stream));
-        set_error("%s: frame %d: %s", what, i, dec->message(st_host[i]));
-        return SFE_ERR_ARG;
+        return reject(i, st_host[i]);
       }
-    rc = fe_render_chunk(fe, f0, n, k, what);
-    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
+    rc = fe_render_host_chunk(fe, f0, n, k, what);
+    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, f0, n);
     if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
+  }
+  if (rc != SFE_OK) return rc;
+  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
+}
+
+// sfe_frontend_run_dev[_geometry]; geometry: one id per frame, or null (every frame geometry 0)
+static int fe_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t *geometry, const double *poses_host,
+                      int n_frames, const char *what) {
+  SFE_REQUIRE(fe && frames_dev && poses_host, "%s: null argument", what);
+  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
+              fe->max_frames);
+  SFE_REQUIRE(!fe->img_dst || !fe->img_dst_host, "%s: feature images are set to go to host memory; this flavour "
+              "writes them to device memory (sfe_frontend_set_feature_images with dst_is_host = 0)", what);
+  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  if (rc != SFE_OK || n_frames == 0) return rc;
+  sfe_ctx *ctx = fe->ctx;
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  // a run of a geometry smaller than the slots is packed into fe->frames at its natural stride, one copy per run (a
+  // run of one frame, or of a geometry that fills its slots, is read where it is)
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  for (GeoRun &r : fe->runs) {
+    const size_t gb = fe_geo_bytes(fe, r.g);
+    r.frames = frames_dev + (size_t)r.f0 * fbytes;
+    if (gb == fbytes || r.n == 1) continue;
+    uint8_t *dst = fe_slot_frame(fe, r, r.f0);
+    SFE_CUDA(cudaMemcpy2DAsync(dst, gb, r.frames, fbytes, gb, r.n, cudaMemcpyDeviceToDevice, ctx->stream));
+    r.frames = dst;
+  }
+  if (fe->img_dst) {  // (one run)
+    const GeoRun &r = fe->runs[0];
+    rc = feature_image_run(ctx, ctx->stream, fe->geo[r.g], r.frames, n_frames, fe->img_lut, fe->img_dst, what);
+    if (rc != SFE_OK) return rc;
+  }
+  // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
+  if (fe->overlap > 0 && !fe->timer.on) return fe_run_overlapped(fe, poses_host, n_frames);
+  rc = fe_features(fe, ctx->stream, 0, n_frames);
+  if (rc != SFE_OK) return rc;
+  rc = fe_match(fe, ctx->stream, 0, n_frames);
+  if (rc != SFE_OK) return rc;
+  return fe_update_carry(fe, ctx->stream, poses_host, n_frames);
+}
+
+// sfe_frontend_run_host[_geometry]: frame i at bytes + offsets[i] with its geometry's size (offsets and geometry null:
+// bytes + i * R * B, geometry 0).  Chunks of frames stream in on the copy stream, run by run into their places in
+// fe->frames; the feature stages of chunk k run while chunk k+1 copies.
+static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const int32_t *geometry,
+                           const double *poses_host, int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
+                           int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host, const char *what) {
+  SFE_REQUIRE(fe && bytes && poses_host && T_host && iters_host && inliers_host && status_host && (!geometry || offsets),
+              "%s: null argument", what);
+  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
+              fe->max_frames);
+  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  if (rc != SFE_OK) return rc;
+  if (offsets) {
+    SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
+    for (int i = 0; i < n_frames; ++i) {
+      const sfe_maps *m = fe->geo[geometry[i]];
+      SFE_REQUIRE(offsets[i + 1] - offsets[i] == (int64_t)m->R * m->B, "%s: frame %d has %lld bytes; its geometry %d "
+                  "takes %d x %d = %lld", what, i, (long long)(offsets[i + 1] - offsets[i]), geometry[i], m->R, m->B,
+                  (long long)m->R * m->B);
+    }
+  }
+  if (n_frames == 0) return SFE_OK;
+  rc = fe_host_begin(fe, n_frames, chunk_frames, what);
+  if (rc != SFE_OK) return rc;
+  ImagesDrained drained{fe};
+  rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc != SFE_OK) return rc;
+  sfe_ctx *ctx = fe->ctx;
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  // the copies into fe->frames come after earlier work on ctx->stream that may still read it (the frames
+  // sfe_frontend_run_dev_geometry packs there)
+  rc = fe_order(ctx->stream, fe->ev_done, fe->copy_stream);
+  int k = 0;
+  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
+    const int n = std::min(chunk_frames, n_frames - f0);
+    rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) {
+      const size_t src = offsets ? (size_t)offsets[a] : (size_t)a * fbytes;
+      const size_t len = offsets ? (size_t)(offsets[a + m] - offsets[a]) : (size_t)m * fbytes;
+      SFE_CUDA(cudaMemcpyAsync(fe_slot_frame(fe, r, a), bytes + src, len, cudaMemcpyHostToDevice, fe->copy_stream));
+      return SFE_OK;
+    });
+    if (rc != SFE_OK) return rc;
+    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
+    SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
+    rc = fe_render_host_chunk(fe, f0, n, k, what);
+    if (rc != SFE_OK) return rc;
+    rc = fe_features(fe, ctx->stream, f0, n);
+    if (rc != SFE_OK) return rc;
+    rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
   }
   if (rc != SFE_OK) return rc;
   return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
@@ -684,27 +889,13 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
 extern "C" {
 
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
-  SFE_REQUIRE(fe && frames_dev && poses_host, "sfe_frontend_run_dev: null argument");
-  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_dev: %d frames exceed max_frames %d",
-              n_frames, fe->max_frames);
-  SFE_REQUIRE(!fe->img_dst || !fe->img_dst_host, "sfe_frontend_run_dev: feature images are set to go to host memory; "
-              "this flavour writes them to device memory (sfe_frontend_set_feature_images with dst_is_host = 0)");
-  if (n_frames == 0) return SFE_OK;
-  SFE_CUDA(cudaSetDevice(fe->ctx->device));
-  int rc = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  if (fe->img_dst) {
-    rc = feature_image_run(fe->ctx, fe->ctx->stream, fe->maps, frames_dev, n_frames, fe->img_lut, fe->img_dst,
-                           "sfe_frontend_run_dev");
-    if (rc != SFE_OK) return rc;
-  }
-  // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
-  if (fe->overlap > 0 && !fe->timer.on) return fe_run_overlapped(fe, frames_dev, poses_host, n_frames);
-  rc = fe_features(fe, fe->ctx->stream, frames_dev, 0, n_frames);
-  if (rc != SFE_OK) return rc;
-  rc = fe_match(fe, fe->ctx->stream, 0, n_frames);
-  if (rc != SFE_OK) return rc;
-  return fe_update_carry(fe, fe->ctx->stream, poses_host, n_frames);
+  return fe_run_dev(fe, frames_dev, nullptr, poses_host, n_frames, "sfe_frontend_run_dev");
+}
+
+int sfe_frontend_run_dev_geometry(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t *geometry,
+                                  const double *poses_host, int n_frames) {
+  SFE_REQUIRE(geometry != nullptr, "sfe_frontend_run_dev_geometry: null geometry");
+  return fe_run_dev(fe, frames_dev, geometry, poses_host, n_frames, "sfe_frontend_run_dev_geometry");
 }
 
 int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, const int32_t **iters, const int32_t **inliers,
@@ -726,48 +917,51 @@ int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, const int3
 int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const double *poses_host, int n_frames,
                           int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                           int32_t *status_host, int32_t *npoints_host) {
-  SFE_REQUIRE(fe && frames_host && poses_host && T_host && iters_host && inliers_host && status_host,
-              "sfe_frontend_run_host: null argument");
-  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "sfe_frontend_run_host: %d frames exceed max_frames %d",
-              n_frames, fe->max_frames);
-  if (n_frames == 0) return SFE_OK;
-  int rc = fe_host_begin(fe, n_frames, chunk_frames, "sfe_frontend_run_host");
-  if (rc != SFE_OK) return rc;
-  ImagesDrained drained{fe};
-  rc = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
-  // frame chunks stream in on the copy stream; the feature stages of chunk k run while chunk k+1 copies
-  int k = 0;
-  for (int f0 = 0; f0 < n_frames; f0 += chunk_frames, ++k) {
-    const int n = std::min(chunk_frames, n_frames - f0);
-    SFE_CUDA(cudaMemcpyAsync(fe->frames + (size_t)f0 * fbytes, frames_host + (size_t)f0 * fbytes, (size_t)n * fbytes,
-                             cudaMemcpyHostToDevice, fe->copy_stream));
-    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
-    SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
-    rc = fe_render_chunk(fe, f0, n, k, "sfe_frontend_run_host");
-    if (rc != SFE_OK) return rc;
-    rc = fe_features(fe, ctx->stream, fe->frames + (size_t)f0 * fbytes, f0, n);
-    if (rc != SFE_OK) return rc;
-    rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
-    if (rc != SFE_OK) return rc;
-  }
-  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
+  return fe_run_raw_host(fe, frames_host, nullptr, nullptr, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                         inliers_host, status_host, npoints_host, "sfe_frontend_run_host");
+}
+
+int sfe_frontend_run_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                   const int32_t *geometry, const double *poses_host, int n_frames, int chunk_frames,
+                                   float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                                   int32_t *npoints_host) {
+  SFE_REQUIRE(offsets && geometry, "sfe_frontend_run_host_geometry: null offsets / geometry");
+  return fe_run_raw_host(fe, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host, iters_host,
+                         inliers_host, status_host, npoints_host, "sfe_frontend_run_host_geometry");
 }
 
 int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                                int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
                                int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                                inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
+  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames, T_host,
+                                iters_host, inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
 }
 
 int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                               int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                                inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
+  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames, T_host,
+                                iters_host, inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
+}
+
+int sfe_frontend_run_jpeg_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                        const int32_t *geometry, const double *poses_host, int n_frames,
+                                        int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
+                                        int32_t *status_host, int32_t *npoints_host) {
+  SFE_REQUIRE(geometry != nullptr, "sfe_frontend_run_jpeg_host_geometry: null geometry");
+  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host,
+                                iters_host, inliers_host, status_host, npoints_host,
+                                "sfe_frontend_run_jpeg_host_geometry");
+}
+
+int sfe_frontend_run_png_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
+                                       const int32_t *geometry, const double *poses_host, int n_frames,
+                                       int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
+                                       int32_t *status_host, int32_t *npoints_host) {
+  SFE_REQUIRE(geometry != nullptr, "sfe_frontend_run_png_host_geometry: null geometry");
+  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host,
+                                iters_host, inliers_host, status_host, npoints_host,
+                                "sfe_frontend_run_png_host_geometry");
 }
 
 }  // extern "C"

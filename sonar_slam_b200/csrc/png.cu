@@ -697,8 +697,8 @@ struct PngState final : StreamDecoder {
   // Inflate is serial within a frame and latency-bound: a chunk of 32 frames (warps) per SM keeps every scheduler
   // busy.  A 512 x 512 ping takes about 0.5 MB of scratch, so a chunk of ~4k frames takes about 2 GB.
   int chunk_frames(const sfe_ctx *ctx) const override { return std::max(256, ctx->sm_count * 32); }
-  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B) override {
-    bt.parse(bytes, offsets, n, R, B, parse_png, SFE_PNG_SIZE);
+  void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, const int32_t *shape) override {
+    bt.parse(bytes, offsets, n, R, B, shape, parse_png, SFE_PNG_SIZE);
   }
   int frame_status(int i) const override { return bt.hdr[i].status; }
   const char *message(int status) const override { return sfe_png_status_message(status); }
@@ -751,7 +751,7 @@ int PngState::decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) {
   png_inflate_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, s, st);
   timer.toc(ctx->stream);
   timer.tic(ctx->stream, SFE_PNG_T_UNFILTER);
-  png_unfilter_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, s, st, out_dev, (int64_t)bt.R * bt.B);
+  png_unfilter_kernel<<<wblocks, 32 * PNG_WARPS, 0, ctx->stream>>>(desc, nf, s, st, out_dev, (int64_t)bt.R_of(f0) * bt.B_of(f0));
   timer.toc(ctx->stream);
   ctx->launches += 3;
   SFE_CUDA(cudaGetLastError());

@@ -88,7 +88,7 @@ int decode_all(sfe_ctx *ctx, StreamDecoder *(*decoder)(sfe_ctx *), const uint8_t
   if (n == 0) return SFE_OK;
   SFE_CUDA(cudaSetDevice(ctx->device));
   StreamDecoder *dec = decoder(ctx);
-  dec->parse(bytes, offsets, n, R, B);
+  dec->parse(bytes, offsets, n, R, B, nullptr);
   const size_t fb = (size_t)R * B;
   const int chunk = dec->chunk_frames(ctx);
   const bool via_out = !out_dev;

@@ -45,16 +45,20 @@ struct StreamBatch {
   const uint8_t *bytes = nullptr;
   const int64_t *offsets = nullptr;
   int n = 0, R = 0, B = 0;
+  const int32_t *shape = nullptr;  // optional int32 [n][2]: frame i must be shape[2i] x shape[2i + 1] instead of R x B
   std::vector<Header> hdr;
 
-  // Header::status 0 is a stream the decoder takes; one whose frame is not R x B gets size_status instead
-  void parse(const uint8_t *bytes_, const int64_t *offsets_, int n_, int R_, int B_,
+  int R_of(int i) const { return shape ? shape[2 * i] : R; }
+  int B_of(int i) const { return shape ? shape[2 * i + 1] : B; }
+
+  // Header::status 0 is a stream the decoder takes; one whose frame is not R x B (or its own shape) gets size_status
+  void parse(const uint8_t *bytes_, const int64_t *offsets_, int n_, int R_, int B_, const int32_t *shape_,
              void (*parse_header)(const uint8_t *, int64_t, Header &), int size_status) {
-    bytes = bytes_, offsets = offsets_, n = n_, R = R_, B = B_;
+    bytes = bytes_, offsets = offsets_, n = n_, R = R_, B = B_, shape = shape_;
     hdr.resize(n);
     for (int i = 0; i < n; ++i) {
       parse_header(bytes + offsets[i], offsets[i + 1] - offsets[i], hdr[i]);
-      if (hdr[i].status == 0 && (hdr[i].H != R || hdr[i].W != B)) hdr[i].status = size_status;
+      if (hdr[i].status == 0 && (hdr[i].H != R_of(i) || hdr[i].W != B_of(i))) hdr[i].status = size_status;
     }
   }
 };
@@ -70,13 +74,15 @@ struct StreamDecoder {
 
   virtual ~StreamDecoder();
   virtual int chunk_frames(const sfe_ctx *ctx) const = 0;  // chunk size of the decode entry points
-  virtual void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B) = 0;
+  // shape: null (every frame R x B) or int32 [n][2], each frame's own R x B (valid until the call's last decode_chunk)
+  virtual void parse(const uint8_t *bytes, const int64_t *offsets, int n, int R, int B, const int32_t *shape) = 0;
   virtual int frame_status(int i) const = 0;  // after parse: 0 when the decoder takes frame i
   virtual const char *message(int status) const = 0;
-  // after parse: every buffer sized for the largest chunk of `chunk` frames, and out_bytes of `out`
+  // after parse: every buffer sized for the largest chunk of `chunk` frames, and out_bytes of `out`; a decode_chunk of
+  // any subset of consecutive frames of such a chunk fits too
   virtual int reserve(sfe_ctx *ctx, int chunk, size_t out_bytes) = 0;
-  // frames [f0, f0 + nf) into out_dev (uint8 [nf][R][B]), their statuses into `status` at [f0, f0 + nf); asynchronous
-  // on ctx->stream, the bytes go in through the stager
+  // frames [f0, f0 + nf) into out_dev (uint8 [nf][R][B], R x B = frame f0's shape: the frames of one decode_chunk share
+  // it), their statuses into `status` at [f0, f0 + nf); asynchronous on ctx->stream, the bytes go in through the stager
   virtual int decode_chunk(sfe_ctx *ctx, int f0, int nf, uint8_t *out_dev) = 0;
 
  protected:

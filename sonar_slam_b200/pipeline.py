@@ -4,6 +4,9 @@ Python face of include/sonarfe.h's sfe_frontend_*: one call per backlog of frame
 in host memory (`run_host`, the end-to-end path: frames are copied in chunks overlapped with the
 kernels) or already on the device (`run_dev`).  See csrc/pipeline.cu for what is computed and how
 it maps onto the reference's FeatureExtraction.callback / SLAM.add_sequential_scan_matching.
+
+A front end may hold several sonar geometries (add_geometry): every run flavour then takes `geometry=`, one id per
+frame, and a bag whose range setting changes is fed as one sequence.
 """
 import contextlib
 import ctypes
@@ -27,13 +30,59 @@ class FrontEnd:
             setattr(p, k, v)
         self.params = p
         self.max_frames = int(max_frames)
+        self.geometries = [maps]  # id -> Maps (kept alive: the front end references them)
         h = ctypes.c_void_p()
         _lib.check(self.lib.sfe_frontend_create(ctx.handle, maps.handle, ctypes.byref(p), self.max_frames,
                                                 ctypes.byref(h)), "sfe_frontend_create")
         self.handle = h
 
+    def add_geometry(self, maps):
+        """Register a further sonar geometry (sfe_frontend_add_geometry) and return its id; the creation maps are
+        geometry 0.  Its polar shape must fit the frame slots the front end was created with (maps.R <= R,
+        maps.B <= B); at most _lib.MAX_GEOMETRIES geometries."""
+        gid = ctypes.c_int()
+        _lib.check(self.lib.sfe_frontend_add_geometry(self.handle, maps.handle, ctypes.byref(gid)),
+                   "sfe_frontend_add_geometry")
+        self.geometries.append(maps)
+        return gid.value
+
+    def _geometry(self, geometry, n):
+        """geometry= of a run call -> int32 [n] (or None)."""
+        if geometry is None:
+            return None
+        g = np.ascontiguousarray(geometry, np.int32).reshape(-1)
+        if len(g) != n:
+            raise ValueError(f"FrontEnd: geometry has {len(g)} ids for {n} frames")
+        return g
+
+    def _image_maps(self, geometry):
+        """The geometry whose feature images a call writes: its frames' one geometry (several: the C side refuses)."""
+        if geometry is None or len(geometry) == 0 or not 0 <= geometry[0] < len(self.geometries):
+            return self.maps
+        return self.geometries[geometry[0]]
+
+    def pack_frames(self, frames, geometry):
+        """Raw frames of several geometries -> (uint8 bytes [total], int64 offsets [n + 1]), frame i =
+        bytes[offsets[i]:offsets[i + 1]] row-major [R_g, B_g] (the host form of sfe_frontend_run_host_geometry).
+        frames: a sequence of uint8 [R_g, B_g] arrays, or (bytes, offsets) already packed, which is checked."""
+        if isinstance(frames, tuple):
+            buf, off = frames
+            buf = np.ascontiguousarray(buf, np.uint8).reshape(-1)
+            off = np.ascontiguousarray(off, np.int64)
+            if off.ndim != 1 or len(off) == 0 or off[0] < 0 or off[-1] > buf.size:
+                raise ValueError(f"FrontEnd: frame offsets overrun the packed buffer ({buf.size} bytes)")
+            return buf, off
+        for i, f in enumerate(frames):
+            g = int(geometry[i]) if i < len(geometry) else 0
+            if 0 <= g < len(self.geometries):
+                m = self.geometries[g]
+                if np.shape(f) != (m.R, m.B):
+                    raise ValueError(f"FrontEnd: frame {i} has shape {np.shape(f)}; its geometry {g} is "
+                                     f"{m.R} x {m.B}")
+        return _streams.pack(np.ascontiguousarray(f, np.uint8).tobytes() for f in frames)
+
     @contextlib.contextmanager
-    def _images(self, images, n, on_device, lut):
+    def _images(self, images, n, on_device, lut, maps=None):
         """Feature images of the frames of one run call (sfe_frontend_set_feature_images), off again afterwards.
         images: uint8 [n, rows, cols, 3] C-contiguous -- a numpy array for the host flavours, a CUDA tensor on the
         context's device for run_dev; lut: uint8 [256, 3] BGR table (default feature_image.JET)."""
@@ -41,7 +90,8 @@ class FrontEnd:
             yield
             return
         from . import feature_image
-        shape = (n, self.maps.rows, self.maps.cols, 3)
+        maps = maps or self.maps
+        shape = (n, maps.rows, maps.cols, 3)
         if on_device:
             import torch
             if not (isinstance(images, torch.Tensor) and images.is_cuda and images.dtype == torch.uint8
@@ -61,13 +111,26 @@ class FrontEnd:
         finally:
             self.lib.sfe_frontend_set_feature_images(self.handle, None, None, 0)
 
-    def run_host(self, frames, poses, chunk_frames=256, out=None, images=None, image_lut=None):
+    def run_host(self, frames, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
         """frames: uint8 [n,R,B] numpy (pinned memory gives full copy bandwidth); poses: float64 [n,3].
         Returns dict(T [n,3,3] f32, iterations, inliers, status, npoints).  images: an optional uint8
         [n, rows, cols, 3] numpy array that receives every frame's feature image (feature_image.py; colour table
-        image_lut, default JET); the results are the same with and without it."""
-        frames = np.ascontiguousarray(frames, np.uint8)
+        image_lut, default JET); the results are the same with and without it.
+        geometry: one id per frame (add_geometry); frames are then a sequence of uint8 [R_g, B_g] arrays or
+        (bytes, offsets) from pack_frames (sfe_frontend_run_host_geometry)."""
         poses = np.ascontiguousarray(poses, np.float64)
+        if geometry is not None:
+            n = len(frames[1]) - 1 if isinstance(frames, tuple) else len(frames)
+            geometry = self._geometry(geometry, n)
+            buf, off = self.pack_frames(frames, geometry)
+            o = out or self.alloc_results(n)
+            with self._images(images, n, False, image_lut, self._image_maps(geometry)):
+                _lib.check(self.lib.sfe_frontend_run_host_geometry(
+                    self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(geometry), _lib.ptr(poses), n,
+                    int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]),
+                    _lib.ptr(o["status"]), _lib.ptr(o["npoints"])), "sfe_frontend_run_host_geometry")
+            return o
+        frames = np.ascontiguousarray(frames, np.uint8)
         n = len(frames)
         o = out or self.alloc_results(n)
         with self._images(images, n, False, image_lut):
@@ -77,27 +140,33 @@ class FrontEnd:
                                                       _lib.ptr(o["npoints"])), "sfe_frontend_run_host")
         return o
 
-    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None):
+    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
         """run_host on compressed pings: streams is a sequence of JPEG bytes objects (or (bytes, offsets) from
         jpeg.pack); the compressed bytes are copied and decoded on the device instead of copying raw frames
         (sfe_frontend_run_jpeg_host).  A stream that is rejected or fails to decode raises, naming the frame.
-        images / image_lut: as run_host."""
-        return self._run_compressed("sfe_frontend_run_jpeg_host", streams, poses, chunk_frames, out, images, image_lut)
+        images / image_lut / geometry: as run_host (with geometry, every stream must decode to its geometry's
+        R_g x B_g)."""
+        return self._run_compressed("sfe_frontend_run_jpeg_host", streams, poses, chunk_frames, out, images, image_lut,
+                                    geometry)
 
-    def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None):
+    def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
         """run_jpeg_host for PNG streams (sfe_frontend_run_png_host)."""
-        return self._run_compressed("sfe_frontend_run_png_host", streams, poses, chunk_frames, out, images, image_lut)
+        return self._run_compressed("sfe_frontend_run_png_host", streams, poses, chunk_frames, out, images, image_lut,
+                                    geometry)
 
-    def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut):
+    def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut, geometry):
         buf, off = _streams.packed(streams)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
+        geometry = self._geometry(geometry, n)
         o = out or self.alloc_results(n)
-        with self._images(images, n, False, image_lut):
-            _lib.check(getattr(self.lib, name)(self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(poses), n,
-                                               int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                               _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])),
-                       name)
+        head = (self.handle, _lib.ptr(buf), _lib.ptr(off))
+        if geometry is not None:
+            name, head = name + "_geometry", head + (_lib.ptr(geometry),)
+        with self._images(images, n, False, image_lut, self._image_maps(geometry)):
+            _lib.check(getattr(self.lib, name)(*head, _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]),
+                                               _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]),
+                                               _lib.ptr(o["status"]), _lib.ptr(o["npoints"])), name)
         return o
 
     @staticmethod
@@ -105,13 +174,21 @@ class FrontEnd:
         return dict(T=np.empty((n, 3, 3), np.float32), iterations=np.empty(n, np.int32),
                     inliers=np.empty(n, np.int32), status=np.empty(n, np.int32), npoints=np.empty(n, np.int32))
 
-    def run_dev(self, frames_ptr, poses, n, images=None, image_lut=None):
+    def run_dev(self, frames_ptr, poses, n, images=None, image_lut=None, geometry=None):
         """frames_ptr: device address of uint8 [n,R,B]; poses: float64 [n,3] numpy (host).  Asynchronous.
-        images: an optional uint8 [n, rows, cols, 3] CUDA tensor that receives every frame's feature image."""
+        images: an optional uint8 [n, rows, cols, 3] CUDA tensor that receives every frame's feature image.
+        geometry: one id per frame (add_geometry); frame i of geometry g then occupies the first R_g * B_g bytes of
+        its R * B slot, row-major [R_g, B_g] (sfe_frontend_run_dev_geometry)."""
         poses = np.ascontiguousarray(poses, np.float64)
-        with self._images(images, int(n), True, image_lut):
-            _lib.check(self.lib.sfe_frontend_run_dev(self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(poses),
-                                                         int(n)), "sfe_frontend_run_dev")
+        geometry = self._geometry(geometry, int(n))
+        with self._images(images, int(n), True, image_lut, self._image_maps(geometry)):
+            if geometry is None:
+                _lib.check(self.lib.sfe_frontend_run_dev(self.handle, ctypes.c_void_p(int(frames_ptr)),
+                                                         _lib.ptr(poses), int(n)), "sfe_frontend_run_dev")
+            else:
+                _lib.check(self.lib.sfe_frontend_run_dev_geometry(self.handle, ctypes.c_void_p(int(frames_ptr)),
+                                                                  _lib.ptr(geometry), _lib.ptr(poses), int(n)),
+                           "sfe_frontend_run_dev_geometry")
 
     def results_dev(self):
         """Device addresses of the last run's results: dict(T, iterations, inliers, status, cloud_xy,
