@@ -167,6 +167,13 @@ SFE_API int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t
 SFE_API int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
                                    int n_max, double radius, int min_points, float *out_pts_dev,
                                    int32_t *out_idx_dev, int32_t *out_count_dev);
+/* the batched front end's per-frame down-sample: clouds of up to frame_points (<= 8191) points in its frame-class
+ * kernel, larger ones in a launch laid out for n_max; cnt_dev (optional) holds the clouds' point counts, else
+ * off_dev[c + 1] - off_dev[c].  2-column clouds only.  Same results as sfe_downsample_dev. */
+SFE_API int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev,
+                                      const int32_t *cnt_dev, int n_clouds, int n_max, int frame_points,
+                                      float resolution, float *out_pts_dev, int32_t *out_idx_dev,
+                                      int32_t *out_count_dev);
 /* single-cloud host flavours: n points in, *n_out points out (out buffers hold n entries) */
 SFE_API int sfe_downsample_host(sfe_ctx *ctx, const float *pts_host, int n, int dim, float resolution,
                                 float *out_pts_host, int32_t *out_idx_host, int32_t *n_out);

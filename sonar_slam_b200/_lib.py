@@ -92,6 +92,8 @@ _EXTRA_SIGNATURES = {
     "sfe_downsample_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
     "sfe_remove_outlier_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_int, c_void_p, c_void_p,
                                c_void_p],
+    "sfe_downsample_frames_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
+                                  c_void_p, c_void_p],
     "sfe_downsample_host": [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
     "sfe_remove_outlier_host": [c_void_p, c_void_p, c_int, c_int, c_double, c_int, c_void_p, c_void_p, c_void_p],
     "sfe_match_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p],

@@ -233,6 +233,16 @@ int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_de
                         out_idx_dev, out_count_dev, DS_ANY_SIZE, SCR_CLOUD);
 }
 
+int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, const int32_t *cnt_dev,
+                              int n_clouds, int n_max, int frame_points, float resolution, float *out_pts_dev,
+                              int32_t *out_idx_dev, int32_t *out_count_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_downsample_frames_dev: null context");
+  SFE_REQUIRE(frame_points > 0, "sfe_downsample_frames_dev: frame_points must be positive (got %d)", frame_points);
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  return downsample_run(ctx, ctx->stream, {pts_dev, off_dev, cnt_dev, n_max}, n_clouds, 2, resolution, out_pts_dev,
+                        out_idx_dev, out_count_dev, frame_points, SCR_CLOUD, true);
+}
+
 int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
                            int n_max, double radius, int min_points, float *out_pts_dev, int32_t *out_idx_dev,
                            int32_t *out_count_dev) {

@@ -88,7 +88,7 @@ enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC =
        SCR_DS_GRID = 7 };
 // Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
 // different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
-enum { WORK_CART = 0, WORK_ICP = 1, SFE_WORK_COUNTERS = 2 };
+enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, SFE_WORK_COUNTERS = 3 };
 
 // (re)allocate if too small, stream-ordered on `stream` (default: ctx->stream).  A buffer must only grow on a stream
 // that is ordered after every earlier user of the block and before every later one: the stream that uses it.

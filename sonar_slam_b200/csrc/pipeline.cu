@@ -34,10 +34,14 @@ constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 896;
 static_assert(FE_ICP_SMALL_SRC <= 640, "the small ICP class must stay within icp_run's 128-thread CTAs");
 // Size classes of the cloud filters (cloud.cu: two launches by cloud size).  Config-4 replay: 3-5 k raw Cartesian
 // points per frame, ~580 after the voxel filter, ~400 after the outlier filter, window submaps <= 1.8 k raw points.
-// The outlier filter and the submap down-sampling gain from a small-cloud class; the per-frame down-sampling is best
-// left as one launch (with a class boundary at 4608 or 5632 points too many frames land in the second, poorly
-// filled launch).  Chosen on the replay; not re-measured on H100.
-constexpr int FE_DS_SPLIT = 0, FE_RO_SPLIT = 1024, FE_SUBMAP_SPLIT = 2048;
+// The outlier filter and the submap down-sampling gain from a small-cloud class (chosen on the replay; not
+// re-measured on H100).
+constexpr int FE_RO_SPLIT = 1024, FE_SUBMAP_SPLIT = 2048;
+// Frame class of the per-frame down-sampling (cloud.cu: downsample_frame_kernel), from the raw clouds of bench.py's
+// 4096-frame bag (tools/ds_sizes.py): mean 3378, p99.9 5602, max 5647 points.  6144 leaves a 9 % margin over the
+// largest; larger clouds take the capacity launch.  At 6144 points the frame kernel needs 97 KB of dynamic shared
+// memory (16 bytes per point: the sorted points are staged there), so an H100 SM holds 2 of its 512-thread CTAs.
+constexpr int FE_DS_FRAME = 6144;
 // Default schedule of sfe_frontend_run_dev (sfe_frontend_set_overlap): serial.  On an H100 (700 W) the overlapped
 // schedule measured slower at every sub-batch size tried on the config-4 replay (DESIGN.md section 4).
 constexpr int FE_OVERLAP_FRAMES = 0;
@@ -488,12 +492,11 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const int32_t *cur_cnt = fe->cnt_a;
   if (p.resolution > 0.f) {
     fe->timer.tic(st, SFE_FE_DOWNSAMPLE);
-    static const int ds_split = [] {  // development switch: SFE_FE_DS_SPLIT=<points> (0: one launch)
-      const char *e = getenv("SFE_FE_DS_SPLIT");
-      return e ? atoi(e) : FE_DS_SPLIT;
-    }();
+    // development switch: SFE_FE_DS_SPLIT=<points> takes downsample_kernel's layouts instead of the frame class
+    // (0: one capacity launch)
+    static const char *ds_split = getenv("SFE_FE_DS_SPLIT");
     rc = downsample_run(ctx, st, {cur, fe->off_pts + f0, cur_cnt + f0, (int)cap}, n, 2, p.resolution, fe->xy_b, fe->idx,
-                        fe->cnt_b + f0, ds_split, SCR_CLOUD);
+                        fe->cnt_b + f0, ds_split ? atoi(ds_split) : FE_DS_FRAME, SCR_CLOUD, !ds_split);
     fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
     cur = fe->xy_b, cur_cnt = fe->cnt_b;

@@ -37,10 +37,12 @@ int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint
 int feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *frames, int F,
                       const uint8_t *lut_bgr, uint8_t *out, const char *what);  // what: the caller, for errors
 // n_split > 0: two launches by cloud size (cloud.cu), 0: one launch, DS_ANY_SIZE: clouds of any size (one-CTA kernel
-// up to the device's limit, grid-wide path above it)
+// up to the device's limit, grid-wide path above it).  frame_class: the first of the two launches is the front end's
+// frame kernel (n_split at most 8191 points)
 constexpr int DS_ANY_SIZE = -1;
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
-                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot);
+                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot,
+                   bool frame_class = false);
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
                        int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split);
 // problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu), (0, 0): one launch

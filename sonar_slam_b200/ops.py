@@ -98,6 +98,21 @@ def downsample(pts, off, n_max, resolution, ctx=None):
     return dict(pts=out, idx=idx, count=cnt)
 
 
+def downsample_frames(pts, off, n_max, resolution, frame_points, cnt=None, ctx=None):
+    """The front end's per-frame down-sample on packed clouds: clouds of up to `frame_points` points in its frame-class
+    kernel, larger ones in a launch laid out for n_max (pts [total,2] f32, off [n+1] i32, optional cnt [n] i32, cuda).
+    Same results as downsample()."""
+    ctx = ctx or context(pts.device)
+    n = off.numel() - 1
+    out = torch.empty_like(pts)
+    idx = torch.empty((pts.shape[0],), dtype=torch.int32, device=pts.device)
+    count = torch.empty((n,), dtype=torch.int32, device=pts.device)
+    _lib.check(ctx.lib.sfe_downsample_frames_dev(ctx.handle, _dp(pts), _dp(off), _dp(cnt) if cnt is not None else None,
+                                                 n, int(n_max), int(frame_points), float(resolution), _dp(out),
+                                                 _dp(idx), _dp(count)), "sfe_downsample_frames_dev")
+    return dict(pts=out, idx=idx, count=count)
+
+
 def remove_outlier(pts, off, n_max, radius, min_points, ctx=None):
     ctx = ctx or context(pts.device)
     n = off.numel() - 1

@@ -1,12 +1,18 @@
 #!/bin/bash
-# experimental build of libsonarfe where every down-sampled cloud takes the grid-wide path -> scratch/lib_dsgrid.so
-# (run after the main build; tools/bench_map_downsample.py compares it with the one-CTA kernel)
+# experimental builds of libsonarfe with cloud.cu knobs (run after the main build):
+#   scratch/lib_dsgrid.so    every down-sampled cloud takes the grid-wide path (tools/bench_map_downsample.py compares
+#                            it with the one-CTA kernel)
+#   scratch/lib_dsphases.so  per-phase cycle counts of the down-sample kernels (-DSFE_DS_PHASE_CLOCKS, tools/ds_phases.py)
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p scratch
 B=sonar_slam_b200/build
 FL="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr"
-nvcc $FL -DSFE_DS_GRID_ALL -c sonar_slam_b200/csrc/cloud.cu -o scratch/cloud_dsgrid.o
 objs=$(ls $B/*.o | grep -v "/cloud.o")
-nvcc -shared -o scratch/lib_dsgrid.so scratch/cloud_dsgrid.o $objs -gencode arch=compute_90a,code=sm_90a -lcudart
-ls -la scratch/lib_dsgrid.so
+build() { tag=$1; shift
+  nvcc $FL "$@" -c sonar_slam_b200/csrc/cloud.cu -o scratch/cloud_$tag.o
+  nvcc -shared -o scratch/lib_$tag.so scratch/cloud_$tag.o $objs -gencode arch=compute_90a,code=sm_90a -lcudart
+}
+build dsgrid -DSFE_DS_GRID_ALL
+build dsphases -DSFE_DS_PHASE_CLOCKS
+ls -la scratch/lib_dsgrid.so scratch/lib_dsphases.so
