@@ -185,7 +185,11 @@ SFE_API int sfe_remove_outlier_host(sfe_ctx *ctx, const float *pts_host, int n, 
  * for every query point the index of the nearest reference point and the SQUARED float32 distance;
  * no reference point within max_dist -> id -1, dist +inf; ties -> lowest reference index.
  * Batched over n_pairs (ref cloud p, query cloud p), both packed [total][2] with CSR offsets;
- * ids / dists are indexed like the query points.  Only knn = 1 (what the reference uses). */
+ * ids / dists are indexed like the query points.  Only knn = 1 (what the reference uses).
+ * References of any size: those that fit one CTA's shared memory (24 k points on an H100) run one CTA per pair; larger
+ * ones (whole maps) are sorted once into a grid in global memory and searched by the whole device, with the same
+ * results.  Their workspace holds 40 bytes for each of n_pairs * n_ref_max slot points (at most 2^31 - 1), 6 bytes
+ * per n_ref_max point of cell table per pair, and CUB's temporary storage. */
 SFE_API int sfe_match_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev, const float *in_pts_dev,
                           const int32_t *in_off_dev, int n_pairs, int n_ref_max, float max_dist, int32_t *ids_dev,
                           float *dists_dev);
@@ -240,7 +244,14 @@ SFE_API const char *sfe_icp_status_message(int status);
  * (ids NULL: cloud p) from the initial guess guess[p] (3x3 row-major float32, as ICP.compute's third
  * argument); clouds packed [total][2] with CSR offsets, ns_max / nt_max = largest source / target.
  * Outputs per problem: T (3x3 row-major; = guess when status != 0, like pcl.cpp:207-210), iterations
- * made, inlier count of the last iteration (pairs with non-zero weight), status. */
+ * made, inlier count of the last iteration (pairs with non-zero weight), status.
+ * Targets of any size: the problems whose target fits one CTA's shared memory next to the sources (22 k points
+ * next to 1 500-point sources on an H100) run as before; the others read their target from a map grid built once
+ * per distinct target cloud in global memory (mean, normals and grid computed once, not per guess), with the same
+ * results.  Sources stay limited to 65 535 points and to what fits shared memory (about 31 bytes per point, 7 000
+ * points).  Map workspace: 40 bytes (48 point-to-plane) for each of slots * nt_max slot points (at most 2^31 - 1),
+ * 6 bytes per nt_max point of cell table per slot, 28 bytes per problem and CUB's temporary storage; slots =
+ * n_problems for sfe_icp_dev, min(n_problems, n_tgt_clouds) for the host flavours. */
 SFE_API int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev, const int32_t *src_off_dev,
                         const float *tgt_pts_dev, const int32_t *tgt_off_dev, const int32_t *src_id_dev,
                         const int32_t *tgt_id_dev, int n_problems, int ns_max, int nt_max, const float *guess_dev,

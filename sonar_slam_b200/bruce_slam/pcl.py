@@ -75,6 +75,8 @@ def density_filter(*args, **kwargs):
 
 
 def match(mat_ref, mat_in, knn, max_dist):
+    """libnabo KD-tree match, knn = 1: (ids [1,N] int32, squared dists [1,N] float32).  References of any size (whole
+    maps run as a grid in global memory, with the same results)."""
     if int(knn) != 1:
         raise NotImplementedError("pcl.match: only knn = 1 is implemented (the only value the reference uses, "
                                   "slam.py:418)")
@@ -181,7 +183,8 @@ class ICP(object):
     def compute_batch(self, source, target, guesses):
         """All `guesses` (iterable of 3x3) on the same cloud pair in one launch (N1: the loop of
         SLAM.compute_icp_with_cov, slam.py:346-358).  Returns dict(messages, T[n,3,3], iterations,
-        inliers, status)."""
+        inliers, status).  The target may be of any size (a whole map): above one CTA's shared memory it is
+        sorted once into a grid in global memory that every guess reads, with the same results."""
         if self.params is None:
             raise RuntimeError("You must setup a matcher before running ICP")
         src = _points(source, "source", cols=(2,))

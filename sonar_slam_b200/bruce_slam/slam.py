@@ -84,6 +84,8 @@ class SLAM(object):
 
     # ---- slam.py:325-387 (the up-to-30 ICP runs go to the GPU as ONE batch instead of a timed loop)
     def compute_icp_with_cov(self, source_points, target_points, guesses):
+        """slam.py:325-387: the guesses run as one ICP batch.  target_points may be the whole map (the loop-closure
+        target of initialize_nonsequential_scan_matching): it is gridded once on the device and shared by every guess."""
         from sklearn.covariance import MinCovDet
         source_points = np.array(source_points, np.float32)
         target_points = np.array(target_points, np.float32)

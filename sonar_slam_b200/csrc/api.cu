@@ -456,9 +456,10 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
     SFE_CUDA(cudaMemcpyAsync(d_ids, src_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_ids + P, tgt_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
-    int rc = icp_run(ctx, ctx->stream, prm,
-                     {{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
-                      d_guess, d_T, d_res, d_res + P, d_res + 2 * P}, 0, 0);
+    IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
+                   d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
+    pb.n_tgt_clouds = n_tgt_clouds;
+    int rc = icp_run(ctx, ctx->stream, prm, pb, 0, 0);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));

@@ -17,13 +17,19 @@ namespace sfe {
 
 constexpr int GRID_MAX_CELLS = 16384;  // 16-bit offsets, two per 32-bit word
 
-struct GridView {
-  const float2 *pts;        // points sorted by cell
-  const uint16_t *cstart;   // [ncells + 1] first sorted position of every cell
-  const uint16_t *orig;     // sorted position -> index in the caller's cloud
+// Idx: type of the cell offsets and original indices.  uint16_t for the grids a CTA builds in shared memory
+// (GridView); int for the map grids built once per target cloud in global memory (icp.cu, MapGridView), whose
+// offsets are absolute positions in the workspace's sorted-point array.
+template <typename Idx>
+struct GridViewT {
+  const float2 *pts;   // points sorted by cell
+  const Idx *cstart;   // [ncells + 1] first sorted position of every cell
+  const Idx *orig;     // sorted position -> index in the caller's cloud
   int n, nx, ny;
   float ox, oy, cell, inv_cell;
 };
+using GridView = GridViewT<uint16_t>;
+using MapGridView = GridViewT<int>;
 
 __device__ __forceinline__ float dist2_rn(float dx, float dy) {
   return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
@@ -64,13 +70,14 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int *warp_sums /* [33
 }
 
 // Choose grid geometry for n points with bounding box [minx,maxx] x [miny,maxy].
+template <typename Idx>
 __device__ __forceinline__ void grid_geometry(int n, float minx, float miny, float maxx, float maxy, float min_cell,
-                                              GridView &g, int max_cells, float cell_scale = 1.0f) {
+                                              GridViewT<Idx> &g, int max_cells, float cell_scale = 1.0f) {
   const float w = maxx - minx, h = maxy - miny;
   float cell = cell_scale * sqrtf((w * h) / (float)(n > 0 ? n : 1));
   if (!(cell > min_cell)) cell = min_cell;
   if (!(cell > 1e-6f)) cell = 1.f;
-  // keep the cell table within max_cells (<= GRID_MAX_CELLS)
+  // keep the cell table within max_cells (<= GRID_MAX_CELLS for the 16-bit grids)
   for (int it = 0; it < 32; ++it) {
     const float inv = 1.f / cell;
     const long long nx = (long long)(w * inv) + 1, ny = (long long)(h * inv) + 1;
@@ -160,7 +167,8 @@ __device__ __forceinline__ void nn_update(float d2, int p, NNResult &r) {
 // load followed by its use costs the full latency per candidate), and the best / tie bookkeeping only runs
 // when one of the four is at least as close as the current best -- O(log n) times per query.  Positions past
 // the end are clamped to e - 1: re-evaluating a candidate never changes the result (same position, no tie).
-__device__ __forceinline__ void nn_scan(const GridView &g, int s, int e, float qx, float qy, NNResult &r) {
+template <typename Idx>
+__device__ __forceinline__ void nn_scan(const GridViewT<Idx> &g, int s, int e, float qx, float qy, NNResult &r) {
   const int last = e - 1;
   for (int p = s; p < e; p += 4) {
     const int p1 = min(p + 1, last), p2 = min(p + 2, last), p3 = min(p + 3, last);
@@ -178,7 +186,8 @@ __device__ __forceinline__ void nn_scan(const GridView &g, int s, int e, float q
 
 // rare: among the points of the cell rectangle [xa, xb] x [ya, yb] at exactly distance r.d2, keep the lowest
 // original index
-static __device__ __noinline__ void nn_resolve_tie_rect(const GridView &g, int xa, int xb, int ya, int yb, float qx,
+template <typename Idx>
+static __device__ __noinline__ void nn_resolve_tie_rect(const GridViewT<Idx> &g, int xa, int xb, int ya, int yb, float qx,
                                                         float qy, NNResult &r) {
   if (g.orig == nullptr || r.pos < 0) return;
   int best = r.pos;
@@ -191,13 +200,15 @@ static __device__ __noinline__ void nn_resolve_tie_rect(const GridView &g, int x
   r.tie = 0;
 }
 
-__device__ __forceinline__ void nn_resolve_tie(const GridView &g, int cx, int cy, int k, float qx, float qy, NNResult &r) {
+template <typename Idx>
+__device__ __forceinline__ void nn_resolve_tie(const GridViewT<Idx> &g, int cx, int cy, int k, float qx, float qy, NNResult &r) {
   nn_resolve_tie_rect(g, max(cx - k, 0), min(cx + k, g.nx - 1), max(cy - k, 0), min(cy + k, g.ny - 1), qx, qy, r);
 }
 
 // conservative lower bound (squared) on the distance from the query to anything outside the
 // (2k+1)^2 block of cells around cell (cx, cy); +inf when the block covers the whole grid
-__device__ __forceinline__ float nn_block_bound2(const GridView &g, float qx, float qy, int cx, int cy, int k) {
+template <typename Idx>
+__device__ __forceinline__ float nn_block_bound2(const GridViewT<Idx> &g, float qx, float qy, int cx, int cy, int k) {
   const int x0 = cx - k, x1 = cx + k, y0 = cy - k, y1 = cy + k;
   float bound = INFINITY;
   if (x0 > 0) bound = fminf(bound, qx - (g.ox + (float)x0 * g.cell));
@@ -210,7 +221,8 @@ __device__ __forceinline__ float nn_block_bound2(const GridView &g, float qx, fl
 }
 
 // scan the whole (2k+1)^2 block as one contiguous point range per cell row
-__device__ __forceinline__ void nn_scan_block(const GridView &g, int cx, int cy, int k, float qx, float qy, NNResult &r) {
+template <typename Idx>
+__device__ __forceinline__ void nn_scan_block(const GridViewT<Idx> &g, int cx, int cy, int k, float qx, float qy, NNResult &r) {
   const int xa = max(cx - k, 0), xb = min(cx + k, g.nx - 1);
   for (int y = max(cy - k, 0); y <= min(cy + k, g.ny - 1); ++y)
     nn_scan(g, g.cstart[y * g.nx + xa], g.cstart[y * g.nx + xb + 1], qx, qy, r);
@@ -224,7 +236,8 @@ __device__ __forceinline__ void nn_scan_block(const GridView &g, int cx, int cy,
 // scanned as row spans (two offset loads per row), so a query far from every point costs O(k) cell
 // look-ups; once a candidate at distance d exists, one last block of radius ceil(d / cell) + 1 settles it.
 // Re-scanning inner cells is harmless (same candidates, same tie rule).
-__device__ __forceinline__ int nn_search(const GridView &g, float qx, float qy, float max_d2, float stop_d2,
+template <typename Idx>
+__device__ __forceinline__ int nn_search(const GridViewT<Idx> &g, float qx, float qy, float max_d2, float stop_d2,
                                          int k_done, NNResult &r) {
   if (g.n <= 0) return 1;
   const int cx = grid_cell_coord(qx, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(qy, g.oy, g.inv_cell, g.ny);
@@ -282,7 +295,8 @@ __device__ __forceinline__ void nn_update2(float d2, int p, NNResult2 &r) {
   }
 }
 
-__device__ __forceinline__ void nn_scan_block2(const GridView &g, int cx, int cy, int k, float qx, float qy, NNResult2 &r) {
+template <typename Idx>
+__device__ __forceinline__ void nn_scan_block2(const GridViewT<Idx> &g, int cx, int cy, int k, float qx, float qy, NNResult2 &r) {
   const int xa = max(cx - k, 0), xb = min(cx + k, g.nx - 1);
   for (int y = max(cy - k, 0); y <= min(cy + k, g.ny - 1); ++y) {
     const int s = g.cstart[y * g.nx + xa], e = g.cstart[y * g.nx + xb + 1], last = e - 1;
@@ -302,7 +316,8 @@ __device__ __forceinline__ void nn_scan_block2(const GridView &g, int cx, int cy
 }
 
 // exact nearest neighbour (accepted only when d2 <= max_d2, like nn_query) + *lb2
-__device__ __forceinline__ NNResult nn_query_certified(const GridView &g, float qx, float qy, float max_d2, float *lb2) {
+template <typename Idx>
+__device__ __forceinline__ NNResult nn_query_certified(const GridViewT<Idx> &g, float qx, float qy, float max_d2, float *lb2) {
   NNResult out;
   out.d2 = INFINITY, out.pos = -1, out.tie = 0;
   *lb2 = 0.f;
@@ -339,7 +354,8 @@ __device__ __forceinline__ NNResult nn_query_certified(const GridView &g, float 
 // radius d + margin settles the nearest neighbour exactly (as nn_query_seeded does) AND shows that every other
 // point is farther than min(runner-up met, d + margin).  A small margin keeps the scan as narrow as the plain seeded
 // search; the caller sizes it to a few of the point's recent steps, so that one search serves several iterations.
-__device__ __forceinline__ NNResult nn_query_seeded_certified(const GridView &g, float qx, float qy, float max_d2,
+template <typename Idx>
+__device__ __forceinline__ NNResult nn_query_seeded_certified(const GridViewT<Idx> &g, float qx, float qy, float max_d2,
                                                               int seed, float margin, float *lb2) {
   const float2 t = g.pts[seed];
   const float d0 = dist2_rn(qx - t.x, qy - t.y);
@@ -381,7 +397,8 @@ __device__ __forceinline__ NNResult nn_query_seeded_certified(const GridView &g,
 // contiguous point range; a butterfly picks the closest candidate, and ties (equal float32 distance at different
 // positions, within a lane or across lanes) fall back to the exact lowest-original-index rule.  Blocks are nested,
 // so the best of the last block scanned is the best of everything scanned.  Result = nn_search's, on every lane.
-__device__ __forceinline__ void nn_scan_block_warp(const GridView &g, int cx, int cy, int k, float qx, float qy,
+template <typename Idx>
+__device__ __forceinline__ void nn_scan_block_warp(const GridViewT<Idx> &g, int cx, int cy, int k, float qx, float qy,
                                                    NNResult &r) {
   const int lane = threadIdx.x & 31, grp = lane >> 3, sub = lane & 7;
   const int xa = max(cx - k, 0), xb = min(cx + k, g.nx - 1);
@@ -412,7 +429,8 @@ __device__ __forceinline__ void nn_scan_block_warp(const GridView &g, int cx, in
 
 // returns 1: r = exact nearest neighbour (if any within max_d2); 0: every point is farther than sqrt(stop_d2)
 // (r is then not the NN).  `r` may carry a candidate from an earlier partial scan of the block of radius k_done.
-__device__ __forceinline__ int nn_search_warp(const GridView &g, float qx, float qy, float max_d2, float stop_d2,
+template <typename Idx>
+__device__ __forceinline__ int nn_search_warp(const GridViewT<Idx> &g, float qx, float qy, float max_d2, float stop_d2,
                                               int k_done, NNResult &r) {
   if (g.n <= 0) return 1;
   const int cx = grid_cell_coord(qx, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(qy, g.oy, g.inv_cell, g.ny);
@@ -447,7 +465,8 @@ __device__ __forceinline__ int nn_search_warp(const GridView &g, float qx, float
 }
 
 // exact nearest neighbour of (qx,qy); accepted only when d2 <= max_d2
-__device__ __forceinline__ NNResult nn_query(const GridView &g, float qx, float qy, float max_d2) {
+template <typename Idx>
+__device__ __forceinline__ NNResult nn_query(const GridViewT<Idx> &g, float qx, float qy, float max_d2) {
   NNResult r;
   r.d2 = INFINITY;
   r.pos = -1;
@@ -464,7 +483,8 @@ __device__ __forceinline__ NNResult nn_query(const GridView &g, float qx, float 
 // The candidate's distance d bounds the answer, so only the cells that overlap the disc of radius d around the
 // query can hold the nearest neighbour or a tie with it -- typically 1-4 cells instead of the 3x3 block and its
 // successors.  The result (position, distance, tie rule) is the same as nn_query's.
-__device__ __forceinline__ NNResult nn_query_seeded(const GridView &g, float qx, float qy, float max_d2, int seed) {
+template <typename Idx>
+__device__ __forceinline__ NNResult nn_query_seeded(const GridViewT<Idx> &g, float qx, float qy, float max_d2, int seed) {
   const float2 t = g.pts[seed];
   const float d0 = dist2_rn(qx - t.x, qy - t.y);
   if (!(d0 <= max_d2)) return nn_query(g, qx, qy, max_d2);  // the seed itself is not acceptable any more (or NaN)
@@ -488,7 +508,8 @@ __device__ __forceinline__ NNResult nn_query_seeded(const GridView &g, float qx,
 // shared memory that is idle while the normals are computed (stride = CTA size, one column per thread): a list in
 // local memory spills past the little L1 that a CTA's shared-memory carve-out leaves, so local arrays (stride 1) are only the fallback for CTAs without that room.
 constexpr int GRID_KNN_MAX = 16;
-__device__ inline float2 grid_surface_normal(const GridView &g, int p, int knn, float *bd, uint16_t *bi, int stride) {
+template <typename Idx, typename B>
+__device__ inline float2 grid_surface_normal(const GridViewT<Idx> &g, int p, int knn, float *bd, B *bi, int stride) {
   const float2 q = g.pts[p];
   const int cx = grid_cell_coord(q.x, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(q.y, g.oy, g.inv_cell, g.ny);
   int k = 0;
@@ -504,7 +525,7 @@ __device__ inline float2 grid_surface_normal(const GridView &g, int p, int knn, 
         bd[at * stride] = bd[(at - 1) * stride], bi[at * stride] = bi[(at - 1) * stride];
         --at;
       }
-      bd[at * stride] = d2, bi[at * stride] = (uint16_t)j;
+      bd[at * stride] = d2, bi[at * stride] = (B)j;
       if (k == knn) kth = bd[(k - 1) * stride];
     }
   };

@@ -19,6 +19,11 @@
 // CTAs are persistent over the problem list (batch of keyframe pairs / of initial guesses).
 #include <algorithm>
 #include <mutex>
+#include <type_traits>
+
+#include <climits>
+
+#include <cub/cub.cuh>
 
 #include "grid.cuh"
 #include "stages.cuh"
@@ -37,6 +42,14 @@ constexpr float ICP_PRUNED = 3.0e38f;    // "finite, but farther than we needed 
 
 enum { ICP_OK = 0, ICP_NO_OUTLIER = 1, ICP_NO_POINT = 2, ICP_NAN_ROT = 3, ICP_NAN_TRANS = 4, ICP_NOT_RIGID = 5,
        ICP_EMPTY_REF = 6, ICP_SKIPPED = 7, ICP_TOO_LARGE = 8 };
+
+// One map grid: a target cloud too large for the in-CTA layout, built once per call in global memory (map_build).
+struct MapGrid {
+  float mean[2];  // reference mean (the kernel's sequential float32 sum; 0 for match)
+  float bbox[4];  // bounding box of the centred points
+  float ox, oy, cell, inv_cell;
+  int nx, ny, n, pad;
+};
 
 struct IcpBatch {
   const float *src_pts;
@@ -68,6 +81,18 @@ struct IcpBatch {
   int slot_by_smid;   // workspace slot = %smid (one CTA per SM, one CTA per problem) instead of blockIdx.x
   int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
 };
+
+// The map class (icp_map_kernel): problem p reads its target from the grid in slot map_slot[p] (map_build)
+struct IcpMapArgs {
+  const int *map_slot;
+  const MapGrid *map_grid;
+  const float2 *map_pts;   // centred points of every slot, sorted by (slot, cell)
+  const int *map_cstart;   // [slot][map_cell_cap]: absolute position in map_pts of every cell's first point
+  const int *map_orig;     // sorted position -> index in the target cloud
+  const float2 *map_nrm;   // point-to-plane: normal at every sorted position
+  int map_cell_cap;
+};
+
 
 // Per-phase cycle counts (development build, -DSFE_ICP_PHASE_CLOCKS; tools/build_icp_variants.sh, tools/icp_phases.py):
 // thread 0 of every CTA reads clock64() at the phase boundaries below and adds its totals to a global array when the
@@ -340,8 +365,8 @@ __device__ __forceinline__ float seq_sum4_warp(int n, float *scratch, F term4) {
 // (a gather from global memory, ~700 cycles) requested for eight batches at once so that its latency is paid once
 // per 256 points, not once per batch.  `scratch` = 2 x 320 floats (nine rows 36 floats apart, 32 used).  term9(i, m, n, v): the nine terms of kept
 // pair i (match m, normal n).  Lane c (c < 9) returns the sum of component c.
-template <typename F>
-__device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const uint16_t *match, const float2 *nrm, F term9) {
+template <int NONE, typename Pos, typename F>
+__device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const Pos *match, const float2 *nrm, F term9) {
   const int lane = threadIdx.x & 31;
   float s = 0.f;
   int it = 0;
@@ -351,8 +376,8 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const uint
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const int i = chunk + 32 * k + lane;
-      mm[k] = i < n ? match[i] : 0xffff;
-      nn[k] = mm[k] != 0xffff ? nrm[mm[k]] : make_float2(0.f, 0.f);
+      mm[k] = i < n ? match[i] : NONE;
+      nn[k] = mm[k] != NONE ? nrm[mm[k]] : make_float2(0.f, 0.f);
     }
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -360,7 +385,7 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const uint
       float *buf = scratch + (it & 1) * 320;
       ++it;
       float v[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (mm[k] != 0xffff) term9(chunk + 32 * k + lane, mm[k], nn[k], v);
+      if (mm[k] != NONE) term9(chunk + 32 * k + lane, mm[k], nn[k], v);
 #pragma unroll
       for (int c = 0; c < 9; ++c) buf[c * 36 + lane] = v[c];
       __syncwarp();
@@ -413,771 +438,24 @@ __device__ __forceinline__ float seq_sum_warp_global(const float *p, int n, int 
 // __launch_bounds__(512) build capped the 128-thread class at 64 registers and spilled).
 // PLANE: errorMinimizer = PointToPlaneErrorMinimizer (sfe_icp_params.minimizer 1); a separate instantiation so that
 // the shipped point-to-point kernels keep their register allocation.
+// MAP: the target is a map grid in global memory (icp_map_kernel): no set-up per problem, 32-bit target positions,
+// and shared memory holds IcpShared and the source arrays only.
+// The kernel body lives in icp_kernel_body.cuh and is included into both kernels below, so that each kernel's code is
+// the body itself: behind a device-function wrapper the shipped instantiations compiled with larger stack frames.  The
+// body reads `MAP` (a value-dependent constant, so the other class's branches are discarded per instantiation) and,
+// in the map class, the map arguments `mp`.
 template <int THREADS, int MINB, bool PLANE>
 __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match u16 ns_max]
-  //         [prev u16 ns_max][qstate u8 ns_max][slack f32 ns_max][order u16 ns_max]
-  IcpShared &sh = *reinterpret_cast<IcpShared *>(smem_raw);
-  size_t off = (sizeof(IcpShared) + 15) & ~size_t(15);
-  float2 *sorted = reinterpret_cast<float2 *>(smem_raw + off);
-  off += sizeof(float2) * (size_t)b.nt_max;
-  uint32_t *cells = reinterpret_cast<uint32_t *>(smem_raw + off);
-  off += sizeof(uint32_t) * (size_t)((b.max_cells + 2) / 2 + 1);
-  off = (off + 7) & ~size_t(7);
-  float2 *reading = reinterpret_cast<float2 *>(smem_raw + off);
-  off += sizeof(float2) * (size_t)b.ns_max;
-  float *dist = reinterpret_cast<float *>(smem_raw + off);
-  off += sizeof(float) * (size_t)b.ns_max;
-  uint16_t *match = reinterpret_cast<uint16_t *>(smem_raw + off);
-  off += sizeof(uint16_t) * (size_t)b.ns_max;
-  uint16_t *prev = reinterpret_cast<uint16_t *>(smem_raw + off);  // NN of the previous iteration (search seed)
-  off += sizeof(uint16_t) * (size_t)b.ns_max;
-  uint8_t *qstate = reinterpret_cast<uint8_t *>(smem_raw + off);
-  off += ((size_t)b.ns_max + 3) & ~size_t(3);
-  // certified-match margin per source point (metres): every target point other than prev[i] is farther from the
-  // point's current position than (distance to prev[i]) as long as that distance stays below slack[i]
-  float *slack = reinterpret_cast<float *>(smem_raw + off);
-  off += sizeof(float) * (size_t)b.ns_max;
-  // processing order of the source points in the search passes: sorted by a coarse cell of the target grid, so that
-  // the lanes of a warp look at neighbouring cells (similar amounts of work, the same shared-memory lines); results
-  // are stored by point index and the sums run in point order, so the order is invisible in the results
-  uint16_t *order = reinterpret_cast<uint16_t *>(smem_raw + off);
-  if (b.use_order) off += sizeof(uint16_t) * (size_t)b.ns_max;
-  off = (off + 15) & ~size_t(15);
-  // PLANE only: 640 floats for seq_sum9_warp.  dist[] is dead between the weights (3c) and the next iteration's
-  // search, which rewrites all of it: launches with room for 640 source points (the front end's small class is
-  // exactly that; 2 000 x 20 000 points leave nothing to spare at all) park the scratch there, smaller ones get
-  // their own 2.5 KB.
-  float *pl_scratch = b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
-  (void)pl_scratch;
+  constexpr bool MAP = THREADS < 0;  // false
+  constexpr IcpMapArgs mp{};         // (named by the discarded map-class branches only)
+#include "icp_kernel_body.cuh"
+}
 
-  const int tid = threadIdx.x, nthr = blockDim.x;
-  ICP_PH_DECL
-  int red_phase = 0, tot_phase = 0, sel_pass = 0;  // rotation counters of the one-barrier reductions (CTA-uniform)
-  for (int h = threadIdx.x; h < 3 * 256; h += blockDim.x) (&sh.hist[0][0])[h] = 0;
-  // Problems that allow one CTA per SM (config 3: ~200 KB of shared memory) are launched one CTA per problem, not
-  // as persistent CTAs: problems of unequal length (checker mode: 4-40 iterations) balance themselves, and SMs
-  // free up every few milliseconds so that concurrent NCCL send/recv kernels (the config-5 scatter) get scheduled.
-  // The per-CTA global workspace is then indexed by the SM the CTA runs on.
-  const unsigned slot = b.slot_by_smid ? icp_smid() : blockIdx.x;
-  if (b.slot_by_smid && slot >= ICP_SM_SLOTS) __trap();
-  uint16_t *orig = b.orig_ws + (size_t)slot * b.nt_max;
-  const sfe_icp_params prm = b.prm;
-  const float max_d2 = __fmul_rn(prm.matcher_max_dist, prm.matcher_max_dist);
-  const float out_d2 = (prm.flags & 1) ? prm.outlier_max_dist : __fmul_rn(prm.outlier_max_dist, prm.outlier_max_dist);
-  const int smooth = min(prm.smooth_length, ICP_HIST - 1);
-  // Default: every sum over points is a sequential float32 sum in point order, as in oracle/icp_ref.c -- results
-  // are bit-identical to the oracle.  flags bit 1: float32 terms accumulated in float64 (order-independent,
-  // ~1e-4 closer to exact arithmetic; deviates from the oracle by up to ~2e-3 m on
-  // ill-conditioned scans because the float32-sequential sums themselves are that noisy).
-  const bool seq = (prm.flags & 2) == 0;
-
-  // Persistent CTAs take problems from a work counter: problems differ in length (cloud sizes, early exits), and with
-  // a static share the batch ends when the CTAs that drew the most work finish.  Problem p's results do not depend
-  // on the CTA that solves it.  The index is broadcast through sh.status, which thread 0 rewrites only after the
-  // next problem's first barrier.
-  for (int p = blockIdx.x; p < b.P; p = b.next ? next_work_item(b.next, &sh.status) : p + (int)gridDim.x) {
-    const int si = b.src_id ? b.src_id[p] : p, ti = b.tgt_id ? b.tgt_id[p] : p;
-    const float *src = b.src_pts + 2 * (size_t)b.src_off[si];
-    const int ns = b.src_cnt ? b.src_cnt[si] : b.src_off[si + 1] - b.src_off[si];
-    const float *tgt = b.tgt_pts + 2 * (size_t)b.tgt_off[ti];
-    const int nt = b.tgt_cnt ? b.tgt_cnt[ti] : b.tgt_off[ti + 1] - b.tgt_off[ti];
-    const float *guess = b.guess + 9 * (size_t)p;
-    if (b.class_mode == 1 && (ns > b.ns_max || nt > b.nt_max)) continue;
-    if (b.class_mode == 2 && ns <= b.class_ns && nt <= b.class_nt) continue;
-    __syncthreads();  // previous problem fully retired before shared state is reused
-
-    // ---- admission checks (thread 0), failure leaves T = guess
-    if (tid == 0) {
-      int st = ICP_OK;
-      if (ns > b.ns_max || nt > b.nt_max || (b.raw_cnt && b.raw_cnt[si] > b.raw_cap)) st = ICP_TOO_LARGE;
-      else if (ns < b.min_points || nt < b.min_points) st = ICP_SKIPPED;
-      else if (nt <= 0) st = ICP_EMPTY_REF;
-      const float det = __fsub_rn(__fmul_rn(guess[0], guess[4]), __fmul_rn(guess[1], guess[3]));
-      if (st == ICP_OK && (!(fabsf(__fsub_rn(1.0f, det)) <= 0.001f))) st = ICP_NOT_RIGID;
-      sh.status = st;
-      sh.count = 0, sh.inliers = 0;
-    }
-    __syncthreads();
-    if (sh.status != ICP_OK) {
-      if (tid < 9) b.T_out[9 * (size_t)p + tid] = guess[tid];
-      if (tid == 0) b.iters[p] = 0, b.inliers[p] = 0, b.status[p] = sh.status;
-      continue;
-    }
-
-    ICP_PH_START();
-    // ---- 1. mean of the reference, bounding box of the centred reference
-    {
-      float mx, my;
-      if (seq) {
-        if (tid < 64) {  // warps 0 and 1: x and y
-          const float sum = seq_sum_warp_global(tgt + (tid >> 5), nt, 2);
-          if ((tid & 31) == 0) sh.seq[tid >> 5] = __fdiv_rn(sum, (float)nt);
-        }
-        __syncthreads();
-        mx = sh.seq[0], my = sh.seq[1];
-      } else {
-        double s[2] = {0.0, 0.0}, tot[2];
-        for (int i = tid; i < nt; i += nthr) s[0] += (double)tgt[2 * i], s[1] += (double)tgt[2 * i + 1];
-        block_sum<2>(s, sh.red, red_phase, tot);
-        mx = (float)(tot[0] / (double)nt), my = (float)(tot[1] / (double)nt);
-      }
-      float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
-      for (int i = tid; i < nt; i += nthr) {
-        const float x = tgt[2 * i] - mx, y = tgt[2 * i + 1] - my;
-        mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
-      }
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) {
-        mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
-        mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
-        mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
-        mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
-      }
-      float *fr = sh.wred;
-      if ((tid & 31) == 0) {
-        fr[(tid >> 5) * 4 + 0] = mn_x, fr[(tid >> 5) * 4 + 1] = mn_y;
-        fr[(tid >> 5) * 4 + 2] = mxx, fr[(tid >> 5) * 4 + 3] = mxy;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
-        for (int w = 0; w < (nthr >> 5); ++w) {
-          a = fminf(a, fr[w * 4 + 0]), bb = fminf(bb, fr[w * 4 + 1]);
-          c = fmaxf(c, fr[w * 4 + 2]), d = fmaxf(d, fr[w * 4 + 3]);
-        }
-        sh.bbox[0] = a, sh.bbox[1] = bb, sh.bbox[2] = c, sh.bbox[3] = d;
-        sh.mean[0] = mx, sh.mean[1] = my;
-      }
-      __syncthreads();
-    }
-    const float mx = sh.mean[0], my = sh.mean[1];
-    GridView g;
-    grid_geometry(nt, sh.bbox[0], sh.bbox[1], sh.bbox[2], sh.bbox[3], 0.05f, g, b.max_cells, b.cell_scale);
-    grid_build(tgt, 2, nt, mx, my, g, sorted, cells, orig, sh.scan);
-    // coarse occupancy: which 8x8 blocks of cells hold any point (answers "is anything within maxDist?"
-    // for far-away source points without walking the fine grid)
-    {
-      const int cnx = (g.nx + ICP_COARSE - 1) / ICP_COARSE, cny = (g.ny + ICP_COARSE - 1) / ICP_COARSE;
-      if (tid == 0) sh.cnx = cnx, sh.cny = cny;
-      for (int w = tid; w < ICP_COARSE_WORDS; w += nthr) sh.coarse[w] = 0;
-      __syncthreads();
-      if (cnx * cny <= ICP_COARSE_WORDS * 32) {
-        for (int cc = tid; cc < cnx * cny; cc += nthr) {
-          const int ccy = cc / cnx, ccx = cc - ccy * cnx;
-          bool occ = false;
-          for (int y = ccy * ICP_COARSE; y < min((ccy + 1) * ICP_COARSE, g.ny) && !occ; ++y) {
-            const int xa = ccx * ICP_COARSE, xb = min((ccx + 1) * ICP_COARSE, g.nx);
-            occ = g.cstart[y * g.nx + xb] > g.cstart[y * g.nx + xa];
-          }
-          if (occ) atomicOr(&sh.coarse[cc >> 5], 1u << (cc & 31));
-        }
-      } else if (tid == 0) {
-        sh.cnx = 0;  // too many coarse cells: the test is skipped
-      }
-      __syncthreads();
-    }
-
-    // ---- 1b. point-to-plane: normals of the (centred) target, one thread per sorted position, kept in global
-    // memory (8 B per target point; the iterations gather them through L2)
-    float2 *nrm = nullptr;
-    if constexpr (PLANE) {
-      nrm = b.nrm_ws + (size_t)slot * b.nt_max;
-      const int knn = min(max(prm.normals_knn, 1), GRID_KNN_MAX);
-      // best-knn list per thread: the per-source arrays (reading .. slack) are idle until step 2
-      unsigned char *scr = reinterpret_cast<unsigned char *>(reading);
-      const size_t scr_bytes = (size_t)(reinterpret_cast<unsigned char *>(slack + b.ns_max) - scr);
-      if (scr_bytes >= (size_t)nthr * knn * 6) {
-        float *bd = reinterpret_cast<float *>(scr) + tid;
-        uint16_t *bi = reinterpret_cast<uint16_t *>(scr + sizeof(float) * (size_t)nthr * knn) + tid;
-        for (int j = tid; j < nt; j += nthr) nrm[j] = grid_surface_normal(g, j, knn, bd, bi, nthr);
-      } else {
-        float bd[GRID_KNN_MAX];
-        uint16_t bi[GRID_KNN_MAX];
-        for (int j = tid; j < nt; j += nthr) nrm[j] = grid_surface_normal(g, j, knn, bd, bi, 1);
-      }
-      // (published to the CTA, and the scratch released, by the barriers of step 2)
-    }
-
-    // ---- 2. reading into the centred frame; T_iter = I; checker history
-    if (tid == 0) {
-      const float Tinv[9] = {1.f, 0.f, -mx, 0.f, 1.f, -my, 0.f, 0.f, 1.f};
-      float T0[9];
-      mat3_mul_rn(Tinv, guess, T0);
-#pragma unroll
-      for (int i = 0; i < 9; ++i) sh.T0[i] = T0[i], sh.Ti[i] = sh.Tprev[i] = (i % 4 == 0) ? 1.f : 0.f;
-      rot_to_quat(sh.Ti, sh.hq_w[0], sh.hq_z[0]);
-      sh.ht_x[0] = 0.f, sh.ht_y[0] = 0.f;
-      sh.hn = 1;
-      sh.iterate = 1;
-      sh.todo_n = 0;
-    }
-    __syncthreads();
-    for (int i = tid; i < ns; i += nthr) {
-      reading[i] = apply_T(sh.T0, src[2 * i], src[2 * i + 1]);
-      prev[i] = 0xffff;
-      slack[i] = 0.f;
-    }
-    __syncthreads();
-    if (b.use_order) {  // counting sort of the point indices by a 16 x 16 bucket grid over the target's bounding box.  Counters: the
-       // radix-select histogram that the next selection pass neither fills nor expects to be clear (pass p fills
-       // hist[p % 3] and clears hist[(p + 1) % 3]; hist[(p + 2) % 3] is cleared by pass p + 1 before it is used)
-      int *cnt = sh.hist[(sel_pass + 2) % 3];
-      for (int h = tid; h < 256; h += nthr) cnt[h] = 0;
-      __syncthreads();
-      const float bw = fmaxf(sh.bbox[2] - sh.bbox[0], 1e-6f) * (1.f / 16.f), bh = fmaxf(sh.bbox[3] - sh.bbox[1], 1e-6f) * (1.f / 16.f);
-      auto bucket = [&](int i) {
-        const int bx = min(max((int)((reading[i].x - sh.bbox[0]) / bw), 0), 15);
-        const int by = min(max((int)((reading[i].y - sh.bbox[1]) / bh), 0), 15);
-        return by * 16 + bx;
-      };
-      for (int i = tid; i < ns; i += nthr) atomicAdd(&cnt[bucket(i)], 1);
-      __syncthreads();
-      if (tid < 32) {  // exclusive scan of the 256 counters by one warp (8 per lane)
-        int c[8], sum = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) c[j] = cnt[tid * 8 + j], sum += c[j];
-        int incl = sum;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const int t = __shfl_up_sync(0xffffffffu, incl, d);
-          if (tid >= d) incl += t;
-        }
-        int run = incl - sum;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) cnt[tid * 8 + j] = run, run += c[j];
-      }
-      __syncthreads();
-      for (int i = tid; i < ns; i += nthr) order[atomicAdd(&cnt[bucket(i)], 1)] = (uint16_t)i;
-      __syncthreads();
-    }
-
-    ICP_PH_MARK(0);
-    // ---- 3. iterations
-    while (true) {
-      float Ti[9];
-#pragma unroll
-      for (int i = 0; i < 9; ++i) Ti[i] = sh.Ti[i];
-      // 3a. match.  Exact nearest neighbours are only needed for the pairs that can get a non-zero weight:
-      //   pass A  every source point scans its 3x3 block of cells: that either settles its nearest neighbour
-      //           or at least yields a candidate, i.e. an UPPER bound on its NN distance;
-      //   pass B  points without a candidate inside maxDist learn whether ANY target point lies within
-      //           maxDist (they then count as "finite" in the trimmed quantile) -- from the coarse
-      //           occupancy grid when that is conclusive, else from a search that stops at the first hit;
-      //   pass C  with n_finite known, kk = floor(n_finite * ratio).  The kk-th smallest of the upper bounds
-      //           (maxDist^2 for a finite point without candidate) bounds the kk-th smallest true distance
-      //           from above: call it U.  An unsettled point whose search proves "farther than U" has weight
-      //           0 and needs no exact distance.  Results are identical to an exhaustive search (same
-      //           quantile element, same kept pairs); the far outliers of a scan stop costing O(area).
-      int n_fin = 0, total_fin = -1;
-      const bool small = ns <= b.small_mult * nthr && nt <= 4096;  // few, cheap searches: one exact pass, no pruning
-      // Certified matches.  A search that scans at least the 3x3 block also yields a lower bound L on the distance
-      // from the point to every target point OTHER than its match (grid.cuh: nn_query_certified).  The point then
-      // moves a little every iteration; by the triangle inequality every other target point stays farther than
-      // L - (path length since).  slack[i] holds that margin, shrunk by safety terms far above float32 rounding:
-      // while the distance to the old match is below it, the old match is the unique nearest neighbour -- the
-      // answer an exhaustive search would give, ties impossible -- and costs one distance instead of a search.
-      // Used for the small problems of the front end (window submaps thinned to 0.5 m: runner-ups are decimetres
-      // away and a certificate lasts several iterations).
-      float Tp[9];
-#pragma unroll
-      for (int i = 0; i < 9; ++i) Tp[i] = sh.Tprev[i];
-      auto certified = [&](int i, const float2 q, int seed, float &d2_out, float &step) -> bool {
-        const float2 qo = apply_T(Tp, reading[i].x, reading[i].y);
-        step = sqrtf(dist2_rn(q.x - qo.x, q.y - qo.y));
-        const float sl = slack[i] - (step * 1.00001f + 2e-5f);
-        slack[i] = sl;
-        const float2 t = sorted[seed];
-        const float d2 = dist2_rn(q.x - t.x, q.y - t.y);
-        d2_out = d2;
-        return d2 <= max_d2 && sqrtf(d2) * 1.00001f + 1e-4f < sl;
-      };
-      auto certify = [&](int i, float lb2) {  // margin after a certifying search
-        slack[i] = lb2 < 3.0e38f ? sqrtf(lb2) * 0.99999f - 1e-4f : 3.0e38f;
-      };
-      // certificate size: a few of the point's steps (steps shrink as the scan converges), a fraction of a cell at most
-      auto margin_for = [&](float step) { return fminf(fmaxf(b.margin_mult * step, 0.01f * g.cell), 0.35f * g.cell); };
-      if (small) {
-        if constexpr (THREADS <= 256) {
-          // Two halves, so that the lanes of a warp stay on one code path.  First every point tests its certificate
-          // (one distance; points without a seed search at once: that is the first iteration, all lanes together);
-          // the points whose certificate failed are only LISTED -- in match[], which the weights (3c) rewrite from
-          // prev[], with the counter in todo_n (zeroed by the single-thread step of the previous iteration).  Then the
-          // list is searched densely.  In one loop the re-search ran with 2.4 of 32 lanes active and took 25 % of this
-          // kernel's warp instructions on the front end's problems (tools/ncu_call_sites.py).
-          uint16_t *todo = match;
-          for (int base = 0; base < ns; base += nthr) {
-            const int ii = base + tid;
-            bool later = false;
-            int i = 0;
-            if (ii < ns) {
-              i = b.use_order ? order[ii] : ii;
-              const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-              const int seed = prev[i];
-              float d2s, step, lb2;
-              if (seed == 0xffff) {
-                const NNResult r = nn_query_certified(g, q.x, q.y, max_d2, &lb2);
-                certify(i, lb2);
-                dist[i] = r.d2;
-                prev[i] = r.pos >= 0 ? (uint16_t)r.pos : (uint16_t)0xffff;
-                n_fin += r.pos >= 0;
-              } else if (certified(i, q, seed, d2s, step)) {
-                dist[i] = d2s;  // prev[i] stays
-                n_fin += 1;
-              } else {
-                later = true;
-              }
-            }
-            const unsigned m = __ballot_sync(0xffffffffu, later);
-            if (m) {  // one shared-memory atomic per warp
-              const int lane = tid & 31, lead = __ffs(m) - 1;
-              int at = 0;
-              if (lane == lead) at = atomicAdd(&sh.todo_n, __popc(m));
-              at = __shfl_sync(0xffffffffu, at, lead);
-              if (later) todo[at + __popc(m & ((1u << lane) - 1u))] = (uint16_t)i;
-            }
-          }
-          __syncthreads();
-          const int n_todo = sh.todo_n;
-          for (int k = tid; k < n_todo; k += nthr) {
-            const int i = todo[k];
-            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-            const float2 qo = apply_T(Tp, reading[i].x, reading[i].y);
-            const float step = sqrtf(dist2_rn(q.x - qo.x, q.y - qo.y));
-            float lb2;
-            const NNResult r = nn_query_seeded_certified(g, q.x, q.y, max_d2, prev[i], margin_for(step), &lb2);
-            certify(i, lb2);
-            dist[i] = r.d2;
-            prev[i] = r.pos >= 0 ? (uint16_t)r.pos : (uint16_t)0xffff;
-            n_fin += r.pos >= 0;
-          }
-          // the matches are prev[] now (3c reads them there); this barrier also publishes prev[] and dist[]
-          total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);
-        } else {
-          // (512-thread CTAs rarely see a problem this small: the single loop is kept there, and with it the code of the
-          //  config-3 instantiation)
-          for (int ii = tid; ii < ns; ii += nthr) {
-            const int i = b.use_order ? order[ii] : ii;
-            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-            const int seed = prev[i];
-            NNResult r;
-            float d2s, step, lb2;
-            if (seed == 0xffff) {
-              r = nn_query_certified(g, q.x, q.y, max_d2, &lb2);
-              certify(i, lb2);
-            } else if (certified(i, q, seed, d2s, step)) {
-              r.d2 = d2s, r.pos = seed, r.tie = 0;
-            } else {
-              r = nn_query_seeded_certified(g, q.x, q.y, max_d2, seed, margin_for(step), &lb2);
-              certify(i, lb2);
-            }
-            dist[i] = r.d2;
-            match[i] = prev[i] = r.pos >= 0 ? (uint16_t)r.pos : (uint16_t)0xffff;
-            n_fin += r.pos >= 0;
-          }
-        }
-      }
-      const float stop_a = (0.999f * g.cell) * (0.999f * g.cell);
-      for (int ii = tid; ii < ns && !small; ii += nthr) {
-        const int i = b.use_order ? order[ii] : ii;
-        const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-        NNResult r;
-        r.d2 = INFINITY, r.pos = -1, r.tie = 0;
-        int exact;
-        const int seed = prev[i];
-        // (no certificates here: a 20 000-point target puts the runner-up a centimetre from the match, so a
-        // certificate rarely outlives an iteration, and checking it costs more than it saves)
-        const float2 ts = sorted[seed != 0xffff ? seed : 0];
-        if (seed != 0xffff && dist2_rn(q.x - ts.x, q.y - ts.y) <= stop_a) {
-          r = nn_query_seeded(g, q.x, q.y, max_d2, seed);  // last iteration's match is still close: settle it now
-          exact = 1;
-        } else {
-          exact = nn_search(g, q.x, q.y, max_d2, stop_a, -1, r);  // own cell, then at most the 3x3 block
-        }
-        if (exact) prev[i] = (r.pos >= 0 && r.d2 <= max_d2) ? (uint16_t)r.pos : (uint16_t)0xffff;
-        const bool fin = r.pos >= 0 && r.d2 <= max_d2;
-        dist[i] = fin ? r.d2 : INFINITY;
-        match[i] = fin ? (uint16_t)r.pos : (uint16_t)0xffff;
-        qstate[i] = (exact ? 1 : 0) | (fin ? 2 : 0) | ((fin || exact) ? 4 : 0);  // settled / finite / known
-        n_fin += fin;
-      }
-      // pass B: finiteness of the points that have no candidate yet
-      for (int ii = tid; ii < ns && !small; ii += nthr) {
-        const int i = b.use_order ? order[ii] : ii;
-        if (qstate[i] & 4) continue;
-        const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-        int verdict = -1;  // 1 finite, 0 not, -1 unknown
-        if (sh.cnx > 0) {
-          const float C = g.cell * (float)ICP_COARSE, rad = prm.matcher_max_dist;
-          const int xa = max(0, (int)floorf((q.x - rad - g.ox) / C) - 1), xb = min(sh.cnx - 1, (int)floorf((q.x + rad - g.ox) / C) + 1);
-          const int ya = max(0, (int)floorf((q.y - rad - g.oy) / C) - 1), yb = min(sh.cny - 1, (int)floorf((q.y + rad - g.oy) / C) + 1);
-          if (xa > xb || ya > yb) {
-            verdict = 0;
-          } else if ((xb - xa + 1) * (yb - ya + 1) <= 256) {
-            const float r_in = rad * (1.f - 1e-4f) - g.cell * 1e-3f, r_out = rad * (1.f + 1e-4f) + g.cell * 1e-3f;
-            bool any_maybe = false;
-            for (int cy2 = ya; cy2 <= yb && verdict != 1; ++cy2)
-              for (int cx2 = xa; cx2 <= xb; ++cx2) {
-                const int cc = cy2 * sh.cnx + cx2;
-                if (!((sh.coarse[cc >> 5] >> (cc & 31)) & 1u)) continue;
-                const float x0 = g.ox + (float)cx2 * C, x1 = x0 + C, y0 = g.oy + (float)cy2 * C, y1 = y0 + C;
-                const float nx_ = fmaxf(fmaxf(x0 - q.x, q.x - x1), 0.f), ny_ = fmaxf(fmaxf(y0 - q.y, q.y - y1), 0.f);
-                const float fx_ = fmaxf(fabsf(x0 - q.x), fabsf(x1 - q.x)), fy_ = fmaxf(fabsf(y0 - q.y), fabsf(y1 - q.y));
-                if (fx_ * fx_ + fy_ * fy_ <= r_in * r_in) {
-                  verdict = 1;  // an occupied block lies entirely inside the acceptance disc
-                  break;
-                }
-                if (nx_ * nx_ + ny_ * ny_ <= r_out * r_out) any_maybe = true;
-              }
-            if (verdict != 1 && !any_maybe) verdict = 0;
-          }
-        }
-        if (verdict < 0) {  // inconclusive: grow the block until the first point inside maxDist shows up
-          NNResult r;
-          r.d2 = INFINITY, r.pos = -1, r.tie = 0;
-          const int cx = grid_cell_coord(q.x, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(q.y, g.oy, g.inv_cell, g.ny);
-          const int kmax = max(g.nx, g.ny);
-          verdict = 0;
-          for (int k = 2;; k = min(2 * k, kmax)) {
-            nn_scan_block(g, cx, cy, k, q.x, q.y, r);
-            if (r.d2 <= max_d2) {
-              verdict = 1;
-              break;
-            }
-            const float b2 = nn_block_bound2(g, q.x, q.y, cx, cy, k);
-            if (b2 == INFINITY || b2 > max_d2 || k >= kmax) break;
-          }
-        }
-        qstate[i] |= 4 | (verdict ? 2 : 0) | (verdict ? 0 : 1);  // "nothing within maxDist" is a settled answer
-        n_fin += verdict;
-        dist[i] = verdict ? max_d2 : INFINITY;  // upper bound of a finite point without candidate
-      }
-      if (total_fin < 0) total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);  // (its barrier also publishes dist[] / qstate[])
-      // pass C: settle what still matters
-      if (!small) {
-        float stop_d2 = INFINITY;
-        if (prm.trim_ratio >= 0.f) {
-          if (prm.trim_ratio < 1.0f && total_fin > 0) {
-            int kk = (int)(size_t)__fmul_rn((float)total_fin, prm.trim_ratio);
-            if (kk >= total_fin) kk = total_fin - 1;
-            stop_d2 = block_select_kth(dist, ns, kk, sh, sel_pass);  // kk-th smallest upper bound >= kk-th smallest distance
-          }
-        } else if (prm.outlier_max_dist > 0.f) {
-          stop_d2 = out_d2;
-        }
-        // the unsettled points are few (the scan's outliers) and their searches long: every warp takes the
-        // unsettled points of its 32 lanes one after the other and searches for each with all 32 lanes
-        for (int i0 = tid & ~31; i0 < ns; i0 += nthr) {
-          const int i = i0 + (tid & 31) < ns ? (b.use_order ? (int)order[i0 + (tid & 31)] : i0 + (tid & 31)) : ns;
-          const bool mine = i < ns && !(qstate[i] & 1);
-          float2 q = make_float2(0.f, 0.f);
-          int cand = -1;
-          float cand_d2 = INFINITY;
-          if (mine) {
-            q = apply_T(Ti, reading[i].x, reading[i].y);
-            cand = match[i] == 0xffff ? -1 : (int)match[i];
-            cand_d2 = cand >= 0 ? dist[i] : INFINITY;
-          }
-          unsigned todo = __ballot_sync(0xffffffffu, mine);
-          while (todo) {
-            const int L = __ffs(todo) - 1;
-            todo &= todo - 1;
-            const float qx = __shfl_sync(0xffffffffu, q.x, L), qy = __shfl_sync(0xffffffffu, q.y, L);
-            NNResult r;
-            r.pos = __shfl_sync(0xffffffffu, cand, L);
-            r.d2 = __shfl_sync(0xffffffffu, cand_d2, L);
-            r.tie = 1;  // pass A did not resolve ties; a block scan below replaces this flag with what it finds
-            const int exact = nn_search_warp(g, qx, qy, max_d2, stop_d2, 1, r);
-            if ((tid & 31) == L) {
-              if (exact) {
-                const bool fin = r.pos >= 0 && r.d2 <= max_d2;  // == the finiteness found in pass B
-                dist[i] = fin ? r.d2 : INFINITY;
-                match[i] = prev[i] = fin ? (uint16_t)r.pos : (uint16_t)0xffff;
-              } else {
-                dist[i] = ICP_PRUNED;  // finite, farther than the quantile bound: weight 0
-                match[i] = 0xffff;
-              }
-            }
-          }
-        }
-        __syncthreads();
-      }
-
-      ICP_PH_MARK(1);
-      // 3b. trimmed-distance limit = element floor(float(n)*ratio) of the ascending finite distances
-      float limit = INFINITY;
-      if (prm.trim_ratio >= 0.f) {
-        if (total_fin == 0) {
-          if (tid == 0) sh.status = ICP_NO_OUTLIER;
-          __syncthreads();
-          break;
-        }
-        if (prm.trim_ratio == 1.0f) {
-          float m = 0.f;
-          for (int i = tid; i < ns; i += nthr)
-            if (dist[i] < INFINITY) m = fmaxf(m, dist[i]);
-#pragma unroll
-          for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
-          float *fr = sh.wred;
-          if ((tid & 31) == 0) fr[tid >> 5] = m;
-          __syncthreads();
-          m = 0.f;
-          for (int w = 0; w < (nthr >> 5); ++w) m = fmaxf(m, fr[w]);
-          limit = m;
-          __syncthreads();
-        } else {
-          int kk = (int)(size_t)__fmul_rn((float)total_fin, prm.trim_ratio);
-          if (kk >= total_fin) kk = total_fin - 1;
-          limit = block_select_kth(dist, ns, kk, sh, sel_pass);
-        }
-      }
-
-      ICP_PH_MARK(2);
-      // 3c. kept pairs.  The candidate match of point i is prev[i] on the one-pass path (its re-search list took
-      // match[] meanwhile) and match[i] after the pruning passes; match[i] becomes the candidate or 0xffff (dropped).
-      const uint16_t *cand = small ? prev : match;
-      auto kept = [&](int i) -> int {
-        const int m = cand[i];
-        bool keep = m != 0xffff;
-        if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
-        if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
-        return keep ? m : 0xffff;
-      };
-      // Sequential mode: the sums are warp 0's alone, so warp 0 also forms the fit and, on the one-pass path, the
-      // weights, with warp-level synchronisation only; the other warps go straight to the barrier that ends the
-      // iteration.  (The pruned path's 2 000-point sources keep the weights parallel: measured slower on warp 0.)
-      // Float64 mode: every thread takes part in the block_sum reductions.
-      int n_keep = 0;
-      float mrx = 0.f, mry = 0.f, mfx = 0.f, mfy = 0.f;
-      double t4[4] = {0, 0, 0, 0};
-      float pl[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};  // PLANE: A00 A01 A02 A11 A12 A22, sum F (q-r).n (thread 0)
-      if (seq && !small) {  // big problems (long serial sums): every thread forms the weights of its points
-        int cnt = 0;
-        for (int i = tid; i < ns; i += nthr) {
-          const int m = kept(i);
-          match[i] = (uint16_t)m;
-          cnt += m != 0xffff;
-        }
-        n_keep = block_total(cnt, &sh.tot[0][0], tot_phase);  // (its barrier publishes match[])
-      }
-      ICP_PH_MARK(3);
-      if (!seq || tid < 32) {
-        if (!seq) {
-          double s5[5] = {0, 0, 0, 0, 0}, t5[5];
-          for (int i = tid; i < ns; i += nthr) {
-            const int m = kept(i);
-            match[i] = (uint16_t)m;
-            if (m == 0xffff) continue;
-            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-            const float2 r = sorted[m];
-            s5[0] += 1.0, s5[1] += (double)q.x, s5[2] += (double)q.y, s5[3] += (double)r.x, s5[4] += (double)r.y;
-          }
-          block_sum<5>(s5, sh.red, red_phase, t5);
-          n_keep = (int)t5[0];
-          mrx = (float)t5[1], mry = (float)t5[2], mfx = (float)t5[3], mfy = (float)t5[4];
-        } else if (PLANE) {
-          if (small) {
-            int cnt = 0;
-            for (int i = tid; i < ns; i += 32) {
-              const int m = kept(i);
-              match[i] = (uint16_t)m;
-              cnt += m != 0xffff;
-            }
-            n_keep = __reduce_add_sync(0xffffffffu, cnt);
-            __syncwarp();  // (seq_sum9_warp's lanes read other lanes' match[] entries)
-          }
-        } else {
-          // the four sums (step x, step y, matched reference x, y); dropped pairs add +0
-          int cnt = 0;
-          const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
-            const int m = small ? kept(i) : match[i];
-            if (small) match[i] = (uint16_t)m;
-            if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
-            ++cnt;
-            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-            const float2 r = sorted[m];
-            return make_float4(q.x, q.y, r.x, r.y);
-          });
-          if (small) n_keep = __reduce_add_sync(0xffffffffu, cnt);
-          mrx = __shfl_sync(0xffffffffu, sum, 0), mry = __shfl_sync(0xffffffffu, sum, 1);
-          mfx = __shfl_sync(0xffffffffu, sum, 2), mfy = __shfl_sync(0xffffffffu, sum, 3);
-          __syncwarp();  // (seq_buf and match[] are read again by other lanes below)
-        }
-        ICP_PH_MARK(4);
-        if (n_keep == 0) {
-          if (tid == 0) sh.status = ICP_NO_POINT;
-        } else {
-          if constexpr (PLANE) {
-            // 3c'/3d'. point-to-plane normal equations over the kept pairs (oracle/icp_ref.c, minimizer 1):
-            //   c = q.x n.y - q.y n.x,  F = (c, n.x, n.y),  A = sum F F^T,  b = -sum F ((q - r).n)
-            auto terms = [&](int i, int m, float2 n, float (&v)[9]) {
-              const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-              const float2 r = sorted[m];
-              const float cr = __fsub_rn(__fmul_rn(q.x, n.y), __fmul_rn(q.y, n.x));
-              const float dp = __fadd_rn(__fmul_rn(__fsub_rn(q.x, r.x), n.x), __fmul_rn(__fsub_rn(q.y, r.y), n.y));
-              v[0] = __fmul_rn(cr, cr), v[1] = __fmul_rn(cr, n.x), v[2] = __fmul_rn(cr, n.y), v[3] = __fmul_rn(n.x, n.x);
-              v[4] = __fmul_rn(n.x, n.y), v[5] = __fmul_rn(n.y, n.y), v[6] = __fmul_rn(cr, dp), v[7] = __fmul_rn(n.x, dp);
-              v[8] = __fmul_rn(n.y, dp);
-            };
-            if (seq) {  // nine sequential sums in one pass; dropped pairs add +0
-              const float sum = seq_sum9_warp(ns, pl_scratch, match, nrm, terms);
-#pragma unroll
-              for (int k = 0; k < 9; ++k) pl[k] = __shfl_sync(0xffffffffu, sum, k);
-            } else {
-              double s5[5] = {0, 0, 0, 0, 0}, s4[4] = {0, 0, 0, 0}, o5[5], o4[4];
-              for (int i = tid; i < ns; i += nthr) {
-                const int m = match[i];
-                if (m == 0xffff) continue;
-                float v[9];
-                terms(i, m, nrm[m], v);
-#pragma unroll
-                for (int k = 0; k < 5; ++k) s5[k] += (double)v[k];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) s4[k] += (double)v[5 + k];
-              }
-              block_sum<5>(s5, sh.red, red_phase, o5);
-              block_sum<4>(s4, sh.red, red_phase, o4);
-#pragma unroll
-              for (int k = 0; k < 5; ++k) pl[k] = (float)o5[k];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) pl[5 + k] = (float)o4[k];
-            }
-          } else {
-            const float winv = __fdiv_rn(1.0f, (float)n_keep);
-            mrx = __fmul_rn(mrx, winv), mry = __fmul_rn(mry, winv);
-            mfx = __fmul_rn(mfx, winv), mfy = __fmul_rn(mfy, winv);
-
-            // 3d. cross-covariance of the centred pairs
-            if (seq) {  // m00 = qx*px, m01 = qx*py, m10 = qy*px, m11 = qy*py
-              const float sum = seq_sum4_warp<(THREADS >= SFE_SEQ_PIPE_MIN)>(ns, sh.seq_buf, [&](int i) -> float4 {
-                const int m = match[i];
-                if (m == 0xffff) return make_float4(0.f, 0.f, 0.f, 0.f);
-                const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-                const float2 r = sorted[m];
-                const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
-                const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
-                return make_float4(__fmul_rn(qx, px), __fmul_rn(qx, py), __fmul_rn(qy, px), __fmul_rn(qy, py));
-              });
-#pragma unroll
-              for (int k = 0; k < 4; ++k) t4[k] = (double)__shfl_sync(0xffffffffu, sum, k);
-            } else {
-              double s4[4] = {0, 0, 0, 0};
-              for (int i = tid; i < ns; i += nthr) {
-                if (match[i] == 0xffff) continue;
-                const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
-                const float2 r = sorted[match[i]];
-                const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
-                const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
-                s4[0] += (double)__fmul_rn(qx, px), s4[1] += (double)__fmul_rn(qx, py);
-                s4[2] += (double)__fmul_rn(qy, px), s4[3] += (double)__fmul_rn(qy, py);
-              }
-              block_sum<4>(s4, sh.red, red_phase, t4);
-            }
-          }
-
-          ICP_PH_MARK(5);
-          // 3e. rigid fit, T_iter update, checkers (one thread)
-          if (tid == 0) {
-            float c = 1.f, s = 0.f, tx, ty;
-            if constexpr (PLANE) {
-              // A x = b by Cholesky (A.llt()); an unknown whose pivot is not positive stays 0
-              const float a00 = pl[0], a01 = pl[1], a02 = pl[2], a11 = pl[3], a12 = pl[4], a22 = pl[5];
-              const float b0 = -pl[6], b1 = -pl[7], b2 = -pl[8];
-              float l00 = 0.f, l10 = 0.f, l20 = 0.f, l11 = 0.f, l21 = 0.f, l22 = 0.f;
-              const bool p0 = a00 > 0.f;
-              if (p0) l00 = __fsqrt_rn(a00), l10 = __fdiv_rn(a01, l00), l20 = __fdiv_rn(a02, l00);
-              const float d1 = __fsub_rn(a11, __fmul_rn(l10, l10));
-              const bool p1 = d1 > 0.f;
-              if (p1) l11 = __fsqrt_rn(d1), l21 = __fdiv_rn(__fsub_rn(a12, __fmul_rn(l20, l10)), l11);
-              const float d2 = __fsub_rn(__fsub_rn(a22, __fmul_rn(l20, l20)), __fmul_rn(l21, l21));
-              const bool p2 = d2 > 0.f;
-              if (p2) l22 = __fsqrt_rn(d2);
-              const float y0 = p0 ? __fdiv_rn(b0, l00) : 0.f;
-              const float y1 = p1 ? __fdiv_rn(__fsub_rn(b1, __fmul_rn(l10, y0)), l11) : 0.f;
-              const float y2 = p2 ? __fdiv_rn(__fsub_rn(__fsub_rn(b2, __fmul_rn(l20, y0)), __fmul_rn(l21, y1)), l22) : 0.f;
-              const float x2 = p2 ? __fdiv_rn(y2, l22) : 0.f;
-              const float x1 = p1 ? __fdiv_rn(__fsub_rn(y1, __fmul_rn(l21, x2)), l11) : 0.f;
-              const float x0 = p0 ? __fdiv_rn(__fsub_rn(__fsub_rn(y0, __fmul_rn(l10, x1)), __fmul_rn(l20, x2)), l00) : 0.f;
-              c = (float)cos((double)x0), s = (float)sin((double)x0);  // Rotation2D(x0)
-              tx = x1, ty = x2;
-            } else {
-              const float m00 = (float)t4[0], m01 = (float)t4[1], m10 = (float)t4[2], m11 = (float)t4[3];
-              const float a = __fadd_rn(m00, m11), bq = __fsub_rn(m10, m01);
-              const float h = sqrtf(__fadd_rn(__fmul_rn(a, a), __fmul_rn(bq, bq)));
-              if (h > 0.f) c = __fdiv_rn(a, h), s = __fdiv_rn(bq, h);
-              tx = __fsub_rn(mfx, __fadd_rn(__fmul_rn(c, mrx), __fmul_rn(-s, mry)));
-              ty = __fsub_rn(mfy, __fadd_rn(__fmul_rn(s, mrx), __fmul_rn(c, mry)));
-            }
-            const float dT[9] = {c, -s, tx, s, c, ty, 0.f, 0.f, 1.f};
-            float Tn[9];
-            mat3_mul_rn(dT, Ti, Tn);
-#pragma unroll
-            for (int i = 0; i < 9; ++i) sh.Tprev[i] = Ti[i], sh.Ti[i] = Tn[i];
-            sh.todo_n = 0;  // the next iteration's list counter (read before this iteration's n_fin total)
-            sh.inliers = n_keep;
-            const int count = ++sh.count;
-            bool counter_stop = false;
-            if (count >= prm.max_iterations) sh.iterate = 0, counter_stop = true;
-            if (!counter_stop && smooth > 0) {
-              int hn = sh.hn;
-              if (hn == ICP_HIST) {
-                for (int i = 0; i + 1 < ICP_HIST; ++i)
-                  sh.hq_w[i] = sh.hq_w[i + 1], sh.hq_z[i] = sh.hq_z[i + 1], sh.ht_x[i] = sh.ht_x[i + 1],
-                  sh.ht_y[i] = sh.ht_y[i + 1];
-                hn = ICP_HIST - 1;
-              }
-              rot_to_quat(Tn, sh.hq_w[hn], sh.hq_z[hn]);
-              sh.ht_x[hn] = Tn[2], sh.ht_y[hn] = Tn[5];
-              ++hn;
-              sh.hn = hn;
-              float vr = 0.f, vt = 0.f;
-              if (hn > smooth) {
-                for (int i = hn - 1; i >= hn - smooth; --i) {
-                  const float dw = __fadd_rn(__fmul_rn(sh.hq_w[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_z[i], sh.hq_z[i - 1]));
-                  const float dz = __fsub_rn(__fmul_rn(sh.hq_z[i], sh.hq_w[i - 1]), __fmul_rn(sh.hq_w[i], sh.hq_z[i - 1]));
-                  vr = __fadd_rn(vr, fabsf(__fmul_rn(2.0f, atan2f(fabsf(dz), fabsf(dw)))));
-                  const float ex = __fsub_rn(sh.ht_x[i], sh.ht_x[i - 1]), ey = __fsub_rn(sh.ht_y[i], sh.ht_y[i - 1]);
-                  vt = __fadd_rn(vt, fabsf(sqrtf(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)))));
-                }
-                vr = __fdiv_rn(vr, (float)smooth);
-                vt = __fdiv_rn(vt, (float)smooth);
-                if (vr < prm.min_diff_rot && vt < prm.min_diff_trans) sh.iterate = 0;
-              }
-              if (vr != vr)
-                sh.status = ICP_NAN_ROT;
-              else if (vt != vt)
-                sh.status = ICP_NAN_TRANS;
-            }
-          }
-        }
-      }
-      __syncthreads();
-      ICP_PH_MARK(6);
-      if (sh.status != ICP_OK || !sh.iterate) break;
-    }
-
-    // ---- 4. back to the caller's frame
-    if (tid == 0) {
-      if (sh.status == ICP_OK) {
-        const float Tm[9] = {1.f, 0.f, mx, 0.f, 1.f, my, 0.f, 0.f, 1.f};
-        float tmp[9], out[9], Ti[9], T0[9];
-#pragma unroll
-        for (int i = 0; i < 9; ++i) Ti[i] = sh.Ti[i], T0[i] = sh.T0[i];
-        mat3_mul_rn(Tm, Ti, tmp);
-        mat3_mul_rn(tmp, T0, out);
-#pragma unroll
-        for (int i = 0; i < 9; ++i) b.T_out[9 * (size_t)p + i] = out[i];
-      } else {
-#pragma unroll
-        for (int i = 0; i < 9; ++i) b.T_out[9 * (size_t)p + i] = guess[i];
-      }
-      b.iters[p] = sh.count;
-      b.inliers[p] = sh.inliers;
-      b.status[p] = sh.status;
-    }
-  }
-  ICP_PH_FLUSH();
+// the map class: every problem's target is a map grid (map_build); one instantiation per CTA size
+template <int THREADS, int MINB, bool PLANE>
+__global__ void __launch_bounds__(THREADS, MINB) icp_map_kernel(const IcpBatch b, const IcpMapArgs mp) {
+  constexpr bool MAP = THREADS > 0;  // true
+#include "icp_kernel_body.cuh"
 }
 
 // pcl.match: nearest reference point (within max_dist) of every query point; one CTA per (ref, query) pair
@@ -1191,6 +469,12 @@ struct MatchBatch {
   int32_t *ids;  // [total queries]
   float *dists;
   uint16_t *orig_ws;
+  // map class (match_map_kernel): pair p reads its reference from the grid in slot map_slot[p] (map_build)
+  const int *map_slot;
+  const MapGrid *map_grid;
+  const float2 *map_pts;
+  const int *map_cstart, *map_orig;
+  int map_cell_cap;
 };
 
 __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) {
@@ -1210,6 +494,7 @@ __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) 
     const int ns = b.in_off[p + 1] - b.in_off[p];
     int32_t *ids = b.ids + b.in_off[p];
     float *dists = b.dists + b.in_off[p];
+    if (nt > b.nt_max) continue;  // the map class's (match_map_kernel)
     __syncthreads();
     if (nt <= 0) {
       for (int i = tid; i < ns; i += nthr) ids[i] = -1, dists[i] = INFINITY;
@@ -1252,6 +537,303 @@ __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) 
   }
 }
 
+// The map class of pcl.match: references held as map grids in global memory.  The whole grid works on one pair's
+// queries at a time (a map match is one large reference and a few thousand queries, not many small pairs).
+__global__ void __launch_bounds__(ICP_THREADS) match_map_kernel(const MatchBatch b) {
+  const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
+  for (int p = 0; p < b.P; ++p) {
+    const int ms = b.map_slot[p];
+    if (ms < 0) continue;
+    const MapGrid &mg = b.map_grid[ms];
+    MapGridView g;
+    g.pts = b.map_pts, g.cstart = b.map_cstart + (size_t)ms * b.map_cell_cap, g.orig = b.map_orig;
+    g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
+    const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
+    const int ns = b.in_off[p + 1] - b.in_off[p];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) {
+      const NNResult r = nn_query(g, in[2 * i], in[2 * i + 1], max_d2);
+      b.ids[b.in_off[p] + i] = r.pos >= 0 ? (int32_t)g.orig[r.pos] : -1;
+      b.dists[b.in_off[p] + i] = r.d2;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------- map grids
+// Targets too large for the in-CTA layout get one grid each per call, in global memory, shared by every problem that
+// names the same target cloud.  Slots: the distinct map-class targets, numbered in target order on the device (a sort
+// of the problems by target id), so nothing depends on how many problems share a target or in which order they come.
+// Per slot: the mean (the kernel's own sequential float32 sum in point order; 0 for match), the bounding box of the
+// centred points, the geometry (grid_geometry, up to 1.5 cells per point), a stable radix sort of (slot, cell, index),
+// the centred points in that order with their original indices, the cell starts, and for point-to-plane the normals
+// (grid_surface_normal, one thread per point).  No coarse occupancy map: pass B of the pruned path searches instead.
+constexpr int MAP_THREADS = 256;
+constexpr unsigned MAP_NONE = 0xffffffffu;
+
+struct MapWs {  // device pointers into scratch[SCR_MAP]
+  int *slot;       // [P] slot of every problem, -1: not in the map class
+  int *n_slots;    // [1]
+  int *slot_tgt;   // [slot_cap] target cloud of every slot
+  MapGrid *grid;   // [slot_cap]
+  float2 *pts;     // [slot_cap * nt_max] centred points sorted by (slot, cell, index); padding at the end
+  int *orig;       // [slot_cap * nt_max]
+  int *cstart;     // [slot_cap][cell_cap]
+  float2 *nrm;     // [slot_cap * nt_max] point-to-plane only
+  int cell_cap;
+};
+
+__device__ __forceinline__ int map_count(const PackedClouds &t, int c) {
+  return t.cnt ? t.cnt[c] : t.off[c + 1] - t.off[c];
+}
+
+__global__ void map_flag_kernel(const PackedClouds t, const int *tgt_id, int P, int limit, unsigned *key, int *val,
+                                int *slot) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const int ti = tgt_id ? tgt_id[p] : p;
+  key[p] = map_count(t, ti) > limit ? (unsigned)ti : MAP_NONE;
+  val[p] = p;
+  slot[p] = -1;
+}
+
+__global__ void map_head_kernel(const unsigned *key, int P, int *head) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < P) head[i] = key[i] != MAP_NONE && (i == 0 || key[i] != key[i - 1]);
+}
+
+__global__ void map_slot_kernel(const unsigned *key, const int *val, const int *head, const int *sid, int P, int *slot,
+                                int *slot_tgt, int *n_slots) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P) return;
+  if (key[i] != MAP_NONE) {
+    slot[val[i]] = sid[i] - 1;
+    if (head[i]) slot_tgt[sid[i] - 1] = (int)key[i];
+  }
+  if (i == P - 1) *n_slots = sid[i];
+}
+
+// one CTA per slot: mean, bounding box, geometry
+__global__ void __launch_bounds__(ICP_THREADS) map_setup_kernel(const PackedClouds t, const int *slot_tgt,
+                                                                 const int *n_slots, int center, int seq, MapGrid *grid) {
+  __shared__ float mean[2];
+  __shared__ float wred[4 * 16];
+  __shared__ double red[2 * 5 * 16];
+  const int s = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
+  if (s >= *n_slots) return;
+  const int ti = slot_tgt[s], nt = map_count(t, ti);
+  const float *tgt = t.pts + 2 * (size_t)t.off[ti];
+  float mx = 0.f, my = 0.f;
+  if (center) {  // as icp_body's set-up
+    if (seq) {
+      if (tid < 64) {
+        const float sum = seq_sum_warp_global(tgt + (tid >> 5), nt, 2);
+        if ((tid & 31) == 0) mean[tid >> 5] = __fdiv_rn(sum, (float)nt);
+      }
+      __syncthreads();
+      mx = mean[0], my = mean[1];
+    } else {  // (float64 mode: the reduction tree of a 512-thread CTA, not the in-CTA launch's -- that mode is not
+              //  bit-reproducible across CTA sizes anyway)
+      double sm[2] = {0.0, 0.0}, tot[2];
+      int phase = 0;
+      for (int i = tid; i < nt; i += nthr) sm[0] += (double)tgt[2 * i], sm[1] += (double)tgt[2 * i + 1];
+      block_sum<2>(sm, red, phase, tot);
+      mx = (float)(tot[0] / (double)nt), my = (float)(tot[1] / (double)nt);
+    }
+  }
+  float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
+  for (int i = tid; i < nt; i += nthr) {
+    const float x = tgt[2 * i] - mx, y = tgt[2 * i + 1] - my;
+    mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
+    mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
+    mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
+    mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
+  }
+  if ((tid & 31) == 0) {
+    wred[(tid >> 5) * 4 + 0] = mn_x, wred[(tid >> 5) * 4 + 1] = mn_y;
+    wred[(tid >> 5) * 4 + 2] = mxx, wred[(tid >> 5) * 4 + 3] = mxy;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
+    for (int w = 0; w < (nthr >> 5); ++w) {
+      a = fminf(a, wred[w * 4 + 0]), bb = fminf(bb, wred[w * 4 + 1]);
+      c = fmaxf(c, wred[w * 4 + 2]), d = fmaxf(d, wred[w * 4 + 3]);
+    }
+    MapGridView g;
+    grid_geometry(nt, a, bb, c, d, 0.05f, g, nt + nt / 2 > 256 ? nt + nt / 2 : 256);
+    MapGrid m;
+    m.mean[0] = mx, m.mean[1] = my;
+    m.bbox[0] = a, m.bbox[1] = bb, m.bbox[2] = c, m.bbox[3] = d;
+    m.ox = g.ox, m.oy = g.oy, m.cell = g.cell, m.inv_cell = g.inv_cell;
+    m.nx = g.nx, m.ny = g.ny, m.n = nt, m.pad = 0;
+    grid[s] = m;
+  }
+}
+
+// sort key of every (slot, point): slot above, cell below; unused positions get the padding key (all ones)
+__global__ void map_keys_kernel(const PackedClouds t, const int *slot_tgt, const int *n_slots, const MapGrid *grid,
+                                int nt_max, unsigned long long *key, int *val) {
+  const int s = blockIdx.y;
+  const bool live = s < *n_slots;
+  const int ti = live ? slot_tgt[s] : 0, nt = live ? map_count(t, ti) : 0;
+  const float *tgt = t.pts + 2 * (size_t)(live ? t.off[ti] : 0);
+  MapGrid m;
+  if (live) m = grid[s];
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nt_max; j += gridDim.x * blockDim.x) {
+    const size_t i = (size_t)s * nt_max + j;
+    if (j < nt) {
+      const float x = tgt[2 * j] - m.mean[0], y = tgt[2 * j + 1] - m.mean[1];
+      const int c = grid_cell_coord(y, m.oy, m.inv_cell, m.ny) * m.nx + grid_cell_coord(x, m.ox, m.inv_cell, m.nx);
+      key[i] = ((unsigned long long)s << 32) | (unsigned)c;
+      val[i] = j;
+    } else {
+      key[i] = ~0ull;
+      val[i] = 0;
+    }
+  }
+}
+
+// after the sort: centred points in sorted order and every cell's first position (absolute in pts)
+__global__ void map_scatter_kernel(const PackedClouds t, const int *slot_tgt, const MapGrid *grid,
+                                   const unsigned long long *key, const int *val, int N, int cell_cap, float2 *pts,
+                                   int *cstart) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const unsigned long long k = key[i];
+  if (k == ~0ull) return;
+  const int s = (int)(k >> 32), c = (int)(k & 0xffffffffu), j = val[i];
+  const MapGrid &m = grid[s];
+  const float *src = t.pts + 2 * ((size_t)t.off[slot_tgt[s]] + j);
+  pts[i] = make_float2(src[0] - m.mean[0], src[1] - m.mean[1]);
+  int *cs = cstart + (size_t)s * cell_cap;
+  const int pc = (i > 0 && (int)(key[i - 1] >> 32) == s) ? (int)(key[i - 1] & 0xffffffffu) : -1;
+  for (int cc = pc + 1; cc <= c; ++cc) cs[cc] = i;
+  if (i + 1 == N || (key[i + 1] >> 32) != (unsigned long long)s)
+    for (int cc = c + 1; cc <= m.nx * m.ny; ++cc) cs[cc] = i + 1;  // through the sentinel entry ncells
+}
+
+// point-to-plane: the normal at every sorted position, once per target
+__global__ void map_normals_kernel(const unsigned long long *key, const MapGrid *grid, const float2 *pts,
+                                   const int *cstart, const int *orig, int N, int cell_cap, int knn, float2 *nrm) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const unsigned long long k = key[i];
+  if (k == ~0ull) return;
+  const int s = (int)(k >> 32);
+  const MapGrid &m = grid[s];
+  MapGridView g;
+  g.pts = pts, g.cstart = cstart + (size_t)s * cell_cap, g.orig = orig;
+  g.n = m.n, g.nx = m.nx, g.ny = m.ny, g.ox = m.ox, g.oy = m.oy, g.cell = m.cell, g.inv_cell = m.inv_cell;
+  float bd[GRID_KNN_MAX];
+  int bi[GRID_KNN_MAX];
+  nrm[i] = grid_surface_normal(g, i, knn, bd, bi, 1);
+}
+
+// Builds the map grids of the problems whose target has more than `limit` points.  slot_cap bounds the number of
+// distinct such targets.  Workspace (scratch[SCR_MAP]): 40 bytes per slot point (48 with normals) for slot_cap *
+// nt_max slot points, 4 * (1.5 nt_max + 257) bytes of cell table per slot, 28 bytes per problem, CUB's temporary
+// storage.  knn > 0: normals too.
+static int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, const int *tgt_id, int P, int limit,
+                     int slot_cap, bool center, bool seq, int knn, MapWs &w) {
+  const int nt_max = t.n_max;
+  const long long slots = (long long)slot_cap * nt_max;
+  SFE_REQUIRE(slots < INT_MAX, "map grids: %d targets of up to %d points exceed %d slot points", slot_cap, nt_max,
+              INT_MAX - 1);
+  SFE_REQUIRE(slot_cap <= 65535, "map grids: at most 65535 distinct map-sized targets per call (got up to %d)",
+              slot_cap);
+  const int N = (int)slots;
+  w.cell_cap = (nt_max + nt_max / 2 > 256 ? nt_max + nt_max / 2 : 256) + 1;
+  int slot_bits = 1;
+  while ((1ll << slot_bits) < slot_cap) ++slot_bits;
+  const int end_bit = 32 + slot_bits;
+
+  cub::DoubleBuffer<unsigned> pkeys;
+  cub::DoubleBuffer<int> pvals;
+  cub::DoubleBuffer<unsigned long long> keys;
+  cub::DoubleBuffer<int> vals;
+  size_t psort_bytes = 0, scan_bytes = 0, sort_bytes = 0;
+  SFE_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, psort_bytes, pkeys, pvals, P, 0, 32, st));
+  SFE_CUDA(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int *)nullptr, (int *)nullptr, P, st));
+  SFE_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, vals, N, 0, end_bit, st));
+  size_t temp_bytes = psort_bytes > scan_bytes ? psort_bytes : scan_bytes;
+  if (sort_bytes > temp_bytes) temp_bytes = sort_bytes;
+  char *base = nullptr;
+  size_t used = 0;
+  auto take = [&](size_t bytes) {
+    void *p = base ? base + used : nullptr;
+    used += (bytes + 255) & ~size_t(255);
+    return p;
+  };
+  unsigned *pk0, *pk1;
+  int *pv0, *pv1, *head, *sid;
+  unsigned long long *k0, *k1;
+  int *v0, *v1;
+  void *temp;
+  for (int pass = 0; pass < 2; ++pass) {  // pass 0 sizes the block, pass 1 carves it
+    used = 0;
+    pk0 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
+    pk1 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
+    pv0 = (int *)take(sizeof(int) * (size_t)P);
+    pv1 = (int *)take(sizeof(int) * (size_t)P);
+    head = (int *)take(sizeof(int) * (size_t)P);
+    sid = (int *)take(sizeof(int) * (size_t)P);
+    w.slot = (int *)take(sizeof(int) * (size_t)P);
+    w.n_slots = (int *)take(sizeof(int));
+    w.slot_tgt = (int *)take(sizeof(int) * (size_t)slot_cap);
+    w.grid = (MapGrid *)take(sizeof(MapGrid) * (size_t)slot_cap);
+    k0 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
+    k1 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
+    v0 = (int *)take(sizeof(int) * (size_t)N);
+    v1 = (int *)take(sizeof(int) * (size_t)N);
+    w.pts = (float2 *)take(sizeof(float2) * (size_t)N);
+    w.nrm = knn > 0 ? (float2 *)take(sizeof(float2) * (size_t)N) : nullptr;
+    w.cstart = (int *)take(sizeof(int) * (size_t)slot_cap * w.cell_cap);
+    temp = take(temp_bytes);
+    if (pass == 0) {
+      int rc = ensure(ctx, ctx->scratch[SCR_MAP], used, st);
+      if (rc != SFE_OK) return rc;
+      base = (char *)ctx->scratch[SCR_MAP].ptr;
+    }
+  }
+  const int pb = (P + MAP_THREADS - 1) / MAP_THREADS;
+  map_flag_kernel<<<pb, MAP_THREADS, 0, st>>>(t, tgt_id, P, limit, pk0, pv0, w.slot);
+  SFE_CUDA(cudaGetLastError());
+  pkeys = cub::DoubleBuffer<unsigned>(pk0, pk1);
+  pvals = cub::DoubleBuffer<int>(pv0, pv1);
+  SFE_CUDA(cub::DeviceRadixSort::SortPairs(temp, psort_bytes, pkeys, pvals, P, 0, 32, st));
+  map_head_kernel<<<pb, MAP_THREADS, 0, st>>>(pkeys.Current(), P, head);
+  SFE_CUDA(cudaGetLastError());
+  SFE_CUDA(cub::DeviceScan::InclusiveSum(temp, scan_bytes, (const int *)head, sid, P, st));
+  map_slot_kernel<<<pb, MAP_THREADS, 0, st>>>(pkeys.Current(), pvals.Current(), head, sid, P, w.slot, w.slot_tgt,
+                                              w.n_slots);
+  SFE_CUDA(cudaGetLastError());
+  map_setup_kernel<<<slot_cap, ICP_THREADS, 0, st>>>(t, w.slot_tgt, w.n_slots, center ? 1 : 0, seq ? 1 : 0, w.grid);
+  SFE_CUDA(cudaGetLastError());
+  int bps = (nt_max + 4 * MAP_THREADS - 1) / (4 * MAP_THREADS);
+  bps = bps < 1 ? 1 : (bps > 256 ? 256 : bps);
+  map_keys_kernel<<<dim3(bps, slot_cap), MAP_THREADS, 0, st>>>(t, w.slot_tgt, w.n_slots, w.grid, nt_max, k0, v0);
+  SFE_CUDA(cudaGetLastError());
+  keys = cub::DoubleBuffer<unsigned long long>(k0, k1);
+  vals = cub::DoubleBuffer<int>(v0, v1);
+  SFE_CUDA(cub::DeviceRadixSort::SortPairs(temp, sort_bytes, keys, vals, N, 0, end_bit, st));
+  w.orig = vals.Current();
+  const int nb = (N + MAP_THREADS - 1) / MAP_THREADS;
+  map_scatter_kernel<<<nb, MAP_THREADS, 0, st>>>(t, w.slot_tgt, w.grid, keys.Current(), w.orig, N, w.cell_cap, w.pts,
+                                                 w.cstart);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches += 9;  // six kernels, the two sorts and the scan counted once each
+  if (knn > 0) {
+    map_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), w.grid, w.pts, w.cstart, w.orig, N, w.cell_cap, knn,
+                                                   w.nrm);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  return SFE_OK;
+}
+
 // ---------------------------------------------------------------------------- host side
 static int pick_max_cells(int nt_max) {
   int c = nt_max + nt_max / 2;  // the grid aims at one point per cell; the slack absorbs elongated bounding boxes
@@ -1260,39 +842,73 @@ static int pick_max_cells(int nt_max) {
   return c;
 }
 
+// Shared memory of icp_kernel's layout for problems of up to ns_max x nt_max points (both >= 1) after big problems
+// traded cell-table entries (coarser cells) for room; *max_cells receives the table's size.
+static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, int optin, int *max_cells) {
+  const bool use_order = ns_max > 1024;
+  auto smem_for = [&](int mc) {
+    return ((sizeof(IcpShared) + 15) & ~size_t(15)) + sizeof(float2) * (size_t)nt_max +
+           sizeof(uint32_t) * (size_t)((mc + 2) / 2 + 1) + 8 + sizeof(float2) * (size_t)ns_max +
+           sizeof(float) * (size_t)ns_max + 2 * sizeof(uint16_t) * (size_t)ns_max + (size_t)ns_max + 4 +
+           sizeof(float) * (size_t)ns_max + (use_order ? sizeof(uint16_t) * (size_t)ns_max : 0) + 16 +
+           (plane && ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
+  };
+  int mc = pick_max_cells(nt_max);
+  while (smem_for(mc) > (size_t)optin && mc > nt_max / 4 + 256) mc -= mc / 8;
+  *max_cells = mc;
+  return smem_for(mc);
+}
+
+// The largest target icp_kernel's layout holds next to sources of ns_max points (0: none): targets above it are the
+// map class.
+static int icp_cta_limit(int ns_max, bool plane, int optin) {
+  int lo = 0, hi = 65535, mc;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (icp_cta_smem(ns_max, mid, plane, optin, &mc) <= (size_t)optin) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+static size_t match_cta_smem(int nt_max) {
+  return sizeof(float2) * (size_t)nt_max + sizeof(uint32_t) * (size_t)((pick_max_cells(nt_max) + 2) / 2 + 1) + 16;
+}
+
+static int match_cta_limit(int optin) {
+  int lo = 0, hi = 65535;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) / 2;
+    if (match_cta_smem(mid) <= (size_t)optin) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+static void icp_tuning(IcpBatch &b) {
+  // One-pass exact path (per-lane searches with certified matches, no pruning passes) for problems of up to
+  // 5 source points per thread (chosen on the config-4 replay, sources of ~360 points in 128-thread CTAs: a lower
+  // limit sends more problems down the slower pruned path; not re-measured on H100).
+  static const int mult = [] {  // development switch: SFE_ICP_SMALL_MULT
+    const char *e = getenv("SFE_ICP_SMALL_MULT");
+    return e ? atoi(e) : 5;
+  }();
+  b.small_mult = mult;
+  static const float mm = [] {  // development switch: SFE_ICP_MARGIN_MULT
+    const char *e = getenv("SFE_ICP_MARGIN_MULT");
+    return e ? (float)atof(e) : 6.f;
+  }();
+  b.margin_mult = mm;
+}
+
 // One launch over the batch, laid out for problems of up to ns_max x nt_max points; b.class_mode is its size class.
 static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max) {
   b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
-  b.max_cells = pick_max_cells(b.nt_max);
   b.use_order = b.ns_max > 1024;
   b.cell_scale = 1.0f;
   b.prm = *prm;
-  {
-    // One-pass exact path (per-lane searches with certified matches, no pruning passes) for problems of up to
-    // 5 source points per thread (chosen on the config-4 replay, sources of ~360 points in 128-thread CTAs: a lower
-    // limit sends more problems down the slower pruned path; not re-measured on H100).
-    static const int mult = [] {  // development switch: SFE_ICP_SMALL_MULT
-      const char *e = getenv("SFE_ICP_SMALL_MULT");
-      return e ? atoi(e) : 5;
-    }();
-    b.small_mult = mult;
-    static const float mm = [] {  // development switch: SFE_ICP_MARGIN_MULT
-      const char *e = getenv("SFE_ICP_MARGIN_MULT");
-      return e ? (float)atof(e) : 6.f;
-    }();
-    b.margin_mult = mm;
-  }
-  auto smem_for = [&](int max_cells) {
-    return ((sizeof(IcpShared) + 15) & ~size_t(15)) + sizeof(float2) * (size_t)b.nt_max +
-           sizeof(uint32_t) * (size_t)((max_cells + 2) / 2 + 1) + 8 + sizeof(float2) * (size_t)b.ns_max +
-           sizeof(float) * (size_t)b.ns_max + 2 * sizeof(uint16_t) * (size_t)b.ns_max + (size_t)b.ns_max + 4 +
-           sizeof(float) * (size_t)b.ns_max + (b.use_order ? sizeof(uint16_t) * (size_t)b.ns_max : 0) + 16 +
-           (prm->minimizer == 1 && b.ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
-  };
-  // big problems: trade cell-table entries (coarser cells) for room before giving up
-  while (smem_for(b.max_cells) > (size_t)ctx->max_smem_optin && b.max_cells > b.nt_max / 4 + 256)
-    b.max_cells -= b.max_cells / 8;
-  const size_t smem = smem_for(b.max_cells);
+  icp_tuning(b);
+  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, prm->minimizer == 1, ctx->max_smem_optin, &b.max_cells);
   if (smem > (size_t)ctx->max_smem_optin) {
     set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %d)", ns_max, nt_max, smem,
               ctx->max_smem_optin);
@@ -1359,12 +975,64 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
   return SFE_OK;
 }
 
+// The map class: problems whose target has more than `limit` points, their targets read from map grids.  Shared memory
+// holds IcpShared and the source arrays only.
+static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max,
+                          int limit, int slot_cap) {
+  const bool plane = prm->minimizer == 1;
+  MapWs w;
+  int rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, b.tgt_id, b.P, limit, slot_cap, true,
+                     (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
+  if (rc != SFE_OK) return rc;
+  b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max;
+  b.use_order = b.ns_max > 1024;
+  b.cell_scale = 1.0f;
+  b.prm = *prm;
+  icp_tuning(b);
+  // the other problems are the in-CTA launch's; with no in-CTA launch (limit 0) this one takes all of them (targets of
+  // 0 points are then reported here, SFE_ICP_EMPTY_REF, before any map grid is read)
+  b.class_mode = limit > 0 ? 2 : 0, b.class_ns = b.ns_max, b.class_nt = limit;
+  IcpMapArgs m{w.slot, w.grid, w.pts, w.cstart, w.orig, w.nrm, w.cell_cap};
+  const size_t ns = (size_t)b.ns_max;
+  const size_t smem = ((sizeof(IcpShared) + 15) & ~size_t(15)) + 8 + ns * (sizeof(float2) + 4 * sizeof(float)) + ns +
+                      4 + (b.use_order ? sizeof(uint16_t) * ns : 0) + 16 +
+                      (plane && b.ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
+  if (smem > (size_t)ctx->max_smem_optin) {
+    set_error("icp: sources of %d points need %zu B of shared memory per CTA (limit %d)", ns_max, smem,
+              ctx->max_smem_optin);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  const int threads = b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS);
+  const void *fn = plane ? (threads == 128   ? (const void *)icp_map_kernel<128, 7, true>
+                            : threads == 256 ? (const void *)icp_map_kernel<256, 4, true>
+                                             : (const void *)icp_map_kernel<512, 1, true>)
+                         : (threads == 128   ? (const void *)icp_map_kernel<128, 7, false>
+                            : threads == 256 ? (const void *)icp_map_kernel<256, 4, false>
+                                             : (const void *)icp_map_kernel<512, 1, false>);
+  SFE_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 1;
+  SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
+  if (per_sm < 1) per_sm = 1;
+  int grid = ctx->sm_count * per_sm;
+  if (grid > b.P) grid = b.P;
+  if (grid < b.P) {  // persistent CTAs
+    b.next = ctx->work + WORK_ICP;
+    SFE_CUDA(cudaMemsetAsync(b.next, 0, sizeof(int), st));
+  }
+  void *args[] = {(void *)&b, (void *)&m};
+  SFE_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(threads), args, smem, st));
+  ctx->launches++;
+  return SFE_OK;
+}
+
 }  // namespace sfe
 
 // Size classes (IcpBatch::class_mode): a small class (both sizes positive, clamped to the capacities src.n_max x
 // tgt.n_max) that is smaller on either axis gets a first launch laid out for it, whose smaller shared-memory footprint
 // fits more CTAs per SM; a second launch, laid out for the capacities, takes the problems that did not fit.
-// Otherwise one launch takes every problem and reports oversize ones itself (SFE_ICP_TOO_LARGE).
+// Otherwise one launch takes every problem and reports oversize ones itself (SFE_ICP_TOO_LARGE) -- unless the
+// largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit and the map
+// class (map grids in global memory, icp_map_kernel) takes the rest.
 int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
                  int small_nt) {
   const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
@@ -1374,8 +1042,9 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
                   pb.status,
               "icp: null pointer");
-  SFE_REQUIRE(nt_max <= 65535 && ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d, %d)",
-              ns_max, nt_max);
+  const bool classes = small_ns > 0 && small_nt > 0;
+  SFE_REQUIRE(ns_max <= 65535 && (nt_max <= 65535 || !classes),
+              "icp: clouds of more than 65535 points are not supported (got %d, %d)", ns_max, nt_max);
   SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
   SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "icp: unknown error minimizer %d", prm->minimizer);
   SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
@@ -1389,9 +1058,23 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P;
+  if (!classes) {
+#ifdef SFE_ICP_MAP_ALL  // development build (tools/build_icp_map_variant.sh): every target takes the map class
+    const int limit = 0;
+#else
+    const int limit = icp_cta_limit(ns_max > 0 ? ns_max : 1, prm->minimizer == 1, ctx->max_smem_optin);
+#endif
+    if (nt_max <= limit) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
+    if (limit > 0) {
+      b.class_mode = 1;
+      int rc = icp_launch(ctx, st, prm, b, ns_max, limit);
+      if (rc != SFE_OK) return rc;
+    }
+    const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
+    return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap);
+  }
   const int ns_small = std::min(small_ns, ns_max), nt_small = std::min(small_nt, nt_max);
-  if (small_ns <= 0 || small_nt <= 0 || (ns_small == ns_max && nt_small == nt_max))
-    return icp_launch(ctx, st, prm, b, ns_max, nt_max);
+  if (ns_small == ns_max && nt_small == nt_max) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
   b.class_mode = 1;
   int rc = icp_launch(ctx, st, prm, b, ns_small, nt_small);
   if (rc != SFE_OK) return rc;
@@ -1399,6 +1082,8 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   return icp_launch(ctx, st, prm, b, ns_max, nt_max);
 }
 
+// References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in
+// match_map_kernel, in the same call.
 int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P,
                    float max_dist, int32_t *ids, float *dists) {
   const int nt_max = ref.n_max;
@@ -1407,12 +1092,16 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   if (P == 0) return SFE_OK;
   SFE_REQUIRE(ref.pts && ref.off && in.pts && in.off && ids && dists, "match: null pointer");
   SFE_REQUIRE(!ref.cnt && !in.cnt, "match: per-cloud counts are not supported");
-  SFE_REQUIRE(nt_max <= 65535, "match: reference clouds of more than 65535 points are not supported (got %d)", nt_max);
+  cudaFuncAttributes fa;  // the dynamic layout shares the opt-in limit with the kernel's static shared memory
+  SFE_CUDA(cudaFuncGetAttributes(&fa, match_kernel));
+  const int limit = match_cta_limit(ctx->max_smem_optin - (int)fa.sharedSizeBytes);
   MatchBatch b{};
   b.ref_pts = ref.pts, b.ref_off = ref.off, b.in_pts = in.pts, b.in_off = in.off;
-  b.P = P, b.nt_max = nt_max > 0 ? nt_max : 1, b.max_cells = pick_max_cells(b.nt_max), b.max_dist = max_dist;
+  b.P = P, b.max_dist = max_dist;
   b.ids = ids, b.dists = dists;
-  const size_t smem = sizeof(float2) * (size_t)b.nt_max + sizeof(uint32_t) * (size_t)((b.max_cells + 2) / 2 + 1) + 16;
+  const int nt_cta = std::min(nt_max, limit);
+  b.nt_max = nt_cta > 0 ? nt_cta : 1, b.max_cells = pick_max_cells(b.nt_max);
+  const size_t smem = match_cta_smem(b.nt_max);
   if (smem > (size_t)ctx->max_smem_optin) {
     set_error("match: a %d-point reference needs %zu B of shared memory per CTA (limit %d)", nt_max, smem,
               ctx->max_smem_optin);
@@ -1428,6 +1117,15 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
   match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  if (nt_max <= limit) return SFE_OK;
+  MapWs w;
+  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, nullptr, P, limit, P, false, true, 0, w);
+  if (rc != SFE_OK) return rc;
+  b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
+  b.map_cell_cap = w.cell_cap;
+  match_map_kernel<<<ctx->sm_count * 4, ICP_THREADS, 0, st>>>(b);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;

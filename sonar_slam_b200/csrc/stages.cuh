@@ -28,6 +28,7 @@ struct IcpProblems {
   int min_points;
   const int *raw_cnt;
   int raw_cap;
+  int n_tgt_clouds;  // number of target clouds when the caller knows it (bounds the map grids, icp.cu), else 0
 };
 
 int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
@@ -45,10 +46,12 @@ int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_
                    bool frame_class = false);
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
                        int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split);
-// problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu), (0, 0): one launch
+// problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu); (0, 0): one launch,
+// or, when the largest target does not fit one CTA, one for the targets that do and the map class for the rest
 int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
             int small_nt);
-// nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used
+// nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
+// of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
               int32_t *ids, float *dists);
 

@@ -126,6 +126,8 @@ def remove_outlier(pts, off, n_max, radius, min_points, ctx=None):
 
 
 def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, ctx=None):
+    """Batched pcl.match (include/sonarfe.h: sfe_match_dev).  References of any size: those above one CTA's shared
+    memory (whole maps) are searched as map grids in global memory, with the same results."""
     ctx = ctx or context(ref_pts.device)
     n = ref_off.numel() - 1
     ids = torch.empty((in_pts.shape[0],), dtype=torch.int32, device=in_pts.device)
@@ -136,7 +138,11 @@ def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, ctx=None):
 
 
 def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, src_id=None, tgt_id=None, ctx=None):
-    """Batched ICP (include/sonarfe.h: sfe_icp_dev).  guess: [P,3,3] f32 cuda.  Returns dict of cuda tensors."""
+    """Batched ICP (include/sonarfe.h: sfe_icp_dev).  guess: [P,3,3] f32 cuda.  Returns dict of cuda tensors.
+
+    Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
+    map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources: at most 65 535
+    points and what fits shared memory (about 7 000)."""
     ctx = ctx or context(src_pts.device)
     prm = params or _lib.IcpParams()
     guess = guess.contiguous()
