@@ -160,6 +160,13 @@ SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uin
  * sfe_remove_outlier_*  bruce_slam.pcl.remove_outlier (pcl.cpp:54-74): PCL RadiusOutlierRemoval:
  *                       keep a point iff at least min_points OTHER points lie within `radius`;
  *                       input order is preserved.
+ *                       Any cloud size is accepted: clouds that fit one CTA's shared memory
+ *                       (24 445 points on an H100) run one CTA each; larger ones (whole maps) run
+ *                       in the same call in a map class (the map grid of sfe_match_dev in global
+ *                       memory, one thread per point), with the same results.  A call with a cloud
+ *                       above that limit takes at most 65 535 clouds and n_clouds * n_max slots
+ *                       (at most 2^31 - 1); its workspace holds 48 bytes per slot, a cell table of
+ *                       6 bytes per n_max point and 28 bytes per cloud, and CUB's temporary storage.
  */
 SFE_API int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
                                int n_max, float resolution, float *out_pts_dev, int32_t *out_idx_dev,

@@ -27,6 +27,7 @@ def _points(a, name, cols=(2, 3)):
 
 
 def remove_outlier(mat_in, radius, min_points):
+    """Points with at least min_points others within radius, in input order.  Any size, whole maps included."""
     pts = _points(mat_in, "points")
     n, dim = pts.shape
     if n == 0:

@@ -18,7 +18,7 @@ namespace sfe {
 constexpr int GRID_MAX_CELLS = 16384;  // 16-bit offsets, two per 32-bit word
 
 // Idx: type of the cell offsets and original indices.  uint16_t for the grids a CTA builds in shared memory
-// (GridView); int for the map grids built once per target cloud in global memory (icp.cu, MapGridView), whose
+// (GridView); int for the map grids built once per cloud in global memory (map_grid.cu, MapGridView), whose
 // offsets are absolute positions in the workspace's sorted-point array.
 template <typename Idx>
 struct GridViewT {
@@ -67,6 +67,65 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int *warp_sums /* [33
   total = warp_sums[32];
   __syncthreads();
   return excl;
+}
+
+// Sum K doubles over the CTA with ONE barrier: every warp publishes its partial sums, and after the barrier
+// every warp reduces the (<= 16) partials itself with a butterfly, so all threads hold the bit-identical total.
+// `scratch` has two halves used alternately (`phase` counts the calls): the half written by call n is last read
+// before call n+1's barrier and not rewritten before call n+2.
+template <int K>
+__device__ __forceinline__ void block_sum(double (&v)[K], double *scratch /* [2][5][16] smem */, int &phase,
+                                          double (&out)[K]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  static_assert(K <= 5, "scratch holds five partial sums per warp");
+  double *half = scratch + (phase & 1) * (5 * 16);
+  ++phase;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double x = v[k];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
+    if (lane == 0) half[k * 16 + warp] = x;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double x = lane < nwarps ? half[k * 16 + lane] : 0.0;
+#pragma unroll
+    for (int d = 8; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);  // nwarps <= 16
+    out[k] = __shfl_sync(0xffffffffu, x, 0);
+  }
+}
+
+// One sequential sum over values in global memory, p[0], p[stride], ... (the reference cloud's mean, once per
+// problem): lane j holds term base + j and a shuffle hands term j to every lane, so all lanes carry the same
+// running sum; eight batches (256 terms) are requested at once and the next eight are in flight while these are
+// added, so the L2 latency hides behind the ~1000-cycle add chain
+__device__ __forceinline__ float seq_sum_warp_global(const float *p, int n, int stride) {
+  const int lane = threadIdx.x & 31;
+  float s = 0.f, cur[8], nxt[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int i = k * 32 + lane;
+    cur[k] = i < n ? p[(size_t)i * stride] : 0.f;
+  }
+  for (int base = 0; base < n; base += 256) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int i = base + 256 + k * 32 + lane;
+      nxt[k] = i < n ? p[(size_t)i * stride] : 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      if (base + k * 32 < n) {  // (warp-uniform)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) s = __fadd_rn(s, __shfl_sync(0xffffffffu, cur[k], j));
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) cur[k] = nxt[k];
+  }
+  return s;
 }
 
 // Choose grid geometry for n points with bounding box [minx,maxx] x [miny,maxy].

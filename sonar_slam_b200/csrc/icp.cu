@@ -43,14 +43,6 @@ constexpr float ICP_PRUNED = 3.0e38f;    // "finite, but farther than we needed 
 enum { ICP_OK = 0, ICP_NO_OUTLIER = 1, ICP_NO_POINT = 2, ICP_NAN_ROT = 3, ICP_NAN_TRANS = 4, ICP_NOT_RIGID = 5,
        ICP_EMPTY_REF = 6, ICP_SKIPPED = 7, ICP_TOO_LARGE = 8 };
 
-// One map grid: a target cloud too large for the in-CTA layout, built once per call in global memory (map_build).
-struct MapGrid {
-  float mean[2];  // reference mean (the kernel's sequential float32 sum; 0 for match)
-  float bbox[4];  // bounding box of the centred points
-  float ox, oy, cell, inv_cell;
-  int nx, ny, n, pad;
-};
-
 struct IcpBatch {
   const float *src_pts;
   const int *src_off;
@@ -170,34 +162,6 @@ __device__ __forceinline__ void rot_to_quat(const float *T, float &qw, float &qz
     qz = __fmul_rn(0.5f, t);
     t = __fdiv_rn(0.5f, t);
     qw = __fmul_rn(__fsub_rn(m10, m01), t);
-  }
-}
-
-// Sum K doubles over the CTA with ONE barrier: every warp publishes its partial sums, and after the barrier
-// every warp reduces the (<= 16) partials itself with a butterfly, so all threads hold the bit-identical total.
-// `scratch` has two halves used alternately (`phase` counts the calls): the half written by call n is last read
-// before call n+1's barrier and not rewritten before call n+2.
-template <int K>
-__device__ __forceinline__ void block_sum(double (&v)[K], double *scratch /* [2][5][16] smem */, int &phase,
-                                          double (&out)[K]) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  static_assert(K <= 5, "scratch holds five partial sums per warp");
-  double *half = scratch + (phase & 1) * (5 * 16);
-  ++phase;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double x = v[k];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
-    if (lane == 0) half[k * 16 + warp] = x;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double x = lane < nwarps ? half[k * 16 + lane] : 0.0;
-#pragma unroll
-    for (int d = 8; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);  // nwarps <= 16
-    out[k] = __shfl_sync(0xffffffffu, x, 0);
   }
 }
 
@@ -403,37 +367,6 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const Pos 
   return s;
 }
 
-// One sequential sum over values in global memory, p[0], p[stride], ... (the reference cloud's mean, once per
-// problem): lane j holds term base + j and a shuffle hands term j to every lane, so all lanes carry the same
-// running sum; eight batches (256 terms) are requested at once and the next eight are in flight while these are
-// added, so the L2 latency hides behind the ~1000-cycle add chain
-__device__ __forceinline__ float seq_sum_warp_global(const float *p, int n, int stride) {
-  const int lane = threadIdx.x & 31;
-  float s = 0.f, cur[8], nxt[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const int i = k * 32 + lane;
-    cur[k] = i < n ? p[(size_t)i * stride] : 0.f;
-  }
-  for (int base = 0; base < n; base += 256) {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int i = base + 256 + k * 32 + lane;
-      nxt[k] = i < n ? p[(size_t)i * stride] : 0.f;
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (base + k * 32 < n) {  // (warp-uniform)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) s = __fadd_rn(s, __shfl_sync(0xffffffffu, cur[k], j));
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) cur[k] = nxt[k];
-  }
-  return s;
-}
-
 // One instantiation per CTA size so that the register budget follows the launch shape (a single
 // __launch_bounds__(512) build capped the 128-thread class at 64 registers and spilled).
 // PLANE: errorMinimizer = PointToPlaneErrorMinimizer (sfe_icp_params.minimizer 1); a separate instantiation so that
@@ -556,282 +489,6 @@ __global__ void __launch_bounds__(ICP_THREADS) match_map_kernel(const MatchBatch
       b.dists[b.in_off[p] + i] = r.d2;
     }
   }
-}
-
-// ---------------------------------------------------------------------------- map grids
-// Targets too large for the in-CTA layout get one grid each per call, in global memory, shared by every problem that
-// names the same target cloud.  Slots: the distinct map-class targets, numbered in target order on the device (a sort
-// of the problems by target id), so nothing depends on how many problems share a target or in which order they come.
-// Per slot: the mean (the kernel's own sequential float32 sum in point order; 0 for match), the bounding box of the
-// centred points, the geometry (grid_geometry, up to 1.5 cells per point), a stable radix sort of (slot, cell, index),
-// the centred points in that order with their original indices, the cell starts, and for point-to-plane the normals
-// (grid_surface_normal, one thread per point).  No coarse occupancy map: pass B of the pruned path searches instead.
-constexpr int MAP_THREADS = 256;
-constexpr unsigned MAP_NONE = 0xffffffffu;
-
-struct MapWs {  // device pointers into scratch[SCR_MAP]
-  int *slot;       // [P] slot of every problem, -1: not in the map class
-  int *n_slots;    // [1]
-  int *slot_tgt;   // [slot_cap] target cloud of every slot
-  MapGrid *grid;   // [slot_cap]
-  float2 *pts;     // [slot_cap * nt_max] centred points sorted by (slot, cell, index); padding at the end
-  int *orig;       // [slot_cap * nt_max]
-  int *cstart;     // [slot_cap][cell_cap]
-  float2 *nrm;     // [slot_cap * nt_max] point-to-plane only
-  int cell_cap;
-};
-
-__device__ __forceinline__ int map_count(const PackedClouds &t, int c) {
-  return t.cnt ? t.cnt[c] : t.off[c + 1] - t.off[c];
-}
-
-__global__ void map_flag_kernel(const PackedClouds t, const int *tgt_id, int P, int limit, unsigned *key, int *val,
-                                int *slot) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= P) return;
-  const int ti = tgt_id ? tgt_id[p] : p;
-  key[p] = map_count(t, ti) > limit ? (unsigned)ti : MAP_NONE;
-  val[p] = p;
-  slot[p] = -1;
-}
-
-__global__ void map_head_kernel(const unsigned *key, int P, int *head) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < P) head[i] = key[i] != MAP_NONE && (i == 0 || key[i] != key[i - 1]);
-}
-
-__global__ void map_slot_kernel(const unsigned *key, const int *val, const int *head, const int *sid, int P, int *slot,
-                                int *slot_tgt, int *n_slots) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= P) return;
-  if (key[i] != MAP_NONE) {
-    slot[val[i]] = sid[i] - 1;
-    if (head[i]) slot_tgt[sid[i] - 1] = (int)key[i];
-  }
-  if (i == P - 1) *n_slots = sid[i];
-}
-
-// one CTA per slot: mean, bounding box, geometry
-__global__ void __launch_bounds__(ICP_THREADS) map_setup_kernel(const PackedClouds t, const int *slot_tgt,
-                                                                 const int *n_slots, int center, int seq, MapGrid *grid) {
-  __shared__ float mean[2];
-  __shared__ float wred[4 * 16];
-  __shared__ double red[2 * 5 * 16];
-  const int s = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
-  if (s >= *n_slots) return;
-  const int ti = slot_tgt[s], nt = map_count(t, ti);
-  const float *tgt = t.pts + 2 * (size_t)t.off[ti];
-  float mx = 0.f, my = 0.f;
-  if (center) {  // as icp_body's set-up
-    if (seq) {
-      if (tid < 64) {
-        const float sum = seq_sum_warp_global(tgt + (tid >> 5), nt, 2);
-        if ((tid & 31) == 0) mean[tid >> 5] = __fdiv_rn(sum, (float)nt);
-      }
-      __syncthreads();
-      mx = mean[0], my = mean[1];
-    } else {  // (float64 mode: the reduction tree of a 512-thread CTA, not the in-CTA launch's -- that mode is not
-              //  bit-reproducible across CTA sizes anyway)
-      double sm[2] = {0.0, 0.0}, tot[2];
-      int phase = 0;
-      for (int i = tid; i < nt; i += nthr) sm[0] += (double)tgt[2 * i], sm[1] += (double)tgt[2 * i + 1];
-      block_sum<2>(sm, red, phase, tot);
-      mx = (float)(tot[0] / (double)nt), my = (float)(tot[1] / (double)nt);
-    }
-  }
-  float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
-  for (int i = tid; i < nt; i += nthr) {
-    const float x = tgt[2 * i] - mx, y = tgt[2 * i + 1] - my;
-    mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
-  }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
-    mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
-    mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
-    mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
-  }
-  if ((tid & 31) == 0) {
-    wred[(tid >> 5) * 4 + 0] = mn_x, wred[(tid >> 5) * 4 + 1] = mn_y;
-    wred[(tid >> 5) * 4 + 2] = mxx, wred[(tid >> 5) * 4 + 3] = mxy;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
-    for (int w = 0; w < (nthr >> 5); ++w) {
-      a = fminf(a, wred[w * 4 + 0]), bb = fminf(bb, wred[w * 4 + 1]);
-      c = fmaxf(c, wred[w * 4 + 2]), d = fmaxf(d, wred[w * 4 + 3]);
-    }
-    MapGridView g;
-    grid_geometry(nt, a, bb, c, d, 0.05f, g, nt + nt / 2 > 256 ? nt + nt / 2 : 256);
-    MapGrid m;
-    m.mean[0] = mx, m.mean[1] = my;
-    m.bbox[0] = a, m.bbox[1] = bb, m.bbox[2] = c, m.bbox[3] = d;
-    m.ox = g.ox, m.oy = g.oy, m.cell = g.cell, m.inv_cell = g.inv_cell;
-    m.nx = g.nx, m.ny = g.ny, m.n = nt, m.pad = 0;
-    grid[s] = m;
-  }
-}
-
-// sort key of every (slot, point): slot above, cell below; unused positions get the padding key (all ones)
-__global__ void map_keys_kernel(const PackedClouds t, const int *slot_tgt, const int *n_slots, const MapGrid *grid,
-                                int nt_max, unsigned long long *key, int *val) {
-  const int s = blockIdx.y;
-  const bool live = s < *n_slots;
-  const int ti = live ? slot_tgt[s] : 0, nt = live ? map_count(t, ti) : 0;
-  const float *tgt = t.pts + 2 * (size_t)(live ? t.off[ti] : 0);
-  MapGrid m;
-  if (live) m = grid[s];
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nt_max; j += gridDim.x * blockDim.x) {
-    const size_t i = (size_t)s * nt_max + j;
-    if (j < nt) {
-      const float x = tgt[2 * j] - m.mean[0], y = tgt[2 * j + 1] - m.mean[1];
-      const int c = grid_cell_coord(y, m.oy, m.inv_cell, m.ny) * m.nx + grid_cell_coord(x, m.ox, m.inv_cell, m.nx);
-      key[i] = ((unsigned long long)s << 32) | (unsigned)c;
-      val[i] = j;
-    } else {
-      key[i] = ~0ull;
-      val[i] = 0;
-    }
-  }
-}
-
-// after the sort: centred points in sorted order and every cell's first position (absolute in pts)
-__global__ void map_scatter_kernel(const PackedClouds t, const int *slot_tgt, const MapGrid *grid,
-                                   const unsigned long long *key, const int *val, int N, int cell_cap, float2 *pts,
-                                   int *cstart) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  const unsigned long long k = key[i];
-  if (k == ~0ull) return;
-  const int s = (int)(k >> 32), c = (int)(k & 0xffffffffu), j = val[i];
-  const MapGrid &m = grid[s];
-  const float *src = t.pts + 2 * ((size_t)t.off[slot_tgt[s]] + j);
-  pts[i] = make_float2(src[0] - m.mean[0], src[1] - m.mean[1]);
-  int *cs = cstart + (size_t)s * cell_cap;
-  const int pc = (i > 0 && (int)(key[i - 1] >> 32) == s) ? (int)(key[i - 1] & 0xffffffffu) : -1;
-  for (int cc = pc + 1; cc <= c; ++cc) cs[cc] = i;
-  if (i + 1 == N || (key[i + 1] >> 32) != (unsigned long long)s)
-    for (int cc = c + 1; cc <= m.nx * m.ny; ++cc) cs[cc] = i + 1;  // through the sentinel entry ncells
-}
-
-// point-to-plane: the normal at every sorted position, once per target
-__global__ void map_normals_kernel(const unsigned long long *key, const MapGrid *grid, const float2 *pts,
-                                   const int *cstart, const int *orig, int N, int cell_cap, int knn, float2 *nrm) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  const unsigned long long k = key[i];
-  if (k == ~0ull) return;
-  const int s = (int)(k >> 32);
-  const MapGrid &m = grid[s];
-  MapGridView g;
-  g.pts = pts, g.cstart = cstart + (size_t)s * cell_cap, g.orig = orig;
-  g.n = m.n, g.nx = m.nx, g.ny = m.ny, g.ox = m.ox, g.oy = m.oy, g.cell = m.cell, g.inv_cell = m.inv_cell;
-  float bd[GRID_KNN_MAX];
-  int bi[GRID_KNN_MAX];
-  nrm[i] = grid_surface_normal(g, i, knn, bd, bi, 1);
-}
-
-// Builds the map grids of the problems whose target has more than `limit` points.  slot_cap bounds the number of
-// distinct such targets.  Workspace (scratch[SCR_MAP]): 40 bytes per slot point (48 with normals) for slot_cap *
-// nt_max slot points, 4 * (1.5 nt_max + 257) bytes of cell table per slot, 28 bytes per problem, CUB's temporary
-// storage.  knn > 0: normals too.
-static int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, const int *tgt_id, int P, int limit,
-                     int slot_cap, bool center, bool seq, int knn, MapWs &w) {
-  const int nt_max = t.n_max;
-  const long long slots = (long long)slot_cap * nt_max;
-  SFE_REQUIRE(slots < INT_MAX, "map grids: %d targets of up to %d points exceed %d slot points", slot_cap, nt_max,
-              INT_MAX - 1);
-  SFE_REQUIRE(slot_cap <= 65535, "map grids: at most 65535 distinct map-sized targets per call (got up to %d)",
-              slot_cap);
-  const int N = (int)slots;
-  w.cell_cap = (nt_max + nt_max / 2 > 256 ? nt_max + nt_max / 2 : 256) + 1;
-  int slot_bits = 1;
-  while ((1ll << slot_bits) < slot_cap) ++slot_bits;
-  const int end_bit = 32 + slot_bits;
-
-  cub::DoubleBuffer<unsigned> pkeys;
-  cub::DoubleBuffer<int> pvals;
-  cub::DoubleBuffer<unsigned long long> keys;
-  cub::DoubleBuffer<int> vals;
-  size_t psort_bytes = 0, scan_bytes = 0, sort_bytes = 0;
-  SFE_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, psort_bytes, pkeys, pvals, P, 0, 32, st));
-  SFE_CUDA(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int *)nullptr, (int *)nullptr, P, st));
-  SFE_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, vals, N, 0, end_bit, st));
-  size_t temp_bytes = psort_bytes > scan_bytes ? psort_bytes : scan_bytes;
-  if (sort_bytes > temp_bytes) temp_bytes = sort_bytes;
-  char *base = nullptr;
-  size_t used = 0;
-  auto take = [&](size_t bytes) {
-    void *p = base ? base + used : nullptr;
-    used += (bytes + 255) & ~size_t(255);
-    return p;
-  };
-  unsigned *pk0, *pk1;
-  int *pv0, *pv1, *head, *sid;
-  unsigned long long *k0, *k1;
-  int *v0, *v1;
-  void *temp;
-  for (int pass = 0; pass < 2; ++pass) {  // pass 0 sizes the block, pass 1 carves it
-    used = 0;
-    pk0 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
-    pk1 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
-    pv0 = (int *)take(sizeof(int) * (size_t)P);
-    pv1 = (int *)take(sizeof(int) * (size_t)P);
-    head = (int *)take(sizeof(int) * (size_t)P);
-    sid = (int *)take(sizeof(int) * (size_t)P);
-    w.slot = (int *)take(sizeof(int) * (size_t)P);
-    w.n_slots = (int *)take(sizeof(int));
-    w.slot_tgt = (int *)take(sizeof(int) * (size_t)slot_cap);
-    w.grid = (MapGrid *)take(sizeof(MapGrid) * (size_t)slot_cap);
-    k0 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
-    k1 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
-    v0 = (int *)take(sizeof(int) * (size_t)N);
-    v1 = (int *)take(sizeof(int) * (size_t)N);
-    w.pts = (float2 *)take(sizeof(float2) * (size_t)N);
-    w.nrm = knn > 0 ? (float2 *)take(sizeof(float2) * (size_t)N) : nullptr;
-    w.cstart = (int *)take(sizeof(int) * (size_t)slot_cap * w.cell_cap);
-    temp = take(temp_bytes);
-    if (pass == 0) {
-      int rc = ensure(ctx, ctx->scratch[SCR_MAP], used, st);
-      if (rc != SFE_OK) return rc;
-      base = (char *)ctx->scratch[SCR_MAP].ptr;
-    }
-  }
-  const int pb = (P + MAP_THREADS - 1) / MAP_THREADS;
-  map_flag_kernel<<<pb, MAP_THREADS, 0, st>>>(t, tgt_id, P, limit, pk0, pv0, w.slot);
-  SFE_CUDA(cudaGetLastError());
-  pkeys = cub::DoubleBuffer<unsigned>(pk0, pk1);
-  pvals = cub::DoubleBuffer<int>(pv0, pv1);
-  SFE_CUDA(cub::DeviceRadixSort::SortPairs(temp, psort_bytes, pkeys, pvals, P, 0, 32, st));
-  map_head_kernel<<<pb, MAP_THREADS, 0, st>>>(pkeys.Current(), P, head);
-  SFE_CUDA(cudaGetLastError());
-  SFE_CUDA(cub::DeviceScan::InclusiveSum(temp, scan_bytes, (const int *)head, sid, P, st));
-  map_slot_kernel<<<pb, MAP_THREADS, 0, st>>>(pkeys.Current(), pvals.Current(), head, sid, P, w.slot, w.slot_tgt,
-                                              w.n_slots);
-  SFE_CUDA(cudaGetLastError());
-  map_setup_kernel<<<slot_cap, ICP_THREADS, 0, st>>>(t, w.slot_tgt, w.n_slots, center ? 1 : 0, seq ? 1 : 0, w.grid);
-  SFE_CUDA(cudaGetLastError());
-  int bps = (nt_max + 4 * MAP_THREADS - 1) / (4 * MAP_THREADS);
-  bps = bps < 1 ? 1 : (bps > 256 ? 256 : bps);
-  map_keys_kernel<<<dim3(bps, slot_cap), MAP_THREADS, 0, st>>>(t, w.slot_tgt, w.n_slots, w.grid, nt_max, k0, v0);
-  SFE_CUDA(cudaGetLastError());
-  keys = cub::DoubleBuffer<unsigned long long>(k0, k1);
-  vals = cub::DoubleBuffer<int>(v0, v1);
-  SFE_CUDA(cub::DeviceRadixSort::SortPairs(temp, sort_bytes, keys, vals, N, 0, end_bit, st));
-  w.orig = vals.Current();
-  const int nb = (N + MAP_THREADS - 1) / MAP_THREADS;
-  map_scatter_kernel<<<nb, MAP_THREADS, 0, st>>>(t, w.slot_tgt, w.grid, keys.Current(), w.orig, N, w.cell_cap, w.pts,
-                                                 w.cstart);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches += 9;  // six kernels, the two sorts and the scan counted once each
-  if (knn > 0) {
-    map_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), w.grid, w.pts, w.cstart, w.orig, N, w.cell_cap, knn,
-                                                   w.nrm);
-    SFE_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  return SFE_OK;
 }
 
 // ---------------------------------------------------------------------------- host side
@@ -981,7 +638,7 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
                           int limit, int slot_cap) {
   const bool plane = prm->minimizer == 1;
   MapWs w;
-  int rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, b.tgt_id, b.P, limit, slot_cap, true,
+  int rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, limit, slot_cap, true,
                      (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
   if (rc != SFE_OK) return rc;
   b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max;
@@ -1121,7 +778,7 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   ctx->launches++;
   if (nt_max <= limit) return SFE_OK;
   MapWs w;
-  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, nullptr, P, limit, P, false, true, 0, w);
+  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, limit, P, false, true, 0, w);
   if (rc != SFE_OK) return rc;
   b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
   b.map_cell_cap = w.cell_cap;

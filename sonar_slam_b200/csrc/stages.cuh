@@ -44,6 +44,8 @@ constexpr int DS_ANY_SIZE = -1;
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
                    float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot,
                    bool frame_class = false);
+// n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
+// the map class above it)
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
                        int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split);
 // problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu); (0, 0): one launch,
@@ -54,5 +56,32 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpP
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
               int32_t *ids, float *dists);
+
+// One map grid: a cloud too large for a one-CTA layout, built once per call in global memory (map_build).
+struct MapGrid {
+  float mean[2];  // cloud mean (icp_kernel's sequential float32 sum; 0 when the grid is not centred)
+  float bbox[4];  // bounding box of the centred points
+  float ox, oy, cell, inv_cell;
+  int nx, ny, n, pad;
+};
+
+struct MapWs {  // device pointers into scratch[SCR_MAP]
+  int *slot;       // [P] slot of every problem, -1: not in the map class
+  int *n_slots;    // [1]
+  int *slot_tgt;   // [slot_cap] cloud of every slot
+  MapGrid *grid;   // [slot_cap]
+  float2 *pts;     // [slot_cap * nt_max] (centred) x, y sorted by (slot, cell, index); padding at the end
+  int *orig;       // [slot_cap * nt_max] sorted position -> index in the slot's cloud
+  int *cstart;     // [slot_cap][cell_cap]: absolute position in pts of every cell's first point, entry nx * ny = end
+  float2 *nrm;     // [slot_cap * nt_max] point-to-plane only
+  int cell_cap;
+};
+
+// Map grids (map_grid.cu) of the clouds with more than `limit` points among those that P problems name (problem p:
+// cloud tgt_id[p], or p with tgt_id null); slot_cap bounds the number of distinct such clouds.  Points are read from
+// t.pts with a stride of `dim` floats (x, y first).  center: points centred on the cloud's mean (seq: icp_kernel's
+// sequential float32 sum, else a float64 sum); knn > 0: point-to-plane normals too.
+int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, const int *tgt_id, int P, int limit,
+              int slot_cap, bool center, bool seq, int knn, MapWs &w);
 
 }  // namespace sfe

@@ -114,6 +114,9 @@ def downsample_frames(pts, off, n_max, resolution, frame_points, cnt=None, ctx=N
 
 
 def remove_outlier(pts, off, n_max, radius, min_points, ctx=None):
+    """Batched pcl.remove_outlier (include/sonarfe.h: sfe_remove_outlier_dev) on packed clouds (pts [total,2|3] f32, off
+    [n+1] i32, cuda).  Clouds of any size: those above one CTA's shared memory (whole maps) run in the map class, a grid
+    in global memory with one thread per point, with the same results."""
     ctx = ctx or context(pts.device)
     n = off.numel() - 1
     out = torch.empty_like(pts)
