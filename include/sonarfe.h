@@ -152,11 +152,12 @@ SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uin
  *                       depth-first order.  The two-argument overload (points + descriptors,
  *                       pcl.cpp:143) is served by gathering descriptors with out_idx.
  *                       Any cloud size is accepted: clouds that fit one CTA's shared memory
- *                       (57 084 points on an H100) run one CTA each; larger ones (whole maps)
+ *                       (13 880 points on an H100) run one CTA each; larger ones (whole maps)
  *                       run in the same call on a grid-wide path (radix sort of path keys,
- *                       medoid sums one thread per member), with the same results.  Its
- *                       workspace holds 48 bytes for each of n_clouds * n_max slots (at most
- *                       2^31 - 1).  Trees stop at 15 levels (16 km at a 0.5 m resolution).
+ *                       medoid sums one thread per member), with the same results.  A call
+ *                       with a cloud above that limit takes at most 65 535 clouds and
+ *                       n_clouds * n_max slots (at most 2^31 - 1); its workspace holds 48 bytes
+ *                       per slot.  Trees stop at 15 levels (16 km at a 0.5 m resolution).
  * sfe_remove_outlier_*  bruce_slam.pcl.remove_outlier (pcl.cpp:54-74): PCL RadiusOutlierRemoval:
  *                       keep a point iff at least min_points OTHER points lie within `radius`;
  *                       input order is preserved.
@@ -174,8 +175,9 @@ SFE_API int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t
 SFE_API int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
                                    int n_max, double radius, int min_points, float *out_pts_dev,
                                    int32_t *out_idx_dev, int32_t *out_count_dev);
-/* the batched front end's per-frame down-sample: clouds of up to frame_points (<= 8191) points in its frame-class
- * kernel, larger ones in a launch laid out for n_max; cnt_dev (optional) holds the clouds' point counts, else
+/* the batched front end's per-frame down-sample: clouds of up to frame_points points in a launch laid out for them,
+ * larger ones in a launch laid out for n_max (at most 65 535; layouts above the one-CTA shared-memory limit keep
+ * their workspace in global memory, 16 bytes per point per SM); cnt_dev (optional) holds the clouds' point counts, else
  * off_dev[c + 1] - off_dev[c].  2-column clouds only.  Same results as sfe_downsample_dev. */
 SFE_API int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev,
                                       const int32_t *cnt_dev, int n_clouds, int n_max, int frame_points,

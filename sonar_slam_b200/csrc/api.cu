@@ -230,7 +230,7 @@ int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_de
   SFE_REQUIRE(ctx != nullptr, "sfe_downsample_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
   return downsample_run(ctx, ctx->stream, {pts_dev, off_dev, nullptr, n_max}, n_clouds, dim, resolution, out_pts_dev,
-                        out_idx_dev, out_count_dev, DS_ANY_SIZE, SCR_CLOUD);
+                        out_idx_dev, out_count_dev, DS_ANY_SIZE, SCR_CLOUD, WORK_DS);
 }
 
 int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, const int32_t *cnt_dev,
@@ -240,7 +240,7 @@ int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t 
   SFE_REQUIRE(frame_points > 0, "sfe_downsample_frames_dev: frame_points must be positive (got %d)", frame_points);
   SFE_CUDA(cudaSetDevice(ctx->device));
   return downsample_run(ctx, ctx->stream, {pts_dev, off_dev, cnt_dev, n_max}, n_clouds, 2, resolution, out_pts_dev,
-                        out_idx_dev, out_count_dev, frame_points, SCR_CLOUD, true);
+                        out_idx_dev, out_count_dev, frame_points, SCR_CLOUD, WORK_DS);
 }
 
 int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
@@ -281,7 +281,7 @@ static int cloud_filter_host(sfe_ctx *ctx, int which, const float *pts_host, int
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
     const PackedClouds in{d_pts, d_off, nullptr, n};
     int rc = which == 0 ? downsample_run(ctx, ctx->stream, in, 1, dim, resolution, d_out, d_idx, d_cnt, DS_ANY_SIZE,
-                                         SCR_CLOUD)
+                                         SCR_CLOUD, WORK_DS)
                         : remove_outlier_run(ctx, ctx->stream, in, 1, dim, radius, min_points, d_out, d_idx, d_cnt, 0);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(n_out, d_cnt, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));

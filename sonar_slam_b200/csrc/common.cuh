@@ -88,7 +88,8 @@ enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC =
        SCR_DS_GRID = 7, SCR_MAP = 8, SCR_RO_MAP = 9 };
 // Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
 // different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
-enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, SFE_WORK_COUNTERS = 3 };
+// (WORK_DS_SUBMAP: the window submaps' down-sample runs next to the frames' in the overlapped schedule)
+enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, WORK_DS_SUBMAP = 3, SFE_WORK_COUNTERS = 4 };
 
 // (re)allocate if too small, stream-ordered on `stream` (default: ctx->stream).  A buffer must only grow on a stream
 // that is ordered after every earlier user of the block and before every later one: the stream that uses it.

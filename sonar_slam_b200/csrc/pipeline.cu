@@ -492,11 +492,8 @@ static int fe_features(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const int32_t *cur_cnt = fe->cnt_a;
   if (p.resolution > 0.f) {
     fe->timer.tic(st, SFE_FE_DOWNSAMPLE);
-    // development switch: SFE_FE_DS_SPLIT=<points> takes downsample_kernel's layouts instead of the frame class
-    // (0: one capacity launch)
-    static const char *ds_split = getenv("SFE_FE_DS_SPLIT");
     rc = downsample_run(ctx, st, {cur, fe->off_pts + f0, cur_cnt + f0, (int)cap}, n, 2, p.resolution, fe->xy_b, fe->idx,
-                        fe->cnt_b + f0, ds_split ? atoi(ds_split) : FE_DS_FRAME, SCR_CLOUD, !ds_split);
+                        fe->cnt_b + f0, FE_DS_FRAME, SCR_CLOUD, WORK_DS);
     fe->timer.toc(st);
     if (rc != SFE_OK) return rc;
     cur = fe->xy_b, cur_cnt = fe->cnt_b;
@@ -551,9 +548,9 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const float *tgt = fe->tgt_a;
   const int32_t *tcnt = fe->tcnt_a;
   if (p.submap_resolution > 0.f) {
-    // (its own sort workspace: in the overlapped schedule it runs next to the frame down-sampling)
+    // (its own workspace and work counter: in the overlapped schedule it runs next to the frame down-sampling)
     int rc = downsample_run(ctx, st, {fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, tcap}, n, 2, p.submap_resolution,
-                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_SUBMAP);
+                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_SUBMAP, WORK_DS_SUBMAP);
     if (rc != SFE_OK) return rc;
     tgt = fe->tgt_b, tcnt = fe->tcnt_b;
   }

@@ -37,13 +37,12 @@ int cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint
                     int cap, int32_t *ij, float *xy, int32_t *count);
 int feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *frames, int F,
                       const uint8_t *lut_bgr, uint8_t *out, const char *what);  // what: the caller, for errors
-// n_split > 0: two launches by cloud size (cloud.cu), 0: one launch, DS_ANY_SIZE: clouds of any size (one-CTA kernel
-// up to the device's limit, grid-wide path above it).  frame_class: the first of the two launches is the front end's
-// frame kernel (n_split at most 8191 points)
+// n_split > 0: two launches of the one-CTA kernel by cloud size (cloud.cu; n_max at most 65 535 points),
+// DS_ANY_SIZE: clouds of any size (one-CTA kernel up to the device's limit, grid-wide path above it).  slot: scratch
+// buffer, counter: work counter (WORK_*) of the one-CTA launches.
 constexpr int DS_ANY_SIZE = -1;
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
-                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot,
-                   bool frame_class = false);
+                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot, int counter);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
 // the map class above it)
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,

@@ -99,8 +99,9 @@ def downsample(pts, off, n_max, resolution, ctx=None):
 
 
 def downsample_frames(pts, off, n_max, resolution, frame_points, cnt=None, ctx=None):
-    """The front end's per-frame down-sample on packed clouds: clouds of up to `frame_points` points in its frame-class
-    kernel, larger ones in a launch laid out for n_max (pts [total,2] f32, off [n+1] i32, optional cnt [n] i32, cuda).
+    """The front end's per-frame down-sample on packed clouds: clouds of up to `frame_points` points in a launch laid
+    out for them, larger ones in a launch laid out for n_max <= 65535 (pts [total,2] f32, off [n+1] i32, optional cnt
+    [n] i32, cuda).
     Same results as downsample()."""
     ctx = ctx or context(pts.device)
     n = off.numel() - 1

@@ -1,11 +1,6 @@
-"""GPU: the front end's per-frame down-sample (cloud.cu, downsample_frame_kernel behind ops.downsample_frames) compared
-exactly (indices, order, float32 points, counts) with the CPU oracle, on the bench bag's raw clouds and on the edge
-cases of its frame class; and the front end with the frame class against the layouts it replaced."""
-import json
-import os
-import subprocess
-import sys
-
+"""GPU: the front end's split down-sample (cloud.cu, downsample_cta_kernel behind ops.downsample_frames) compared
+exactly (indices, order, float32 points, counts) with the CPU oracle, on the bench bag's raw clouds, on the edge cases
+of its frame and submap classes, and on capacity launches whose workspace is in global memory."""
 import numpy as np
 import pytest
 import torch
@@ -15,8 +10,9 @@ from sonar_slam_b200 import ops, synth
 
 pytestmark = pytest.mark.gpu
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FRAME = 6144  # pipeline.cu, FE_DS_FRAME
+SUBMAP = 2048  # pipeline.cu, FE_SUBMAP_SPLIT
+MAX_POINTS = 65535  # cloud.cu, DSF_MAX_POINTS: the largest layout of the one-CTA kernel
 
 
 def _check(clouds, res, frame_points=FRAME, n_max=None, with_cnt=True):
@@ -96,48 +92,34 @@ def test_class_limit_and_capacity_launch():
     _check([past, at[:7]], 0.5, frame_points=FRAME, n_max=frame + 1)
 
 
-_FRONT_END = r"""
-import json, sys
-import numpy as np
-from oracle import featx_ref
-from sonar_slam_b200 import _lib, ops, pipeline, synth
-F = 160
-d = synth.make_trajectory_frames(F, seed=0)
-geo = featx_ref.Geometry(30.0 / 512, 512, d["bearings"])
-ctx = ops.context(0)
-maps = _lib.Maps(ctx, geo.map_x, geo.map_y, 512, 512, geo.width, geo.height)
-out = {}
-for mini in (0, 1):
-    fe = pipeline.FrontEnd(ctx, maps, max_frames=F, icp=_lib.IcpParams(smooth_length=0, max_iterations=20,
-                                                                     minimizer=mini))
-    fe.run_dev(d["frames"].cuda().data_ptr(), d["poses_odom"], F)
-    r = fe.results_dev()
-    cnt = ctx.to_host(r["cloud_count"], (F,), np.int32)
-    xy = ctx.to_host(r["cloud_xy"], (F, r["cloud_stride"], 2), np.float32).view(np.uint32)
-    out[mini] = {"T": ctx.to_host(r["T"], (F, 9), np.float32).view(np.uint32).tolist(),
-                 "status": ctx.to_host(r["status"], (F,), np.int32).tolist(),
-                 "iterations": ctx.to_host(r["iterations"], (F,), np.int32).tolist(),
-                 "inliers": ctx.to_host(r["inliers"], (F,), np.int32).tolist(),
-                 "cloud_count": cnt.tolist(), "clouds": [xy[i, :c].tolist() for i, c in enumerate(cnt)]}
-    fe.close()
-json.dump(out, open(sys.argv[1], "w"))
-"""
+@pytest.mark.parametrize("res", [4.0, 0.5, 0.1, 0.02])  # D = 4, 7, 10, 12
+def test_submap_class(bag_raw, res):
+    """The front end's window submaps: clouds of up to FE_SUBMAP_SPLIT points in a launch laid out for them, the
+    capacity launch laid out for 3 frames of 8192 points (workspace in global memory)."""
+    clouds = [c[:SUBMAP] for c in bag_raw[:5]] + [bag_raw[5][:700], np.zeros((0, 2), np.float32), bag_raw[6][:SUBMAP + 1]]
+    _check(clouds, res, frame_points=SUBMAP, n_max=3 * 8192)
 
 
-def test_front_end_equals_the_former_layouts(tmp_path):
-    """SFE_FE_DS_SPLIT (read once per process) takes downsample_kernel's layouts instead of the frame class: 0 the
-    former single capacity launch, 4096 two launches of it."""
-    script = tmp_path / "fe.py"
-    script.write_text(_FRONT_END)
-    runs = {}
-    for split in (None, "0", "4096"):
-        env = dict(os.environ)
-        env.pop("SFE_FE_DS_SPLIT", None)
-        env["PYTHONPATH"] = REPO + os.pathsep + env.get("PYTHONPATH", "")
-        if split is not None:
-            env["SFE_FE_DS_SPLIT"] = split
-        path = tmp_path / f"out_{split}.json"
-        subprocess.run([sys.executable, str(script), str(path)], cwd=REPO, env=env, check=True, timeout=600)
-        runs[split] = json.load(open(path))
-    assert sum(s == 0 for s in runs[None]["0"]["status"]) >= 80  # the bag exercises the scan matcher
-    assert runs[None] == runs["0"] == runs["4096"]
+def test_capacity_launch_in_global_memory():
+    """Layouts above the shared-memory limit (about 13.9 k points on an H100) keep their workspace in global memory:
+    clouds either side of the split, one of MAX_POINTS points, and a 15-level tree (two blobs 0.75 * res * 2^15
+    apart)."""
+    rng = np.random.default_rng(8)
+    res = 0.5
+    a = rng.uniform(0, 20 * res, (MAX_POINTS // 2, 2))
+    b = rng.uniform(0, 20 * res, (MAX_POINTS - MAX_POINTS // 2, 2)) + 0.75 * res * 2 ** 15
+    deep = np.concatenate([a, b]).astype(np.float32)
+    wide = rng.uniform(-300, 300, (40000, 2)).astype(np.float32)
+    small = rng.uniform(-30, 30, (3000, 2)).astype(np.float32)
+    clouds = [small, deep, wide[:FRAME], np.zeros((0, 2), np.float32), wide, small[:1]]
+    _check(clouds, res, frame_points=FRAME, n_max=MAX_POINTS)
+    # both launches in global memory: the split itself above the shared-memory limit
+    _check([wide, wide[:20000], deep[:30000], small], res, frame_points=20000, n_max=MAX_POINTS)
+
+
+def test_capacity_layout_above_the_limit_is_rejected():
+    from sonar_slam_b200 import _lib
+    pts = torch.zeros((MAX_POINTS + 1, 2), dtype=torch.float32, device="cuda")
+    off = torch.tensor([0, MAX_POINTS + 1], dtype=torch.int32, device="cuda")
+    with pytest.raises(_lib.SonarFEError, match="not supported"):
+        ops.downsample_frames(pts, off, MAX_POINTS + 1, 0.5, FRAME)

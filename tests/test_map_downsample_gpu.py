@@ -13,11 +13,26 @@ pytestmark = pytest.mark.gpu
 RESOLUTIONS = (0.5, 0.13, 7.0)
 
 
+DSF_STATIC_SMEM = 8624  # static shared memory of cloud.cu's downsample_cta_kernel<512, false> (tools/ptxas_table.py)
+
+
 def _cta_limit():
-    """Largest cloud the one-CTA kernel lays out: its layout needs 4 bytes per point + 16 of the device's opt-in
-    shared memory less 4 KiB (cloud.cu, downsample_cta_smem)."""
+    """Largest cloud the one-CTA kernel lays out in shared memory (cloud.cu, downsample_cta_limit): the largest n
+    whose layout (dsf_layout: two 16-bit index lists, 32-bit keys, head bits and float2 points, each array 16-byte
+    aligned) fits the device's opt-in shared memory less the kernel's static shared memory."""
     import torch
-    return (torch.cuda.get_device_properties(0).shared_memory_per_block_optin - 4096 - 16) // 4
+    budget = torch.cuda.get_device_properties(0).shared_memory_per_block_optin - DSF_STATIC_SMEM
+
+    def a16(x):
+        return (x + 15) // 16 * 16
+
+    def total(n):
+        return a16(4 * n) + a16(4 * n) + a16(4 * (n // 32 + 1)) + 8 * n
+
+    n = min(budget * 8 // 129, 32 * 512 - 1)
+    while n > 0 and total(n) > budget:
+        n -= 1
+    return n
 
 
 @functools.lru_cache(maxsize=None)
@@ -87,9 +102,9 @@ def test_one_point_repeated_is_one_leaf(gpu_ctx):
 
 
 @pytest.mark.parametrize("delta", [-1, 0, 1])
-def test_sizes_around_the_one_cta_limit(gpu_ctx, delta):
-    """limit - 1 and limit run in the one-CTA kernel (1 launch), limit + 1 on the grid-wide path (the one-CTA launch
-    for the small class plus 8); all three equal the oracle."""
+def test_sizes_around_the_shared_memory_limit(gpu_ctx, delta):
+    """limit - 1 and limit run in the one-CTA kernel with its layout in shared memory (1 launch), limit + 1 on the
+    grid-wide path (the one-CTA launch for the small class plus 8); all three equal the oracle."""
     from sonar_slam_b200 import _lib
     ctx = _lib.default_context()
     pts = _map(200000)[: _cta_limit() + delta]

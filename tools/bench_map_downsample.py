@@ -1,7 +1,7 @@
 """Whole-map down-sampling (pcl.downsample on SLAM.get_points-sized clouds): device time of sfe_downsample_dev on
 resident data (CUDA events), pcl.downsample end to end (copy in, kernels, copy out) and the CPU oracle on one thread,
-every result checked against the oracle; then a sweep of single clouds from 16 k points to the one-CTA limit with
-both paths (the grid-wide one from a build where every cloud takes it: tools/build_ds_variants.sh).
+every result checked against the oracle; then a sweep of single clouds either side of the one-CTA limit, as shipped
+and from a build where every cloud takes the grid-wide path (tools/build_ds_variants.sh).
 Prints one JSON line.
 
     python tools/bench_map_downsample.py [--out FILE] [--grid-lib scratch/lib_dsgrid.so]
@@ -94,11 +94,9 @@ def main():
         res["clouds"][name] = dict(points=len(pts), kept=len(want), device_ms=round(dev, 4),
                                    pcl_e2e_ms=round(median(e2e), 3), oracle_cpu_1thread_ms=round(cpu, 2), exact=exact)
 
-    props = torch.cuda.get_device_properties(0)
-    limit = (props.shared_memory_per_block_optin - 4096 - 16) // 4  # cloud.cu: downsample_cta_smem
-    sizes = [16384, 24576, 32768, 40960, 49152, limit]
-    res["one_cta_limit"] = limit
-    res["sweep_one_cta_ms"] = sweep(sizes)
+    # either side of the one-CTA limit (13 880 points on an H100: cloud.cu, downsample_cta_limit)
+    sizes = [4096, 8192, 13000, 16384, 24576, 57084]
+    res["sweep_ms"] = sweep(sizes)
     if os.path.exists(args.grid_lib):
         env = dict(os.environ, SFE_LIB_PATH=os.path.abspath(args.grid_lib))
         p = subprocess.run([sys.executable, os.path.abspath(__file__), "--sweep", ",".join(map(str, sizes))],

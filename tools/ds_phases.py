@@ -3,11 +3,10 @@ bench.py's workload.
 
     bash tools/build_ds_variants.sh           # scratch/lib_dsphases.so, built with -DSFE_DS_PHASE_CLOCKS
     SFE_LIB_PATH=scratch/lib_dsphases.so python tools/ds_phases.py [--frames 4096] [--steps 3]
-    SFE_FE_DS_SPLIT=0 SFE_LIB_PATH=...   # the same for the former layout (downsample_kernel, one capacity launch)
 
 Runs the same seeded bag and front-end parameters as bench.py (sfe_frontend_run_dev) and prints, from thread 0 of
 every CTA (cloud.cu: DS_PH_MARK), SM cycles per cloud for each phase, the down-sample stage time by CUDA events, and
-the CTAs per SM of the launches.  The window submaps' down-sample runs downsample_kernel too and would add its clouds
+the CTAs per SM of the last launch.  The window submaps' down-sample runs the same kernel and would add its clouds
 to the same counters, so the submap thinning is switched off here (submap_resolution = 0; ICP then matches unthinned
 targets, which does not touch the frame filters)."""
 import argparse
@@ -37,7 +36,7 @@ def main():
         sys.exit(f"{_lib.LIB_PATH} was built without -DSFE_DS_PHASE_CLOCKS (see tools/build_ds_variants.sh)")
     lib.sfe_ds_phase_clocks.argtypes = [ctypes.POINTER(ctypes.c_ulonglong), ctypes.c_int]
     lib.sfe_ds_phase_clocks.restype = ctypes.c_int
-    buf = (ctypes.c_ulonglong * 12)()
+    buf = (ctypes.c_ulonglong * 11)()
 
     def clocks(reset):
         if lib.sfe_ds_phase_clocks(buf, 1 if reset else 0) != 0:
@@ -63,14 +62,12 @@ def main():
     stage = fe.get_timing()
     fe.set_timing(False)
     c = clocks(reset=True)
-    cyc, cnt, per_sm = c[:5], c[5:10], c[10:12]
+    cyc, cnt, per_sm = c[:5], c[5:10], c[10]
     clouds = max(cnt[0], 1)
     rows = [{"phase": name, "cycles": cyc[k] / clouds, "count": cnt[k]} for k, name in enumerate(PHASES)]
     total = sum(r["cycles"] for r in rows)
     prop = torch.cuda.get_device_properties(0)
-    layout = os.environ.get("SFE_FE_DS_SPLIT")
-    print(f"{prop.name}, {prop.multi_processor_count} SMs; {F} frames x {args.steps} steps; "
-          f"layout: {'SFE_FE_DS_SPLIT=' + layout if layout is not None else 'frame class'}")
+    print(f"{prop.name}, {prop.multi_processor_count} SMs; {F} frames x {args.steps} steps")
     print(f"clouds {cnt[0] // args.steps} per step")
     print(f"{'phase':28s} {'cycles per cloud':>17s} {'share':>8s}")
     for r in rows:
@@ -78,11 +75,11 @@ def main():
     print(f"{'total':28s} {total:17.0f}")
     ds_ms = stage["downsample"][0] / args.steps
     print(f"downsample stage (CUDA events): {ds_ms:.3f} ms per step")
-    print(f"CTAs per SM (frame kernel / downsample_kernel, 0 = none): {per_sm}")
+    print(f"CTAs per SM of the last launch: {per_sm}")
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"rows": rows, "cloud_cycles": total, "downsample_ms_per_step": ds_ms, "ctas_per_sm": per_sm,
-                       "layout": layout, "gpu": prop.name}, f, indent=1)
+                       "gpu": prop.name}, f, indent=1)
 
 
 if __name__ == "__main__":

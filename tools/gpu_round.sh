@@ -18,7 +18,6 @@ for s in $steps; do
     stages)   timeout 600 python tools/bench_stages.py 4096 1184 > gpurun_out/${tag}_stages.log 2>&1; cat gpurun_out/${tag}_stages.log ;;
     bench)    timeout 900 python bench.py > gpurun_out/${tag}_bench.json 2> gpurun_out/${tag}_bench.err; tail -c 3000 gpurun_out/${tag}_bench.json; tail -3 gpurun_out/${tag}_bench.err ;;
     bench_plane) timeout 900 python bench.py --minimizer plane --pairs 0 --cpu-sample 64 > gpurun_out/${tag}_bench_plane.json 2> gpurun_out/${tag}_bench_plane.err; tail -c 2500 gpurun_out/${tag}_bench_plane.json; tail -3 gpurun_out/${tag}_bench_plane.err ;;
-    stage_sweep) for v in 0 4800 5056; do echo "SFE_FE_DS_SPLIT=$v"; SFE_FE_DS_SPLIT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
     icp_sweep) for v in 2 3 5; do echo "SFE_ICP_SMALL_MULT=$v"; SFE_ICP_SMALL_MULT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
     margin_sweep) for v in 2 4 6 10 16 32; do echo "SFE_ICP_MARGIN_MULT=$v"; SFE_ICP_MARGIN_MULT=$v timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 3 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3))"; done ;;
     icp_variants) for so in sonar_slam_b200/libsonarfe.so scratch/lib_*.so; do echo "== $so"; SFE_LIB_PATH=$PWD/$so timeout 300 python bench.py --pairs 0 --cpu-sample 8 --steps 5 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read()); print({k: round(v,3) for k,v in d['stage_ms_per_step'].items()}, round(d['ms_per_step'],3), round(d['config3_icp']['fixed20']['ms_per_wave'],3))"; done ;;

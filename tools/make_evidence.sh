@@ -44,7 +44,7 @@ fi
   if [ -f $G/${tag}_prof_pipeline.ncu-rep ]; then
     echo "== icp_kernel<128,6,false>, the front end's class, 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi6ELb0 icp.cu 12
     echo "== cart_scatter_kernel, 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep cart_scatter $td/featx.sm_90a.cubin cart_scatter featx.cu 10
-    echo "== downsample_kernel (frames), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "downsample#2" $td/cloud.sm_90a.cubin downsample_kernel cloud.cu 12
+    echo "== downsample_cta_kernel (frames), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "downsample#2" $td/cloud.sm_90a.cubin downsample_cta_kernel cloud.cu 12
   fi
   [ -f $G/${tag}_prof_plane.ncu-rep ] && { echo "== icp_kernel<128,6,true> (point-to-plane), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_plane.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi6ELb1 icp.cu 10; }
   rm -rf $td
