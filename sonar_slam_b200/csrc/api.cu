@@ -3,6 +3,8 @@
 #include <cudaTypedefs.h>
 
 #include <algorithm>
+#include <iterator>
+#include <map>
 #include <mutex>
 #include <vector>
 
@@ -42,6 +44,48 @@ int ensure_pinned(sfe_ctx *ctx, size_t bytes) {
   ctx->pinned = nullptr, ctx->pinned_cap = 0;
   SFE_CUDA(cudaMallocHost(&ctx->pinned, bytes * 2));
   ctx->pinned_cap = bytes * 2;
+  return SFE_OK;
+}
+
+static std::mutex g_fn_mu;                                    // guards the two tables below
+static std::map<const void *, size_t> g_static_smem;          // kernel -> its static shared memory
+static std::map<std::pair<int, const void *>, size_t> g_dyn;  // (device, kernel) -> dynamic shared memory allowed
+
+int cta_smem_budget(const sfe_ctx *ctx, const void *fn, size_t *budget) {
+  std::lock_guard<std::mutex> lock(g_fn_mu);
+  auto it = g_static_smem.find(fn);
+  if (it == g_static_smem.end()) {  // a property of the kernel, the same on every device: read once
+    cudaFuncAttributes attr;
+    SFE_CUDA(cudaFuncGetAttributes(&attr, fn));
+    it = g_static_smem.emplace(fn, attr.sharedSizeBytes).first;
+  }
+  *budget = (size_t)ctx->max_smem_optin - it->second;
+  return SFE_OK;
+}
+
+int raise_smem_limit(const sfe_ctx *ctx, const void *fn, size_t bytes) {
+  std::lock_guard<std::mutex> lock(g_fn_mu);
+  size_t &cur = g_dyn[{ctx->device, fn}];
+  if (bytes > cur) {
+    SFE_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    cur = bytes;
+  }
+  return SFE_OK;
+}
+
+int ctas_per_sm(sfe_ctx *ctx, const void *fn, int threads, size_t bytes, int *per_sm) {
+  int rc = raise_smem_limit(ctx, fn, bytes);
+  if (rc != SFE_OK) return rc;
+  for (const auto &e : ctx->occ)
+    if (e.fn == fn && e.smem == bytes && e.threads == threads) {
+      *per_sm = e.per_sm;
+      return SFE_OK;
+    }
+  int q = 1;
+  SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&q, fn, threads, bytes));
+  *per_sm = q < 1 ? 1 : q;
+  ctx->occ[ctx->occ_next] = {fn, bytes, threads, *per_sm};
+  ctx->occ_next = (ctx->occ_next + 1) % (int)std::size(ctx->occ);
   return SFE_OK;
 }
 
@@ -210,19 +254,6 @@ int sfe_cfar_host(sfe_ctx *ctx, const void *img_host, int dtype, int n_frames, i
 }  // extern "C"
 
 // ============================================================================ clouds / match / ICP
-namespace sfe {
-// carve `n` sub-buffers out of one grow-only scratch block (256 B aligned each)
-struct Carver {
-  char *base = nullptr;
-  size_t off = 0;
-  void *take(size_t bytes) {
-    void *p = base ? base + off : nullptr;
-    off += (bytes + 255) & ~size_t(255);
-    return p;
-  }
-};
-}  // namespace sfe
-
 extern "C" {
 
 int sfe_downsample_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim, int n_max,

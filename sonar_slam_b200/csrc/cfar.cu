@@ -945,8 +945,8 @@ static int launch_u8_gate4(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_
   const size_t smem = cg_off_omask(lut_n) + (m ? CF_CH * CG_W : 0);
 #define SFE_GO(M_, B_)                                                                                              \
   do {                                                                                                              \
-    SFE_CUDA(cudaFuncSetAttribute(cfar_u8_gate4_kernel<ALG, M_, B_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                                  (int)smem));                                                                      \
+    const int rc = raise_smem_limit(ctx, (const void *)cfar_u8_gate4_kernel<ALG, M_, B_>, smem);                    \
+    if (rc != SFE_OK) return rc;                                                                                    \
     cfar_u8_gate4_kernel<ALG, M_, B_><<<grid, CF_W, smem, st>>>(in_map, p, lut, lut_n, gate_add);          \
   } while (0)
   if (m && b) SFE_GO(true, true);
@@ -968,7 +968,8 @@ static int launch_exact(sfe_ctx *ctx, cudaStream_t st, const InT *img, const Cfa
         set_error("OS-CFAR: train_hs=%d needs %zu B of shared memory (max %d)", p.T, smem, ctx->max_smem_optin);
         return SFE_ERR_UNSUPPORTED;
       }
-      SFE_CUDA(cudaFuncSetAttribute(cfar_exact_kernel<InT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      const int rc = raise_smem_limit(ctx, (const void *)cfar_exact_kernel<InT>, smem);
+      if (rc != SFE_OK) return rc;
     }
   }
   cfar_exact_kernel<InT><<<p.F * p.strips, CF_W, smem, st>>>(img, p, only_flagged);

@@ -62,8 +62,10 @@ struct sfe_ctx {
   // thread-local statics: a new context may get a recycled device address, two contexts may share a thread)
   double cfar_lut_key[6] = {-1, 0, 0, 0, 0, 0};  // parameters of the table held in scratch[SCR_CFAR_LUT]
   const void *cfar_lut_buf = nullptr;            // ... and the buffer it was uploaded to (null = none)
-  struct OccEntry { size_t smem; int threads, per_sm, variant; } icp_occ[8] = {};
-  int icp_occ_next = 0;
+  // CTAs per SM of the persistent one-CTA launches (sfe::ctas_per_sm), by (kernel, threads, dynamic bytes); room for
+  // every configuration one front-end step launches
+  struct OccEntry { const void *fn; size_t smem; int threads, per_sm; } occ[16] = {};
+  int occ_next = 0;
   sfe::JpegState *jpeg = nullptr;       // JPEG decoder state, created on first use
   sfe::PngState *png = nullptr;         // PNG decoder state, created on first use
   cudaStream_t copy_stream = nullptr;   // host flavours that overlap copies with kernels (featx.cu), created on first use
@@ -96,6 +98,40 @@ enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, WORK_DS_SUBMAP = 3, SFE_WORK_CO
 int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes);
 int ensure(sfe_ctx *ctx, Buffer &b, size_t bytes, cudaStream_t stream);
 int ensure_pinned(sfe_ctx *ctx, size_t bytes);
+
+// Carves sub-buffers out of one grow-only scratch block, 256 B aligned each.  Two passes over the same take() calls:
+// the first (base null) sizes the block in `off`, the second, after ensure() and with base set, hands out pointers.
+struct Carver {
+  char *base = nullptr;
+  size_t off = 0;
+  void *take(size_t bytes) {
+    void *p = base ? base + off : nullptr;
+    off += (bytes + 255) & ~size_t(255);
+    return p;
+  }
+};
+
+// ---------------------------------------------------------------- one-CTA launches (api.cu)
+// The largest n <= cap whose layout bytes_of(n) fits `budget`; bytes_of must not decrease with n.
+template <class BytesOf>
+int largest_layout(int cap, size_t budget, BytesOf bytes_of) {
+  int lo = 0, hi = cap;
+  while (lo < hi) {
+    const int mid = lo + (hi - lo + 1) / 2;
+    if (bytes_of(mid) <= budget) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+// *budget = the dynamic shared memory one CTA of `fn` may take on ctx's device: the opt-in limit less fn's static
+// shared memory.
+int cta_smem_budget(const sfe_ctx *ctx, const void *fn, size_t *budget);
+// Lets `fn` take `bytes` of dynamic shared memory.  The attribute belongs to (function, device), not to a context, so
+// it is only ever raised, process-wide: a launch on another thread's context never finds it lowered under its layout.
+int raise_smem_limit(const sfe_ctx *ctx, const void *fn, size_t bytes);
+// raise_smem_limit, then *per_sm = CTAs of `fn` per SM with `threads` threads and `bytes` of dynamic shared memory (at
+// least 1), cached in the context.
+int ctas_per_sm(sfe_ctx *ctx, const void *fn, int threads, size_t bytes, int *per_sm);
 
 // ---------------------------------------------------------------- compressed pings (jpeg.cu, png.cu)
 // Orientation (tag 0x0112 of IFD0) of a TIFF structure, as carried by JPEG's APP1 "Exif" segment and PNG's eXIf

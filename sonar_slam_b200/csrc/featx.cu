@@ -437,8 +437,10 @@ static int launch_cart(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const u
   const int wpr = (m->B + 31) / 32;
   const size_t smem = (size_t)FPB * m->R * wpr * sizeof(uint32_t);
   if (smem > (size_t)ctx->max_smem_optin - 1024) return SFE_ERR_UNSUPPORTED;
-  if (smem > 40 * 1024)
-    SFE_CUDA(cudaFuncSetAttribute(cart_points_kernel<FPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem > 40 * 1024) {
+    const int rc = raise_smem_limit(ctx, (const void *)cart_points_kernel<FPB>, smem);
+    if (rc != SFE_OK) return rc;
+  }
   const int grid = (F + FPB - 1) / FPB;
   cart_points_kernel<FPB><<<grid, FX_THREADS, smem, st>>>(
       (const MapEntry *)m->table, m->rows * m->cols, m->cols, m->rows, m->R, m->B, wpr, mask, bits, F, cap, m->width,
@@ -487,10 +489,10 @@ int sfe::cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const
     const size_t smem = sizeof(uint32_t) * (pw + cw + (pw + 1) / 2 + 1);
     // (the emission's rank table of Cartesian word pairs reuses the polar plane: it must fit there)
     if (m->inv_off != nullptr && smem <= (size_t)ctx->max_smem_optin - 2048 && (cw + 1) / 2 <= pw && !ctx_force_gather(ctx)) {
-      SFE_CUDA(cudaFuncSetAttribute(cart_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      int per_sm = 1;
-      SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cart_scatter_kernel, FXS_THREADS, smem));
-      int grid = ctx->sm_count * (per_sm < 1 ? 1 : per_sm);
+      int per_sm;
+      const int rc = ctas_per_sm(ctx, (const void *)cart_scatter_kernel, FXS_THREADS, smem, &per_sm);
+      if (rc != SFE_OK) return rc;
+      int grid = ctx->sm_count * per_sm;
       if (grid > F) grid = F;
       SFE_CUDA(cudaMemsetAsync(ctx->work + WORK_CART, 0, sizeof(int), st));
       cart_scatter_kernel<<<grid, FXS_THREADS, smem, st>>>(

@@ -97,6 +97,25 @@ __device__ __forceinline__ void block_sum(double (&v)[K], double *scratch /* [2]
   }
 }
 
+// (min x, min y, max x, max y) over the CTA from every thread's partial bounds: warp shuffles, then thread 0 over the
+// warps' results in `red` (shared, one entry per warp).  The result is valid in thread 0 only; min and max are exact,
+// so the order does not matter.
+__device__ __forceinline__ float4 block_bounds(float4 m, float4 *red) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    m.x = fminf(m.x, __shfl_xor_sync(0xffffffffu, m.x, d));
+    m.y = fminf(m.y, __shfl_xor_sync(0xffffffffu, m.y, d));
+    m.z = fmaxf(m.z, __shfl_xor_sync(0xffffffffu, m.z, d));
+    m.w = fmaxf(m.w, __shfl_xor_sync(0xffffffffu, m.w, d));
+  }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+      m.x = fminf(m.x, red[w].x), m.y = fminf(m.y, red[w].y), m.z = fmaxf(m.z, red[w].z), m.w = fmaxf(m.w, red[w].w);
+  return m;
+}
+
 // One sequential sum over values in global memory, p[0], p[stride], ... (the reference cloud's mean, once per
 // problem): lane j holds term base + j and a shuffle hands term j to every lane, so all lanes carry the same
 // running sum; eight batches (256 terms) are requested at once and the next eight are in flight while these are

@@ -18,7 +18,6 @@
 //   Counter / Differential checkers on one thread.
 // CTAs are persistent over the problem list (batch of keyframe pairs / of initial guesses).
 #include <algorithm>
-#include <mutex>
 #include <type_traits>
 
 #include <climits>
@@ -501,7 +500,7 @@ static int pick_max_cells(int nt_max) {
 
 // Shared memory of icp_kernel's layout for problems of up to ns_max x nt_max points (both >= 1) after big problems
 // traded cell-table entries (coarser cells) for room; *max_cells receives the table's size.
-static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, int optin, int *max_cells) {
+static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, size_t budget, int *max_cells) {
   const bool use_order = ns_max > 1024;
   auto smem_for = [&](int mc) {
     return ((sizeof(IcpShared) + 15) & ~size_t(15)) + sizeof(float2) * (size_t)nt_max +
@@ -511,35 +510,32 @@ static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, int optin, int *m
            (plane && ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
   };
   int mc = pick_max_cells(nt_max);
-  while (smem_for(mc) > (size_t)optin && mc > nt_max / 4 + 256) mc -= mc / 8;
+  while (smem_for(mc) > budget && mc > nt_max / 4 + 256) mc -= mc / 8;
   *max_cells = mc;
   return smem_for(mc);
-}
-
-// The largest target icp_kernel's layout holds next to sources of ns_max points (0: none): targets above it are the
-// map class.
-static int icp_cta_limit(int ns_max, bool plane, int optin) {
-  int lo = 0, hi = 65535, mc;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) / 2;
-    if (icp_cta_smem(ns_max, mid, plane, optin, &mc) <= (size_t)optin) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
 }
 
 static size_t match_cta_smem(int nt_max) {
   return sizeof(float2) * (size_t)nt_max + sizeof(uint32_t) * (size_t)((pick_max_cells(nt_max) + 2) / 2 + 1) + 16;
 }
 
-static int match_cta_limit(int optin) {
-  int lo = 0, hi = 65535;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) / 2;
-    if (match_cta_smem(mid) <= (size_t)optin) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
+// CTA size follows the source size (one NN query per thread and iteration is the sweet spot)
+// (chosen on the config-4 replay for ~360-point sources; not re-measured on H100)
+static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 1536 ? 256 : ICP_THREADS); }
+
+// icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget).
+// 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers.
+static const void *icp_kernel_for(int threads, size_t smem, bool plane) {
+  if (threads == 128) return plane ? (const void *)icp_kernel<128, 7, true> : (const void *)icp_kernel<128, 7, false>;
+  if (threads == 256) return plane ? (const void *)icp_kernel<256, 4, true> : (const void *)icp_kernel<256, 4, false>;
+  if (smem <= 110 * 1024) return plane ? (const void *)icp_kernel<512, 2, true> : (const void *)icp_kernel<512, 2, false>;
+  return plane ? (const void *)icp_kernel<512, 1, true> : (const void *)icp_kernel<512, 1, false>;
+}
+
+// Shared memory icp_kernel's layouts may take next to sources of ns_max points: the budget of the instantiation that
+// runs the largest of them.
+static int icp_cta_budget(const sfe_ctx *ctx, int ns_max, bool plane, size_t *budget) {
+  return cta_smem_budget(ctx, icp_kernel_for(icp_threads(ns_max), ctx->max_smem_optin, plane), budget);
 }
 
 static void icp_tuning(IcpBatch &b) {
@@ -565,50 +561,20 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
   b.cell_scale = 1.0f;
   b.prm = *prm;
   icp_tuning(b);
-  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, prm->minimizer == 1, ctx->max_smem_optin, &b.max_cells);
-  if (smem > (size_t)ctx->max_smem_optin) {
-    set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %d)", ns_max, nt_max, smem,
-              ctx->max_smem_optin);
+  const bool plane = prm->minimizer == 1;
+  size_t budget;
+  int rc = icp_cta_budget(ctx, b.ns_max, plane, &budget);
+  if (rc != SFE_OK) return rc;
+  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, budget, &b.max_cells);
+  if (smem > budget) {
+    set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, nt_max, smem,
+              budget);
     return SFE_ERR_UNSUPPORTED;
   }
-  // CTA size follows the source size (one NN query per thread and iteration is the sweet spot)
-  // (chosen on the config-4 replay for ~360-point sources; not re-measured on H100)
-  const int threads = b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS);
-  // instantiation: (threads, register budget).  512-thread CTAs whose shared memory allows only one per SM get the
-  // full 128 registers.
-  const int variant = threads == 128 ? 0 : (threads == 256 ? 1 : (smem > 110 * 1024 ? 3 : 2));
-  const bool plane = prm->minimizer == 1;
-  const void *fn = plane ? (variant == 0   ? (const void *)icp_kernel<128, 7, true>
-                            : variant == 1 ? (const void *)icp_kernel<256, 4, true>
-                            : variant == 2 ? (const void *)icp_kernel<512, 2, true>
-                                           : (const void *)icp_kernel<512, 1, true>)
-                         : (variant == 0   ? (const void *)icp_kernel<128, 7, false>
-                            : variant == 1 ? (const void *)icp_kernel<256, 4, false>
-                            : variant == 2 ? (const void *)icp_kernel<512, 2, false>
-                                           : (const void *)icp_kernel<512, 1, false>);
-  // the attribute / occupancy queries are cached in the context per (variant, smem): the front end calls this per
-  // copy chunk
-  {  // the attribute belongs to (function, device), not to a context: only ever raise it, process-wide
-    static std::mutex mu;
-    static size_t attr[64][8] = {};
-    std::lock_guard<std::mutex> lock(mu);
-    size_t &cur = attr[ctx->device & 63][variant + (plane ? 4 : 0)];
-    if (smem > cur) {
-      SFE_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      cur = smem;
-    }
-  }
-  int c_per_sm = 0;
-  for (const auto &e : ctx->icp_occ)
-    if (e.per_sm > 0 && e.smem == smem && e.threads == threads && e.variant == variant + (plane ? 4 : 0)) c_per_sm = e.per_sm;
-  if (c_per_sm == 0) {
-    int q = 1;
-    SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&q, fn, threads, smem));
-    c_per_sm = q < 1 ? 1 : q;
-    ctx->icp_occ[ctx->icp_occ_next] = {smem, threads, c_per_sm, variant + (plane ? 4 : 0)};
-    ctx->icp_occ_next = (ctx->icp_occ_next + 1) % 8;
-  }
-  const int per_sm = c_per_sm;
+  const int threads = icp_threads(b.ns_max);
+  const void *fn = icp_kernel_for(threads, smem, plane);
+  int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
+  if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
 #ifdef SFE_ICP_PHASE_CLOCKS
   icp_phase_per_sm[threads == 128 ? 0 : threads == 256 ? 1 : 2] = per_sm;
 #endif
@@ -618,7 +584,7 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
   if (per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
   const size_t orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
   const size_t nrm_bytes = plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0;
-  int rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes, st);
+  rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes, st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
   b.nrm_ws = plane ? (float2 *)((char *)ctx->scratch[SCR_ICP].ptr + orig_bytes) : nullptr;
@@ -659,17 +625,15 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
               ctx->max_smem_optin);
     return SFE_ERR_UNSUPPORTED;
   }
-  const int threads = b.ns_max <= 640 ? 128 : (b.ns_max <= 1536 ? 256 : ICP_THREADS);
+  const int threads = icp_threads(b.ns_max);
   const void *fn = plane ? (threads == 128   ? (const void *)icp_map_kernel<128, 7, true>
                             : threads == 256 ? (const void *)icp_map_kernel<256, 4, true>
                                              : (const void *)icp_map_kernel<512, 1, true>)
                          : (threads == 128   ? (const void *)icp_map_kernel<128, 7, false>
                             : threads == 256 ? (const void *)icp_map_kernel<256, 4, false>
                                              : (const void *)icp_map_kernel<512, 1, false>);
-  SFE_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 1;
-  SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
-  if (per_sm < 1) per_sm = 1;
+  int per_sm;
+  if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
   int grid = ctx->sm_count * per_sm;
   if (grid > b.P) grid = b.P;
   if (grid < b.P) {  // persistent CTAs
@@ -716,15 +680,20 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P;
   if (!classes) {
-#ifdef SFE_ICP_MAP_ALL  // development build (tools/build_icp_map_variant.sh): every target takes the map class
-    const int limit = 0;
-#else
-    const int limit = icp_cta_limit(ns_max > 0 ? ns_max : 1, prm->minimizer == 1, ctx->max_smem_optin);
-#endif
+    // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
+    const int ns = ns_max > 0 ? ns_max : 1;
+    const bool plane = prm->minimizer == 1;
+    size_t budget;
+    int rc = icp_cta_budget(ctx, ns, plane, &budget);
+    if (rc != SFE_OK) return rc;
+    int mc;
+    const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
+      return icp_cta_smem(ns, nt, plane, budget, &mc);
+    });
     if (nt_max <= limit) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
     if (limit > 0) {
       b.class_mode = 1;
-      int rc = icp_launch(ctx, st, prm, b, ns_max, limit);
+      rc = icp_launch(ctx, st, prm, b, ns_max, limit);
       if (rc != SFE_OK) return rc;
     }
     const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
@@ -749,9 +718,11 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   if (P == 0) return SFE_OK;
   SFE_REQUIRE(ref.pts && ref.off && in.pts && in.off && ids && dists, "match: null pointer");
   SFE_REQUIRE(!ref.cnt && !in.cnt, "match: per-cloud counts are not supported");
-  cudaFuncAttributes fa;  // the dynamic layout shares the opt-in limit with the kernel's static shared memory
-  SFE_CUDA(cudaFuncGetAttributes(&fa, match_kernel));
-  const int limit = match_cta_limit(ctx->max_smem_optin - (int)fa.sharedSizeBytes);
+  size_t budget;
+  int rc = cta_smem_budget(ctx, (const void *)match_kernel, &budget);
+  if (rc != SFE_OK) return rc;
+  // (MAP_CLASS_ALL: references of one point are taken by both kernels, with the same result)
+  const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, match_cta_smem);
   MatchBatch b{};
   b.ref_pts = ref.pts, b.ref_off = ref.off, b.in_pts = in.pts, b.in_off = in.off;
   b.P = P, b.max_dist = max_dist;
@@ -764,13 +735,11 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
               ctx->max_smem_optin);
     return SFE_ERR_UNSUPPORTED;
   }
-  SFE_CUDA(cudaFuncSetAttribute(match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 1;
-  SFE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, match_kernel, ICP_THREADS, smem));
-  if (per_sm < 1) per_sm = 1;
+  int per_sm;
+  if ((rc = ctas_per_sm(ctx, (const void *)match_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
   int grid = ctx->sm_count * per_sm;
   if (grid > P) grid = P;
-  int rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
+  rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
   match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);

@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(MAP_SETUP_THREADS) map_setup_kernel(const Pack
                                                                        const int *n_slots, int center, int seq,
                                                                        MapGrid *grid) {
   __shared__ float mean[2];
-  __shared__ float wred[4 * 16];
+  __shared__ float4 bred[MAP_SETUP_THREADS / 32];
   __shared__ double red[2 * 5 * 16];
   const int s = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
   if (s >= *n_slots) return;
@@ -82,34 +82,18 @@ __global__ void __launch_bounds__(MAP_SETUP_THREADS) map_setup_kernel(const Pack
       mx = (float)(tot[0] / (double)nt), my = (float)(tot[1] / (double)nt);
     }
   }
-  float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
+  float4 bnd = make_float4(INFINITY, INFINITY, -INFINITY, -INFINITY);
   for (int i = tid; i < nt; i += nthr) {
     const float x = tgt[dim * i] - mx, y = tgt[dim * i + 1] - my;
-    mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
+    bnd.x = fminf(bnd.x, x), bnd.y = fminf(bnd.y, y), bnd.z = fmaxf(bnd.z, x), bnd.w = fmaxf(bnd.w, y);
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
-    mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
-    mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
-    mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
-  }
-  if ((tid & 31) == 0) {
-    wred[(tid >> 5) * 4 + 0] = mn_x, wred[(tid >> 5) * 4 + 1] = mn_y;
-    wred[(tid >> 5) * 4 + 2] = mxx, wred[(tid >> 5) * 4 + 3] = mxy;
-  }
-  __syncthreads();
+  bnd = block_bounds(bnd, bred);
   if (tid == 0) {
-    float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
-    for (int w = 0; w < (nthr >> 5); ++w) {
-      a = fminf(a, wred[w * 4 + 0]), bb = fminf(bb, wred[w * 4 + 1]);
-      c = fmaxf(c, wred[w * 4 + 2]), d = fmaxf(d, wred[w * 4 + 3]);
-    }
     MapGridView g;
-    grid_geometry(nt, a, bb, c, d, 0.05f, g, nt + nt / 2 > 256 ? nt + nt / 2 : 256);
+    grid_geometry(nt, bnd.x, bnd.y, bnd.z, bnd.w, 0.05f, g, nt + nt / 2 > 256 ? nt + nt / 2 : 256);
     MapGrid m;
     m.mean[0] = mx, m.mean[1] = my;
-    m.bbox[0] = a, m.bbox[1] = bb, m.bbox[2] = c, m.bbox[3] = d;
+    m.bbox[0] = bnd.x, m.bbox[1] = bnd.y, m.bbox[2] = bnd.z, m.bbox[3] = bnd.w;
     m.ox = g.ox, m.oy = g.oy, m.cell = g.cell, m.inv_cell = g.inv_cell;
     m.nx = g.nx, m.ny = g.ny, m.n = nt, m.pad = 0;
     grid[s] = m;
@@ -203,42 +187,36 @@ int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, con
   SFE_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, vals, N, 0, end_bit, st));
   size_t temp_bytes = psort_bytes > scan_bytes ? psort_bytes : scan_bytes;
   if (sort_bytes > temp_bytes) temp_bytes = sort_bytes;
-  char *base = nullptr;
-  size_t used = 0;
-  auto take = [&](size_t bytes) {
-    void *p = base ? base + used : nullptr;
-    used += (bytes + 255) & ~size_t(255);
-    return p;
-  };
+  Carver cv;
   unsigned *pk0, *pk1;
   int *pv0, *pv1, *head, *sid;
   unsigned long long *k0, *k1;
   int *v0, *v1;
   void *temp;
-  for (int pass = 0; pass < 2; ++pass) {  // pass 0 sizes the block, pass 1 carves it
-    used = 0;
-    pk0 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
-    pk1 = (unsigned *)take(sizeof(unsigned) * (size_t)P);
-    pv0 = (int *)take(sizeof(int) * (size_t)P);
-    pv1 = (int *)take(sizeof(int) * (size_t)P);
-    head = (int *)take(sizeof(int) * (size_t)P);
-    sid = (int *)take(sizeof(int) * (size_t)P);
-    w.slot = (int *)take(sizeof(int) * (size_t)P);
-    w.n_slots = (int *)take(sizeof(int));
-    w.slot_tgt = (int *)take(sizeof(int) * (size_t)slot_cap);
-    w.grid = (MapGrid *)take(sizeof(MapGrid) * (size_t)slot_cap);
-    k0 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
-    k1 = (unsigned long long *)take(sizeof(unsigned long long) * (size_t)N);
-    v0 = (int *)take(sizeof(int) * (size_t)N);
-    v1 = (int *)take(sizeof(int) * (size_t)N);
-    w.pts = (float2 *)take(sizeof(float2) * (size_t)N);
-    w.nrm = knn > 0 ? (float2 *)take(sizeof(float2) * (size_t)N) : nullptr;
-    w.cstart = (int *)take(sizeof(int) * (size_t)slot_cap * w.cell_cap);
-    temp = take(temp_bytes);
+  for (int pass = 0; pass < 2; ++pass) {
+    cv.off = 0;
+    pk0 = (unsigned *)cv.take(sizeof(unsigned) * (size_t)P);
+    pk1 = (unsigned *)cv.take(sizeof(unsigned) * (size_t)P);
+    pv0 = (int *)cv.take(sizeof(int) * (size_t)P);
+    pv1 = (int *)cv.take(sizeof(int) * (size_t)P);
+    head = (int *)cv.take(sizeof(int) * (size_t)P);
+    sid = (int *)cv.take(sizeof(int) * (size_t)P);
+    w.slot = (int *)cv.take(sizeof(int) * (size_t)P);
+    w.n_slots = (int *)cv.take(sizeof(int));
+    w.slot_tgt = (int *)cv.take(sizeof(int) * (size_t)slot_cap);
+    w.grid = (MapGrid *)cv.take(sizeof(MapGrid) * (size_t)slot_cap);
+    k0 = (unsigned long long *)cv.take(sizeof(unsigned long long) * (size_t)N);
+    k1 = (unsigned long long *)cv.take(sizeof(unsigned long long) * (size_t)N);
+    v0 = (int *)cv.take(sizeof(int) * (size_t)N);
+    v1 = (int *)cv.take(sizeof(int) * (size_t)N);
+    w.pts = (float2 *)cv.take(sizeof(float2) * (size_t)N);
+    w.nrm = knn > 0 ? (float2 *)cv.take(sizeof(float2) * (size_t)N) : nullptr;
+    w.cstart = (int *)cv.take(sizeof(int) * (size_t)slot_cap * w.cell_cap);
+    temp = cv.take(temp_bytes);
     if (pass == 0) {
-      int rc = ensure(ctx, ctx->scratch[SCR_MAP], used, st);
+      int rc = ensure(ctx, ctx->scratch[SCR_MAP], cv.off, st);
       if (rc != SFE_OK) return rc;
-      base = (char *)ctx->scratch[SCR_MAP].ptr;
+      cv.base = (char *)ctx->scratch[SCR_MAP].ptr;
     }
   }
   const int pb = (P + MAP_THREADS - 1) / MAP_THREADS;

@@ -83,4 +83,13 @@ struct MapWs {  // device pointers into scratch[SCR_MAP]
 int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, const int *tgt_id, int P, int limit,
               int slot_cap, bool center, bool seq, int knn, MapWs &w);
 
+// Measurement build (-DSFE_MAP_CLASS_ALL, tools/build_map_class_variant.sh): downsample_run, remove_outlier_run,
+// icp_run and match_run dispatch with a one-CTA limit of 0, so every non-empty cloud takes the large-cloud path and can
+// be compared with the one-CTA kernel on clouds both hold.
+#ifdef SFE_MAP_CLASS_ALL
+constexpr bool MAP_CLASS_ALL = true;
+#else
+constexpr bool MAP_CLASS_ALL = false;
+#endif
+
 }  // namespace sfe

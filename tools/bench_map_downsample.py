@@ -1,10 +1,10 @@
 """Whole-map down-sampling (pcl.downsample on SLAM.get_points-sized clouds): device time of sfe_downsample_dev on
 resident data (CUDA events), pcl.downsample end to end (copy in, kernels, copy out) and the CPU oracle on one thread,
 every result checked against the oracle; then a sweep of single clouds either side of the one-CTA limit, as shipped
-and from a build where every cloud takes the grid-wide path (tools/build_ds_variants.sh).
+and from a build where every cloud takes the grid-wide path (tools/build_map_class_variant.sh).
 Prints one JSON line.
 
-    python tools/bench_map_downsample.py [--out FILE] [--grid-lib scratch/lib_dsgrid.so]
+    python tools/bench_map_downsample.py [--out FILE] [--grid-lib scratch/lib_mapclass.so]
 """
 import argparse
 import json
@@ -53,8 +53,8 @@ def sweep(sizes):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
-    ap.add_argument("--grid-lib", default=os.path.join(REPO, "scratch", "lib_dsgrid.so"),
-                    help="library built with SFE_DS_GRID_ALL (every cloud on the grid-wide path)")
+    ap.add_argument("--grid-lib", default=os.path.join(REPO, "scratch", "lib_mapclass.so"),
+                    help="library built with SFE_MAP_CLASS_ALL (every cloud on the grid-wide path)")
     ap.add_argument("--sweep", default=None, help=argparse.SUPPRESS)  # child mode: comma-separated sizes
     args = ap.parse_args()
     import torch

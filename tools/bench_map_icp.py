@@ -6,10 +6,10 @@
   cov_ms             SLAM.compute_icp_with_cov end to end (the batch plus scikit-learn's MinCovDet), median of 10
   cpu_ms             the CPU oracle's 30 ICP runs on one thread
 every device result checked against the oracle.  Then one 16 k target that both layouts hold, through the shipped build
-(in-CTA kernel) and through scratch/lib_icpmap.so (tools/build_icp_map_variant.sh: every target in the map class): what
+(in-CTA kernel) and through scratch/lib_mapclass.so (tools/build_map_class_variant.sh: every target in the map class): what
 reading the target from a global-memory grid costs.  Prints one JSON line.
 
-    python tools/bench_map_icp.py [--out FILE] [--map-lib scratch/lib_icpmap.so]
+    python tools/bench_map_icp.py [--out FILE] [--map-lib scratch/lib_mapclass.so]
 """
 import argparse
 import json
@@ -104,7 +104,7 @@ def measure(tgt, src, guesses, cpu=True):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
-    ap.add_argument("--map-lib", default=os.path.join(REPO, "scratch", "lib_icpmap.so"))
+    ap.add_argument("--map-lib", default=os.path.join(REPO, "scratch", "lib_mapclass.so"))
     ap.add_argument("--one", type=int, default=0, help=argparse.SUPPRESS)  # child: the 16 k target only
     args = ap.parse_args()
     import torch
@@ -124,7 +124,7 @@ def main():
         env = dict(os.environ)
         if lib:
             if not os.path.exists(lib):
-                forced[tag] = "not measured: build it with tools/build_icp_map_variant.sh"
+                forced[tag] = "not measured: build it with tools/build_map_class_variant.sh"
                 continue
             env["SFE_LIB_PATH"] = lib
         out = subprocess.run([sys.executable, __file__, "--one", "16000"], env=env, capture_output=True, text=True)

@@ -2,9 +2,9 @@
 sfe_remove_outlier_dev on resident data (CUDA events), pcl.remove_outlier end to end (copy in, kernels, copy out) and
 the CPU oracle on one thread, every result checked against the oracle; then a sweep of single clouds from 4 k points to
 the one-CTA limit with both paths (the map class from a build where every cloud takes it:
-tools/build_ro_map_variant.sh).  Prints one JSON line.
+tools/build_map_class_variant.sh).  Prints one JSON line.
 
-    python tools/bench_map_outlier.py [--out FILE] [--map-lib scratch/lib_romap.so]
+    python tools/bench_map_outlier.py [--out FILE] [--map-lib scratch/lib_mapclass.so]
 """
 import argparse
 import json
@@ -67,8 +67,8 @@ def cta_limit(optin):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="also write the JSON result to this file")
-    ap.add_argument("--map-lib", default=os.path.join(REPO, "scratch", "lib_romap.so"),
-                    help="library built with SFE_RO_MAP_ALL (every cloud in the map class)")
+    ap.add_argument("--map-lib", default=os.path.join(REPO, "scratch", "lib_mapclass.so"),
+                    help="library built with SFE_MAP_CLASS_ALL (every cloud in the map class)")
     ap.add_argument("--sweep", default=None, help=argparse.SUPPRESS)  # child mode: comma-separated sizes
     args = ap.parse_args()
     import torch

@@ -1,8 +1,7 @@
 #!/bin/bash
-# experimental builds of libsonarfe with cloud.cu knobs (run after the main build):
-#   scratch/lib_dsgrid.so    every down-sampled cloud takes the grid-wide path (tools/bench_map_downsample.py compares
-#                            it with the one-CTA kernel)
+# experimental build of libsonarfe with cloud.cu knobs (run after the main build):
 #   scratch/lib_dsphases.so  per-phase cycle counts of the down-sample kernels (-DSFE_DS_PHASE_CLOCKS, tools/ds_phases.py)
+# (the build in which every cloud takes the grid-wide path: tools/build_map_class_variant.sh)
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p scratch
@@ -13,6 +12,5 @@ build() { tag=$1; shift
   nvcc $FL "$@" -c sonar_slam_b200/csrc/cloud.cu -o scratch/cloud_$tag.o
   nvcc -shared -o scratch/lib_$tag.so scratch/cloud_$tag.o $objs -gencode arch=compute_90a,code=sm_90a -lcudart
 }
-build dsgrid -DSFE_DS_GRID_ALL
 build dsphases -DSFE_DS_PHASE_CLOCKS
-ls -la scratch/lib_dsgrid.so scratch/lib_dsphases.so
+ls -la scratch/lib_dsphases.so
