@@ -474,6 +474,54 @@ SFE_API int sfe_fov_select_host(sfe_ctx *ctx, const float *pts_host, int n, cons
                                 const double *range_bound_host, const double *bearing_bound_host, int n_frames,
                                 uint8_t *sel_host);
 
+/* ------------------------------------------------------------------ resident keyframe map (row N3)
+ * SLAM.get_points (slam.py:229-292) without re-sending the map: the keyframe clouds are stored once on the device, in
+ * local coordinates, and every call assembles the requested keyframes under that call's poses and down-samples the
+ * result like bruce_slam.pcl.downsample (sfe_downsample_*), with the same results as the host lines
+ *     np.concatenate([transform_points(kf.points, pose) (, key)]) -> pcl.downsample(points (, keys), resolution)
+ * Poses are not stored: the caller computes each entry's transform on the host, as get_points does.
+ *
+ * A map belongs to the context it was created with (its stream runs every call) and is destroyed before it.  Its arena
+ * of float32 (x, y) points starts with room for `initial_points` (0: 65 536) and doubles when an append needs more,
+ * keeping the stored clouds (device-to-device copy on the context's stream).  Clouds get consecutive slot ids from 0 in
+ * append order; the map holds at most 2^31 - 2 points.
+ *
+ * Appends (slots_host int32 [n_clouds] receives the slot ids assigned; may be NULL):
+ *   _append_host  points float32 [sum counts][2] packed in cloud order, counts int32 [n_clouds] (>= 0), host memory;
+ *                 returns when the points are on the device.
+ *   _append_dev   clouds already on the device in sfe_frontend_results_dev's layout: cloud c = cloud_count_dev[c]
+ *                 points at cloud_xy_dev + 2 * c * cloud_stride (a count above cloud_stride keeps cloud_stride points,
+ *                 as the front end's window assembly does).  The counts are read back (one small copy) and returned in
+ *                 counts_host int32 [n_clouds] (may be NULL).
+ * Assemble: n_entries entries (all in HOST memory: they index the map's host-side table) of
+ *     slots_host      int32 [K]     the cloud of entry k (repeats allowed)
+ *     keys_host       float32 [K]   the key every point of entry k carries (NULL when no keys are requested)
+ *     transforms_host float32 [K][6] {r00, r01, r10, r11, tx, ty} = that entry's pose.matrix().astype(float32)
+ *                     (Keyframe.transform_points, slam_objects.py:195); points move as x' = fma(y, r01, x * r00) + tx
+ * The entries' points, moved, form one cloud in entry order (N = sum of the entries' counts, at most 2^31 - 2); it is
+ * down-sampled at `resolution` (> 0): out_pts float32 [M][2], with out_keys non-NULL out_keys float32 [M] (the key of
+ * the entry each kept point came from), n_out = M.  The outputs must hold `capacity` >= N rows (else SFE_ERR_CAPACITY).
+ * Bad slots, negative counts, totals above the limit and a non-positive resolution are rejected before any device
+ * work.  Workspace, kept with the map between calls: 12 bytes per assembled point (16 with keys; the host flavour 8 (12)
+ * more for its device-side outputs) and 36 bytes per entry (the uploaded table), plus the down-sample's own (48 bytes
+ * per point above the one-CTA limit, in the context).
+ *   _assemble_dev   outputs in device memory, asynchronous on the context's stream.
+ *   _assemble_host  outputs in host memory (only the M kept rows are copied back); returns when they are there. */
+typedef struct sfe_keyframe_map sfe_keyframe_map;
+SFE_API int sfe_keyframe_map_create(sfe_ctx *ctx, int initial_points, sfe_keyframe_map **out);
+SFE_API void sfe_keyframe_map_destroy(sfe_keyframe_map *km);
+SFE_API int sfe_keyframe_map_size(const sfe_keyframe_map *km, int *n_clouds, int64_t *n_points);
+SFE_API int sfe_keyframe_map_append_host(sfe_keyframe_map *km, const float *pts_host, const int32_t *counts_host,
+                                         int n_clouds, int32_t *slots_host);
+SFE_API int sfe_keyframe_map_append_dev(sfe_keyframe_map *km, const float *cloud_xy_dev, const int32_t *cloud_count_dev,
+                                        int cloud_stride, int n_clouds, int32_t *slots_host, int32_t *counts_host);
+SFE_API int sfe_keyframe_map_assemble_dev(sfe_keyframe_map *km, const int32_t *slots_host, const float *keys_host,
+                                          const float *transforms_host, int n_entries, float resolution, int capacity,
+                                          float *out_pts_dev, float *out_keys_dev, int32_t *n_out_dev);
+SFE_API int sfe_keyframe_map_assemble_host(sfe_keyframe_map *km, const int32_t *slots_host, const float *keys_host,
+                                           const float *transforms_host, int n_entries, float resolution, int capacity,
+                                           float *out_pts_host, float *out_keys_host, int32_t *n_out);
+
 /* ------------------------------------------------------------------ compressed pings (row N4)
  * feature_extraction.py:210-213 (compressed_images: True): cv2.cvtColor(cv2.imdecode(buf, IMREAD_COLOR), BGR2GRAY),
  * i.e. libjpeg-turbo's default decompression (JDCT_ISLOW, fancy upsampling) followed by OpenCV's fixed-point

@@ -52,6 +52,8 @@ def load():
         lib.sfe_maps_destroy.restype = None
         lib.sfe_costmap_destroy.argtypes = [c_void_p]
         lib.sfe_costmap_destroy.restype = None
+        lib.sfe_keyframe_map_destroy.argtypes = [c_void_p]
+        lib.sfe_keyframe_map_destroy.restype = None
         lib.sfe_icp_status_message.argtypes = [c_int]
         lib.sfe_icp_status_message.restype = ctypes.c_char_p
         lib.sfe_icp_params_default.argtypes = [c_void_p]
@@ -112,6 +114,14 @@ _EXTRA_SIGNATURES = {
                               c_void_p],
     "sfe_fov_select_dev": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
     "sfe_fov_select_host": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p],
+    "sfe_keyframe_map_create": [c_void_p, c_int, ctypes.POINTER(c_void_p)],
+    "sfe_keyframe_map_size": [c_void_p, ctypes.POINTER(c_int), ctypes.POINTER(ctypes.c_int64)],
+    "sfe_keyframe_map_append_host": [c_void_p, c_void_p, c_void_p, c_int, c_void_p],
+    "sfe_keyframe_map_append_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
+    "sfe_keyframe_map_assemble_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
+                                      c_void_p, c_void_p],
+    "sfe_keyframe_map_assemble_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
+                                       c_void_p, c_void_p],
     "sfe_icp_host": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p,
                      c_void_p, c_void_p],
     "sfe_icp_batch_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,

@@ -7,6 +7,8 @@ The pose-graph part of SLAM (ISAM2, PCM, keyframe logic) is out of this library'
 with the caller; `Pose2` below is a minimal stand-in for gtsam.Pose2 (x, y, theta, matrix,
 between, compose) used when gtsam is not importable.
 """
+import weakref
+
 import numpy as np
 
 from . import pcl
@@ -68,7 +70,7 @@ class SLAM(object):
         self.icp_odom_sigmas = np.array([0.1, 0.1, 0.01])
         self.icp = pcl.ICP()
         self.icp_ssm = pcl.ICP()
-        self.keyframes = []
+        self.keyframes = KeyframeList()  # a list; get_points serves it from the device-resident map
         # the two OculusProperty fields the loop-closure pre-filter reads (sonar.py:151,158)
         self.oculus = type("OculusProperty", (), {"max_range": 30.0, "horizontal_aperture": np.radians(130.0)})()
 
@@ -304,12 +306,21 @@ class SLAM(object):
 
     # ---- slam.py:229-292 for (points, pose) keyframe tuples
     def get_points(self, frames=None, ref_frame=None, return_keys=False):
-        """self.keyframes: list of objects with .points ([N,2] float32) and .pose (Pose2)."""
+        """self.keyframes: list of objects with .points ([N,2] float32) and .pose (Pose2).
+
+        With the KeyframeList SLAM() starts with, and every selected .points a float32 [N, 2] array, the clouds are
+        served from the device-resident map (KeyframeList) and only the poses travel; the results are the same.
+        Otherwise (a list or dict the caller assigned, other dtypes) the lines below run on the host."""
         if frames is None:
             frames = range(len(self.keyframes))
         ref_pose = None
         if ref_frame is not None:
             ref_pose = ref_frame if isinstance(ref_frame, Pose2) else self.keyframes[ref_frame].pose
+        if isinstance(self.keyframes, KeyframeList):
+            frames = list(frames)
+            kfs = [self.keyframes[key] for key in frames]  # IndexError here, before any device work
+            if all(_resident_cloud(kf.points) for kf in kfs):
+                return self._get_points_resident(frames, kfs, ref_pose, return_keys)
         all_points = [np.zeros((0, 3 if return_keys else 2), np.float32)]
         for key in frames:
             kf = self.keyframes[key]
@@ -322,3 +333,63 @@ class SLAM(object):
         if return_keys:
             return pcl.downsample(all_points[:, :2], all_points[:, (2,)], self.point_resolution)
         return pcl.downsample(all_points, self.point_resolution)
+
+    def _get_points_resident(self, frames, kfs, ref_pose, return_keys):
+        """get_points from the device-resident map: the transforms are the host path's float32 matrices, the keys its
+        float64 `key * np.ones` values rounded to float32 as pcl.downsample's descriptors are."""
+        if not any(len(kf.points) for kf in kfs):  # pcl.downsample hands empty input straight back
+            pts = np.zeros((0, 2), np.float32)
+            return (pts, np.zeros((0, 1), np.float32)) if return_keys else pts
+        slots = self.keyframes.slots([kf.points for kf in kfs])
+        tf = np.empty((len(kfs), 6), np.float32)
+        for k, kf in enumerate(kfs):
+            T = (ref_pose.between(kf.pose) if ref_pose is not None else kf.pose).matrix().astype(np.float32)
+            tf[k] = T[0, 0], T[0, 1], T[1, 0], T[1, 1], T[0, 2], T[1, 2]
+        keys = np.asarray(frames, np.float64).astype(np.float32) if return_keys else None
+        out = self.keyframes.map.assemble(slots, keys, tf, self.point_resolution, return_keys)
+        if return_keys:
+            return out[0], out[1].reshape(-1, 1)
+        return out
+
+
+def _resident_cloud(points):
+    return isinstance(points, np.ndarray) and points.dtype == np.float32 and points.ndim == 2 and points.shape[1] == 2
+
+
+class KeyframeList(list):
+    """The list SLAM() keeps its keyframes in: a plain list whose keyframes' clouds are mirrored in a device-resident
+    KeyframeMap (sonar_slam_b200/keyframe_map.py), created on first use on the thread's default context.
+
+    The mirror is lazy: get_points uploads, in one append per call, every selected keyframe whose `.points` array has
+    not been uploaded yet, and records which array object each slot came from.  A keyframe whose `.points` is replaced
+    by another array gets a new slot.  An array edited in place after its upload is NOT detected (the reference never
+    edits a keyframe's cloud; assign a new array instead)."""
+
+    def __init__(self, *args):
+        super().__init__(*args)
+        self.map = None
+        self._uploaded = {}  # id(points) -> (weak reference to the array, slot)
+
+    def slots(self, clouds):
+        """Slot of every array in `clouds`, appending those not stored yet (each array once)."""
+        from .. import keyframe_map
+        if self.map is None:
+            self.map = keyframe_map.KeyframeMap(_lib.default_context())
+        slots = np.empty(len(clouds), np.int32)
+        new, where = [], {}
+        for i, p in enumerate(clouds):
+            e = self._uploaded.get(id(p))
+            if e is not None and e[0]() is p:
+                slots[i] = e[1]
+                continue
+            j = where.setdefault(id(p), len(new))
+            if j == len(new):
+                new.append(p)
+            slots[i] = -1 - j
+        if new:
+            got = self.map.append(new)
+            for p, s in zip(new, got):
+                self._uploaded[id(p)] = (weakref.ref(p), int(s))
+            pending = slots < 0
+            slots[pending] = got[-1 - slots[pending]]
+        return slots
