@@ -12,6 +12,7 @@ float32; results are fresh float32 arrays.  Not provided: density_filter (dead c
 reference: its only call site is commented out, feature_extraction.py:246) and
 ICP.getCovariance (never called from Python) -- both raise NotImplementedError.
 """
+import math
 import os
 
 import numpy as np
@@ -158,6 +159,11 @@ def parse_icp_yaml(text):
             prm.smooth_length = int(p.get("smoothLength", 3))
         else:
             raise NotImplementedError(f"ICP yaml: transformation checker {name} ({_SUPPORTED})")
+    for f in ("matcher_max_dist", "outlier_max_dist", "trim_ratio", "min_diff_rot", "min_diff_trans"):
+        if math.isnan(getattr(prm, f)):
+            raise ValueError(f"ICP yaml: {f} is NaN")
+    if prm.trim_ratio > 1.0:  # the quantile element floor(n * ratio) would lie past the sorted distances
+        raise ValueError(f"ICP yaml: TrimmedDistOutlierFilter ratio {prm.trim_ratio} is above 1")
     return prm
 
 

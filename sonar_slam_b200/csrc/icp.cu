@@ -21,6 +21,7 @@
 #include <type_traits>
 
 #include <climits>
+#include <cmath>
 
 #include <cub/cub.cuh>
 
@@ -672,6 +673,11 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
               "icp: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", prm->normals_knn, GRID_KNN_MAX);
   SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
               ICP_HIST - 1);
+  SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
+                  !std::isnan(prm->trim_ratio) && !std::isnan(prm->min_diff_rot) && !std::isnan(prm->min_diff_trans),
+              "icp: a NaN parameter (maxDist, ratio or minDiff*) is not supported");
+  // (the quantile element floor(n * ratio) lies past the sorted distances for a ratio above 1)
+  SFE_REQUIRE(prm->trim_ratio <= 1.0f, "icp: TrimmedDistOutlierFilter ratio %g is above 1", (double)prm->trim_ratio);
   IcpBatch b{};
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;

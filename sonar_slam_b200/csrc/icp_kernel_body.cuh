@@ -418,8 +418,12 @@
         int verdict = -1;  // 1 finite, 0 not, -1 unknown
         if (sh.cnx > 0) {
           const float C = g.cell * (float)ICP_COARSE, rad = prm.matcher_max_dist;
-          const int xa = max(0, (int)floorf((q.x - rad - g.ox) / C) - 1), xb = min(sh.cnx - 1, (int)floorf((q.x + rad - g.ox) / C) + 1);
-          const int ya = max(0, (int)floorf((q.y - rad - g.oy) / C) - 1), yb = min(sh.cny - 1, (int)floorf((q.y + rad - g.oy) / C) + 1);
+          // the window is clamped to [0, n] / [-1, n - 1] in float before the int conversion: a maxDist of inf or
+          // 1e9 m would otherwise saturate and overflow it into an empty window ("nothing within maxDist")
+          auto lo = [&](float v, int n) { return (int)fminf(fmaxf(floorf(v / C) - 1.f, 0.f), (float)n); };
+          auto hi = [&](float v, int n) { return (int)fminf(fmaxf(floorf(v / C) + 1.f, -1.f), (float)(n - 1)); };
+          const int xa = lo(q.x - rad - g.ox, sh.cnx), xb = hi(q.x + rad - g.ox, sh.cnx);
+          const int ya = lo(q.y - rad - g.oy, sh.cny), yb = hi(q.y + rad - g.oy, sh.cny);
           if (xa > xb || ya > yb) {
             verdict = 0;
           } else if ((xb - xa + 1) * (yb - ya + 1) <= 256) {
@@ -459,7 +463,9 @@
         }
         qstate[i] |= 4 | (verdict ? 2 : 0) | (verdict ? 0 : 1);  // "nothing within maxDist" is a settled answer
         n_fin += verdict;
-        dist[i] = verdict ? max_d2 : INFINITY;  // upper bound of a finite point without candidate
+        // upper bound of a finite point without candidate; kept finite (maxDist = inf) so that pass C's selection
+        // counts it among the total_fin finite entries
+        dist[i] = verdict ? fminf(max_d2, ICP_PRUNED) : INFINITY;
       }
       if (total_fin < 0) total_fin = block_total(n_fin, &sh.tot[0][0], tot_phase);  // (its barrier also publishes dist[] / qstate[])
       // pass C: settle what still matters
