@@ -265,6 +265,14 @@ SFE_API int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *sr
                         const float *tgt_pts_dev, const int32_t *tgt_off_dev, const int32_t *src_id_dev,
                         const int32_t *tgt_id_dev, int n_problems, int ns_max, int nt_max, const float *guess_dev,
                         float *T_dev, int32_t *iters_dev, int32_t *inliers_dev, int32_t *status_dev);
+/* sfe_icp_dev (problem p: clouds p / p) through the batched front end's size classes: each class its own launch,
+ * problems largest first; same results.  class_dev (device [2 * n_problems] or NULL): class_dev[p] = the class that
+ * solved problem p (the front end's classes in order, the capacity launch last), class_dev[n_problems + p] = its place in that
+ * class's work list. */
+SFE_API int sfe_frontend_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev,
+                                 const int32_t *src_off_dev, const float *tgt_pts_dev, const int32_t *tgt_off_dev,
+                                 int n_problems, int ns_max, int nt_max, const float *guess_dev, float *T_dev,
+                                 int32_t *iters_dev, int32_t *inliers_dev, int32_t *status_dev, int32_t *class_dev);
 /* One source / target pair from host memory, n_guesses initial guesses (1 = ICP.compute; >1 = the
  * loop of SLAM.compute_icp_with_cov, slam.py:346-358, run as one batch). */
 SFE_API int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host,

@@ -102,6 +102,8 @@ _EXTRA_SIGNATURES = {
     "sfe_match_host": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p],
     "sfe_icp_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                     c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_frontend_icp_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_copy_to_host": [c_void_p, c_void_p, c_void_p, ctypes.c_uint64],
     "sfe_frontend_create": [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(c_void_p)],
     "sfe_frontend_set_timing": [c_void_p, c_int],

@@ -416,7 +416,7 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
   SFE_CUDA(cudaSetDevice(ctx->device));
   return icp_run(ctx, ctx->stream, prm,
                  {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
-                  tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, 0, 0);
+                  tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, nullptr, 0);
 }
 
 int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host, int nt,
@@ -490,7 +490,7 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
     IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
                    d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
     pb.n_tgt_clouds = n_tgt_clouds;
-    int rc = icp_run(ctx, ctx->stream, prm, pb, 0, 0);
+    int rc = icp_run(ctx, ctx->stream, prm, pb, nullptr, 0);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));

@@ -72,6 +72,8 @@ struct IcpBatch {
   int small_mult;     // problems with ns <= small_mult * blockDim.x (and nt <= 4096) take the one-pass exact path
   int slot_by_smid;   // workspace slot = %smid (one CTA per SM, one CTA per problem) instead of blockIdx.x
   int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
+  const int *list;    // icp_run's classes: this launch's problems, largest first (icp_classify_kernel), or null: 0 .. P-1
+  const int *list_n;  // ... and their number
 };
 
 // The map class (icp_map_kernel): problem p reads its target from the grid in slot map_slot[p] (map_build)
@@ -118,6 +120,12 @@ static int icp_phase_per_sm[3];  // CTAs per SM of the last 128 / 256 / 512-thre
 #define ICP_PH_MARK(k) ((void)0)
 #define ICP_PH_FLUSH() ((void)0)
 #endif
+
+// Problem of work item k: entry k of the launch's class list (P past its end), or k itself without a list
+__device__ __forceinline__ int icp_work_item(const IcpBatch &b, int k) {
+  if (!b.list) return k;
+  return k < *b.list_n ? b.list[k] : b.P;
+}
 
 constexpr int ICP_SM_SLOTS = 256;  // >= %nsmid on every sm_90 part
 __device__ __forceinline__ unsigned icp_smid() {
@@ -525,8 +533,11 @@ static size_t match_cta_smem(int nt_max) {
 static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 1536 ? 256 : ICP_THREADS); }
 
 // icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget).
-// 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers.
-static const void *icp_kernel_for(int threads, size_t smem, bool plane) {
+// 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers.  dense (icp_run's classes):
+// 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get them (IcpClass::dense).
+static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense = false) {
+  if (threads == 128 && dense)
+    return plane ? (const void *)icp_kernel<128, 8, true> : (const void *)icp_kernel<128, 8, false>;
   if (threads == 128) return plane ? (const void *)icp_kernel<128, 7, true> : (const void *)icp_kernel<128, 7, false>;
   if (threads == 256) return plane ? (const void *)icp_kernel<256, 4, true> : (const void *)icp_kernel<256, 4, false>;
   if (smem <= 110 * 1024) return plane ? (const void *)icp_kernel<512, 2, true> : (const void *)icp_kernel<512, 2, false>;
@@ -535,8 +546,8 @@ static const void *icp_kernel_for(int threads, size_t smem, bool plane) {
 
 // Shared memory icp_kernel's layouts may take next to sources of ns_max points: the budget of the instantiation that
 // runs the largest of them.
-static int icp_cta_budget(const sfe_ctx *ctx, int ns_max, bool plane, size_t *budget) {
-  return cta_smem_budget(ctx, icp_kernel_for(icp_threads(ns_max), ctx->max_smem_optin, plane), budget);
+static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, size_t *budget, bool dense = false) {
+  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense), budget);
 }
 
 static void icp_tuning(IcpBatch &b) {
@@ -555,8 +566,17 @@ static void icp_tuning(IcpBatch &b) {
   b.margin_mult = mm;
 }
 
-// One launch over the batch, laid out for problems of up to ns_max x nt_max points; b.class_mode is its size class.
-static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max) {
+// One launch of icp_kernel over the batch, laid out for problems of up to ns_max x nt_max points in `threads`-thread
+// CTAs: sized by icp_plan, its workspace (orig_ws, nrm_ws) placed and the kernel enqueued by icp_enqueue.
+struct IcpLaunch {
+  IcpBatch b;
+  const void *fn;
+  int threads, grid;
+  size_t smem, orig_bytes, ws_bytes;
+};
+
+static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max, int threads,
+                    IcpLaunch &L, bool dense = false) {
   b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
   b.use_order = b.ns_max > 1024;
   b.cell_scale = 1.0f;
@@ -564,7 +584,7 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
   icp_tuning(b);
   const bool plane = prm->minimizer == 1;
   size_t budget;
-  int rc = icp_cta_budget(ctx, b.ns_max, plane, &budget);
+  int rc = icp_cta_budget(ctx, threads, plane, &budget, dense);
   if (rc != SFE_OK) return rc;
   const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, budget, &b.max_cells);
   if (smem > budget) {
@@ -572,8 +592,7 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
               budget);
     return SFE_ERR_UNSUPPORTED;
   }
-  const int threads = icp_threads(b.ns_max);
-  const void *fn = icp_kernel_for(threads, smem, plane);
+  const void *fn = icp_kernel_for(threads, smem, plane, dense);
   int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
   if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
 #ifdef SFE_ICP_PHASE_CLOCKS
@@ -583,19 +602,137 @@ static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, 
   if (grid > b.P) grid = b.P;
   int slots = grid;
   if (per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
-  const size_t orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
-  const size_t nrm_bytes = plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0;
-  rc = ensure(ctx, ctx->scratch[SCR_ICP], orig_bytes + nrm_bytes, st);
-  if (rc != SFE_OK) return rc;
-  b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
-  b.nrm_ws = plane ? (float2 *)((char *)ctx->scratch[SCR_ICP].ptr + orig_bytes) : nullptr;
-  if (!b.slot_by_smid && grid < b.P) {  // persistent CTAs
-    b.next = ctx->work + WORK_ICP;
-    SFE_CUDA(cudaMemsetAsync(b.next, 0, sizeof(int), st));
-  }
+  L.orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
+  L.ws_bytes = L.orig_bytes + (plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0);
+  L.b = b, L.fn = fn, L.threads = threads, L.grid = grid, L.smem = smem;
+  return SFE_OK;
+}
+
+// ws: L.ws_bytes of device memory; next: the launch's work counter, zero when the kernel starts
+static int icp_enqueue(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L, char *ws, int *next) {
+  IcpBatch &b = L.b;
+  b.orig_ws = (uint16_t *)ws;
+  b.nrm_ws = b.prm.minimizer == 1 ? (float2 *)(ws + L.orig_bytes) : nullptr;
+  if (!b.slot_by_smid && (L.grid < b.P || b.list)) b.next = next;  // persistent CTAs; a list is always walked so
   void *args[] = {(void *)&b};
-  SFE_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(threads), args, smem, st));
+  SFE_CUDA(cudaLaunchKernel(L.fn, dim3(L.grid), dim3(L.threads), args, L.smem, st));
   ctx->launches++;
+  return SFE_OK;
+}
+
+// One launch over the batch in icp_threads' CTAs; b.class_mode is its size class.
+static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max) {
+  IcpLaunch L;
+  int rc = icp_plan(ctx, prm, b, ns_max, nt_max, icp_threads(ns_max > 0 ? ns_max : 1), L);
+  if (rc != SFE_OK) return rc;
+  rc = ensure(ctx, ctx->scratch[SCR_ICP], L.ws_bytes, st);
+  if (rc != SFE_OK) return rc;
+  if (!L.b.slot_by_smid && L.grid < L.b.P) SFE_CUDA(cudaMemsetAsync(ctx->work + WORK_ICP, 0, sizeof(int), st));
+  return icp_enqueue(ctx, st, L, (char *)ctx->scratch[SCR_ICP].ptr, ctx->work + WORK_ICP);
+}
+
+// Work lists of icp_run's classes.  Problem p goes to the first class c whose bounds it fits (the last class takes
+// every other problem); lists[c][0 .. n[c]) holds class c's problems by decreasing cost -- source size in steps of
+// ICP_COST_STEP points, ties in index order -- so that a launch ends on its shortest problems.  One CTA: warp w counts,
+// then places, a contiguous segment of the problem indices; segments are laid out in warp order inside every (class,
+// size step) run.  Also zeroes the classes' work counters next[c].
+constexpr int ICP_COST_STEP = 32, ICP_COST_STEPS = 32;  // (sources of 992 points and more share the last step)
+struct IcpClassBounds {
+  int n, ns[ICP_MAX_CLASSES + 1], nt[ICP_MAX_CLASSES + 1];
+};
+
+__global__ void __launch_bounds__(1024) icp_classify_kernel(const IcpBatch b, const IcpClassBounds cb, int *lists,
+                                                            int *n, int *next) {
+  constexpr int KEYS = (ICP_MAX_CLASSES + 1) * ICP_COST_STEPS;
+  __shared__ int cnt[32][KEYS];  // per warp: its problems per (class, cost step), then where the next one goes
+  __shared__ int run_len[KEYS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, P = b.P;
+  const int seg = (P + 31) / 32, lo = min(warp * seg, P), hi = min(lo + seg, P);
+  auto key_of = [&](int p) {
+    const int si = b.src_id ? b.src_id[p] : p, ti = b.tgt_id ? b.tgt_id[p] : p;
+    const int ns = b.src_cnt ? b.src_cnt[si] : b.src_off[si + 1] - b.src_off[si];
+    const int nt = b.tgt_cnt ? b.tgt_cnt[ti] : b.tgt_off[ti + 1] - b.tgt_off[ti];
+    int c = 0;
+    while (c + 1 < cb.n && (ns > cb.ns[c] || nt > cb.nt[c])) ++c;
+    return c * ICP_COST_STEPS + (ICP_COST_STEPS - 1 - min(max(ns, 0) / ICP_COST_STEP, ICP_COST_STEPS - 1));
+  };
+  for (int k = lane; k < KEYS; k += 32) cnt[warp][k] = 0;
+  __syncwarp();
+  for (int p = lo + lane; p < hi; p += 32) atomicAdd(&cnt[warp][key_of(p)], 1);
+  __syncthreads();
+  const int key = threadIdx.x;
+  if (key < KEYS) {
+    int s = 0;
+    for (int w = 0; w < 32; ++w) s += cnt[w][key];
+    run_len[key] = s;
+  }
+  __syncthreads();
+  if (key < KEYS) {  // exclusive scan in (cost step, warp) order within the key's class
+    const int c = key / ICP_COST_STEPS;
+    int at = 0;
+    for (int k = c * ICP_COST_STEPS; k < key; ++k) at += run_len[k];
+    if (key % ICP_COST_STEPS == ICP_COST_STEPS - 1) n[c] = at + run_len[key], next[c] = 0;
+    for (int w = 0; w < 32; ++w) {
+      const int v = cnt[w][key];
+      cnt[w][key] = at, at += v;
+    }
+  }
+  __syncthreads();
+  for (int base = lo; base < hi; base += 32) {  // in index order: lanes with the same key take consecutive places
+    const int p = base + lane;
+    const int k = p < hi ? key_of(p) : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, k);
+    if (k >= 0) lists[(size_t)(k / ICP_COST_STEPS) * P + cnt[warp][k] + __popc(peers & ((1u << lane) - 1u))] = p;
+    __syncwarp();
+    if (k >= 0 && lane == __ffs(peers) - 1) cnt[warp][k] += __popc(peers);
+    __syncwarp();
+  }
+}
+
+// class_of[p] = the class whose list holds p, class_of[P + p] = its place there (icp_run's class_of)
+__global__ void icp_class_of_kernel(const int *lists, const int *n, int n_classes, int P, int *class_of) {
+  for (int c = 0; c < n_classes; ++c)
+    for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n[c]; k += gridDim.x * blockDim.x) {
+      const int p = lists[(size_t)c * P + k];
+      class_of[p] = c, class_of[P + p] = k;
+    }
+}
+
+// icp_run's class path: the classify kernel, then one launch per class, the widest first
+static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpBatch &b,
+                           const IcpClass *classes, int n_classes, int ns_max, int nt_max, int *class_of) {
+  IcpLaunch L[ICP_MAX_CLASSES + 1];
+  IcpClassBounds cb{};
+  cb.n = n_classes + 1;
+  size_t ws_bytes = 0;
+  for (int c = 0; c < cb.n; ++c) {
+    const bool cap = c == n_classes;
+    cb.ns[c] = cap ? ns_max : std::min(classes[c].ns, ns_max);
+    cb.nt[c] = cap ? nt_max : std::min(classes[c].nt, nt_max);
+    const int threads = icp_threads(cb.ns[c] > 0 ? cb.ns[c] : 1);
+    int rc = icp_plan(ctx, prm, b, cb.ns[c], cb.nt[c], threads, L[c], !cap && classes[c].dense && threads == 128);
+    if (rc != SFE_OK) return rc;
+    ws_bytes = std::max(ws_bytes, L[c].ws_bytes);  // (the launches run one after the other)
+  }
+  // SCR_ICP: [work counters n, next][lists [class][P]][the launches' workspace]
+  const size_t head = 256, list_bytes = ((size_t)cb.n * b.P * sizeof(int) + 255) & ~size_t(255);
+  int rc = ensure(ctx, ctx->scratch[SCR_ICP], head + list_bytes + ws_bytes, st);
+  if (rc != SFE_OK) return rc;
+  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
+  int *n = (int *)base, *next = n + ICP_MAX_CLASSES + 1, *lists = (int *)(base + head);
+  icp_classify_kernel<<<1, 1024, 0, st>>>(b, cb, lists, n, next);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  for (int c = cb.n - 1; c >= 0; --c) {
+    L[c].b.list = lists + (size_t)c * b.P, L[c].b.list_n = n + c;
+    rc = icp_enqueue(ctx, st, L[c], base + head + list_bytes, next + c);
+    if (rc != SFE_OK) return rc;
+  }
+  if (class_of) {
+    icp_class_of_kernel<<<ctx->sm_count, 256, 0, st>>>(lists, n, cb.n, b.P, class_of);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
   return SFE_OK;
 }
 
@@ -649,14 +786,13 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
 
 }  // namespace sfe
 
-// Size classes (IcpBatch::class_mode): a small class (both sizes positive, clamped to the capacities src.n_max x
-// tgt.n_max) that is smaller on either axis gets a first launch laid out for it, whose smaller shared-memory footprint
-// fits more CTAs per SM; a second launch, laid out for the capacities, takes the problems that did not fit.
-// Otherwise one launch takes every problem and reports oversize ones itself (SFE_ICP_TOO_LARGE) -- unless the
-// largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit and the map
-// class (map grids in global memory, icp_map_kernel) takes the rest.
-int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
-                 int small_nt) {
+// Size classes: every listed class gets a launch laid out for it, whose smaller shared-memory footprint fits more
+// CTAs per SM, and a last launch, laid out for the capacities src.n_max x tgt.n_max, takes the problems that fit none
+// (and reports oversize ones, SFE_ICP_TOO_LARGE).  Without classes one launch takes every problem (IcpBatch::class_mode
+// 0) -- unless the largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit
+// (class_mode 1) and the map class (map grids in global memory, icp_map_kernel) takes the rest.
+int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
+                 const IcpClass *class_list, int n_classes, int *class_of) {
   const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
   SFE_REQUIRE(ctx && prm, "icp: null context or parameters");
   SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp: negative sizes");
@@ -664,7 +800,12 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
                   pb.status,
               "icp: null pointer");
-  const bool classes = small_ns > 0 && small_nt > 0;
+  SFE_REQUIRE(n_classes >= 0 && n_classes <= ICP_MAX_CLASSES && (n_classes == 0 || class_list),
+              "icp: %d size classes (at most %d)", n_classes, ICP_MAX_CLASSES);
+  for (int c = 0; c < n_classes; ++c)
+    SFE_REQUIRE(class_list[c].ns > 0 && class_list[c].nt > 0, "icp: size class %d of %d x %d points", c,
+                class_list[c].ns, class_list[c].nt);
+  const bool classes = n_classes > 0;
   SFE_REQUIRE(ns_max <= 65535 && (nt_max <= 65535 || !classes),
               "icp: clouds of more than 65535 points are not supported (got %d, %d)", ns_max, nt_max);
   SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
@@ -690,7 +831,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     const int ns = ns_max > 0 ? ns_max : 1;
     const bool plane = prm->minimizer == 1;
     size_t budget;
-    int rc = icp_cta_budget(ctx, ns, plane, &budget);
+    int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget);
     if (rc != SFE_OK) return rc;
     int mc;
     const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
@@ -705,13 +846,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
     return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap);
   }
-  const int ns_small = std::min(small_ns, ns_max), nt_small = std::min(small_nt, nt_max);
-  if (ns_small == ns_max && nt_small == nt_max) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
-  b.class_mode = 1;
-  int rc = icp_launch(ctx, st, prm, b, ns_small, nt_small);
-  if (rc != SFE_OK) return rc;
-  b.class_mode = 2, b.class_ns = ns_small, b.class_nt = nt_small;
-  return icp_launch(ctx, st, prm, b, ns_max, nt_max);
+  return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
 }
 
 // References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in

@@ -4,6 +4,9 @@
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
   //         [prev Pos ns_max][qstate u8 ns_max][slack f32 ns_max][order u16 ns_max]   (MAP: no sorted, no cells)
+  // CTA sizes: the reference mean takes warps 0 and 1 (one per coordinate); the per-warp partials (wred, tot, red) and
+  // block_total's final read (one lane per warp) hold at most 16 warps; the rest of the body loops over blockDim.x.
+  static_assert(THREADS % 32 == 0 && THREADS >= 64 && THREADS <= 512, "icp_kernel: 2 to 16 warps per CTA");
   using Pos = std::conditional_t<MAP, int, uint16_t>;  // a target point's sorted position
   constexpr int NONE = MAP ? -1 : 0xffff;               // "no match"
   IcpShared &sh = *reinterpret_cast<IcpShared *>(smem_raw);
@@ -64,8 +67,9 @@
   // Persistent CTAs take problems from a work counter: problems differ in length (cloud sizes, early exits), and with
   // a static share the batch ends when the CTAs that drew the most work finish.  Problem p's results do not depend
   // on the CTA that solves it.  The index is broadcast through sh.status, which thread 0 rewrites only after the
-  // next problem's first barrier.
-  for (int p = blockIdx.x; p < b.P; p = b.next ? next_work_item(b.next, &sh.status) : p + (int)gridDim.x) {
+  // next problem's first barrier.  With a class list (always from a counter) the work items are that list's entries.
+  for (int p = icp_work_item(b, blockIdx.x); p < b.P;
+       p = b.next ? icp_work_item(b, next_work_item(b.next, &sh.status)) : p + (int)gridDim.x) {
     const int si = b.src_id ? b.src_id[p] : p, ti = b.tgt_id ? b.tgt_id[p] : p;
     const float *src = b.src_pts + 2 * (size_t)b.src_off[si];
     const int ns = b.src_cnt ? b.src_cnt[si] : b.src_off[si + 1] - b.src_off[si];

@@ -26,12 +26,17 @@ namespace sfe {
 // (the ICP target) mean 406, max 779.  The class takes every frame of that bag: a second launch that holds only a
 // few frames costs a full problem latency at its tail.  The source cap has no margin over the bag's largest source
 // (639): above 5 points per thread (640 for 128 threads, icp.cu: small_mult) a problem leaves the one-pass path, so a
-// larger cap would only admit problems that take the slower pruned path.  At 640 / 896 points a 128-thread CTA needs 29 KB of shared
-// memory and the 128-thread instantiation is held to 72 registers, so an H100 SM holds 7 problems (6 at the former
-// 640 / 1536 class with 80 registers).
-constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 896;
+// larger cap would only admit problems that take the slower pruned path.  The target cap keeps 3 % over the bag's
+// largest target (779): at 640 / 800 points a 128-thread CTA needs 27.4 KB of shared memory, which with the 1 KB the
+// driver reserves per CTA lets an H100 SM (228 KB) hold 8 of them (810 is the largest target that does), and the
+// class runs icp_kernel's 64-register instantiation (IcpClass::dense), so 8 problems are in flight per SM (7 at the
+// former 640 / 896 class with 72 registers; DESIGN.md section 4).
+constexpr int FE_ICP_SMALL_SRC = 640, FE_ICP_SMALL_TGT = 800;
 // (the class is sized for 128-thread CTAs, which icp_run's CTA-size rule gives sources of up to 640 points)
 static_assert(FE_ICP_SMALL_SRC <= 640, "the small ICP class must stay within icp_run's 128-thread CTAs");
+// icp_run's class list (a problem takes the first class it fits; the capacity class takes the rest)
+static const IcpClass FE_ICP_CLASSES[] = {{FE_ICP_SMALL_SRC, FE_ICP_SMALL_TGT, true}};
+constexpr int FE_ICP_N_CLASSES = sizeof(FE_ICP_CLASSES) / sizeof(FE_ICP_CLASSES[0]);
 // Size classes of the cloud filters (cloud.cu: two launches by cloud size).  Config-4 replay: 3-5 k raw Cartesian
 // points per frame, ~580 after the voxel filter, ~400 after the outlier filter, window submaps <= 1.8 k raw points.
 // The outlier filter and the submap down-sampling gain from a small-cloud class (chosen on the replay; not
@@ -563,7 +568,7 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   pb.raw_cnt = fe->cnt_a + f0, pb.raw_cap = cap;  // the source's Cartesian points before the filters
   pb.guess = fe->guess + 9 * (size_t)f0, pb.T_out = fe->T + 9 * (size_t)f0;
   pb.iters = fe->iters + f0, pb.inliers = fe->inliers + f0, pb.status = fe->status + f0;
-  const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_SMALL_SRC, FE_ICP_SMALL_TGT);
+  const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES);
   fe->timer.toc(st);
   return rc;
 }
@@ -887,6 +892,17 @@ static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t
 }
 
 extern "C" {
+
+int sfe_frontend_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev, const int32_t *src_off_dev,
+                         const float *tgt_pts_dev, const int32_t *tgt_off_dev, int n_problems, int ns_max, int nt_max,
+                         const float *guess_dev, float *T_dev, int32_t *iters_dev, int32_t *inliers_dev,
+                         int32_t *status_dev, int32_t *class_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_frontend_icp_dev: null context");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  IcpProblems pb{{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, nullptr,
+                 nullptr, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev};
+  return icp_run(ctx, ctx->stream, prm, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, class_dev);
+}
 
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {
   return fe_run_dev(fe, frames_dev, nullptr, poses_host, n_frames, "sfe_frontend_run_dev");

@@ -47,10 +47,22 @@ int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_
 // the map class above it)
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
                        int min_points, float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split);
-// problems that fit a small size class (small_ns, small_nt) get a launch of their own (icp.cu); (0, 0): one launch,
-// or, when the largest target does not fit one CTA, one for the targets that do and the map class for the rest
-int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, int small_ns,
-            int small_nt);
+// One size class of icp_run: problems whose source has at most ns and whose target at most nt points, solved in a
+// launch laid out for that size.  dense: 128-thread CTAs take icp_kernel's 64-register instantiation, for layouts that
+// fit 8 CTAs per SM (more problems in flight; the one-pass iteration is latency-bound).
+struct IcpClass {
+  int ns, nt;
+  bool dense;
+};
+constexpr int ICP_MAX_CLASSES = 3;  // classes an icp_run call may list (the capacity class comes on top)
+// n_classes > 0: every problem goes to the first listed class it fits, the others to a capacity class laid out for
+// src.n_max x tgt.n_max; one launch per class, the widest first, each taking its problems largest first from a list
+// built on the device (icp.cu).  n_classes 0: one launch, or, when the largest target does not fit one CTA, one for
+// the targets that do and the map class for the rest.  class_of (device [P], may be null; classes only): receives
+// every problem's class (0 .. n_classes, the capacity class last) and, in class_of[P + p], its place in that class's
+// list.
+int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, const IcpClass *classes,
+            int n_classes, int *class_of = nullptr);
 // nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
