@@ -194,7 +194,7 @@ SFE_API int sfe_remove_outlier_host(sfe_ctx *ctx, const float *pts_host, int n, 
  * for every query point the index of the nearest reference point and the SQUARED float32 distance;
  * no reference point within max_dist -> id -1, dist +inf; ties -> lowest reference index.
  * Batched over n_pairs (ref cloud p, query cloud p), both packed [total][2] with CSR offsets;
- * ids / dists are indexed like the query points.  Only knn = 1 (what the reference uses).
+ * ids / dists are indexed like the query points.
  * References of any size: those that fit one CTA's shared memory (24 k points on an H100) run one CTA per pair; larger
  * ones (whole maps) are sorted once into a grid in global memory and searched by the whole device, with the same
  * results.  Their workspace holds 40 bytes for each of n_pairs * n_ref_max slot points (at most 2^31 - 1), 6 bytes
@@ -204,6 +204,20 @@ SFE_API int sfe_match_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t 
                           float *dists_dev);
 SFE_API int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in,
                            float max_dist, int32_t *ids_host, float *dists_host);
+/* k nearest neighbours, knn = 1 .. 16 (libnabo's exact k-NN search with a radius, as KDTreeMatcher runs it): for every
+ * query point the knn reference points nearest to it among those with squared float32 distance <= max_dist^2 (the
+ * radius test and distance expression above), in ascending squared distance, ties -> lower reference index.  Row j
+ * of ids / dists holds every query's j-th neighbour: ids / dists are [knn][total query points] (for one pair the
+ * binding's [knn, N]); slots with no neighbour left hold id -1, dist +inf.  Row 0 is sfe_match_*'s result, and rows
+ * 0 .. k-1 do not depend on knn >= k.  knn = 1 runs sfe_match_*'s kernels; knn outside 1 .. 16 is SFE_ERR_ARG.
+ * References that fit one CTA's shared memory next to the 6 * 512 * knn bytes of the per-thread lists run one CTA per
+ * pair (24.1 k points at knn 2 down to 18.7 k at knn 16 on an H100); larger ones go to the map grids, whose workspace is
+ * sfe_match_dev's. */
+SFE_API int sfe_match_knn_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev,
+                              const float *in_pts_dev, const int32_t *in_off_dev, int n_pairs, int n_ref_max, int knn,
+                              float max_dist, int32_t *ids_dev, float *dists_dev);
+SFE_API int sfe_match_knn_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int knn,
+                               float max_dist, int32_t *ids_host, float *dists_host);
 
 /* ------------------------------------------------------------------ ICP scan matcher
  * bruce_slam.pcl.ICP (pcl.cpp:185-213): libpointmatcher PointMatcher<float>::ICP configured by

@@ -5,6 +5,7 @@ bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libson
     downsample(points[N,2], resolution)                         -> float32[M,2]        (pcl.cpp:128)
     downsample(points[N,2], desc[N,d], resolution)              -> (points, desc)      (pcl.cpp:143)
     match(ref[N_t,2], in[N_s,2], knn, max_dist)                 -> (int32[knn,N_s], float32[knn,N_s])  (:161)
+    match_knn(ref[N_t,2], in[N_s,2], knn, max_dist)             -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
@@ -90,6 +91,30 @@ def match(mat_ref, mat_in, knn, max_dist):
         ctx = _lib.default_context()
         _lib.check(ctx.lib.sfe_match_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts),
                                           float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match")
+    return ids, dists
+
+
+KNN_MAX = 16  # the largest knn match_knn serves (GRID_KNN_MAX, csrc/grid.cuh)
+
+
+def match_knn(mat_ref, mat_in, knn, max_dist):
+    """libnabo KD-tree match for any knn up to 16 (what pcl.cpp:161-174 computes for knn > 1): for every query point
+    its knn nearest reference points within max_dist, nearest first (ties: lower reference index), as (ids [knn,N]
+    int32, squared dists [knn,N] float32); slots with no neighbour left hold -1 / +inf.  Row 0 is match(..., 1, ...)'s
+    result.  References of any size (whole maps run as a grid in global memory, with the same results)."""
+    knn = int(knn)
+    if knn < 1:
+        raise ValueError(f"pcl.match_knn: knn must be at least 1 (got {knn})")
+    if knn > KNN_MAX:
+        raise NotImplementedError(f"pcl.match_knn: knn {knn} is not supported (at most {KNN_MAX})")
+    ref = _points(mat_ref, "ref", cols=(2,))
+    pts = _points(mat_in, "in", cols=(2,))
+    ids = np.empty((knn, len(pts)), np.int32)
+    dists = np.empty((knn, len(pts)), np.float32)
+    if len(pts):
+        ctx = _lib.default_context()
+        _lib.check(ctx.lib.sfe_match_knn_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts), knn,
+                                              float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match_knn")
     return ids, dists
 
 

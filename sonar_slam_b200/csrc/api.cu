@@ -8,6 +8,7 @@
 #include <mutex>
 #include <vector>
 
+#include "grid.cuh"
 #include "stages.cuh"
 
 namespace sfe {
@@ -343,21 +344,33 @@ int sfe_match_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off
                    {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, max_dist, ids_dev, dists_dev);
 }
 
-int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, float max_dist,
-                   int32_t *ids_host, float *dists_host) {
-  SFE_REQUIRE(ctx != nullptr, "sfe_match_host: null context");
-  SFE_REQUIRE(n_ref >= 0 && n_in >= 0, "sfe_match_host: negative point count");
-  if (n_in == 0) return SFE_OK;
-  SFE_REQUIRE(in_host && ids_host && dists_host && (ref_host || n_ref == 0), "sfe_match_host: null pointer");
+int sfe_match_knn_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev, const float *in_pts_dev,
+                      const int32_t *in_off_dev, int n_pairs, int n_ref_max, int knn, float max_dist, int32_t *ids_dev,
+                      float *dists_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_match_knn_dev: null context");
   SFE_CUDA(cudaSetDevice(ctx->device));
+  return match_knn_run(ctx, ctx->stream, {ref_pts_dev, ref_off_dev, nullptr, n_ref_max},
+                       {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, knn, max_dist, ids_dev, dists_dev);
+}
+
+// sfe_match_host and sfe_match_knn_host (`name` in messages): one pair, results [knn][n_in]
+static int match_host(sfe_ctx *ctx, const char *name, const float *ref_host, int n_ref, const float *in_host, int n_in,
+                      int knn, float max_dist, int32_t *ids_host, float *dists_host) {
+  SFE_REQUIRE(ctx != nullptr, "%s: null context", name);
+  SFE_REQUIRE(n_ref >= 0 && n_in >= 0, "%s: negative point count", name);
+  SFE_REQUIRE(knn >= 1 && knn <= GRID_KNN_MAX, "%s: knn %d is not supported (1..%d)", name, knn, GRID_KNN_MAX);
+  if (n_in == 0) return SFE_OK;
+  SFE_REQUIRE(in_host && ids_host && dists_host && (ref_host || n_ref == 0), "%s: null pointer", name);
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  const size_t out = (size_t)knn * n_in;
   Carver cv;
   for (int pass = 0; pass < 2; ++pass) {
     cv.off = 0;
     float *d_ref = (float *)cv.take(sizeof(float) * 2 * (size_t)(n_ref > 0 ? n_ref : 1));
     float *d_in = (float *)cv.take(sizeof(float) * 2 * (size_t)n_in);
     int32_t *d_off = (int32_t *)cv.take(4 * sizeof(int32_t));
-    int32_t *d_ids = (int32_t *)cv.take(sizeof(int32_t) * (size_t)n_in);
-    float *d_d = (float *)cv.take(sizeof(float) * (size_t)n_in);
+    int32_t *d_ids = (int32_t *)cv.take(sizeof(int32_t) * out);
+    float *d_d = (float *)cv.take(sizeof(float) * out);
     if (pass == 0) {
       int rc = ensure(ctx, ctx->stage_in[1], cv.off);
       if (rc != SFE_OK) return rc;
@@ -369,14 +382,24 @@ int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *
       SFE_CUDA(cudaMemcpyAsync(d_ref, ref_host, sizeof(float) * 2 * (size_t)n_ref, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_in, in_host, sizeof(float) * 2 * (size_t)n_in, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
-    int rc = match_run(ctx, ctx->stream, {d_ref, d_off, nullptr, n_ref}, {d_in, d_off + 2, nullptr, n_in}, 1, max_dist,
-                       d_ids, d_d);
+    int rc = match_knn_run(ctx, ctx->stream, {d_ref, d_off, nullptr, n_ref}, {d_in, d_off + 2, nullptr, n_in}, 1, knn,
+                           max_dist, d_ids, d_d);
     if (rc != SFE_OK) return rc;
-    SFE_CUDA(cudaMemcpyAsync(ids_host, d_ids, sizeof(int32_t) * (size_t)n_in, cudaMemcpyDeviceToHost, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(dists_host, d_d, sizeof(float) * (size_t)n_in, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(ids_host, d_ids, sizeof(int32_t) * out, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(dists_host, d_d, sizeof(float) * out, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   return SFE_OK;
+}
+
+int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, float max_dist,
+                   int32_t *ids_host, float *dists_host) {
+  return match_host(ctx, "sfe_match_host", ref_host, n_ref, in_host, n_in, 1, max_dist, ids_host, dists_host);
+}
+
+int sfe_match_knn_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int knn,
+                       float max_dist, int32_t *ids_host, float *dists_host) {
+  return match_host(ctx, "sfe_match_knn_host", ref_host, n_ref, in_host, n_in, knn, max_dist, ids_host, dists_host);
 }
 
 void sfe_icp_params_default(sfe_icp_params *p) {

@@ -576,37 +576,34 @@ __device__ __forceinline__ NNResult nn_query_seeded(const GridViewT<Idx> &g, flo
   return r;  // r.pos >= 0: the seed's own cell is inside the rectangle
 }
 
-// ---- surface normals (point-to-plane minimiser, icp.yaml:18-19 + a SurfaceNormalDataPointsFilter{knn} on the
-// reference; statement: oracle/icp_ref.c orc_surface_normals).  For the grid point at sorted position p: its knn
-// nearest grid points (itself included) in ascending (squared distance, original index) order, found ring by ring
-// around its cell until the k-th distance is below the bound of everything outside the rings scanned; then mean,
-// 2x2 covariance and the unit eigenvector of the smaller eigenvalue in closed form -- every operation a float32
-// IEEE operation in the oracle's order, so the normals are bit-identical to the oracle's.
-// The running best-knn list is the caller's: bd[j * stride], bi[j * stride], j < knn.  The scan matcher hands out
-// shared memory that is idle while the normals are computed (stride = CTA size, one column per thread): a list in
-// local memory spills past the little L1 that a CTA's shared-memory carve-out leaves, so local arrays (stride 1) are only the fallback for CTAs without that room.
+// ---- k nearest neighbours: a best-knn list per query in ascending (squared distance, original index) order, held
+// by the caller as bd[j * stride] (distances), bi[j * stride] (sorted positions), j < knn, and filled ring by ring of
+// cells around the query's cell until the knn-th distance is below the bound of everything outside the rings scanned.
+// Shared by the surface normals below and the k-nearest-neighbour matcher (grid_knn_query).
 constexpr int GRID_KNN_MAX = 16;
+
+// Offer the grid point at sorted position j, at squared distance d2, to the list: k = entries so far (grows to knn),
+// kth = the knn-th distance (+inf until knn points are listed).  While the list is not full, d2 must be below +inf.
 template <typename Idx, typename B>
-__device__ inline float2 grid_surface_normal(const GridViewT<Idx> &g, int p, int knn, float *bd, B *bi, int stride) {
-  const float2 q = g.pts[p];
-  const int cx = grid_cell_coord(q.x, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(q.y, g.oy, g.inv_cell, g.ny);
-  int k = 0;
-  float kth = INFINITY;
-  auto offer = [&](int s, int e) {
-    for (int j = s; j < e; ++j) {
-      const float2 t = g.pts[j];
-      const float d2 = dist2_rn(q.x - t.x, q.y - t.y);
-      if (d2 > kth) continue;  // kth = the knn-th distance so far (+inf until knn points are listed)
-      if (d2 == kth && g.orig[j] > g.orig[bi[(k - 1) * stride]]) continue;
-      int at = k < knn ? k++ : knn - 1;
-      while (at > 0 && (d2 < bd[(at - 1) * stride] || (d2 == bd[(at - 1) * stride] && g.orig[j] < g.orig[bi[(at - 1) * stride]]))) {
-        bd[at * stride] = bd[(at - 1) * stride], bi[at * stride] = bi[(at - 1) * stride];
-        --at;
-      }
-      bd[at * stride] = d2, bi[at * stride] = (B)j;
-      if (k == knn) kth = bd[(k - 1) * stride];
-    }
-  };
+__device__ __forceinline__ void knn_offer(const GridViewT<Idx> &g, float d2, int j, int knn, float *bd, B *bi,
+                                          int stride, int &k, float &kth) {
+  if (d2 > kth) return;
+  if (d2 == kth && g.orig[j] > g.orig[bi[(k - 1) * stride]]) return;
+  int at = k < knn ? k++ : knn - 1;
+  while (at > 0 && (d2 < bd[(at - 1) * stride] || (d2 == bd[(at - 1) * stride] && g.orig[j] < g.orig[bi[(at - 1) * stride]]))) {
+    bd[at * stride] = bd[(at - 1) * stride], bi[at * stride] = bi[(at - 1) * stride];
+    --at;
+  }
+  bd[at * stride] = d2, bi[at * stride] = (B)j;
+  if (k == knn) kth = bd[(k - 1) * stride];
+}
+
+// The ring loop: offer(s, e) gets every ring's cells as contiguous ranges of sorted positions, ring 0 being the cell
+// (cx, cy) itself.  Stops when `kth` (the caller's, updated by offer) is below the bound of every unscanned cell, when
+// that bound exceeds lim2 (nothing outside can be accepted), or when the rings cover the grid.
+template <typename Idx, typename F>
+__device__ __forceinline__ void knn_rings(const GridViewT<Idx> &g, float qx, float qy, int cx, int cy, const float &kth,
+                                          float lim2, F &&offer) {
   for (int kr = 0;; ++kr) {
     const int x0 = cx - kr, x1 = cx + kr, y0 = cy - kr, y1 = cy + kr;
     for (int y = max(y0, 0); y <= min(y1, g.ny - 1); ++y) {
@@ -618,9 +615,51 @@ __device__ inline float2 grid_surface_normal(const GridViewT<Idx> &g, int p, int
         if (x1 <= g.nx - 1) offer(g.cstart[row + x1], g.cstart[row + x1 + 1]);
       }
     }
-    const float b2 = nn_block_bound2(g, q.x, q.y, cx, cy, kr);
-    if (b2 == INFINITY || kth < b2) break;
+    const float b2 = nn_block_bound2(g, qx, qy, cx, cy, kr);
+    if (b2 == INFINITY || kth < b2 || b2 > lim2) break;
   }
+}
+
+// The knn nearest grid points of (qx, qy) among those with squared distance <= max_d2 (nn_query's radius test and
+// distance expression; +inf and NaN distances never count, as in nn_query).  Returns how many were listed (<= knn);
+// list entry 0 is nn_query's answer.
+template <typename Idx, typename B>
+__device__ __forceinline__ int grid_knn_query(const GridViewT<Idx> &g, float qx, float qy, float max_d2, int knn,
+                                              float *bd, B *bi, int stride) {
+  if (g.n <= 0) return 0;
+  const int cx = grid_cell_coord(qx, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(qy, g.oy, g.inv_cell, g.ny);
+  int k = 0;
+  float kth = INFINITY;
+  knn_rings(g, qx, qy, cx, cy, kth, max_d2, [&](int s, int e) {
+    for (int j = s; j < e; ++j) {
+      const float2 t = g.pts[j];
+      const float d2 = dist2_rn(qx - t.x, qy - t.y);
+      if (d2 <= max_d2 && d2 < INFINITY) knn_offer(g, d2, j, knn, bd, bi, stride, k, kth);
+    }
+  });
+  return k;
+}
+
+// ---- surface normals (point-to-plane minimiser, icp.yaml:18-19 + a SurfaceNormalDataPointsFilter{knn} on the
+// reference; statement: oracle/icp_ref.c orc_surface_normals).  For the grid point at sorted position p: its knn
+// nearest grid points (itself included) in ascending (squared distance, original index) order (knn_rings); then mean,
+// 2x2 covariance and the unit eigenvector of the smaller eigenvalue in closed form -- every operation a float32
+// IEEE operation in the oracle's order, so the normals are bit-identical to the oracle's.
+// The scan matcher hands out shared memory that is idle while the normals are computed for the list (stride = CTA
+// size, one column per thread): a list in local memory spills past the little L1 that a CTA's shared-memory carve-out
+// leaves, so local arrays (stride 1) are only the fallback for CTAs without that room.
+template <typename Idx, typename B>
+__device__ inline float2 grid_surface_normal(const GridViewT<Idx> &g, int p, int knn, float *bd, B *bi, int stride) {
+  const float2 q = g.pts[p];
+  const int cx = grid_cell_coord(q.x, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(q.y, g.oy, g.inv_cell, g.ny);
+  int k = 0;
+  float kth = INFINITY;
+  knn_rings(g, q.x, q.y, cx, cy, kth, INFINITY, [&](int s, int e) {
+    for (int j = s; j < e; ++j) {
+      const float2 t = g.pts[j];
+      knn_offer(g, dist2_rn(q.x - t.x, q.y - t.y), j, knn, bd, bi, stride, k, kth);
+    }
+  });
   float sx = 0.f, sy = 0.f;
   for (int j = 0; j < k; ++j) sx = __fadd_rn(sx, g.pts[bi[j * stride]].x), sy = __fadd_rn(sy, g.pts[bi[j * stride]].y);
   const float kf = (float)k, mx = __fdiv_rn(sx, kf), my = __fdiv_rn(sy, kf);

@@ -418,6 +418,42 @@ struct MatchBatch {
   int map_cell_cap;
 };
 
+// One pair's reference of nt points (nt >= 1) in match_kernel's layout: the bounding box over the CTA, the grid
+// geometry and the counting sort into sorted / cells (shared), original indices in orig.  All threads call it.
+__device__ __forceinline__ void match_ref_grid(const MatchBatch &b, const float *ref, int nt, float2 *sorted,
+                                               uint32_t *cells, uint16_t *orig, int *scan, float *bbox_w, float *bbox,
+                                               GridView &g) {
+  const int tid = threadIdx.x, nthr = blockDim.x;
+  float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
+  for (int i = tid; i < nt; i += nthr) {
+    const float x = ref[2 * i], y = ref[2 * i + 1];
+    mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
+    mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
+    mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
+    mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
+  }
+  if ((tid & 31) == 0) {
+    bbox_w[(tid >> 5) * 4 + 0] = mn_x, bbox_w[(tid >> 5) * 4 + 1] = mn_y;
+    bbox_w[(tid >> 5) * 4 + 2] = mxx, bbox_w[(tid >> 5) * 4 + 3] = mxy;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
+    for (int w = 0; w < (nthr >> 5); ++w) {
+      a = fminf(a, bbox_w[w * 4 + 0]), bb = fminf(bb, bbox_w[w * 4 + 1]);
+      c = fmaxf(c, bbox_w[w * 4 + 2]), d = fmaxf(d, bbox_w[w * 4 + 3]);
+    }
+    bbox[0] = a, bbox[1] = bb, bbox[2] = c, bbox[3] = d;
+  }
+  __syncthreads();
+  grid_geometry(nt, bbox[0], bbox[1], bbox[2], bbox[3], 0.05f, g, b.max_cells);
+  grid_build(ref, 2, nt, 0.f, 0.f, g, sorted, cells, orig, scan);
+}
+
 __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int scan[36];
@@ -441,35 +477,8 @@ __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) 
       for (int i = tid; i < ns; i += nthr) ids[i] = -1, dists[i] = INFINITY;
       continue;
     }
-    float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
-    for (int i = tid; i < nt; i += nthr) {
-      const float x = ref[2 * i], y = ref[2 * i + 1];
-      mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      mn_x = fminf(mn_x, __shfl_xor_sync(0xffffffffu, mn_x, d));
-      mn_y = fminf(mn_y, __shfl_xor_sync(0xffffffffu, mn_y, d));
-      mxx = fmaxf(mxx, __shfl_xor_sync(0xffffffffu, mxx, d));
-      mxy = fmaxf(mxy, __shfl_xor_sync(0xffffffffu, mxy, d));
-    }
-    if ((tid & 31) == 0) {
-      bbox_w[(tid >> 5) * 4 + 0] = mn_x, bbox_w[(tid >> 5) * 4 + 1] = mn_y;
-      bbox_w[(tid >> 5) * 4 + 2] = mxx, bbox_w[(tid >> 5) * 4 + 3] = mxy;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      float a = INFINITY, bb = INFINITY, c = -INFINITY, d = -INFINITY;
-      for (int w = 0; w < (nthr >> 5); ++w) {
-        a = fminf(a, bbox_w[w * 4 + 0]), bb = fminf(bb, bbox_w[w * 4 + 1]);
-        c = fmaxf(c, bbox_w[w * 4 + 2]), d = fmaxf(d, bbox_w[w * 4 + 3]);
-      }
-      bbox[0] = a, bbox[1] = bb, bbox[2] = c, bbox[3] = d;
-    }
-    __syncthreads();
     GridView g;
-    grid_geometry(nt, bbox[0], bbox[1], bbox[2], bbox[3], 0.05f, g, b.max_cells);
-    grid_build(ref, 2, nt, 0.f, 0.f, g, sorted, cells, orig, scan);
+    match_ref_grid(b, ref, nt, sorted, cells, orig, scan, bbox_w, bbox, g);
     for (int i = tid; i < ns; i += nthr) {
       const NNResult r = nn_query(g, in[2 * i], in[2 * i + 1], max_d2);
       ids[i] = r.pos >= 0 ? (int32_t)orig[r.pos] : -1;
@@ -495,6 +504,80 @@ __global__ void __launch_bounds__(ICP_THREADS) match_map_kernel(const MatchBatch
       const NNResult r = nn_query(g, in[2 * i], in[2 * i + 1], max_d2);
       b.ids[b.in_off[p] + i] = r.pos >= 0 ? (int32_t)g.orig[r.pos] : -1;
       b.dists[b.in_off[p] + i] = r.d2;
+    }
+  }
+}
+
+// pcl.match with knn > 1 (grid_knn_query).  Output rows: neighbour j of query i of pair p goes to j * total + in_off[p]
+// + i (total = in_off[P]); the first `found` slots hold the neighbours, the others -1 / +inf.
+template <typename Idx, typename B>
+__device__ __forceinline__ void match_knn_rows(const Idx *orig, int found, int knn, const float *bd, const B *bi,
+                                               int stride, int32_t *ids, float *dists, size_t total) {
+  for (int j = 0; j < knn; ++j) {
+    const bool hit = j < found;
+    ids[j * total] = hit ? (int32_t)orig[bi[j * stride]] : -1;
+    dists[j * total] = hit ? bd[j * stride] : INFINITY;
+  }
+}
+
+// The in-CTA class: match_kernel's layout, then from byte list_off the best-knn lists, one column per thread
+// (distances [knn][blockDim.x], then uint16 sorted positions [knn][blockDim.x]).
+__global__ void __launch_bounds__(ICP_THREADS) match_knn_kernel(const MatchBatch b, int knn, int list_off) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ int scan[36];
+  __shared__ float bbox_w[4 * 32];
+  __shared__ float bbox[4];
+  float2 *sorted = reinterpret_cast<float2 *>(smem_raw);
+  uint32_t *cells = reinterpret_cast<uint32_t *>(smem_raw + sizeof(float2) * (size_t)b.nt_max);
+  const int tid = threadIdx.x, nthr = blockDim.x;
+  float *bd = reinterpret_cast<float *>(smem_raw + list_off) + tid;
+  uint16_t *bi = reinterpret_cast<uint16_t *>(smem_raw + list_off + sizeof(float) * (size_t)nthr * knn) + tid;
+  uint16_t *orig = b.orig_ws + (size_t)blockIdx.x * b.nt_max;
+  const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
+  const size_t total = (size_t)b.in_off[b.P];
+  for (int p = blockIdx.x; p < b.P; p += gridDim.x) {
+    const float *ref = b.ref_pts + 2 * (size_t)b.ref_off[p];
+    const int nt = b.ref_off[p + 1] - b.ref_off[p];
+    const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
+    const int ns = b.in_off[p + 1] - b.in_off[p];
+    int32_t *ids = b.ids + b.in_off[p];
+    float *dists = b.dists + b.in_off[p];
+    if (nt > b.nt_max) continue;  // the map class's (match_knn_map_kernel)
+    __syncthreads();
+    if (nt <= 0) {
+      for (int i = tid; i < ns; i += nthr) match_knn_rows(orig, 0, knn, bd, bi, nthr, ids + i, dists + i, total);
+      continue;
+    }
+    GridView g;
+    match_ref_grid(b, ref, nt, sorted, cells, orig, scan, bbox_w, bbox, g);
+    for (int i = tid; i < ns; i += nthr) {
+      const int found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
+      match_knn_rows(orig, found, knn, bd, bi, nthr, ids + i, dists + i, total);
+    }
+  }
+}
+
+// The map class of knn > 1: match_map_kernel with the best-knn lists in dynamic shared memory (distances
+// [knn][blockDim.x], then int sorted positions [knn][blockDim.x]).
+__global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchBatch b, int knn) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int tid = threadIdx.x, nthr = blockDim.x;
+  float *bd = reinterpret_cast<float *>(smem_raw) + tid;
+  int *bi = reinterpret_cast<int *>(smem_raw + sizeof(float) * (size_t)nthr * knn) + tid;
+  const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
+  const size_t total = (size_t)b.in_off[b.P];
+  for (int p = 0; p < b.P; ++p) {
+    const int ms = b.map_slot[p];
+    if (ms < 0) continue;
+    const MapGrid &mg = b.map_grid[ms];
+    MapGridView g;
+    g.pts = b.map_pts, g.cstart = b.map_cstart + (size_t)ms * b.map_cell_cap, g.orig = b.map_orig;
+    g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
+    const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
+    const int ns = b.in_off[p + 1] - b.in_off[p];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) {
+      const int found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
+      match_knn_rows(g.orig, found, knn, bd, bi, nthr, b.ids + b.in_off[p] + i, b.dists + b.in_off[p] + i, total);
     }
   }
 }
@@ -893,6 +976,59 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
   b.map_cell_cap = w.cell_cap;
   match_map_kernel<<<ctx->sm_count * 4, ICP_THREADS, 0, st>>>(b);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return SFE_OK;
+}
+
+// knn 1: match_run.  knn > 1: references whose layout fits one CTA next to the best-knn lists run in match_knn_kernel,
+// larger ones as map grids in match_knn_map_kernel, in the same call.
+int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, int knn,
+                       float max_dist, int32_t *ids, float *dists) {
+  SFE_REQUIRE(knn >= 1 && knn <= GRID_KNN_MAX, "match: knn %d is not supported (1..%d)", knn, GRID_KNN_MAX);
+  if (knn == 1) return match_run(ctx, st, ref, in, P, max_dist, ids, dists);
+  const int nt_max = ref.n_max;
+  SFE_REQUIRE(ctx, "match: null context");
+  SFE_REQUIRE(P >= 0 && nt_max >= 0, "match: negative sizes");
+  if (P == 0) return SFE_OK;
+  SFE_REQUIRE(ref.pts && ref.off && in.pts && in.off && ids && dists, "match: null pointer");
+  SFE_REQUIRE(!ref.cnt && !in.cnt, "match: per-cloud counts are not supported");
+  const size_t lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(uint16_t));
+  auto list_off = [](int nt) { return (match_cta_smem(nt) + 15) & ~size_t(15); };
+  size_t budget;
+  int rc = cta_smem_budget(ctx, (const void *)match_knn_kernel, &budget);
+  if (rc != SFE_OK) return rc;
+  const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) { return list_off(nt) + lists; });
+  MatchBatch b{};
+  b.ref_pts = ref.pts, b.ref_off = ref.off, b.in_pts = in.pts, b.in_off = in.off;
+  b.P = P, b.max_dist = max_dist;
+  b.ids = ids, b.dists = dists;
+  const int nt_cta = std::min(nt_max, limit);
+  b.nt_max = nt_cta > 0 ? nt_cta : 1, b.max_cells = pick_max_cells(b.nt_max);
+  const size_t smem = list_off(b.nt_max) + lists;
+  if (smem > budget) {
+    set_error("match: knn %d needs %zu B of shared memory per CTA (limit %zu)", knn, smem, budget);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  int per_sm;
+  if ((rc = ctas_per_sm(ctx, (const void *)match_knn_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
+  int grid = ctx->sm_count * per_sm;
+  if (grid > P) grid = P;
+  rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
+  if (rc != SFE_OK) return rc;
+  b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
+  match_knn_kernel<<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  if (nt_max <= limit) return SFE_OK;
+  MapWs w;
+  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, limit, P, false, true, 0, w);
+  if (rc != SFE_OK) return rc;
+  b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
+  b.map_cell_cap = w.cell_cap;
+  const size_t map_lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(int));
+  if ((rc = ctas_per_sm(ctx, (const void *)match_knn_map_kernel, ICP_THREADS, map_lists, &per_sm)) != SFE_OK) return rc;
+  match_knn_map_kernel<<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;

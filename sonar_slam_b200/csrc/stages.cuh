@@ -67,6 +67,10 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpP
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
               int32_t *ids, float *dists);
+// the knn (1 .. GRID_KNN_MAX) nearest reference points of every input point: ids / dists [knn][in.off[P]], neighbour j
+// of every point in row j; knn 1 is match_run
+int match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, int knn,
+                  float max_dist, int32_t *ids, float *dists);
 
 // One map grid: a cloud too large for a one-CTA layout, built once per call in global memory (map_build).
 struct MapGrid {

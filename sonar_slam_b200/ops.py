@@ -129,15 +129,26 @@ def remove_outlier(pts, off, n_max, radius, min_points, ctx=None):
     return dict(pts=out, idx=idx, count=cnt)
 
 
-def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, ctx=None):
-    """Batched pcl.match (include/sonarfe.h: sfe_match_dev).  References of any size: those above one CTA's shared
-    memory (whole maps) are searched as map grids in global memory, with the same results."""
+def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, knn=None, ctx=None):
+    """Batched pcl.match (include/sonarfe.h: sfe_match_dev).  Without knn: the nearest reference point of every query,
+    ids int32 and squared dists float32 [total query points].  With knn (1 .. 16, sfe_match_knn_dev): [knn, total]
+    tensors whose row j holds every query's j-th nearest reference point within max_dist (-1 / +inf where there is
+    none).  References of any size: those above one CTA's shared memory (whole maps) are searched as map grids in
+    global memory, with the same results."""
+    if knn is not None and int(knn) < 1:
+        raise ValueError(f"ops.match: knn must be at least 1 (got {knn})")
     ctx = ctx or context(ref_pts.device)
     n = ref_off.numel() - 1
-    ids = torch.empty((in_pts.shape[0],), dtype=torch.int32, device=in_pts.device)
-    d = torch.empty((in_pts.shape[0],), dtype=torch.float32, device=in_pts.device)
-    _lib.check(ctx.lib.sfe_match_dev(ctx.handle, _dp(ref_pts), _dp(ref_off), _dp(in_pts), _dp(in_off), n,
-                                     int(n_ref_max), float(max_dist), _dp(ids), _dp(d)), "sfe_match_dev")
+    shape = (in_pts.shape[0],) if knn is None else (int(knn), in_pts.shape[0])
+    ids = torch.empty(shape, dtype=torch.int32, device=in_pts.device)
+    d = torch.empty(shape, dtype=torch.float32, device=in_pts.device)
+    if knn is None:
+        _lib.check(ctx.lib.sfe_match_dev(ctx.handle, _dp(ref_pts), _dp(ref_off), _dp(in_pts), _dp(in_off), n,
+                                         int(n_ref_max), float(max_dist), _dp(ids), _dp(d)), "sfe_match_dev")
+    else:
+        _lib.check(ctx.lib.sfe_match_knn_dev(ctx.handle, _dp(ref_pts), _dp(ref_off), _dp(in_pts), _dp(in_off), n,
+                                             int(n_ref_max), int(knn), float(max_dist), _dp(ids), _dp(d)),
+                   "sfe_match_knn_dev")
     return dict(ids=ids, dists=d)
 
 
