@@ -258,7 +258,8 @@ enum {
   SFE_ICP_NAN_TRANS = 4,    /* ConvergenceError "abs translation norm not a number" */
   SFE_ICP_NOT_RIGID = 5,    /* TransformationError: the initial guess is not a rigid transform */
   SFE_ICP_EMPTY_REF = 6,    /* the target cloud is empty */
-  SFE_ICP_SKIPPED = 7,      /* front-end pipeline only: fewer than min_points source/target points (slam.py:654-663) */
+  SFE_ICP_SKIPPED = 7,      /* front-end pipeline only: fewer than min_points source/target points (slam.py:654-663),
+                               or the scan match is off (sfe_frontend_set_scan_match) */
   SFE_ICP_TOO_LARGE = 8     /* front-end pipeline only: a cloud exceeded the configured capacity */
 };
 SFE_API const char *sfe_icp_status_message(int status);
@@ -418,6 +419,25 @@ SFE_API int sfe_frontend_get_timing(sfe_frontend *fe, double *stage_ms, int64_t 
 SFE_API int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const double *poses_host,
                                   int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
                                   int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host);
+/* Every frame's filtered cloud, packed.  With dst != NULL, every later run call on this handle (all flavours) also
+ * writes the clouds of its frames one after another: frame i's cloud is dst[offsets[i] .. offsets[i + 1]) as float32
+ * (x, y) pairs, in the front end's flip_lateral convention (1: SLAM's (x, -z); 0: FeatureExtraction.callback's
+ * (p0, p1)), the points those of sfe_frontend_results_dev's strided clouds; offsets int64 [n_frames + 1], offsets[0] =
+ * 0.  Both live in host memory (on_host != 0) for the host, geometry, JPEG and PNG flavours and in device memory
+ * (on_host = 0) for sfe_frontend_run_dev[_geometry]; a call of the other kind is rejected before any device work.
+ * The host flavours copy each chunk's clouds out while later chunks compute; run_dev writes them on the device and then
+ * waits for the call to finish, to check the capacity.  A call whose clouds need more than capacity_points points fails
+ * with SFE_ERR_CAPACITY, its message stating the total needed: offsets is filled all the same, no point is written
+ * past the capacity, the other outputs are unspecified and the carried window (sfe_frontend_set_carry) stays as it
+ * was, so a retry with a larger buffer continues the sequence.  dst = NULL (the default) turns it off; the other
+ * results are the same with and without clouds. */
+SFE_API int sfe_frontend_set_clouds(sfe_frontend *fe, float *dst, int64_t capacity_points, int64_t *offsets,
+                                    int on_host);
+/* enable = 0: every run flavour computes the clouds only.  The window submaps and ICP are not launched; every frame's
+ * status is SFE_ICP_SKIPPED (SFE_ICP_TOO_LARGE where its Cartesian cloud overflowed cap_points), T the identity,
+ * iterations and inliers 0.  With carry on the carried window still advances, so turning the scan match back on
+ * continues the sequence.  enable != 0: the default. */
+SFE_API int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable);
 /* Several sonar geometries in one front end: a bag whose range setting changes (num_ranges, range_resolution, beam
  * count) is fed as one sequence, and the first frames after a change are matched against the keyframes before it, as
  * the reference's window of metric keyframe clouds does (slam.py:632-633).

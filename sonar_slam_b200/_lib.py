@@ -23,6 +23,10 @@ class SonarFEError(RuntimeError):
     pass
 
 
+ERR_CAPACITY = -3  # SFE_ERR_CAPACITY: a caller-provided output buffer was too small
+ICP_SKIPPED, ICP_TOO_LARGE = 7, 8  # SFE_ICP_SKIPPED, SFE_ICP_TOO_LARGE
+
+
 def load():
     """Load (building first if sources are newer and nvcc is present) and type the library."""
     global _lib
@@ -112,6 +116,8 @@ _EXTRA_SIGNATURES = {
     "sfe_frontend_set_timing": [c_void_p, c_int],
     "sfe_frontend_set_carry": [c_void_p, c_int],
     "sfe_frontend_set_overlap": [c_void_p, c_int],
+    "sfe_frontend_set_clouds": [c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_int],
+    "sfe_frontend_set_scan_match": [c_void_p, c_int],
     "sfe_frontend_get_timing": [c_void_p, c_void_p, c_void_p],
     "sfe_frontend_run_dev": [c_void_p, c_void_p, c_void_p, c_int],
     "sfe_frontend_results_dev": [c_void_p] + [ctypes.POINTER(c_void_p)] * 6 + [ctypes.POINTER(ctypes.c_int32)],

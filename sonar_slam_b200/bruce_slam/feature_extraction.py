@@ -225,3 +225,110 @@ class FeatureExtraction(object):
         if self.outlier_filter_min_points > 1 and len(points) > 0:
             points = pcl.remove_outlier(points, self.outlier_filter_radius, self.outlier_filter_min_points)
         return self.publish_features(sonar_msg, points)
+
+    def callback_batch(self, sonar_msgs, max_frames=256):
+        """callback() over a sequence of pings: returns the list of `feature_msg`s that calling callback on each
+        message in turn would leave, byte for byte, and leaves `points` / `feature_msg` as the last call would
+        (`locs` and the feature images are not produced).  The pings that are not skipped go through the batched front
+        end (pipeline.FrontEnd) with its scan match off, at most `max_frames` per call: streams that sonar_slam_b200.jpeg
+        or .png accepts as run_jpeg_host / run_png_host, everything else decoded by ping_image and sent through
+        run_host; each geometry is a front-end geometry (add_geometry).  A ping whose Cartesian cloud overflows the
+        front end's cap_points, or whose stream the device decoder rejects after all, takes callback()."""
+        from .. import jpeg, png
+        msgs = list(sonar_msgs)
+        points = [None] * len(msgs)
+        if self.detector is None:
+            self.configure()
+        ctx = _lib.default_context()
+        # the pings with device work, by how they reach the device: (message index, geometry maps, image or stream)
+        groups = {jpeg: [], png: [], None: []}
+        for i, m in enumerate(msgs):
+            if m.ping_id % self.skip != 0:
+                points[i] = np.array([[np.nan, np.nan]])
+                continue
+            img = getattr(m, "image", None)
+            data = getattr(m.ping if img is None else img, "data", None)
+            codec = None
+            if self.compressed_images and isinstance(data, (bytes, bytearray, memoryview)):
+                codec = png if bytes(data[:8]) == png.SIGNATURE else jpeg
+                info = codec.inspect([data])[0]
+                if info[0] == codec.OK:
+                    R, B, img = int(info[1]), int(info[2]), bytes(data)
+                else:
+                    codec = None
+            if codec is None:
+                img = self.ping_image(m)
+                if img.dtype != np.uint8 or img.ndim != 2:
+                    raise TypeError("FeatureExtraction.callback: the ping image must be uint8 [num_ranges, num_beams]")
+                R, B = img.shape
+            self.generate_map_xy(m)
+            groups[codec].append((i, self._batch_maps(ctx, B), img))
+        for codec, items in groups.items():
+            for s in range(0, len(items), max_frames):
+                part = items[s:s + max_frames]
+                try:
+                    clouds = self._batch_clouds(ctx, codec, part, max_frames)
+                except _lib.SonarFEError:
+                    if codec is None:
+                        raise
+                    clouds = [None] * len(part)  # a stream the device decoder rejects: callback's own path decides
+                for (i, _, _), c in zip(part, clouds):
+                    points[i] = c if c is not None else self.callback(msgs[i])
+        out = []
+        for m, p in zip(msgs, points):
+            self.publish_features(m, p)
+            out.append(self.feature_msg)
+        return out
+
+    def _batch_maps(self, ctx, num_beams):
+        """The device maps of the geometry generate_map_xy set last, kept for later batches."""
+        cache = self.__dict__.setdefault("_batch_maps_cache", {})
+        key = (id(ctx), self.rows, self.cols, num_beams, self.width, self.height, self.res)
+        if key not in cache:
+            cache[key] = _lib.Maps(ctx, self.map_x, self.map_y, self.rows, num_beams, self.width, self.height)
+        return cache[key]
+
+    def _batch_clouds(self, ctx, codec, part, max_frames):
+        """The filtered clouds of `part` ((index, maps, image or stream) each) from one front-end call per group of
+        geometries that share frame slots; None where a Cartesian cloud overflowed cap_points."""
+        from .. import pipeline
+        prm = self.detector.params[self.alg]
+        kw = dict(cfar_alg=_ALG[self.alg], train_hs=int(prm[0]), guard_hs=int(prm[1]),
+                  rank=int(prm[2]) if self.alg == "OS" else 0, tau=float(prm[-1]), gate_enable=1,
+                  gate_threshold=float(self.threshold), resolution=float(self.resolution),
+                  outlier_radius=float(self.outlier_filter_radius),
+                  outlier_min_points=int(self.outlier_filter_min_points), flip_lateral=0)
+        # a front end's geometry 0 sets its frame slots; every other geometry must fit them
+        heads = []
+        for maps in sorted({id(m): m for _, m, _ in part}.values(), key=lambda m: -m.R * m.B):
+            home = next((h for h in heads if maps.R <= h[0].R and maps.B <= h[0].B), None)
+            if home is None:
+                heads.append([maps])
+            else:
+                home.append(maps)
+        cache = self.__dict__.setdefault("_batch_frontends", {})
+        clouds = [None] * len(part)
+        for geos in heads:
+            key = (tuple(id(m) for m in geos), max_frames, tuple(sorted(kw.items())))
+            if key not in cache:
+                fe = pipeline.FrontEnd(ctx, geos[0], max_frames, **kw)
+                for m in geos[1:]:
+                    fe.add_geometry(m)
+                fe.set_scan_match(False)
+                cache[key] = fe
+            fe = cache[key]
+            gid = {id(m): g for g, m in enumerate(geos)}
+            sel = [k for k, (_, m, _) in enumerate(part) if id(m) in gid]
+            geometry = np.array([gid[id(part[k][1])] for k in sel], np.int32)
+            frames = [part[k][2] for k in sel]
+            poses = np.zeros((len(sel), 3))
+            if codec is not None:
+                run = fe.run_jpeg_host if codec.__name__.endswith("jpeg") else fe.run_png_host
+                res = run(frames, poses, geometry=geometry, clouds=True)
+            else:
+                res = fe.run_host(frames, poses, geometry=geometry, clouds=True)
+            off = res["cloud_offsets"]
+            for j, k in enumerate(sel):
+                if res["status"][j] != _lib.ICP_TOO_LARGE:
+                    clouds[k] = res["clouds"][off[j]:off[j + 1]].copy()
+        return clouds

@@ -14,6 +14,7 @@
 // array, so all stages run without packing or host round trips; the host flavour overlaps the
 // host->device copy of frame chunk k+1 with the kernels of chunk k on two streams.
 #include <algorithm>
+#include <cub/block/block_scan.cuh>
 #include <functional>
 #include <vector>
 
@@ -81,6 +82,51 @@ __global__ void flip_lateral_kernel(float *__restrict__ xy, const int32_t *__res
 __global__ void fill_offsets_kernel(int32_t *off, int n, int stride) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i <= n) off[i] = i * stride;
+}
+
+// Packed clouds (sfe_frontend_set_clouds), step 1: the exclusive scan of the clouds' sizes of frames [f0, f0 + n),
+// off[f + 1] = off[f] + min(cnt[f], cap), continuing from off[f0] (which an earlier chunk's scan wrote; f0 = 0 starts
+// at 0).  One CTA: a call has at most max_frames frames, a few tiles.
+constexpr int FE_SCAN_THREADS = 256;
+__global__ void __launch_bounds__(FE_SCAN_THREADS)
+    cloud_offsets_kernel(const int32_t *__restrict__ cnt, int cap, int f0, int n, int64_t *__restrict__ off) {
+  using Scan = cub::BlockScan<int64_t, FE_SCAN_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  int64_t base = f0 == 0 ? 0 : off[f0];
+  if (f0 == 0 && threadIdx.x == 0) off[0] = 0;
+  for (int t0 = 0; t0 < n; t0 += FE_SCAN_THREADS) {
+    const int i = t0 + threadIdx.x;
+    int64_t incl, tile;
+    Scan(tmp).InclusiveSum(i < n ? (int64_t)min(cnt[f0 + i], cap) : 0, incl, tile);
+    if (i < n) off[f0 + 1 + i] = base + incl;
+    base += tile;
+    __syncthreads();  // tmp is reused by the next tile
+  }
+}
+
+// Step 2: frame f's cloud (min(cnt[f], cap) points at its slot of `clouds`) to dst + 2 (off[f] - off[f0]), for the
+// frames [f0, f0 + n), one CTA each; points at or past `limit` (numbered like off) are not written.
+__global__ void __launch_bounds__(256)
+    gather_clouds_kernel(const float *__restrict__ clouds, const int32_t *__restrict__ cnt, int cap,
+                         const int64_t *__restrict__ off, int f0, int64_t limit, float *__restrict__ dst) {
+  const int f = f0 + blockIdx.x;
+  const int64_t o = off[f];
+  const int m = 2 * (int)max((int64_t)0, min((int64_t)min(cnt[f], cap), limit - o));
+  const float *src = clouds + 2 * (size_t)f * cap;
+  float *out = dst + 2 * (o - off[f0]);
+  for (int i = threadIdx.x; i < m; i += blockDim.x) out[i] = src[i];
+}
+
+// The scan match turned off (sfe_frontend_set_scan_match): the results icp_run gives a problem it skips, without
+// the problem -- TOO_LARGE where the raw Cartesian cloud overflowed its cap, SKIPPED elsewhere.
+__global__ void skip_match_kernel(const int32_t *__restrict__ raw_cnt, int cap, int n, float *__restrict__ T,
+                                  int32_t *__restrict__ iters, int32_t *__restrict__ inliers,
+                                  int32_t *__restrict__ status) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int q = 0; q < 9; ++q) T[9 * (size_t)i + q] = (q % 4 == 0) ? 1.f : 0.f;
+  iters[i] = 0, inliers[i] = 0;
+  status[i] = raw_cnt[i] > cap ? SFE_ICP_TOO_LARGE : SFE_ICP_SKIPPED;
 }
 
 // Target assembly (slam.py:229-292 without the final downsample): for frame i gather the clouds of frames
@@ -181,6 +227,16 @@ struct sfe_frontend {
   size_t img_stage_bytes = 0;
   cudaStream_t img_stream = nullptr;  // copies the images out, next to the frame copies of copy_stream
   cudaEvent_t ev_img_ready[2] = {}, ev_img_copied[2] = {};
+  // packed clouds (sfe_frontend_set_clouds): the caller's destination and offsets; the device-side offsets and their
+  // pinned copy of the host flavours, and the events that hand each chunk's clouds to copy_stream (allocated on first
+  // use)
+  float *cloud_dst = nullptr;      // null: off
+  int64_t cloud_capacity = 0;
+  int64_t *cloud_offsets = nullptr;
+  int cloud_on_host = 0;
+  int64_t *cloud_off = nullptr, *cloud_off_host = nullptr;  // [max_frames + 1]
+  cudaEvent_t ev_cloud[2] = {};
+  int scan_match = 1;  // sfe_frontend_set_scan_match
   StageTimer timer;  // optional per-stage timing, on ctx->stream (the serial schedule)
 };
 
@@ -304,10 +360,13 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   cudaStreamSynchronize(fe->ctx->stream);
   void *bufs[] = {fe->frames, fe->bits, fe->ij, fe->xy_a, fe->xy_b, fe->idx, fe->cnt_a, fe->cnt_b, fe->cnt_c,
                   fe->off_pts, fe->off_tgt, fe->tgt_a, fe->tgt_b, fe->tgt_idx, fe->tcnt_a, fe->tcnt_b, fe->rel,
-                  fe->guess, fe->T, fe->iters, fe->inliers, fe->status, fe->carry_xy, fe->carry_cnt};
+                  fe->guess, fe->T, fe->iters, fe->inliers, fe->status, fe->carry_xy, fe->carry_cnt, fe->cloud_off};
   for (void *b : bufs)
     if (b) cudaFree(b);
   delete[] fe->carry_poses;
+  if (fe->cloud_off_host) cudaFreeHost(fe->cloud_off_host);
+  for (cudaEvent_t ev : fe->ev_cloud)
+    if (ev) cudaEventDestroy(ev);
   for (int k = 0; k < 2; ++k) {
     if (fe->rel_host[k]) cudaFreeHost(fe->rel_host[k]);
     if (fe->ev_rel[k]) cudaEventDestroy(fe->ev_rel[k]);
@@ -381,11 +440,12 @@ static int fe_render_chunk(sfe_frontend *fe, const sfe_maps *m, const uint8_t *f
   return SFE_OK;
 }
 
-// A host flavour returns only after the image copies it enqueued have landed, on every path.
-struct ImagesDrained {
+// A host flavour returns only after the image and cloud copies it enqueued have landed, on every path.
+struct CopiesDrained {
   const sfe_frontend *fe;
-  ~ImagesDrained() {
+  ~CopiesDrained() {
     if (fe->img_dst && fe->img_stream) cudaStreamSynchronize(fe->img_stream);
+    if (fe->cloud_dst) cudaStreamSynchronize(fe->copy_stream);
   }
 };
 
@@ -543,6 +603,13 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
   const sfe_frontend_params &p = fe->p;
   const int cap = p.cap_points, tcap = p.window * cap;
+  if (!fe->scan_match) {
+    skip_match_kernel<<<(n + 255) / 256, 256, 0, st>>>(fe->cnt_a + f0, cap, n, fe->T + 9 * (size_t)f0, fe->iters + f0,
+                                                       fe->inliers + f0, fe->status + f0);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+    return SFE_OK;
+  }
   const int32_t *cnt;
   const float *cloud = fe_cloud(fe, &cnt);
   fe->timer.tic(st, SFE_FE_SUBMAP);
@@ -603,6 +670,89 @@ static int fe_update_carry(sfe_frontend *fe, cudaStream_t st, const double *pose
   return SFE_OK;
 }
 
+// Packed clouds of the host flavours (sfe_frontend_set_clouds).  fe_clouds_chunk packs the clouds of chunk k = frames
+// [f0, f0 + n), once its filters ran, into that chunk's own slots of the filter buffer that does not hold the final
+// clouds (fe_cloud_stage: its content there is dead by then, and nothing writes those slots again before the call
+// returns), and copies the chunk's offsets into the pinned copy.  fe_clouds_out waits for both, then copies the points
+// that fit the capacity to the caller on copy_stream, next to the kernels of the chunks after it.
+struct CloudChunk {
+  int f0 = 0, n = 0, k = 0;
+};
+
+static float *fe_cloud_stage(sfe_frontend *fe) {
+  const int32_t *cnt;
+  return fe_cloud(fe, &cnt) == fe->xy_a ? fe->xy_b : fe->xy_a;
+}
+
+static int fe_clouds_chunk(sfe_frontend *fe, int f0, int n, int k) {
+  if (!fe->cloud_dst) return SFE_OK;
+  sfe_ctx *ctx = fe->ctx;
+  const int cap = fe->p.cap_points;
+  const int32_t *cnt;
+  const float *cloud = fe_cloud(fe, &cnt);
+  cloud_offsets_kernel<<<1, FE_SCAN_THREADS, 0, ctx->stream>>>(cnt, cap, f0, n, fe->cloud_off);
+  gather_clouds_kernel<<<n, 256, 0, ctx->stream>>>(cloud, cnt, cap, fe->cloud_off, f0, INT64_MAX,
+                                                   fe_cloud_stage(fe) + 2 * (size_t)f0 * cap);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  SFE_CUDA(cudaMemcpyAsync(fe->cloud_off_host + f0, fe->cloud_off + f0, sizeof(int64_t) * (n + 1),
+                           cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaEventRecord(fe->ev_cloud[k & 1], ctx->stream));
+  return SFE_OK;
+}
+
+static int fe_clouds_out(sfe_frontend *fe, const CloudChunk &c) {
+  if (!fe->cloud_dst || c.n == 0) return SFE_OK;
+  SFE_CUDA(cudaEventSynchronize(fe->ev_cloud[c.k & 1]));
+  const int64_t a = fe->cloud_off_host[c.f0], b = std::min(fe->cloud_off_host[c.f0 + c.n], fe->cloud_capacity);
+  if (b > a)
+    SFE_CUDA(cudaMemcpyAsync(fe->cloud_dst + 2 * a, fe_cloud_stage(fe) + 2 * (size_t)c.f0 * fe->p.cap_points,
+                             2 * sizeof(float) * (b - a), cudaMemcpyDeviceToHost, fe->copy_stream));
+  return SFE_OK;
+}
+
+static int fe_clouds_check(const sfe_frontend *fe, int64_t total, const char *what) {
+  if (total <= fe->cloud_capacity) return SFE_OK;
+  set_error("%s: the clouds of this call need %lld points; the destination holds %lld (sfe_frontend_set_clouds)", what,
+            (long long)total, (long long)fe->cloud_capacity);
+  return SFE_ERR_CAPACITY;
+}
+
+// the end of a host flavour's clouds: every copy has landed, the offsets go to the caller, the capacity is checked
+static int fe_clouds_finish(sfe_frontend *fe, int n_frames, const char *what) {
+  if (!fe->cloud_dst) return SFE_OK;
+  SFE_CUDA(cudaStreamSynchronize(fe->copy_stream));
+  memcpy(fe->cloud_offsets, fe->cloud_off_host, sizeof(int64_t) * (n_frames + 1));
+  return fe_clouds_check(fe, fe->cloud_off_host[n_frames], what);
+}
+
+// run_dev's clouds: one scan and one gather over the call's frames straight into the caller's device buffers, then
+// the wait for the total
+static int fe_clouds_dev(sfe_frontend *fe, int n_frames, const char *what) {
+  if (!fe->cloud_dst) return SFE_OK;
+  sfe_ctx *ctx = fe->ctx;
+  const int cap = fe->p.cap_points;
+  const int32_t *cnt;
+  const float *cloud = fe_cloud(fe, &cnt);
+  cloud_offsets_kernel<<<1, FE_SCAN_THREADS, 0, ctx->stream>>>(cnt, cap, 0, n_frames, fe->cloud_offsets);
+  gather_clouds_kernel<<<n_frames, 256, 0, ctx->stream>>>(cloud, cnt, cap, fe->cloud_offsets, 0, fe->cloud_capacity,
+                                                          fe->cloud_dst);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  SFE_CUDA(cudaMemcpyAsync(fe->cloud_off_host, fe->cloud_offsets + n_frames, sizeof(int64_t), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+  SFE_CUDA(cudaStreamSynchronize(ctx->stream));
+  return fe_clouds_check(fe, fe->cloud_off_host[0], what);
+}
+
+// the destination kind a flavour writes to, checked before any device work
+static int fe_clouds_args(const sfe_frontend *fe, bool host_flavour, const char *what) {
+  SFE_REQUIRE(!fe->cloud_dst || (fe->cloud_on_host != 0) == host_flavour, "%s: clouds are set to go to %s memory; "
+              "this flavour writes them to %s memory (sfe_frontend_set_clouds with on_host %s)", what,
+              fe->cloud_on_host ? "host" : "device", host_flavour ? "host" : "device", host_flavour ? "!= 0" : "= 0");
+  return SFE_OK;
+}
+
 int sfe_frontend_set_carry(sfe_frontend *fe, int enable) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_carry: null handle");
   fe->carry_on = enable != 0;
@@ -630,6 +780,31 @@ int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_hos
   if (dst) memcpy(fe->img_lut, lut_bgr_host, sizeof(fe->img_lut));
   fe->img_dst = dst;
   fe->img_dst_host = dst_is_host != 0;
+  return SFE_OK;
+}
+
+int sfe_frontend_set_clouds(sfe_frontend *fe, float *dst, int64_t capacity_points, int64_t *offsets, int on_host) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_clouds: null handle");
+  if (dst) {
+    SFE_REQUIRE(offsets != nullptr, "sfe_frontend_set_clouds: null offsets");
+    SFE_REQUIRE(capacity_points >= 0, "sfe_frontend_set_clouds: negative capacity %lld", (long long)capacity_points);
+    SFE_CUDA(cudaSetDevice(fe->ctx->device));
+    const size_t bytes = sizeof(int64_t) * (fe->max_frames + 1);
+    if (!fe->cloud_off) SFE_CUDA(cudaMalloc((void **)&fe->cloud_off, bytes));
+    if (!fe->cloud_off_host) SFE_CUDA(cudaMallocHost((void **)&fe->cloud_off_host, bytes));
+    for (cudaEvent_t &ev : fe->ev_cloud)
+      if (!ev) SFE_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  }
+  fe->cloud_dst = dst;
+  fe->cloud_capacity = capacity_points;
+  fe->cloud_offsets = offsets;
+  fe->cloud_on_host = on_host != 0;
+  return SFE_OK;
+}
+
+int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_scan_match: null handle");
+  fe->scan_match = enable != 0;
   return SFE_OK;
 }
 
@@ -668,7 +843,7 @@ static int fe_order(cudaStream_t before, cudaEvent_t ev, cudaStream_t after) {
 // streams fork from ctx->stream (after the pose upload and anything the caller enqueued there) and join back into it,
 // so ctx->stream orders later work -- the next call included -- after the whole batch.  With several geometries a
 // sub-batch runs CFAR and the Cartesian points once per run inside it, the rest once.
-static int fe_run_overlapped(sfe_frontend *fe, const double *poses_host, int n_frames) {
+static int fe_run_overlapped(sfe_frontend *fe, int n_frames) {
   sfe_ctx *ctx = fe->ctx;
   const int S = fe->overlap;
   int rc = fe_order(ctx->stream, fe->ev_fork, fe->feat_stream);
@@ -679,7 +854,6 @@ static int fe_run_overlapped(sfe_frontend *fe, const double *poses_host, int n_f
     if (rc == SFE_OK) rc = fe_order(fe->feat_stream, fe->ev_feat, fe->match_stream);
     if (rc == SFE_OK) rc = fe_match(fe, fe->match_stream, f0, n);
   }
-  if (rc == SFE_OK) rc = fe_update_carry(fe, fe->match_stream, poses_host, n_frames);
   // join on every path, so that whatever did get enqueued is ordered before later work on ctx->stream
   const int rj = fe_order(fe->feat_stream, fe->ev_join, ctx->stream);
   const int rm = fe_order(fe->match_stream, fe->ev_join, ctx->stream);
@@ -702,11 +876,15 @@ static int fe_render_host_chunk(sfe_frontend *fe, int f0, int n, int k, const ch
   return fe_render_chunk(fe, fe->geo[r.g], fe_run_frame(fe, r, f0), f0, n, k, what);
 }
 
-// The end of a host flavour: the carried window moves on, the results go to the host and the call waits for them.
-static int fe_host_finish(sfe_frontend *fe, const double *poses_host, int n_frames, float *T_host, int32_t *iters_host,
-                          int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
+// The end of a host flavour: the last chunk's clouds go out (a call whose clouds overflow stops here, its carried window
+// as it was), the carried window moves on, the results go to the host and the call waits for them.
+static int fe_host_finish(sfe_frontend *fe, const CloudChunk &last, const double *poses_host, int n_frames,
+                          float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
+                          int32_t *npoints_host, const char *what) {
   sfe_ctx *ctx = fe->ctx;
-  int rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
+  int rc = fe_clouds_out(fe, last);
+  if (rc == SFE_OK) rc = fe_clouds_finish(fe, n_frames, what);
+  if (rc == SFE_OK) rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
   SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
@@ -735,7 +913,8 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
               fe->max_frames);
   SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
-  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  int rc = fe_clouds_args(fe, true, what);
+  if (rc == SFE_OK) rc = fe_geometry_runs(fe, geometry, n_frames, what);
   if (rc != SFE_OK || n_frames == 0) return rc;
   const int32_t *shape = nullptr;  // each frame's R x B, checked by the decoder
   if (geometry) {
@@ -746,7 +925,7 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
   }
   rc = fe_host_begin(fe, n_frames, chunk_frames, what);
   if (rc != SFE_OK) return rc;
-  ImagesDrained drained{fe};
+  CopiesDrained drained{fe};
   sfe_ctx *ctx = fe->ctx;
   StreamDecoder *dec = decoder(ctx);
   dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, shape);
@@ -780,6 +959,7 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
   };
   rc = decode(0, 0);
   int k = 0;
+  CloudChunk prev;
   for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
     const int n = std::min(chunk_frames, n_frames - f0);
     if (f0 + chunk_frames < n_frames) rc = decode(f0 + chunk_frames, k + 1);
@@ -792,10 +972,14 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
       }
     rc = fe_render_host_chunk(fe, f0, n, k, what);
     if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, f0, n);
+    if (rc == SFE_OK) rc = fe_clouds_chunk(fe, f0, n, k);
     if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
+    if (rc == SFE_OK) rc = fe_clouds_out(fe, prev);
+    prev = {f0, n, k};
   }
   if (rc != SFE_OK) return rc;
-  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
+  return fe_host_finish(fe, prev, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host,
+                        what);
 }
 
 // sfe_frontend_run_dev[_geometry]; geometry: one id per frame, or null (every frame geometry 0)
@@ -806,7 +990,8 @@ static int fe_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t
               fe->max_frames);
   SFE_REQUIRE(!fe->img_dst || !fe->img_dst_host, "%s: feature images are set to go to host memory; this flavour "
               "writes them to device memory (sfe_frontend_set_feature_images with dst_is_host = 0)", what);
-  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  int rc = fe_clouds_args(fe, false, what);
+  if (rc == SFE_OK) rc = fe_geometry_runs(fe, geometry, n_frames, what);
   if (rc != SFE_OK || n_frames == 0) return rc;
   sfe_ctx *ctx = fe->ctx;
   SFE_CUDA(cudaSetDevice(ctx->device));
@@ -829,10 +1014,14 @@ static int fe_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t
     if (rc != SFE_OK) return rc;
   }
   // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
-  if (fe->overlap > 0 && !fe->timer.on) return fe_run_overlapped(fe, poses_host, n_frames);
-  rc = fe_features(fe, ctx->stream, 0, n_frames);
-  if (rc != SFE_OK) return rc;
-  rc = fe_match(fe, ctx->stream, 0, n_frames);
+  if (fe->overlap > 0 && !fe->timer.on) {
+    rc = fe_run_overlapped(fe, n_frames);
+  } else {
+    rc = fe_features(fe, ctx->stream, 0, n_frames);
+    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, 0, n_frames);
+  }
+  // a call whose clouds overflow leaves the carried window as it was
+  if (rc == SFE_OK) rc = fe_clouds_dev(fe, n_frames, what);
   if (rc != SFE_OK) return rc;
   return fe_update_carry(fe, ctx->stream, poses_host, n_frames);
 }
@@ -847,7 +1036,8 @@ static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t
               "%s: null argument", what);
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
               fe->max_frames);
-  int rc = fe_geometry_runs(fe, geometry, n_frames, what);
+  int rc = fe_clouds_args(fe, true, what);
+  if (rc == SFE_OK) rc = fe_geometry_runs(fe, geometry, n_frames, what);
   if (rc != SFE_OK) return rc;
   if (offsets) {
     SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
@@ -861,7 +1051,7 @@ static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t
   if (n_frames == 0) return SFE_OK;
   rc = fe_host_begin(fe, n_frames, chunk_frames, what);
   if (rc != SFE_OK) return rc;
-  ImagesDrained drained{fe};
+  CopiesDrained drained{fe};
   rc = fe_upload_poses(fe, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
   sfe_ctx *ctx = fe->ctx;
@@ -870,6 +1060,7 @@ static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t
   // sfe_frontend_run_dev_geometry packs there)
   rc = fe_order(ctx->stream, fe->ev_done, fe->copy_stream);
   int k = 0;
+  CloudChunk prev;
   for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
     const int n = std::min(chunk_frames, n_frames - f0);
     rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) {
@@ -884,11 +1075,15 @@ static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t
     rc = fe_render_host_chunk(fe, f0, n, k, what);
     if (rc != SFE_OK) return rc;
     rc = fe_features(fe, ctx->stream, f0, n);
+    if (rc == SFE_OK) rc = fe_clouds_chunk(fe, f0, n, k);
     if (rc != SFE_OK) return rc;
     rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
+    if (rc == SFE_OK) rc = fe_clouds_out(fe, prev);
+    prev = {f0, n, k};
   }
   if (rc != SFE_OK) return rc;
-  return fe_host_finish(fe, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host);
+  return fe_host_finish(fe, prev, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host,
+                        what);
 }
 
 extern "C" {

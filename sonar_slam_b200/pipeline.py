@@ -111,50 +111,115 @@ class FrontEnd:
         finally:
             self.lib.sfe_frontend_set_feature_images(self.handle, None, None, 0)
 
-    def run_host(self, frames, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
+    def _with_clouds(self, clouds, n, on_device, name, call):
+        """Run `call()` (one run call, returning its status code) with packed clouds when `clouds` asks for them
+        (sfe_frontend_set_clouds), off again afterwards; returns None or (points float32 [total, 2], offsets int64
+        [n + 1]) -- numpy arrays for the host flavours, CUDA tensors on the context's device for run_dev.
+        clouds: None / False (none), True (a buffer of the bound n * cap_points: every frame's cloud has at most
+        cap_points points; a numpy buffer only commits the pages written), an int (that capacity in points; a call whose
+        clouds need more is run once more with a buffer of the total it reports -- it left the carried window as it
+        was), or, for run_dev, (points, offsets) CUDA tensors of the caller, float32 [capacity, 2] and int64 [n + 1]
+        contiguous, which are filled (a call that overflows them raises)."""
+        if clouds is None or clouds is False:
+            _lib.check(call(), name)
+            return None
+        own = not isinstance(clouds, tuple)
+        if own:
+            cap = n * self.params.cap_points if clouds is True else int(clouds)
+            if cap < 0:
+                raise ValueError(f"FrontEnd: clouds capacity {cap} is negative")
+        else:
+            if not on_device:
+                raise ValueError("FrontEnd: caller-provided cloud buffers are for run_dev; the host flavours take "
+                                 "clouds=True or a capacity")
+            import torch
+            pts, off = clouds
+            for t, dt, shape in ((pts, torch.float32, None), (off, torch.int64, (n + 1,))):
+                if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dt and t.is_contiguous()
+                        and (t.shape == shape if shape else (t.dim() == 2 and t.shape[1] == 2))):
+                    raise ValueError("FrontEnd.run_dev: clouds must be contiguous CUDA tensors float32 [capacity, 2] "
+                                     f"and int64 [{n + 1}]")
+            cap = pts.shape[0]
+        for attempt in (0, 1):
+            if own and on_device:
+                import torch
+                dev = torch.device("cuda", self.ctx.device)
+                pts = torch.empty((max(cap, 1), 2), dtype=torch.float32, device=dev)
+                off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+            elif own:
+                pts, off = np.empty((max(cap, 1), 2), np.float32), np.zeros(n + 1, np.int64)
+            if on_device:
+                dst, offsets = ctypes.c_void_p(pts.data_ptr()), ctypes.c_void_p(off.data_ptr())
+            else:
+                dst, offsets = _lib.ptr(pts), _lib.ptr(off)
+            _lib.check(self.lib.sfe_frontend_set_clouds(self.handle, dst, cap, offsets, 0 if on_device else 1),
+                       "sfe_frontend_set_clouds")
+            try:
+                rc = call()
+            finally:
+                self.lib.sfe_frontend_set_clouds(self.handle, None, 0, None, 0)
+            if rc == _lib.ERR_CAPACITY and own and attempt == 0 and clouds is not True:
+                cap = int(off[-1])
+                continue
+            _lib.check(rc, name)
+            return pts[:int(off[-1])], off
+
+    def run_host(self, frames, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None,
+                 clouds=None):
         """frames: uint8 [n,R,B] numpy (pinned memory gives full copy bandwidth); poses: float64 [n,3].
         Returns dict(T [n,3,3] f32, iterations, inliers, status, npoints).  images: an optional uint8
         [n, rows, cols, 3] numpy array that receives every frame's feature image (feature_image.py; colour table
         image_lut, default JET); the results are the same with and without it.
         geometry: one id per frame (add_geometry); frames are then a sequence of uint8 [R_g, B_g] arrays or
-        (bytes, offsets) from pack_frames (sfe_frontend_run_host_geometry)."""
+        (bytes, offsets) from pack_frames (sfe_frontend_run_host_geometry).
+        clouds: True or a capacity in points (see _with_clouds) adds every frame's filtered cloud, packed: "clouds"
+        float32 [total, 2] and "cloud_offsets" int64 [n + 1], frame i = clouds[cloud_offsets[i]:cloud_offsets[i + 1]]
+        in the flip_lateral convention; the other results are the same with and without them."""
         poses = np.ascontiguousarray(poses, np.float64)
         if geometry is not None:
             n = len(frames[1]) - 1 if isinstance(frames, tuple) else len(frames)
             geometry = self._geometry(geometry, n)
             buf, off = self.pack_frames(frames, geometry)
             o = out or self.alloc_results(n)
+            name = "sfe_frontend_run_host_geometry"
             with self._images(images, n, False, image_lut, self._image_maps(geometry)):
-                _lib.check(self.lib.sfe_frontend_run_host_geometry(
+                packed = self._with_clouds(clouds, n, False, name, lambda: self.lib.sfe_frontend_run_host_geometry(
                     self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(geometry), _lib.ptr(poses), n,
                     int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]),
-                    _lib.ptr(o["status"]), _lib.ptr(o["npoints"])), "sfe_frontend_run_host_geometry")
-            return o
+                    _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
+            return self._packed_into(o, packed)
         frames = np.ascontiguousarray(frames, np.uint8)
         n = len(frames)
         o = out or self.alloc_results(n)
         with self._images(images, n, False, image_lut):
-            _lib.check(self.lib.sfe_frontend_run_host(self.handle, _lib.ptr(frames), _lib.ptr(poses), n,
-                                                      int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                                                      _lib.ptr(o["inliers"]), _lib.ptr(o["status"]),
-                                                      _lib.ptr(o["npoints"])), "sfe_frontend_run_host")
+            packed = self._with_clouds(clouds, n, False, "sfe_frontend_run_host", lambda: self.lib.sfe_frontend_run_host(
+                self.handle, _lib.ptr(frames), _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]),
+                _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
+        return self._packed_into(o, packed)
+
+    @staticmethod
+    def _packed_into(o, packed):
+        if packed is not None:
+            o["clouds"], o["cloud_offsets"] = packed
         return o
 
-    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
+    def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None,
+                      clouds=None):
         """run_host on compressed pings: streams is a sequence of JPEG bytes objects (or (bytes, offsets) from
         jpeg.pack); the compressed bytes are copied and decoded on the device instead of copying raw frames
         (sfe_frontend_run_jpeg_host).  A stream that is rejected or fails to decode raises, naming the frame.
-        images / image_lut / geometry: as run_host (with geometry, every stream must decode to its geometry's
+        images / image_lut / geometry / clouds: as run_host (with geometry, every stream must decode to its geometry's
         R_g x B_g)."""
         return self._run_compressed("sfe_frontend_run_jpeg_host", streams, poses, chunk_frames, out, images, image_lut,
-                                    geometry)
+                                    geometry, clouds)
 
-    def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None):
+    def run_png_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None,
+                     clouds=None):
         """run_jpeg_host for PNG streams (sfe_frontend_run_png_host)."""
         return self._run_compressed("sfe_frontend_run_png_host", streams, poses, chunk_frames, out, images, image_lut,
-                                    geometry)
+                                    geometry, clouds)
 
-    def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut, geometry):
+    def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut, geometry, clouds):
         buf, off = _streams.packed(streams)
         poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
@@ -164,31 +229,35 @@ class FrontEnd:
         if geometry is not None:
             name, head = name + "_geometry", head + (_lib.ptr(geometry),)
         with self._images(images, n, False, image_lut, self._image_maps(geometry)):
-            _lib.check(getattr(self.lib, name)(*head, _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]),
-                                               _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]),
-                                               _lib.ptr(o["status"]), _lib.ptr(o["npoints"])), name)
-        return o
+            packed = self._with_clouds(clouds, n, False, name, lambda: getattr(self.lib, name)(
+                *head, _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
+                _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
+        return self._packed_into(o, packed)
 
     @staticmethod
     def alloc_results(n):
         return dict(T=np.empty((n, 3, 3), np.float32), iterations=np.empty(n, np.int32),
                     inliers=np.empty(n, np.int32), status=np.empty(n, np.int32), npoints=np.empty(n, np.int32))
 
-    def run_dev(self, frames_ptr, poses, n, images=None, image_lut=None, geometry=None):
+    def run_dev(self, frames_ptr, poses, n, images=None, image_lut=None, geometry=None, clouds=None):
         """frames_ptr: device address of uint8 [n,R,B]; poses: float64 [n,3] numpy (host).  Asynchronous.
         images: an optional uint8 [n, rows, cols, 3] CUDA tensor that receives every frame's feature image.
         geometry: one id per frame (add_geometry); frame i of geometry g then occupies the first R_g * B_g bytes of
-        its R * B slot, row-major [R_g, B_g] (sfe_frontend_run_dev_geometry)."""
+        its R * B slot, row-major [R_g, B_g] (sfe_frontend_run_dev_geometry).
+        clouds: True, a capacity or (points, offsets) CUDA tensors (see _with_clouds): every frame's filtered cloud,
+        packed on the device, and the call returns (points [total, 2], offsets [n + 1]) CUDA tensors once the call has
+        finished; without clouds it returns None."""
         poses = np.ascontiguousarray(poses, np.float64)
-        geometry = self._geometry(geometry, int(n))
-        with self._images(images, int(n), True, image_lut, self._image_maps(geometry)):
+        n = int(n)
+        geometry = self._geometry(geometry, n)
+        with self._images(images, n, True, image_lut, self._image_maps(geometry)):
             if geometry is None:
-                _lib.check(self.lib.sfe_frontend_run_dev(self.handle, ctypes.c_void_p(int(frames_ptr)),
-                                                         _lib.ptr(poses), int(n)), "sfe_frontend_run_dev")
-            else:
-                _lib.check(self.lib.sfe_frontend_run_dev_geometry(self.handle, ctypes.c_void_p(int(frames_ptr)),
-                                                                  _lib.ptr(geometry), _lib.ptr(poses), int(n)),
-                           "sfe_frontend_run_dev_geometry")
+                return self._with_clouds(clouds, n, True, "sfe_frontend_run_dev", lambda: self.lib.sfe_frontend_run_dev(
+                    self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(poses), n))
+            return self._with_clouds(clouds, n, True, "sfe_frontend_run_dev_geometry",
+                                     lambda: self.lib.sfe_frontend_run_dev_geometry(
+                                         self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(geometry),
+                                         _lib.ptr(poses), n))
 
     def results_dev(self):
         """Device addresses of the last run's results: dict(T, iterations, inliers, status, cloud_xy,
@@ -212,6 +281,12 @@ class FrontEnd:
         many frames with the scan matching of the previous one on two streams; 0 (the default) runs every stage over
         the whole batch one after another.  The results are the same either way."""
         _lib.check(self.lib.sfe_frontend_set_overlap(self.handle, int(sub_batch_frames)), "sfe_frontend_set_overlap")
+
+    def set_scan_match(self, enable=True):
+        """False: every run flavour stops after the feature stages (sfe_frontend_set_scan_match): no window submaps,
+        no ICP; status SKIPPED (TOO_LARGE where a Cartesian cloud overflowed cap_points), T the identity.  The clouds
+        are the same either way; with carry on the carried window still advances."""
+        _lib.check(self.lib.sfe_frontend_set_scan_match(self.handle, 1 if enable else 0), "sfe_frontend_set_scan_match")
 
     STAGES = ("cfar", "cart_points", "downsample", "remove_outlier", "submap", "icp")
 
