@@ -26,8 +26,9 @@
 extern "C" {
 #endif
 
-#define SFE_VERSION 201 /* round 2: + sfe_fov_select_*, sfe_frontend_set_carry, sfe_frontend_params.flip_lateral, sfe_icp_params.flags bit 1;
-                            201: + sfe_icp_params.minimizer / normals_knn (point-to-plane, icp.yaml:18-19) */
+#define SFE_VERSION 202 /* round 2: + sfe_fov_select_*, sfe_frontend_set_carry, sfe_frontend_params.flip_lateral, sfe_icp_params.flags bit 1;
+                            201: + sfe_icp_params.minimizer / normals_knn (point-to-plane, icp.yaml:18-19);
+                            202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch) */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -391,14 +392,6 @@ SFE_API int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, co
  * exactly as if the batches had been one call -- a replay can be fed in pieces of any size without a cold window at
  * every seam.  enable = 0 (the default) drops the carried frames: every call starts cold (frame 0 SFE_ICP_SKIPPED). */
 SFE_API int sfe_frontend_set_carry(sfe_frontend *fe, int enable);
-/* Schedule of sfe_frontend_run_dev.  sub_batch_frames > 0: the batch is processed in sub-batches
- * of that many frames on two streams of the front end, the feature stages (CFAR, cloud, filters) of one sub-batch
- * running while the submap assembly and ICP of the previous one do; both streams fork from and join back into the
- * context's stream, so the call stays ordered on it like any other.  0 (the default): every stage over the whole batch,
- * one after another on the context's stream.  The results are bit-identical either way.  With per-stage timing on
- * (sfe_frontend_set_timing) run_dev always takes the serial schedule, so that each stage is timed alone.  The host
- * and compressed flavours keep their chunked schedule on the context's stream. */
-SFE_API int sfe_frontend_set_overlap(sfe_frontend *fe, int sub_batch_frames);
 /* Feature images from the front end.  With dst != NULL, every later run call on this handle also writes frame i's
  * feature image (as sfe_feature_image_dev, table lut_bgr_host, copied by this call) to dst + i * rows * cols * 3.
  * sfe_frontend_run_dev needs dst in device memory (dst_is_host = 0; asynchronous like the rest of the call);
@@ -409,7 +402,7 @@ SFE_API int sfe_frontend_set_overlap(sfe_frontend *fe, int sub_batch_frames);
  * results are the same with and without images. */
 SFE_API int sfe_frontend_set_feature_images(sfe_frontend *fe, const uint8_t *lut_bgr_host, uint8_t *dst,
                                             int dst_is_host);
-/* Optional per-stage device timing (CUDA events on the launch stream around every stage's kernels).
+/* Optional per-stage device timing (CUDA events on the context's stream around every stage's kernels).
  * get_timing synchronises, adds the intervals recorded since the last call to running totals and
  * returns the totals: stage_ms[SFE_FE_STAGES], stage_calls[SFE_FE_STAGES] (may be NULL). */
 enum { SFE_FE_CFAR = 0, SFE_FE_CART = 1, SFE_FE_DOWNSAMPLE = 2, SFE_FE_OUTLIER = 3, SFE_FE_SUBMAP = 4,

@@ -115,7 +115,6 @@ _EXTRA_SIGNATURES = {
     "sfe_frontend_create": [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(c_void_p)],
     "sfe_frontend_set_timing": [c_void_p, c_int],
     "sfe_frontend_set_carry": [c_void_p, c_int],
-    "sfe_frontend_set_overlap": [c_void_p, c_int],
     "sfe_frontend_set_clouds": [c_void_p, c_void_p, ctypes.c_int64, c_void_p, c_int],
     "sfe_frontend_set_scan_match": [c_void_p, c_int],
     "sfe_frontend_get_timing": [c_void_p, c_void_p, c_void_p],

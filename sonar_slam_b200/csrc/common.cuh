@@ -38,6 +38,9 @@ struct Buffer {  // grow-only device scratch
   void *ptr = nullptr;
   size_t cap = 0;
 };
+// the slots of sfe_ctx::scratch, one per subsystem
+enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_DS_GRID = 6,
+       SCR_MAP = 7, SCR_RO_MAP = 8, SCR_COUNT = 9 };
 
 struct JpegState;  // jpeg.cu
 struct PngState;   // png.cu
@@ -52,7 +55,7 @@ struct sfe_ctx {
   bool owns_stream = false;
   int sm_count = 0;
   int max_smem_optin = 0;
-  sfe::Buffer scratch[10];  // per-subsystem scratch (see SCR_* below)
+  sfe::Buffer scratch[sfe::SCR_COUNT];  // per-subsystem scratch
   sfe::Buffer stage_in[2];  // device staging for the *_host entry points
   sfe::Buffer stage_out[4];
   void *pinned = nullptr;   // small pinned host block for async result reads
@@ -86,12 +89,9 @@ struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
 };
 
 namespace sfe {
-enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_SUBMAP = 6,
-       SCR_DS_GRID = 7, SCR_MAP = 8, SCR_RO_MAP = 9 };
 // Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
 // different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
-// (WORK_DS_SUBMAP: the window submaps' down-sample runs next to the frames' in the overlapped schedule)
-enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, WORK_DS_SUBMAP = 3, SFE_WORK_COUNTERS = 4 };
+enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, SFE_WORK_COUNTERS = 3 };
 
 // (re)allocate if too small, stream-ordered on `stream` (default: ctx->stream).  A buffer must only grow on a stream
 // that is ordered after every earlier user of the block and before every later one: the stream that uses it.

@@ -48,9 +48,6 @@ constexpr int FE_RO_SPLIT = 1024, FE_SUBMAP_SPLIT = 2048;
 // largest; larger clouds take the capacity launch.  At 6144 points the frame kernel needs 97 KB of dynamic shared
 // memory (16 bytes per point: the sorted points are staged there), so an H100 SM holds 2 of its 512-thread CTAs.
 constexpr int FE_DS_FRAME = 6144;
-// Default schedule of sfe_frontend_run_dev (sfe_frontend_set_overlap): serial.  On an H100 (700 W) the overlapped
-// schedule measured slower at every sub-batch size tried on the config-4 replay (DESIGN.md section 4).
-constexpr int FE_OVERLAP_FRAMES = 0;
 
 // T_ab = pose_a^-1 * pose_b as float32 3x3 (gtsam Pose2::between, then matrix().astype(float32)).
 // Evaluated on the host in double (libm), so the float32 matrices the kernels see are the ones a
@@ -192,7 +189,7 @@ struct sfe_frontend {
   std::vector<GeoRun> runs;
   std::vector<int32_t> frame_shape;
   // device buffers (sized for max_frames)
-  uint8_t *frames = nullptr;      // [max_frames][R][B]      (host flavour only)
+  uint8_t *frames = nullptr;      // [max_frames][R][B]: the host flavours' frames, run_dev_geometry's packed runs
   uint32_t *bits = nullptr;       // [max_frames][R][wpr]
   int32_t *ij = nullptr;          // [max_frames][cap][2]
   float *xy_a = nullptr, *xy_b = nullptr;  // [max_frames][cap][2] ping-pong
@@ -214,11 +211,6 @@ struct sfe_frontend {
   double *carry_poses = nullptr;   // host [window][3]
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_copy[2] = {}, ev_done = nullptr;
-  // overlapped run_dev (sfe_frontend_set_overlap): sub-batch size (0: serial on ctx->stream), the two streams and the
-  // events that fork them from ctx->stream, hand each sub-batch from features to match, and join them back
-  int overlap = 0;
-  cudaStream_t feat_stream = nullptr, match_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_feat = nullptr, ev_join = nullptr;
   // feature images (sfe_frontend_set_feature_images)
   uint8_t img_lut[256 * 3] = {};
   uint8_t *img_dst = nullptr;      // null: off
@@ -237,25 +229,8 @@ struct sfe_frontend {
   int64_t *cloud_off = nullptr, *cloud_off_host = nullptr;  // [max_frames + 1]
   cudaEvent_t ev_cloud[2] = {};
   int scan_match = 1;  // sfe_frontend_set_scan_match
-  StageTimer timer;  // optional per-stage timing, on ctx->stream (the serial schedule)
+  StageTimer timer;  // optional per-stage timing, on ctx->stream
 };
-
-// The streams of the overlapped schedule.  The match side (submap + ICP) is the longer chain, so its CTAs go first
-// when both sides have work ready; SFE_FE_OVERLAP_PRIO=features|equal (development switch, read when a front end is
-// created) gives the feature side the higher priority or neither.
-static cudaError_t fe_create_overlap_streams(sfe_frontend *fe) {
-  int least = 0, greatest = 0;
-  cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
-  const char *sw = getenv("SFE_FE_OVERLAP_PRIO");
-  int p_feat = least, p_match = greatest;
-  if (sw && strcmp(sw, "features") == 0) p_feat = greatest, p_match = least;
-  if (sw && strcmp(sw, "equal") == 0) p_feat = p_match = least;
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&fe->feat_stream, cudaStreamNonBlocking, p_feat);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&fe->match_stream, cudaStreamNonBlocking, p_match);
-  for (cudaEvent_t *ev : {&fe->ev_fork, &fe->ev_feat, &fe->ev_join})
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
-  return e;
-}
 
 extern "C" {
 
@@ -339,7 +314,6 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_copy[0], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_copy[1], cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&fe->ev_done, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = fe_create_overlap_streams(fe);
   if (e != cudaSuccess) {
     sfe::set_error("sfe_frontend_create: %s", cudaGetErrorString(e));
     sfe_frontend_destroy(fe);
@@ -349,7 +323,6 @@ int sfe_frontend_create(sfe_ctx *ctx, const sfe_maps *maps, const sfe_frontend_p
   fill_offsets_kernel<<<(max_frames + 256) / 256, 256, 0, ctx->stream>>>(fe->off_tgt, max_frames, (int)tcap);
   SFE_CUDA(cudaGetLastError());
   ctx->launches += 2;
-  fe->overlap = FE_OVERLAP_FRAMES;
   *out = fe;
   return SFE_OK;
 }
@@ -375,13 +348,6 @@ void sfe_frontend_destroy(sfe_frontend *fe) {
   for (auto &ev : fe->ev_copy)
     if (ev) cudaEventDestroy(ev);
   if (fe->ev_done) cudaEventDestroy(fe->ev_done);
-  for (cudaStream_t st : {fe->feat_stream, fe->match_stream})
-    if (st) {
-      cudaStreamSynchronize(st);
-      cudaStreamDestroy(st);
-    }
-  for (cudaEvent_t ev : {fe->ev_fork, fe->ev_feat, fe->ev_join})
-    if (ev) cudaEventDestroy(ev);
   if (fe->img_stream) {
     cudaStreamSynchronize(fe->img_stream);
     cudaStreamDestroy(fe->img_stream);
@@ -525,8 +491,9 @@ static int fe_for_pieces(const sfe_frontend *fe, int f0, int n,
 static const float *fe_cloud(const sfe_frontend *fe, const int32_t **cnt);
 
 // stages 1-2 on frames [f0, f0+n) of run r: CFAR (bit plane) -> Cartesian points, with the run's geometry
-static int fe_polar(sfe_frontend *fe, cudaStream_t st, const GeoRun &r, int f0, int n) {
+static int fe_polar(sfe_frontend *fe, const GeoRun &r, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
+  cudaStream_t st = ctx->stream;
   const sfe_frontend_params &p = fe->p;
   const sfe_maps *m = fe->geo[r.g];
   const size_t cap = p.cap_points, wpr = (m->B + 31) / 32;
@@ -546,11 +513,12 @@ static int fe_polar(sfe_frontend *fe, cudaStream_t st, const GeoRun &r, int f0, 
 // stages 1-3 on frames [f0, f0+n): CFAR (bit plane) -> Cartesian points once per run of one geometry, then
 // downsample -> outlier removal over all n frames.
 // Final per-frame clouds end in xy_a / cnt_c (or wherever the last enabled filter wrote; see cloud()).
-static int fe_features(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
+static int fe_features(sfe_frontend *fe, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
+  cudaStream_t st = ctx->stream;
   const sfe_frontend_params &p = fe->p;
   const size_t cap = p.cap_points;
-  int rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) { return fe_polar(fe, st, r, a, m); });
+  int rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) { return fe_polar(fe, r, a, m); });
   if (rc != SFE_OK) return rc;
   // feature_extraction.py:241-249
   const float *cur = fe->xy_a;
@@ -599,8 +567,9 @@ static const float *fe_cloud(const sfe_frontend *fe, const int32_t **cnt) {
 }
 
 // stage 4-5 on frames [f0, f0+n): targets from the window of previous frames (which may precede f0), then ICP
-static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
+static int fe_match(sfe_frontend *fe, int f0, int n) {
   sfe_ctx *ctx = fe->ctx;
+  cudaStream_t st = ctx->stream;
   const sfe_frontend_params &p = fe->p;
   const int cap = p.cap_points, tcap = p.window * cap;
   if (!fe->scan_match) {
@@ -620,9 +589,8 @@ static int fe_match(sfe_frontend *fe, cudaStream_t st, int f0, int n) {
   const float *tgt = fe->tgt_a;
   const int32_t *tcnt = fe->tcnt_a;
   if (p.submap_resolution > 0.f) {
-    // (its own workspace and work counter: in the overlapped schedule it runs next to the frame down-sampling)
     int rc = downsample_run(ctx, st, {fe->tgt_a, fe->off_tgt + f0, fe->tcnt_a + f0, tcap}, n, 2, p.submap_resolution,
-                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_SUBMAP, WORK_DS_SUBMAP);
+                            fe->tgt_b, fe->tgt_idx, fe->tcnt_b + f0, FE_SUBMAP_SPLIT, SCR_CLOUD, WORK_DS);
     if (rc != SFE_OK) return rc;
     tgt = fe->tgt_b, tcnt = fe->tcnt_b;
   }
@@ -808,13 +776,6 @@ int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable) {
   return SFE_OK;
 }
 
-int sfe_frontend_set_overlap(sfe_frontend *fe, int sub_batch_frames) {
-  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_overlap: null handle");
-  SFE_REQUIRE(sub_batch_frames >= 0, "sfe_frontend_set_overlap: negative sub-batch size %d", sub_batch_frames);
-  fe->overlap = sub_batch_frames;
-  return SFE_OK;
-}
-
 int sfe_frontend_set_timing(sfe_frontend *fe, int enable) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_timing: null handle");
   fe->timer.reset(enable != 0);
@@ -836,39 +797,6 @@ static int fe_order(cudaStream_t before, cudaEvent_t ev, cudaStream_t after) {
   return SFE_OK;
 }
 
-// The overlapped schedule of run_dev (DESIGN.md section 4): the batch in sub-batches of fe->overlap frames, the
-// feature stages of every sub-batch on feat_stream, submap + ICP of sub-batch k on match_stream once the features of
-// sub-batch k are done -- its window reaches back only into sub-batches <= k.  So the HBM-bound CFAR of sub-batch k+1
-// runs next to the latency-bound ICP of sub-batch k, and each stage's tail is filled by the other side's CTAs.  Both
-// streams fork from ctx->stream (after the pose upload and anything the caller enqueued there) and join back into it,
-// so ctx->stream orders later work -- the next call included -- after the whole batch.  With several geometries a
-// sub-batch runs CFAR and the Cartesian points once per run inside it, the rest once.
-static int fe_run_overlapped(sfe_frontend *fe, int n_frames) {
-  sfe_ctx *ctx = fe->ctx;
-  const int S = fe->overlap;
-  int rc = fe_order(ctx->stream, fe->ev_fork, fe->feat_stream);
-  if (rc == SFE_OK) rc = fe_order(ctx->stream, fe->ev_fork, fe->match_stream);
-  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += S) {
-    const int n = std::min(S, n_frames - f0);
-    rc = fe_features(fe, fe->feat_stream, f0, n);
-    if (rc == SFE_OK) rc = fe_order(fe->feat_stream, fe->ev_feat, fe->match_stream);
-    if (rc == SFE_OK) rc = fe_match(fe, fe->match_stream, f0, n);
-  }
-  // join on every path, so that whatever did get enqueued is ordered before later work on ctx->stream
-  const int rj = fe_order(fe->feat_stream, fe->ev_join, ctx->stream);
-  const int rm = fe_order(fe->match_stream, fe->ev_join, ctx->stream);
-  return rc != SFE_OK ? rc : (rj != SFE_OK ? rj : rm);
-}
-
-// The start of a host flavour after its argument checks, for n_frames > 0: the device, the default chunk size, the
-// feature-image staging (of the call's one geometry) and every run's place in fe->frames.
-static int fe_host_begin(sfe_frontend *fe, int n_frames, int &chunk_frames, const char *what) {
-  SFE_CUDA(cudaSetDevice(fe->ctx->device));
-  if (chunk_frames <= 0) chunk_frames = 256;
-  for (GeoRun &r : fe->runs) r.frames = fe->frames + (size_t)r.f0 * fe->p.R * fe->p.B;
-  return fe_images_begin(fe, fe->geo[fe->runs[0].g], n_frames, chunk_frames, what);
-}
-
 // feature images of chunk [f0, f0 + n) of a host flavour (the call has one run when images are on)
 static int fe_render_host_chunk(sfe_frontend *fe, int f0, int n, int k, const char *what) {
   if (!fe->img_dst) return SFE_OK;
@@ -876,46 +804,140 @@ static int fe_render_host_chunk(sfe_frontend *fe, int f0, int n, int k, const ch
   return fe_render_chunk(fe, fe->geo[r.g], fe_run_frame(fe, r, f0), f0, n, k, what);
 }
 
+// What a host flavour's call returns in host memory (npoints may be null)
+struct HostResults {
+  float *T;
+  int32_t *iters, *inliers, *status, *npoints;
+};
+
 // The end of a host flavour: the last chunk's clouds go out (a call whose clouds overflow stops here, its carried window
 // as it was), the carried window moves on, the results go to the host and the call waits for them.
 static int fe_host_finish(sfe_frontend *fe, const CloudChunk &last, const double *poses_host, int n_frames,
-                          float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
-                          int32_t *npoints_host, const char *what) {
+                          const HostResults &out, const char *what) {
   sfe_ctx *ctx = fe->ctx;
   int rc = fe_clouds_out(fe, last);
   if (rc == SFE_OK) rc = fe_clouds_finish(fe, n_frames, what);
   if (rc == SFE_OK) rc = fe_update_carry(fe, ctx->stream, poses_host, n_frames);
   if (rc != SFE_OK) return rc;
-  SFE_CUDA(cudaMemcpyAsync(T_host, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(iters_host, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(inliers_host, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  SFE_CUDA(cudaMemcpyAsync(status_host, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
-  if (npoints_host) {
+  SFE_CUDA(cudaMemcpyAsync(out.T, fe->T, sizeof(float) * 9 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(out.iters, fe->iters, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(out.inliers, fe->inliers, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  SFE_CUDA(cudaMemcpyAsync(out.status, fe->status, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+  if (out.npoints) {
     const int32_t *cnt;
     fe_cloud(fe, &cnt);
-    SFE_CUDA(cudaMemcpyAsync(npoints_host, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(out.npoints, cnt, 4 * (size_t)n_frames, cudaMemcpyDeviceToHost, ctx->stream));
   }
   SFE_CUDA(cudaStreamSynchronize(ctx->stream));
   return SFE_OK;
 }
 
-// The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
-// fe->frames.  Chunk k+1 is decoded (its bytes on the copy stream) before the host waits for chunk k's decode status,
-// so the wait overlaps device work; the front-end stages of a chunk are enqueued only once its frames decoded.
-// geometry: one id per frame, or null (every frame geometry 0, R x B).
-static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sfe_ctx *), const uint8_t *bytes,
-                                  const int64_t *offsets, const int32_t *geometry, const double *poses_host,
-                                  int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
-                                  int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host,
-                                  const char *what) {
-  SFE_REQUIRE(fe && bytes && offsets && poses_host && T_host && iters_host && inliers_host && status_host,
-              "%s: null argument", what);
+// The checks every host flavour makes first, before its own and before any device work: null arguments (inputs_ok:
+// those of the flavour's frame inputs), the frame count, the clouds' destination and the geometry runs.
+static int fe_host_args(sfe_frontend *fe, bool inputs_ok, const int32_t *geometry, const double *poses_host,
+                        int n_frames, const HostResults &out, const char *what) {
+  SFE_REQUIRE(fe && inputs_ok && poses_host && out.T && out.iters && out.inliers && out.status, "%s: null argument",
+              what);
   SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
               fe->max_frames);
-  SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
   int rc = fe_clouds_args(fe, true, what);
   if (rc == SFE_OK) rc = fe_geometry_runs(fe, geometry, n_frames, what);
-  if (rc != SFE_OK || n_frames == 0) return rc;
+  return rc;
+}
+
+// How a host flavour's frames get into their slots of fe->frames.  begin(chunk_frames) runs once the call has its
+// device, chunk size and image staging, before the pose upload: the flavour's last checks and its set-up.
+// stage(f0, n, k), if set, enqueues chunk k = frames [f0, f0 + n) into its slots one chunk ahead; ready(f0, n, k)
+// makes chunk k usable on ctx->stream.
+struct HostFrames {
+  std::function<int(int)> begin;
+  std::function<int(int, int, int)> stage, ready;
+};
+
+// The chunk loop of every host flavour.  A flavour that stages ahead has chunk k+1 staged before chunk k is waited for,
+// so its decode runs next to the kernels of chunk k.  Once chunk k is ready its feature images, feature stages, clouds
+// and scan match are enqueued (its window reaches back only into chunks already processed), and the clouds of chunk
+// k-1 go out.
+static int fe_run_host(sfe_frontend *fe, const HostFrames &in, const double *poses_host, int n_frames,
+                       int chunk_frames, const HostResults &out, const char *what) {
+  if (n_frames == 0) return SFE_OK;
+  // the device, the default chunk size, every run's place in fe->frames, the feature-image staging (of the call's one
+  // geometry)
+  SFE_CUDA(cudaSetDevice(fe->ctx->device));
+  if (chunk_frames <= 0) chunk_frames = 256;
+  for (GeoRun &r : fe->runs) r.frames = fe->frames + (size_t)r.f0 * fe->p.R * fe->p.B;
+  int rc = fe_images_begin(fe, fe->geo[fe->runs[0].g], n_frames, chunk_frames, what);
+  if (rc != SFE_OK) return rc;
+  CopiesDrained drained{fe};
+  rc = in.begin(chunk_frames);
+  if (rc == SFE_OK) rc = fe_upload_poses(fe, poses_host, n_frames);
+  if (rc == SFE_OK && in.stage) rc = in.stage(0, std::min(chunk_frames, n_frames), 0);
+  int k = 0;
+  CloudChunk prev;
+  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
+    const int n = std::min(chunk_frames, n_frames - f0), next = f0 + chunk_frames;
+    if (in.stage && next < n_frames) rc = in.stage(next, std::min(chunk_frames, n_frames - next), k + 1);
+    if (rc == SFE_OK) rc = in.ready(f0, n, k);
+    if (rc == SFE_OK) rc = fe_render_host_chunk(fe, f0, n, k, what);
+    if (rc == SFE_OK) rc = fe_features(fe, f0, n);
+    if (rc == SFE_OK) rc = fe_clouds_chunk(fe, f0, n, k);
+    if (rc == SFE_OK) rc = fe_match(fe, f0, n);
+    if (rc == SFE_OK) rc = fe_clouds_out(fe, prev);
+    prev = {f0, n, k};
+  }
+  if (rc != SFE_OK) return rc;
+  return fe_host_finish(fe, prev, poses_host, n_frames, out, what);
+}
+
+// sfe_frontend_run_host[_geometry]: frame i at bytes + offsets[i] with its geometry's size (offsets and geometry null:
+// bytes + i * R * B, geometry 0).  Chunks of frames stream in on the copy stream, run by run into their places in
+// fe->frames, while the kernels of the chunk before run.
+static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const int32_t *geometry,
+                           const double *poses_host, int n_frames, int chunk_frames, const HostResults &out,
+                           const char *what) {
+  int rc = fe_host_args(fe, bytes && (!geometry || offsets), geometry, poses_host, n_frames, out, what);
+  if (rc != SFE_OK) return rc;
+  if (offsets) {
+    SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
+    for (int i = 0; i < n_frames; ++i) {
+      const sfe_maps *m = fe->geo[geometry[i]];
+      SFE_REQUIRE(offsets[i + 1] - offsets[i] == (int64_t)m->R * m->B, "%s: frame %d has %lld bytes; its geometry %d "
+                  "takes %d x %d = %lld", what, i, (long long)(offsets[i + 1] - offsets[i]), geometry[i], m->R, m->B,
+                  (long long)m->R * m->B);
+    }
+  }
+  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
+  HostFrames in;
+  // the copies into fe->frames come after earlier work on ctx->stream that may still read it (the frames
+  // sfe_frontend_run_dev_geometry packs there)
+  in.begin = [&](int) { return fe_order(fe->ctx->stream, fe->ev_done, fe->copy_stream); };
+  // No stage ahead: chunk k is copied only once the kernels of chunk k-1 are enqueued.  A copy from pageable host
+  // memory returns only when its bytes are staged, so a copy issued a chunk ahead would hold back those kernels.
+  in.ready = [&](int f0, int n, int k) -> int {
+    const int r = fe_for_pieces(fe, f0, n, [&](const GeoRun &run, int a, int m) {
+      const size_t src = offsets ? (size_t)offsets[a] : (size_t)a * fbytes;
+      const size_t len = offsets ? (size_t)(offsets[a + m] - offsets[a]) : (size_t)m * fbytes;
+      SFE_CUDA(cudaMemcpyAsync(fe_slot_frame(fe, run, a), bytes + src, len, cudaMemcpyHostToDevice, fe->copy_stream));
+      return SFE_OK;
+    });
+    if (r != SFE_OK) return r;
+    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
+    SFE_CUDA(cudaStreamWaitEvent(fe->ctx->stream, fe->ev_copy[k & 1], 0));
+    return SFE_OK;
+  };
+  return fe_run_host(fe, in, poses_host, n_frames, chunk_frames, out, what);
+}
+
+// The raw-frame copy of sfe_frontend_run_host replaced by the copy of the compressed bytes and the decode into
+// fe->frames.  The host waits for chunk k's decode status once chunk k+1 is decoding, so the wait overlaps device work;
+// the front-end stages of a chunk are enqueued only once its frames decoded.  geometry: one id per frame, or null
+// (every frame geometry 0, R x B).
+static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sfe_ctx *), const uint8_t *bytes,
+                                  const int64_t *offsets, const int32_t *geometry, const double *poses_host,
+                                  int n_frames, int chunk_frames, const HostResults &out, const char *what) {
+  int rc = fe_host_args(fe, bytes && offsets, geometry, poses_host, n_frames, out, what);
+  if (rc != SFE_OK) return rc;
+  SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
   const int32_t *shape = nullptr;  // each frame's R x B, checked by the decoder
   if (geometry) {
     fe->frame_shape.resize(2 * (size_t)n_frames);
@@ -923,12 +945,10 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
       fe->frame_shape[2 * i] = fe->geo[geometry[i]]->R, fe->frame_shape[2 * i + 1] = fe->geo[geometry[i]]->B;
     shape = fe->frame_shape.data();
   }
-  rc = fe_host_begin(fe, n_frames, chunk_frames, what);
-  if (rc != SFE_OK) return rc;
-  CopiesDrained drained{fe};
   sfe_ctx *ctx = fe->ctx;
-  StreamDecoder *dec = decoder(ctx);
-  dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, shape);
+  StreamDecoder *dec = nullptr;
+  int32_t *st_host = nullptr;       // each frame's decode status, read back chunk by chunk
+  const int32_t *st_dev = nullptr;
   auto reject = [&](int i, int status) {
     if (geometry)
       set_error("%s: frame %d (geometry %d, %d x %d): %s", what, i, geometry[i], shape[2 * i], shape[2 * i + 1],
@@ -937,19 +957,22 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
       set_error("%s: frame %d: %s", what, i, dec->message(status));
     return SFE_ERR_ARG;
   };
-  for (int i = 0; i < n_frames; ++i)
-    if (dec->frame_status(i) != 0) return reject(i, dec->frame_status(i));
-  rc = dec->reserve(ctx, chunk_frames, 0);
-  if (rc == SFE_OK) rc = ensure_pinned(ctx, 4 * (size_t)n_frames);
-  if (rc == SFE_OK) rc = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  int32_t *st_host = static_cast<int32_t *>(ctx->pinned);
-  const int32_t *st_dev = static_cast<const int32_t *>(dec->status.ptr);
-  auto decode = [&](int f0, int k) -> int {
-    const int n = std::min(chunk_frames, n_frames - f0);
+  HostFrames in;
+  in.begin = [&](int chunk_frames) -> int {
+    dec = decoder(ctx);
+    dec->parse(bytes, offsets, n_frames, fe->p.R, fe->p.B, shape);
+    for (int i = 0; i < n_frames; ++i)
+      if (dec->frame_status(i) != 0) return reject(i, dec->frame_status(i));
+    int r = dec->reserve(ctx, chunk_frames, 0);
+    if (r == SFE_OK) r = ensure_pinned(ctx, 4 * (size_t)n_frames);
+    st_host = static_cast<int32_t *>(ctx->pinned);
+    st_dev = static_cast<const int32_t *>(dec->status.ptr);
+    return r;
+  };
+  in.stage = [&](int f0, int n, int k) -> int {
     // a decode_chunk takes frames of one shape: a chunk that crosses a geometry change decodes run by run, each part
     // into its place in its run (every part is a subset of the chunk, which reserve() sized the decoder for)
-    int r = fe_for_pieces(fe, f0, n, [&](const GeoRun &run, int a, int m) {
+    const int r = fe_for_pieces(fe, f0, n, [&](const GeoRun &run, int a, int m) {
       return dec->decode_chunk(ctx, a, m, fe_slot_frame(fe, run, a));
     });
     if (r != SFE_OK) return r;
@@ -957,29 +980,16 @@ static int fe_run_compressed_host(sfe_frontend *fe, StreamDecoder *(*decoder)(sf
     SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], ctx->stream));
     return SFE_OK;
   };
-  rc = decode(0, 0);
-  int k = 0;
-  CloudChunk prev;
-  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
-    const int n = std::min(chunk_frames, n_frames - f0);
-    if (f0 + chunk_frames < n_frames) rc = decode(f0 + chunk_frames, k + 1);
-    if (rc != SFE_OK) break;
+  in.ready = [&](int f0, int n, int k) -> int {
     SFE_CUDA(cudaEventSynchronize(fe->ev_copy[k & 1]));
     for (int i = f0; i < f0 + n; ++i)
       if (st_host[i] != 0) {
         SFE_CUDA(cudaStreamSynchronize(ctx->stream));
         return reject(i, st_host[i]);
       }
-    rc = fe_render_host_chunk(fe, f0, n, k, what);
-    if (rc == SFE_OK) rc = fe_features(fe, ctx->stream, f0, n);
-    if (rc == SFE_OK) rc = fe_clouds_chunk(fe, f0, n, k);
-    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, f0, n);
-    if (rc == SFE_OK) rc = fe_clouds_out(fe, prev);
-    prev = {f0, n, k};
-  }
-  if (rc != SFE_OK) return rc;
-  return fe_host_finish(fe, prev, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host,
-                        what);
+    return SFE_OK;
+  };
+  return fe_run_host(fe, in, poses_host, n_frames, chunk_frames, out, what);
 }
 
 // sfe_frontend_run_dev[_geometry]; geometry: one id per frame, or null (every frame geometry 0)
@@ -1013,77 +1023,12 @@ static int fe_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const int32_t
     rc = feature_image_run(ctx, ctx->stream, fe->geo[r.g], r.frames, n_frames, fe->img_lut, fe->img_dst, what);
     if (rc != SFE_OK) return rc;
   }
-  // per-stage timing records its events on ctx->stream and times every stage alone: serial schedule
-  if (fe->overlap > 0 && !fe->timer.on) {
-    rc = fe_run_overlapped(fe, n_frames);
-  } else {
-    rc = fe_features(fe, ctx->stream, 0, n_frames);
-    if (rc == SFE_OK) rc = fe_match(fe, ctx->stream, 0, n_frames);
-  }
+  rc = fe_features(fe, 0, n_frames);
+  if (rc == SFE_OK) rc = fe_match(fe, 0, n_frames);
   // a call whose clouds overflow leaves the carried window as it was
   if (rc == SFE_OK) rc = fe_clouds_dev(fe, n_frames, what);
   if (rc != SFE_OK) return rc;
   return fe_update_carry(fe, ctx->stream, poses_host, n_frames);
-}
-
-// sfe_frontend_run_host[_geometry]: frame i at bytes + offsets[i] with its geometry's size (offsets and geometry null:
-// bytes + i * R * B, geometry 0).  Chunks of frames stream in on the copy stream, run by run into their places in
-// fe->frames; the feature stages of chunk k run while chunk k+1 copies.
-static int fe_run_raw_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const int32_t *geometry,
-                           const double *poses_host, int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
-                           int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host, const char *what) {
-  SFE_REQUIRE(fe && bytes && poses_host && T_host && iters_host && inliers_host && status_host && (!geometry || offsets),
-              "%s: null argument", what);
-  SFE_REQUIRE(n_frames >= 0 && n_frames <= fe->max_frames, "%s: %d frames exceed max_frames %d", what, n_frames,
-              fe->max_frames);
-  int rc = fe_clouds_args(fe, true, what);
-  if (rc == SFE_OK) rc = fe_geometry_runs(fe, geometry, n_frames, what);
-  if (rc != SFE_OK) return rc;
-  if (offsets) {
-    SFE_REQUIRE(offsets_ok(offsets, n_frames), "%s: offsets must be non-decreasing", what);
-    for (int i = 0; i < n_frames; ++i) {
-      const sfe_maps *m = fe->geo[geometry[i]];
-      SFE_REQUIRE(offsets[i + 1] - offsets[i] == (int64_t)m->R * m->B, "%s: frame %d has %lld bytes; its geometry %d "
-                  "takes %d x %d = %lld", what, i, (long long)(offsets[i + 1] - offsets[i]), geometry[i], m->R, m->B,
-                  (long long)m->R * m->B);
-    }
-  }
-  if (n_frames == 0) return SFE_OK;
-  rc = fe_host_begin(fe, n_frames, chunk_frames, what);
-  if (rc != SFE_OK) return rc;
-  CopiesDrained drained{fe};
-  rc = fe_upload_poses(fe, poses_host, n_frames);
-  if (rc != SFE_OK) return rc;
-  sfe_ctx *ctx = fe->ctx;
-  const size_t fbytes = (size_t)fe->p.R * fe->p.B;
-  // the copies into fe->frames come after earlier work on ctx->stream that may still read it (the frames
-  // sfe_frontend_run_dev_geometry packs there)
-  rc = fe_order(ctx->stream, fe->ev_done, fe->copy_stream);
-  int k = 0;
-  CloudChunk prev;
-  for (int f0 = 0; rc == SFE_OK && f0 < n_frames; f0 += chunk_frames, ++k) {
-    const int n = std::min(chunk_frames, n_frames - f0);
-    rc = fe_for_pieces(fe, f0, n, [&](const GeoRun &r, int a, int m) {
-      const size_t src = offsets ? (size_t)offsets[a] : (size_t)a * fbytes;
-      const size_t len = offsets ? (size_t)(offsets[a + m] - offsets[a]) : (size_t)m * fbytes;
-      SFE_CUDA(cudaMemcpyAsync(fe_slot_frame(fe, r, a), bytes + src, len, cudaMemcpyHostToDevice, fe->copy_stream));
-      return SFE_OK;
-    });
-    if (rc != SFE_OK) return rc;
-    SFE_CUDA(cudaEventRecord(fe->ev_copy[k & 1], fe->copy_stream));
-    SFE_CUDA(cudaStreamWaitEvent(ctx->stream, fe->ev_copy[k & 1], 0));
-    rc = fe_render_host_chunk(fe, f0, n, k, what);
-    if (rc != SFE_OK) return rc;
-    rc = fe_features(fe, ctx->stream, f0, n);
-    if (rc == SFE_OK) rc = fe_clouds_chunk(fe, f0, n, k);
-    if (rc != SFE_OK) return rc;
-    rc = fe_match(fe, ctx->stream, f0, n);  // its window only reaches back into chunks already processed
-    if (rc == SFE_OK) rc = fe_clouds_out(fe, prev);
-    prev = {f0, n, k};
-  }
-  if (rc != SFE_OK) return rc;
-  return fe_host_finish(fe, prev, poses_host, n_frames, T_host, iters_host, inliers_host, status_host, npoints_host,
-                        what);
 }
 
 extern "C" {
@@ -1128,8 +1073,8 @@ int sfe_frontend_results_dev(const sfe_frontend *fe, const float **T, const int3
 int sfe_frontend_run_host(sfe_frontend *fe, const uint8_t *frames_host, const double *poses_host, int n_frames,
                           int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                           int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_raw_host(fe, frames_host, nullptr, nullptr, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                         inliers_host, status_host, npoints_host, "sfe_frontend_run_host");
+  return fe_run_raw_host(fe, frames_host, nullptr, nullptr, poses_host, n_frames, chunk_frames,
+                         {T_host, iters_host, inliers_host, status_host, npoints_host}, "sfe_frontend_run_host");
 }
 
 int sfe_frontend_run_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
@@ -1137,22 +1082,25 @@ int sfe_frontend_run_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const
                                    float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host,
                                    int32_t *npoints_host) {
   SFE_REQUIRE(offsets && geometry, "sfe_frontend_run_host_geometry: null offsets / geometry");
-  return fe_run_raw_host(fe, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host, iters_host,
-                         inliers_host, status_host, npoints_host, "sfe_frontend_run_host_geometry");
+  return fe_run_raw_host(fe, bytes, offsets, geometry, poses_host, n_frames, chunk_frames,
+                         {T_host, iters_host, inliers_host, status_host, npoints_host},
+                         "sfe_frontend_run_host_geometry");
 }
 
 int sfe_frontend_run_jpeg_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                                int n_frames, int chunk_frames, float *T_host, int32_t *iters_host,
                                int32_t *inliers_host, int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames, T_host,
-                                iters_host, inliers_host, status_host, npoints_host, "sfe_frontend_run_jpeg_host");
+  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames,
+                                {T_host, iters_host, inliers_host, status_host, npoints_host},
+                                "sfe_frontend_run_jpeg_host");
 }
 
 int sfe_frontend_run_png_host(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets, const double *poses_host,
                               int n_frames, int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                               int32_t *status_host, int32_t *npoints_host) {
-  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames, T_host,
-                                iters_host, inliers_host, status_host, npoints_host, "sfe_frontend_run_png_host");
+  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, nullptr, poses_host, n_frames, chunk_frames,
+                                {T_host, iters_host, inliers_host, status_host, npoints_host},
+                                "sfe_frontend_run_png_host");
 }
 
 int sfe_frontend_run_jpeg_host_geometry(sfe_frontend *fe, const uint8_t *bytes, const int64_t *offsets,
@@ -1160,8 +1108,8 @@ int sfe_frontend_run_jpeg_host_geometry(sfe_frontend *fe, const uint8_t *bytes, 
                                         int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                                         int32_t *status_host, int32_t *npoints_host) {
   SFE_REQUIRE(geometry != nullptr, "sfe_frontend_run_jpeg_host_geometry: null geometry");
-  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host,
-                                iters_host, inliers_host, status_host, npoints_host,
+  return fe_run_compressed_host(fe, jpeg_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames,
+                                {T_host, iters_host, inliers_host, status_host, npoints_host},
                                 "sfe_frontend_run_jpeg_host_geometry");
 }
 
@@ -1170,8 +1118,8 @@ int sfe_frontend_run_png_host_geometry(sfe_frontend *fe, const uint8_t *bytes, c
                                        int chunk_frames, float *T_host, int32_t *iters_host, int32_t *inliers_host,
                                        int32_t *status_host, int32_t *npoints_host) {
   SFE_REQUIRE(geometry != nullptr, "sfe_frontend_run_png_host_geometry: null geometry");
-  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames, T_host,
-                                iters_host, inliers_host, status_host, npoints_host,
+  return fe_run_compressed_host(fe, png_decoder, bytes, offsets, geometry, poses_host, n_frames, chunk_frames,
+                                {T_host, iters_host, inliers_host, status_host, npoints_host},
                                 "sfe_frontend_run_png_host_geometry");
 }
 

@@ -175,33 +175,17 @@ class FrontEnd:
         clouds: True or a capacity in points (see _with_clouds) adds every frame's filtered cloud, packed: "clouds"
         float32 [total, 2] and "cloud_offsets" int64 [n + 1], frame i = clouds[cloud_offsets[i]:cloud_offsets[i + 1]]
         in the flip_lateral convention; the other results are the same with and without them."""
-        poses = np.ascontiguousarray(poses, np.float64)
-        if geometry is not None:
+        if geometry is None:
+            frames = np.ascontiguousarray(frames, np.uint8)
+            n = len(frames)
+            head = (_lib.ptr(frames),)
+        else:
             n = len(frames[1]) - 1 if isinstance(frames, tuple) else len(frames)
             geometry = self._geometry(geometry, n)
             buf, off = self.pack_frames(frames, geometry)
-            o = out or self.alloc_results(n)
-            name = "sfe_frontend_run_host_geometry"
-            with self._images(images, n, False, image_lut, self._image_maps(geometry)):
-                packed = self._with_clouds(clouds, n, False, name, lambda: self.lib.sfe_frontend_run_host_geometry(
-                    self.handle, _lib.ptr(buf), _lib.ptr(off), _lib.ptr(geometry), _lib.ptr(poses), n,
-                    int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]),
-                    _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
-            return self._packed_into(o, packed)
-        frames = np.ascontiguousarray(frames, np.uint8)
-        n = len(frames)
-        o = out or self.alloc_results(n)
-        with self._images(images, n, False, image_lut):
-            packed = self._with_clouds(clouds, n, False, "sfe_frontend_run_host", lambda: self.lib.sfe_frontend_run_host(
-                self.handle, _lib.ptr(frames), _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]),
-                _lib.ptr(o["iterations"]), _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
-        return self._packed_into(o, packed)
-
-    @staticmethod
-    def _packed_into(o, packed):
-        if packed is not None:
-            o["clouds"], o["cloud_offsets"] = packed
-        return o
+            head = (_lib.ptr(buf), _lib.ptr(off))
+        return self._run_host("sfe_frontend_run_host", head, poses, n, chunk_frames, out, images, image_lut, geometry,
+                              clouds)
 
     def run_jpeg_host(self, streams, poses, chunk_frames=256, out=None, images=None, image_lut=None, geometry=None,
                       clouds=None):
@@ -221,18 +205,30 @@ class FrontEnd:
 
     def _run_compressed(self, name, streams, poses, chunk_frames, out, images, image_lut, geometry, clouds):
         buf, off = _streams.packed(streams)
-        poses = np.ascontiguousarray(poses, np.float64)
         n = len(off) - 1
-        geometry = self._geometry(geometry, n)
+        return self._run_host(name, (_lib.ptr(buf), _lib.ptr(off)), poses, n, chunk_frames, out, images, image_lut,
+                              self._geometry(geometry, n), clouds)
+
+    def _run_host(self, name, head, poses, n, chunk_frames, out, images, image_lut, geometry, clouds):
+        """A host flavour's call (see _run) into `out` or new result arrays, with the packed clouds added."""
         o = out or self.alloc_results(n)
-        head = (self.handle, _lib.ptr(buf), _lib.ptr(off))
+        tail = (int(chunk_frames),) + tuple(_lib.ptr(o[k]) for k in ("T", "iterations", "inliers", "status", "npoints"))
+        packed = self._run(name, head, poses, n, geometry, False, images, image_lut, clouds, tail)
+        if packed is not None:
+            o["clouds"], o["cloud_offsets"] = packed
+        return o
+
+    def _run(self, name, head, poses, n, geometry, on_device, images, image_lut, clouds, tail=()):
+        """One run call: entry point `name` (its _geometry form when geometry is given) with the leading arguments
+        `head`, then the geometry, poses, n and `tail`; the call's feature images and packed clouds around it (the
+        latter returned, see _with_clouds)."""
+        poses = np.ascontiguousarray(poses, np.float64)
+        head = (self.handle,) + head
         if geometry is not None:
             name, head = name + "_geometry", head + (_lib.ptr(geometry),)
-        with self._images(images, n, False, image_lut, self._image_maps(geometry)):
-            packed = self._with_clouds(clouds, n, False, name, lambda: getattr(self.lib, name)(
-                *head, _lib.ptr(poses), n, int(chunk_frames), _lib.ptr(o["T"]), _lib.ptr(o["iterations"]),
-                _lib.ptr(o["inliers"]), _lib.ptr(o["status"]), _lib.ptr(o["npoints"])))
-        return self._packed_into(o, packed)
+        with self._images(images, n, on_device, image_lut, self._image_maps(geometry)):
+            return self._with_clouds(clouds, n, on_device, name,
+                                     lambda: getattr(self.lib, name)(*head, _lib.ptr(poses), n, *tail))
 
     @staticmethod
     def alloc_results(n):
@@ -247,17 +243,9 @@ class FrontEnd:
         clouds: True, a capacity or (points, offsets) CUDA tensors (see _with_clouds): every frame's filtered cloud,
         packed on the device, and the call returns (points [total, 2], offsets [n + 1]) CUDA tensors once the call has
         finished; without clouds it returns None."""
-        poses = np.ascontiguousarray(poses, np.float64)
         n = int(n)
-        geometry = self._geometry(geometry, n)
-        with self._images(images, n, True, image_lut, self._image_maps(geometry)):
-            if geometry is None:
-                return self._with_clouds(clouds, n, True, "sfe_frontend_run_dev", lambda: self.lib.sfe_frontend_run_dev(
-                    self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(poses), n))
-            return self._with_clouds(clouds, n, True, "sfe_frontend_run_dev_geometry",
-                                     lambda: self.lib.sfe_frontend_run_dev_geometry(
-                                         self.handle, ctypes.c_void_p(int(frames_ptr)), _lib.ptr(geometry),
-                                         _lib.ptr(poses), n))
+        return self._run("sfe_frontend_run_dev", (ctypes.c_void_p(int(frames_ptr)),), poses, n,
+                         self._geometry(geometry, n), True, images, image_lut, clouds)
 
     def results_dev(self):
         """Device addresses of the last run's results: dict(T, iterations, inliers, status, cloud_xy,
@@ -275,12 +263,6 @@ class FrontEnd:
         """Continue the frame sequence across calls: the last `window` clouds and poses stay on the device and serve
         as the window of the next call's first frames (sfe_frontend_set_carry).  False: every call starts cold."""
         _lib.check(self.lib.sfe_frontend_set_carry(self.handle, 1 if enable else 0), "sfe_frontend_set_carry")
-
-    def set_overlap(self, sub_batch_frames):
-        """Schedule of run_dev (sfe_frontend_set_overlap): > 0 overlaps the feature stages of one sub-batch of that
-        many frames with the scan matching of the previous one on two streams; 0 (the default) runs every stage over
-        the whole batch one after another.  The results are the same either way."""
-        _lib.check(self.lib.sfe_frontend_set_overlap(self.handle, int(sub_batch_frames)), "sfe_frontend_set_overlap")
 
     def set_scan_match(self, enable=True):
         """False: every run flavour stops after the feature stages (sfe_frontend_set_scan_match): no window submaps,

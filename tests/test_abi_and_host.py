@@ -15,14 +15,14 @@ def _declared_symbols():
     return sorted(set(re.findall(r"SFE_API[^;(]*?\b(sfe_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_and_its_version():
     from sonar_slam_b200 import _lib
     lib = _lib.load()
     names = _declared_symbols()
     assert len(names) >= 8
     for n in names:
         assert hasattr(lib, n), f"libsonarfe.so does not export {n}"
-    assert lib.sfe_version() == 201
+    assert lib.sfe_version() == 202
 
 
 def test_no_cpu_fallback_context_creation_fails_loudly_without_gpu():

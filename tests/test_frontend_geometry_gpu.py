@@ -123,13 +123,10 @@ def test_host_flavour_equals_oracle_chain(reference):
     assert reference["status"][0] == 7
 
 
-def test_device_flavour_serial_and_overlapped(gpu_ctx, bag, reference):
+def test_device_flavour(gpu_ctx, bag, reference):
     fe = _front_end(gpu_ctx, bag)
-    slots = _slots(bag["frames"])
-    for sub_batch in (0, 1, 5, 16):
-        fe.set_overlap(sub_batch)
-        fe.run_dev(slots.data_ptr(), bag["poses"], N, geometry=GEOMETRY)
-        _assert_same(_device_results(gpu_ctx, fe, N), reference, ("run_dev", sub_batch))
+    fe.run_dev(_slots(bag["frames"]).data_ptr(), bag["poses"], N, geometry=GEOMETRY)
+    _assert_same(_device_results(gpu_ctx, fe, N), reference, "run_dev")
 
 
 @pytest.mark.parametrize("chunk", [1, 5, 64])

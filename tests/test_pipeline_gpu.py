@@ -209,3 +209,34 @@ def test_carried_window_stitches_batches(gpu_ctx):
     cold = fe.run_host(frames[12:26], poses[12:26], chunk_frames=8)
     assert cold["status"][0] == 7 and np.array_equal(cold["T"][3:], whole["T"][15:26])
     assert not np.array_equal(cold["T"][1], whole["T"][13])   # a two-frame window instead of three
+
+
+def test_carried_run_dev_calls_back_to_back(gpu_ctx):
+    """Three run_dev calls with the window carried across them, enqueued without a host sync in between: the next
+    call's pose upload (double-buffered pinned staging) and feature stages must not overtake the previous call's scan
+    match or carry copies.  The pieces shrink, so afterwards the result slots hold frames of all three calls -- slot i
+    frame 230 + i, 140 + i or i -- each as one run_host call over the whole sequence computes it."""
+    n, pieces = 270, [(0, 140), (140, 230), (230, 270)]
+    d = synth.make_trajectory_frames(n, seed=4)
+    frames, poses = d["frames"].numpy(), d["poses_odom"]
+    geo = featx_ref.Geometry(30.0 / 512, 512, d["bearings"])
+    maps = _lib.Maps(gpu_ctx, geo.map_x, geo.map_y, 512, 512, geo.width, geo.height)
+    whole = pipeline.FrontEnd(gpu_ctx, maps, max_frames=n, min_points=30).run_host(frames, poses, clouds=True)
+    fe = pipeline.FrontEnd(gpu_ctx, maps, max_frames=n, min_points=30)
+    fe.set_carry(True)
+    dev = torch.from_numpy(frames).cuda()
+    for a, b in pieces:
+        fe.run_dev(dev[a:].data_ptr(), poses[a:b], b - a)
+    m = pieces[0][1]
+    frame = np.concatenate([np.arange(230, 270), np.arange(180, 230), np.arange(90, 140)])
+    r = fe.results_dev()
+    assert np.array_equal(gpu_ctx.to_host(r["T"], (m, 9), np.float32).view(np.uint32),
+                          whole["T"].reshape(n, 9)[frame].view(np.uint32))
+    for k in ("iterations", "inliers", "status"):
+        assert np.array_equal(gpu_ctx.to_host(r[k], (m,), np.int32), whole[k][frame]), k
+    assert np.array_equal(gpu_ctx.to_host(r["cloud_count"], (m,), np.int32), whole["npoints"][frame])
+    xy = gpu_ctx.to_host(r["cloud_xy"], (m, r["cloud_stride"], 2), np.float32).view(np.uint32)
+    off = whole["cloud_offsets"]
+    for i, f in enumerate(frame):
+        assert np.array_equal(xy[i, :off[f + 1] - off[f]], whole["clouds"][off[f]:off[f + 1]].view(np.uint32)), i
+    assert whole["status"][230] != 7 and (whole["status"] == 0).sum() >= n // 2   # a carried window; matches
