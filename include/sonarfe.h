@@ -303,6 +303,36 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
                                const int32_t *tgt_id_host, int n_problems, const float *guess_host, float *T_host,
                                int32_t *iters_host, int32_t *inliers_host, int32_t *status_host);
 
+/* More of libpointmatcher's ICP modules than sfe_icp_params carries: distance data filters on the reading (source) and
+ * reference (target) clouds, and the MinDist / MedianDist outlier filters.
+ *   data filters   applied once per problem before the iterations, in the listed order; the survivors keep their
+ *                  input order.  Reading filters see the source in its input frame (before the guess), reference
+ *                  filters the target in its input frame (before centring: mean, grid and normals come from the
+ *                  survivors).  SFE_ICP_DATA_MAX_DIST {dim, dist}: dim -1 keeps sqrtf(x*x + y*y) < |dist|, dim 0 / 1
+ *                  keeps coordinate < dist; SFE_ICP_DATA_MIN_DIST the mirror (> |dist|, coordinate > dist).  A target
+ *                  the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
+ *                  SFE_ICP_NO_OUTLIER with a quantile filter (trim_ratio or median_factor) on, else SFE_ICP_NO_POINT.
+ *   min_dist       MinDistOutlierFilter minDist (< 0: off): keep pairs with d^2 > minDist^2 (sfe_icp_params.flags
+ *                  bit 0: d^2 > minDist, as for MaxDist)
+ *   median_factor  MedianDistOutlierFilter factor (< 0: off): keep d^2 <= factor * median, median = element
+ *                  floor(n_finite * 0.5) of the ascending finite squared distances (no finite one: SFE_ICP_NO_OUTLIER)
+ * Outlier weights are the product over the chain (with sfe_icp_params' MaxDist and TrimmedDist). */
+enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_MAX_DATA_FILTERS = 4 };
+typedef struct {
+  int kind; /* SFE_ICP_DATA_MAX_DIST or SFE_ICP_DATA_MIN_DIST */
+  int dim;  /* -1 radial, 0 x, 1 y */
+  float dist;
+} sfe_icp_data_filter;
+typedef struct {
+  float min_dist;
+  float median_factor;
+  int n_reading, n_reference; /* 0 .. SFE_ICP_MAX_DATA_FILTERS */
+  sfe_icp_data_filter reading[SFE_ICP_MAX_DATA_FILTERS], reference[SFE_ICP_MAX_DATA_FILTERS];
+} sfe_icp_filters;
+/* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
+ * the default).  Checked here: no NaN, kind and dim known, counts in range; SFE_ERR_ARG leaves the setting as it was. */
+SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);
+
 /* ------------------------------------------------------------------ robust covariance of ICP samples (row N1)
  * SLAM.compute_icp_with_cov, slam.py:365-371: MinCovDet(store_precision=False, support_fraction=0.8).fit(samples),
  * batched over n_problems candidates.  The algorithm is scikit-learn 1.9's (sklearn/covariance/_robust_covariance.py:
@@ -431,6 +461,10 @@ SFE_API int sfe_frontend_set_clouds(sfe_frontend *fe, float *dst, int64_t capaci
  * iterations and inliers 0.  With carry on the carried window still advances, so turning the scan match back on
  * continues the sequence.  enable != 0: the default. */
 SFE_API int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable);
+/* The ICP filters (sfe_icp_filters) of this front end's scan match, from the next run call on (copied; NULL: none, the
+ * default).  The reading filters see each frame's cloud, the reference filters its window submap; the min_points test
+ * still counts the clouds before the filters (slam.py checks them before ICP runs). */
+SFE_API int sfe_frontend_set_icp_filters(sfe_frontend *fe, const sfe_icp_filters *filters);
 /* Several sonar geometries in one front end: a bag whose range setting changes (num_ranges, range_resolution, beam
  * count) is fed as one sequence, and the first frames after a change are matched against the keyframes before it, as
  * the reference's window of metric keyframe clouds does (slam.py:632-633).

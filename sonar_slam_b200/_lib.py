@@ -136,6 +136,8 @@ _EXTRA_SIGNATURES = {
                      c_void_p, c_void_p],
     "sfe_icp_batch_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sfe_icp_set_filters": [c_void_p, c_void_p],
+    "sfe_frontend_set_icp_filters": [c_void_p, c_void_p],
     "sfe_mincovdet_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_mincovdet_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
@@ -184,6 +186,55 @@ class IcpParams(ctypes.Structure):
                  min_diff_rot=0.01, min_diff_trans=0.1, smooth_length=4, flags=0, minimizer=0, normals_knn=5):
         super().__init__(matcher_max_dist, outlier_max_dist, trim_ratio, max_iterations, min_diff_rot,
                          min_diff_trans, smooth_length, flags, minimizer, normals_knn)
+
+
+MAX_DIST, MIN_DIST = 1, 2  # SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST: the kinds of an IcpDataFilter
+MAX_DATA_FILTERS = 4       # SFE_ICP_MAX_DATA_FILTERS per cloud
+
+
+class IcpDataFilter(ctypes.Structure):
+    """sfe_icp_data_filter: MaxDist / MinDistDataPointsFilter {dim, dist}."""
+    _fields_ = [("kind", c_int), ("dim", c_int), ("dist", c_float)]
+
+
+class IcpFilters(ctypes.Structure):
+    """sfe_icp_filters (include/sonarfe.h): the MinDist / MedianDist outlier filters (< 0: off) and up to four distance
+    data filters per cloud.  reading / reference: sequences of (kind, dim, dist), kind MAX_DIST or MIN_DIST."""
+    _fields_ = [("min_dist", c_float), ("median_factor", c_float), ("n_reading", c_int), ("n_reference", c_int),
+                ("reading", IcpDataFilter * MAX_DATA_FILTERS), ("reference", IcpDataFilter * MAX_DATA_FILTERS)]
+
+    def __init__(self, min_dist=-1.0, median_factor=-1.0, reading=(), reference=()):
+        if len(reading) > MAX_DATA_FILTERS or len(reference) > MAX_DATA_FILTERS:
+            raise ValueError(f"IcpFilters: at most {MAX_DATA_FILTERS} data filters per cloud")
+        super().__init__(min_dist, median_factor, len(reading), len(reference))
+        for arr, fl in ((self.reading, reading), (self.reference, reference)):
+            for k, (kind, dim, dist) in enumerate(fl):
+                arr[k] = IcpDataFilter(int(kind), int(dim), float(dist))
+
+    def data_filters(self, which):
+        """[(kind, dim, dist), ...] of 'reading' or 'reference'."""
+        arr, n = (self.reading, self.n_reading) if which == "reading" else (self.reference, self.n_reference)
+        return [(arr[k].kind, arr[k].dim, arr[k].dist) for k in range(n)]
+
+
+class IcpConfig(IcpParams):
+    """IcpParams as an ICP YAML configures it (bruce_slam.pcl.parse_icp_yaml): the same structure, passed by reference
+    where IcpParams is, plus `.filters` -- the IcpFilters of the modules IcpParams does not carry, or None."""
+
+    def __init__(self, *args, filters=None, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.filters = filters
+
+
+def icp_filters_of(params, filters=None):
+    """The filters a call with these ICP parameters runs: `filters` when given, else params.filters (IcpConfig)."""
+    return filters if filters is not None else getattr(params, "filters", None)
+
+
+def set_icp_filters(ctx, filters):
+    """sfe_icp_set_filters on ctx (None: no filter), so a call never inherits an earlier call's filters."""
+    check(ctx.lib.sfe_icp_set_filters(ctx.handle, ctypes.byref(filters) if filters is not None else None),
+          "sfe_icp_set_filters")
 
 
 FrontendParams._fields_ = [

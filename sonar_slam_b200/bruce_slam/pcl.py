@@ -7,6 +7,7 @@ bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libson
     match(ref[N_t,2], in[N_s,2], knn, max_dist)                 -> (int32[knn,N_s], float32[knn,N_s])  (:161)
     match_knn(ref[N_t,2], in[N_s,2], knn, max_dist)             -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
+        (the YAML's distance data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
 float32; results are fresh float32 arrays.  Not provided: density_filter (dead code in the
@@ -119,12 +120,27 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
 
 
 # ------------------------------------------------------------------------------------------ ICP
-_SUPPORTED = ("only the module chain of the shipped bruce_slam/config/icp.yaml is implemented, plus its commented-out "
-              "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference")
+_SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are implemented, plus its commented-out "
+              "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference, the Max/MinDist data "
+              "filters and the MinDist / MedianDist outlier filters")
+_DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
+
+
+def _data_filter(name, p):
+    """MaxDist / MinDistDataPointsFilter {dim, maxDist | minDist} -> (kind, dim, dist); upstream defaults dim -1, 1 m."""
+    key, kind = _DATA_FILTERS[name]
+    dim, dist = int(p.get("dim", -1)), float(p.get(key, 1.0))
+    if dim not in (-1, 0, 1):  # libpointmatcher: InvalidParameter for a dimension the 2-D cloud does not have
+        raise ValueError(f"ICP yaml: {name} dim {dim} (2-D clouds: -1, 0 or 1)")
+    if math.isnan(dist):
+        raise ValueError(f"ICP yaml: {name} {key} is NaN")
+    return kind, dim, dist
 
 
 def parse_icp_yaml(text):
-    """libpointmatcher ICP YAML (the subset icp.yaml uses) -> _lib.IcpParams."""
+    """libpointmatcher ICP YAML (the subset described by _SUPPORTED) -> _lib.IcpConfig: the IcpParams the shipped modules
+    set, with `.filters` = the _lib.IcpFilters of the distance data filters and the MinDist / MedianDist outlier
+    filters (None when the YAML has none of them)."""
     import yaml
     cfg = yaml.safe_load(text) or {}
 
@@ -136,13 +152,31 @@ def parse_icp_yaml(text):
             return name, (prm or {})
         raise ValueError(f"ICP yaml: cannot parse module {node!r}")
 
-    prm = _lib.IcpParams(outlier_max_dist=-1.0, trim_ratio=-1.0, max_iterations=40, smooth_length=0)
-    if cfg.get("readingDataPointsFilters"):
-        raise NotImplementedError(f"ICP yaml: readingDataPointsFilters are not supported ({_SUPPORTED})")
+    def add_data_filter(chain, name, p, which):
+        f = _data_filter(name, p)
+        if (name,) + f in chain:
+            raise ValueError(f"ICP yaml: {name} {p} appears twice in {which}DataPointsFilters")
+        if len(chain) == _lib.MAX_DATA_FILTERS:
+            raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} {which}DataPointsFilters")
+        chain.append((name,) + f)
+
+    prm = _lib.IcpConfig(outlier_max_dist=-1.0, trim_ratio=-1.0, max_iterations=40, smooth_length=0)
+    reading, reference, outlier = [], [], {}
+    for node in cfg.get("readingDataPointsFilters") or []:
+        name, p = one(node)
+        if name not in _DATA_FILTERS:
+            raise NotImplementedError(f"ICP yaml: reading filter {name} ({_SUPPORTED})")
+        add_data_filter(reading, name, p, "reading")
     have_normals = False
     for node in cfg.get("referenceDataPointsFilters") or []:
         name, p = one(node)
-        # the one reference filter point-to-plane needs: it attaches the "normals" descriptor
+        if name in _DATA_FILTERS:
+            if have_normals:  # the normals would describe points the filter then removes
+                raise NotImplementedError(f"ICP yaml: {name} after SurfaceNormalDataPointsFilter ({_SUPPORTED}: the "
+                                          "distance filters go before it)")
+            add_data_filter(reference, name, p, "reference")
+            continue
+        # the one other reference filter: point-to-plane needs it, it attaches the "normals" descriptor
         if name != "SurfaceNormalDataPointsFilter" or float(p.get("epsilon", 0)) != 0:
             raise NotImplementedError(f"ICP yaml: reference filter {name} {p} ({_SUPPORTED})")
         if not int(p.get("keepNormals", 1)):
@@ -161,6 +195,14 @@ def parse_icp_yaml(text):
             prm.outlier_max_dist = float(p.get("maxDist", 1.0))
         elif name == "TrimmedDistOutlierFilter":
             prm.trim_ratio = float(p.get("ratio", 0.85))
+        elif name in ("MinDistOutlierFilter", "MedianDistOutlierFilter"):
+            if name in outlier:
+                raise ValueError(f"ICP yaml: {name} appears twice in outlierFilters")
+            # upstream defaults: minDist 1, factor 3
+            v = float(p.get("minDist", 1.0)) if name == "MinDistOutlierFilter" else float(p.get("factor", 3.0))
+            if not math.isfinite(v) or v < 0:
+                raise ValueError(f"ICP yaml: {name} {p} needs a finite, non-negative value")
+            outlier[name] = v
         else:
             raise NotImplementedError(f"ICP yaml: outlier filter {name} ({_SUPPORTED})")
     name, p = one(cfg.get("errorMinimizer", "PointToPointErrorMinimizer"))
@@ -189,6 +231,10 @@ def parse_icp_yaml(text):
             raise ValueError(f"ICP yaml: {f} is NaN")
     if prm.trim_ratio > 1.0:  # the quantile element floor(n * ratio) would lie past the sorted distances
         raise ValueError(f"ICP yaml: TrimmedDistOutlierFilter ratio {prm.trim_ratio} is above 1")
+    if reading or reference or outlier:
+        prm.filters = _lib.IcpFilters(min_dist=outlier.get("MinDistOutlierFilter", -1.0),
+                                      median_factor=outlier.get("MedianDistOutlierFilter", -1.0),
+                                      reading=[f[1:] for f in reading], reference=[f[1:] for f in reference])
     return prm
 
 
@@ -227,6 +273,7 @@ class ICP(object):
         iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
         ctx = _lib.default_context()
         import ctypes
+        _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
         _lib.check(ctx.lib.sfe_icp_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), len(src), _lib.ptr(tgt),
                                         len(tgt), _lib.ptr(g), n, _lib.ptr(T), _lib.ptr(iters), _lib.ptr(inl),
                                         _lib.ptr(st)), "ICP.compute")
@@ -265,6 +312,7 @@ class ICP(object):
         iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
         ctx = _lib.default_context()
         import ctypes
+        _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
         _lib.check(ctx.lib.sfe_icp_batch_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), _lib.ptr(soff),
                                               len(srcs), _lib.ptr(tgt), _lib.ptr(toff), len(tgts), _lib.ptr(ids),
                                               _lib.ptr(ids), n, _lib.ptr(g), _lib.ptr(T), _lib.ptr(iters),

@@ -439,7 +439,19 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
   SFE_CUDA(cudaSetDevice(ctx->device));
   return icp_run(ctx, ctx->stream, prm,
                  {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
-                  tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, nullptr, 0);
+                  tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, nullptr, 0, nullptr,
+                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+}
+
+int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_icp_set_filters: null context");
+  if (filters) {
+    const int rc = icp_filters_check(filters, "sfe_icp_set_filters");
+    if (rc != SFE_OK) return rc;
+    ctx->icp_filters = *filters;
+  }
+  ctx->has_icp_filters = filters != nullptr;
+  return SFE_OK;
 }
 
 int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host, int nt,
@@ -512,8 +524,8 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
     SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
     IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
                    d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
-    pb.n_tgt_clouds = n_tgt_clouds;
-    int rc = icp_run(ctx, ctx->stream, prm, pb, nullptr, 0);
+    pb.n_tgt_clouds = n_tgt_clouds, pb.n_src_clouds = n_src_clouds;
+    int rc = icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr, ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));

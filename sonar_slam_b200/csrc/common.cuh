@@ -40,7 +40,7 @@ struct Buffer {  // grow-only device scratch
 };
 // the slots of sfe_ctx::scratch, one per subsystem
 enum { SCR_CFAR_FLAGS = 0, SCR_FEATX = 1, SCR_CLOUD = 2, SCR_ICP = 3, SCR_MISC = 4, SCR_CFAR_LUT = 5, SCR_DS_GRID = 6,
-       SCR_MAP = 7, SCR_RO_MAP = 8, SCR_COUNT = 9 };
+       SCR_MAP = 7, SCR_RO_MAP = 8, SCR_ICP_FILTER = 9, SCR_COUNT = 10 };
 
 struct JpegState;  // jpeg.cu
 struct PngState;   // png.cu
@@ -74,6 +74,8 @@ struct sfe_ctx {
   cudaStream_t copy_stream = nullptr;   // host flavours that overlap copies with kernels (featx.cu), created on first use
   cudaEvent_t copy_ev[4] = {};
   int *work = nullptr;  // device [SFE_WORK_COUNTERS]: work counters of the persistent kernels (sfe::next_work_item)
+  sfe_icp_filters icp_filters = {};  // sfe_icp_set_filters
+  bool has_icp_filters = false;
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)

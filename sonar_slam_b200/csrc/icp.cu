@@ -74,6 +74,11 @@ struct IcpBatch {
   int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
   const int *list;    // icp_run's classes: this launch's problems, largest first (icp_classify_kernel), or null: 0 .. P-1
   const int *list_n;  // ... and their number
+  // sfe_icp_filters (the FILT kernels only): outlier filters MinDist (keep d2 > min_d2; < 0 off) and MedianDist (keep
+  // d2 <= median_factor * median; < 0 off); gate_src_cnt / gate_tgt_cnt (may be null): the clouds' sizes before the
+  // data filters, which the min_points test reads
+  float min_d2, median_factor;
+  const int *gate_src_cnt, *gate_tgt_cnt;
 };
 
 // The map class (icp_map_kernel): problem p reads its target from the grid in slot map_slot[p] (map_build)
@@ -385,10 +390,22 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const Pos 
 // the body itself: behind a device-function wrapper the shipped instantiations compiled with larger stack frames.  The
 // body reads `MAP` (a value-dependent constant, so the other class's branches are discarded per instantiation) and,
 // in the map class, the map arguments `mp`.
+// FILT (icp_filt_kernel, icp_map_filt_kernel): the batch runs sfe_icp_filters -- the MinDist / MedianDist outlier filters
+// and the min_points gate on the clouds before the data filters; kernels of their own, so that the shipped ones keep
+// their code and register allocation.
 template <int THREADS, int MINB, bool PLANE>
 __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
   constexpr bool MAP = THREADS < 0;  // false
+  constexpr bool FILT = THREADS < 0;  // false
   constexpr IcpMapArgs mp{};         // (named by the discarded map-class branches only)
+#include "icp_kernel_body.cuh"
+}
+
+template <int THREADS, int MINB, bool PLANE>
+__global__ void __launch_bounds__(THREADS, MINB) icp_filt_kernel(const IcpBatch b) {
+  constexpr bool MAP = THREADS < 0;  // false
+  constexpr bool FILT = THREADS > 0;  // true
+  constexpr IcpMapArgs mp{};
 #include "icp_kernel_body.cuh"
 }
 
@@ -396,7 +413,83 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
 template <int THREADS, int MINB, bool PLANE>
 __global__ void __launch_bounds__(THREADS, MINB) icp_map_kernel(const IcpBatch b, const IcpMapArgs mp) {
   constexpr bool MAP = THREADS > 0;  // true
+  constexpr bool FILT = THREADS < 0;  // false
 #include "icp_kernel_body.cuh"
+}
+
+template <int THREADS, int MINB, bool PLANE>
+__global__ void __launch_bounds__(THREADS, MINB) icp_map_filt_kernel(const IcpBatch b, const IcpMapArgs mp) {
+  constexpr bool MAP = THREADS > 0;  // true
+  constexpr bool FILT = THREADS > 0;  // true
+#include "icp_kernel_body.cuh"
+}
+
+// Data filters of sfe_icp_filters (MaxDist / MinDistDataPointsFilter): cloud c of a batch (cloud id[c], or c with id
+// null) -> its survivors, in input order, at out_pts + 2 * c * n_max; out_off[c] = c * n_max, out_cnt[c] = their number,
+// out_raw[c] = the cloud's size before the filters.  A cloud of more than n_max points is passed on uncompacted with its
+// size (the ICP launch then reports it, SFE_ICP_TOO_LARGE).  One CTA per cloud.
+struct IcpDataFilters {
+  int n;
+  sfe_icp_data_filter f[SFE_ICP_MAX_DATA_FILTERS];
+};
+constexpr int ICP_DF_THREADS = 256;
+
+__device__ __forceinline__ bool icp_data_keep(const IcpDataFilters &df, float x, float y) {
+  bool keep = true;
+  for (int k = 0; k < df.n; ++k) {
+    const sfe_icp_data_filter &f = df.f[k];
+    bool kk;
+    if (f.dim < 0) {  // sqrtf of the unfused float32 x*x + y*y (oracle/icp_filters_ref.c)
+      const float r = __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+      kk = f.kind == SFE_ICP_DATA_MAX_DIST ? r < fabsf(f.dist) : r > fabsf(f.dist);
+    } else {
+      const float v = f.dim == 0 ? x : y;
+      kk = f.kind == SFE_ICP_DATA_MAX_DIST ? v < f.dist : v > f.dist;
+    }
+    keep = keep && kk;
+  }
+  return keep;
+}
+
+__global__ void __launch_bounds__(ICP_DF_THREADS) icp_data_filter_kernel(const PackedClouds in, const int *id,
+                                                                         int n_clouds, const IcpDataFilters df,
+                                                                         float *out_pts, int *out_off, int *out_cnt,
+                                                                         int *out_raw) {
+  __shared__ int warp_n[ICP_DF_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int c = blockIdx.x; c < n_clouds; c += gridDim.x) {
+    const int ci = id ? id[c] : c;
+    const int n = in.cnt ? in.cnt[ci] : in.off[ci + 1] - in.off[ci];
+    const float *src = in.pts + 2 * (size_t)in.off[ci];
+    float *dst = out_pts + 2 * (size_t)c * in.n_max;
+    if (tid == 0) out_off[c] = c * in.n_max, out_raw[c] = n;
+    if (c == n_clouds - 1 && tid == 0) out_off[n_clouds] = n_clouds * in.n_max;
+    if (n > in.n_max) {
+      if (tid == 0) out_cnt[c] = n;
+      continue;
+    }
+    int base = 0;
+    for (int i0 = 0; i0 < n; i0 += ICP_DF_THREADS) {
+      const int i = i0 + tid;
+      float x = 0.f, y = 0.f;
+      const bool keep = i < n && (x = src[2 * i], y = src[2 * i + 1], icp_data_keep(df, x, y));
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      if (lane == 0) warp_n[warp] = __popc(m);
+      __syncthreads();
+      int before = base, total = 0;
+      for (int w = 0; w < ICP_DF_THREADS / 32; ++w) {
+        if (w < warp) before += warp_n[w];
+        total += warp_n[w];
+      }
+      if (keep) {
+        const int at = before + __popc(m & ((1u << lane) - 1u));
+        dst[2 * at] = x, dst[2 * at + 1] = y;
+      }
+      base += total;
+      __syncthreads();  // warp_n is rewritten by the next chunk
+    }
+    if (tid == 0) out_cnt[c] = base;
+  }
 }
 
 // pcl.match: nearest reference point (within max_dist) of every query point; one CTA per (ref, query) pair
@@ -583,6 +676,26 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
 }
 
 // ---------------------------------------------------------------------------- host side
+int icp_filters_check(const sfe_icp_filters *f, const char *what) {
+  SFE_REQUIRE(!std::isnan(f->min_dist) && !std::isnan(f->median_factor),
+              "%s: a NaN MinDist / MedianDist outlier filter setting is not supported", what);
+  SFE_REQUIRE(f->median_factor < 0.f || std::isfinite(f->median_factor), "%s: MedianDistOutlierFilter factor %g",
+              what, (double)f->median_factor);
+  SFE_REQUIRE(f->n_reading >= 0 && f->n_reading <= SFE_ICP_MAX_DATA_FILTERS && f->n_reference >= 0 &&
+                  f->n_reference <= SFE_ICP_MAX_DATA_FILTERS,
+              "%s: %d reading / %d reference data filters (0..%d each)", what, f->n_reading, f->n_reference,
+              SFE_ICP_MAX_DATA_FILTERS);
+  for (int side = 0; side < 2; ++side)
+    for (int k = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
+      const sfe_icp_data_filter &d = side ? f->reference[k] : f->reading[k];
+      SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST,
+                  "%s: unknown data filter kind %d", what, d.kind);
+      SFE_REQUIRE(d.dim >= -1 && d.dim <= 1, "%s: data filter dim %d (2-D clouds: -1, 0 or 1)", what, d.dim);
+      SFE_REQUIRE(!std::isnan(d.dist), "%s: a NaN data filter distance is not supported", what);
+    }
+  return SFE_OK;
+}
+
 static int pick_max_cells(int nt_max) {
   int c = nt_max + nt_max / 2;  // the grid aims at one point per cell; the slack absorbs elongated bounding boxes
   if (c < 256) c = 256;
@@ -618,19 +731,26 @@ static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 153
 // icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget).
 // 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers.  dense (icp_run's classes):
 // 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get them (IcpClass::dense).
-static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense = false) {
-  if (threads == 128 && dense)
-    return plane ? (const void *)icp_kernel<128, 8, true> : (const void *)icp_kernel<128, 8, false>;
-  if (threads == 128) return plane ? (const void *)icp_kernel<128, 7, true> : (const void *)icp_kernel<128, 7, false>;
-  if (threads == 256) return plane ? (const void *)icp_kernel<256, 4, true> : (const void *)icp_kernel<256, 4, false>;
-  if (smem <= 110 * 1024) return plane ? (const void *)icp_kernel<512, 2, true> : (const void *)icp_kernel<512, 2, false>;
-  return plane ? (const void *)icp_kernel<512, 1, true> : (const void *)icp_kernel<512, 1, false>;
+// filt: icp_filt_kernel's instantiation instead (sfe_icp_filters)
+template <int THREADS, int MINB>
+static const void *icp_kernel_of(bool plane, bool filt) {
+  if (filt) return plane ? (const void *)icp_filt_kernel<THREADS, MINB, true> : (const void *)icp_filt_kernel<THREADS, MINB, false>;
+  return plane ? (const void *)icp_kernel<THREADS, MINB, true> : (const void *)icp_kernel<THREADS, MINB, false>;
+}
+
+static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense = false, bool filt = false) {
+  if (threads == 128 && dense) return icp_kernel_of<128, 8>(plane, filt);
+  if (threads == 128) return icp_kernel_of<128, 7>(plane, filt);
+  if (threads == 256) return icp_kernel_of<256, 4>(plane, filt);
+  if (smem <= 110 * 1024) return icp_kernel_of<512, 2>(plane, filt);
+  return icp_kernel_of<512, 1>(plane, filt);
 }
 
 // Shared memory icp_kernel's layouts may take next to sources of ns_max points: the budget of the instantiation that
 // runs the largest of them.
-static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, size_t *budget, bool dense = false) {
-  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense), budget);
+static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, size_t *budget, bool dense = false,
+                          bool filt = false) {
+  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense, filt), budget);
 }
 
 static void icp_tuning(IcpBatch &b) {
@@ -665,9 +785,10 @@ static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_
   b.cell_scale = 1.0f;
   b.prm = *prm;
   icp_tuning(b);
-  const bool plane = prm->minimizer == 1;
+  const bool plane = prm->minimizer == 1, filt = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f ||
+                                                   b.median_factor >= 0.f;
   size_t budget;
-  int rc = icp_cta_budget(ctx, threads, plane, &budget, dense);
+  int rc = icp_cta_budget(ctx, threads, plane, &budget, dense, filt);
   if (rc != SFE_OK) return rc;
   const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, budget, &b.max_cells);
   if (smem > budget) {
@@ -675,7 +796,7 @@ static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_
               budget);
     return SFE_ERR_UNSUPPORTED;
   }
-  const void *fn = icp_kernel_for(threads, smem, plane, dense);
+  const void *fn = icp_kernel_for(threads, smem, plane, dense, filt);
   int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
   if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
 #ifdef SFE_ICP_PHASE_CLOCKS
@@ -822,7 +943,7 @@ static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *
 // The map class: problems whose target has more than `limit` points, their targets read from map grids.  Shared memory
 // holds IcpShared and the source arrays only.
 static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max,
-                          int limit, int slot_cap) {
+                          int limit, int slot_cap, bool filt) {
   const bool plane = prm->minimizer == 1;
   MapWs w;
   int rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, limit, slot_cap, true,
@@ -853,6 +974,13 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
                          : (threads == 128   ? (const void *)icp_map_kernel<128, 7, false>
                             : threads == 256 ? (const void *)icp_map_kernel<256, 4, false>
                                              : (const void *)icp_map_kernel<512, 1, false>);
+  if (filt)
+    fn = plane ? (threads == 128   ? (const void *)icp_map_filt_kernel<128, 7, true>
+                  : threads == 256 ? (const void *)icp_map_filt_kernel<256, 4, true>
+                                   : (const void *)icp_map_filt_kernel<512, 1, true>)
+               : (threads == 128   ? (const void *)icp_map_filt_kernel<128, 7, false>
+                  : threads == 256 ? (const void *)icp_map_filt_kernel<256, 4, false>
+                                   : (const void *)icp_map_filt_kernel<512, 1, false>);
   int per_sm;
   if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
   int grid = ctx->sm_count * per_sm;
@@ -874,8 +1002,34 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
 // (and reports oversize ones, SFE_ICP_TOO_LARGE).  Without classes one launch takes every problem (IcpBatch::class_mode
 // 0) -- unless the largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit
 // (class_mode 1) and the map class (map grids in global memory, icp_map_kernel) takes the rest.
-int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
-                 const IcpClass *class_list, int n_classes, int *class_of) {
+namespace sfe {
+// Data filters: the clouds of one side of the batch, compacted into scratch[SCR_ICP_FILTER] (icp_data_filter_kernel),
+// once per cloud when the cloud count is known (no ids: one per problem), else once per problem (the ids then name the
+// compacted clouds no more).  Two passes over the Carver: the first sizes the block, the second launches.
+static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const IcpDataFilters &df, PackedClouds &c, const int *&id,
+                           int n_clouds, int P, Carver &cv, const int *&gate) {
+  const int jobs = id && n_clouds > 0 ? n_clouds : P;
+  const int n_max = c.n_max > 0 ? c.n_max : 1;
+  float *pts = (float *)cv.take(sizeof(float) * 2 * (size_t)jobs * n_max);
+  int *off = (int *)cv.take(sizeof(int) * (size_t)(jobs + 1));
+  int *cnt = (int *)cv.take(sizeof(int) * (size_t)jobs);
+  int *raw = (int *)cv.take(sizeof(int) * (size_t)jobs);
+  if (!cv.base) return SFE_OK;
+  const bool per_problem = id && n_clouds <= 0;
+  icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
+      {c.pts, c.off, c.cnt, n_max}, per_problem ? id : nullptr, jobs, df, pts, off, cnt, raw);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  c = {pts, off, cnt, c.n_max};
+  if (per_problem) id = nullptr;
+  gate = raw;
+  return SFE_OK;
+}
+}  // namespace sfe
+
+int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb_in,
+                 const IcpClass *class_list, int n_classes, int *class_of, const sfe_icp_filters *filt) {
+  IcpProblems pb = pb_in;
   const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
   SFE_REQUIRE(ctx && prm, "icp: null context or parameters");
   SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp: negative sizes");
@@ -902,7 +1056,43 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
               "icp: a NaN parameter (maxDist, ratio or minDiff*) is not supported");
   // (the quantile element floor(n * ratio) lies past the sorted distances for a ratio above 1)
   SFE_REQUIRE(prm->trim_ratio <= 1.0f, "icp: TrimmedDistOutlierFilter ratio %g is above 1", (double)prm->trim_ratio);
+  if (filt) {
+    int rc = icp_filters_check(filt, "icp");
+    if (rc != SFE_OK) return rc;
+  }
+  const int *gate_src = nullptr, *gate_tgt = nullptr;
+  if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
+    IcpDataFilters rd{filt->n_reading, {}}, rf{filt->n_reference, {}};
+    for (int k = 0; k < SFE_ICP_MAX_DATA_FILTERS; ++k) rd.f[k] = filt->reading[k], rf.f[k] = filt->reference[k];
+    Carver cv;
+    for (int pass = 0; pass < 2; ++pass) {
+      IcpProblems q = pb;
+      if (rd.n > 0) {
+        int rc = icp_filter_side(ctx, st, rd, q.src, q.src_id, q.n_src_clouds, q.P, cv, gate_src);
+        if (rc != SFE_OK) return rc;
+      }
+      if (rf.n > 0) {
+        int rc = icp_filter_side(ctx, st, rf, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv, gate_tgt);
+        if (rc != SFE_OK) return rc;
+        if (q.tgt_id != pb.tgt_id) q.n_tgt_clouds = q.P;  // one compacted target per problem
+      }
+      if (pass == 0) {
+        int rc = ensure(ctx, ctx->scratch[SCR_ICP_FILTER], cv.off, st);
+        if (rc != SFE_OK) return rc;
+        cv.base = (char *)ctx->scratch[SCR_ICP_FILTER].ptr, cv.off = 0;
+      } else {
+        pb = q;
+      }
+    }
+  }
   IcpBatch b{};
+  b.min_d2 = b.median_factor = -1.f;
+  if (filt) {
+    b.min_d2 = filt->min_dist < 0.f ? -1.f : (prm->flags & 1) ? filt->min_dist : filt->min_dist * filt->min_dist;
+    b.median_factor = filt->median_factor;
+    b.gate_src_cnt = gate_src, b.gate_tgt_cnt = gate_tgt;
+  }
+  const bool filt_on = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;
   b.raw_cnt = pb.raw_cnt, b.raw_cap = pb.raw_cap;
@@ -914,7 +1104,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     const int ns = ns_max > 0 ? ns_max : 1;
     const bool plane = prm->minimizer == 1;
     size_t budget;
-    int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget);
+    int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget, false, filt_on);
     if (rc != SFE_OK) return rc;
     int mc;
     const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
@@ -927,7 +1117,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
       if (rc != SFE_OK) return rc;
     }
     const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-    return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap);
+    return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap, filt_on);
   }
   return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
 }

@@ -1,6 +1,7 @@
 // Body of icp_kernel and icp_map_kernel (icp.cu): included inside both kernel definitions, never on its own.
-// In scope there: the batch `b`, the constant `MAP` (true: the target is a map grid, read through `mp`) and the
-// template parameters THREADS and PLANE.
+// In scope there: the batch `b`, the constants `MAP` (true: the target is a map grid, read through `mp`) and `FILT`
+// (true: the batch runs sfe_icp_filters, icp_filt_kernel / icp_map_filt_kernel) and the template parameters THREADS and
+// PLANE.
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
   //         [prev Pos ns_max][qstate u8 ns_max][slack f32 ns_max][order u16 ns_max]   (MAP: no sorted, no cells)
@@ -84,7 +85,10 @@
     if (tid == 0) {
       int st = ICP_OK;
       if (ns > b.ns_max || nt > b.nt_max || (b.raw_cnt && b.raw_cnt[si] > b.raw_cap)) st = ICP_TOO_LARGE;
-      else if (ns < b.min_points || nt < b.min_points) st = ICP_SKIPPED;
+      else if (!FILT && (ns < b.min_points || nt < b.min_points)) st = ICP_SKIPPED;
+      else if (FILT && ((b.gate_src_cnt ? b.gate_src_cnt[si] : ns) < b.min_points ||
+                        (b.gate_tgt_cnt ? b.gate_tgt_cnt[ti] : nt) < b.min_points))
+        st = ICP_SKIPPED;  // (the clouds before the data filters, as the SLAM node counts them before ICP)
       else if (nt <= 0) st = ICP_EMPTY_REF;
       const float det = __fsub_rn(__fmul_rn(guess[0], guess[4]), __fmul_rn(guess[1], guess[3]));
       if (st == ICP_OK && (!(fabsf(__fsub_rn(1.0f, det)) <= 0.001f))) st = ICP_NOT_RIGID;
@@ -475,7 +479,37 @@
       // pass C: settle what still matters
       if (!small) {
         float stop_d2 = INFINITY;
-        if (prm.trim_ratio >= 0.f) {
+        if constexpr (FILT) {
+          // Several filters (sfe_icp_filters).  Every rank a selection needs must be exact, and so must every distance
+          // the upper-limit filters together could keep.  U_k = the k-th smallest upper bound >= the k-th smallest
+          // distance, so a search bounded by stop_d2 >= U_k leaves the k smallest distances exact: the selections of
+          // 3b see the true elements.  A pair kept by the chain has d2 <= min(out_d2, trim limit, factor * median) <=
+          // min(out_d2, U_ktrim, factor * U_kmed) (both limits are at most their upper bounds, the float32 product is
+          // monotone), so with stop_d2 at least that minimum every keepable pair is exact, and a pruned point (stored
+          // as ICP_PRUNED) fails the filter whose bound is the minimum.  Hence
+          //   stop_d2 = max(U_k of each active selection, min(out_d2, U_ktrim, factor * U_kmed)).
+          // MinDist keeps far pairs, so it bounds nothing: alone it allows no pruning.
+          const bool q_trim = prm.trim_ratio >= 0.f, q_med = b.median_factor >= 0.f;
+          if (!((q_trim || q_med) && total_fin == 0)) {
+            float u_trim = INFINITY, u_med = INFINITY, sel = -INFINITY;
+            if (q_trim && prm.trim_ratio < 1.0f) {
+              int kk = (int)(size_t)__fmul_rn((float)total_fin, prm.trim_ratio);
+              if (kk >= total_fin) kk = total_fin - 1;
+              u_trim = block_select_kth(dist, ns, kk, sh, sel_pass);
+            }
+            if (q_trim) sel = u_trim;
+            if (q_med) {
+              int kk = (int)(size_t)__fmul_rn((float)total_fin, 0.5f);
+              if (kk >= total_fin) kk = total_fin - 1;
+              u_med = block_select_kth(dist, ns, kk, sh, sel_pass);
+              sel = fmaxf(sel, u_med);
+            }
+            float upper = q_trim ? u_trim : INFINITY;
+            if (prm.outlier_max_dist > 0.f) upper = fminf(upper, out_d2);
+            if (q_med) upper = fminf(upper, __fmul_rn(b.median_factor, u_med));
+            stop_d2 = fmaxf(sel, upper);
+          }
+        } else if (prm.trim_ratio >= 0.f) {
           if (prm.trim_ratio < 1.0f && total_fin > 0) {
             int kk = (int)(size_t)__fmul_rn((float)total_fin, prm.trim_ratio);
             if (kk >= total_fin) kk = total_fin - 1;
@@ -523,15 +557,24 @@
       }
 
       ICP_PH_MARK(1);
-      // 3b. trimmed-distance limit = element floor(float(n)*ratio) of the ascending finite distances
-      float limit = INFINITY;
-      if (prm.trim_ratio >= 0.f) {
+      // 3b. trimmed-distance limit = element floor(float(n)*ratio) of the ascending finite distances (FILT: and the
+      // median-distance limit)
+      float limit = INFINITY, med_limit = INFINITY;
+      if (prm.trim_ratio >= 0.f || (FILT && b.median_factor >= 0.f)) {
         if (total_fin == 0) {
           if (tid == 0) sh.status = ICP_NO_OUTLIER;
           __syncthreads();
           break;
         }
-        if (prm.trim_ratio == 1.0f) {
+        if constexpr (FILT) {  // MedianDistOutlierFilter: factor * getDistsQuantile(0.5), a float32 product
+          if (b.median_factor >= 0.f) {
+            int kk = (int)(size_t)__fmul_rn((float)total_fin, 0.5f);
+            if (kk >= total_fin) kk = total_fin - 1;
+            med_limit = __fmul_rn(b.median_factor, block_select_kth(dist, ns, kk, sh, sel_pass));
+          }
+        }
+        if (FILT && prm.trim_ratio < 0.f) {  // (the median alone)
+        } else if (prm.trim_ratio == 1.0f) {
           float m = 0.f;
           for (int i = tid; i < ns; i += nthr)
             if (dist[i] < INFINITY) m = fmaxf(m, dist[i]);
@@ -550,6 +593,7 @@
           limit = block_select_kth(dist, ns, kk, sh, sel_pass);
         }
       }
+      (void)med_limit;
 
       ICP_PH_MARK(2);
       // 3c. kept pairs.  The candidate match of point i is prev[i] on the one-pass path (its re-search list took
@@ -560,6 +604,10 @@
         bool keep = m != NONE;
         if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
         if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
+        if constexpr (FILT) {
+          if (b.min_d2 >= 0.f) keep = keep && (dist[i] > b.min_d2);
+          if (b.median_factor >= 0.f) keep = keep && (dist[i] <= med_limit);
+        }
         return keep ? m : NONE;
       };
       // Sequential mode: the sums are warp 0's alone, so warp 0 also forms the fit and, on the one-pass path, the

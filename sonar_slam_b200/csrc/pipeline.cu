@@ -229,6 +229,8 @@ struct sfe_frontend {
   int64_t *cloud_off = nullptr, *cloud_off_host = nullptr;  // [max_frames + 1]
   cudaEvent_t ev_cloud[2] = {};
   int scan_match = 1;  // sfe_frontend_set_scan_match
+  sfe_icp_filters icp_filters = {};  // sfe_frontend_set_icp_filters
+  bool has_icp_filters = false;
   StageTimer timer;  // optional per-stage timing, on ctx->stream
 };
 
@@ -603,7 +605,8 @@ static int fe_match(sfe_frontend *fe, int f0, int n) {
   pb.raw_cnt = fe->cnt_a + f0, pb.raw_cap = cap;  // the source's Cartesian points before the filters
   pb.guess = fe->guess + 9 * (size_t)f0, pb.T_out = fe->T + 9 * (size_t)f0;
   pb.iters = fe->iters + f0, pb.inliers = fe->inliers + f0, pb.status = fe->status + f0;
-  const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES);
+  const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, nullptr,
+                         fe->has_icp_filters ? &fe->icp_filters : nullptr);
   fe->timer.toc(st);
   return rc;
 }
@@ -773,6 +776,17 @@ int sfe_frontend_set_clouds(sfe_frontend *fe, float *dst, int64_t capacity_point
 int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable) {
   SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_scan_match: null handle");
   fe->scan_match = enable != 0;
+  return SFE_OK;
+}
+
+int sfe_frontend_set_icp_filters(sfe_frontend *fe, const sfe_icp_filters *filters) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_icp_filters: null handle");
+  if (filters) {
+    const int rc = icp_filters_check(filters, "sfe_frontend_set_icp_filters");
+    if (rc != SFE_OK) return rc;
+    fe->icp_filters = *filters;
+  }
+  fe->has_icp_filters = filters != nullptr;
   return SFE_OK;
 }
 
@@ -1041,7 +1055,8 @@ int sfe_frontend_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *s
   SFE_CUDA(cudaSetDevice(ctx->device));
   IcpProblems pb{{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, nullptr,
                  nullptr, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev};
-  return icp_run(ctx, ctx->stream, prm, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, class_dev);
+  return icp_run(ctx, ctx->stream, prm, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, class_dev,
+                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
 }
 
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {

@@ -29,6 +29,7 @@ struct IcpProblems {
   const int *raw_cnt;
   int raw_cap;
   int n_tgt_clouds;  // number of target clouds when the caller knows it (bounds the map grids, icp.cu), else 0
+  int n_src_clouds;  // number of source clouds when the caller knows it (the data filters run once per cloud), else 0
 };
 
 int cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int F, int R, int B, int alg, int T, int G,
@@ -61,8 +62,12 @@ constexpr int ICP_MAX_CLASSES = 3;  // classes an icp_run call may list (the cap
 // the targets that do and the map class for the rest.  class_of (device [P], may be null; classes only): receives
 // every problem's class (0 .. n_classes, the capacity class last) and, in class_of[P + p], its place in that class's
 // list.
+// filt (may be null): sfe_icp_filters -- data filters compacted into scratch once per cloud before the launches, and
+// the outlier filters in icp_kernel's FILT instantiations; min_points then counts the clouds before the data filters.
 int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, const IcpClass *classes,
-            int n_classes, int *class_of = nullptr);
+            int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr);
+// SFE_OK, or SFE_ERR_ARG with a message naming `what`: NaN, unknown kind, dim outside -1 .. 1, counts out of range
+int icp_filters_check(const sfe_icp_filters *f, const char *what);
 // nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,

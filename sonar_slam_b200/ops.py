@@ -152,8 +152,10 @@ def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, knn=None, ctx=N
     return dict(ids=ids, dists=d)
 
 
-def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, src_id=None, tgt_id=None, ctx=None):
+def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, src_id=None, tgt_id=None, ctx=None,
+        filters=None):
     """Batched ICP (include/sonarfe.h: sfe_icp_dev).  guess: [P,3,3] f32 cuda.  Returns dict of cuda tensors.
+    filters: _lib.IcpFilters (sfe_icp_set_filters), default params.filters when params is a parsed _lib.IcpConfig.
 
     Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
     map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources: at most 65 535
@@ -166,6 +168,7 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
     iters = torch.empty((P,), dtype=torch.int32, device=guess.device)
     inl = torch.empty_like(iters)
     st = torch.empty_like(iters)
+    _lib.set_icp_filters(ctx, _lib.icp_filters_of(prm, filters))
     _lib.check(ctx.lib.sfe_icp_dev(ctx.handle, ctypes.byref(prm), _dp(src_pts), _dp(src_off), _dp(tgt_pts),
                                    _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, int(ns_max), int(nt_max), _dp(guess),
                                    _dp(T), _dp(iters), _dp(inl), _dp(st)), "sfe_icp_dev")

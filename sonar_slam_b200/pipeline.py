@@ -17,9 +17,10 @@ from . import _lib, _streams
 
 
 class FrontEnd:
-    def __init__(self, ctx, maps, max_frames, **overrides):
+    def __init__(self, ctx, maps, max_frames, icp_filters=None, **overrides):
         """overrides: any field of sfe_frontend_params (e.g. tau=..., window=3, cap_points=4096) or
-        `icp=_lib.IcpParams(...)`."""
+        `icp=_lib.IcpParams(...)`.  icp_filters: _lib.IcpFilters of the scan match (sfe_frontend_set_icp_filters),
+        default icp.filters when `icp` is a parsed _lib.IcpConfig."""
         self.ctx, self.maps, self.lib = ctx, maps, ctx.lib
         p = _lib.FrontendParams()
         self.lib.sfe_frontend_params_default(ctypes.byref(p))
@@ -35,6 +36,9 @@ class FrontEnd:
         _lib.check(self.lib.sfe_frontend_create(ctx.handle, maps.handle, ctypes.byref(p), self.max_frames,
                                                 ctypes.byref(h)), "sfe_frontend_create")
         self.handle = h
+        filters = _lib.icp_filters_of(overrides.get("icp"), icp_filters)
+        if filters is not None:
+            _lib.check(self.lib.sfe_frontend_set_icp_filters(h, ctypes.byref(filters)), "sfe_frontend_set_icp_filters")
 
     def add_geometry(self, maps):
         """Register a further sonar geometry (sfe_frontend_add_geometry) and return its id; the creation maps are
