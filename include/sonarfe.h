@@ -28,7 +28,9 @@ extern "C" {
 
 #define SFE_VERSION 202 /* round 2: + sfe_fov_select_*, sfe_frontend_set_carry, sfe_frontend_params.flip_lateral, sfe_icp_params.flags bit 1;
                             201: + sfe_icp_params.minimizer / normals_knn (point-to-plane, icp.yaml:18-19);
-                            202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch) */
+                            202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch); later
+                                 additions that change no existing entry point: sfe_match_dim_*, sfe_match_knn_dim_*,
+                                 sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -142,7 +144,7 @@ SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uin
                                    const uint8_t *lut_bgr_host, uint8_t *out_host);
 
 /* ------------------------------------------------------------------ point-cloud filters
- * Clouds are packed: pts [total][dim] float32 (dim = 2: x,y; remove_outlier also takes 3: x,y,z),
+ * Clouds are packed: pts [total][dim] float32 (dim = 2: x,y; dim = 3: x,y,z),
  * off [n_clouds + 1] int32 offsets (cloud c = rows off[c] .. off[c+1]-1), n_max = largest cloud.
  * Results are compacted in place of each cloud: out_pts rows off[c] .. off[c]+out_count[c]-1, and
  * out_idx gives, for every surviving point, its row inside its input cloud.
@@ -159,6 +161,10 @@ SFE_API int sfe_feature_image_host(sfe_ctx *ctx, const sfe_maps *maps, const uin
  *                       with a cloud above that limit takes at most 65 535 clouds and
  *                       n_clouds * n_max slots (at most 2^31 - 1); its workspace holds 48 bytes
  *                       per slot.  Trees stop at 15 levels (16 km at a 0.5 m resolution).
+ *                       dim = 3 (libpointmatcher's 3-D Octree): an octree on the bounding cube
+ *                       (half-size = the largest half-extent, children by x, y, z > centre), the
+ *                       3-D medoid sum; the one-CTA limit is lower (24 bytes per point of shared
+ *                       memory instead of 16), the grid-wide workspace 52 bytes per slot.
  * sfe_remove_outlier_*  bruce_slam.pcl.remove_outlier (pcl.cpp:54-74): PCL RadiusOutlierRemoval:
  *                       keep a point iff at least min_points OTHER points lie within `radius`;
  *                       input order is preserved.
@@ -184,6 +190,9 @@ SFE_API int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const 
                                       const int32_t *cnt_dev, int n_clouds, int n_max, int frame_points,
                                       float resolution, float *out_pts_dev, int32_t *out_idx_dev,
                                       int32_t *out_count_dev);
+/* *limit = the largest cloud of `dim` columns that sfe_downsample_* runs in one CTA on this context's device (larger
+ * clouds take the grid-wide path) */
+SFE_API int sfe_downsample_cta_limit(sfe_ctx *ctx, int dim, int32_t *limit);
 /* single-cloud host flavours: n points in, *n_out points out (out buffers hold n entries) */
 SFE_API int sfe_downsample_host(sfe_ctx *ctx, const float *pts_host, int n, int dim, float resolution,
                                 float *out_pts_host, int32_t *out_idx_host, int32_t *n_out);
@@ -219,6 +228,21 @@ SFE_API int sfe_match_knn_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int3
                               float max_dist, int32_t *ids_dev, float *dists_dev);
 SFE_API int sfe_match_knn_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int knn,
                                float max_dist, int32_t *ids_host, float *dists_host);
+/* sfe_match_* and sfe_match_knn_* for clouds of `dim` columns (2: the calls above, same kernels and results; 3: x, y, z
+ * in both clouds).  3-D: squared float32 distance (dx*dx + dy*dy) + dz*dz, every other rule as above; the search runs on
+ * a grid of x, y (exact: the 3-D distance is never below the xy one), so a reference tall in z over a small xy
+ * footprint is searched column by column.  The one-CTA / map-grid split is sfe_match_knn_*'s at every knn (its lists
+ * included at knn = 1); the map grids' workspace is sfe_match_dev's.  dim outside 2 .. 3 is SFE_ERR_ARG. */
+SFE_API int sfe_match_dim_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev,
+                              const float *in_pts_dev, const int32_t *in_off_dev, int n_pairs, int dim, int n_ref_max,
+                              float max_dist, int32_t *ids_dev, float *dists_dev);
+SFE_API int sfe_match_dim_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int dim,
+                               float max_dist, int32_t *ids_host, float *dists_host);
+SFE_API int sfe_match_knn_dim_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev,
+                                  const float *in_pts_dev, const int32_t *in_off_dev, int n_pairs, int dim,
+                                  int n_ref_max, int knn, float max_dist, int32_t *ids_dev, float *dists_dev);
+SFE_API int sfe_match_knn_dim_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in,
+                                   int dim, int knn, float max_dist, int32_t *ids_host, float *dists_host);
 
 /* ------------------------------------------------------------------ ICP scan matcher
  * bruce_slam.pcl.ICP (pcl.cpp:185-213): libpointmatcher PointMatcher<float>::ICP configured by

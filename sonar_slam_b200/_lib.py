@@ -101,12 +101,19 @@ _EXTRA_SIGNATURES = {
     "sfe_downsample_frames_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                                   c_void_p, c_void_p],
     "sfe_downsample_host": [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
+    "sfe_downsample_cta_limit": [c_void_p, c_int, c_void_p],
     "sfe_remove_outlier_host": [c_void_p, c_void_p, c_int, c_int, c_double, c_int, c_void_p, c_void_p, c_void_p],
     "sfe_match_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p],
     "sfe_match_host": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p],
     "sfe_match_knn_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
                           c_void_p],
     "sfe_match_knn_host": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p],
+    "sfe_match_dim_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p,
+                          c_void_p],
+    "sfe_match_dim_host": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p],
+    "sfe_match_knn_dim_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
+                              c_void_p, c_void_p],
+    "sfe_match_knn_dim_host": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p],
     "sfe_icp_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                     c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_frontend_icp_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,

@@ -2,15 +2,17 @@
 bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libsonarfe.
 
     remove_outlier(points[N,2|3], radius, min_points)          -> float32[M,2|3]      (pcl.cpp:54)
-    downsample(points[N,2], resolution)                         -> float32[M,2]        (pcl.cpp:128)
-    downsample(points[N,2], desc[N,d], resolution)              -> (points, desc)      (pcl.cpp:143)
-    match(ref[N_t,2], in[N_s,2], knn, max_dist)                 -> (int32[knn,N_s], float32[knn,N_s])  (:161)
-    match_knn(ref[N_t,2], in[N_s,2], knn, max_dist)             -> the same for knn 1 .. 16 (match serves knn = 1)
+    downsample(points[N,2|3], resolution)                       -> float32[M,2|3]      (pcl.cpp:128)
+    downsample(points[N,2|3], desc[N,d], resolution)            -> (points, desc)      (pcl.cpp:143)
+    match(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)             -> (int32[knn,N_s], float32[knn,N_s])  (:161)
+    match_knn(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)         -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
         (the YAML's distance data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
-float32; results are fresh float32 arrays.  Not provided: density_filter (dead code in the
+float32; results are fresh float32 arrays.  Three columns are x, y, z, as fromEigen (pcl.cpp:18-50) reads them:
+downsample then builds libpointmatcher's octree instead of the quadtree, match measures 3-D distances, and the
+reference and query of a match must have the same number of columns.  ICP takes 2-column clouds only.  Not provided: density_filter (dead code in the
 reference: its only call site is commented out, feature_extraction.py:246) and
 ICP.getCovariance (never called from Python) -- both raise NotImplementedError.
 """
@@ -52,7 +54,7 @@ def downsample(mat_in, *args):
         desc, resolution = args
     else:
         raise TypeError("pcl.downsample: incompatible function arguments")
-    pts = _points(mat_in, "points", cols=(2,))
+    pts = _points(mat_in, "points")
     if desc is not None:
         desc = np.asarray(desc)
         if desc.ndim != 2 or len(desc) != len(pts):
@@ -65,7 +67,7 @@ def downsample(mat_in, *args):
     out = np.empty_like(pts)
     idx = np.empty(n, np.int32)
     m = np.zeros(1, np.int32)
-    _lib.check(ctx.lib.sfe_downsample_host(ctx.handle, _lib.ptr(pts), n, 2, float(resolution), _lib.ptr(out),
+    _lib.check(ctx.lib.sfe_downsample_host(ctx.handle, _lib.ptr(pts), n, pts.shape[1], float(resolution), _lib.ptr(out),
                                            _lib.ptr(idx), _lib.ptr(m)), "downsample")
     k = int(m[0])
     if desc is None:
@@ -78,20 +80,34 @@ def density_filter(*args, **kwargs):
                               "out, feature_extraction.py:246) and is not provided")
 
 
+def _match_clouds(mat_ref, mat_in):
+    """ref and in as float32 [N,2] or [N,3] arrays with the same number of columns (libnabo rejects a query whose
+    dimension differs from the tree's)."""
+    ref = _points(mat_ref, "ref")
+    pts = _points(mat_in, "in")
+    if ref.shape[1] != pts.shape[1]:
+        raise TypeError(f"pcl: incompatible function arguments (ref has {ref.shape[1]} columns, in has "
+                        f"{pts.shape[1]})")
+    return ref, pts
+
+
 def match(mat_ref, mat_in, knn, max_dist):
     """libnabo KD-tree match, knn = 1: (ids [1,N] int32, squared dists [1,N] float32).  References of any size (whole
-    maps run as a grid in global memory, with the same results)."""
+    maps run as a grid in global memory, with the same results).  [N,3] clouds: 3-D distances."""
     if int(knn) != 1:
         raise NotImplementedError("pcl.match: only knn = 1 is implemented (the only value the reference uses, "
                                   "slam.py:418)")
-    ref = _points(mat_ref, "ref", cols=(2,))
-    pts = _points(mat_in, "in", cols=(2,))
+    ref, pts = _match_clouds(mat_ref, mat_in)
     ids = np.empty((1, len(pts)), np.int32)
     dists = np.empty((1, len(pts)), np.float32)
     if len(pts):
         ctx = _lib.default_context()
-        _lib.check(ctx.lib.sfe_match_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts),
-                                          float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match")
+        if pts.shape[1] == 3:
+            _lib.check(ctx.lib.sfe_match_dim_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts), 3,
+                                                  float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match")
+        else:
+            _lib.check(ctx.lib.sfe_match_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts),
+                                              float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match")
     return ids, dists
 
 
@@ -102,20 +118,25 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
     """libnabo KD-tree match for any knn up to 16 (what pcl.cpp:161-174 computes for knn > 1): for every query point
     its knn nearest reference points within max_dist, nearest first (ties: lower reference index), as (ids [knn,N]
     int32, squared dists [knn,N] float32); slots with no neighbour left hold -1 / +inf.  Row 0 is match(..., 1, ...)'s
-    result.  References of any size (whole maps run as a grid in global memory, with the same results)."""
+    result.  References of any size (whole maps run as a grid in global memory, with the same results).  [N,3] clouds:
+    3-D distances."""
     knn = int(knn)
     if knn < 1:
         raise ValueError(f"pcl.match_knn: knn must be at least 1 (got {knn})")
     if knn > KNN_MAX:
         raise NotImplementedError(f"pcl.match_knn: knn {knn} is not supported (at most {KNN_MAX})")
-    ref = _points(mat_ref, "ref", cols=(2,))
-    pts = _points(mat_in, "in", cols=(2,))
+    ref, pts = _match_clouds(mat_ref, mat_in)
     ids = np.empty((knn, len(pts)), np.int32)
     dists = np.empty((knn, len(pts)), np.float32)
     if len(pts):
         ctx = _lib.default_context()
-        _lib.check(ctx.lib.sfe_match_knn_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts), knn,
-                                              float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match_knn")
+        if pts.shape[1] == 3:
+            _lib.check(ctx.lib.sfe_match_knn_dim_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts), 3,
+                                                      knn, float(max_dist), _lib.ptr(ids), _lib.ptr(dists)),
+                       "match_knn")
+        else:
+            _lib.check(ctx.lib.sfe_match_knn_host(ctx.handle, _lib.ptr(ref), len(ref), _lib.ptr(pts), len(pts), knn,
+                                                  float(max_dist), _lib.ptr(ids), _lib.ptr(dists)), "match_knn")
     return ids, dists
 
 

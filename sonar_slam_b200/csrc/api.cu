@@ -275,6 +275,16 @@ int sfe_downsample_frames_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t 
                         out_idx_dev, out_count_dev, frame_points, SCR_CLOUD, WORK_DS);
 }
 
+int sfe_downsample_cta_limit(sfe_ctx *ctx, int dim, int32_t *limit) {
+  SFE_REQUIRE(ctx && limit, "sfe_downsample_cta_limit: null pointer");
+  SFE_REQUIRE(dim == 2 || dim == 3, "sfe_downsample_cta_limit: points must have 2 or 3 columns (got %d)", dim);
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  int n;
+  const int rc = downsample_cta_limit(ctx, &n, dim);
+  if (rc == SFE_OK) *limit = n;
+  return rc;
+}
+
 int sfe_remove_outlier_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int dim,
                            int n_max, double radius, int min_points, float *out_pts_dev, int32_t *out_idx_dev,
                            int32_t *out_count_dev) {
@@ -353,12 +363,31 @@ int sfe_match_knn_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref
                        {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, knn, max_dist, ids_dev, dists_dev);
 }
 
-// sfe_match_host and sfe_match_knn_host (`name` in messages): one pair, results [knn][n_in]
+int sfe_match_dim_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev, const float *in_pts_dev,
+                      const int32_t *in_off_dev, int n_pairs, int dim, int n_ref_max, float max_dist, int32_t *ids_dev,
+                      float *dists_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_match_dim_dev: null context");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  return match_knn_run(ctx, ctx->stream, {ref_pts_dev, ref_off_dev, nullptr, n_ref_max},
+                       {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, 1, max_dist, ids_dev, dists_dev, dim);
+}
+
+int sfe_match_knn_dim_dev(sfe_ctx *ctx, const float *ref_pts_dev, const int32_t *ref_off_dev, const float *in_pts_dev,
+                          const int32_t *in_off_dev, int n_pairs, int dim, int n_ref_max, int knn, float max_dist,
+                          int32_t *ids_dev, float *dists_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_match_knn_dim_dev: null context");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  return match_knn_run(ctx, ctx->stream, {ref_pts_dev, ref_off_dev, nullptr, n_ref_max},
+                       {in_pts_dev, in_off_dev, nullptr, 0}, n_pairs, knn, max_dist, ids_dev, dists_dev, dim);
+}
+
+// sfe_match[_knn][_dim]_host (`name` in messages): one pair of dim-column clouds, results [knn][n_in]
 static int match_host(sfe_ctx *ctx, const char *name, const float *ref_host, int n_ref, const float *in_host, int n_in,
-                      int knn, float max_dist, int32_t *ids_host, float *dists_host) {
+                      int knn, float max_dist, int32_t *ids_host, float *dists_host, int dim = 2) {
   SFE_REQUIRE(ctx != nullptr, "%s: null context", name);
   SFE_REQUIRE(n_ref >= 0 && n_in >= 0, "%s: negative point count", name);
   SFE_REQUIRE(knn >= 1 && knn <= GRID_KNN_MAX, "%s: knn %d is not supported (1..%d)", name, knn, GRID_KNN_MAX);
+  SFE_REQUIRE(dim == 2 || dim == 3, "%s: points must have 2 or 3 columns (got %d)", name, dim);
   if (n_in == 0) return SFE_OK;
   SFE_REQUIRE(in_host && ids_host && dists_host && (ref_host || n_ref == 0), "%s: null pointer", name);
   SFE_CUDA(cudaSetDevice(ctx->device));
@@ -366,8 +395,8 @@ static int match_host(sfe_ctx *ctx, const char *name, const float *ref_host, int
   Carver cv;
   for (int pass = 0; pass < 2; ++pass) {
     cv.off = 0;
-    float *d_ref = (float *)cv.take(sizeof(float) * 2 * (size_t)(n_ref > 0 ? n_ref : 1));
-    float *d_in = (float *)cv.take(sizeof(float) * 2 * (size_t)n_in);
+    float *d_ref = (float *)cv.take(sizeof(float) * dim * (size_t)(n_ref > 0 ? n_ref : 1));
+    float *d_in = (float *)cv.take(sizeof(float) * dim * (size_t)n_in);
     int32_t *d_off = (int32_t *)cv.take(4 * sizeof(int32_t));
     int32_t *d_ids = (int32_t *)cv.take(sizeof(int32_t) * out);
     float *d_d = (float *)cv.take(sizeof(float) * out);
@@ -379,11 +408,11 @@ static int match_host(sfe_ctx *ctx, const char *name, const float *ref_host, int
     }
     const int32_t off[4] = {0, n_ref, 0, n_in};
     if (n_ref > 0)
-      SFE_CUDA(cudaMemcpyAsync(d_ref, ref_host, sizeof(float) * 2 * (size_t)n_ref, cudaMemcpyHostToDevice, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(d_in, in_host, sizeof(float) * 2 * (size_t)n_in, cudaMemcpyHostToDevice, ctx->stream));
+      SFE_CUDA(cudaMemcpyAsync(d_ref, ref_host, sizeof(float) * dim * (size_t)n_ref, cudaMemcpyHostToDevice, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_in, in_host, sizeof(float) * dim * (size_t)n_in, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_off, off, sizeof(off), cudaMemcpyHostToDevice, ctx->stream));
     int rc = match_knn_run(ctx, ctx->stream, {d_ref, d_off, nullptr, n_ref}, {d_in, d_off + 2, nullptr, n_in}, 1, knn,
-                           max_dist, d_ids, d_d);
+                           max_dist, d_ids, d_d, dim);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(ids_host, d_ids, sizeof(int32_t) * out, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(dists_host, d_d, sizeof(float) * out, cudaMemcpyDeviceToHost, ctx->stream));
@@ -400,6 +429,17 @@ int sfe_match_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *
 int sfe_match_knn_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int knn,
                        float max_dist, int32_t *ids_host, float *dists_host) {
   return match_host(ctx, "sfe_match_knn_host", ref_host, n_ref, in_host, n_in, knn, max_dist, ids_host, dists_host);
+}
+
+int sfe_match_dim_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int dim,
+                       float max_dist, int32_t *ids_host, float *dists_host) {
+  return match_host(ctx, "sfe_match_dim_host", ref_host, n_ref, in_host, n_in, 1, max_dist, ids_host, dists_host, dim);
+}
+
+int sfe_match_knn_dim_host(sfe_ctx *ctx, const float *ref_host, int n_ref, const float *in_host, int n_in, int dim,
+                           int knn, float max_dist, int32_t *ids_host, float *dists_host) {
+  return match_host(ctx, "sfe_match_knn_dim_host", ref_host, n_ref, in_host, n_in, knn, max_dist, ids_host, dists_host,
+                    dim);
 }
 
 void sfe_icp_params_default(sfe_icp_params *p) {

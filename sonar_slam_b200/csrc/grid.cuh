@@ -640,6 +640,30 @@ __device__ __forceinline__ int grid_knn_query(const GridViewT<Idx> &g, float qx,
   return k;
 }
 
+// grid_knn_query for a 3-D query (qx, qy, qz) on the grid of the points' x, y: zof(j) is the z of sorted position j, and
+// the distance is (dx*dx + dy*dy) + dz*dz, each operation rounded separately.  Adding dz*dz >= 0 never lowers the
+// rounded xy distance, so the rings' xy bound still ends the search exactly; a cloud tall in z over a small xy
+// footprint puts many points in every cell, and the search then scans those columns whole.
+template <typename Idx, typename B, typename Z>
+__device__ __forceinline__ int grid_knn_query3(const GridViewT<Idx> &g, float qx, float qy, float qz, const Z &zof,
+                                               float max_d2, int knn, float *bd, B *bi, int stride) {
+  if (g.n <= 0) return 0;
+  const int cx = grid_cell_coord(qx, g.ox, g.inv_cell, g.nx), cy = grid_cell_coord(qy, g.oy, g.inv_cell, g.ny);
+  int k = 0;
+  float kth = INFINITY;
+  knn_rings(g, qx, qy, cx, cy, kth, max_d2, [&](int s, int e) {
+    for (int j = s; j < e; ++j) {
+      const float2 t = g.pts[j];
+      const float d2xy = dist2_rn(qx - t.x, qy - t.y);
+      if (!(d2xy <= max_d2) || d2xy > kth) continue;  // the 3-D distance is at least d2xy
+      const float dz = qz - zof(j);
+      const float d2 = __fadd_rn(d2xy, __fmul_rn(dz, dz));
+      if (d2 <= max_d2 && d2 < INFINITY) knn_offer(g, d2, j, knn, bd, bi, stride, k, kth);
+    }
+  });
+  return k;
+}
+
 // ---- surface normals (point-to-plane minimiser, icp.yaml:18-19 + a SurfaceNormalDataPointsFilter{knn} on the
 // reference; statement: oracle/icp_ref.c orc_surface_normals).  For the grid point at sorted position p: its knn
 // nearest grid points (itself included) in ascending (squared distance, original index) order (knn_rings); then mean,

@@ -513,13 +513,15 @@ struct MatchBatch {
 
 // One pair's reference of nt points (nt >= 1) in match_kernel's layout: the bounding box over the CTA, the grid
 // geometry and the counting sort into sorted / cells (shared), original indices in orig.  All threads call it.
+// DIM 3: rows of x, y, z; the grid holds x, y.
+template <int DIM = 2>
 __device__ __forceinline__ void match_ref_grid(const MatchBatch &b, const float *ref, int nt, float2 *sorted,
                                                uint32_t *cells, uint16_t *orig, int *scan, float *bbox_w, float *bbox,
                                                GridView &g) {
   const int tid = threadIdx.x, nthr = blockDim.x;
   float mn_x = INFINITY, mn_y = INFINITY, mxx = -INFINITY, mxy = -INFINITY;
   for (int i = tid; i < nt; i += nthr) {
-    const float x = ref[2 * i], y = ref[2 * i + 1];
+    const float x = ref[DIM * i], y = ref[DIM * i + 1];
     mn_x = fminf(mn_x, x), mxx = fmaxf(mxx, x), mn_y = fminf(mn_y, y), mxy = fmaxf(mxy, y);
   }
 #pragma unroll
@@ -544,7 +546,7 @@ __device__ __forceinline__ void match_ref_grid(const MatchBatch &b, const float 
   }
   __syncthreads();
   grid_geometry(nt, bbox[0], bbox[1], bbox[2], bbox[3], 0.05f, g, b.max_cells);
-  grid_build(ref, 2, nt, 0.f, 0.f, g, sorted, cells, orig, scan);
+  grid_build(ref, DIM, nt, 0.f, 0.f, g, sorted, cells, orig, scan);
 }
 
 __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) {
@@ -614,7 +616,9 @@ __device__ __forceinline__ void match_knn_rows(const Idx *orig, int found, int k
 }
 
 // The in-CTA class: match_kernel's layout, then from byte list_off the best-knn lists, one column per thread
-// (distances [knn][blockDim.x], then uint16 sorted positions [knn][blockDim.x]).
+// (distances [knn][blockDim.x], then uint16 sorted positions [knn][blockDim.x]).  DIM 3: [x, y, z] clouds, any knn
+// (grid_knn_query3 on the grid of x, y; z read from the reference's rows through the original indices).
+template <int DIM>
 __global__ void __launch_bounds__(ICP_THREADS) match_knn_kernel(const MatchBatch b, int knn, int list_off) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int scan[36];
@@ -629,9 +633,9 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_kernel(const MatchBatch
   const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
   const size_t total = (size_t)b.in_off[b.P];
   for (int p = blockIdx.x; p < b.P; p += gridDim.x) {
-    const float *ref = b.ref_pts + 2 * (size_t)b.ref_off[p];
+    const float *ref = b.ref_pts + DIM * (size_t)b.ref_off[p];
     const int nt = b.ref_off[p + 1] - b.ref_off[p];
-    const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
+    const float *in = b.in_pts + DIM * (size_t)b.in_off[p];
     const int ns = b.in_off[p + 1] - b.in_off[p];
     int32_t *ids = b.ids + b.in_off[p];
     float *dists = b.dists + b.in_off[p];
@@ -642,16 +646,22 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_kernel(const MatchBatch
       continue;
     }
     GridView g;
-    match_ref_grid(b, ref, nt, sorted, cells, orig, scan, bbox_w, bbox, g);
+    match_ref_grid<DIM>(b, ref, nt, sorted, cells, orig, scan, bbox_w, bbox, g);
     for (int i = tid; i < ns; i += nthr) {
-      const int found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
+      int found;
+      if constexpr (DIM == 3)
+        found = grid_knn_query3(g, in[3 * i], in[3 * i + 1], in[3 * i + 2],
+                                [&](int j) { return ref[3 * (size_t)orig[j] + 2]; }, max_d2, knn, bd, bi, nthr);
+      else
+        found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
       match_knn_rows(orig, found, knn, bd, bi, nthr, ids + i, dists + i, total);
     }
   }
 }
 
 // The map class of knn > 1: match_map_kernel with the best-knn lists in dynamic shared memory (distances
-// [knn][blockDim.x], then int sorted positions [knn][blockDim.x]).
+// [knn][blockDim.x], then int sorted positions [knn][blockDim.x]).  DIM 3 as match_knn_kernel's.
+template <int DIM>
 __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchBatch b, int knn) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, nthr = blockDim.x;
@@ -666,10 +676,16 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
     MapGridView g;
     g.pts = b.map_pts, g.cstart = b.map_cstart + (size_t)ms * b.map_cell_cap, g.orig = b.map_orig;
     g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
-    const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
+    const float *in = b.in_pts + DIM * (size_t)b.in_off[p];
     const int ns = b.in_off[p + 1] - b.in_off[p];
+    const float *ref = b.ref_pts + DIM * (size_t)b.ref_off[p];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) {
-      const int found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
+      int found;
+      if constexpr (DIM == 3)
+        found = grid_knn_query3(g, in[3 * i], in[3 * i + 1], in[3 * i + 2],
+                                [&](int j) { return ref[3 * (size_t)g.orig[j] + 2]; }, max_d2, knn, bd, bi, nthr);
+      else
+        found = grid_knn_query(g, in[2 * i], in[2 * i + 1], max_d2, knn, bd, bi, nthr);
       match_knn_rows(g.orig, found, knn, bd, bi, nthr, b.ids + b.in_off[p] + i, b.dists + b.in_off[p] + i, total);
     }
   }
@@ -1171,12 +1187,14 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
   return SFE_OK;
 }
 
-// knn 1: match_run.  knn > 1: references whose layout fits one CTA next to the best-knn lists run in match_knn_kernel,
-// larger ones as map grids in match_knn_map_kernel, in the same call.
+// 2-D clouds, knn 1: match_run.  Otherwise (knn > 1, or [x, y, z] clouds at any knn): references whose layout fits one
+// CTA next to the best-knn lists run in match_knn_kernel, larger ones as map grids in match_knn_map_kernel, in the same
+// call; the split comes from the same limit search for both dims.
 int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, int knn,
-                       float max_dist, int32_t *ids, float *dists) {
+                       float max_dist, int32_t *ids, float *dists, int dim) {
   SFE_REQUIRE(knn >= 1 && knn <= GRID_KNN_MAX, "match: knn %d is not supported (1..%d)", knn, GRID_KNN_MAX);
-  if (knn == 1) return match_run(ctx, st, ref, in, P, max_dist, ids, dists);
+  SFE_REQUIRE(dim == 2 || dim == 3, "match: points must have 2 or 3 columns (got %d)", dim);
+  if (knn == 1 && dim == 2) return match_run(ctx, st, ref, in, P, max_dist, ids, dists);
   const int nt_max = ref.n_max;
   SFE_REQUIRE(ctx, "match: null context");
   SFE_REQUIRE(P >= 0 && nt_max >= 0, "match: negative sizes");
@@ -1185,8 +1203,9 @@ int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, c
   SFE_REQUIRE(!ref.cnt && !in.cnt, "match: per-cloud counts are not supported");
   const size_t lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(uint16_t));
   auto list_off = [](int nt) { return (match_cta_smem(nt) + 15) & ~size_t(15); };
+  const void *cta_kernel = dim == 3 ? (const void *)match_knn_kernel<3> : (const void *)match_knn_kernel<2>;
   size_t budget;
-  int rc = cta_smem_budget(ctx, (const void *)match_knn_kernel, &budget);
+  int rc = cta_smem_budget(ctx, cta_kernel, &budget);
   if (rc != SFE_OK) return rc;
   const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) { return list_off(nt) + lists; });
   MatchBatch b{};
@@ -1201,24 +1220,27 @@ int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, c
     return SFE_ERR_UNSUPPORTED;
   }
   int per_sm;
-  if ((rc = ctas_per_sm(ctx, (const void *)match_knn_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
+  if ((rc = ctas_per_sm(ctx, cta_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
   int grid = ctx->sm_count * per_sm;
   if (grid > P) grid = P;
   rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
   if (rc != SFE_OK) return rc;
   b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
-  match_knn_kernel<<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
+  if (dim == 3) match_knn_kernel<3><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
+  else match_knn_kernel<2><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   if (nt_max <= limit) return SFE_OK;
   MapWs w;
-  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, limit, P, false, true, 0, w);
+  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, dim, nullptr, P, limit, P, false, true, 0, w);
   if (rc != SFE_OK) return rc;
   b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
   b.map_cell_cap = w.cell_cap;
   const size_t map_lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(int));
-  if ((rc = ctas_per_sm(ctx, (const void *)match_knn_map_kernel, ICP_THREADS, map_lists, &per_sm)) != SFE_OK) return rc;
-  match_knn_map_kernel<<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
+  const void *map_kernel = dim == 3 ? (const void *)match_knn_map_kernel<3> : (const void *)match_knn_map_kernel<2>;
+  if ((rc = ctas_per_sm(ctx, map_kernel, ICP_THREADS, map_lists, &per_sm)) != SFE_OK) return rc;
+  if (dim == 3) match_knn_map_kernel<3><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
+  else match_knn_map_kernel<2><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;

@@ -44,6 +44,8 @@ int feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const ui
 constexpr int DS_ANY_SIZE = -1;
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
                    float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot, int counter);
+// the largest cloud of `dim` columns (2 or 3) downsample_run's one-CTA kernel lays out in shared memory on this device
+int downsample_cta_limit(const sfe_ctx *ctx, int *limit, int dim);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
 // the map class above it)
 int remove_outlier_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, double radius,
@@ -73,9 +75,9 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what);
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,
               int32_t *ids, float *dists);
 // the knn (1 .. GRID_KNN_MAX) nearest reference points of every input point: ids / dists [knn][in.off[P]], neighbour j
-// of every point in row j; knn 1 is match_run
+// of every point in row j; knn 1 of 2-D clouds is match_run.  dim 3: [x, y, z] rows in both clouds.
 int match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, int knn,
-                  float max_dist, int32_t *ids, float *dists);
+                  float max_dist, int32_t *ids, float *dists, int dim = 2);
 
 // One map grid: a cloud too large for a one-CTA layout, built once per call in global memory (map_build).
 struct MapGrid {

@@ -87,7 +87,8 @@ def _offsets(counts, device):
 
 
 def downsample(pts, off, n_max, resolution, ctx=None):
-    """Batched pcl.downsample on packed clouds (pts [total,2] f32, off [n+1] i32, cuda)."""
+    """Batched pcl.downsample on packed clouds (pts [total,2|3] f32, off [n+1] i32, cuda): the quadtree for 2 columns,
+    the octree for 3."""
     ctx = ctx or context(pts.device)
     n = off.numel() - 1
     out = torch.empty_like(pts)
@@ -96,6 +97,15 @@ def downsample(pts, off, n_max, resolution, ctx=None):
     _lib.check(ctx.lib.sfe_downsample_dev(ctx.handle, _dp(pts), _dp(off), n, int(pts.shape[1]), int(n_max),
                                           float(resolution), _dp(out), _dp(idx), _dp(cnt)), "sfe_downsample_dev")
     return dict(pts=out, idx=idx, count=cnt)
+
+
+def downsample_cta_limit(dim=2, ctx=None, device=0):
+    """The largest cloud of `dim` columns downsample() runs in one CTA on this device (sfe_downsample_cta_limit);
+    larger clouds take the grid-wide path."""
+    ctx = ctx or context(device)
+    out = np.zeros(1, np.int32)
+    _lib.check(ctx.lib.sfe_downsample_cta_limit(ctx.handle, int(dim), _lib.ptr(out)), "sfe_downsample_cta_limit")
+    return int(out[0])
 
 
 def downsample_frames(pts, off, n_max, resolution, frame_points, cnt=None, ctx=None):
@@ -134,15 +144,23 @@ def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, knn=None, ctx=N
     ids int32 and squared dists float32 [total query points].  With knn (1 .. 16, sfe_match_knn_dev): [knn, total]
     tensors whose row j holds every query's j-th nearest reference point within max_dist (-1 / +inf where there is
     none).  References of any size: those above one CTA's shared memory (whole maps) are searched as map grids in
-    global memory, with the same results."""
+    global memory, with the same results.  [total,3] points (both clouds): the 3-D distance (sfe_match_*_dim_dev)."""
     if knn is not None and int(knn) < 1:
         raise ValueError(f"ops.match: knn must be at least 1 (got {knn})")
+    dim = int(ref_pts.shape[1])
+    if dim not in (2, 3) or int(in_pts.shape[1]) != dim:
+        raise ValueError(f"ops.match: reference and query points must both have 2 or 3 columns (got {dim} and "
+                         f"{int(in_pts.shape[1])})")
     ctx = ctx or context(ref_pts.device)
     n = ref_off.numel() - 1
     shape = (in_pts.shape[0],) if knn is None else (int(knn), in_pts.shape[0])
     ids = torch.empty(shape, dtype=torch.int32, device=in_pts.device)
     d = torch.empty(shape, dtype=torch.float32, device=in_pts.device)
-    if knn is None:
+    if dim == 3:
+        _lib.check(ctx.lib.sfe_match_knn_dim_dev(ctx.handle, _dp(ref_pts), _dp(ref_off), _dp(in_pts), _dp(in_off), n, 3,
+                                                 int(n_ref_max), 1 if knn is None else int(knn), float(max_dist),
+                                                 _dp(ids), _dp(d)), "sfe_match_knn_dim_dev")
+    elif knn is None:
         _lib.check(ctx.lib.sfe_match_dev(ctx.handle, _dp(ref_pts), _dp(ref_off), _dp(in_pts), _dp(in_off), n,
                                          int(n_ref_max), float(max_dist), _dp(ids), _dp(d)), "sfe_match_dev")
     else:
