@@ -30,7 +30,8 @@ extern "C" {
                             201: + sfe_icp_params.minimizer / normals_knn (point-to-plane, icp.yaml:18-19);
                             202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch); later
                                  additions that change no existing entry point: sfe_match_dim_*, sfe_match_knn_dim_*,
-                                 sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host */
+                                 sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
+                                 sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -353,6 +354,32 @@ typedef struct {
   int n_reading, n_reference; /* 0 .. SFE_ICP_MAX_DATA_FILTERS */
   sfe_icp_data_filter reading[SFE_ICP_MAX_DATA_FILTERS], reference[SFE_ICP_MAX_DATA_FILTERS];
 } sfe_icp_filters;
+/* sfe_icp_dev, sfe_icp_host and sfe_icp_batch_host for clouds of `dim` columns; guesses and results are (dim + 1)^2
+ * row-major float32.  dim 2: the calls above, same launches and results.  dim 3: x, y, z in both clouds, libpointmatcher's
+ * 3-D point-to-point chain (oracle/icp3_ref.c): exact 3-D nearest neighbours ((dx*dx + dy*dy) + dz*dz, ties to the lower
+ * index, on a grid of x, y), the MaxDist and Trimmed weights, R = U V^T from a float32 restatement of Eigen's JacobiSVD of
+ * the 3x3 cross-covariance with the reflection fix (a planar cloud whose 2-D fit would be a reflection gets a rotation
+ * that flips z), Counter and Differential checkers on quaternions.  Same statuses and messages.  Targets above
+ * sfe_icp_cta_limit(ctx, 3, ns_max) read map grids (sfe_icp_dev's workspace, plus 4 bytes per slot point).  dim 3 with
+ * minimizer 1, flags bit 1 or ICP filters set on ctx is SFE_ERR_UNSUPPORTED, and nothing is launched; dim outside
+ * 2 .. 3 is SFE_ERR_ARG. */
+SFE_API int sfe_icp_dim_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev,
+                            const int32_t *src_off_dev, const float *tgt_pts_dev, const int32_t *tgt_off_dev,
+                            const int32_t *src_id_dev, const int32_t *tgt_id_dev, int n_problems, int dim, int ns_max,
+                            int nt_max, const float *guess_dev, float *T_dev, int32_t *iters_dev, int32_t *inliers_dev,
+                            int32_t *status_dev);
+SFE_API int sfe_icp_dim_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns,
+                             const float *tgt_host, int nt, int dim, const float *guess_host, int n_guesses,
+                             float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host);
+SFE_API int sfe_icp_batch_dim_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host,
+                                   const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
+                                   const int32_t *tgt_off_host, int n_tgt_clouds, const int32_t *src_id_host,
+                                   const int32_t *tgt_id_host, int n_problems, int dim, const float *guess_host,
+                                   float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host);
+/* *limit = the largest target of `dim` columns that sfe_icp_dim_* solves in one CTA next to sources of ns points on this
+ * context's device (dim 2: the shipped point-to-point chain without filters); larger targets take the map class */
+SFE_API int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit);
+
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
  * the default).  Checked here: no NaN, kind and dim known, counts in range; SFE_ERR_ARG leaves the setting as it was. */
 SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);

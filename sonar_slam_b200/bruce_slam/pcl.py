@@ -8,11 +8,14 @@ bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libson
     match_knn(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)         -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
         (the YAML's distance data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
+    ICP().compute(source[N,3], target[M,3], guess 4x4)          -> (message, float32[4,4])   (3-D, point-to-point)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
 float32; results are fresh float32 arrays.  Three columns are x, y, z, as fromEigen (pcl.cpp:18-50) reads them:
 downsample then builds libpointmatcher's octree instead of the quadtree, match measures 3-D distances, and the
-reference and query of a match must have the same number of columns.  ICP takes 2-column clouds only.  Not provided: density_filter (dead code in the
+reference and query of a match must have the same number of columns.  ICP registers 3-column clouds with 4x4 guesses
+through libpointmatcher's 3-D point-to-point chain (the 3-D scan matcher takes no point-to-plane minimiser and no ICP
+filters: a YAML selecting them raises NotImplementedError on 3-column input).  Not provided: density_filter (dead code in the
 reference: its only call site is commented out, feature_extraction.py:246) and
 ICP.getCovariance (never called from Python) -- both raise NotImplementedError.
 """
@@ -279,69 +282,115 @@ class ICP(object):
         res = self.compute_batch(source, target, [guess])
         return res["messages"][0], res["T"][0]
 
-    def compute_batch(self, source, target, guesses):
-        """All `guesses` (iterable of 3x3) on the same cloud pair in one launch (N1: the loop of
-        SLAM.compute_icp_with_cov, slam.py:346-358).  Returns dict(messages, T[n,3,3], iterations,
-        inliers, status).  The target may be of any size (a whole map): above one CTA's shared memory it is
-        sorted once into a grid in global memory that every guess reads, with the same results."""
+    def _dim(self, srcs, tgts):
+        """The clouds' column count (2 or 3), after the checks the reference's module and the 3-D chain make: source
+        and target with the same number of columns (TypeError), and for 3 columns a configuration the 3-D scan matcher
+        runs (NotImplementedError, before any device call)."""
         if self.params is None:
             raise RuntimeError("You must setup a matcher before running ICP")
-        src = _points(source, "source", cols=(2,))
-        tgt = _points(target, "target", cols=(2,))
-        g = np.ascontiguousarray(np.asarray(guesses, dtype=np.float32).reshape(-1, 3, 3))
-        n = len(g)
-        T = np.empty((n, 3, 3), np.float32)
-        iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
-        ctx = _lib.default_context()
-        import ctypes
-        _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
-        _lib.check(ctx.lib.sfe_icp_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), len(src), _lib.ptr(tgt),
-                                        len(tgt), _lib.ptr(g), n, _lib.ptr(T), _lib.ptr(iters), _lib.ptr(inl),
-                                        _lib.ptr(st)), "ICP.compute")
+        dims = {c.shape[1] for c in list(srcs) + list(tgts) if c.shape[1] in (2, 3)}  # (empty [0,k] arrays pass _points)
+        if len(dims) > 1:
+            raise TypeError(f"pcl: incompatible function arguments (ICP clouds have {sorted(dims)} columns; source and "
+                            "target must have the same number)")
+        dim = dims.pop() if dims else 2
+        if dim == 3:
+            if self.params.minimizer != 0:
+                raise NotImplementedError("ICP on 3-column clouds: PointToPlaneErrorMinimizer is not implemented in 3-D "
+                                          "(3-D normals and the 6x6 system); use PointToPointErrorMinimizer")
+            if self.params.flags & 2:
+                raise NotImplementedError("ICP on 3-column clouds: float64 accumulation (flags bit 1) is not implemented")
+            if _lib.icp_filters_of(self.params) is not None:
+                raise NotImplementedError("ICP on 3-column clouds: data filters and MinDist / MedianDist outlier filters "
+                                          "are not implemented in 3-D")
+        return dim
+
+    @staticmethod
+    def _guesses(guesses, dim):
+        g = np.asarray(guesses, dtype=np.float32)
+        if dim == 3 and (g.ndim < 2 or g.shape[-2:] != (4, 4)):
+            raise ValueError(f"ICP on 3-column clouds takes 4x4 guesses (got shape {list(g.shape)})")
+        return np.ascontiguousarray(g.reshape(-1, dim + 1, dim + 1))
+
+    @staticmethod
+    def _results(ctx, st):
         msgs = [ctx.lib.sfe_icp_status_message(int(s)).decode() for s in st]
         for s, m in zip(st, msgs):
             if int(s) in (5, 6):  # not ConvergenceErrors in libpointmatcher: they propagate as exceptions
                 raise RuntimeError(m)
+        return msgs
+
+    def compute_batch(self, source, target, guesses):
+        """All `guesses` (iterable of 3x3, or 4x4 for 3-column clouds) on the same cloud pair in one launch (N1: the
+        loop of SLAM.compute_icp_with_cov, slam.py:346-358).  Returns dict(messages, T[n,3,3] (or [n,4,4]),
+        iterations, inliers, status).  The target may be of any size (a whole map): above one CTA's shared memory it is
+        sorted once into a grid in global memory that every guess reads, with the same results."""
+        if self.params is None:
+            raise RuntimeError("You must setup a matcher before running ICP")
+        src = _points(source, "source")
+        tgt = _points(target, "target")
+        dim = self._dim([src], [tgt])
+        g = self._guesses(guesses, dim)
+        n = len(g)
+        T = np.empty((n, dim + 1, dim + 1), np.float32)
+        iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
+        ctx = _lib.default_context()
+        import ctypes
+        _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
+        if dim == 3:
+            _lib.check(ctx.lib.sfe_icp_dim_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), len(src),
+                                                _lib.ptr(tgt), len(tgt), 3, _lib.ptr(g), n, _lib.ptr(T),
+                                                _lib.ptr(iters), _lib.ptr(inl), _lib.ptr(st)), "ICP.compute")
+        else:
+            _lib.check(ctx.lib.sfe_icp_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), len(src),
+                                            _lib.ptr(tgt), len(tgt), _lib.ptr(g), n, _lib.ptr(T), _lib.ptr(iters),
+                                            _lib.ptr(inl), _lib.ptr(st)), "ICP.compute")
+        msgs = self._results(ctx, st)
         return dict(messages=msgs, T=T, iterations=iters, inliers=inl, status=st)
 
     def compute_pairs(self, sources, targets, guesses):
-        """Many cloud pairs, each with its own guesses, in ONE launch (sfe_icp_batch_host): pair k aligns sources[k]
-        to targets[k] from every 3x3 in guesses[k].  Returns a list with compute_batch's dict for every pair."""
+        """Many cloud pairs, each with its own guesses, in ONE launch (sfe_icp_batch_host, or sfe_icp_batch_dim_host
+        for 3-column clouds): pair k aligns sources[k] to targets[k] from every 3x3 (4x4) in guesses[k].  Returns a
+        list with compute_batch's dict for every pair."""
         if self.params is None:
             raise RuntimeError("You must setup a matcher before running ICP")
-        srcs = [_points(s, "source", cols=(2,)) for s in sources]
-        tgts = [_points(t, "target", cols=(2,)) for t in targets]
-        gs = [np.asarray(g, dtype=np.float32).reshape(-1, 3, 3) for g in guesses]
-        if not (len(srcs) == len(tgts) == len(gs)):
+        srcs = [_points(s, "source") for s in sources]
+        tgts = [_points(t, "target") for t in targets]
+        if not (len(srcs) == len(tgts) == len(guesses)):
             raise ValueError("sources, targets and guesses must have one entry per pair")
+        dim = self._dim(srcs, tgts)
+        gs = [self._guesses(g, dim) for g in guesses]
         counts = np.array([len(g) for g in gs], np.int64)
         n = int(counts.sum())
         if n == 0:
-            return [dict(messages=[], T=np.empty((0, 3, 3), np.float32), iterations=np.zeros(0, np.int32),
+            return [dict(messages=[], T=np.empty((0, dim + 1, dim + 1), np.float32), iterations=np.zeros(0, np.int32),
                          inliers=np.zeros(0, np.int32), status=np.zeros(0, np.int32)) for _ in gs]
 
         def packed(clouds):
             off = np.zeros(len(clouds) + 1, np.int32)
             off[1:] = np.cumsum([len(c) for c in clouds])
-            return np.ascontiguousarray(np.concatenate(clouds + [np.zeros((0, 2), np.float32)]), np.float32), off
+            return np.ascontiguousarray(np.concatenate(clouds + [np.zeros((0, dim), np.float32)]), np.float32), off
 
         src, soff = packed(srcs)
         tgt, toff = packed(tgts)
         ids = np.ascontiguousarray(np.repeat(np.arange(len(gs), dtype=np.int32), counts))
         g = np.ascontiguousarray(np.concatenate(gs))
-        T = np.empty((n, 3, 3), np.float32)
+        T = np.empty((n, dim + 1, dim + 1), np.float32)
         iters, inl, st = (np.zeros(n, np.int32) for _ in range(3))
         ctx = _lib.default_context()
         import ctypes
         _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
-        _lib.check(ctx.lib.sfe_icp_batch_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), _lib.ptr(soff),
-                                              len(srcs), _lib.ptr(tgt), _lib.ptr(toff), len(tgts), _lib.ptr(ids),
-                                              _lib.ptr(ids), n, _lib.ptr(g), _lib.ptr(T), _lib.ptr(iters),
-                                              _lib.ptr(inl), _lib.ptr(st)), "ICP.compute_pairs")
-        msgs = [ctx.lib.sfe_icp_status_message(int(s)).decode() for s in st]
-        for s, m in zip(st, msgs):
-            if int(s) in (5, 6):  # as in compute_batch: not ConvergenceErrors, they propagate as exceptions
-                raise RuntimeError(m)
+        if dim == 3:
+            _lib.check(ctx.lib.sfe_icp_batch_dim_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src),
+                                                      _lib.ptr(soff), len(srcs), _lib.ptr(tgt), _lib.ptr(toff),
+                                                      len(tgts), _lib.ptr(ids), _lib.ptr(ids), n, 3, _lib.ptr(g),
+                                                      _lib.ptr(T), _lib.ptr(iters), _lib.ptr(inl), _lib.ptr(st)),
+                       "ICP.compute_pairs")
+        else:
+            _lib.check(ctx.lib.sfe_icp_batch_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), _lib.ptr(soff),
+                                                  len(srcs), _lib.ptr(tgt), _lib.ptr(toff), len(tgts), _lib.ptr(ids),
+                                                  _lib.ptr(ids), n, _lib.ptr(g), _lib.ptr(T), _lib.ptr(iters),
+                                                  _lib.ptr(inl), _lib.ptr(st)), "ICP.compute_pairs")
+        msgs = self._results(ctx, st)
         out, a = [], 0
         for c in counts:
             b = a + int(c)

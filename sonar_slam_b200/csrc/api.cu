@@ -506,44 +506,62 @@ int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host,
                             guess_host, T_host, iters_host, inliers_host, status_host);
 }
 
-int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host, const int32_t *src_off_host,
-                       int n_src_clouds, const float *tgt_pts_host, const int32_t *tgt_off_host, int n_tgt_clouds,
-                       const int32_t *src_id_host, const int32_t *tgt_id_host, int n_problems, const float *guess_host,
-                       float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
-  SFE_REQUIRE(ctx && prm, "sfe_icp_batch_host: null context or parameters");
-  SFE_REQUIRE(n_src_clouds >= 1 && n_tgt_clouds >= 1 && n_problems >= 0, "sfe_icp_batch_host: bad sizes");
+// sfe_icp[_batch]_dim_host's checks for dim 3, before anything is copied or launched: what the 3-D chain does not have
+static int icp3_supported(const sfe_ctx *ctx, const sfe_icp_params *prm, const char *name) {
+  const char *what = prm->minimizer != 0     ? "the point-to-plane error minimizer"
+                     : (prm->flags & 2)      ? "float64 accumulation (flags bit 1)"
+                     : ctx->has_icp_filters ? "ICP filters (sfe_icp_set_filters)"
+                                             : nullptr;
+  if (!what) return SFE_OK;
+  set_error("%s: %s is not supported on [x, y, z] clouds by the 3-D scan matcher", name, what);
+  return SFE_ERR_UNSUPPORTED;
+}
+
+// sfe_icp_batch_host and sfe_icp_batch_dim_host (`name` in messages): clouds of `dim` columns, (dim + 1)^2 guesses
+static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *prm, const float *src_pts_host,
+                          const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
+                          const int32_t *tgt_off_host, int n_tgt_clouds, const int32_t *src_id_host,
+                          const int32_t *tgt_id_host, int n_problems, int dim, const float *guess_host, float *T_host,
+                          int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
+  SFE_REQUIRE(ctx && prm, "%s: null context or parameters", name);
+  SFE_REQUIRE(dim == 2 || dim == 3, "%s: points must have 2 or 3 columns (got %d)", name, dim);
+  if (dim == 3) {
+    const int rc = icp3_supported(ctx, prm, name);
+    if (rc != SFE_OK) return rc;
+  }
+  SFE_REQUIRE(n_src_clouds >= 1 && n_tgt_clouds >= 1 && n_problems >= 0, "%s: bad sizes", name);
   if (n_problems == 0) return SFE_OK;
   SFE_REQUIRE(src_off_host && tgt_off_host && src_id_host && tgt_id_host && guess_host && T_host && iters_host &&
                   inliers_host && status_host,
-              "sfe_icp_batch_host: null pointer");
+              "%s: null pointer", name);
   int ns_max = 0, nt_max = 0;
   for (int c = 0; c < n_src_clouds; ++c) {
-    SFE_REQUIRE(src_off_host[c + 1] >= src_off_host[c], "sfe_icp_batch_host: source offsets decrease at %d", c);
+    SFE_REQUIRE(src_off_host[c + 1] >= src_off_host[c], "%s: source offsets decrease at %d", name, c);
     ns_max = std::max(ns_max, src_off_host[c + 1] - src_off_host[c]);
   }
   for (int c = 0; c < n_tgt_clouds; ++c) {
-    SFE_REQUIRE(tgt_off_host[c + 1] >= tgt_off_host[c], "sfe_icp_batch_host: target offsets decrease at %d", c);
+    SFE_REQUIRE(tgt_off_host[c + 1] >= tgt_off_host[c], "%s: target offsets decrease at %d", name, c);
     nt_max = std::max(nt_max, tgt_off_host[c + 1] - tgt_off_host[c]);
   }
-  SFE_REQUIRE(src_off_host[0] == 0 && tgt_off_host[0] == 0, "sfe_icp_batch_host: offsets must start at 0");
+  SFE_REQUIRE(src_off_host[0] == 0 && tgt_off_host[0] == 0, "%s: offsets must start at 0", name);
   const int ns = src_off_host[n_src_clouds], nt = tgt_off_host[n_tgt_clouds];
-  SFE_REQUIRE((src_pts_host || ns == 0) && (tgt_pts_host || nt == 0), "sfe_icp_batch_host: null cloud pointer");
+  SFE_REQUIRE((src_pts_host || ns == 0) && (tgt_pts_host || nt == 0), "%s: null cloud pointer", name);
   for (int p = 0; p < n_problems; ++p)
     SFE_REQUIRE(src_id_host[p] >= 0 && src_id_host[p] < n_src_clouds && tgt_id_host[p] >= 0 &&
                     tgt_id_host[p] < n_tgt_clouds,
-                "sfe_icp_batch_host: problem %d names cloud %d / %d", p, src_id_host[p], tgt_id_host[p]);
+                "%s: problem %d names cloud %d / %d", name, p, src_id_host[p], tgt_id_host[p]);
   SFE_CUDA(cudaSetDevice(ctx->device));
-  const size_t P = (size_t)n_problems;
+  const size_t P = (size_t)n_problems, TS = (size_t)(dim + 1) * (dim + 1);
   Carver cv;
   for (int pass = 0; pass < 2; ++pass) {
     cv.off = 0;
-    float *d_src = (float *)cv.take(sizeof(float) * 2 * (size_t)(ns > 0 ? ns : 1));
-    float *d_tgt = (float *)cv.take(sizeof(float) * 2 * (size_t)(nt > 0 ? nt : 1));
+    float *d_src = (float *)cv.take(sizeof(float) * dim * (size_t)(ns > 0 ? ns : 1));
+    float *d_tgt = (float *)cv.take(sizeof(float) * dim * (size_t)(nt > 0 ? nt : 1));
     int32_t *d_soff = (int32_t *)cv.take(sizeof(int32_t) * (size_t)(n_src_clouds + 1));
     int32_t *d_toff = (int32_t *)cv.take(sizeof(int32_t) * (size_t)(n_tgt_clouds + 1));
     int32_t *d_ids = (int32_t *)cv.take(sizeof(int32_t) * 2 * P);
-    float *d_guess = (float *)cv.take(sizeof(float) * 9 * P);
-    float *d_T = (float *)cv.take(sizeof(float) * 9 * P);
+    float *d_guess = (float *)cv.take(sizeof(float) * TS * P);
+    float *d_T = (float *)cv.take(sizeof(float) * TS * P);
     int32_t *d_res = (int32_t *)cv.take(sizeof(int32_t) * 3 * P);
     if (pass == 0) {
       int rc = ensure(ctx, ctx->stage_in[1], cv.off);
@@ -552,28 +570,88 @@ int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src
       continue;
     }
     if (ns > 0)
-      SFE_CUDA(cudaMemcpyAsync(d_src, src_pts_host, sizeof(float) * 2 * (size_t)ns, cudaMemcpyHostToDevice, ctx->stream));
+      SFE_CUDA(cudaMemcpyAsync(d_src, src_pts_host, sizeof(float) * dim * (size_t)ns, cudaMemcpyHostToDevice,
+                               ctx->stream));
     if (nt > 0)
-      SFE_CUDA(cudaMemcpyAsync(d_tgt, tgt_pts_host, sizeof(float) * 2 * (size_t)nt, cudaMemcpyHostToDevice, ctx->stream));
+      SFE_CUDA(cudaMemcpyAsync(d_tgt, tgt_pts_host, sizeof(float) * dim * (size_t)nt, cudaMemcpyHostToDevice,
+                               ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_soff, src_off_host, sizeof(int32_t) * (size_t)(n_src_clouds + 1), cudaMemcpyHostToDevice,
                              ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_toff, tgt_off_host, sizeof(int32_t) * (size_t)(n_tgt_clouds + 1), cudaMemcpyHostToDevice,
                              ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_ids, src_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(d_ids + P, tgt_id_host, sizeof(int32_t) * P, cudaMemcpyHostToDevice, ctx->stream));
-    SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * 9 * P, cudaMemcpyHostToDevice, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(d_guess, guess_host, sizeof(float) * TS * P, cudaMemcpyHostToDevice, ctx->stream));
     IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
                    d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
     pb.n_tgt_clouds = n_tgt_clouds, pb.n_src_clouds = n_src_clouds;
-    int rc = icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr, ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+    int rc = dim == 3 ? icp3_run(ctx, ctx->stream, prm, pb)
+                      : icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr,
+                                ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
     if (rc != SFE_OK) return rc;
-    SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * 9 * P, cudaMemcpyDeviceToHost, ctx->stream));
+    SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * TS * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(inliers_host, d_res + P, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(status_host, d_res + 2 * P, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   return SFE_OK;
+}
+
+int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host, const int32_t *src_off_host,
+                       int n_src_clouds, const float *tgt_pts_host, const int32_t *tgt_off_host, int n_tgt_clouds,
+                       const int32_t *src_id_host, const int32_t *tgt_id_host, int n_problems, const float *guess_host,
+                       float *T_host, int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
+  return icp_batch_host(ctx, "sfe_icp_batch_host", prm, src_pts_host, src_off_host, n_src_clouds, tgt_pts_host,
+                        tgt_off_host, n_tgt_clouds, src_id_host, tgt_id_host, n_problems, 2, guess_host, T_host,
+                        iters_host, inliers_host, status_host);
+}
+
+int sfe_icp_batch_dim_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host,
+                           const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
+                           const int32_t *tgt_off_host, int n_tgt_clouds, const int32_t *src_id_host,
+                           const int32_t *tgt_id_host, int n_problems, int dim, const float *guess_host, float *T_host,
+                           int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
+  return icp_batch_host(ctx, "sfe_icp_batch_dim_host", prm, src_pts_host, src_off_host, n_src_clouds, tgt_pts_host,
+                        tgt_off_host, n_tgt_clouds, src_id_host, tgt_id_host, n_problems, dim, guess_host, T_host,
+                        iters_host, inliers_host, status_host);
+}
+
+int sfe_icp_dim_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host, int ns, const float *tgt_host,
+                     int nt, int dim, const float *guess_host, int n_guesses, float *T_host, int32_t *iters_host,
+                     int32_t *inliers_host, int32_t *status_host) {
+  SFE_REQUIRE(ns >= 0 && nt >= 0 && n_guesses >= 0, "sfe_icp_dim_host: negative size");
+  if (n_guesses == 0) return SFE_OK;
+  const int32_t src_off[2] = {0, ns}, tgt_off[2] = {0, nt};
+  std::vector<int32_t> zero((size_t)n_guesses, 0);
+  return icp_batch_host(ctx, "sfe_icp_dim_host", prm, src_host, src_off, 1, tgt_host, tgt_off, 1, zero.data(),
+                        zero.data(), n_guesses, dim, guess_host, T_host, iters_host, inliers_host, status_host);
+}
+
+int sfe_icp_dim_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev, const int32_t *src_off_dev,
+                    const float *tgt_pts_dev, const int32_t *tgt_off_dev, const int32_t *src_id_dev,
+                    const int32_t *tgt_id_dev, int n_problems, int dim, int ns_max, int nt_max, const float *guess_dev,
+                    float *T_dev, int32_t *iters_dev, int32_t *inliers_dev, int32_t *status_dev) {
+  SFE_REQUIRE(ctx != nullptr && prm != nullptr, "sfe_icp_dim_dev: null context or parameters");
+  SFE_REQUIRE(dim == 2 || dim == 3, "sfe_icp_dim_dev: points must have 2 or 3 columns (got %d)", dim);
+  if (dim == 2)
+    return sfe_icp_dev(ctx, prm, src_pts_dev, src_off_dev, tgt_pts_dev, tgt_off_dev, src_id_dev, tgt_id_dev, n_problems,
+                       ns_max, nt_max, guess_dev, T_dev, iters_dev, inliers_dev, status_dev);
+  const int rc = icp3_supported(ctx, prm, "sfe_icp_dim_dev");
+  if (rc != SFE_OK) return rc;
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  return icp3_run(ctx, ctx->stream, prm,
+                  {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
+                   tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev});
+}
+
+int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit) {
+  SFE_REQUIRE(ctx && limit, "sfe_icp_cta_limit: null pointer");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  int n;
+  const int rc = icp_cta_limit(ctx, dim, ns, &n);
+  if (rc == SFE_OK) *limit = n;
+  return rc;
 }
 
 }  // extern "C"

@@ -1011,7 +1011,22 @@ static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *p
   return SFE_OK;
 }
 
+// The largest target icp_kernel's layout holds next to sources of ns points (the map class takes larger ones)
+static int icp2_limit(const sfe_ctx *ctx, int ns, bool plane, bool filt, int *limit) {
+  ns = ns > 0 ? ns : 1;
+  size_t budget;
+  int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget, false, filt);
+  if (rc != SFE_OK) return rc;
+  int mc;
+  *limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
+    return icp_cta_smem(ns, nt, plane, budget, &mc);
+  });
+  return SFE_OK;
+}
+
 }  // namespace sfe
+
+#include "icp3.cuh"
 
 // Size classes: every listed class gets a launch laid out for it, whose smaller shared-memory footprint fits more
 // CTAs per SM, and a last launch, laid out for the capacities src.n_max x tgt.n_max, takes the problems that fit none
@@ -1117,15 +1132,9 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.P = pb.P;
   if (!classes) {
     // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
-    const int ns = ns_max > 0 ? ns_max : 1;
-    const bool plane = prm->minimizer == 1;
-    size_t budget;
-    int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget, false, filt_on);
+    int limit;
+    int rc = icp2_limit(ctx, ns_max, prm->minimizer == 1, filt_on, &limit);
     if (rc != SFE_OK) return rc;
-    int mc;
-    const int limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
-      return icp_cta_smem(ns, nt, plane, budget, &mc);
-    });
     if (nt_max <= limit) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
     if (limit > 0) {
       b.class_mode = 1;
@@ -1136,6 +1145,99 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap, filt_on);
   }
   return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
+}
+
+int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
+  SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
+  SFE_REQUIRE(ns >= 0 && ns <= 65535, "icp: sources of %d points are not supported (0..65535)", ns);
+  return dim == 2 ? icp2_limit(ctx, ns, false, false, limit) : icp3_limit(ctx, ns > 0 ? ns : 1, limit);
+}
+
+// [x, y, z] clouds: targets up to icp3_limit in icp3_kernel (one CTA, its grid in shared memory), larger ones as map
+// grids (map_build with dim 3, plus their z by sorted position) in icp3_map_kernel, in the same call.
+int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb) {
+  const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
+  SFE_REQUIRE(ctx && prm, "icp (3-D): null context or parameters");
+  SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp (3-D): negative sizes");
+  if (prm->minimizer != 0 || (prm->flags & 2)) {
+    set_error("icp (3-D): %s is not supported on [x, y, z] clouds (point-to-point with float32 sums only)",
+              prm->minimizer != 0 ? "the point-to-plane error minimizer" : "float64 accumulation (flags bit 1)");
+    return SFE_ERR_UNSUPPORTED;
+  }
+  SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
+  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
+              ICP_HIST - 1);
+  SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
+                  !std::isnan(prm->trim_ratio) && !std::isnan(prm->min_diff_rot) && !std::isnan(prm->min_diff_trans),
+              "icp: a NaN parameter (maxDist, ratio or minDiff*) is not supported");
+  SFE_REQUIRE(prm->trim_ratio <= 1.0f, "icp: TrimmedDistOutlierFilter ratio %g is above 1", (double)prm->trim_ratio);
+  if (pb.P == 0) return SFE_OK;
+  SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
+                  pb.status,
+              "icp (3-D): null pointer");
+  SFE_REQUIRE(!pb.src.cnt && !pb.tgt.cnt, "icp (3-D): per-cloud counts are not supported");
+  SFE_REQUIRE(ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d)", ns_max);
+  const int ns = ns_max > 0 ? ns_max : 1;
+  int limit;
+  int rc = icp3_limit(ctx, ns, &limit);
+  if (rc != SFE_OK) return rc;
+  Icp3Batch b{};
+  b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
+  b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
+  b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
+  b.P = pb.P, b.ns_max = ns, b.prm = *prm;
+  const bool map = nt_max > limit;
+  const size_t map_smem = icp3_map_smem(ns);
+  if ((map && map_smem > (size_t)ctx->max_smem_optin) || (limit == 0 && !map)) {
+    set_error("icp (3-D): sources of %d points need %zu B of shared memory per CTA (limit %d)", ns_max, map_smem,
+              ctx->max_smem_optin);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
+  // SCR_ICP: [work counters][in-CTA orig_ws][map class: z by map-grid position][z mean per slot]
+  size_t cta_smem = 0, orig_bytes = 0;
+  int cta_grid = 0, nt_cta = std::min(nt_max, limit);
+  if (limit > 0) {
+    size_t budget;
+    if ((rc = cta_smem_budget(ctx, (const void *)icp3_kernel, &budget)) != SFE_OK) return rc;
+    cta_smem = icp3_cta_smem(ns, nt_cta > 0 ? nt_cta : 1, budget, &b.max_cells);
+    int per_sm;
+    if ((rc = ctas_per_sm(ctx, (const void *)icp3_kernel, ICP3_THREADS, cta_smem, &per_sm)) != SFE_OK) return rc;
+    cta_grid = std::min(ctx->sm_count * per_sm, pb.P);
+    orig_bytes = ((size_t)cta_grid * (nt_cta > 0 ? nt_cta : 1) * sizeof(uint16_t) + 255) & ~size_t(255);
+  }
+  const size_t z_bytes = map ? (((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255)) : 0;
+  rc = ensure(ctx, ctx->scratch[SCR_ICP], 256 + orig_bytes + z_bytes + (map ? sizeof(float) * (size_t)slot_cap : 0), st);
+  if (rc != SFE_OK) return rc;
+  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
+  int *counters = (int *)base;
+  if (cta_grid < pb.P || map) SFE_CUDA(cudaMemsetAsync(counters, 0, 2 * sizeof(int), st));
+  if (limit > 0) {
+    b.nt_max = nt_cta > 0 ? nt_cta : 1, b.class_nt = b.nt_max;
+    b.orig_ws = (uint16_t *)(base + 256);
+    b.next = cta_grid < pb.P ? counters : nullptr;
+    icp3_kernel<<<cta_grid, ICP3_THREADS, cta_smem, st>>>(b);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  if (!map) return SFE_OK;
+  MapWs w;
+  rc = map_build(ctx, st, {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, pb.P, limit, slot_cap, true, true, 0, w);
+  if (rc != SFE_OK) return rc;
+  float *zs = (float *)(base + 256 + orig_bytes), *zm = (float *)(base + 256 + orig_bytes + z_bytes);
+  icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
+  int per_sm;
+  if ((rc = ctas_per_sm(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, &per_sm)) != SFE_OK) return rc;
+  const int grid = std::min(ctx->sm_count * per_sm, pb.P);
+  b.next = grid < pb.P ? counters + 1 : nullptr;
+  const IcpMapArgs m{w.slot, w.grid, w.pts, w.cstart, w.orig, nullptr, w.cell_cap};
+  icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, m);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return SFE_OK;
 }
 
 // References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in

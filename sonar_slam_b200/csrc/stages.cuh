@@ -70,6 +70,13 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpP
             int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr);
 // SFE_OK, or SFE_ERR_ARG with a message naming `what`: NaN, unknown kind, dim outside -1 .. 1, counts out of range
 int icp_filters_check(const sfe_icp_filters *f, const char *what);
+// icp_run on [x, y, z] clouds (icp3.cuh; statement oracle/icp3_ref.c): guess and T_out are [P][16] row-major 4x4,
+// point-to-point with float32 sums only (SFE_ERR_UNSUPPORTED otherwise); no counts, classes or filters.  Targets above
+// icp_cta_limit(ctx, 3, ns) read map grids, with the same results.
+int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb);
+// *limit = the largest target of `dim` columns that icp_run (dim 2: shipped point-to-point chain, no filters) or
+// icp3_run (dim 3) solves in one CTA next to sources of ns points; larger targets take the map class
+int icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit);
 // nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,

@@ -177,20 +177,42 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
 
     Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
     map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources: at most 65 535
-    points and what fits shared memory (about 7 000)."""
+    points and what fits shared memory (about 7 000).
+    [total,3] points (both clouds) with [P,4,4] guesses: the 3-D point-to-point chain (sfe_icp_dim_dev), which takes no
+    filters, point-to-plane or float64 accumulation."""
+    cols = [int(a.shape[1]) if a.dim() == 2 else 0 for a in (src_pts, tgt_pts)]
+    dim = 3 if 3 in cols else 2
+    if dim == 3 and cols != [3, 3]:
+        raise ValueError(f"ops.icp: source and target points must have the same number of columns (got {cols})")
+    if dim == 3 and (guess.dim() != 3 or tuple(guess.shape[1:]) != (4, 4)):
+        raise ValueError(f"ops.icp: 3-column points take [P,4,4] guesses (got {list(guess.shape)})")
     ctx = ctx or context(src_pts.device)
     prm = params or _lib.IcpParams()
     guess = guess.contiguous()
     P = guess.shape[0]
-    T = torch.empty((P, 3, 3), dtype=torch.float32, device=guess.device)
+    T = torch.empty((P, dim + 1, dim + 1), dtype=torch.float32, device=guess.device)
     iters = torch.empty((P,), dtype=torch.int32, device=guess.device)
     inl = torch.empty_like(iters)
     st = torch.empty_like(iters)
     _lib.set_icp_filters(ctx, _lib.icp_filters_of(prm, filters))
-    _lib.check(ctx.lib.sfe_icp_dev(ctx.handle, ctypes.byref(prm), _dp(src_pts), _dp(src_off), _dp(tgt_pts),
-                                   _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, int(ns_max), int(nt_max), _dp(guess),
-                                   _dp(T), _dp(iters), _dp(inl), _dp(st)), "sfe_icp_dev")
+    if dim == 3:
+        _lib.check(ctx.lib.sfe_icp_dim_dev(ctx.handle, ctypes.byref(prm), _dp(src_pts), _dp(src_off), _dp(tgt_pts),
+                                           _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, 3, int(ns_max), int(nt_max),
+                                           _dp(guess), _dp(T), _dp(iters), _dp(inl), _dp(st)), "sfe_icp_dim_dev")
+    else:
+        _lib.check(ctx.lib.sfe_icp_dev(ctx.handle, ctypes.byref(prm), _dp(src_pts), _dp(src_off), _dp(tgt_pts),
+                                       _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, int(ns_max), int(nt_max), _dp(guess),
+                                       _dp(T), _dp(iters), _dp(inl), _dp(st)), "sfe_icp_dev")
     return dict(T=T, iterations=iters, inliers=inl, status=st)
+
+
+def icp_cta_limit(dim, ns, ctx=None, device=0):
+    """The largest target of `dim` columns icp() solves in one CTA next to sources of ns points on this device
+    (sfe_icp_cta_limit; dim 2: the shipped point-to-point chain without filters); larger targets take the map class."""
+    ctx = ctx or context(device)
+    out = np.zeros(1, np.int32)
+    _lib.check(ctx.lib.sfe_icp_cta_limit(ctx.handle, int(dim), int(ns), _lib.ptr(out)), "sfe_icp_cta_limit")
+    return int(out[0])
 
 
 def mincovdet(samples, n, subsets, float32=False, ctx=None):

@@ -114,6 +114,71 @@ def se2(x, y, theta):
     return np.array([[c, -s, x], [s, c, y], [0.0, 0.0, 1.0]])
 
 
+def se3(t, axis, angle):
+    """4x4 rigid transform: rotation by `angle` about the unit vector along `axis` (Rodrigues), then translation t."""
+    k = np.asarray(axis, np.float64)
+    k = k / np.linalg.norm(k)
+    K = np.array([[0.0, -k[2], k[1]], [k[2], 0.0, -k[0]], [-k[1], k[0], 0.0]])
+    T = np.eye(4)
+    T[:3, :3] = np.eye(3) + np.sin(angle) * K + (1.0 - np.cos(angle)) * (K @ K)
+    T[:3, 3] = t
+    return T
+
+
+def make_icp_pair3(seed, n_source=2000, n_target=20000, extent=60.0, outlier_frac=0.2, max_t=1.0, max_rot=0.1,
+                   sensor_range=30.0, half_aperture_deg=65.0, height=4.0, max_tilt=0.3):
+    """Config-3 pair in 3-D: make_icp_pair's scene with walls `height` metres tall over an undulating floor.  Returns
+    (source[N_s,3] f32, target[N_t,3] f32, T_gt 4x4 f64).
+
+    target: wall and floor samples (sigma 0.03 m in x, y and z; a quarter on the floor), thinned on a 0.15 m voxel
+            grid, in a frame centred on the sensor pose;
+    source: wall and floor samples inside the sonar wedge (sigma 0.05 m) with `outlier_frac` outliers uniform in the wedge and
+            in height, expressed in a frame displaced by T_gt^-1, so that T_gt maps source onto target.  T_gt turns by
+            up to `max_rot` rad about an axis tilted up to `max_tilt` rad from z, and moves up to `max_t` m per axis.
+    """
+    rng = np.random.default_rng(seed)
+    n_seg = max(6, int(48 * n_target / 20000))
+    walls = make_walls(rng, n_segments=n_seg, extent=extent, min_len=15.0, max_len=50.0)
+
+    def sample(n, sigma):  # wall points, and a quarter on an undulating floor (it pins z and the tilt)
+        nf = n // 4
+        xy = sample_walls(rng, walls, n - nf, sigma)
+        walls_z = rng.uniform(0.0, height, n - nf)
+        fxy = rng.uniform(0.0, extent, (nf, 2))
+        floor_z = 0.4 * np.sin(fxy[:, 0] / 7.0) * np.cos(fxy[:, 1] / 5.0)
+        return np.r_[np.c_[xy, walls_z], np.c_[fxy, floor_z]] + rng.normal(0.0, sigma, (n, 3))
+
+    tgt = sample(4 * n_target, 0.03)
+    keys = np.floor(tgt / 0.15).astype(np.int64)
+    _, first = np.unique((keys[:, 0] * 1000003 + keys[:, 1]) * 1000003 + keys[:, 2], return_index=True)
+    tgt = tgt[np.sort(first)]
+    rng.shuffle(tgt)
+    tgt = tgt[:n_target]
+    pose = se2(rng.uniform(0.3, 0.5) * extent, rng.uniform(0.3, 0.7) * extent, rng.uniform(-0.5, 0.5))
+    inv = np.linalg.inv(pose)
+    to_sensor = lambda p: np.c_[p[:, :2] @ inv[:2, :2].T + inv[:2, 2], p[:, 2]]
+    tgt_s = to_sensor(tgt)
+    cand = to_sensor(sample(40 * n_source, 0.05))
+    r = np.hypot(cand[:, 0], cand[:, 1])
+    b = np.arctan2(cand[:, 1], cand[:, 0])
+    cand = cand[(r < sensor_range) & (r > 0.5) & (np.abs(b) < np.deg2rad(half_aperture_deg))]
+    n_in = int(round(n_source * (1.0 - outlier_frac)))
+    if len(cand) < n_in:  # sparse view: pad with resampled structure points
+        pad = cand[rng.integers(0, len(cand), n_in - len(cand))] if len(cand) else rng.uniform(-5, 5, (n_in, 3))
+        cand = np.concatenate([cand, pad + rng.normal(0, 0.05, pad.shape)])
+    src = cand[:n_in]
+    rr = rng.uniform(0.5, sensor_range, n_source - n_in)
+    bb = rng.uniform(-1, 1, n_source - n_in) * np.deg2rad(half_aperture_deg)
+    src = np.concatenate([src, np.c_[rr * np.cos(bb), rr * np.sin(bb), rng.uniform(0.0, height, n_source - n_in)]])
+    rng.shuffle(src)
+    tilt, az = rng.uniform(0.0, max_tilt), rng.uniform(0.0, 2 * np.pi)
+    axis = [np.sin(tilt) * np.cos(az), np.sin(tilt) * np.sin(az), np.cos(tilt)]
+    T_gt = se3(rng.uniform(-max_t, max_t, 3), axis, rng.uniform(-max_rot, max_rot))
+    Ti = np.linalg.inv(T_gt)
+    src = src @ Ti[:3, :3].T + Ti[:3, 3]
+    return src.astype(np.float32), tgt_s.astype(np.float32), T_gt
+
+
 def make_icp_pair(seed, n_source=2000, n_target=20000, extent=60.0, outlier_frac=0.2,
                   max_t=1.0, max_rot=0.1, sensor_range=30.0, half_aperture_deg=65.0):
     """Config-3 pair.  Returns (source[N_s,2] f32, target[N_t,2] f32, T_gt 3x3 f64).
