@@ -506,17 +506,6 @@ int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_host,
                             guess_host, T_host, iters_host, inliers_host, status_host);
 }
 
-// sfe_icp[_batch]_dim_host's checks for dim 3, before anything is copied or launched: what the 3-D chain does not have
-static int icp3_supported(const sfe_ctx *ctx, const sfe_icp_params *prm, const char *name) {
-  const char *what = prm->minimizer != 0     ? "the point-to-plane error minimizer"
-                     : (prm->flags & 2)      ? "float64 accumulation (flags bit 1)"
-                     : ctx->has_icp_filters ? "ICP filters (sfe_icp_set_filters)"
-                                             : nullptr;
-  if (!what) return SFE_OK;
-  set_error("%s: %s is not supported on [x, y, z] clouds by the 3-D scan matcher", name, what);
-  return SFE_ERR_UNSUPPORTED;
-}
-
 // sfe_icp_batch_host and sfe_icp_batch_dim_host (`name` in messages): clouds of `dim` columns, (dim + 1)^2 guesses
 static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *prm, const float *src_pts_host,
                           const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
@@ -525,10 +514,9 @@ static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *
                           int32_t *iters_host, int32_t *inliers_host, int32_t *status_host) {
   SFE_REQUIRE(ctx && prm, "%s: null context or parameters", name);
   SFE_REQUIRE(dim == 2 || dim == 3, "%s: points must have 2 or 3 columns (got %d)", name, dim);
-  if (dim == 3) {
-    const int rc = icp3_supported(ctx, prm, name);
-    if (rc != SFE_OK) return rc;
-  }
+  const sfe_icp_filters *filt = ctx->has_icp_filters ? &ctx->icp_filters : nullptr;
+  const int rc = icp_params_check(prm, dim, filt, name);  // (before anything is copied)
+  if (rc != SFE_OK) return rc;
   SFE_REQUIRE(n_src_clouds >= 1 && n_tgt_clouds >= 1 && n_problems >= 0, "%s: bad sizes", name);
   if (n_problems == 0) return SFE_OK;
   SFE_REQUIRE(src_off_host && tgt_off_host && src_id_host && tgt_id_host && guess_host && T_host && iters_host &&
@@ -585,9 +573,8 @@ static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *
     IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
                    d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
     pb.n_tgt_clouds = n_tgt_clouds, pb.n_src_clouds = n_src_clouds;
-    int rc = dim == 3 ? icp3_run(ctx, ctx->stream, prm, pb)
-                      : icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr,
-                                ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+    int rc = dim == 3 ? icp3_run(ctx, ctx->stream, prm, pb, filt)
+                      : icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr, filt);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * TS * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
@@ -637,12 +624,11 @@ int sfe_icp_dim_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pt
   if (dim == 2)
     return sfe_icp_dev(ctx, prm, src_pts_dev, src_off_dev, tgt_pts_dev, tgt_off_dev, src_id_dev, tgt_id_dev, n_problems,
                        ns_max, nt_max, guess_dev, T_dev, iters_dev, inliers_dev, status_dev);
-  const int rc = icp3_supported(ctx, prm, "sfe_icp_dim_dev");
-  if (rc != SFE_OK) return rc;
   SFE_CUDA(cudaSetDevice(ctx->device));
   return icp3_run(ctx, ctx->stream, prm,
                   {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
-                   tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev});
+                   tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev},
+                  ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
 }
 
 int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit) {

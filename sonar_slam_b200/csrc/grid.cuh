@@ -12,6 +12,7 @@
 // product and the sum rounded separately; ties go to the lowest ORIGINAL index.
 #pragma once
 #include "common.cuh"
+#include "stages.cuh"
 
 namespace sfe {
 
@@ -30,6 +31,15 @@ struct GridViewT {
 };
 using GridView = GridViewT<uint16_t>;
 using MapGridView = GridViewT<int>;
+
+// the grid of map slot `slot` (map_build)
+__device__ __forceinline__ MapGridView map_grid_view(const MapArgs &m, int slot) {
+  const MapGrid &mg = m.grid[slot];
+  MapGridView g;
+  g.pts = m.pts, g.cstart = m.cstart + (size_t)slot * m.cell_cap, g.orig = m.orig;
+  g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
+  return g;
+}
 
 __device__ __forceinline__ float dist2_rn(float dx, float dy) {
   return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));

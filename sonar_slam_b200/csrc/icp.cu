@@ -81,17 +81,6 @@ struct IcpBatch {
   const int *gate_src_cnt, *gate_tgt_cnt;
 };
 
-// The map class (icp_map_kernel): problem p reads its target from the grid in slot map_slot[p] (map_build)
-struct IcpMapArgs {
-  const int *map_slot;
-  const MapGrid *map_grid;
-  const float2 *map_pts;   // centred points of every slot, sorted by (slot, cell)
-  const int *map_cstart;   // [slot][map_cell_cap]: absolute position in map_pts of every cell's first point
-  const int *map_orig;     // sorted position -> index in the target cloud
-  const float2 *map_nrm;   // point-to-plane: normal at every sorted position
-  int map_cell_cap;
-};
-
 
 // Per-phase cycle counts (development build, -DSFE_ICP_PHASE_CLOCKS; tools/build_icp_variants.sh, tools/icp_phases.py):
 // thread 0 of every CTA reads clock64() at the phase boundaries below and adds its totals to a global array when the
@@ -380,49 +369,7 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const Pos 
   return s;
 }
 
-// One instantiation per CTA size so that the register budget follows the launch shape (a single
-// __launch_bounds__(512) build capped the 128-thread class at 64 registers and spilled).
-// PLANE: errorMinimizer = PointToPlaneErrorMinimizer (sfe_icp_params.minimizer 1); a separate instantiation so that
-// the shipped point-to-point kernels keep their register allocation.
-// MAP: the target is a map grid in global memory (icp_map_kernel): no set-up per problem, 32-bit target positions,
-// and shared memory holds IcpShared and the source arrays only.
-// The kernel body lives in icp_kernel_body.cuh and is included into both kernels below, so that each kernel's code is
-// the body itself: behind a device-function wrapper the shipped instantiations compiled with larger stack frames.  The
-// body reads `MAP` (a value-dependent constant, so the other class's branches are discarded per instantiation) and,
-// in the map class, the map arguments `mp`.
-// FILT (icp_filt_kernel, icp_map_filt_kernel): the batch runs sfe_icp_filters -- the MinDist / MedianDist outlier filters
-// and the min_points gate on the clouds before the data filters; kernels of their own, so that the shipped ones keep
-// their code and register allocation.
-template <int THREADS, int MINB, bool PLANE>
-__global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b) {
-  constexpr bool MAP = THREADS < 0;  // false
-  constexpr bool FILT = THREADS < 0;  // false
-  constexpr IcpMapArgs mp{};         // (named by the discarded map-class branches only)
 #include "icp_kernel_body.cuh"
-}
-
-template <int THREADS, int MINB, bool PLANE>
-__global__ void __launch_bounds__(THREADS, MINB) icp_filt_kernel(const IcpBatch b) {
-  constexpr bool MAP = THREADS < 0;  // false
-  constexpr bool FILT = THREADS > 0;  // true
-  constexpr IcpMapArgs mp{};
-#include "icp_kernel_body.cuh"
-}
-
-// the map class: every problem's target is a map grid (map_build); one instantiation per CTA size
-template <int THREADS, int MINB, bool PLANE>
-__global__ void __launch_bounds__(THREADS, MINB) icp_map_kernel(const IcpBatch b, const IcpMapArgs mp) {
-  constexpr bool MAP = THREADS > 0;  // true
-  constexpr bool FILT = THREADS < 0;  // false
-#include "icp_kernel_body.cuh"
-}
-
-template <int THREADS, int MINB, bool PLANE>
-__global__ void __launch_bounds__(THREADS, MINB) icp_map_filt_kernel(const IcpBatch b, const IcpMapArgs mp) {
-  constexpr bool MAP = THREADS > 0;  // true
-  constexpr bool FILT = THREADS > 0;  // true
-#include "icp_kernel_body.cuh"
-}
 
 // Data filters of sfe_icp_filters (MaxDist / MinDistDataPointsFilter): cloud c of a batch (cloud id[c], or c with id
 // null) -> its survivors, in input order, at out_pts + 2 * c * n_max; out_off[c] = c * n_max, out_cnt[c] = their number,
@@ -503,12 +450,7 @@ struct MatchBatch {
   int32_t *ids;  // [total queries]
   float *dists;
   uint16_t *orig_ws;
-  // map class (match_map_kernel): pair p reads its reference from the grid in slot map_slot[p] (map_build)
-  const int *map_slot;
-  const MapGrid *map_grid;
-  const float2 *map_pts;
-  const int *map_cstart, *map_orig;
-  int map_cell_cap;
+  MapArgs map;  // map class (match_map_kernel): pair p reads its reference from the grid in slot map.slot[p]
 };
 
 // One pair's reference of nt points (nt >= 1) in match_kernel's layout: the bounding box over the CTA, the grid
@@ -587,12 +529,9 @@ __global__ void __launch_bounds__(ICP_THREADS) match_kernel(const MatchBatch b) 
 __global__ void __launch_bounds__(ICP_THREADS) match_map_kernel(const MatchBatch b) {
   const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
   for (int p = 0; p < b.P; ++p) {
-    const int ms = b.map_slot[p];
+    const int ms = b.map.slot[p];
     if (ms < 0) continue;
-    const MapGrid &mg = b.map_grid[ms];
-    MapGridView g;
-    g.pts = b.map_pts, g.cstart = b.map_cstart + (size_t)ms * b.map_cell_cap, g.orig = b.map_orig;
-    g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
+    const MapGridView g = map_grid_view(b.map, ms);
     const float *in = b.in_pts + 2 * (size_t)b.in_off[p];
     const int ns = b.in_off[p + 1] - b.in_off[p];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) {
@@ -670,12 +609,9 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
   const float max_d2 = __fmul_rn(b.max_dist, b.max_dist);
   const size_t total = (size_t)b.in_off[b.P];
   for (int p = 0; p < b.P; ++p) {
-    const int ms = b.map_slot[p];
+    const int ms = b.map.slot[p];
     if (ms < 0) continue;
-    const MapGrid &mg = b.map_grid[ms];
-    MapGridView g;
-    g.pts = b.map_pts, g.cstart = b.map_cstart + (size_t)ms * b.map_cell_cap, g.orig = b.map_orig;
-    g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
+    const MapGridView g = map_grid_view(b.map, ms);
     const float *in = b.in_pts + DIM * (size_t)b.in_off[p];
     const int ns = b.in_off[p + 1] - b.in_off[p];
     const float *ref = b.ref_pts + DIM * (size_t)b.ref_off[p];
@@ -692,6 +628,30 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
 }
 
 // ---------------------------------------------------------------------------- host side
+int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what) {
+  if (dim == 3 && (prm->minimizer != 0 || (prm->flags & 2) || filt)) {
+    set_error("%s: %s is not supported on [x, y, z] clouds by the 3-D scan matcher", what,
+              prm->minimizer != 0 ? "the point-to-plane error minimizer"
+              : (prm->flags & 2)  ? "float64 accumulation (flags bit 1)"
+                                  : "ICP filters (sfe_icp_set_filters)");
+    return SFE_ERR_UNSUPPORTED;
+  }
+  SFE_REQUIRE(prm->max_iterations >= 1, "%s: maxIterationCount must be >= 1", what);
+  SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "%s: unknown error minimizer %d", what, prm->minimizer);
+  SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
+              "%s: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", what, prm->normals_knn,
+              GRID_KNN_MAX);
+  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "%s: smoothLength %d is not supported (at most %d)", what,
+              prm->smooth_length, ICP_HIST - 1);
+  SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
+                  !std::isnan(prm->trim_ratio) && !std::isnan(prm->min_diff_rot) && !std::isnan(prm->min_diff_trans),
+              "%s: a NaN parameter (maxDist, ratio or minDiff*) is not supported", what);
+  // (the quantile element floor(n * ratio) lies past the sorted distances for a ratio above 1)
+  SFE_REQUIRE(prm->trim_ratio <= 1.0f, "%s: TrimmedDistOutlierFilter ratio %g is above 1", what,
+              (double)prm->trim_ratio);
+  return filt ? icp_filters_check(filt, what) : SFE_OK;
+}
+
 int icp_filters_check(const sfe_icp_filters *f, const char *what) {
   SFE_REQUIRE(!std::isnan(f->min_dist) && !std::isnan(f->median_factor),
               "%s: a NaN MinDist / MedianDist outlier filter setting is not supported", what);
@@ -719,19 +679,24 @@ static int pick_max_cells(int nt_max) {
   return c;
 }
 
-// Shared memory of icp_kernel's layout for problems of up to ns_max x nt_max points (both >= 1) after big problems
-// traded cell-table entries (coarser cells) for room; *max_cells receives the table's size.
-static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, size_t budget, int *max_cells) {
+// Shared memory of icp_kernel's layout for sources of up to ns_max points (>= 1).  In-CTA class: targets of up to
+// nt_max points (>= 1), 16-bit target positions, after big problems traded cell-table entries (coarser cells) for room;
+// *max_cells receives the table's size.  Map class: 32-bit target positions and no target arrays (*max_cells 0).
+static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, bool map, size_t budget, int *max_cells) {
   const bool use_order = ns_max > 1024;
+  const size_t pos = map ? sizeof(int) : sizeof(uint16_t);  // match[] and prev[]
   auto smem_for = [&](int mc) {
-    return ((sizeof(IcpShared) + 15) & ~size_t(15)) + sizeof(float2) * (size_t)nt_max +
-           sizeof(uint32_t) * (size_t)((mc + 2) / 2 + 1) + 8 + sizeof(float2) * (size_t)ns_max +
-           sizeof(float) * (size_t)ns_max + 2 * sizeof(uint16_t) * (size_t)ns_max + (size_t)ns_max + 4 +
-           sizeof(float) * (size_t)ns_max + (use_order ? sizeof(uint16_t) * (size_t)ns_max : 0) + 16 +
-           (plane && ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
+    return ((sizeof(IcpShared) + 15) & ~size_t(15)) +
+           (map ? 0 : sizeof(float2) * (size_t)nt_max + sizeof(uint32_t) * (size_t)((mc + 2) / 2 + 1)) + 8 +
+           sizeof(float2) * (size_t)ns_max + sizeof(float) * (size_t)ns_max + 2 * pos * (size_t)ns_max +
+           (size_t)ns_max + 4 + sizeof(float) * (size_t)ns_max + (use_order ? sizeof(uint16_t) * (size_t)ns_max : 0) +
+           16 + (plane && ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
   };
-  int mc = pick_max_cells(nt_max);
-  while (smem_for(mc) > budget && mc > nt_max / 4 + 256) mc -= mc / 8;
+  int mc = 0;
+  if (!map) {
+    mc = pick_max_cells(nt_max);
+    while (smem_for(mc) > budget && mc > nt_max / 4 + 256) mc -= mc / 8;
+  }
   *max_cells = mc;
   return smem_for(mc);
 }
@@ -744,29 +709,37 @@ static size_t match_cta_smem(int nt_max) {
 // (chosen on the config-4 replay for ~360-point sources; not re-measured on H100)
 static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 1536 ? 256 : ICP_THREADS); }
 
-// icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget).
-// 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers.  dense (icp_run's classes):
-// 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get them (IcpClass::dense).
-// filt: icp_filt_kernel's instantiation instead (sfe_icp_filters)
-template <int THREADS, int MINB>
+// icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget), then
+// the flags.  In-CTA class: 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers;
+// dense (icp_run's classes): 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get
+// them (IcpClass::dense).  Map class: one instantiation per CTA size.  filt: sfe_icp_filters.
+template <int THREADS, int MINB, bool MAP>
 static const void *icp_kernel_of(bool plane, bool filt) {
-  if (filt) return plane ? (const void *)icp_filt_kernel<THREADS, MINB, true> : (const void *)icp_filt_kernel<THREADS, MINB, false>;
-  return plane ? (const void *)icp_kernel<THREADS, MINB, true> : (const void *)icp_kernel<THREADS, MINB, false>;
+  if (filt)
+    return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true>
+                 : (const void *)icp_kernel<THREADS, MINB, false, MAP, true>;
+  return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, false>
+               : (const void *)icp_kernel<THREADS, MINB, false, MAP, false>;
 }
 
-static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense = false, bool filt = false) {
-  if (threads == 128 && dense) return icp_kernel_of<128, 8>(plane, filt);
-  if (threads == 128) return icp_kernel_of<128, 7>(plane, filt);
-  if (threads == 256) return icp_kernel_of<256, 4>(plane, filt);
-  if (smem <= 110 * 1024) return icp_kernel_of<512, 2>(plane, filt);
-  return icp_kernel_of<512, 1>(plane, filt);
+static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool map) {
+  if (map) {
+    if (threads == 128) return icp_kernel_of<128, 7, true>(plane, filt);
+    if (threads == 256) return icp_kernel_of<256, 4, true>(plane, filt);
+    return icp_kernel_of<512, 1, true>(plane, filt);
+  }
+  if (threads == 128 && dense) return icp_kernel_of<128, 8, false>(plane, filt);
+  if (threads == 128) return icp_kernel_of<128, 7, false>(plane, filt);
+  if (threads == 256) return icp_kernel_of<256, 4, false>(plane, filt);
+  if (smem <= 110 * 1024) return icp_kernel_of<512, 2, false>(plane, filt);
+  return icp_kernel_of<512, 1, false>(plane, filt);
 }
 
 // Shared memory icp_kernel's layouts may take next to sources of ns_max points: the budget of the instantiation that
 // runs the largest of them.
-static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, size_t *budget, bool dense = false,
-                          bool filt = false) {
-  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense, filt), budget);
+static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, bool dense, bool filt, bool map,
+                          size_t *budget) {
+  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense, filt, map), budget);
 }
 
 static void icp_tuning(IcpBatch &b) {
@@ -786,16 +759,19 @@ static void icp_tuning(IcpBatch &b) {
 }
 
 // One launch of icp_kernel over the batch, laid out for problems of up to ns_max x nt_max points in `threads`-thread
-// CTAs: sized by icp_plan, its workspace (orig_ws, nrm_ws) placed and the kernel enqueued by icp_enqueue.
+// CTAs: sized by icp_plan, its workspace (orig_ws, nrm_ws) placed and the kernel enqueued by icp_enqueue.  The map
+// class (icp_plan's map) reads its targets through m, which the caller sets after map_build; in-CTA launches leave m
+// zero.
 struct IcpLaunch {
   IcpBatch b;
+  MapArgs m;
   const void *fn;
   int threads, grid;
   size_t smem, orig_bytes, ws_bytes;
 };
 
 static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max, int threads,
-                    IcpLaunch &L, bool dense = false) {
+                    IcpLaunch &L, bool dense = false, bool map = false) {
   b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
   b.use_order = b.ns_max > 1024;
   b.cell_scale = 1.0f;
@@ -804,15 +780,18 @@ static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_
   const bool plane = prm->minimizer == 1, filt = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f ||
                                                    b.median_factor >= 0.f;
   size_t budget;
-  int rc = icp_cta_budget(ctx, threads, plane, &budget, dense, filt);
+  int rc = icp_cta_budget(ctx, threads, plane, dense, filt, map, &budget);
   if (rc != SFE_OK) return rc;
-  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, budget, &b.max_cells);
+  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, map, budget, &b.max_cells);
   if (smem > budget) {
-    set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, nt_max, smem,
-              budget);
+    if (map)
+      set_error("icp: sources of %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, smem, budget);
+    else
+      set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, nt_max,
+                smem, budget);
     return SFE_ERR_UNSUPPORTED;
   }
-  const void *fn = icp_kernel_for(threads, smem, plane, dense, filt);
+  const void *fn = icp_kernel_for(threads, smem, plane, dense, filt, map);
   int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
   if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
 #ifdef SFE_ICP_PHASE_CLOCKS
@@ -820,11 +799,11 @@ static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_
 #endif
   int grid = ctx->sm_count * per_sm;
   if (grid > b.P) grid = b.P;
-  int slots = grid;
-  if (per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
+  int slots = map ? 0 : grid;  // (the map class has no per-CTA workspace)
+  if (!map && per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
   L.orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
   L.ws_bytes = L.orig_bytes + (plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0);
-  L.b = b, L.fn = fn, L.threads = threads, L.grid = grid, L.smem = smem;
+  L.b = b, L.m = {}, L.fn = fn, L.threads = threads, L.grid = grid, L.smem = smem;
   return SFE_OK;
 }
 
@@ -834,18 +813,15 @@ static int icp_enqueue(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L, char *ws, in
   b.orig_ws = (uint16_t *)ws;
   b.nrm_ws = b.prm.minimizer == 1 ? (float2 *)(ws + L.orig_bytes) : nullptr;
   if (!b.slot_by_smid && (L.grid < b.P || b.list)) b.next = next;  // persistent CTAs; a list is always walked so
-  void *args[] = {(void *)&b};
+  void *args[] = {(void *)&b, (void *)&L.m};
   SFE_CUDA(cudaLaunchKernel(L.fn, dim3(L.grid), dim3(L.threads), args, L.smem, st));
   ctx->launches++;
   return SFE_OK;
 }
 
-// One launch over the batch in icp_threads' CTAs; b.class_mode is its size class.
-static int icp_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max) {
-  IcpLaunch L;
-  int rc = icp_plan(ctx, prm, b, ns_max, nt_max, icp_threads(ns_max > 0 ? ns_max : 1), L);
-  if (rc != SFE_OK) return rc;
-  rc = ensure(ctx, ctx->scratch[SCR_ICP], L.ws_bytes, st);
+// icp_run's launches without classes: L's workspace at scratch[SCR_ICP], its work counter WORK_ICP
+static int icp_launch(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L) {
+  int rc = ensure(ctx, ctx->scratch[SCR_ICP], L.ws_bytes, st);
   if (rc != SFE_OK) return rc;
   if (!L.b.slot_by_smid && L.grid < L.b.P) SFE_CUDA(cudaMemsetAsync(ctx->work + WORK_ICP, 0, sizeof(int), st));
   return icp_enqueue(ctx, st, L, (char *)ctx->scratch[SCR_ICP].ptr, ctx->work + WORK_ICP);
@@ -956,71 +932,71 @@ static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *
   return SFE_OK;
 }
 
-// The map class: problems whose target has more than `limit` points, their targets read from map grids.  Shared memory
-// holds IcpShared and the source arrays only.
-static int icp_map_launch(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max,
-                          int limit, int slot_cap, bool filt) {
-  const bool plane = prm->minimizer == 1;
-  MapWs w;
-  int rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, limit, slot_cap, true,
-                     (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
-  if (rc != SFE_OK) return rc;
-  b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max;
-  b.use_order = b.ns_max > 1024;
-  b.cell_scale = 1.0f;
-  b.prm = *prm;
-  icp_tuning(b);
-  // the other problems are the in-CTA launch's; with no in-CTA launch (limit 0) this one takes all of them (targets of
-  // 0 points are then reported here, SFE_ICP_EMPTY_REF, before any map grid is read)
-  b.class_mode = limit > 0 ? 2 : 0, b.class_ns = b.ns_max, b.class_nt = limit;
-  IcpMapArgs m{w.slot, w.grid, w.pts, w.cstart, w.orig, w.nrm, w.cell_cap};
-  const size_t ns = (size_t)b.ns_max;
-  const size_t smem = ((sizeof(IcpShared) + 15) & ~size_t(15)) + 8 + ns * (sizeof(float2) + 4 * sizeof(float)) + ns +
-                      4 + (b.use_order ? sizeof(uint16_t) * ns : 0) + 16 +
-                      (plane && b.ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
-  if (smem > (size_t)ctx->max_smem_optin) {
-    set_error("icp: sources of %d points need %zu B of shared memory per CTA (limit %d)", ns_max, smem,
-              ctx->max_smem_optin);
-    return SFE_ERR_UNSUPPORTED;
-  }
-  const int threads = icp_threads(b.ns_max);
-  const void *fn = plane ? (threads == 128   ? (const void *)icp_map_kernel<128, 7, true>
-                            : threads == 256 ? (const void *)icp_map_kernel<256, 4, true>
-                                             : (const void *)icp_map_kernel<512, 1, true>)
-                         : (threads == 128   ? (const void *)icp_map_kernel<128, 7, false>
-                            : threads == 256 ? (const void *)icp_map_kernel<256, 4, false>
-                                             : (const void *)icp_map_kernel<512, 1, false>);
-  if (filt)
-    fn = plane ? (threads == 128   ? (const void *)icp_map_filt_kernel<128, 7, true>
-                  : threads == 256 ? (const void *)icp_map_filt_kernel<256, 4, true>
-                                   : (const void *)icp_map_filt_kernel<512, 1, true>)
-               : (threads == 128   ? (const void *)icp_map_filt_kernel<128, 7, false>
-                  : threads == 256 ? (const void *)icp_map_filt_kernel<256, 4, false>
-                                   : (const void *)icp_map_filt_kernel<512, 1, false>);
-  int per_sm;
-  if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
-  int grid = ctx->sm_count * per_sm;
-  if (grid > b.P) grid = b.P;
-  if (grid < b.P) {  // persistent CTAs
-    b.next = ctx->work + WORK_ICP;
-    SFE_CUDA(cudaMemsetAsync(b.next, 0, sizeof(int), st));
-  }
-  void *args[] = {(void *)&b, (void *)&m};
-  SFE_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(threads), args, smem, st));
-  ctx->launches++;
-  return SFE_OK;
-}
-
 // The largest target icp_kernel's layout holds next to sources of ns points (the map class takes larger ones)
 static int icp2_limit(const sfe_ctx *ctx, int ns, bool plane, bool filt, int *limit) {
   ns = ns > 0 ? ns : 1;
   size_t budget;
-  int rc = icp_cta_budget(ctx, icp_threads(ns), plane, &budget, false, filt);
+  int rc = icp_cta_budget(ctx, icp_threads(ns), plane, false, filt, false, &budget);
   if (rc != SFE_OK) return rc;
   int mc;
   *limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
-    return icp_cta_smem(ns, nt, plane, budget, &mc);
+    return icp_cta_smem(ns, nt, plane, false, budget, &mc);
   });
+  return SFE_OK;
+}
+
+
+// A persistent launch of fn over P problems: ctas_per_sm CTAs per SM, at most one per problem
+static int persistent_grid(sfe_ctx *ctx, const void *fn, int threads, size_t smem, int P, int *grid) {
+  int per_sm;
+  const int rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm);
+  if (rc != SFE_OK) return rc;
+  *grid = std::min(ctx->sm_count * per_sm, P);
+  return SFE_OK;
+}
+
+// The one-CTA kernel of split_run: fn (null: no one-CTA launch) in `threads`-thread CTAs with `smem` bytes of layout
+// for targets of up to nt points (>= 1); counted: it takes its problems from a work counter when its grid is smaller
+// than P.
+struct SplitCta {
+  const void *fn;
+  int threads;
+  size_t smem;
+  int nt;
+  bool counted;
+};
+
+// One call of P problems split at `limit` target points (icp3_run, match_run, match_knn_run): the one-CTA kernel takes
+// the targets of up to `limit` points in a persistent launch (persistent_grid), each CTA with a row of c.nt original
+// indices (orig_ws); when the largest target, tgt.n_max, is above the limit, map_build builds map grids of the larger
+// targets (`dim` columns; problem p's target tgt_id[p], or p with tgt_id null; slot_cap distinct ones; centred or not)
+// and the map class reads them.  Workspace, scratch[SCR_ICP]: [two work counters][orig_ws][the map class's `extra`
+// bytes]; with c.counted both counters are zeroed whenever a launch may take problems from them.
+// cta(grid, orig_ws, next) enqueues the one-CTA kernel (next: its work counter, or null);
+// map(MapWs, extra workspace, next) enqueues the map class, last its map kernel (next: the second work counter) and
+// returns an SFE_* code.
+template <typename Cta, typename Map>
+static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, int limit, const PackedClouds &tgt,
+                     int dim, const int *tgt_id, int slot_cap, bool center, size_t extra, Cta cta, Map map) {
+  const bool map_class = tgt.n_max > limit;
+  int grid = 0, rc;
+  if (c.fn && (rc = persistent_grid(ctx, c.fn, c.threads, c.smem, P, &grid)) != SFE_OK) return rc;
+  const size_t head = 256, orig_bytes = ((size_t)grid * c.nt * sizeof(uint16_t) + 255) & ~size_t(255);
+  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP], head + orig_bytes + (map_class ? extra : 0), st)) != SFE_OK) return rc;
+  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
+  int *next = (int *)base;
+  if (c.counted && (grid < P || map_class)) SFE_CUDA(cudaMemsetAsync(next, 0, 2 * sizeof(int), st));
+  if (c.fn) {
+    cta(grid, (uint16_t *)(base + head), c.counted && grid < P ? next : nullptr);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  if (!map_class) return SFE_OK;
+  MapWs w;
+  if ((rc = map_build(ctx, st, tgt, dim, tgt_id, P, limit, slot_cap, center, true, 0, w)) != SFE_OK) return rc;
+  if ((rc = map(w, base + head + orig_bytes, next + 1)) != SFE_OK) return rc;
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
   return SFE_OK;
 }
 
@@ -1032,7 +1008,7 @@ static int icp2_limit(const sfe_ctx *ctx, int ns, bool plane, bool filt, int *li
 // CTAs per SM, and a last launch, laid out for the capacities src.n_max x tgt.n_max, takes the problems that fit none
 // (and reports oversize ones, SFE_ICP_TOO_LARGE).  Without classes one launch takes every problem (IcpBatch::class_mode
 // 0) -- unless the largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit
-// (class_mode 1) and the map class (map grids in global memory, icp_map_kernel) takes the rest.
+// (class_mode 1) and the map class (map grids in global memory, icp_kernel's MAP instantiations) takes the rest.
 namespace sfe {
 // Data filters: the clouds of one side of the batch, compacted into scratch[SCR_ICP_FILTER] (icp_data_filter_kernel),
 // once per cloud when the cloud count is known (no ids: one per problem), else once per problem (the ids then name the
@@ -1076,21 +1052,8 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   const bool classes = n_classes > 0;
   SFE_REQUIRE(ns_max <= 65535 && (nt_max <= 65535 || !classes),
               "icp: clouds of more than 65535 points are not supported (got %d, %d)", ns_max, nt_max);
-  SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
-  SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "icp: unknown error minimizer %d", prm->minimizer);
-  SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
-              "icp: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", prm->normals_knn, GRID_KNN_MAX);
-  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
-              ICP_HIST - 1);
-  SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
-                  !std::isnan(prm->trim_ratio) && !std::isnan(prm->min_diff_rot) && !std::isnan(prm->min_diff_trans),
-              "icp: a NaN parameter (maxDist, ratio or minDiff*) is not supported");
-  // (the quantile element floor(n * ratio) lies past the sorted distances for a ratio above 1)
-  SFE_REQUIRE(prm->trim_ratio <= 1.0f, "icp: TrimmedDistOutlierFilter ratio %g is above 1", (double)prm->trim_ratio);
-  if (filt) {
-    int rc = icp_filters_check(filt, "icp");
-    if (rc != SFE_OK) return rc;
-  }
+  int rc = icp_params_check(prm, 2, filt, "icp");
+  if (rc != SFE_OK) return rc;
   const int *gate_src = nullptr, *gate_tgt = nullptr;
   if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
     IcpDataFilters rd{filt->n_reading, {}}, rf{filt->n_reference, {}};
@@ -1099,16 +1062,16 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     for (int pass = 0; pass < 2; ++pass) {
       IcpProblems q = pb;
       if (rd.n > 0) {
-        int rc = icp_filter_side(ctx, st, rd, q.src, q.src_id, q.n_src_clouds, q.P, cv, gate_src);
+        rc = icp_filter_side(ctx, st, rd, q.src, q.src_id, q.n_src_clouds, q.P, cv, gate_src);
         if (rc != SFE_OK) return rc;
       }
       if (rf.n > 0) {
-        int rc = icp_filter_side(ctx, st, rf, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv, gate_tgt);
+        rc = icp_filter_side(ctx, st, rf, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv, gate_tgt);
         if (rc != SFE_OK) return rc;
         if (q.tgt_id != pb.tgt_id) q.n_tgt_clouds = q.P;  // one compacted target per problem
       }
       if (pass == 0) {
-        int rc = ensure(ctx, ctx->scratch[SCR_ICP_FILTER], cv.off, st);
+        rc = ensure(ctx, ctx->scratch[SCR_ICP_FILTER], cv.off, st);
         if (rc != SFE_OK) return rc;
         cv.base = (char *)ctx->scratch[SCR_ICP_FILTER].ptr, cv.off = 0;
       } else {
@@ -1123,28 +1086,38 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     b.median_factor = filt->median_factor;
     b.gate_src_cnt = gate_src, b.gate_tgt_cnt = gate_tgt;
   }
-  const bool filt_on = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;
   b.raw_cnt = pb.raw_cnt, b.raw_cap = pb.raw_cap;
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P;
-  if (!classes) {
-    // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
-    int limit;
-    int rc = icp2_limit(ctx, ns_max, prm->minimizer == 1, filt_on, &limit);
-    if (rc != SFE_OK) return rc;
-    if (nt_max <= limit) return icp_launch(ctx, st, prm, b, ns_max, nt_max);
-    if (limit > 0) {
-      b.class_mode = 1;
-      rc = icp_launch(ctx, st, prm, b, ns_max, limit);
-      if (rc != SFE_OK) return rc;
-    }
-    const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-    return icp_map_launch(ctx, st, prm, b, ns_max, nt_max, limit, slot_cap, filt_on);
+  if (classes) return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
+  // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
+  const bool plane = prm->minimizer == 1;
+  const int ns = ns_max > 0 ? ns_max : 1, threads = icp_threads(ns);
+  int limit;
+  rc = icp2_limit(ctx, ns, plane, b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f,
+                  &limit);
+  if (rc != SFE_OK) return rc;
+  IcpLaunch L;
+  if (nt_max <= limit || limit > 0) {
+    b.class_mode = nt_max <= limit ? 0 : 1;
+    if ((rc = icp_plan(ctx, prm, b, ns_max, std::min(nt_max, limit), threads, L)) != SFE_OK) return rc;
+    if ((rc = icp_launch(ctx, st, L)) != SFE_OK) return rc;
   }
-  return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
+  if (nt_max <= limit) return SFE_OK;
+  // the map class takes the other problems; with no in-CTA launch (limit 0) all of them (targets of 0 points are then
+  // reported here, SFE_ICP_EMPTY_REF, before any map grid is read)
+  b.class_mode = limit > 0 ? 2 : 0, b.class_ns = ns, b.class_nt = limit;
+  if ((rc = icp_plan(ctx, prm, b, ns_max, nt_max, threads, L, false, true)) != SFE_OK) return rc;
+  const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
+  MapWs w;
+  rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, limit, slot_cap, true,
+                 (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
+  if (rc != SFE_OK) return rc;
+  L.m = w.args();
+  return icp_launch(ctx, st, L);
 }
 
 int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
@@ -1155,22 +1128,13 @@ int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
 
 // [x, y, z] clouds: targets up to icp3_limit in icp3_kernel (one CTA, its grid in shared memory), larger ones as map
 // grids (map_build with dim 3, plus their z by sorted position) in icp3_map_kernel, in the same call.
-int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb) {
+int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
+                  const sfe_icp_filters *filt) {
   const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
   SFE_REQUIRE(ctx && prm, "icp (3-D): null context or parameters");
   SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp (3-D): negative sizes");
-  if (prm->minimizer != 0 || (prm->flags & 2)) {
-    set_error("icp (3-D): %s is not supported on [x, y, z] clouds (point-to-point with float32 sums only)",
-              prm->minimizer != 0 ? "the point-to-plane error minimizer" : "float64 accumulation (flags bit 1)");
-    return SFE_ERR_UNSUPPORTED;
-  }
-  SFE_REQUIRE(prm->max_iterations >= 1, "icp: maxIterationCount must be >= 1");
-  SFE_REQUIRE(prm->smooth_length < ICP_HIST, "icp: smoothLength %d is not supported (at most %d)", prm->smooth_length,
-              ICP_HIST - 1);
-  SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
-                  !std::isnan(prm->trim_ratio) && !std::isnan(prm->min_diff_rot) && !std::isnan(prm->min_diff_trans),
-              "icp: a NaN parameter (maxDist, ratio or minDiff*) is not supported");
-  SFE_REQUIRE(prm->trim_ratio <= 1.0f, "icp: TrimmedDistOutlierFilter ratio %g is above 1", (double)prm->trim_ratio);
+  int rc = icp_params_check(prm, 3, filt, "icp (3-D)");
+  if (rc != SFE_OK) return rc;
   if (pb.P == 0) return SFE_OK;
   SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
                   pb.status,
@@ -1179,8 +1143,7 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
   SFE_REQUIRE(ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d)", ns_max);
   const int ns = ns_max > 0 ? ns_max : 1;
   int limit;
-  int rc = icp3_limit(ctx, ns, &limit);
-  if (rc != SFE_OK) return rc;
+  if ((rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
   Icp3Batch b{};
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
@@ -1194,50 +1157,36 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
     return SFE_ERR_UNSUPPORTED;
   }
   const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-  // SCR_ICP: [work counters][in-CTA orig_ws][map class: z by map-grid position][z mean per slot]
-  size_t cta_smem = 0, orig_bytes = 0;
-  int cta_grid = 0, nt_cta = std::min(nt_max, limit);
+  const int nt_cta = std::min(nt_max, limit);
+  b.nt_max = nt_cta > 0 ? nt_cta : 1, b.class_nt = b.nt_max;
+  size_t cta_smem = 0;
   if (limit > 0) {
     size_t budget;
     if ((rc = cta_smem_budget(ctx, (const void *)icp3_kernel, &budget)) != SFE_OK) return rc;
-    cta_smem = icp3_cta_smem(ns, nt_cta > 0 ? nt_cta : 1, budget, &b.max_cells);
-    int per_sm;
-    if ((rc = ctas_per_sm(ctx, (const void *)icp3_kernel, ICP3_THREADS, cta_smem, &per_sm)) != SFE_OK) return rc;
-    cta_grid = std::min(ctx->sm_count * per_sm, pb.P);
-    orig_bytes = ((size_t)cta_grid * (nt_cta > 0 ? nt_cta : 1) * sizeof(uint16_t) + 255) & ~size_t(255);
+    cta_smem = icp3_cta_smem(ns, b.nt_max, budget, &b.max_cells);
   }
-  const size_t z_bytes = map ? (((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255)) : 0;
-  rc = ensure(ctx, ctx->scratch[SCR_ICP], 256 + orig_bytes + z_bytes + (map ? sizeof(float) * (size_t)slot_cap : 0), st);
-  if (rc != SFE_OK) return rc;
-  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
-  int *counters = (int *)base;
-  if (cta_grid < pb.P || map) SFE_CUDA(cudaMemsetAsync(counters, 0, 2 * sizeof(int), st));
-  if (limit > 0) {
-    b.nt_max = nt_cta > 0 ? nt_cta : 1, b.class_nt = b.nt_max;
-    b.orig_ws = (uint16_t *)(base + 256);
-    b.next = cta_grid < pb.P ? counters : nullptr;
-    icp3_kernel<<<cta_grid, ICP3_THREADS, cta_smem, st>>>(b);
-    SFE_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  if (!map) return SFE_OK;
-  MapWs w;
-  rc = map_build(ctx, st, {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, pb.P, limit, slot_cap, true, true, 0, w);
-  if (rc != SFE_OK) return rc;
-  float *zs = (float *)(base + 256 + orig_bytes), *zm = (float *)(base + 256 + orig_bytes + z_bytes);
-  icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
-  int per_sm;
-  if ((rc = ctas_per_sm(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, &per_sm)) != SFE_OK) return rc;
-  const int grid = std::min(ctx->sm_count * per_sm, pb.P);
-  b.next = grid < pb.P ? counters + 1 : nullptr;
-  const IcpMapArgs m{w.slot, w.grid, w.pts, w.cstart, w.orig, nullptr, w.cell_cap};
-  icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, m);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return SFE_OK;
+  // the map class's workspace: z by map-grid position, z mean per slot
+  const size_t z_bytes = ((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255);
+  return split_run(
+      ctx, st, {limit > 0 ? (const void *)icp3_kernel : nullptr, ICP3_THREADS, cta_smem, b.nt_max, true}, pb.P, limit,
+      {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, slot_cap, true, z_bytes + sizeof(float) * slot_cap,
+      [&](int grid, uint16_t *orig_ws, int *next) {
+        b.orig_ws = orig_ws, b.next = next;
+        icp3_kernel<<<grid, ICP3_THREADS, cta_smem, st>>>(b);
+      },
+      [&](const MapWs &w, char *ws, int *next) -> int {
+        float *zs = (float *)ws, *zm = (float *)(ws + z_bytes);
+        icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
+        SFE_CUDA(cudaGetLastError());
+        ctx->launches++;
+        b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
+        int grid;
+        const int rc = persistent_grid(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, pb.P, &grid);
+        if (rc != SFE_OK) return rc;
+        b.next = grid < pb.P ? next : nullptr;
+        icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, w.args());
+        return SFE_OK;
+      });
 }
 
 // References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in
@@ -1267,26 +1216,18 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
               ctx->max_smem_optin);
     return SFE_ERR_UNSUPPORTED;
   }
-  int per_sm;
-  if ((rc = ctas_per_sm(ctx, (const void *)match_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
-  int grid = ctx->sm_count * per_sm;
-  if (grid > P) grid = P;
-  rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
-  if (rc != SFE_OK) return rc;
-  b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
-  match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  if (nt_max <= limit) return SFE_OK;
-  MapWs w;
-  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, limit, P, false, true, 0, w);
-  if (rc != SFE_OK) return rc;
-  b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
-  b.map_cell_cap = w.cell_cap;
-  match_map_kernel<<<ctx->sm_count * 4, ICP_THREADS, 0, st>>>(b);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return SFE_OK;
+  return split_run(
+      ctx, st, {(const void *)match_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit,
+      {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, false, 0,
+      [&](int grid, uint16_t *orig_ws, int *) {
+        b.orig_ws = orig_ws;
+        match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);
+      },
+      [&](const MapWs &w, char *, int *) -> int {
+        b.map = w.args();
+        match_map_kernel<<<ctx->sm_count * 4, ICP_THREADS, 0, st>>>(b);
+        return SFE_OK;
+      });
 }
 
 // 2-D clouds, knn 1: match_run.  Otherwise (knn > 1, or [x, y, z] clouds at any knn): references whose layout fits one
@@ -1321,31 +1262,25 @@ int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, c
     set_error("match: knn %d needs %zu B of shared memory per CTA (limit %zu)", knn, smem, budget);
     return SFE_ERR_UNSUPPORTED;
   }
-  int per_sm;
-  if ((rc = ctas_per_sm(ctx, cta_kernel, ICP_THREADS, smem, &per_sm)) != SFE_OK) return rc;
-  int grid = ctx->sm_count * per_sm;
-  if (grid > P) grid = P;
-  rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * b.nt_max * sizeof(uint16_t), st);
-  if (rc != SFE_OK) return rc;
-  b.orig_ws = (uint16_t *)ctx->scratch[SCR_ICP].ptr;
-  if (dim == 3) match_knn_kernel<3><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
-  else match_knn_kernel<2><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  if (nt_max <= limit) return SFE_OK;
-  MapWs w;
-  rc = map_build(ctx, st, {ref.pts, ref.off, nullptr, nt_max}, dim, nullptr, P, limit, P, false, true, 0, w);
-  if (rc != SFE_OK) return rc;
-  b.map_slot = w.slot, b.map_grid = w.grid, b.map_pts = w.pts, b.map_cstart = w.cstart, b.map_orig = w.orig;
-  b.map_cell_cap = w.cell_cap;
-  const size_t map_lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(int));
-  const void *map_kernel = dim == 3 ? (const void *)match_knn_map_kernel<3> : (const void *)match_knn_map_kernel<2>;
-  if ((rc = ctas_per_sm(ctx, map_kernel, ICP_THREADS, map_lists, &per_sm)) != SFE_OK) return rc;
-  if (dim == 3) match_knn_map_kernel<3><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
-  else match_knn_map_kernel<2><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return SFE_OK;
+  return split_run(
+      ctx, st, {cta_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, {ref.pts, ref.off, nullptr, nt_max}, dim,
+      nullptr, P, false, 0,
+      [&](int grid, uint16_t *orig_ws, int *) {
+        b.orig_ws = orig_ws;
+        if (dim == 3) match_knn_kernel<3><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
+        else match_knn_kernel<2><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
+      },
+      [&](const MapWs &w, char *, int *) -> int {
+        b.map = w.args();
+        const size_t map_lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(int));
+        const void *map_kernel = dim == 3 ? (const void *)match_knn_map_kernel<3> : (const void *)match_knn_map_kernel<2>;
+        int per_sm;
+        const int rc = ctas_per_sm(ctx, map_kernel, ICP_THREADS, map_lists, &per_sm);
+        if (rc != SFE_OK) return rc;
+        if (dim == 3) match_knn_map_kernel<3><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
+        else match_knn_map_kernel<2><<<ctx->sm_count * per_sm, ICP_THREADS, map_lists, st>>>(b, knn);
+        return SFE_OK;
+      });
 }
 
 #ifdef SFE_ICP_PHASE_CLOCKS

@@ -292,7 +292,7 @@ __device__ __noinline__ void icp3_update(Icp3Shared &sh, const sfe_icp_params &p
 // Shared layout: [Icp3Shared][sorted float2 nt_max][z f32 nt_max][cells u32]  (MAP: none of these three)
 //                [reading f32 3 ns_max][dist f32 ns_max][match Pos ns_max][seq_sum9_warp scratch]
 template <bool MAP>
-__device__ __forceinline__ void icp3_body(const Icp3Batch &b, const IcpMapArgs &mp) {
+__device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using Pos = std::conditional_t<MAP, int, uint16_t>;
   constexpr int NONE = MAP ? -1 : 0xffff;
@@ -353,12 +353,11 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const IcpMapArgs &
     std::conditional_t<MAP, MapGridView, GridView> g;
     const float *zp;
     if constexpr (MAP) {
-      const int ms = mp.map_slot[p];
-      const MapGrid &mg = mp.map_grid[ms];
+      const int ms = mp.slot[p];
+      const MapGrid &mg = mp.grid[ms];
       if (tid == 0) sh.mean[0] = mg.mean[0], sh.mean[1] = mg.mean[1], sh.mean[2] = b.map_zm[ms];
-      g.pts = mp.map_pts, g.cstart = mp.map_cstart + (size_t)ms * mp.map_cell_cap, g.orig = mp.map_orig;
-      g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
-      sorted = const_cast<float2 *>(mp.map_pts);
+      g = map_grid_view(mp, ms);
+      sorted = const_cast<float2 *>(mp.pts);
       zp = b.map_z;
       __syncthreads();
     } else {
@@ -539,11 +538,11 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const IcpMapArgs &
 }
 
 __global__ void __launch_bounds__(ICP3_THREADS, 1) icp3_kernel(const Icp3Batch b) {
-  constexpr IcpMapArgs mp{};
+  constexpr MapArgs mp{};
   icp3_body<false>(b, mp);
 }
 
-__global__ void __launch_bounds__(ICP3_THREADS, 2) icp3_map_kernel(const Icp3Batch b, const IcpMapArgs mp) {
+__global__ void __launch_bounds__(ICP3_THREADS, 2) icp3_map_kernel(const Icp3Batch b, const MapArgs mp) {
   icp3_body<true>(b, mp);
 }
 

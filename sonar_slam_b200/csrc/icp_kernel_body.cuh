@@ -1,7 +1,18 @@
-// Body of icp_kernel and icp_map_kernel (icp.cu): included inside both kernel definitions, never on its own.
-// In scope there: the batch `b`, the constants `MAP` (true: the target is a map grid, read through `mp`) and `FILT`
-// (true: the batch runs sfe_icp_filters, icp_filt_kernel / icp_map_filt_kernel) and the template parameters THREADS and
-// PLANE.
+// The 2-D ICP kernel, icp_kernel (included by icp.cu only, after its helpers and IcpBatch).
+//
+// One instantiation per CTA size, THREADS with MINB CTAs per SM, so that the register budget follows the launch shape
+// (a single __launch_bounds__(512) build capped the 128-thread class at 64 registers and spilled).  The flags are
+// instantiations of their own so that the shipped point-to-point kernels keep their code and register allocation:
+//   PLANE: errorMinimizer = PointToPlaneErrorMinimizer (sfe_icp_params.minimizer 1);
+//   MAP:   the map class -- the target is a map grid in global memory, read through `mp` (map_build): no set-up per
+//          problem, 32-bit target positions, and shared memory holds IcpShared and the source arrays only.  The in-CTA
+//          class ignores `mp`; it comes after `b`, so `b` has the same parameter offsets in both classes;
+//   FILT:  the batch runs sfe_icp_filters -- the MinDist / MedianDist outlier filters and the min_points gate on the
+//          clouds before the data filters.
+// The body is written in the kernel itself: behind a device-function wrapper the shipped instantiations compiled with
+// larger stack frames.
+template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT>
+__global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, const MapArgs mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
   //         [prev Pos ns_max][qstate u8 ns_max][slack f32 ns_max][order u16 ns_max]   (MAP: no sorted, no cells)
@@ -104,7 +115,7 @@
 
     ICP_PH_START();
     if constexpr (MAP) {  // ---- 1. (map class) mean and bounding box were computed once for the whole call
-      const MapGrid &mg = mp.map_grid[mp.map_slot[p]];
+      const MapGrid &mg = mp.grid[mp.slot[p]];
       if (tid == 0) {
         sh.mean[0] = mg.mean[0], sh.mean[1] = mg.mean[1];
 #pragma unroll
@@ -161,11 +172,8 @@
     const float mx = sh.mean[0], my = sh.mean[1];
     std::conditional_t<MAP, MapGridView, GridView> g;
     if constexpr (MAP) {  // the grid too (map_build)
-      const int ms = mp.map_slot[p];
-      const MapGrid &mg = mp.map_grid[ms];
-      g.pts = mp.map_pts, g.cstart = mp.map_cstart + (size_t)ms * mp.map_cell_cap, g.orig = mp.map_orig;
-      g.n = mg.n, g.nx = mg.nx, g.ny = mg.ny, g.ox = mg.ox, g.oy = mg.oy, g.cell = mg.cell, g.inv_cell = mg.inv_cell;
-      sorted = const_cast<float2 *>(mp.map_pts);
+      g = map_grid_view(mp, mp.slot[p]);
+      sorted = const_cast<float2 *>(mp.pts);
     } else {
     grid_geometry(nt, sh.bbox[0], sh.bbox[1], sh.bbox[2], sh.bbox[3], 0.05f, g, b.max_cells, b.cell_scale);
     grid_build(tgt, 2, nt, mx, my, g, sorted, cells, orig, sh.scan);
@@ -197,7 +205,7 @@
     // memory (8 B per target point; the iterations gather them through L2)
     float2 *nrm = nullptr;
     if constexpr (PLANE && MAP) {
-      nrm = const_cast<float2 *>(mp.map_nrm);  // computed once per target by map_build
+      nrm = const_cast<float2 *>(mp.nrm);  // computed once per target by map_build
     } else if constexpr (PLANE) {
       nrm = b.nrm_ws + (size_t)slot * b.nt_max;
       const int knn = min(max(prm.normals_knn, 1), GRID_KNN_MAX);
@@ -844,3 +852,4 @@
     }
   }
   ICP_PH_FLUSH();
+}

@@ -1,6 +1,6 @@
 // Map grids (sm_90a): clouds too large for a one-CTA layout, sorted into a uniform grid in global memory once per call.
 //
-// Shared by the scan matcher and the nearest-neighbour matcher (icp.cu: icp_map_kernel, match_map_kernel) and the
+// Shared by the scan matcher and the nearest-neighbour matcher (icp.cu: icp_kernel's map class, match_map_kernel) and the
 // radius outlier filter (cloud.cu: ro_map_count_kernel).  The grid is the one grid.cuh describes -- row-major cells,
 // every cell's points contiguous -- with 32-bit absolute cell starts and original indices (MapGridView).
 #include <climits>
@@ -143,17 +143,12 @@ __global__ void map_scatter_kernel(const PackedClouds t, int dim, const int *slo
 }
 
 // point-to-plane: the normal at every sorted position, once per target
-__global__ void map_normals_kernel(const unsigned long long *key, const MapGrid *grid, const float2 *pts,
-                                   const int *cstart, const int *orig, int N, int cell_cap, int knn, float2 *nrm) {
+__global__ void map_normals_kernel(const unsigned long long *key, const MapArgs m, int N, int knn, float2 *nrm) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   const unsigned long long k = key[i];
   if (k == ~0ull) return;
-  const int s = (int)(k >> 32);
-  const MapGrid &m = grid[s];
-  MapGridView g;
-  g.pts = pts, g.cstart = cstart + (size_t)s * cell_cap, g.orig = orig;
-  g.n = m.n, g.nx = m.nx, g.ny = m.ny, g.ox = m.ox, g.oy = m.oy, g.cell = m.cell, g.inv_cell = m.inv_cell;
+  const MapGridView g = map_grid_view(m, (int)(k >> 32));
   float bd[GRID_KNN_MAX];
   int bi[GRID_KNN_MAX];
   nrm[i] = grid_surface_normal(g, i, knn, bd, bi, 1);
@@ -247,8 +242,7 @@ int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, con
   SFE_CUDA(cudaGetLastError());
   ctx->launches += 9;  // six kernels, the two sorts and the scan counted once each
   if (knn > 0) {
-    map_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), w.grid, w.pts, w.cstart, w.orig, N, w.cell_cap, knn,
-                                                   w.nrm);
+    map_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), w.args(), N, knn, w.nrm);
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;
   }

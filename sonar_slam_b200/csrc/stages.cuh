@@ -70,10 +70,15 @@ int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpP
             int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr);
 // SFE_OK, or SFE_ERR_ARG with a message naming `what`: NaN, unknown kind, dim outside -1 .. 1, counts out of range
 int icp_filters_check(const sfe_icp_filters *f, const char *what);
+// SFE_OK, or an error with a message naming `what`: the settings prm and the filters filt (may be null) that icp_run
+// (dim 2) or icp3_run (dim 3) does not solve.  The 3-D chain refuses point-to-plane, float64 accumulation and filters
+// (SFE_ERR_UNSUPPORTED).
+int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what);
 // icp_run on [x, y, z] clouds (icp3.cuh; statement oracle/icp3_ref.c): guess and T_out are [P][16] row-major 4x4,
-// point-to-point with float32 sums only (SFE_ERR_UNSUPPORTED otherwise); no counts, classes or filters.  Targets above
+// point-to-point with float32 sums only; no counts, classes or filters (icp_params_check).  Targets above
 // icp_cta_limit(ctx, 3, ns) read map grids, with the same results.
-int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb);
+int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
+             const sfe_icp_filters *filt = nullptr);
 // *limit = the largest target of `dim` columns that icp_run (dim 2: shipped point-to-point chain, no filters) or
 // icp3_run (dim 3) solves in one CTA next to sources of ns points; larger targets take the map class
 int icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit);
@@ -94,6 +99,17 @@ struct MapGrid {
   int nx, ny, n, pad;
 };
 
+// What the map-class kernels read of map_build's grids: problem p's target is the grid in slot slot[p] (map_grid_view)
+struct MapArgs {
+  const int *slot;
+  const MapGrid *grid;
+  const float2 *pts;
+  const int *cstart;
+  const int *orig;
+  const float2 *nrm;
+  int cell_cap;
+};
+
 struct MapWs {  // device pointers into scratch[SCR_MAP]
   int *slot;       // [P] slot of every problem, -1: not in the map class
   int *n_slots;    // [1]
@@ -104,6 +120,7 @@ struct MapWs {  // device pointers into scratch[SCR_MAP]
   int *cstart;     // [slot_cap][cell_cap]: absolute position in pts of every cell's first point, entry nx * ny = end
   float2 *nrm;     // [slot_cap * nt_max] point-to-plane only
   int cell_cap;
+  MapArgs args() const { return {slot, grid, pts, cstart, orig, nrm, cell_cap}; }
 };
 
 // Map grids (map_grid.cu) of the clouds with more than `limit` points among those that P problems name (problem p:

@@ -123,7 +123,7 @@ def test_point_to_plane_equals_oracle(gpu_ctx):
 @pytest.mark.parametrize("delta", [0, 1])
 def test_target_at_the_limit_and_one_past(gpu_ctx, delta):
     """At the limit one icp_kernel launch; one point past it the in-CTA launch (it takes the targets that fit, here
-    none) plus the map class: build (nine launches) and icp_map_kernel."""
+    none) plus the map class: build (nine launches) and icp_kernel's map class."""
     from sonar_slam_b200 import _lib
     ctx = _lib.default_context()
     src, T = _source(_map("80k"), 1500, 4)

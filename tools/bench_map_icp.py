@@ -85,7 +85,7 @@ def measure(tgt, src, guesses, cpu=True):
                 continue
             us = getattr(e, "device_time_total", None)
             us = us if us is not None else e.cuda_time_total
-            if "icp_kernel" in e.name or "icp_map_kernel" in e.name:
+            if "icp_kernel" in e.name:  # both classes: icp_kernel<..., MAP, ...>
                 i += us
             else:
                 b += us
