@@ -31,7 +31,7 @@ extern "C" {
                             202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch); later
                                  additions that change no existing entry point: sfe_match_dim_*, sfe_match_knn_dim_*,
                                  sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
-                                 sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit */
+                                 sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -298,10 +298,16 @@ SFE_API const char *sfe_icp_status_message(int status);
  * Targets of any size: the problems whose target fits one CTA's shared memory next to the sources (22 k points
  * next to 1 500-point sources on an H100) run as before; the others read their target from a map grid built once
  * per distinct target cloud in global memory (mean, normals and grid computed once, not per guess), with the same
- * results.  Sources stay limited to 65 535 points and to what fits shared memory (about 31 bytes per point, 7 000
- * points).  Map workspace: 40 bytes (48 point-to-plane) for each of slots * nt_max slot points (at most 2^31 - 1),
+ * results.  Map workspace: 40 bytes (48 point-to-plane) for each of slots * nt_max slot points (at most 2^31 - 1),
  * 6 bytes per nt_max point of cell table per slot, 28 bytes per problem and CUB's temporary storage; slots =
- * n_problems for sfe_icp_dev, min(n_problems, n_tgt_clouds) for the host flavours. */
+ * n_problems for sfe_icp_dev, min(n_problems, n_tgt_clouds) for the host flavours.
+ * Sources of any size: sources of up to sfe_icp_source_limit points (about 8 400 on an H100, 27 bytes of shared memory
+ * per point) run in the shared-memory layouts as before.  Larger ones take the global-source class: persistent
+ * 512-thread CTAs that keep the per-source-point arrays in a slice of global workspace (29 bytes per ns_max point,
+ * 256-byte aligned) and read every target, small or large, from a map grid.  As many CTAs run as fit the SMs and a
+ * fixed 512 MiB for all slices together, at least one; a source whose one slice exceeds 512 MiB (about 18 million
+ * points) is SFE_ERR_UNSUPPORTED, and nothing is launched.  A call whose targets all fit one CTA next to its sources
+ * still runs in that CTA.  Results are the same in every class. */
 SFE_API int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev, const int32_t *src_off_dev,
                         const float *tgt_pts_dev, const int32_t *tgt_off_dev, const int32_t *src_id_dev,
                         const int32_t *tgt_id_dev, int n_problems, int ns_max, int nt_max, const float *guess_dev,
@@ -321,7 +327,8 @@ SFE_API int sfe_icp_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *s
                          int32_t *inliers_host, int32_t *status_host);
 /* Host-buffer flavour of sfe_icp_dev: packed clouds with CSR offsets (src_off [n_src_clouds + 1], tgt_off
  * [n_tgt_clouds + 1]) and per-problem src_id / tgt_id, all in host memory, so that the guesses of many loop-closure
- * candidates (each its own cloud pair) go out in one launch.  ns_max / nt_max are taken from the offsets. */
+ * candidates (each its own cloud pair) go out in one launch.  ns_max / nt_max are taken from the offsets.  Clouds of
+ * any size, as sfe_icp_dev: sources above sfe_icp_source_limit take the global-source class and its workspace. */
 SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_host,
                                const int32_t *src_off_host, int n_src_clouds, const float *tgt_pts_host,
                                const int32_t *tgt_off_host, int n_tgt_clouds, const int32_t *src_id_host,
@@ -360,7 +367,10 @@ typedef struct {
  * index, on a grid of x, y), the MaxDist and Trimmed weights, R = U V^T from a float32 restatement of Eigen's JacobiSVD of
  * the 3x3 cross-covariance with the reflection fix (a planar cloud whose 2-D fit would be a reflection gets a rotation
  * that flips z), Counter and Differential checkers on quaternions.  Same statuses and messages.  Targets above
- * sfe_icp_cta_limit(ctx, 3, ns_max) read map grids (sfe_icp_dev's workspace, plus 4 bytes per slot point).  dim 3 with
+ * sfe_icp_cta_limit(ctx, 3, ns_max) read map grids (sfe_icp_dev's workspace, plus 4 bytes per slot point).  Sources of
+ * any size, as for dim 2: above sfe_icp_source_limit(ctx, prm, 3) (about 11 000 points on an H100) the global-source
+ * class keeps reading, dist and match in global memory (20 bytes per ns_max point per CTA, two 256-thread CTAs per SM,
+ * all slices within 512 MiB) and reads every target from a map grid.  dim 3 with
  * minimizer 1, flags bit 1 or ICP filters set on ctx is SFE_ERR_UNSUPPORTED, and nothing is launched; dim outside
  * 2 .. 3 is SFE_ERR_ARG. */
 SFE_API int sfe_icp_dim_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_dev,
@@ -379,6 +389,12 @@ SFE_API int sfe_icp_batch_dim_host(sfe_ctx *ctx, const sfe_icp_params *prm, cons
 /* *limit = the largest target of `dim` columns that sfe_icp_dim_* solves in one CTA next to sources of ns points on this
  * context's device (dim 2: the shipped point-to-point chain without filters); larger targets take the map class */
 SFE_API int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit);
+/* *limit = the largest source of `dim` columns that sfe_icp_dev / sfe_icp_dim_* / the host flavours solve in their
+ * shared-memory layouts next to targets of any size, for the settings prm and the ICP filters set on ctx, on this
+ * context's device.  Larger sources take the global-source class (sfe_icp_dev), unless every target of the call fits
+ * one CTA next to them (sfe_icp_cta_limit).  Settings the chain does not run are reported as by sfe_icp_dim_dev; dim
+ * outside 2 .. 3 and null pointers are SFE_ERR_ARG. */
+SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit);
 
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
  * the default).  Checked here: no NaN, kind and dim known, counts in range; SFE_ERR_ARG leaves the setting as it was. */

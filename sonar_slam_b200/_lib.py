@@ -151,6 +151,7 @@ _EXTRA_SIGNATURES = {
     "sfe_icp_batch_dim_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_icp_cta_limit": [c_void_p, c_int, c_int, c_void_p],
+    "sfe_icp_source_limit": [c_void_p, c_void_p, c_int, c_void_p],
     "sfe_frontend_set_icp_filters": [c_void_p, c_void_p],
     "sfe_mincovdet_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],

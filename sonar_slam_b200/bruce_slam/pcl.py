@@ -263,7 +263,8 @@ def parse_icp_yaml(text):
 
 
 class ICP(object):
-    """libpointmatcher PM::ICP as exposed by pcl.cpp:185-213."""
+    """libpointmatcher PM::ICP as exposed by pcl.cpp:185-213.  Sources and targets of any size (map-to-map alignment
+    included): the device picks the launch class from the clouds' sizes, and every class gives the same results."""
 
     def __init__(self):
         self.params = None  # no modules until loadFromYaml, like a default-constructed PM::ICP
@@ -323,7 +324,9 @@ class ICP(object):
         """All `guesses` (iterable of 3x3, or 4x4 for 3-column clouds) on the same cloud pair in one launch (N1: the
         loop of SLAM.compute_icp_with_cov, slam.py:346-358).  Returns dict(messages, T[n,3,3] (or [n,4,4]),
         iterations, inliers, status).  The target may be of any size (a whole map): above one CTA's shared memory it is
-        sorted once into a grid in global memory that every guess reads, with the same results."""
+        sorted once into a grid in global memory that every guess reads, with the same results.  So may the source:
+        above ops.icp_source_limit (about 8 400 points in 2-D, 11 000 in 3-D on an H100) its per-point arrays live in
+        global memory (the global-source class), again with the same results."""
         if self.params is None:
             raise RuntimeError("You must setup a matcher before running ICP")
         src = _points(source, "source")

@@ -640,4 +640,14 @@ int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit) {
   return rc;
 }
 
+int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit) {
+  SFE_REQUIRE(dim == 2 || dim == 3, "sfe_icp_source_limit: points must have 2 or 3 columns (got %d)", dim);
+  SFE_REQUIRE(ctx && prm && limit, "sfe_icp_source_limit: null pointer");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  int n;
+  const int rc = icp_source_limit(ctx, prm, dim, ctx->has_icp_filters ? &ctx->icp_filters : nullptr, &n);
+  if (rc == SFE_OK) *limit = n;
+  return rc;
+}
+
 }  // extern "C"

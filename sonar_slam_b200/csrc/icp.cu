@@ -79,6 +79,10 @@ struct IcpBatch {
   // data filters, which the min_points test reads
   float min_d2, median_factor;
   const int *gate_src_cnt, *gate_tgt_cnt;
+  // global-source class (icp_kernel's GSRC instantiations): CTA c keeps its per-source-point arrays at src_ws + c *
+  // src_ws_stride in global memory
+  unsigned char *src_ws;
+  size_t src_ws_stride;
 };
 
 
@@ -713,13 +717,13 @@ static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 153
 // the flags.  In-CTA class: 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers;
 // dense (icp_run's classes): 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get
 // them (IcpClass::dense).  Map class: one instantiation per CTA size.  filt: sfe_icp_filters.
-template <int THREADS, int MINB, bool MAP>
+template <int THREADS, int MINB, bool MAP, bool GSRC = false>
 static const void *icp_kernel_of(bool plane, bool filt) {
   if (filt)
-    return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true>
-                 : (const void *)icp_kernel<THREADS, MINB, false, MAP, true>;
-  return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, false>
-               : (const void *)icp_kernel<THREADS, MINB, false, MAP, false>;
+    return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true, GSRC>
+                 : (const void *)icp_kernel<THREADS, MINB, false, MAP, true, GSRC>;
+  return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, false, GSRC>
+               : (const void *)icp_kernel<THREADS, MINB, false, MAP, false, GSRC>;
 }
 
 static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool map) {
@@ -812,10 +816,62 @@ static int icp_enqueue(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L, char *ws, in
   IcpBatch &b = L.b;
   b.orig_ws = (uint16_t *)ws;
   b.nrm_ws = b.prm.minimizer == 1 ? (float2 *)(ws + L.orig_bytes) : nullptr;
+  if (b.src_ws_stride) b.src_ws = (unsigned char *)ws;  // (the global-source class: its slices, nothing else)
   if (!b.slot_by_smid && (L.grid < b.P || b.list)) b.next = next;  // persistent CTAs; a list is always walked so
   void *args[] = {(void *)&b, (void *)&L.m};
   SFE_CUDA(cudaLaunchKernel(L.fn, dim3(L.grid), dim3(L.threads), args, L.smem, st));
   ctx->launches++;
+  return SFE_OK;
+}
+
+// The global-source class: sources above what the shared-memory layouts hold (icp_source_limit).  Each persistent CTA
+// keeps its per-source-point arrays in a slice of global workspace; all slices together stay within ICP_SRC_WS_CAP.
+constexpr size_t ICP_SRC_WS_CAP = size_t(512) << 20;
+
+// Bytes of one CTA's slice for sources of up to ns_max points: icp_kernel's reading (8 B), dist, match, prev, slack and
+// order (4 B each) and qstate (1 B) per point, 256-byte aligned
+static size_t icp_src_slice(int ns_max) {
+  const size_t n = (size_t)ns_max;
+  return (28 * n + ((n + 3) & ~size_t(3)) + 255) & ~size_t(255);
+}
+
+// The largest source icp_kernel's shared-memory layouts hold next to targets of any size: the map class's, whose layout
+// holds no target (at most 65 535 points).  Larger sources take the global-source class.
+static int icp2_src_limit(const sfe_ctx *ctx, bool plane, bool filt, int *limit) {
+  size_t budget;
+  int rc = icp_cta_budget(ctx, ICP_THREADS, plane, false, filt, true, &budget);
+  if (rc != SFE_OK) return rc;
+  int mc;
+  *limit = largest_layout(65535, budget, [&](int ns) { return icp_cta_smem(ns, 1, plane, true, budget, &mc); });
+  return SFE_OK;
+}
+
+// The global-source launch: icp_kernel<512, 1, PLANE, true, FILT, true> takes the problems whose source has more than
+// class_ns points (IcpBatch::class_mode 2) and reads every target from a map grid (L.m, set by the caller after
+// map_build).  Persistent CTAs: min(P, SMs x CTAs per SM, the slices ICP_SRC_WS_CAP holds), at least one.
+static int icp_gsrc_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max, int class_ns,
+                         IcpLaunch &L) {
+  b.ns_max = ns_max, b.nt_max = nt_max > 0 ? nt_max : 1;
+  b.use_order = 1, b.cell_scale = 1.0f, b.prm = *prm;
+  icp_tuning(b);
+  b.class_mode = 2, b.class_ns = class_ns, b.class_nt = INT_MAX;
+  const size_t slice = icp_src_slice(ns_max);
+  if (slice > ICP_SRC_WS_CAP) {
+    set_error("icp: a source of %d points needs %zu B of global workspace per CTA (at most %zu)", ns_max, slice,
+              ICP_SRC_WS_CAP);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  b.src_ws_stride = slice;
+  const bool plane = prm->minimizer == 1,
+             filt = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
+  const void *fn = icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt);
+  const size_t smem = ((sizeof(IcpShared) + 15) & ~size_t(15)) + (plane ? ICP_PLANE_SCRATCH * sizeof(float) : 0);
+  int per_sm;
+  const int rc = ctas_per_sm(ctx, fn, ICP_THREADS, smem, &per_sm);
+  if (rc != SFE_OK) return rc;
+  const int grid = std::max(1, std::min({b.P, ctx->sm_count * per_sm, (int)(ICP_SRC_WS_CAP / slice)}));
+  L.b = b, L.m = {}, L.fn = fn, L.threads = ICP_THREADS, L.grid = grid, L.smem = smem;
+  L.orig_bytes = 0, L.ws_bytes = (size_t)grid * slice;
   return SFE_OK;
 }
 
@@ -968,17 +1024,19 @@ struct SplitCta {
 
 // One call of P problems split at `limit` target points (icp3_run, match_run, match_knn_run): the one-CTA kernel takes
 // the targets of up to `limit` points in a persistent launch (persistent_grid), each CTA with a row of c.nt original
-// indices (orig_ws); when the largest target, tgt.n_max, is above the limit, map_build builds map grids of the larger
-// targets (`dim` columns; problem p's target tgt_id[p], or p with tgt_id null; slot_cap distinct ones; centred or not)
-// and the map class reads them.  Workspace, scratch[SCR_ICP]: [two work counters][orig_ws][the map class's `extra`
-// bytes]; with c.counted both counters are zeroed whenever a launch may take problems from them.
+// indices (orig_ws); when the largest target, tgt.n_max, is above map_limit (`limit`, or 0 when icp3_run's
+// global-source class reads every target as a map grid), map_build builds map grids of the targets above map_limit
+// (`dim` columns; problem p's target tgt_id[p], or p with tgt_id null; slot_cap distinct ones; centred or not) and the
+// map class reads them.  Workspace, scratch[SCR_ICP]: [256 B of work counters][orig_ws][the map class's `extra` bytes];
+// with c.counted the first two counters are zeroed whenever a launch may take problems from them.
 // cta(grid, orig_ws, next) enqueues the one-CTA kernel (next: its work counter, or null);
-// map(MapWs, extra workspace, next) enqueues the map class, last its map kernel (next: the second work counter) and
-// returns an SFE_* code.
+// map(MapWs, extra workspace, next) enqueues the map class, last the kernel split_run counts (next: the second work
+// counter; the ones after it are free) and returns an SFE_* code.
 template <typename Cta, typename Map>
-static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, int limit, const PackedClouds &tgt,
-                     int dim, const int *tgt_id, int slot_cap, bool center, size_t extra, Cta cta, Map map) {
-  const bool map_class = tgt.n_max > limit;
+static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, int limit, int map_limit,
+                     const PackedClouds &tgt, int dim, const int *tgt_id, int slot_cap, bool center, size_t extra,
+                     Cta cta, Map map) {
+  const bool map_class = tgt.n_max > map_limit;
   int grid = 0, rc;
   if (c.fn && (rc = persistent_grid(ctx, c.fn, c.threads, c.smem, P, &grid)) != SFE_OK) return rc;
   const size_t head = 256, orig_bytes = ((size_t)grid * c.nt * sizeof(uint16_t) + 255) & ~size_t(255);
@@ -993,7 +1051,7 @@ static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, in
   }
   if (!map_class) return SFE_OK;
   MapWs w;
-  if ((rc = map_build(ctx, st, tgt, dim, tgt_id, P, limit, slot_cap, center, true, 0, w)) != SFE_OK) return rc;
+  if ((rc = map_build(ctx, st, tgt, dim, tgt_id, P, map_limit, slot_cap, center, true, 0, w)) != SFE_OK) return rc;
   if ((rc = map(w, base + head + orig_bytes, next + 1)) != SFE_OK) return rc;
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
@@ -1050,7 +1108,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     SFE_REQUIRE(class_list[c].ns > 0 && class_list[c].nt > 0, "icp: size class %d of %d x %d points", c,
                 class_list[c].ns, class_list[c].nt);
   const bool classes = n_classes > 0;
-  SFE_REQUIRE(ns_max <= 65535 && (nt_max <= 65535 || !classes),
+  SFE_REQUIRE((ns_max <= 65535 && nt_max <= 65535) || !classes,
               "icp: clouds of more than 65535 points are not supported (got %d, %d)", ns_max, nt_max);
   int rc = icp_params_check(prm, 2, filt, "icp");
   if (rc != SFE_OK) return rc;
@@ -1095,35 +1153,70 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   if (classes) return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
   // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
   const bool plane = prm->minimizer == 1;
-  const int ns = ns_max > 0 ? ns_max : 1, threads = icp_threads(ns);
-  int limit;
-  rc = icp2_limit(ctx, ns, plane, b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f,
-                  &limit);
-  if (rc != SFE_OK) return rc;
-  IcpLaunch L;
-  if (nt_max <= limit || limit > 0) {
-    b.class_mode = nt_max <= limit ? 0 : 1;
-    if ((rc = icp_plan(ctx, prm, b, ns_max, std::min(nt_max, limit), threads, L)) != SFE_OK) return rc;
+  const bool filt_on = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
+  int ns = ns_max > 0 ? ns_max : 1, limit = 0, src_limit;
+  if ((rc = icp2_src_limit(ctx, plane, filt_on, &src_limit)) != SFE_OK) return rc;
+  if (ns <= 65535 && (rc = icp2_limit(ctx, ns, plane, filt_on, &limit)) != SFE_OK) return rc;
+  // Sources above src_limit take the global-source class -- unless every target fits an in-CTA layout next to them
+  // (the in-CTA layout holds a few more source points than the map class's next to small targets).  The shared-memory
+  // launches are then laid out for src_limit-point sources and report the larger ones SFE_ICP_TOO_LARGE at admission;
+  // the global-source launch, enqueued after them on the same stream, solves those problems and writes their results
+  // over that status.
+  const bool gsrc = ns > src_limit && !(limit > 0 && nt_max <= limit);
+  IcpLaunch L, G;
+  if (gsrc) {
+    if ((rc = icp_gsrc_plan(ctx, prm, b, ns_max, nt_max, src_limit, G)) != SFE_OK) return rc;
+    ns = src_limit;
+    if ((rc = icp2_limit(ctx, ns, plane, filt_on, &limit)) != SFE_OK) return rc;
+  }
+  const int ns_cta = gsrc ? src_limit : ns_max, threads = icp_threads(ns);
+  if ((nt_max <= limit && !gsrc) || limit > 0) {
+    b.class_mode = nt_max <= limit && !gsrc ? 0 : 1;
+    if ((rc = icp_plan(ctx, prm, b, ns_cta, std::min(nt_max, limit), threads, L)) != SFE_OK) return rc;
     if ((rc = icp_launch(ctx, st, L)) != SFE_OK) return rc;
   }
-  if (nt_max <= limit) return SFE_OK;
+  if (nt_max <= limit && !gsrc) return SFE_OK;
   // the map class takes the other problems; with no in-CTA launch (limit 0) all of them (targets of 0 points are then
   // reported here, SFE_ICP_EMPTY_REF, before any map grid is read)
-  b.class_mode = limit > 0 ? 2 : 0, b.class_ns = ns, b.class_nt = limit;
-  if ((rc = icp_plan(ctx, prm, b, ns_max, nt_max, threads, L, false, true)) != SFE_OK) return rc;
-  const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-  MapWs w;
-  rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, limit, slot_cap, true,
-                 (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
-  if (rc != SFE_OK) return rc;
-  L.m = w.args();
-  return icp_launch(ctx, st, L);
+  const bool map_class = nt_max > limit;
+  if (map_class) {
+    b.class_mode = limit > 0 ? 2 : 0, b.class_ns = ns, b.class_nt = limit;
+    if ((rc = icp_plan(ctx, prm, b, ns_cta, nt_max, threads, L, false, true)) != SFE_OK) return rc;
+  }
+  // (the global-source class reads every target from a map grid; with no target points at all it reads none)
+  MapWs w{};
+  if (nt_max > 0) {
+    const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
+    rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, gsrc ? 0 : limit, slot_cap,
+                   true, (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
+    if (rc != SFE_OK) return rc;
+  }
+  if (map_class) {
+    L.m = w.args();
+    if ((rc = icp_launch(ctx, st, L)) != SFE_OK) return rc;
+  }
+  if (!gsrc) return SFE_OK;
+  G.m = w.args();
+  return icp_launch(ctx, st, G);
 }
 
 int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
   SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
   SFE_REQUIRE(ns >= 0 && ns <= 65535, "icp: sources of %d points are not supported (0..65535)", ns);
   return dim == 2 ? icp2_limit(ctx, ns, false, false, limit) : icp3_limit(ctx, ns > 0 ? ns : 1, limit);
+}
+
+int sfe::icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt,
+                          int *limit) {
+  SFE_REQUIRE(ctx && prm && limit, "icp_source_limit: null pointer");
+  SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
+  const int rc = icp_params_check(prm, dim, filt, "icp_source_limit");
+  if (rc != SFE_OK) return rc;
+  if (dim == 3) return icp3_src_limit(ctx, limit);
+  // (icp_run's choice of the FILT instantiations)
+  const bool filt_on = filt && (filt->n_reading > 0 || filt->n_reference > 0 || filt->min_dist >= 0.f ||
+                                filt->median_factor >= 0.f);
+  return icp2_src_limit(ctx, prm->minimizer == 1, filt_on, limit);
 }
 
 // [x, y, z] clouds: targets up to icp3_limit in icp3_kernel (one CTA, its grid in shared memory), larger ones as map
@@ -1140,15 +1233,38 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
                   pb.status,
               "icp (3-D): null pointer");
   SFE_REQUIRE(!pb.src.cnt && !pb.tgt.cnt, "icp (3-D): per-cloud counts are not supported");
-  SFE_REQUIRE(ns_max <= 65535, "icp: clouds of more than 65535 points are not supported (got %d)", ns_max);
-  const int ns = ns_max > 0 ? ns_max : 1;
-  int limit;
-  if ((rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
+  int ns = ns_max > 0 ? ns_max : 1, limit = 0, src_limit;
+  if ((rc = icp3_src_limit(ctx, &src_limit)) != SFE_OK) return rc;
+  if (ns <= 65535 && (rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
   Icp3Batch b{};
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
-  b.P = pb.P, b.ns_max = ns, b.prm = *prm;
+  b.P = pb.P, b.prm = *prm;
+  // Sources above src_limit take the global-source class (icp3_gsrc_kernel), as in icp_run: unless every target fits
+  // icp3_kernel next to them, the shared-memory launches are laid out for src_limit-point sources and report the larger
+  // ones SFE_ICP_TOO_LARGE, and the global-source launch, enqueued last, solves those and writes over that status.
+  const bool gsrc = ns > src_limit && !(limit > 0 && nt_max <= limit);
+  Icp3Batch g = b;
+  int g_grid = 0;
+  size_t g_bytes = 0;
+  if (gsrc) {
+    g.ns_max = ns_max, g.nt_max = nt_max > 0 ? nt_max : 1, g.class_ns = src_limit;
+    g.src_ws_stride = icp3_src_slice(ns_max);
+    if (g.src_ws_stride > ICP_SRC_WS_CAP) {
+      set_error("icp (3-D): a source of %d points needs %zu B of global workspace per CTA (at most %zu)", ns_max,
+                g.src_ws_stride, ICP_SRC_WS_CAP);
+      return SFE_ERR_UNSUPPORTED;
+    }
+    if ((rc = persistent_grid(ctx, (const void *)icp3_gsrc_kernel, ICP3_THREADS, icp3_gsrc_smem(), pb.P, &g_grid)) !=
+        SFE_OK)
+      return rc;
+    g_grid = std::max(1, std::min(g_grid, (int)(ICP_SRC_WS_CAP / g.src_ws_stride)));
+    g_bytes = (size_t)g_grid * g.src_ws_stride;
+    ns = src_limit;
+    if ((rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
+  }
+  b.ns_max = ns;
   const bool map = nt_max > limit;
   const size_t map_smem = icp3_map_smem(ns);
   if ((map && map_smem > (size_t)ctx->max_smem_optin) || (limit == 0 && !map)) {
@@ -1165,11 +1281,20 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
     if ((rc = cta_smem_budget(ctx, (const void *)icp3_kernel, &budget)) != SFE_OK) return rc;
     cta_smem = icp3_cta_smem(ns, b.nt_max, budget, &b.max_cells);
   }
-  // the map class's workspace: z by map-grid position, z mean per slot
+  // the map class's workspace: z by map-grid position, z mean per slot; then the global-source class's slices
   const size_t z_bytes = ((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255);
-  return split_run(
+  const size_t g_off = (z_bytes + sizeof(float) * slot_cap + 255) & ~size_t(255);
+  auto gsrc_launch = [&](const MapArgs &m, unsigned char *ws, int *next) -> int {
+    g.src_ws = ws;
+    g.next = g_grid < pb.P ? next : nullptr;
+    if (g.next) SFE_CUDA(cudaMemsetAsync(next, 0, sizeof(int), st));
+    icp3_gsrc_kernel<<<g_grid, ICP3_THREADS, icp3_gsrc_smem(), st>>>(g, m);
+    return SFE_OK;
+  };
+  rc = split_run(
       ctx, st, {limit > 0 ? (const void *)icp3_kernel : nullptr, ICP3_THREADS, cta_smem, b.nt_max, true}, pb.P, limit,
-      {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, slot_cap, true, z_bytes + sizeof(float) * slot_cap,
+      gsrc ? 0 : limit, {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, slot_cap, true,
+      gsrc ? g_off + g_bytes : z_bytes + sizeof(float) * slot_cap,
       [&](int grid, uint16_t *orig_ws, int *next) {
         b.orig_ws = orig_ws, b.next = next;
         icp3_kernel<<<grid, ICP3_THREADS, cta_smem, st>>>(b);
@@ -1179,14 +1304,27 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
         icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
         SFE_CUDA(cudaGetLastError());
         ctx->launches++;
-        b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
-        int grid;
-        const int rc = persistent_grid(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, pb.P, &grid);
-        if (rc != SFE_OK) return rc;
-        b.next = grid < pb.P ? next : nullptr;
-        icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, w.args());
-        return SFE_OK;
+        if (map) {
+          b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
+          int grid;
+          const int rc = persistent_grid(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, pb.P, &grid);
+          if (rc != SFE_OK) return rc;
+          b.next = grid < pb.P ? next : nullptr;
+          icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, w.args());
+          if (!gsrc) return SFE_OK;  // (split_run counts the last launch)
+          SFE_CUDA(cudaGetLastError());
+          ctx->launches++;
+        }
+        g.map_z = zs, g.map_zm = zm;
+        return gsrc_launch(w.args(), (unsigned char *)ws + g_off, next + 1);
       });
+  if (rc != SFE_OK || !gsrc || nt_max > 0) return rc;
+  // no target points at all: the global-source launch reports its problems (SFE_ICP_EMPTY_REF, or before that
+  // SFE_ICP_TOO_LARGE / SFE_ICP_NOT_RIGID) without reading a map grid or its slices
+  if ((rc = gsrc_launch(MapArgs{}, nullptr, ctx->work + WORK_ICP)) != SFE_OK) return rc;
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return SFE_OK;
 }
 
 // References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in
@@ -1217,7 +1355,7 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
     return SFE_ERR_UNSUPPORTED;
   }
   return split_run(
-      ctx, st, {(const void *)match_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit,
+      ctx, st, {(const void *)match_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, limit,
       {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, false, 0,
       [&](int grid, uint16_t *orig_ws, int *) {
         b.orig_ws = orig_ws;
@@ -1263,8 +1401,8 @@ int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, c
     return SFE_ERR_UNSUPPORTED;
   }
   return split_run(
-      ctx, st, {cta_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, {ref.pts, ref.off, nullptr, nt_max}, dim,
-      nullptr, P, false, 0,
+      ctx, st, {cta_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, limit, {ref.pts, ref.off, nullptr, nt_max},
+      dim, nullptr, P, false, 0,
       [&](int grid, uint16_t *orig_ws, int *) {
         b.orig_ws = orig_ws;
         if (dim == 3) match_knn_kernel<3><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));

@@ -35,6 +35,11 @@ struct Icp3Batch {
   int *next;             // work counter, or null: CTA c takes problems c, c + gridDim.x, ...
   const float *map_z;    // map class: centred z of every map-grid position
   const float *map_zm;   // map class: z mean of every slot
+  // global-source class (icp3_gsrc_kernel): takes the problems whose source has more than class_ns points; CTA c keeps
+  // reading, dist and match at src_ws + c * src_ws_stride in global memory
+  int class_ns;
+  unsigned char *src_ws;
+  size_t src_ws_stride;
 };
 
 struct Icp3Shared {
@@ -288,11 +293,15 @@ __device__ __noinline__ void icp3_update(Icp3Shared &sh, const sfe_icp_params &p
   else if (vt != vt) sh.s.status = ICP_NAN_TRANS;
 }
 
-// The body of icp3_kernel (MAP false: the target's grid in shared memory) and icp3_map_kernel (MAP true: map grids).
+// The body of icp3_kernel (MAP false: the target's grid in shared memory), icp3_map_kernel (MAP true: map grids) and
+// icp3_gsrc_kernel (MAP and GSRC: map grids, and sources too large for shared memory).
 // Shared layout: [Icp3Shared][sorted float2 nt_max][z f32 nt_max][cells u32]  (MAP: none of these three)
 //                [reading f32 3 ns_max][dist f32 ns_max][match Pos ns_max][seq_sum9_warp scratch]
-template <bool MAP>
+// GSRC: [Icp3Shared][seq_sum9_warp scratch] in shared memory, [reading][dist][match] at the start of the CTA's slice of
+// global workspace.
+template <bool MAP, bool GSRC = false>
 __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp) {
+  static_assert(MAP || !GSRC, "icp3_body: the global-source class reads its targets as map grids");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using Pos = std::conditional_t<MAP, int, uint16_t>;
   constexpr int NONE = MAP ? -1 : 0xffff;
@@ -305,13 +314,18 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp)
   uint32_t *cells = reinterpret_cast<uint32_t *>(smem_raw + off);
   if constexpr (!MAP) off += sizeof(uint32_t) * (size_t)((b.max_cells + 2) / 2 + 1);
   off = (off + 15) & ~size_t(15);
-  float *reading = reinterpret_cast<float *>(smem_raw + off);
+  unsigned char *src_base = smem_raw;  // where reading .. match start (GSRC: the CTA's slice, from 0)
+  const size_t shared_end = off;
+  if constexpr (GSRC) src_base = b.src_ws + (size_t)blockIdx.x * b.src_ws_stride, off = 0;
+  float *reading = reinterpret_cast<float *>(src_base + off);
   off += sizeof(float) * 3 * (size_t)b.ns_max;
-  float *dist = reinterpret_cast<float *>(smem_raw + off);
+  float *dist = reinterpret_cast<float *>(src_base + off);
   off += sizeof(float) * (size_t)b.ns_max;
-  Pos *match = reinterpret_cast<Pos *>(smem_raw + off);
+  Pos *match = reinterpret_cast<Pos *>(src_base + off);
   off += sizeof(Pos) * (size_t)b.ns_max;
   off = (off + 15) & ~size_t(15);
+  if constexpr (GSRC) off = shared_end;  // (the scratch stays in shared memory)
+  (void)shared_end;
   float *scratch = reinterpret_cast<float *>(smem_raw + off);
 
   const int tid = threadIdx.x, nthr = blockDim.x;
@@ -330,8 +344,12 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp)
     const float *tgt = b.tgt_pts + 3 * (size_t)b.tgt_off[ti];
     const int nt = b.tgt_off[ti + 1] - b.tgt_off[ti];
     const float *guess = b.guess + 16 * (size_t)p;
-    if (!MAP && nt > b.class_nt) continue;             // the map class's
-    if (MAP && b.class_nt > 0 && nt <= b.class_nt) continue;  // the in-CTA class's
+    if constexpr (GSRC) {
+      if (ns <= b.class_ns) continue;  // the shared-memory classes'
+    } else {
+      if (!MAP && nt > b.class_nt) continue;             // the map class's
+      if (MAP && b.class_nt > 0 && nt <= b.class_nt) continue;  // the in-CTA class's
+    }
     __syncthreads();  // previous problem fully retired before shared state is reused
 
     if (tid == 0) {  // admission: failure leaves T = guess
@@ -546,6 +564,10 @@ __global__ void __launch_bounds__(ICP3_THREADS, 2) icp3_map_kernel(const Icp3Bat
   icp3_body<true>(b, mp);
 }
 
+__global__ void __launch_bounds__(ICP3_THREADS, 2) icp3_gsrc_kernel(const Icp3Batch b, const MapArgs mp) {
+  icp3_body<true, true>(b, mp);
+}
+
 // Map class: the centred z of every map-grid position and every slot's z mean (icp3_body's sequential sum), one CTA
 // per slot
 __global__ void __launch_bounds__(ICP3_THREADS) icp3_map_z_kernel(const float *tgt_pts, const int *tgt_off, MapWs w,
@@ -583,6 +605,20 @@ static size_t icp3_cta_smem(int ns_max, int nt_max, size_t budget, int *max_cell
 static size_t icp3_map_smem(int ns_max) {
   return ((sizeof(Icp3Shared) + 15) & ~size_t(15)) + 16 + (3 * sizeof(float) + sizeof(float) + sizeof(int)) * (size_t)ns_max +
          16 + ICP3_SCRATCH * sizeof(float);
+}
+
+// The global-source class: one CTA's slice for sources of up to ns_max points (reading 12 B, dist and match 4 B each
+// per point, 256-byte aligned), and icp3_gsrc_kernel's shared memory
+static size_t icp3_src_slice(int ns_max) { return (20 * (size_t)ns_max + 255) & ~size_t(255); }
+static size_t icp3_gsrc_smem() { return ((sizeof(Icp3Shared) + 15) & ~size_t(15)) + ICP3_SCRATCH * sizeof(float); }
+
+// The largest source the shared-memory layouts hold next to targets of any size: icp3_map_kernel's (at most 65 535)
+static int icp3_src_limit(const sfe_ctx *ctx, int *limit) {
+  size_t budget;
+  int rc = cta_smem_budget(ctx, (const void *)icp3_map_kernel, &budget);
+  if (rc != SFE_OK) return rc;
+  *limit = largest_layout(65535, budget, icp3_map_smem);
+  return SFE_OK;
 }
 
 // The largest target icp3_kernel's layout holds next to sources of ns points (0: none; MAP_CLASS_ALL: 0)

@@ -8,19 +8,25 @@
 //          problem, 32-bit target positions, and shared memory holds IcpShared and the source arrays only.  The in-CTA
 //          class ignores `mp`; it comes after `b`, so `b` has the same parameter offsets in both classes;
 //   FILT:  the batch runs sfe_icp_filters -- the MinDist / MedianDist outlier filters and the min_points gate on the
-//          clouds before the data filters.
+//          clouds before the data filters;
+//   GSRC:  the global-source class (MAP only) -- sources too large for shared memory: the per-source-point arrays
+//          (reading .. order) sit in the CTA's slice of global workspace (b.src_ws), with 32-bit entries in order[];
+//          shared memory holds IcpShared and, PLANE, seq_sum9_warp's scratch.
 // The body is written in the kernel itself: behind a device-function wrapper the shipped instantiations compiled with
 // larger stack frames.
-template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT>
+template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT, bool GSRC>
 __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, const MapArgs mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
-  //         [prev Pos ns_max][qstate u8 ns_max][slack f32 ns_max][order u16 ns_max]   (MAP: no sorted, no cells)
+  //         [prev Pos ns_max][qstate u8 ns_max][slack f32 ns_max][order Ord ns_max]   (MAP: no sorted, no cells)
+  // GSRC: [IcpShared][seq_sum9_warp scratch] in shared memory, [reading .. order] at the start of the CTA's slice.
   // CTA sizes: the reference mean takes warps 0 and 1 (one per coordinate); the per-warp partials (wred, tot, red) and
   // block_total's final read (one lane per warp) hold at most 16 warps; the rest of the body loops over blockDim.x.
   static_assert(THREADS % 32 == 0 && THREADS >= 64 && THREADS <= 512, "icp_kernel: 2 to 16 warps per CTA");
-  using Pos = std::conditional_t<MAP, int, uint16_t>;  // a target point's sorted position
-  constexpr int NONE = MAP ? -1 : 0xffff;               // "no match"
+  static_assert(MAP || !GSRC, "icp_kernel: the global-source class reads its targets as map grids");
+  using Pos = std::conditional_t<MAP, int, uint16_t>;   // a target point's sorted position
+  using Ord = std::conditional_t<GSRC, int, uint16_t>;  // a source point's index
+  constexpr int NONE = MAP ? -1 : 0xffff;                // "no match"
   IcpShared &sh = *reinterpret_cast<IcpShared *>(smem_raw);
   size_t off = (sizeof(IcpShared) + 15) & ~size_t(15);
   float2 *sorted = reinterpret_cast<float2 *>(smem_raw + off);  // MAP: set to the slot's points below
@@ -28,31 +34,36 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
   uint32_t *cells = reinterpret_cast<uint32_t *>(smem_raw + off);
   if constexpr (!MAP) off += sizeof(uint32_t) * (size_t)((b.max_cells + 2) / 2 + 1);
   off = (off + 7) & ~size_t(7);
-  float2 *reading = reinterpret_cast<float2 *>(smem_raw + off);
+  unsigned char *src_base = smem_raw;  // where the per-source-point arrays start (GSRC: the CTA's slice, from 0)
+  const size_t shared_end = off;
+  if constexpr (GSRC) src_base = b.src_ws + (size_t)blockIdx.x * b.src_ws_stride, off = 0;
+  float2 *reading = reinterpret_cast<float2 *>(src_base + off);
   off += sizeof(float2) * (size_t)b.ns_max;
-  float *dist = reinterpret_cast<float *>(smem_raw + off);
+  float *dist = reinterpret_cast<float *>(src_base + off);
   off += sizeof(float) * (size_t)b.ns_max;
-  Pos *match = reinterpret_cast<Pos *>(smem_raw + off);
+  Pos *match = reinterpret_cast<Pos *>(src_base + off);
   off += sizeof(Pos) * (size_t)b.ns_max;
-  Pos *prev = reinterpret_cast<Pos *>(smem_raw + off);  // NN of the previous iteration (search seed)
+  Pos *prev = reinterpret_cast<Pos *>(src_base + off);  // NN of the previous iteration (search seed)
   off += sizeof(Pos) * (size_t)b.ns_max;
-  uint8_t *qstate = reinterpret_cast<uint8_t *>(smem_raw + off);
+  uint8_t *qstate = reinterpret_cast<uint8_t *>(src_base + off);
   off += ((size_t)b.ns_max + 3) & ~size_t(3);
   // certified-match margin per source point (metres): every target point other than prev[i] is farther from the
   // point's current position than (distance to prev[i]) as long as that distance stays below slack[i]
-  float *slack = reinterpret_cast<float *>(smem_raw + off);
+  float *slack = reinterpret_cast<float *>(src_base + off);
   off += sizeof(float) * (size_t)b.ns_max;
   // processing order of the source points in the search passes: sorted by a coarse cell of the target grid, so that
   // the lanes of a warp look at neighbouring cells (similar amounts of work, the same shared-memory lines); results
   // are stored by point index and the sums run in point order, so the order is invisible in the results
-  uint16_t *order = reinterpret_cast<uint16_t *>(smem_raw + off);
-  if (b.use_order) off += sizeof(uint16_t) * (size_t)b.ns_max;
+  Ord *order = reinterpret_cast<Ord *>(src_base + off);
+  if (b.use_order) off += sizeof(Ord) * (size_t)b.ns_max;
   off = (off + 15) & ~size_t(15);
+  if constexpr (GSRC) off = (shared_end + 15) & ~size_t(15);  // (the scratch below stays in shared memory)
+  (void)shared_end;
   // PLANE only: 640 floats for seq_sum9_warp.  dist[] is dead between the weights (3c) and the next iteration's
   // search, which rewrites all of it: launches with room for 640 source points (the front end's small class is
   // exactly that; 2 000 x 20 000 points leave nothing to spare at all) park the scratch there, smaller ones get
-  // their own 2.5 KB.
-  float *pl_scratch = b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
+  // their own 2.5 KB.  GSRC: always its own, in shared memory.
+  float *pl_scratch = !GSRC && b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
   (void)pl_scratch;
 
   const int tid = threadIdx.x, nthr = blockDim.x;
@@ -273,7 +284,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
         for (int j = 0; j < 8; ++j) cnt[tid * 8 + j] = run, run += c[j];
       }
       __syncthreads();
-      for (int i = tid; i < ns; i += nthr) order[atomicAdd(&cnt[bucket(i)], 1)] = (uint16_t)i;
+      for (int i = tid; i < ns; i += nthr) order[atomicAdd(&cnt[bucket(i)], 1)] = (Ord)i;
       __syncthreads();
     }
 

@@ -82,6 +82,9 @@ int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const Icp
 // *limit = the largest target of `dim` columns that icp_run (dim 2: shipped point-to-point chain, no filters) or
 // icp3_run (dim 3) solves in one CTA next to sources of ns points; larger targets take the map class
 int icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit);
+// *limit = the largest source of `dim` columns that icp_run / icp3_run solve in their shared-memory layouts next to
+// targets of any size, for the settings prm and filt (may be null); larger sources take the global-source class
+int icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, int *limit);
 // nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,

@@ -176,8 +176,10 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
     filters: _lib.IcpFilters (sfe_icp_set_filters), default params.filters when params is a parsed _lib.IcpConfig.
 
     Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
-    map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources: at most 65 535
-    points and what fits shared memory (about 7 000).
+    map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources of any size:
+    those above icp_source_limit (what the shared-memory layouts hold, about 8 400 points on an H100) take the
+    global-source class -- their per-point arrays in global memory, every target read from a map grid -- with the same
+    results.
     [total,3] points (both clouds) with [P,4,4] guesses: the 3-D point-to-point chain (sfe_icp_dim_dev), which takes no
     filters, point-to-plane or float64 accumulation."""
     cols = [int(a.shape[1]) if a.dim() == 2 else 0 for a in (src_pts, tgt_pts)]
@@ -212,6 +214,19 @@ def icp_cta_limit(dim, ns, ctx=None, device=0):
     ctx = ctx or context(device)
     out = np.zeros(1, np.int32)
     _lib.check(ctx.lib.sfe_icp_cta_limit(ctx.handle, int(dim), int(ns), _lib.ptr(out)), "sfe_icp_cta_limit")
+    return int(out[0])
+
+
+def icp_source_limit(dim, params=None, filters=None, ctx=None, device=0):
+    """The largest source of `dim` columns icp() solves in its shared-memory layouts next to targets of any size, for
+    `params` (default _lib.IcpParams()) and `filters` (as icp() takes them) on this device (sfe_icp_source_limit).
+    Larger sources take the global-source class."""
+    ctx = ctx or context(device)
+    prm = params or _lib.IcpParams()
+    _lib.set_icp_filters(ctx, _lib.icp_filters_of(prm, filters))
+    out = np.zeros(1, np.int32)
+    _lib.check(ctx.lib.sfe_icp_source_limit(ctx.handle, ctypes.byref(prm), int(dim), _lib.ptr(out)),
+               "sfe_icp_source_limit")
     return int(out[0])
 
 

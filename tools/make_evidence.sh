@@ -40,13 +40,13 @@ fi
 {
   echo "# per call site: ncu source page joined with nvdisasm -gi (tools/ncu_call_sites.py) -- round $rnd, gpurun tag $tag"
   td=$(mktemp -d); (cd $td && cuobjdump -xelf all $OLDPWD/sonar_slam_b200/libsonarfe.so > /dev/null 2>&1)
-  [ -f $G/${tag}_prof_icp_config3.ncu-rep ] && { echo "== icp_kernel<512,1,false,false,false>, 296 problems of 2 000 x 20 000 points"; python tools/ncu_call_sites.py $G/${tag}_prof_icp_config3.ncu-rep icp_kernel $td/icp.sm_90a.cubin icp_kernelILi512ELi1ELb0ELb0ELb0E icp.cu 12; }
+  [ -f $G/${tag}_prof_icp_config3.ncu-rep ] && { echo "== icp_kernel<512,1,false,false,false,false>, 296 problems of 2 000 x 20 000 points"; python tools/ncu_call_sites.py $G/${tag}_prof_icp_config3.ncu-rep icp_kernel $td/icp.sm_90a.cubin icp_kernelILi512ELi1ELb0ELb0ELb0ELb0E icp.cu 12; }
   if [ -f $G/${tag}_prof_pipeline.ncu-rep ]; then
-    echo "== icp_kernel<128,8,false,false,false>, the front end's class, 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi8ELb0ELb0ELb0E icp.cu 12
+    echo "== icp_kernel<128,8,false,false,false,false>, the front end's class, 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi8ELb0ELb0ELb0ELb0E icp.cu 12
     echo "== cart_scatter_kernel, 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep cart_scatter $td/featx.sm_90a.cubin cart_scatter featx.cu 10
     echo "== downsample_cta_kernel (frames), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_pipeline.ncu-rep "downsample#2" $td/cloud.sm_90a.cubin downsample_cta_kernel cloud.cu 12
   fi
-  [ -f $G/${tag}_prof_plane.ncu-rep ] && { echo "== icp_kernel<128,8,true,false,false> (point-to-plane), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_plane.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi8ELb1ELb0ELb0E icp.cu 10; }
+  [ -f $G/${tag}_prof_plane.ncu-rep ] && { echo "== icp_kernel<128,8,true,false,false,false> (point-to-plane), 1024 frames"; python tools/ncu_call_sites.py $G/${tag}_prof_plane.ncu-rep "icp_kernel<(int)128" $td/icp.sm_90a.cubin icp_kernelILi128ELi8ELb1ELb0ELb0ELb0E icp.cu 10; }
   rm -rf $td
 } > $P/${rnd}_call_sites.txt 2>&1 || true
 # SASS excerpt: the interior 16-row block of the pipeline's CFAR kernel + the TMA / mbarrier instructions of the library

@@ -22,7 +22,7 @@ def demangle(names):
 
 
 def short(name):
-    """sfe::icp_kernel<128, 7, false, false, false>(sfe::IcpBatch, sfe::MapArgs) -> icp_kernel<128, 7, false, false, false>"""
+    """sfe::icp_kernel<128, 7, false, false, false, false>(sfe::IcpBatch, sfe::MapArgs) -> icp_kernel<128, 7, false, false, false, false>"""
     name = re.sub(r"^void ", "", name).replace("(anonymous namespace)::", "")
     depth, cut = 0, len(name)
     for i, ch in enumerate(name):  # drop the argument list: the first '(' outside template brackets
