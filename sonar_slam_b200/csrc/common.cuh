@@ -93,7 +93,7 @@ struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)
 namespace sfe {
 // Work counters in ctx->work, one per launch site; launches that may run at the same time (on different streams) use
 // different counters, launches on one stream reuse theirs (each zeroes it first, stream-ordered).
-enum { WORK_CART = 0, WORK_ICP = 1, WORK_DS = 2, SFE_WORK_COUNTERS = 3 };
+enum { WORK_CART = 0, WORK_DS = 1, WORK_ICP = 2, SFE_WORK_COUNTERS = 5 };  // WORK_ICP: three, one per launch class
 
 // (re)allocate if too small, stream-ordered on `stream` (default: ctx->stream).  A buffer must only grow on a stream
 // that is ordered after every earlier user of the block and before every later one: the stream that uses it.

@@ -43,6 +43,18 @@ constexpr float ICP_PRUNED = 3.0e38f;    // "finite, but farther than we needed 
 enum { ICP_OK = 0, ICP_NO_OUTLIER = 1, ICP_NO_POINT = 2, ICP_NAN_ROT = 3, ICP_NAN_TRANS = 4, ICP_NOT_RIGID = 5,
        ICP_EMPTY_REF = 6, ICP_SKIPPED = 7, ICP_TOO_LARGE = 8 };
 
+// The problems one launch takes: those with ns_lo < ns <= ns_hi source and nt_lo < nt <= nt_hi target points.  The
+// launches of one call take disjoint boxes that together hold every problem (icp_split_run), so each problem is solved
+// and its results written by exactly one launch.
+struct IcpBox {
+  int ns_lo, ns_hi, nt_lo, nt_hi;
+};
+constexpr IcpBox ICP_BOX_ALL = {INT_MIN, INT_MAX, INT_MIN, INT_MAX};
+
+__device__ __forceinline__ bool icp_takes(const IcpBox &x, int ns, int nt) {
+  return x.ns_lo < ns && ns <= x.ns_hi && x.nt_lo < nt && nt <= x.nt_hi;
+}
+
 struct IcpBatch {
   const float *src_pts;
   const int *src_off;
@@ -53,10 +65,7 @@ struct IcpBatch {
   int min_points;      // problems whose source or target has fewer points are skipped (ICP_SKIPPED)
   const int *raw_cnt;  // optional: un-clamped size of the source's raw cloud; > raw_cap -> ICP_TOO_LARGE
   int raw_cap;
-  // size classes: a batch can be served by two launches with different shared-memory footprints.
-  //   1: this launch only takes problems that fit (ns <= ns_max, nt <= nt_max) and leaves the others untouched;
-  //   2: this launch skips the problems with ns <= class_ns and nt <= class_nt (the other launch's share)
-  int class_mode, class_ns, class_nt;
+  IcpBox box;         // the problems this launch takes (the others are another launch's; ICP_BOX_ALL: every problem)
   const int *src_id;  // may be null (problem p uses source p)
   const int *tgt_id;  // may be null
   const float *guess; // [P][9] row-major 3x3
@@ -739,13 +748,6 @@ static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool den
   return icp_kernel_of<512, 1, false>(plane, filt);
 }
 
-// Shared memory icp_kernel's layouts may take next to sources of ns_max points: the budget of the instantiation that
-// runs the largest of them.
-static int icp_cta_budget(const sfe_ctx *ctx, int threads, bool plane, bool dense, bool filt, bool map,
-                          size_t *budget) {
-  return cta_smem_budget(ctx, icp_kernel_for(threads, ctx->max_smem_optin, plane, dense, filt, map), budget);
-}
-
 static void icp_tuning(IcpBatch &b) {
   // One-pass exact path (per-lane searches with certified matches, no pruning passes) for problems of up to
   // 5 source points per thread (chosen on the config-4 replay, sources of ~360 points in 128-thread CTAs: a lower
@@ -762,68 +764,6 @@ static void icp_tuning(IcpBatch &b) {
   b.margin_mult = mm;
 }
 
-// One launch of icp_kernel over the batch, laid out for problems of up to ns_max x nt_max points in `threads`-thread
-// CTAs: sized by icp_plan, its workspace (orig_ws, nrm_ws) placed and the kernel enqueued by icp_enqueue.  The map
-// class (icp_plan's map) reads its targets through m, which the caller sets after map_build; in-CTA launches leave m
-// zero.
-struct IcpLaunch {
-  IcpBatch b;
-  MapArgs m;
-  const void *fn;
-  int threads, grid;
-  size_t smem, orig_bytes, ws_bytes;
-};
-
-static int icp_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max, int threads,
-                    IcpLaunch &L, bool dense = false, bool map = false) {
-  b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
-  b.use_order = b.ns_max > 1024;
-  b.cell_scale = 1.0f;
-  b.prm = *prm;
-  icp_tuning(b);
-  const bool plane = prm->minimizer == 1, filt = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f ||
-                                                   b.median_factor >= 0.f;
-  size_t budget;
-  int rc = icp_cta_budget(ctx, threads, plane, dense, filt, map, &budget);
-  if (rc != SFE_OK) return rc;
-  const size_t smem = icp_cta_smem(b.ns_max, b.nt_max, plane, map, budget, &b.max_cells);
-  if (smem > budget) {
-    if (map)
-      set_error("icp: sources of %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, smem, budget);
-    else
-      set_error("icp: source %d + target %d points need %zu B of shared memory per CTA (limit %zu)", ns_max, nt_max,
-                smem, budget);
-    return SFE_ERR_UNSUPPORTED;
-  }
-  const void *fn = icp_kernel_for(threads, smem, plane, dense, filt, map);
-  int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
-  if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
-#ifdef SFE_ICP_PHASE_CLOCKS
-  icp_phase_per_sm[threads == 128 ? 0 : threads == 256 ? 1 : 2] = per_sm;
-#endif
-  int grid = ctx->sm_count * per_sm;
-  if (grid > b.P) grid = b.P;
-  int slots = map ? 0 : grid;  // (the map class has no per-CTA workspace)
-  if (!map && per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;  // one CTA per problem
-  L.orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
-  L.ws_bytes = L.orig_bytes + (plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0);
-  L.b = b, L.m = {}, L.fn = fn, L.threads = threads, L.grid = grid, L.smem = smem;
-  return SFE_OK;
-}
-
-// ws: L.ws_bytes of device memory; next: the launch's work counter, zero when the kernel starts
-static int icp_enqueue(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L, char *ws, int *next) {
-  IcpBatch &b = L.b;
-  b.orig_ws = (uint16_t *)ws;
-  b.nrm_ws = b.prm.minimizer == 1 ? (float2 *)(ws + L.orig_bytes) : nullptr;
-  if (b.src_ws_stride) b.src_ws = (unsigned char *)ws;  // (the global-source class: its slices, nothing else)
-  if (!b.slot_by_smid && (L.grid < b.P || b.list)) b.next = next;  // persistent CTAs; a list is always walked so
-  void *args[] = {(void *)&b, (void *)&L.m};
-  SFE_CUDA(cudaLaunchKernel(L.fn, dim3(L.grid), dim3(L.threads), args, L.smem, st));
-  ctx->launches++;
-  return SFE_OK;
-}
-
 // The global-source class: sources above what the shared-memory layouts hold (icp_source_limit).  Each persistent CTA
 // keeps its per-source-point arrays in a slice of global workspace; all slices together stay within ICP_SRC_WS_CAP.
 constexpr size_t ICP_SRC_WS_CAP = size_t(512) << 20;
@@ -835,52 +775,124 @@ static size_t icp_src_slice(int ns_max) {
   return (28 * n + ((n + 3) & ~size_t(3)) + 255) & ~size_t(255);
 }
 
-// The largest source icp_kernel's shared-memory layouts hold next to targets of any size: the map class's, whose layout
-// holds no target (at most 65 535 points).  Larger sources take the global-source class.
-static int icp2_src_limit(const sfe_ctx *ctx, bool plane, bool filt, int *limit) {
-  size_t budget;
-  int rc = icp_cta_budget(ctx, ICP_THREADS, plane, false, filt, true, &budget);
-  if (rc != SFE_OK) return rc;
-  int mc;
-  *limit = largest_layout(65535, budget, [&](int ns) { return icp_cta_smem(ns, 1, plane, true, budget, &mc); });
-  return SFE_OK;
-}
+}  // namespace sfe
 
-// The global-source launch: icp_kernel<512, 1, PLANE, true, FILT, true> takes the problems whose source has more than
-// class_ns points (IcpBatch::class_mode 2) and reads every target from a map grid (L.m, set by the caller after
-// map_build).  Persistent CTAs: min(P, SMs x CTAs per SM, the slices ICP_SRC_WS_CAP holds), at least one.
-static int icp_gsrc_plan(sfe_ctx *ctx, const sfe_icp_params *prm, IcpBatch b, int ns_max, int nt_max, int class_ns,
-                         IcpLaunch &L) {
-  b.ns_max = ns_max, b.nt_max = nt_max > 0 ? nt_max : 1;
-  b.use_order = 1, b.cell_scale = 1.0f, b.prm = *prm;
-  icp_tuning(b);
-  b.class_mode = 2, b.class_ns = class_ns, b.class_nt = INT_MAX;
-  const size_t slice = icp_src_slice(ns_max);
+#include "icp3.cuh"
+
+namespace sfe {
+// The launch classes of an ICP call: in-CTA (the target's grid in shared memory), map (targets read as map_build's
+// grids) and global-source (map grids, and the per-source-point arrays in a slice of global workspace)
+enum { ICP_CTA = 0, ICP_MAP = 1, ICP_GSRC = 2 };
+
+// One dimension's kernels and layouts: icp_kernel's instantiations for the minimizer and the filters (dim 2), or the
+// icp3_body kernels (dim 3).  filt: sfe_icp_filters (icp_filters_on).
+struct IcpDim {
+  int dim;
+  bool plane, filt;
+  int threads(int cls, int ns) const { return dim == 3 ? ICP3_THREADS : cls == ICP_GSRC ? ICP_THREADS : icp_threads(ns); }
+  // class cls's kernel for `threads`-thread CTAs with `smem` bytes of layout; dense: IcpClass::dense
+  const void *kernel(int cls, int threads, size_t smem, bool dense = false) const {
+    if (dim == 3)
+      return cls == ICP_CTA ? (const void *)icp3_kernel
+             : cls == ICP_MAP ? (const void *)icp3_map_kernel
+                              : (const void *)icp3_gsrc_kernel;
+    if (cls == ICP_GSRC) return icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt);
+    return icp_kernel_for(threads, smem, plane, dense, filt, cls == ICP_MAP);
+  }
+  // shared memory class cls may take next to sources of ns points: the budget of the instantiation that runs the
+  // largest of its layouts
+  int budget(const sfe_ctx *ctx, int cls, int ns, size_t *bytes, bool dense = false) const {
+    return cta_smem_budget(ctx, kernel(cls, threads(cls, ns), ctx->max_smem_optin, dense), bytes);
+  }
+  // class cls's layout for sources of ns and targets of nt points (>= 1); *max_cells: the in-CTA cell table's size
+  size_t smem(int cls, int ns, int nt, size_t budget, int *max_cells) const {
+    *max_cells = 0;
+    if (cls == ICP_GSRC)
+      return dim == 3 ? icp3_gsrc_smem()
+                      : ((sizeof(IcpShared) + 15) & ~size_t(15)) + (plane ? ICP_PLANE_SCRATCH * sizeof(float) : 0);
+    if (dim == 3) return cls == ICP_MAP ? icp3_map_smem(ns) : icp3_cta_smem(ns, nt, budget, max_cells);
+    return icp_cta_smem(ns, nt, plane, cls == ICP_MAP, budget, max_cells);
+  }
+  size_t slice(int ns) const { return dim == 3 ? icp3_src_slice(ns) : icp_src_slice(ns); }
+  const char *what() const { return dim == 3 ? "icp (3-D)" : "icp"; }
+};
+
+// One launch of icp_kernel (IcpBatch) or an icp3_body kernel (Icp3Batch): sized by icp_plan, its workspace placed and
+// the kernel enqueued by icp_enqueue.  Its arguments are b, then the map grids m, which the caller sets after map_build
+// (the in-CTA class ignores them).  Workspace: orig_ws (orig_bytes), then nrm_ws (2-D point-to-plane); or the
+// global-source class's slices.
+template <class Batch>
+struct IcpLaunch {
+  Batch b;
+  MapArgs m;
+  const void *fn;
+  int threads, grid;
+  size_t smem, orig_bytes, ws_bytes;
+};
+
+// A launch of class cls over b's problems, laid out for sources of up to ns_max and targets of up to nt_max points.
+// CTAs are persistent, min(P, SMs x CTAs per SM) of them, and in the global-source class no more than the slices
+// ICP_SRC_WS_CAP holds (at least one) -- except 2-D in-CTA layouts that allow one CTA per SM: one CTA per problem, its
+// workspace indexed by SM (IcpBatch::slot_by_smid).
+template <class Batch>
+static int icp_plan(sfe_ctx *ctx, const IcpDim &d, int cls, Batch b, int ns_max, int nt_max, IcpLaunch<Batch> &L,
+                    bool dense = false) {
+  b.ns_max = ns_max > 0 ? ns_max : 1, b.nt_max = nt_max > 0 ? nt_max : 1;
+  const int threads = d.threads(cls, b.ns_max);
+  const size_t slice = cls == ICP_GSRC ? d.slice(b.ns_max) : 0;
   if (slice > ICP_SRC_WS_CAP) {
-    set_error("icp: a source of %d points needs %zu B of global workspace per CTA (at most %zu)", ns_max, slice,
-              ICP_SRC_WS_CAP);
+    set_error("%s: a source of %d points needs %zu B of global workspace per CTA (at most %zu)", d.what(), b.ns_max,
+              slice, ICP_SRC_WS_CAP);
     return SFE_ERR_UNSUPPORTED;
   }
-  b.src_ws_stride = slice;
-  const bool plane = prm->minimizer == 1,
-             filt = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
-  const void *fn = icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt);
-  const size_t smem = ((sizeof(IcpShared) + 15) & ~size_t(15)) + (plane ? ICP_PLANE_SCRATCH * sizeof(float) : 0);
-  int per_sm;
-  const int rc = ctas_per_sm(ctx, fn, ICP_THREADS, smem, &per_sm);
+  size_t budget;
+  int rc = d.budget(ctx, cls, b.ns_max, &budget, dense);
   if (rc != SFE_OK) return rc;
-  const int grid = std::max(1, std::min({b.P, ctx->sm_count * per_sm, (int)(ICP_SRC_WS_CAP / slice)}));
-  L.b = b, L.m = {}, L.fn = fn, L.threads = ICP_THREADS, L.grid = grid, L.smem = smem;
-  L.orig_bytes = 0, L.ws_bytes = (size_t)grid * slice;
+  const size_t smem = d.smem(cls, b.ns_max, b.nt_max, budget, &b.max_cells);
+  if (smem > budget) {
+    set_error("%s: sources of %d points next to targets of %d need %zu B of shared memory per CTA (limit %zu)",
+              d.what(), ns_max, nt_max, smem, budget);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  const void *fn = d.kernel(cls, threads, smem, dense);
+  int per_sm;  // (the front end calls this per copy chunk: the context caches the query)
+  if ((rc = ctas_per_sm(ctx, fn, threads, smem, &per_sm)) != SFE_OK) return rc;
+#ifdef SFE_ICP_PHASE_CLOCKS
+  if (d.dim == 2) icp_phase_per_sm[threads == 128 ? 0 : threads == 256 ? 1 : 2] = per_sm;
+#endif
+  int grid = std::min(ctx->sm_count * per_sm, b.P), slots = cls == ICP_CTA ? grid : 0;
+  if constexpr (std::is_same_v<Batch, IcpBatch>) {
+    b.use_order = cls == ICP_GSRC || b.ns_max > 1024;
+    if (cls == ICP_CTA && per_sm == 1 && b.P > grid) b.slot_by_smid = 1, slots = ICP_SM_SLOTS, grid = b.P;
+  }
+  if (slice) grid = std::max(1, std::min(grid, (int)(ICP_SRC_WS_CAP / slice))), b.src_ws_stride = slice;
+  L.orig_bytes = ((size_t)slots * b.nt_max * sizeof(uint16_t) + 15) & ~size_t(15);
+  L.ws_bytes = slice ? (size_t)grid * slice : L.orig_bytes + (d.plane ? (size_t)slots * b.nt_max * sizeof(float2) : 0);
+  L.b = b, L.m = {}, L.fn = fn, L.threads = threads, L.grid = grid, L.smem = smem;
   return SFE_OK;
 }
 
-// icp_run's launches without classes: L's workspace at scratch[SCR_ICP], its work counter WORK_ICP
-static int icp_launch(sfe_ctx *ctx, cudaStream_t st, IcpLaunch &L) {
-  int rc = ensure(ctx, ctx->scratch[SCR_ICP], L.ws_bytes, st);
-  if (rc != SFE_OK) return rc;
-  if (!L.b.slot_by_smid && L.grid < L.b.P) SFE_CUDA(cudaMemsetAsync(ctx->work + WORK_ICP, 0, sizeof(int), st));
-  return icp_enqueue(ctx, st, L, (char *)ctx->scratch[SCR_ICP].ptr, ctx->work + WORK_ICP);
+// Whether L's CTAs take their problems from a work counter: fewer persistent CTAs than problems, or a class list (walked
+// from a counter unless the launch runs one CTA per problem)
+template <class Batch>
+static bool icp_counted(const IcpLaunch<Batch> &L) {
+  if constexpr (std::is_same_v<Batch, IcpBatch>)
+    if (L.b.list) return !L.b.slot_by_smid;
+  return L.grid < L.b.P;
+}
+
+// ws: L.ws_bytes of device memory; next: the launch's work counter, zero when the kernel starts (icp_counted)
+template <class Batch>
+static int icp_enqueue(sfe_ctx *ctx, cudaStream_t st, IcpLaunch<Batch> &L, char *ws, int *next) {
+  Batch &b = L.b;
+  b.orig_ws = (uint16_t *)ws;
+  if constexpr (std::is_same_v<Batch, IcpBatch>) b.nrm_ws = b.prm.minimizer == 1 ? (float2 *)(ws + L.orig_bytes) : nullptr;
+  if (b.src_ws_stride) b.src_ws = (unsigned char *)ws;  // (the global-source class: its slices, nothing else)
+  if (icp_counted(L)) b.next = next;
+  void *args[] = {(void *)&b, (void *)&L.m};
+  SFE_CUDA(cudaLaunchKernel(L.fn, dim3(L.grid), dim3(L.threads), args, L.smem, st));
+  ctx->launches++;
+  return SFE_OK;
 }
 
 // Work lists of icp_run's classes.  Problem p goes to the first class c whose bounds it fits (the last class takes
@@ -951,9 +963,9 @@ __global__ void icp_class_of_kernel(const int *lists, const int *n, int n_classe
 }
 
 // icp_run's class path: the classify kernel, then one launch per class, the widest first
-static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpBatch &b,
-                           const IcpClass *classes, int n_classes, int ns_max, int nt_max, int *class_of) {
-  IcpLaunch L[ICP_MAX_CLASSES + 1];
+static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const IcpDim &d, const IcpBatch &b, const IcpClass *classes,
+                           int n_classes, int ns_max, int nt_max, int *class_of) {
+  IcpLaunch<IcpBatch> L[ICP_MAX_CLASSES + 1];
   IcpClassBounds cb{};
   cb.n = n_classes + 1;
   size_t ws_bytes = 0;
@@ -962,7 +974,7 @@ static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *
     cb.ns[c] = cap ? ns_max : std::min(classes[c].ns, ns_max);
     cb.nt[c] = cap ? nt_max : std::min(classes[c].nt, nt_max);
     const int threads = icp_threads(cb.ns[c] > 0 ? cb.ns[c] : 1);
-    int rc = icp_plan(ctx, prm, b, cb.ns[c], cb.nt[c], threads, L[c], !cap && classes[c].dense && threads == 128);
+    int rc = icp_plan(ctx, d, ICP_CTA, b, cb.ns[c], cb.nt[c], L[c], !cap && classes[c].dense && threads == 128);
     if (rc != SFE_OK) return rc;
     ws_bytes = std::max(ws_bytes, L[c].ws_bytes);  // (the launches run one after the other)
   }
@@ -988,20 +1000,6 @@ static int icp_run_classes(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *
   return SFE_OK;
 }
 
-// The largest target icp_kernel's layout holds next to sources of ns points (the map class takes larger ones)
-static int icp2_limit(const sfe_ctx *ctx, int ns, bool plane, bool filt, int *limit) {
-  ns = ns > 0 ? ns : 1;
-  size_t budget;
-  int rc = icp_cta_budget(ctx, icp_threads(ns), plane, false, filt, false, &budget);
-  if (rc != SFE_OK) return rc;
-  int mc;
-  *limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) {
-    return icp_cta_smem(ns, nt, plane, false, budget, &mc);
-  });
-  return SFE_OK;
-}
-
-
 // A persistent launch of fn over P problems: ctas_per_sm CTAs per SM, at most one per problem
 static int persistent_grid(sfe_ctx *ctx, const void *fn, int threads, size_t smem, int P, int *grid) {
   int per_sm;
@@ -1011,63 +1009,139 @@ static int persistent_grid(sfe_ctx *ctx, const void *fn, int threads, size_t sme
   return SFE_OK;
 }
 
-// The one-CTA kernel of split_run: fn (null: no one-CTA launch) in `threads`-thread CTAs with `smem` bytes of layout
-// for targets of up to nt points (>= 1); counted: it takes its problems from a work counter when its grid is smaller
-// than P.
+// The one-CTA kernel of split_run: fn in `threads`-thread CTAs with `smem` bytes of layout for targets of up to nt
+// points (>= 1)
 struct SplitCta {
   const void *fn;
   int threads;
   size_t smem;
   int nt;
-  bool counted;
 };
 
-// One call of P problems split at `limit` target points (icp3_run, match_run, match_knn_run): the one-CTA kernel takes
-// the targets of up to `limit` points in a persistent launch (persistent_grid), each CTA with a row of c.nt original
-// indices (orig_ws); when the largest target, tgt.n_max, is above map_limit (`limit`, or 0 when icp3_run's
-// global-source class reads every target as a map grid), map_build builds map grids of the targets above map_limit
-// (`dim` columns; problem p's target tgt_id[p], or p with tgt_id null; slot_cap distinct ones; centred or not) and the
-// map class reads them.  Workspace, scratch[SCR_ICP]: [256 B of work counters][orig_ws][the map class's `extra` bytes];
-// with c.counted the first two counters are zeroed whenever a launch may take problems from them.
-// cta(grid, orig_ws, next) enqueues the one-CTA kernel (next: its work counter, or null);
-// map(MapWs, extra workspace, next) enqueues the map class, last the kernel split_run counts (next: the second work
-// counter; the ones after it are free) and returns an SFE_* code.
+// One call of P problems split at `limit` target points (match_run, match_knn_run): the one-CTA kernel takes the targets
+// of up to `limit` points in a persistent launch (persistent_grid), each CTA with a row of c.nt original indices
+// (orig_ws, in scratch[SCR_ICP]); when the largest target, tgt.n_max, is above `limit`, map_build builds map grids of
+// the larger ones (`dim` columns, problem p's target is cloud p, not centred) and the map class reads them.
+// cta(grid, orig_ws) enqueues the one-CTA kernel; map(MapWs) enqueues the map class and returns an SFE_* code.
 template <typename Cta, typename Map>
-static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, int limit, int map_limit,
-                     const PackedClouds &tgt, int dim, const int *tgt_id, int slot_cap, bool center, size_t extra,
-                     Cta cta, Map map) {
-  const bool map_class = tgt.n_max > map_limit;
-  int grid = 0, rc;
-  if (c.fn && (rc = persistent_grid(ctx, c.fn, c.threads, c.smem, P, &grid)) != SFE_OK) return rc;
-  const size_t head = 256, orig_bytes = ((size_t)grid * c.nt * sizeof(uint16_t) + 255) & ~size_t(255);
-  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP], head + orig_bytes + (map_class ? extra : 0), st)) != SFE_OK) return rc;
-  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
-  int *next = (int *)base;
-  if (c.counted && (grid < P || map_class)) SFE_CUDA(cudaMemsetAsync(next, 0, 2 * sizeof(int), st));
-  if (c.fn) {
-    cta(grid, (uint16_t *)(base + head), c.counted && grid < P ? next : nullptr);
-    SFE_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
-  if (!map_class) return SFE_OK;
+static int split_run(sfe_ctx *ctx, cudaStream_t st, const SplitCta &c, int P, int limit, const PackedClouds &tgt,
+                     int dim, Cta cta, Map map) {
+  int grid, rc;
+  if ((rc = persistent_grid(ctx, c.fn, c.threads, c.smem, P, &grid)) != SFE_OK) return rc;
+  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP], (size_t)grid * c.nt * sizeof(uint16_t), st)) != SFE_OK) return rc;
+  cta(grid, (uint16_t *)ctx->scratch[SCR_ICP].ptr);
+  SFE_CUDA(cudaGetLastError());
+  ctx->launches++;
+  if (tgt.n_max <= limit) return SFE_OK;
   MapWs w;
-  if ((rc = map_build(ctx, st, tgt, dim, tgt_id, P, map_limit, slot_cap, center, true, 0, w)) != SFE_OK) return rc;
-  if ((rc = map(w, base + head + orig_bytes, next + 1)) != SFE_OK) return rc;
+  if ((rc = map_build(ctx, st, tgt, dim, nullptr, P, limit, P, false, true, 0, w)) != SFE_OK) return rc;
+  if ((rc = map(w)) != SFE_OK) return rc;
   SFE_CUDA(cudaGetLastError());
   ctx->launches++;
   return SFE_OK;
 }
 
-}  // namespace sfe
+// How a call of sources of up to ns_max and targets of up to nt_max points splits into launches (icp_run without
+// classes, icp3_run; icp_cta_limit and icp_source_limit report its limits).  S: the largest source the map class's
+// layout holds (at most 65 535 points).  L: the largest target the in-CTA layout holds next to sources of ns_lay points,
+// the size both shared-memory launches are laid out for.  Sources above S take the global-source launch -- unless every
+// target fits the in-CTA layout next to them (it holds a few more source points than the map class's), and ns_lay is
+// then S.  L = 0 (MAP_CLASS_ALL): no in-CTA launch, the map launch takes every target.
+struct IcpSplit {
+  int S, L, ns_lay;
+  bool cta, map, gsrc;
+};
 
-#include "icp3.cuh"
+static int icp_split(const sfe_ctx *ctx, const IcpDim &d, int ns_max, int nt_max, IcpSplit &s) {
+  size_t budget;
+  int mc, rc = d.budget(ctx, ICP_MAP, 65535, &budget);  // (sources that large run in the widest CTAs)
+  if (rc != SFE_OK) return rc;
+  s.S = largest_layout(65535, budget, [&](int ns) { return d.smem(ICP_MAP, ns, 1, budget, &mc); });
+  auto cta_limit = [&](int ns, int *L) -> int {
+    *L = 0;
+    if (MAP_CLASS_ALL || ns > 65535) return SFE_OK;
+    const int rc = d.budget(ctx, ICP_CTA, ns, &budget);
+    if (rc == SFE_OK) *L = largest_layout(65535, budget, [&](int nt) { return d.smem(ICP_CTA, ns, nt, budget, &mc); });
+    return rc;
+  };
+  s.ns_lay = ns_max > 0 ? ns_max : 1;
+  if ((rc = cta_limit(s.ns_lay, &s.L)) != SFE_OK) return rc;
+  s.gsrc = s.ns_lay > s.S && !(s.L > 0 && nt_max <= s.L);
+  if (s.gsrc) {
+    s.ns_lay = s.S;
+    if ((rc = cta_limit(s.S, &s.L)) != SFE_OK) return rc;
+  }
+  s.cta = s.L > 0;
+  s.map = !s.cta || nt_max > s.L;
+  return SFE_OK;
+}
 
-// Size classes: every listed class gets a launch laid out for it, whose smaller shared-memory footprint fits more
-// CTAs per SM, and a last launch, laid out for the capacities src.n_max x tgt.n_max, takes the problems that fit none
-// (and reports oversize ones, SFE_ICP_TOO_LARGE).  Without classes one launch takes every problem (IcpBatch::class_mode
-// 0) -- unless the largest target does not fit icp_kernel's layout: then that launch takes the targets up to its limit
-// (class_mode 1) and the map class (map grids in global memory, icp_kernel's MAP instantiations) takes the rest.
-namespace sfe {
+// Enqueues the launches of icp_split's s on st, in this order: the in-CTA launch; map_build, when a launch reads map
+// grids (the map launch: the targets above L; the global-source launch: every target); dim 3: the grids' z
+// (icp3_map_z_kernel); the map launch; the global-source launch.  Their boxes partition the problems:
+//   without a global-source launch: in-CTA {nt <= L}, map {nt > L} (every nt when there is no in-CTA launch);
+//   with one: in-CTA {ns <= S, nt <= L}, map {ns <= S, nt > L}, global-source {ns > S}.
+// (A launch with no neighbour on one side takes everything on that side.)  Admission reports the sources above
+// src.n_max and the targets above tgt.n_max SFE_ICP_TOO_LARGE in whichever launch takes them.  Workspace,
+// scratch[SCR_ICP]: [dim 3 with map grids: the centred z of every map-grid position, the z mean of every slot][the
+// workspace of one launch at a time]; launch k takes its problems from the work counter ctx->work[WORK_ICP + k].
+template <class Batch>
+static int icp_split_run(sfe_ctx *ctx, cudaStream_t st, const IcpDim &d, const IcpSplit &s, Batch b,
+                         const IcpProblems &pb) {
+  const int nt_max = pb.tgt.n_max, ns_hi = s.gsrc ? s.S : INT_MAX;
+  const bool run[3] = {s.cta, s.map, s.gsrc};
+  const IcpBox box[3] = {{INT_MIN, ns_hi, INT_MIN, s.map ? s.L : INT_MAX},
+                         {INT_MIN, ns_hi, s.cta ? s.L : INT_MIN, INT_MAX},
+                         {s.S, INT_MAX, INT_MIN, INT_MAX}};
+  const int ns[3] = {s.ns_lay, s.ns_lay, pb.src.n_max}, nt[3] = {std::min(nt_max, s.L), nt_max, nt_max};
+  IcpLaunch<Batch> L[3];
+  size_t ws = 0;
+  bool counted = false;
+  int rc;
+  for (int k = 0; k < 3; ++k) {
+    if (!run[k]) continue;
+    b.box = box[k];
+    if ((rc = icp_plan(ctx, d, k, b, ns[k], nt[k], L[k])) != SFE_OK) return rc;
+    // (with no target points every problem fails admission before the global-source launch touches a slice)
+    if (k == ICP_GSRC && nt_max == 0) L[k].ws_bytes = 0;
+    ws = std::max(ws, L[k].ws_bytes), counted = counted || icp_counted(L[k]);
+  }
+  const int grid_limit = s.gsrc ? 0 : s.L;  // (the global-source launch reads every target as a map grid)
+  const bool grids = nt_max > grid_limit;
+  const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
+  const size_t z_bytes = ((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255);
+  const size_t side = grids && d.dim == 3 ? (z_bytes + sizeof(float) * slot_cap + 255) & ~size_t(255) : 0;
+  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP], side + ws, st)) != SFE_OK) return rc;
+  char *base = (char *)ctx->scratch[SCR_ICP].ptr;
+  int *next = ctx->work + WORK_ICP;
+  if (counted) SFE_CUDA(cudaMemsetAsync(next, 0, 3 * sizeof(int), st));
+  if (s.cta && (rc = icp_enqueue(ctx, st, L[ICP_CTA], base + side, next + ICP_CTA)) != SFE_OK) return rc;
+  MapWs w{};
+  if (grids) {
+    const int knn = d.plane ? std::min(std::max(b.prm.normals_knn, 1), GRID_KNN_MAX) : 0;
+    rc = map_build(ctx, st, pb.tgt, d.dim, pb.tgt_id, pb.P, grid_limit, slot_cap, true, (b.prm.flags & 2) == 0, knn, w);
+    if (rc != SFE_OK) return rc;
+    if constexpr (std::is_same_v<Batch, Icp3Batch>) {
+      float *zs = (float *)base, *zm = (float *)(base + z_bytes);
+      icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
+      SFE_CUDA(cudaGetLastError());
+      ctx->launches++;
+      for (int k = ICP_MAP; k <= ICP_GSRC; ++k) L[k].b.map_z = zs, L[k].b.map_zm = zm;
+    }
+  }
+  for (int k = ICP_MAP; k <= ICP_GSRC; ++k) {
+    if (!run[k]) continue;
+    L[k].m = w.args();
+    if ((rc = icp_enqueue(ctx, st, L[k], base + side, next + k)) != SFE_OK) return rc;
+  }
+  return SFE_OK;
+}
+
+// Whether a call with the filters f (may be null) runs icp_kernel's FILT instantiations
+static bool icp_filters_on(const sfe_icp_filters *f) {
+  return f && (f->n_reading > 0 || f->n_reference > 0 || f->min_dist >= 0.f || f->median_factor >= 0.f);
+}
+
 // Data filters: the clouds of one side of the batch, compacted into scratch[SCR_ICP_FILTER] (icp_data_filter_kernel),
 // once per cloud when the cloud count is known (no ids: one per problem), else once per problem (the ids then name the
 // compacted clouds no more).  Two passes over the Carver: the first sizes the block, the second launches.
@@ -1092,6 +1166,11 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const IcpDataFilters &
 }
 }  // namespace sfe
 
+// Size classes: every listed class gets a launch laid out for it, whose smaller shared-memory footprint fits more
+// CTAs per SM, and a last launch, laid out for the capacities src.n_max x tgt.n_max, takes the problems that fit none
+// (and reports oversize ones, SFE_ICP_TOO_LARGE).  Without classes the launches of icp_split_run partition the
+// problems: in-CTA, map class (targets above the in-CTA layout's limit, read as map grids from global memory) and
+// global-source class (sources above the shared-memory layouts).
 int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb_in,
                  const IcpClass *class_list, int n_classes, int *class_of, const sfe_icp_filters *filt) {
   IcpProblems pb = pb_in;
@@ -1150,82 +1229,43 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P;
-  if (classes) return icp_run_classes(ctx, st, prm, b, class_list, n_classes, ns_max, nt_max, class_of);
-  // the largest target icp_kernel's layout holds next to these sources: targets above it are the map class
-  const bool plane = prm->minimizer == 1;
-  const bool filt_on = b.gate_src_cnt || b.gate_tgt_cnt || b.min_d2 >= 0.f || b.median_factor >= 0.f;
-  int ns = ns_max > 0 ? ns_max : 1, limit = 0, src_limit;
-  if ((rc = icp2_src_limit(ctx, plane, filt_on, &src_limit)) != SFE_OK) return rc;
-  if (ns <= 65535 && (rc = icp2_limit(ctx, ns, plane, filt_on, &limit)) != SFE_OK) return rc;
-  // Sources above src_limit take the global-source class -- unless every target fits an in-CTA layout next to them
-  // (the in-CTA layout holds a few more source points than the map class's next to small targets).  The shared-memory
-  // launches are then laid out for src_limit-point sources and report the larger ones SFE_ICP_TOO_LARGE at admission;
-  // the global-source launch, enqueued after them on the same stream, solves those problems and writes their results
-  // over that status.
-  const bool gsrc = ns > src_limit && !(limit > 0 && nt_max <= limit);
-  IcpLaunch L, G;
-  if (gsrc) {
-    if ((rc = icp_gsrc_plan(ctx, prm, b, ns_max, nt_max, src_limit, G)) != SFE_OK) return rc;
-    ns = src_limit;
-    if ((rc = icp2_limit(ctx, ns, plane, filt_on, &limit)) != SFE_OK) return rc;
-  }
-  const int ns_cta = gsrc ? src_limit : ns_max, threads = icp_threads(ns);
-  if ((nt_max <= limit && !gsrc) || limit > 0) {
-    b.class_mode = nt_max <= limit && !gsrc ? 0 : 1;
-    if ((rc = icp_plan(ctx, prm, b, ns_cta, std::min(nt_max, limit), threads, L)) != SFE_OK) return rc;
-    if ((rc = icp_launch(ctx, st, L)) != SFE_OK) return rc;
-  }
-  if (nt_max <= limit && !gsrc) return SFE_OK;
-  // the map class takes the other problems; with no in-CTA launch (limit 0) all of them (targets of 0 points are then
-  // reported here, SFE_ICP_EMPTY_REF, before any map grid is read)
-  const bool map_class = nt_max > limit;
-  if (map_class) {
-    b.class_mode = limit > 0 ? 2 : 0, b.class_ns = ns, b.class_nt = limit;
-    if ((rc = icp_plan(ctx, prm, b, ns_cta, nt_max, threads, L, false, true)) != SFE_OK) return rc;
-  }
-  // (the global-source class reads every target from a map grid; with no target points at all it reads none)
-  MapWs w{};
-  if (nt_max > 0) {
-    const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-    rc = map_build(ctx, st, {b.tgt_pts, b.tgt_off, b.tgt_cnt, nt_max}, 2, b.tgt_id, b.P, gsrc ? 0 : limit, slot_cap,
-                   true, (prm->flags & 2) == 0, plane ? std::min(std::max(prm->normals_knn, 1), GRID_KNN_MAX) : 0, w);
-    if (rc != SFE_OK) return rc;
-  }
-  if (map_class) {
-    L.m = w.args();
-    if ((rc = icp_launch(ctx, st, L)) != SFE_OK) return rc;
-  }
-  if (!gsrc) return SFE_OK;
-  G.m = w.args();
-  return icp_launch(ctx, st, G);
+  b.box = ICP_BOX_ALL;
+  b.cell_scale = 1.0f, b.prm = *prm;
+  icp_tuning(b);
+  const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt)};
+  if (classes) return icp_run_classes(ctx, st, d, b, class_list, n_classes, ns_max, nt_max, class_of);
+  IcpSplit s;
+  if ((rc = icp_split(ctx, d, ns_max, nt_max, s)) != SFE_OK) return rc;
+  return icp_split_run(ctx, st, d, s, b, pb);
 }
 
 int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
   SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
   SFE_REQUIRE(ns >= 0 && ns <= 65535, "icp: sources of %d points are not supported (0..65535)", ns);
-  return dim == 2 ? icp2_limit(ctx, ns, false, false, limit) : icp3_limit(ctx, ns > 0 ? ns : 1, limit);
+  IcpSplit s;
+  const int rc = icp_split(ctx, {dim, false, false}, ns, 0, s);
+  if (rc == SFE_OK) *limit = s.gsrc ? 0 : s.L;  // (a global-source launch: no in-CTA layout holds these sources)
+  return rc;
 }
 
 int sfe::icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt,
                           int *limit) {
   SFE_REQUIRE(ctx && prm && limit, "icp_source_limit: null pointer");
   SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
-  const int rc = icp_params_check(prm, dim, filt, "icp_source_limit");
+  int rc = icp_params_check(prm, dim, filt, "icp_source_limit");
   if (rc != SFE_OK) return rc;
-  if (dim == 3) return icp3_src_limit(ctx, limit);
-  // (icp_run's choice of the FILT instantiations)
-  const bool filt_on = filt && (filt->n_reading > 0 || filt->n_reference > 0 || filt->min_dist >= 0.f ||
-                                filt->median_factor >= 0.f);
-  return icp2_src_limit(ctx, prm->minimizer == 1, filt_on, limit);
+  IcpSplit s;
+  if ((rc = icp_split(ctx, {dim, prm->minimizer == 1, icp_filters_on(filt)}, 1, 0, s)) == SFE_OK) *limit = s.S;
+  return rc;
 }
 
-// [x, y, z] clouds: targets up to icp3_limit in icp3_kernel (one CTA, its grid in shared memory), larger ones as map
-// grids (map_build with dim 3, plus their z by sorted position) in icp3_map_kernel, in the same call.
+// [x, y, z] clouds: the launches of icp_split_run -- icp3_kernel (one CTA, the target's grid in shared memory),
+// icp3_map_kernel (targets as map grids from map_build with dim 3, plus their z by grid position) and icp3_gsrc_kernel
+// (sources above the shared-memory layouts) -- as in icp_run.
 int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
                   const sfe_icp_filters *filt) {
-  const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
   SFE_REQUIRE(ctx && prm, "icp (3-D): null context or parameters");
-  SFE_REQUIRE(pb.P >= 0 && ns_max >= 0 && nt_max >= 0, "icp (3-D): negative sizes");
+  SFE_REQUIRE(pb.P >= 0 && pb.src.n_max >= 0 && pb.tgt.n_max >= 0, "icp (3-D): negative sizes");
   int rc = icp_params_check(prm, 3, filt, "icp (3-D)");
   if (rc != SFE_OK) return rc;
   if (pb.P == 0) return SFE_OK;
@@ -1233,98 +1273,15 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
                   pb.status,
               "icp (3-D): null pointer");
   SFE_REQUIRE(!pb.src.cnt && !pb.tgt.cnt, "icp (3-D): per-cloud counts are not supported");
-  int ns = ns_max > 0 ? ns_max : 1, limit = 0, src_limit;
-  if ((rc = icp3_src_limit(ctx, &src_limit)) != SFE_OK) return rc;
-  if (ns <= 65535 && (rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
   Icp3Batch b{};
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P, b.prm = *prm;
-  // Sources above src_limit take the global-source class (icp3_gsrc_kernel), as in icp_run: unless every target fits
-  // icp3_kernel next to them, the shared-memory launches are laid out for src_limit-point sources and report the larger
-  // ones SFE_ICP_TOO_LARGE, and the global-source launch, enqueued last, solves those and writes over that status.
-  const bool gsrc = ns > src_limit && !(limit > 0 && nt_max <= limit);
-  Icp3Batch g = b;
-  int g_grid = 0;
-  size_t g_bytes = 0;
-  if (gsrc) {
-    g.ns_max = ns_max, g.nt_max = nt_max > 0 ? nt_max : 1, g.class_ns = src_limit;
-    g.src_ws_stride = icp3_src_slice(ns_max);
-    if (g.src_ws_stride > ICP_SRC_WS_CAP) {
-      set_error("icp (3-D): a source of %d points needs %zu B of global workspace per CTA (at most %zu)", ns_max,
-                g.src_ws_stride, ICP_SRC_WS_CAP);
-      return SFE_ERR_UNSUPPORTED;
-    }
-    if ((rc = persistent_grid(ctx, (const void *)icp3_gsrc_kernel, ICP3_THREADS, icp3_gsrc_smem(), pb.P, &g_grid)) !=
-        SFE_OK)
-      return rc;
-    g_grid = std::max(1, std::min(g_grid, (int)(ICP_SRC_WS_CAP / g.src_ws_stride)));
-    g_bytes = (size_t)g_grid * g.src_ws_stride;
-    ns = src_limit;
-    if ((rc = icp3_limit(ctx, ns, &limit)) != SFE_OK) return rc;
-  }
-  b.ns_max = ns;
-  const bool map = nt_max > limit;
-  const size_t map_smem = icp3_map_smem(ns);
-  if ((map && map_smem > (size_t)ctx->max_smem_optin) || (limit == 0 && !map)) {
-    set_error("icp (3-D): sources of %d points need %zu B of shared memory per CTA (limit %d)", ns_max, map_smem,
-              ctx->max_smem_optin);
-    return SFE_ERR_UNSUPPORTED;
-  }
-  const int slot_cap = pb.n_tgt_clouds > 0 ? std::min(pb.n_tgt_clouds, pb.P) : pb.P;
-  const int nt_cta = std::min(nt_max, limit);
-  b.nt_max = nt_cta > 0 ? nt_cta : 1, b.class_nt = b.nt_max;
-  size_t cta_smem = 0;
-  if (limit > 0) {
-    size_t budget;
-    if ((rc = cta_smem_budget(ctx, (const void *)icp3_kernel, &budget)) != SFE_OK) return rc;
-    cta_smem = icp3_cta_smem(ns, b.nt_max, budget, &b.max_cells);
-  }
-  // the map class's workspace: z by map-grid position, z mean per slot; then the global-source class's slices
-  const size_t z_bytes = ((size_t)slot_cap * nt_max * sizeof(float) + 255) & ~size_t(255);
-  const size_t g_off = (z_bytes + sizeof(float) * slot_cap + 255) & ~size_t(255);
-  auto gsrc_launch = [&](const MapArgs &m, unsigned char *ws, int *next) -> int {
-    g.src_ws = ws;
-    g.next = g_grid < pb.P ? next : nullptr;
-    if (g.next) SFE_CUDA(cudaMemsetAsync(next, 0, sizeof(int), st));
-    icp3_gsrc_kernel<<<g_grid, ICP3_THREADS, icp3_gsrc_smem(), st>>>(g, m);
-    return SFE_OK;
-  };
-  rc = split_run(
-      ctx, st, {limit > 0 ? (const void *)icp3_kernel : nullptr, ICP3_THREADS, cta_smem, b.nt_max, true}, pb.P, limit,
-      gsrc ? 0 : limit, {pb.tgt.pts, pb.tgt.off, nullptr, nt_max}, 3, pb.tgt_id, slot_cap, true,
-      gsrc ? g_off + g_bytes : z_bytes + sizeof(float) * slot_cap,
-      [&](int grid, uint16_t *orig_ws, int *next) {
-        b.orig_ws = orig_ws, b.next = next;
-        icp3_kernel<<<grid, ICP3_THREADS, cta_smem, st>>>(b);
-      },
-      [&](const MapWs &w, char *ws, int *next) -> int {
-        float *zs = (float *)ws, *zm = (float *)(ws + z_bytes);
-        icp3_map_z_kernel<<<slot_cap, ICP3_THREADS, 0, st>>>(pb.tgt.pts, pb.tgt.off, w, zs, zm);
-        SFE_CUDA(cudaGetLastError());
-        ctx->launches++;
-        if (map) {
-          b.nt_max = nt_max, b.class_nt = limit, b.map_z = zs, b.map_zm = zm;
-          int grid;
-          const int rc = persistent_grid(ctx, (const void *)icp3_map_kernel, ICP3_THREADS, map_smem, pb.P, &grid);
-          if (rc != SFE_OK) return rc;
-          b.next = grid < pb.P ? next : nullptr;
-          icp3_map_kernel<<<grid, ICP3_THREADS, map_smem, st>>>(b, w.args());
-          if (!gsrc) return SFE_OK;  // (split_run counts the last launch)
-          SFE_CUDA(cudaGetLastError());
-          ctx->launches++;
-        }
-        g.map_z = zs, g.map_zm = zm;
-        return gsrc_launch(w.args(), (unsigned char *)ws + g_off, next + 1);
-      });
-  if (rc != SFE_OK || !gsrc || nt_max > 0) return rc;
-  // no target points at all: the global-source launch reports its problems (SFE_ICP_EMPTY_REF, or before that
-  // SFE_ICP_TOO_LARGE / SFE_ICP_NOT_RIGID) without reading a map grid or its slices
-  if ((rc = gsrc_launch(MapArgs{}, nullptr, ctx->work + WORK_ICP)) != SFE_OK) return rc;
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  return SFE_OK;
+  const IcpDim d{3, false, false};
+  IcpSplit s;
+  if ((rc = icp_split(ctx, d, pb.src.n_max, pb.tgt.n_max, s)) != SFE_OK) return rc;
+  return icp_split_run(ctx, st, d, s, b, pb);
 }
 
 // References that fit one CTA's shared memory run in match_kernel, larger ones (whole maps) as map grids in
@@ -1355,13 +1312,13 @@ int sfe::match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const
     return SFE_ERR_UNSUPPORTED;
   }
   return split_run(
-      ctx, st, {(const void *)match_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, limit,
-      {ref.pts, ref.off, nullptr, nt_max}, 2, nullptr, P, false, 0,
-      [&](int grid, uint16_t *orig_ws, int *) {
+      ctx, st, {(const void *)match_kernel, ICP_THREADS, smem, b.nt_max}, P, limit, {ref.pts, ref.off, nullptr, nt_max},
+      2,
+      [&](int grid, uint16_t *orig_ws) {
         b.orig_ws = orig_ws;
         match_kernel<<<grid, ICP_THREADS, smem, st>>>(b);
       },
-      [&](const MapWs &w, char *, int *) -> int {
+      [&](const MapWs &w) -> int {
         b.map = w.args();
         match_map_kernel<<<ctx->sm_count * 4, ICP_THREADS, 0, st>>>(b);
         return SFE_OK;
@@ -1401,14 +1358,13 @@ int sfe::match_knn_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, c
     return SFE_ERR_UNSUPPORTED;
   }
   return split_run(
-      ctx, st, {cta_kernel, ICP_THREADS, smem, b.nt_max, false}, P, limit, limit, {ref.pts, ref.off, nullptr, nt_max},
-      dim, nullptr, P, false, 0,
-      [&](int grid, uint16_t *orig_ws, int *) {
+      ctx, st, {cta_kernel, ICP_THREADS, smem, b.nt_max}, P, limit, {ref.pts, ref.off, nullptr, nt_max}, dim,
+      [&](int grid, uint16_t *orig_ws) {
         b.orig_ws = orig_ws;
         if (dim == 3) match_knn_kernel<3><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
         else match_knn_kernel<2><<<grid, ICP_THREADS, smem, st>>>(b, knn, (int)list_off(b.nt_max));
       },
-      [&](const MapWs &w, char *, int *) -> int {
+      [&](const MapWs &w) -> int {
         b.map = w.args();
         const size_t map_lists = (size_t)ICP_THREADS * knn * (sizeof(float) + sizeof(int));
         const void *map_kernel = dim == 3 ? (const void *)match_knn_map_kernel<3> : (const void *)match_knn_map_kernel<2>;

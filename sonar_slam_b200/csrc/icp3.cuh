@@ -1,8 +1,8 @@
 // 3-D scan matcher (sm_90a): bruce_slam.pcl.ICP.compute on [x, y, z] clouds with 4x4 guesses, point-to-point.
-// Included by icp.cu only, after its helpers (IcpShared, block_select_kth, block_total, seq_sum9_warp, the map-class
-// arguments).  Algorithm statement and conventions: oracle/icp3_ref.c (same steps, same float32 expressions; every
-// product, sum, quotient and square root below is an IEEE-rounded _rn operation, so no contraction differs from the
-// oracle's -ffp-contract=off).
+// Included by icp.cu only, after its helpers (IcpBox, IcpShared, block_select_kth, block_total, seq_sum9_warp, the
+// map-class arguments, pick_max_cells).  Algorithm statement and conventions: oracle/icp3_ref.c (same steps, same
+// float32 expressions; every product, sum, quotient and square root below is an IEEE-rounded _rn operation, so no
+// contraction differs from the oracle's -ffp-contract=off).
 //
 // One CTA solves one (source, target, guess) problem, persistent over the problem list from a work counter.  The
 // target is centred on its mean and counting-sorted into grid.cuh's grid of x, y; z is kept by sorted position next
@@ -29,15 +29,14 @@ struct Icp3Batch {
   float *T_out;                // [P][16]
   int *iters, *inliers, *status;
   int P, ns_max, nt_max, max_cells;
-  int class_nt;  // in-CTA kernel: takes the targets of at most class_nt points; map kernel: the larger ones (0: all)
+  IcpBox box;  // the problems this launch takes (icp_takes)
   sfe_icp_params prm;
   uint16_t *orig_ws;     // in-CTA: [grid][nt_max] original index of every sorted position
   int *next;             // work counter, or null: CTA c takes problems c, c + gridDim.x, ...
   const float *map_z;    // map class: centred z of every map-grid position
   const float *map_zm;   // map class: z mean of every slot
-  // global-source class (icp3_gsrc_kernel): takes the problems whose source has more than class_ns points; CTA c keeps
-  // reading, dist and match at src_ws + c * src_ws_stride in global memory
-  int class_ns;
+  // global-source class (icp3_gsrc_kernel): CTA c keeps reading, dist and match at src_ws + c * src_ws_stride in global
+  // memory
   unsigned char *src_ws;
   size_t src_ws_stride;
 };
@@ -344,17 +343,12 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp)
     const float *tgt = b.tgt_pts + 3 * (size_t)b.tgt_off[ti];
     const int nt = b.tgt_off[ti + 1] - b.tgt_off[ti];
     const float *guess = b.guess + 16 * (size_t)p;
-    if constexpr (GSRC) {
-      if (ns <= b.class_ns) continue;  // the shared-memory classes'
-    } else {
-      if (!MAP && nt > b.class_nt) continue;             // the map class's
-      if (MAP && b.class_nt > 0 && nt <= b.class_nt) continue;  // the in-CTA class's
-    }
+    if (!icp_takes(b.box, ns, nt)) continue;  // another launch's
     __syncthreads();  // previous problem fully retired before shared state is reused
 
     if (tid == 0) {  // admission: failure leaves T = guess
       int st = ICP_OK;
-      if (ns > b.ns_max) st = ICP_TOO_LARGE;
+      if (ns > b.ns_max || nt > b.nt_max) st = ICP_TOO_LARGE;
       else if (nt <= 0) st = ICP_EMPTY_REF;
       else if (!(fabsf(__fsub_rn(1.0f, det3_rn<4>(guess))) <= 0.001f)) st = ICP_NOT_RIGID;
       sh.s.status = st;
@@ -555,8 +549,8 @@ __device__ __forceinline__ void icp3_body(const Icp3Batch &b, const MapArgs &mp)
   }
 }
 
-__global__ void __launch_bounds__(ICP3_THREADS, 1) icp3_kernel(const Icp3Batch b) {
-  constexpr MapArgs mp{};
+// (mp is not read: the three kernels take the same parameters, as icp_kernel's classes do)
+__global__ void __launch_bounds__(ICP3_THREADS, 1) icp3_kernel(const Icp3Batch b, const MapArgs mp) {
   icp3_body<false>(b, mp);
 }
 
@@ -611,24 +605,5 @@ static size_t icp3_map_smem(int ns_max) {
 // per point, 256-byte aligned), and icp3_gsrc_kernel's shared memory
 static size_t icp3_src_slice(int ns_max) { return (20 * (size_t)ns_max + 255) & ~size_t(255); }
 static size_t icp3_gsrc_smem() { return ((sizeof(Icp3Shared) + 15) & ~size_t(15)) + ICP3_SCRATCH * sizeof(float); }
-
-// The largest source the shared-memory layouts hold next to targets of any size: icp3_map_kernel's (at most 65 535)
-static int icp3_src_limit(const sfe_ctx *ctx, int *limit) {
-  size_t budget;
-  int rc = cta_smem_budget(ctx, (const void *)icp3_map_kernel, &budget);
-  if (rc != SFE_OK) return rc;
-  *limit = largest_layout(65535, budget, icp3_map_smem);
-  return SFE_OK;
-}
-
-// The largest target icp3_kernel's layout holds next to sources of ns points (0: none; MAP_CLASS_ALL: 0)
-static int icp3_limit(const sfe_ctx *ctx, int ns, int *limit) {
-  size_t budget;
-  int rc = cta_smem_budget(ctx, (const void *)icp3_kernel, &budget);
-  if (rc != SFE_OK) return rc;
-  int mc;
-  *limit = MAP_CLASS_ALL ? 0 : largest_layout(65535, budget, [&](int nt) { return icp3_cta_smem(ns, nt, budget, &mc); });
-  return SFE_OK;
-}
 
 }  // namespace sfe

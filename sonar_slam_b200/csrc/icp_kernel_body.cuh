@@ -99,8 +99,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
     const float *tgt = b.tgt_pts + 2 * (size_t)b.tgt_off[ti];
     const int nt = b.tgt_cnt ? b.tgt_cnt[ti] : b.tgt_off[ti + 1] - b.tgt_off[ti];
     const float *guess = b.guess + 9 * (size_t)p;
-    if (b.class_mode == 1 && (ns > b.ns_max || nt > b.nt_max)) continue;
-    if (b.class_mode == 2 && ns <= b.class_ns && nt <= b.class_nt) continue;
+    if (!icp_takes(b.box, ns, nt)) continue;  // another launch's
     __syncthreads();  // previous problem fully retired before shared state is reused
 
     // ---- admission checks (thread 0), failure leaves T = guess

@@ -60,8 +60,9 @@ struct IcpClass {
 constexpr int ICP_MAX_CLASSES = 3;  // classes an icp_run call may list (the capacity class comes on top)
 // n_classes > 0: every problem goes to the first listed class it fits, the others to a capacity class laid out for
 // src.n_max x tgt.n_max; one launch per class, the widest first, each taking its problems largest first from a list
-// built on the device (icp.cu).  n_classes 0: one launch, or, when the largest target does not fit one CTA, one for
-// the targets that do and the map class for the rest.  class_of (device [P], may be null; classes only): receives
+// built on the device (icp.cu).  n_classes 0: launches that partition the problems -- in-CTA, the map class for the
+// targets one CTA does not hold, the global-source class for the sources no shared-memory layout holds -- each problem
+// solved and written by exactly one of them (icp.cu's icp_split_run).  class_of (device [P], may be null; classes only): receives
 // every problem's class (0 .. n_classes, the capacity class last) and, in class_of[P + p], its place in that class's
 // list.
 // filt (may be null): sfe_icp_filters -- data filters compacted into scratch once per cloud before the launches, and
@@ -75,8 +76,9 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what);
 // (SFE_ERR_UNSUPPORTED).
 int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what);
 // icp_run on [x, y, z] clouds (icp3.cuh; statement oracle/icp3_ref.c): guess and T_out are [P][16] row-major 4x4,
-// point-to-point with float32 sums only; no counts, classes or filters (icp_params_check).  Targets above
-// icp_cta_limit(ctx, 3, ns) read map grids, with the same results.
+// point-to-point with float32 sums only; no counts, classes or filters (icp_params_check).  The same launch split as
+// icp_run without classes: targets above icp_cta_limit(ctx, 3, ns) read map grids, sources above icp_source_limit take
+// the global-source class, with the same results.
 int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
              const sfe_icp_filters *filt = nullptr);
 // *limit = the largest target of `dim` columns that icp_run (dim 2: shipped point-to-point chain, no filters) or
