@@ -31,7 +31,8 @@ extern "C" {
                             202: - sfe_frontend_set_overlap (run_dev runs every stage over the whole batch); later
                                  additions that change no existing entry point: sfe_match_dim_*, sfe_match_knn_dim_*,
                                  sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
-                                 sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit */
+                                 sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit,
+                                 SFE_ICP_DATA_OCTREE (a new sfe_icp_data_filter kind; both structs keep their sizes) */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -341,7 +342,13 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  input order.  Reading filters see the source in its input frame (before the guess), reference
  *                  filters the target in its input frame (before centring: mean, grid and normals come from the
  *                  survivors).  SFE_ICP_DATA_MAX_DIST {dim, dist}: dim -1 keeps sqrtf(x*x + y*y) < |dist|, dim 0 / 1
- *                  keeps coordinate < dist; SFE_ICP_DATA_MIN_DIST the mirror (> |dist|, coordinate > dist).  A target
+ *                  keeps coordinate < dist; SFE_ICP_DATA_MIN_DIST the mirror (> |dist|, coordinate > dist).
+ *                  SFE_ICP_DATA_OCTREE {dim, dist}: OctreeGridDataPointsFilter with maxSizeByNode = dist (finite, > 0)
+ *                  and samplingMethod = dim -- the quadtree of sfe_downsample_dev (bounding square, stable 4-way
+ *                  partition, split while 2 * radius > dist and more than one point, at most 15 levels), one point
+ *                  per leaf in depth-first leaf order: 0 the leaf's first (lowest-index) member, 2 its centroid
+ *                  (float32 sequential sums of x and y in member order, each divided by the member count), 3 its
+ *                  medoid (as sfe_downsample_dev).  Later filters and the iterations see the leaf order.  A target
  *                  the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
  *                  SFE_ICP_NO_OUTLIER with a quantile filter (trim_ratio or median_factor) on, else SFE_ICP_NO_POINT.
  *   min_dist       MinDistOutlierFilter minDist (< 0: off): keep pairs with d^2 > minDist^2 (sfe_icp_params.flags
@@ -349,11 +356,11 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *   median_factor  MedianDistOutlierFilter factor (< 0: off): keep d^2 <= factor * median, median = element
  *                  floor(n_finite * 0.5) of the ascending finite squared distances (no finite one: SFE_ICP_NO_OUTLIER)
  * Outlier weights are the product over the chain (with sfe_icp_params' MaxDist and TrimmedDist). */
-enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_MAX_DATA_FILTERS = 4 };
+enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_DATA_OCTREE = 3, SFE_ICP_MAX_DATA_FILTERS = 4 };
 typedef struct {
-  int kind; /* SFE_ICP_DATA_MAX_DIST or SFE_ICP_DATA_MIN_DIST */
-  int dim;  /* -1 radial, 0 x, 1 y */
-  float dist;
+  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST or SFE_ICP_DATA_OCTREE */
+  int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3 */
+  float dist; /* distance filters: the distance; octree: maxSizeByNode */
 } sfe_icp_data_filter;
 typedef struct {
   float min_dist;
@@ -397,7 +404,8 @@ SFE_API int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit);
 SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit);
 
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
- * the default).  Checked here: no NaN, kind and dim known, counts in range; SFE_ERR_ARG leaves the setting as it was. */
+ * the default).  Checked here: no NaN, kind and dim known, an octree's maxSizeByNode finite and positive, counts in
+ * range; SFE_ERR_ARG leaves the setting as it was. */
 SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);
 
 /* ------------------------------------------------------------------ robust covariance of ICP samples (row N1)

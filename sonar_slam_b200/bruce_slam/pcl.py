@@ -7,7 +7,7 @@ bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libson
     match(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)             -> (int32[knn,N_s], float32[knn,N_s])  (:161)
     match_knn(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)         -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
-        (the YAML's distance data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
+        (the YAML's distance and octree data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
     ICP().compute(source[N,3], target[M,3], guess 4x4)          -> (message, float32[4,4])   (3-D, point-to-point)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
@@ -146,7 +146,8 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
 # ------------------------------------------------------------------------------------------ ICP
 _SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are implemented, plus its commented-out "
               "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference, the Max/MinDist data "
-              "filters and the MinDist / MedianDist outlier filters")
+              "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, and the "
+              "MinDist / MedianDist outlier filters")
 _DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
 
 
@@ -161,10 +162,36 @@ def _data_filter(name, p):
     return kind, dim, dist
 
 
+_OCTREE = "OctreeGridDataPointsFilter"
+
+
+def _octree_filter(p):
+    """OctreeGridDataPointsFilter {maxSizeByNode, samplingMethod, maxPointByNode, buildParallel} -> (OCTREE, sampling
+    method, maxSizeByNode): the quadtree of pcl.downsample with one point per leaf -- 0 the first (lowest-index) member,
+    upstream's default; 2 the float32 centroid; 3 the medoid.  maxPointByNode (moot once a size is given) and
+    buildParallel (results do not depend on it) are ignored."""
+    size = float(p.get("maxSizeByNode", 0.0))
+    if not math.isfinite(size) or size < 0:
+        raise ValueError(f"ICP yaml: {_OCTREE} maxSizeByNode {size} must be finite and non-negative")
+    if size == 0:
+        # coincident points make libpointmatcher's point-count recursion depend on float underflow, which the
+        # device's 15-level tree cannot follow
+        raise NotImplementedError(f"ICP yaml: {_OCTREE} without maxSizeByNode (the maxPointByNode criterion) is not "
+                                  "implemented: give maxSizeByNode > 0")
+    method = p.get("samplingMethod", 0)
+    if method not in (0, 1, 2, 3) or isinstance(method, bool):
+        raise ValueError(f"ICP yaml: {_OCTREE} samplingMethod {method!r} (0 first point, 1 random, 2 centroid, "
+                         "3 medoid)")
+    if method == 1:
+        raise NotImplementedError(f"ICP yaml: {_OCTREE} samplingMethod 1 (random sampling) is not implemented: its "
+                                  "result depends on a random generator (0, 2 and 3 are)")
+    return _lib.OCTREE, int(method), size
+
+
 def parse_icp_yaml(text):
     """libpointmatcher ICP YAML (the subset described by _SUPPORTED) -> _lib.IcpConfig: the IcpParams the shipped modules
-    set, with `.filters` = the _lib.IcpFilters of the distance data filters and the MinDist / MedianDist outlier
-    filters (None when the YAML has none of them)."""
+    set, with `.filters` = the _lib.IcpFilters of the distance and octree data filters, in their listed order, and the
+    MinDist / MedianDist outlier filters (None when the YAML has none of them)."""
     import yaml
     cfg = yaml.safe_load(text) or {}
 
@@ -177,8 +204,8 @@ def parse_icp_yaml(text):
         raise ValueError(f"ICP yaml: cannot parse module {node!r}")
 
     def add_data_filter(chain, name, p, which):
-        f = _data_filter(name, p)
-        if (name,) + f in chain:
+        f = _octree_filter(p) if name == _OCTREE else _data_filter(name, p)
+        if name != _OCTREE and (name,) + f in chain:
             raise ValueError(f"ICP yaml: {name} {p} appears twice in {which}DataPointsFilters")
         if len(chain) == _lib.MAX_DATA_FILTERS:
             raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} {which}DataPointsFilters")
@@ -188,16 +215,16 @@ def parse_icp_yaml(text):
     reading, reference, outlier = [], [], {}
     for node in cfg.get("readingDataPointsFilters") or []:
         name, p = one(node)
-        if name not in _DATA_FILTERS:
+        if name not in _DATA_FILTERS and name != _OCTREE:
             raise NotImplementedError(f"ICP yaml: reading filter {name} ({_SUPPORTED})")
         add_data_filter(reading, name, p, "reading")
     have_normals = False
     for node in cfg.get("referenceDataPointsFilters") or []:
         name, p = one(node)
-        if name in _DATA_FILTERS:
+        if name in _DATA_FILTERS or name == _OCTREE:
             if have_normals:  # the normals would describe points the filter then removes
                 raise NotImplementedError(f"ICP yaml: {name} after SurfaceNormalDataPointsFilter ({_SUPPORTED}: the "
-                                          "distance filters go before it)")
+                                          "data filters go before it)")
             add_data_filter(reference, name, p, "reference")
             continue
         # the one other reference filter: point-to-plane needs it, it attaches the "normals" descriptor

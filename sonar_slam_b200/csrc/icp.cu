@@ -411,6 +411,13 @@ __device__ __forceinline__ bool icp_data_keep(const IcpDataFilters &df, float x,
   return keep;
 }
 
+// After an octree stage (downsample_run, which reads at most n_max points of a cloud): the clouds passed on
+// uncompacted keep their size, so that the ICP launch still reports them SFE_ICP_TOO_LARGE
+__global__ void icp_keep_too_large_kernel(const int *in_cnt, int n_clouds, int n_max, int *out_cnt) {
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n_clouds; c += gridDim.x * blockDim.x)
+    if (in_cnt[c] > n_max) out_cnt[c] = in_cnt[c];
+}
+
 __global__ void __launch_bounds__(ICP_DF_THREADS) icp_data_filter_kernel(const PackedClouds in, const int *id,
                                                                          int n_clouds, const IcpDataFilters df,
                                                                          float *out_pts, int *out_off, int *out_cnt,
@@ -677,8 +684,16 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what) {
   for (int side = 0; side < 2; ++side)
     for (int k = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
       const sfe_icp_data_filter &d = side ? f->reference[k] : f->reading[k];
-      SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST,
+      SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST || d.kind == SFE_ICP_DATA_OCTREE,
                   "%s: unknown data filter kind %d", what, d.kind);
+      if (d.kind == SFE_ICP_DATA_OCTREE) {
+        SFE_REQUIRE(d.dim == DS_FIRST || d.dim == DS_CENTROID || d.dim == DS_MEDOID,
+                    "%s: OctreeGridDataPointsFilter samplingMethod %d (0 first point, 2 centroid or 3 medoid)", what,
+                    d.dim);
+        SFE_REQUIRE(std::isfinite(d.dist) && d.dist > 0.f,
+                    "%s: OctreeGridDataPointsFilter maxSizeByNode %g (finite and positive)", what, (double)d.dist);
+        continue;
+      }
       SFE_REQUIRE(d.dim >= -1 && d.dim <= 1, "%s: data filter dim %d (2-D clouds: -1, 0 or 1)", what, d.dim);
       SFE_REQUIRE(!std::isnan(d.dist), "%s: a NaN data filter distance is not supported", what);
     }
@@ -1142,24 +1157,64 @@ static bool icp_filters_on(const sfe_icp_filters *f) {
   return f && (f->n_reading > 0 || f->n_reference > 0 || f->min_dist >= 0.f || f->median_factor >= 0.f);
 }
 
-// Data filters: the clouds of one side of the batch, compacted into scratch[SCR_ICP_FILTER] (icp_data_filter_kernel),
-// once per cloud when the cloud count is known (no ids: one per problem), else once per problem (the ids then name the
-// compacted clouds no more).  Two passes over the Carver: the first sizes the block, the second launches.
-static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const IcpDataFilters &df, PackedClouds &c, const int *&id,
-                           int n_clouds, int P, Carver &cv, const int *&gate) {
+// Data filters: the clouds of one side of the batch, filtered into scratch[SCR_ICP_FILTER] once per cloud when the
+// cloud count is known (no ids: one per problem), else once per problem (the ids then name the filtered clouds no
+// more).  The chain f[0 .. n) runs as stages in its order: every maximal run of distance filters is one
+// icp_data_filter_kernel pass, every octree filter one downsample_run call on the clouds the stage before left.  The
+// first stage is always a compaction pass (with no filter when the chain starts with an octree filter): it lays the
+// clouds out n_max points apart and records their sizes before any filter, the `gate` counts.  Two passes over the
+// Carver: the first sizes the block, the second launches.
+static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_filter *f, int n, PackedClouds &c,
+                           const int *&id, int n_clouds, int P, Carver &cv, const int *&gate) {
   const int jobs = id && n_clouds > 0 ? n_clouds : P;
   const int n_max = c.n_max > 0 ? c.n_max : 1;
-  float *pts = (float *)cv.take(sizeof(float) * 2 * (size_t)jobs * n_max);
+  const size_t pts_bytes = sizeof(float) * 2 * (size_t)jobs * n_max;
+  float *pts = (float *)cv.take(pts_bytes);
   int *off = (int *)cv.take(sizeof(int) * (size_t)(jobs + 1));
   int *cnt = (int *)cv.take(sizeof(int) * (size_t)jobs);
   int *raw = (int *)cv.take(sizeof(int) * (size_t)jobs);
+  bool octree = false;
+  for (int k = 0; k < n; ++k) octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE;
+  // octree chains: a second set of points and counts the stages alternate with, the down-sample's indices, and the
+  // offsets and sizes later compaction passes write (the same offsets; the sizes are not the gate's)
+  float *pts2 = nullptr;
+  int *cnt2 = nullptr, *idx = nullptr, *off2 = nullptr, *raw2 = nullptr;
+  if (octree) {
+    pts2 = (float *)cv.take(pts_bytes);
+    cnt2 = (int *)cv.take(sizeof(int) * (size_t)jobs);
+    idx = (int *)cv.take(sizeof(int) * (size_t)jobs * n_max);
+    off2 = (int *)cv.take(sizeof(int) * (size_t)(jobs + 1));
+    raw2 = (int *)cv.take(sizeof(int) * (size_t)jobs);
+  }
   if (!cv.base) return SFE_OK;
   const bool per_problem = id && n_clouds <= 0;
-  icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
-      {c.pts, c.off, c.cnt, n_max}, per_problem ? id : nullptr, jobs, df, pts, off, cnt, raw);
-  SFE_CUDA(cudaGetLastError());
-  ctx->launches++;
-  c = {pts, off, cnt, c.n_max};
+  PackedClouds cur = c;
+  const int *cur_id = per_problem ? id : nullptr;
+  float *next_pts = pts;
+  int *next_cnt = cnt;
+  for (int k = 0, first = 1; k < n || first; first = 0) {
+    if (!first && f[k].kind == SFE_ICP_DATA_OCTREE) {
+      const int rc = downsample_run(ctx, st, cur, jobs, 2, f[k].dist, next_pts, idx, next_cnt, DS_ANY_SIZE, SCR_CLOUD,
+                                    WORK_DS, f[k].dim);
+      if (rc != SFE_OK) return rc;
+      icp_keep_too_large_kernel<<<std::min((jobs + 255) / 256, ctx->sm_count), 256, 0, st>>>(cur.cnt, jobs, n_max,
+                                                                                             next_cnt);
+      ++k;
+    } else {
+      IcpDataFilters df{0, {}};
+      for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE; ++k) df.f[df.n++] = f[k];
+      icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
+          {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
+          first ? raw : raw2);
+    }
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+    float *prev_pts = (float *)cur.pts;
+    int *prev_cnt = (int *)cur.cnt;
+    cur = {next_pts, off, next_cnt, c.n_max}, cur_id = nullptr;
+    next_pts = first ? pts2 : prev_pts, next_cnt = first ? cnt2 : prev_cnt;
+  }
+  c = cur;
   if (per_problem) id = nullptr;
   gate = raw;
   return SFE_OK;
@@ -1193,17 +1248,17 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   if (rc != SFE_OK) return rc;
   const int *gate_src = nullptr, *gate_tgt = nullptr;
   if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
-    IcpDataFilters rd{filt->n_reading, {}}, rf{filt->n_reference, {}};
-    for (int k = 0; k < SFE_ICP_MAX_DATA_FILTERS; ++k) rd.f[k] = filt->reading[k], rf.f[k] = filt->reference[k];
     Carver cv;
     for (int pass = 0; pass < 2; ++pass) {
       IcpProblems q = pb;
-      if (rd.n > 0) {
-        rc = icp_filter_side(ctx, st, rd, q.src, q.src_id, q.n_src_clouds, q.P, cv, gate_src);
+      if (filt->n_reading > 0) {
+        rc = icp_filter_side(ctx, st, filt->reading, filt->n_reading, q.src, q.src_id, q.n_src_clouds, q.P, cv,
+                             gate_src);
         if (rc != SFE_OK) return rc;
       }
-      if (rf.n > 0) {
-        rc = icp_filter_side(ctx, st, rf, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv, gate_tgt);
+      if (filt->n_reference > 0) {
+        rc = icp_filter_side(ctx, st, filt->reference, filt->n_reference, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv,
+                             gate_tgt);
         if (rc != SFE_OK) return rc;
         if (q.tgt_id != pb.tgt_id) q.n_tgt_clouds = q.P;  // one compacted target per problem
       }

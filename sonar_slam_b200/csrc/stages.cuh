@@ -40,10 +40,14 @@ int feature_image_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const ui
                       const uint8_t *lut_bgr, uint8_t *out, const char *what);  // what: the caller, for errors
 // n_split > 0: two launches of the one-CTA kernel by cloud size (cloud.cu; n_max at most 65 535 points),
 // DS_ANY_SIZE: clouds of any size (one-CTA kernel up to the device's limit, grid-wide path above it).  slot: scratch
-// buffer, counter: work counter (WORK_*) of the one-CTA launches.
+// buffer, counter: work counter (WORK_*) of the one-CTA launches.  sampler: the point every leaf keeps, numbered as
+// libpointmatcher's samplingMethod -- DS_MEDOID (pcl.downsample), or, for 2-D clouds with DS_ANY_SIZE, DS_FIRST (the
+// leaf's lowest-index member) and DS_CENTROID (float32 sequential means); out_idx then names the leaf's first member.
 constexpr int DS_ANY_SIZE = -1;
+enum { DS_FIRST = 0, DS_CENTROID = 2, DS_MEDOID = 3 };
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
-                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot, int counter);
+                   float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot, int counter,
+                   int sampler = DS_MEDOID);
 // the largest cloud of `dim` columns (2 or 3) downsample_run's one-CTA kernel lays out in shared memory on this device
 int downsample_cta_limit(const sfe_ctx *ctx, int *limit, int dim);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
@@ -65,8 +69,9 @@ constexpr int ICP_MAX_CLASSES = 3;  // classes an icp_run call may list (the cap
 // solved and written by exactly one of them (icp.cu's icp_split_run).  class_of (device [P], may be null; classes only): receives
 // every problem's class (0 .. n_classes, the capacity class last) and, in class_of[P + p], its place in that class's
 // list.
-// filt (may be null): sfe_icp_filters -- data filters compacted into scratch once per cloud before the launches, and
-// the outlier filters in icp_kernel's FILT instantiations; min_points then counts the clouds before the data filters.
+// filt (may be null): sfe_icp_filters -- data filters run into scratch once per cloud before the launches (distance
+// filters compacted, octree filters through downsample_run), and the outlier filters in icp_kernel's FILT
+// instantiations; min_points then counts the clouds before the data filters.
 int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, const IcpClass *classes,
             int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr);
 // SFE_OK, or SFE_ERR_ARG with a message naming `what`: NaN, unknown kind, dim outside -1 .. 1, counts out of range

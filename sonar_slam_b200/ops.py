@@ -173,7 +173,8 @@ def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, knn=None, ctx=N
 def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, src_id=None, tgt_id=None, ctx=None,
         filters=None):
     """Batched ICP (include/sonarfe.h: sfe_icp_dev).  guess: [P,3,3] f32 cuda.  Returns dict of cuda tensors.
-    filters: _lib.IcpFilters (sfe_icp_set_filters), default params.filters when params is a parsed _lib.IcpConfig.
+    filters: _lib.IcpFilters (sfe_icp_set_filters), default params.filters when params is a parsed _lib.IcpConfig;
+    its data filters (distance and octree) run on the device before the iterations.
 
     Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
     map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources of any size:
