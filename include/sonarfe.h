@@ -32,7 +32,8 @@ extern "C" {
                                  additions that change no existing entry point: sfe_match_dim_*, sfe_match_knn_dim_*,
                                  sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
                                  sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit,
-                                 SFE_ICP_DATA_OCTREE (a new sfe_icp_data_filter kind; both structs keep their sizes) */
+                                 SFE_ICP_DATA_OCTREE and SFE_ICP_DATA_VOXEL (new sfe_icp_data_filter kinds; both structs
+                                 keep their sizes) */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -348,19 +349,28 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  partition, split while 2 * radius > dist and more than one point, at most 15 levels), one point
  *                  per leaf in depth-first leaf order: 0 the leaf's first (lowest-index) member, 2 its centroid
  *                  (float32 sequential sums of x and y in member order, each divided by the member count), 3 its
- *                  medoid (as sfe_downsample_dev).  Later filters and the iterations see the leaf order.  A target
- *                  the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
+ *                  medoid (as sfe_downsample_dev).  Later filters and the iterations see the leaf order.
+ *                  SFE_ICP_DATA_VOXEL {dim, dist}: VoxelGridDataPointsFilter with vSizeX = vSizeY = dist (finite, > 0)
+ *                  and useCentroid = dim (1; 0 is not supported) -- per axis minB = min / dist, maxB = max / dist,
+ *                  numDiv = 1 + (unsigned)(maxB - minB); point p lies in voxel (unsigned)floorf(x / dist - minBX) +
+ *                  (unsigned)floorf(y / dist - minBY) * numDivX; the first point of every voxel is kept, in point
+ *                  order, holding the voxel's centroid (float32 sequential sums from the first point's coordinates in
+ *                  point order, each divided by (float)count).  A cloud whose numDivX * numDivY does not fit 32 bits
+ *                  (or whose bounds are not finite) makes the call SFE_ERR_UNSUPPORTED after the filter stages and
+ *                  before any ICP launch (the grid spans the cloud the filter receives, known on the device only;
+ *                  the call waits for the stages to check).  A target the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
  *                  SFE_ICP_NO_OUTLIER with a quantile filter (trim_ratio or median_factor) on, else SFE_ICP_NO_POINT.
  *   min_dist       MinDistOutlierFilter minDist (< 0: off): keep pairs with d^2 > minDist^2 (sfe_icp_params.flags
  *                  bit 0: d^2 > minDist, as for MaxDist)
  *   median_factor  MedianDistOutlierFilter factor (< 0: off): keep d^2 <= factor * median, median = element
  *                  floor(n_finite * 0.5) of the ascending finite squared distances (no finite one: SFE_ICP_NO_OUTLIER)
  * Outlier weights are the product over the chain (with sfe_icp_params' MaxDist and TrimmedDist). */
-enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_DATA_OCTREE = 3, SFE_ICP_MAX_DATA_FILTERS = 4 };
+enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_DATA_OCTREE = 3, SFE_ICP_DATA_VOXEL = 4,
+       SFE_ICP_MAX_DATA_FILTERS = 4 };
 typedef struct {
-  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST or SFE_ICP_DATA_OCTREE */
-  int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3 */
-  float dist; /* distance filters: the distance; octree: maxSizeByNode */
+  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST, SFE_ICP_DATA_OCTREE or SFE_ICP_DATA_VOXEL */
+  int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3; voxel: useCentroid, 1 */
+  float dist; /* distance filters: the distance; octree: maxSizeByNode; voxel: vSize */
 } sfe_icp_data_filter;
 typedef struct {
   float min_dist;
@@ -404,8 +414,8 @@ SFE_API int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit);
 SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit);
 
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
- * the default).  Checked here: no NaN, kind and dim known, an octree's maxSizeByNode finite and positive, counts in
- * range; SFE_ERR_ARG leaves the setting as it was. */
+ * the default).  Checked here: no NaN, kind and dim known, an octree's maxSizeByNode and a voxel filter's vSize finite and
+ * positive, counts in range; SFE_ERR_ARG leaves the setting as it was. */
 SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);
 
 /* ------------------------------------------------------------------ robust covariance of ICP samples (row N1)

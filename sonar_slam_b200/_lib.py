@@ -205,12 +205,14 @@ class IcpParams(ctypes.Structure):
 
 MAX_DIST, MIN_DIST = 1, 2  # SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST: the kinds of an IcpDataFilter
 OCTREE = 3                 # SFE_ICP_DATA_OCTREE: OctreeGridDataPointsFilter {dim samplingMethod, dist maxSizeByNode}
+VOXEL = 4                  # SFE_ICP_DATA_VOXEL: VoxelGridDataPointsFilter {dim useCentroid (1), dist vSize}
 MAX_DATA_FILTERS = 4       # SFE_ICP_MAX_DATA_FILTERS per cloud
 
 
 class IcpDataFilter(ctypes.Structure):
-    """sfe_icp_data_filter: MaxDist / MinDistDataPointsFilter {dim, dist}, or OctreeGridDataPointsFilter {dim =
-    samplingMethod (0 first point, 2 centroid, 3 medoid), dist = maxSizeByNode}."""
+    """sfe_icp_data_filter: MaxDist / MinDistDataPointsFilter {dim, dist}, OctreeGridDataPointsFilter {dim =
+    samplingMethod (0 first point, 2 centroid, 3 medoid), dist = maxSizeByNode}, or VoxelGridDataPointsFilter {dim =
+    useCentroid (1), dist = vSize}."""
     _fields_ = [("kind", c_int), ("dim", c_int), ("dist", c_float)]
 
 
@@ -218,7 +220,8 @@ class IcpFilters(ctypes.Structure):
     """sfe_icp_filters (include/sonarfe.h): the MinDist / MedianDist outlier filters (< 0: off) and up to four data
     filters per cloud, run in their order.  reading / reference: sequences of (kind, dim, dist): kind MAX_DIST or
     MIN_DIST with dim -1 (radial), 0 (x) or 1 (y) and the distance; kind OCTREE with dim the samplingMethod (0 first
-    point, 2 centroid, 3 medoid) and dist maxSizeByNode (finite, > 0)."""
+    point, 2 centroid, 3 medoid) and dist maxSizeByNode (finite, > 0); kind VOXEL with dim 1 (useCentroid) and dist
+    vSize (finite, > 0)."""
     _fields_ = [("min_dist", c_float), ("median_factor", c_float), ("n_reading", c_int), ("n_reference", c_int),
                 ("reading", IcpDataFilter * MAX_DATA_FILTERS), ("reference", IcpDataFilter * MAX_DATA_FILTERS)]
 

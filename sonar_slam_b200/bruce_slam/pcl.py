@@ -7,7 +7,8 @@ bruce_slam/src/bruce_slam/cpp/pcl.cpp:176-214, running on the GPU through libson
     match(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)             -> (int32[knn,N_s], float32[knn,N_s])  (:161)
     match_knn(ref[N_t,2|3], in[N_s,2|3], knn, max_dist)         -> the same for knn 1 .. 16 (match serves knn = 1)
     ICP().loadFromYaml(path) / .compute(source, target, guess)  -> (message, float32[3,3])   (:185-212)
-        (the YAML's distance and octree data filters and MinDist / MedianDist outlier filters included: parse_icp_yaml)
+        (the YAML's distance, octree and voxel-grid data filters and MinDist / MedianDist outlier filters included:
+        parse_icp_yaml)
     ICP().compute(source[N,3], target[M,3], guess 4x4)          -> (message, float32[4,4])   (3-D, point-to-point)
 
 Like pybind11 (`const PM::Matrix &` = Eigen float matrix) every array argument is converted to
@@ -146,8 +147,9 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
 # ------------------------------------------------------------------------------------------ ICP
 _SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are implemented, plus its commented-out "
               "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference, the Max/MinDist data "
-              "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, and the "
-              "MinDist / MedianDist outlier filters")
+              "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, the "
+              "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, and the MinDist / MedianDist "
+              "outlier filters")
 _DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
 
 
@@ -188,10 +190,36 @@ def _octree_filter(p):
     return _lib.OCTREE, int(method), size
 
 
+_VOXEL = "VoxelGridDataPointsFilter"
+
+
+def _voxel_filter(p):
+    """VoxelGridDataPointsFilter {vSizeX, vSizeY, vSizeZ, useCentroid, averageExistingDescriptors} -> (VOXEL, 1, vSize):
+    the first point of every voxel, in point order, holding its voxel's float32 centroid.  vSizeZ is moot on 2-D clouds
+    and averageExistingDescriptors on clouds without descriptors; both are ignored."""
+    sx, sy = float(p.get("vSizeX", 1.0)), float(p.get("vSizeY", 1.0))
+    for axis, v in (("vSizeX", sx), ("vSizeY", sy)):
+        if not math.isfinite(v) or v <= 0:
+            raise ValueError(f"ICP yaml: {_VOXEL} {axis} {v} must be finite and positive")
+    if sx != sy:
+        raise NotImplementedError(f"ICP yaml: {_VOXEL} with vSizeX {sx} != vSizeY {sy} is not implemented: give one "
+                                  "size for both axes")
+    centroid = p.get("useCentroid", 1)
+    if centroid not in (0, 1):
+        raise ValueError(f"ICP yaml: {_VOXEL} useCentroid {centroid!r} (0 or 1)")
+    if not centroid:
+        raise NotImplementedError(f"ICP yaml: {_VOXEL} useCentroid 0 (the voxel centre) is not implemented: its "
+                                  "formula cannot be checked against upstream (1, the centroid, is)")
+    return _lib.VOXEL, 1, sx
+
+
+_RESAMPLERS = {_OCTREE: _octree_filter, _VOXEL: _voxel_filter}
+
+
 def parse_icp_yaml(text):
     """libpointmatcher ICP YAML (the subset described by _SUPPORTED) -> _lib.IcpConfig: the IcpParams the shipped modules
-    set, with `.filters` = the _lib.IcpFilters of the distance and octree data filters, in their listed order, and the
-    MinDist / MedianDist outlier filters (None when the YAML has none of them)."""
+    set, with `.filters` = the _lib.IcpFilters of the distance, octree and voxel-grid data filters, in their listed
+    order, and the MinDist / MedianDist outlier filters (None when the YAML has none of them)."""
     import yaml
     cfg = yaml.safe_load(text) or {}
 
@@ -204,8 +232,8 @@ def parse_icp_yaml(text):
         raise ValueError(f"ICP yaml: cannot parse module {node!r}")
 
     def add_data_filter(chain, name, p, which):
-        f = _octree_filter(p) if name == _OCTREE else _data_filter(name, p)
-        if name != _OCTREE and (name,) + f in chain:
+        f = _RESAMPLERS[name](p) if name in _RESAMPLERS else _data_filter(name, p)
+        if name not in _RESAMPLERS and (name,) + f in chain:
             raise ValueError(f"ICP yaml: {name} {p} appears twice in {which}DataPointsFilters")
         if len(chain) == _lib.MAX_DATA_FILTERS:
             raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} {which}DataPointsFilters")
@@ -215,13 +243,13 @@ def parse_icp_yaml(text):
     reading, reference, outlier = [], [], {}
     for node in cfg.get("readingDataPointsFilters") or []:
         name, p = one(node)
-        if name not in _DATA_FILTERS and name != _OCTREE:
+        if name not in _DATA_FILTERS and name not in _RESAMPLERS:
             raise NotImplementedError(f"ICP yaml: reading filter {name} ({_SUPPORTED})")
         add_data_filter(reading, name, p, "reading")
     have_normals = False
     for node in cfg.get("referenceDataPointsFilters") or []:
         name, p = one(node)
-        if name in _DATA_FILTERS or name == _OCTREE:
+        if name in _DATA_FILTERS or name in _RESAMPLERS:
             if have_normals:  # the normals would describe points the filter then removes
                 raise NotImplementedError(f"ICP yaml: {name} after SurfaceNormalDataPointsFilter ({_SUPPORTED}: the "
                                           "data filters go before it)")

@@ -129,20 +129,21 @@ __device__ __forceinline__ float4 block_bounds(float4 m, float4 *red) {
 // One sequential sum over values in global memory, p[0], p[stride], ... (the reference cloud's mean, once per
 // problem): lane j holds term base + j and a shuffle hands term j to every lane, so all lanes carry the same
 // running sum; eight batches (256 terms) are requested at once and the next eight are in flight while these are
-// added, so the L2 latency hides behind the ~1000-cycle add chain
-__device__ __forceinline__ float seq_sum_warp_global(const float *p, int n, int stride) {
+// added, so the L2 latency hides behind the ~1000-cycle add chain.  s0: the value the chain starts from.  Lanes past n
+// hold -0.f, the identity of IEEE addition, so that a chain from -0.f over -0.f terms stays -0.f.
+__device__ __forceinline__ float seq_sum_warp_global(const float *p, int n, int stride, float s0 = 0.f) {
   const int lane = threadIdx.x & 31;
-  float s = 0.f, cur[8], nxt[8];
+  float s = s0, cur[8], nxt[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int i = k * 32 + lane;
-    cur[k] = i < n ? p[(size_t)i * stride] : 0.f;
+    cur[k] = i < n ? p[(size_t)i * stride] : -0.f;
   }
   for (int base = 0; base < n; base += 256) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const int i = base + 256 + k * 32 + lane;
-      nxt[k] = i < n ? p[(size_t)i * stride] : 0.f;
+      nxt[k] = i < n ? p[(size_t)i * stride] : -0.f;
     }
 #pragma unroll
     for (int k = 0; k < 8; ++k) {

@@ -684,8 +684,16 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what) {
   for (int side = 0; side < 2; ++side)
     for (int k = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
       const sfe_icp_data_filter &d = side ? f->reference[k] : f->reading[k];
-      SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST || d.kind == SFE_ICP_DATA_OCTREE,
+      SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST || d.kind == SFE_ICP_DATA_OCTREE ||
+                      d.kind == SFE_ICP_DATA_VOXEL,
                   "%s: unknown data filter kind %d", what, d.kind);
+      if (d.kind == SFE_ICP_DATA_VOXEL) {
+        SFE_REQUIRE(d.dim == 1, "%s: VoxelGridDataPointsFilter useCentroid %d (only 1, the centroid, is supported)",
+                    what, d.dim);
+        SFE_REQUIRE(std::isfinite(d.dist) && d.dist > 0.f,
+                    "%s: VoxelGridDataPointsFilter vSize %g (finite and positive)", what, (double)d.dist);
+        continue;
+      }
       if (d.kind == SFE_ICP_DATA_OCTREE) {
         SFE_REQUIRE(d.dim == DS_FIRST || d.dim == DS_CENTROID || d.dim == DS_MEDOID,
                     "%s: OctreeGridDataPointsFilter samplingMethod %d (0 first point, 2 centroid or 3 medoid)", what,
@@ -1162,10 +1170,11 @@ static bool icp_filters_on(const sfe_icp_filters *f) {
 // more).  The chain f[0 .. n) runs as stages in its order: every maximal run of distance filters is one
 // icp_data_filter_kernel pass, every octree filter one downsample_run call on the clouds the stage before left.  The
 // first stage is always a compaction pass (with no filter when the chain starts with an octree filter): it lays the
-// clouds out n_max points apart and records their sizes before any filter, the `gate` counts.  Two passes over the
-// Carver: the first sizes the block, the second launches.
+// clouds out n_max points apart and records their sizes before any filter, the `gate` counts.  Every voxel filter is
+// one voxel_filter_run call likewise; a cloud whose voxel index would overflow sets *vox_overflow.  Two passes over
+// the Carver: the first sizes the block, the second launches.
 static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_filter *f, int n, PackedClouds &c,
-                           const int *&id, int n_clouds, int P, Carver &cv, const int *&gate) {
+                           const int *&id, int n_clouds, int P, Carver &cv, const int *&gate, int *vox_overflow) {
   const int jobs = id && n_clouds > 0 ? n_clouds : P;
   const int n_max = c.n_max > 0 ? c.n_max : 1;
   const size_t pts_bytes = sizeof(float) * 2 * (size_t)jobs * n_max;
@@ -1174,9 +1183,9 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   int *cnt = (int *)cv.take(sizeof(int) * (size_t)jobs);
   int *raw = (int *)cv.take(sizeof(int) * (size_t)jobs);
   bool octree = false;
-  for (int k = 0; k < n; ++k) octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE;
-  // octree chains: a second set of points and counts the stages alternate with, the down-sample's indices, and the
-  // offsets and sizes later compaction passes write (the same offsets; the sizes are not the gate's)
+  for (int k = 0; k < n; ++k) octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE || f[k].kind == SFE_ICP_DATA_VOXEL;
+  // octree and voxel chains: a second set of points and counts the stages alternate with, the down-sample's indices,
+  // and the offsets and sizes later compaction passes write (the same offsets; the sizes are not the gate's)
   float *pts2 = nullptr;
   int *cnt2 = nullptr, *idx = nullptr, *off2 = nullptr, *raw2 = nullptr;
   if (octree) {
@@ -1193,7 +1202,13 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   float *next_pts = pts;
   int *next_cnt = cnt;
   for (int k = 0, first = 1; k < n || first; first = 0) {
-    if (!first && f[k].kind == SFE_ICP_DATA_OCTREE) {
+    if (!first && f[k].kind == SFE_ICP_DATA_VOXEL) {
+      const int rc = voxel_filter_run(ctx, st, cur, jobs, f[k].dist, next_pts, off, next_cnt, vox_overflow);
+      if (rc != SFE_OK) return rc;
+      icp_keep_too_large_kernel<<<std::min((jobs + 255) / 256, ctx->sm_count), 256, 0, st>>>(cur.cnt, jobs, n_max,
+                                                                                             next_cnt);
+      ++k;
+    } else if (!first && f[k].kind == SFE_ICP_DATA_OCTREE) {
       const int rc = downsample_run(ctx, st, cur, jobs, 2, f[k].dist, next_pts, idx, next_cnt, DS_ANY_SIZE, SCR_CLOUD,
                                     WORK_DS, f[k].dim);
       if (rc != SFE_OK) return rc;
@@ -1202,7 +1217,7 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
       ++k;
     } else {
       IcpDataFilters df{0, {}};
-      for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE; ++k) df.f[df.n++] = f[k];
+      for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE && f[k].kind != SFE_ICP_DATA_VOXEL; ++k) df.f[df.n++] = f[k];
       icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
           {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
           first ? raw : raw2);
@@ -1248,17 +1263,25 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   if (rc != SFE_OK) return rc;
   const int *gate_src = nullptr, *gate_tgt = nullptr;
   if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
+    bool voxel = false;
+    for (int k = 0; k < filt->n_reading; ++k) voxel = voxel || filt->reading[k].kind == SFE_ICP_DATA_VOXEL;
+    for (int k = 0; k < filt->n_reference; ++k) voxel = voxel || filt->reference[k].kind == SFE_ICP_DATA_VOXEL;
     Carver cv;
+    int *vox_overflow = nullptr;
     for (int pass = 0; pass < 2; ++pass) {
       IcpProblems q = pb;
+      if (voxel) {
+        vox_overflow = (int *)cv.take(sizeof(int));
+        if (pass == 1) SFE_CUDA(cudaMemsetAsync(vox_overflow, 0, sizeof(int), st));
+      }
       if (filt->n_reading > 0) {
         rc = icp_filter_side(ctx, st, filt->reading, filt->n_reading, q.src, q.src_id, q.n_src_clouds, q.P, cv,
-                             gate_src);
+                             gate_src, vox_overflow);
         if (rc != SFE_OK) return rc;
       }
       if (filt->n_reference > 0) {
         rc = icp_filter_side(ctx, st, filt->reference, filt->n_reference, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv,
-                             gate_tgt);
+                             gate_tgt, vox_overflow);
         if (rc != SFE_OK) return rc;
         if (q.tgt_id != pb.tgt_id) q.n_tgt_clouds = q.P;  // one compacted target per problem
       }
@@ -1268,6 +1291,18 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
         cv.base = (char *)ctx->scratch[SCR_ICP_FILTER].ptr, cv.off = 0;
       } else {
         pb = q;
+      }
+    }
+    // The voxel grid spans the cloud a voxel stage receives, known on the device only: wait for the stages, and refuse
+    // the call before its ICP launch when a grid would need upstream's 32-bit voxel index to wrap (undefined there)
+    if (voxel) {
+      int overflow = 0;
+      SFE_CUDA(cudaMemcpyAsync(&overflow, vox_overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
+      SFE_CUDA(cudaStreamSynchronize(st));
+      if (overflow) {
+        set_error("icp: VoxelGridDataPointsFilter: a cloud's voxel grid has more than 2^32 - 1 voxels (or its bounds "
+                  "are not finite): its 32-bit voxel index would wrap; use a larger vSize");
+        return SFE_ERR_UNSUPPORTED;
       }
     }
   }

@@ -48,6 +48,11 @@ enum { DS_FIRST = 0, DS_CENTROID = 2, DS_MEDOID = 3 };
 int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int dim, float resolution,
                    float *out_pts, int32_t *out_idx, int32_t *out_count, int n_split, int slot, int counter,
                    int sampler = DS_MEDOID);
+// VoxelGridDataPointsFilter (vSize, useCentroid) on every 2-D cloud of `in` (clouds above in.n_max points are not read):
+// the first point of every voxel, in point order, holding its voxel's centroid, at out_off[c]; out_count[c] its number.
+// A cloud whose voxel index would not fit 32 bits sets *overflow (device) to 1.  Workspace: scratch[SCR_DS_GRID].
+int voxel_filter_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, float vsize, float *out_pts,
+                     int *out_off, int *out_count, int *overflow);
 // the largest cloud of `dim` columns (2 or 3) downsample_run's one-CTA kernel lays out in shared memory on this device
 int downsample_cta_limit(const sfe_ctx *ctx, int *limit, int dim);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
