@@ -33,7 +33,7 @@ extern "C" {
                                  sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
                                  sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit,
                                  SFE_ICP_DATA_OCTREE and SFE_ICP_DATA_VOXEL (new sfe_icp_data_filter kinds; both structs
-                                 keep their sizes) */
+                                 keep their sizes), sfe_ctx_set_grid_sms, sfe_ctx_occupancy */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -70,6 +70,21 @@ SFE_API int sfe_sync(sfe_ctx *ctx);
 SFE_API int sfe_copy_to_host(sfe_ctx *ctx, void *dst_host, const void *src_dev, uint64_t bytes);
 /* number of kernels this context has launched so far (bench.py: gpu_launches) */
 SFE_API uint64_t sfe_launch_count(const sfe_ctx *ctx);
+/* For tests: the number of SMs this context sizes its persistent launches for.  sms >= 1 sets it to min(sms, the
+ * device's SM count), sms <= 0 restores the device's count; *effective (may be NULL) receives the value now in force.
+ * Every persistent or grid-stride launch (Cartesian points, down-sample, outlier removal, match, ICP and the front
+ * end's stages) then runs that many SMs' worth of CTAs, so each CTA takes more work items in a row.  Results must not
+ * change.  The other uses of the count move with it and are claimed not to change results either: the Cartesian
+ * points' dense variants (F >= 2 * and 4 * the count), the costmap's warps per candidate and the PNG front end's
+ * chunk_frames.  Size classes (the ICP class split, source and one-CTA limits, the front end's classes) do not read
+ * it.  Not for concurrent use with other calls on the context. */
+SFE_API int sfe_ctx_set_grid_sms(sfe_ctx *ctx, int sms, int32_t *effective);
+/* For tests: the CTAs per SM of the persistent one-CTA launch configurations (kernel, threads, dynamic shared memory)
+ * this context has sized so far, in the order it first sized them; the context keeps the last 16.  Entry k:
+ * threads[k], smem[k] (bytes) and per_sm[k]; *n receives the number of entries, at most `capacity` are written.  A
+ * capped launch (sfe_ctx_set_grid_sms) runs sms * per_sm CTAs. */
+SFE_API int sfe_ctx_occupancy(const sfe_ctx *ctx, int32_t *threads, int32_t *smem, int32_t *per_sm, int capacity,
+                              int32_t *n);
 
 /* ------------------------------------------------------------------ CFAR
  * Replaces cfar::{ca,soca,goca,os} (cfar.cpp:10,30,53,76) and, with a non-NULL

@@ -1,4 +1,5 @@
 """TEST INFRASTRUCTURE ONLY -- ctypes doorway onto oracle/cloud3_ref.c (down-sample and match on [N,3] clouds).
+octree_literal: a second, literal statement of the 3-D down-sample in Python float32 scalars, with an optional depth cut.
 
 The library is compiled on first use with the flags of oracle/Makefile's restatements (-O3, -ffp-contract=off: every
 float32 product and sum rounded separately) into oracle/_build/libcloud3_ref.so, or into a temporary directory when the
@@ -7,6 +8,7 @@ tree is read-only, and rebuilt whenever cloud3_ref.c is newer.
 import ctypes
 import os
 import subprocess
+import sys
 import tempfile
 
 import numpy as np
@@ -86,3 +88,53 @@ def match_knn3(ref, pts, knn, max_dist):
     lib.orc_match_knn3(ref.ctypes.data_as(_FP), len(ref), pts.ctypes.data_as(_FP), len(pts), knn,
                        ctypes.c_float(max_dist), ids.ctypes.data_as(_IP), d.ctypes.data_as(_FP))
     return ids, d
+
+
+_F = np.float32
+
+
+def octree_literal(pts, resolution, max_depth=None):
+    """A second statement of the 3-D down-sample: the recursive octree of libpointmatcher's Octree_<T,3>, built node by
+    node with float32 scalars (centre = min + extent * 0.5 per axis, half-size = the largest half-extent, split while
+    2 * radius > resolution and more than one point, children by x > cx | y > cy << 1 | z > cz << 2 in index order,
+    medoid = first minimum of the sequential float32 sum of sqrt((dx*dx + dy*dy) + dz*dz)).  max_depth: nodes at that
+    depth become leaves (the device's cut at 15 levels).  Returns the kept indices in output order."""
+    pts = np.asarray(pts, _F)
+    n = len(pts)
+    if n == 0:
+        return np.zeros(0, np.int64)
+    res = _F(resolution)
+    mn, mx = pts.min(0), pts.max(0)
+    ext = [_F(mx[d] - mn[d]) for d in range(3)]
+    ctr = [_F(mn[d] + _F(ext[d] * _F(0.5))) for d in range(3)]
+    radius = max(_F(e * _F(0.5)) for e in ext)
+    out = []
+
+    def leaf(idx):
+        best, med = _F(np.finfo(_F).max), 0
+        for a in idx:
+            acc = _F(0)
+            for b in idx:
+                dx, dy, dz = (_F(pts[a, d] - pts[b, d]) for d in range(3))
+                acc = _F(acc + np.sqrt(_F(_F(_F(dx * dx) + _F(dy * dy)) + _F(dz * dz))))
+            if acc < best:
+                best, med = acc, a
+        out.append(med)
+
+    def build(idx, c, r, depth):
+        if not idx:
+            return
+        if float(r) * 2.0 <= float(res) or len(idx) <= 1 or (max_depth is not None and depth >= max_depth):
+            leaf(idx)
+            return
+        kids = [[] for _ in range(8)]
+        for i in idx:
+            kids[int(pts[i, 0] > c[0]) | int(pts[i, 1] > c[1]) << 1 | int(pts[i, 2] > c[2]) << 2].append(i)
+        hr = _F(r * _F(0.5))
+        for k in range(8):
+            nc = [_F(c[d] + (hr if (k >> d) & 1 else -hr)) for d in range(3)]
+            build(kids[k], nc, hr, depth + 1)
+
+    sys.setrecursionlimit(max(sys.getrecursionlimit(), 10000))
+    build(list(range(n)), ctr, radius, 0)
+    return np.asarray(out, np.int64)

@@ -13,6 +13,7 @@ Chains the oracle pieces exactly as the reference chains its own calls:
                + concatenate + pcl.downsample; guess = between(pose[i-1], pose[i]); ICP.compute.
 """
 import math
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -44,7 +45,15 @@ def transform_points(points, T):
 
 
 def frame_cloud(img, geo, alg="SOCA", train_hs=20, guard_hs=5, rank=10, tau=2.749063720096473, threshold=65,
-                resolution=0.5, radius=1.0, min_points=5, use_reference=False):
+                resolution=0.5, radius=1.0, min_points=5, use_reference=False, cap_points=None):
+    return frame_cloud_raw(img, geo, alg, train_hs, guard_hs, rank, tau, threshold, resolution, radius, min_points,
+                           use_reference, cap_points)[0]
+
+
+def frame_cloud_raw(img, geo, alg="SOCA", train_hs=20, guard_hs=5, rank=10, tau=2.749063720096473, threshold=65,
+                    resolution=0.5, radius=1.0, min_points=5, use_reference=False, cap_points=None):
+    """(frame_cloud, the number of Cartesian points before the filters).  cap_points: the front end's per-frame
+    capacity -- a frame with more points keeps its first cap_points (row-major order) before the filters."""
     if use_reference and orc.have_reference():  # the unmodified reference cfar.cpp (oracle/_ref)
         mask, _ = orc.cfar_reference(alg, img, train_hs, guard_hs, rank, tau)
         mask = np.ascontiguousarray(mask)
@@ -52,12 +61,13 @@ def frame_cloud(img, geo, alg="SOCA", train_hs=20, guard_hs=5, rank=10, tau=2.74
     else:
         mask = orc.cfar_u8(alg, img, train_hs, guard_hs, rank, tau, threshold)
     _, pts = featx_ref.cart_points(mask, geo)
-    pts = pts.astype(np.float32)  # pybind: points -> Eigen float matrix
+    raw = len(pts)
+    pts = pts[:cap_points].astype(np.float32)  # pybind: points -> Eigen float matrix
     if len(pts) and resolution > 0:
         pts, _ = orc.downsample(pts, resolution)
     if min_points > 1 and len(pts) > 0:
         pts, _ = orc.remove_outlier(pts, radius, min_points)
-    return pts
+    return pts, raw
 
 
 def slam_cloud(points, flip_lateral=True):
@@ -71,11 +81,22 @@ def slam_cloud(points, flip_lateral=True):
 
 
 def run(frames, poses, geo, window=3, submap_resolution=0.5, min_points=50, icp_params=None, flip_lateral=True,
-        **feat_kw):
+        cap_points=None, cap_source=None, cap_target=None, icp_filters=None, threads=1, **feat_kw):
     """Returns (clouds, results); clouds = the keyframe clouds as SLAM holds them;
-    results[i] = dict(status, T, iterations, inliers, n_target)."""
+    results[i] = dict(status, T, iterations, inliers, n_target).
+    The batched front end's limits (None: none): cap_points cuts every frame's Cartesian cloud (frame_cloud_raw),
+    and a frame that overflowed it, or whose source / window submap exceeds cap_source / cap_target, is TOO_LARGE (8)
+    before the min_points test.  icp_filters: a voxel_filter_ref.IcpFilters for the scan match (the min_points test
+    counts the clouds before its data filters).  threads: host threads for the frames' clouds and the scan matches
+    (the oracle's C calls release the GIL); the results do not depend on it."""
     prm = icp_params or orc.IcpParams()
-    clouds = [slam_cloud(frame_cloud(f, geo, **feat_kw), flip_lateral) for f in frames]
+    orc._load_port()  # (load, and build if need be, the oracle libraries before any thread calls them)
+    if icp_filters is not None:
+        from . import voxel_filter_ref
+        voxel_filter_ref._load()
+    pool = ThreadPoolExecutor(max(1, int(threads)))
+    made = list(pool.map(lambda f: frame_cloud_raw(f, geo, cap_points=cap_points, **feat_kw), frames))
+    clouds = [slam_cloud(c, flip_lateral) for c, _ in made]
     results = []
     for i in range(len(frames)):
         guess = between(poses[i - 1], poses[i]) if i > 0 else np.eye(3, dtype=np.float32)
@@ -84,10 +105,25 @@ def run(frames, poses, geo, window=3, submap_resolution=0.5, min_points=50, icp_
         if len(tgt) and submap_resolution > 0:
             tgt, _ = orc.downsample(tgt, submap_resolution)
         src = clouds[i]
-        if len(src) < min_points or len(tgt) < min_points:
-            results.append(dict(status=7, T=guess, iterations=0, inliers=0, n_target=len(tgt)))
+        skip = dict(T=guess, iterations=0, inliers=0, n_target=len(tgt))
+        if ((cap_points is not None and made[i][1] > cap_points) or (cap_source is not None and len(src) > cap_source)
+                or (cap_target is not None and len(tgt) > cap_target)):
+            results.append(dict(status=8, **skip))
             continue
-        r = orc.icp(src, tgt, guess, prm)
-        r["n_target"] = len(tgt)
-        results.append(r)
+        if len(src) < min_points or len(tgt) < min_points:
+            results.append(dict(status=7, **skip))
+            continue
+        results.append(pool.submit(_match, src, tgt, guess, prm, icp_filters))
+    results = [r.result() if not isinstance(r, dict) else r for r in results]
+    pool.shutdown()
     return clouds, results
+
+
+def _match(src, tgt, guess, prm, icp_filters):
+    if icp_filters is None:
+        r = orc.icp(src, tgt, guess, prm)
+    else:
+        from . import voxel_filter_ref
+        r = voxel_filter_ref.icp(src, tgt, guess, prm, icp_filters)
+    r["n_target"] = len(tgt)
+    return r

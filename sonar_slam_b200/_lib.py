@@ -119,6 +119,8 @@ _EXTRA_SIGNATURES = {
     "sfe_frontend_icp_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_copy_to_host": [c_void_p, c_void_p, c_void_p, ctypes.c_uint64],
+    "sfe_ctx_set_grid_sms": [c_void_p, c_int, ctypes.POINTER(ctypes.c_int32)],
+    "sfe_ctx_occupancy": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_int32)],
     "sfe_frontend_create": [c_void_p, c_void_p, c_void_p, c_int, ctypes.POINTER(c_void_p)],
     "sfe_frontend_set_timing": [c_void_p, c_int],
     "sfe_frontend_set_carry": [c_void_p, c_int],
@@ -298,6 +300,24 @@ class Context:
     @property
     def launches(self):
         return int(self.lib.sfe_launch_count(self.handle))
+
+    def set_grid_sms(self, n):
+        """For tests: size this context's persistent launches for min(n, the device's) SMs (n <= 0: the device's
+        count), so that each CTA takes more work items in a row; results do not change (sfe_ctx_set_grid_sms).
+        Returns the count now in force."""
+        eff = ctypes.c_int32()
+        check(self.lib.sfe_ctx_set_grid_sms(self.handle, int(n), ctypes.byref(eff)), "sfe_ctx_set_grid_sms")
+        return eff.value
+
+    def occupancy(self):
+        """For tests: [(threads, dynamic shared memory bytes, CTAs per SM), ...] of the persistent one-CTA launch
+        configurations this context has sized, oldest first (the last 16; sfe_ctx_occupancy)."""
+        cap = 16
+        t, s, q = (np.zeros(cap, np.int32) for _ in range(3))
+        n = ctypes.c_int32()
+        check(self.lib.sfe_ctx_occupancy(self.handle, ptr(t), ptr(s), ptr(q), cap, ctypes.byref(n)),
+              "sfe_ctx_occupancy")
+        return [(int(t[k]), int(s[k]), int(q[k])) for k in range(min(n.value, cap))]
 
     def close(self):
         if getattr(self, "handle", None):

@@ -150,7 +150,7 @@ int sfe_ctx_create(int device, void *cuda_stream, int own_stream, sfe_ctx **out)
   }
   sfe_ctx *ctx = new sfe_ctx();
   ctx->device = device;
-  ctx->sm_count = prop.multiProcessorCount;
+  ctx->sm_count = ctx->device_sm_count = prop.multiProcessorCount;
   ctx->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
   if (!own_stream) {
     ctx->stream = (cudaStream_t)cuda_stream;
@@ -205,6 +205,30 @@ int sfe_sync(sfe_ctx *ctx) {
 }
 
 uint64_t sfe_launch_count(const sfe_ctx *ctx) { return ctx ? ctx->launches : 0; }
+
+int sfe_ctx_set_grid_sms(sfe_ctx *ctx, int sms, int32_t *effective) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_ctx_set_grid_sms: null context");
+  ctx->sm_count = sms >= 1 ? std::min(sms, ctx->device_sm_count) : ctx->device_sm_count;
+  if (effective) *effective = ctx->sm_count;
+  return SFE_OK;
+}
+
+int sfe_ctx_occupancy(const sfe_ctx *ctx, int32_t *threads, int32_t *smem, int32_t *per_sm, int capacity,
+                      int32_t *n) {
+  SFE_REQUIRE(ctx && n && capacity >= 0 && (capacity == 0 || (threads && smem && per_sm)),
+              "sfe_ctx_occupancy: null argument");
+  const int size = (int)std::size(ctx->occ);
+  const bool wrapped = ctx->occ[ctx->occ_next].fn != nullptr;  // (the ring is full: its oldest entry is next)
+  int k = 0;
+  for (int i = 0; i < size; ++i) {
+    const auto &e = ctx->occ[((wrapped ? ctx->occ_next : 0) + i) % size];
+    if (!e.fn) continue;
+    if (k < capacity) threads[k] = e.threads, smem[k] = (int32_t)e.smem, per_sm[k] = e.per_sm;
+    ++k;
+  }
+  *n = k;
+  return SFE_OK;
+}
 
 int sfe_copy_to_host(sfe_ctx *ctx, void *dst_host, const void *src_dev, uint64_t bytes) {
   SFE_REQUIRE(ctx && (bytes == 0 || (dst_host && src_dev)), "sfe_copy_to_host: null argument");

@@ -53,7 +53,8 @@ struct sfe_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool owns_stream = false;
-  int sm_count = 0;
+  int sm_count = 0;         // SMs the persistent launches are sized for (sfe_ctx_set_grid_sms; default the device's)
+  int device_sm_count = 0;  // the device's SM count
   int max_smem_optin = 0;
   sfe::Buffer scratch[sfe::SCR_COUNT];  // per-subsystem scratch
   sfe::Buffer stage_in[2];  // device staging for the *_host entry points

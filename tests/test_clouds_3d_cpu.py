@@ -1,63 +1,15 @@
 """CPU-only: the 3-D cloud oracles (oracle/cloud3_ref.c orc_downsample3 / orc_match_brute3 /
 orc_match_knn3) against independent restatements, the z = 0 equivalence with the 2-D oracles, and the argument checks
 `bruce_slam.pcl` / `ops` make on [N,3] clouds before any device work."""
-import sys
-
 import numpy as np
 import pytest
 
 from oracle import cloud3_ref as c3
+from oracle.cloud3_ref import octree_literal
 from oracle import knn_ref
 from oracle import oracle as orc
 
 F = np.float32
-
-
-def octree_literal(pts, resolution, max_depth=None):
-    """A second statement of the 3-D down-sample: the recursive octree of libpointmatcher's Octree_<T,3>, built node by
-    node with float32 scalars (centre = min + extent * 0.5 per axis, half-size = the largest half-extent, split while
-    2 * radius > resolution and more than one point, children by x > cx | y > cy << 1 | z > cz << 2 in index order,
-    medoid = first minimum of the sequential float32 sum of sqrt((dx*dx + dy*dy) + dz*dz)).  max_depth: nodes at that
-    depth become leaves (the device's cut at 15 levels).  Returns the kept indices in output order."""
-    pts = np.asarray(pts, F)
-    n = len(pts)
-    if n == 0:
-        return np.zeros(0, np.int64)
-    res = F(resolution)
-    mn, mx = pts.min(0), pts.max(0)
-    ext = [F(mx[d] - mn[d]) for d in range(3)]
-    ctr = [F(mn[d] + F(ext[d] * F(0.5))) for d in range(3)]
-    radius = max(F(e * F(0.5)) for e in ext)
-    out = []
-
-    def leaf(idx):
-        best, med = F(np.finfo(F).max), 0
-        for a in idx:
-            acc = F(0)
-            for b in idx:
-                dx, dy, dz = (F(pts[a, d] - pts[b, d]) for d in range(3))
-                acc = F(acc + np.sqrt(F(F(F(dx * dx) + F(dy * dy)) + F(dz * dz))))
-            if acc < best:
-                best, med = acc, a
-        out.append(med)
-
-    def build(idx, c, r, depth):
-        if not idx:
-            return
-        if float(r) * 2.0 <= float(res) or len(idx) <= 1 or (max_depth is not None and depth >= max_depth):
-            leaf(idx)
-            return
-        kids = [[] for _ in range(8)]
-        for i in idx:
-            kids[int(pts[i, 0] > c[0]) | int(pts[i, 1] > c[1]) << 1 | int(pts[i, 2] > c[2]) << 2].append(i)
-        hr = F(r * F(0.5))
-        for k in range(8):
-            nc = [F(c[d] + (hr if (k >> d) & 1 else -hr)) for d in range(3)]
-            build(kids[k], nc, hr, depth + 1)
-
-    sys.setrecursionlimit(max(sys.getrecursionlimit(), 10000))
-    build(list(range(n)), ctr, radius, 0)
-    return np.asarray(out, np.int64)
 
 
 def _random(n, seed, spread=(20.0, 20.0, 5.0)):

@@ -12,7 +12,7 @@ from oracle import cloud3_ref as c3
 from sonar_slam_b200 import ops, synth
 from sonar_slam_b200.bruce_slam import pcl
 
-from test_clouds_3d_cpu import octree_literal
+from oracle.cloud3_ref import octree_literal
 
 pytestmark = pytest.mark.gpu
 
