@@ -873,31 +873,32 @@ static int launch_ring(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map,
   return SFE_OK;
 }
 
-template <typename InT, int ALG>
+template <typename InT, int ALG, bool WITH_THR>
 static int launch_ring_out(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
   const bool m = p.mask != nullptr, b = p.bits != nullptr;
-  if (p.thr != nullptr) {  // the "2" variants
-    if (m && b) return launch_ring<InT, ALG, true, true, true>(ctx, st, in_map, out_map, p);
-    if (m) return launch_ring<InT, ALG, true, true, false>(ctx, st, in_map, out_map, p);
-    if (b) return launch_ring<InT, ALG, true, false, true>(ctx, st, in_map, out_map, p);
-    return launch_ring<InT, ALG, true, false, false>(ctx, st, in_map, out_map, p);
-  }
-  if (m && b) return launch_ring<InT, ALG, false, true, true>(ctx, st, in_map, out_map, p);
-  if (m) return launch_ring<InT, ALG, false, true, false>(ctx, st, in_map, out_map, p);
-  if (b) return launch_ring<InT, ALG, false, false, true>(ctx, st, in_map, out_map, p);
+  if (m && b) return launch_ring<InT, ALG, WITH_THR, true, true>(ctx, st, in_map, out_map, p);
+  if (m) return launch_ring<InT, ALG, WITH_THR, true, false>(ctx, st, in_map, out_map, p);
+  if (b) return launch_ring<InT, ALG, WITH_THR, false, true>(ctx, st, in_map, out_map, p);
+  if constexpr (WITH_THR) return launch_ring<InT, ALG, true, false, false>(ctx, st, in_map, out_map, p);
   return SFE_OK;  // nothing to write
 }
 
-template <typename InT>
+template <typename InT, bool WITH_THR>
 static int launch_ring_alg(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_map, const CUtensorMap &out_map, const CfarParams &p) {
   switch (p.alg) {
     case SFE_CFAR_CA:
-      return launch_ring_out<InT, SFE_CFAR_CA>(ctx, st, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_CA, WITH_THR>(ctx, st, in_map, out_map, p);
     case SFE_CFAR_SOCA:
-      return launch_ring_out<InT, SFE_CFAR_SOCA>(ctx, st, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_SOCA, WITH_THR>(ctx, st, in_map, out_map, p);
     default:
-      return launch_ring_out<InT, SFE_CFAR_GOCA>(ctx, st, in_map, out_map, p);
+      return launch_ring_out<InT, SFE_CFAR_GOCA, WITH_THR>(ctx, st, in_map, out_map, p);
   }
+}
+
+// smallest uint8 value x with (double)x > d; 256 when there is none (d >= 255 or NaN)
+static int u8_above(double d) {
+  if (d != d || d >= 255.0) return 256;
+  return d < 0 ? 0 : (int)floor(d) + 1;
 }
 
 // M[S] = smallest uint8 cell value x with (double)x > tau*S/div (the reference's compare) and
@@ -905,20 +906,9 @@ static int launch_ring_alg(sfe_ctx *ctx, cudaStream_t st, const CUtensorMap &in_
 static void build_u8_lut(const CfarParams &p, std::vector<uint16_t> &lut) {
   const int n = (p.alg == SFE_CFAR_CA ? 2 : 1) * CF_T * 255 + 1;
   lut.resize(n);
-  int g = 0;
-  if (p.gate_on) {
-    if (p.gate_d != p.gate_d) g = 256;
-    else if (p.gate_d < 0) g = 0;
-    else if (p.gate_d >= 255.0) g = 256;
-    else g = (int)floor(p.gate_d) + 1;
-  }
+  const int g = p.gate_on ? u8_above(p.gate_d) : 0;
   for (int S = 0; S < n; ++S) {
-    const double d = p.tau * (double)(float)S / p.div;
-    int m;
-    if (d != d) m = 256;
-    else if (d < 0) m = 0;
-    else if (d >= 255.0) m = 256;
-    else m = (int)floor(d) + 1;
+    const int m = u8_above(p.tau * (double)(float)S / p.div);
     lut[S] = (uint16_t)(m > g ? m : g);
   }
 }
@@ -1033,11 +1023,12 @@ int sfe::cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int
       if (rc != SFE_OK) return rc;
       p.flags = (uint8_t *)ctx->scratch[SCR_CFAR_FLAGS].ptr;
       SFE_CUDA(cudaMemsetAsync(p.flags, 0, (size_t)F * p.strips, st));
-      rc = launch_ring_alg<float>(ctx, st, in_map, out_map, p);
+      rc = thr != nullptr ? launch_ring_alg<float, true>(ctx, st, in_map, out_map, p)
+                          : launch_ring_alg<float, false>(ctx, st, in_map, out_map, p);
       if (rc != SFE_OK) return rc;
       return launch_exact<float>(ctx, st, (const float *)img, p, p.flags);  // re-does flagged strips only
     }
-    if (thr == nullptr && isfinite(tau)) {
+    if (thr == nullptr) {  // (tau is finite: `fast` requires a finite tau / div)
       // integer kernels with the threshold table (re-uploaded only when the parameters change; the cache key lives
       // in the context next to the buffer it describes)
       std::vector<uint16_t> lut_host;
@@ -1058,9 +1049,7 @@ int sfe::cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int
       }
       const uint16_t *lut = (const uint16_t *)ctx->scratch[SCR_CFAR_LUT].ptr;
       const int n = lut_n;
-      const char *force = getenv("SFE_CFAR_U8_KERNEL");  // development switch: "lut" / "gate4"
-      const bool want_gate4 = force ? (strcmp(force, "gate4") == 0) : true;
-      if (want_gate4 && g_min >= (force ? 1 : CG_GMIN_LO) && g_min <= 128 && (mask != nullptr || bits != nullptr)) {
+      if (g_min >= CG_GMIN_LO && g_min <= 128 && (mask != nullptr || bits != nullptr)) {
         // gated 4-beams-per-thread kernel: its own tensor map (two [16 x 256] boxes per chunk)
         CUtensorMap in4;
         rc = encode_tensor_map_3d(&in4, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, img, B, R, F, CG_W / 2, CF_CH, 1);
@@ -1080,16 +1069,14 @@ int sfe::cfar_run(sfe_ctx *ctx, cudaStream_t st, const void *img, int dtype, int
         default: return launch_u8_lut<SFE_CFAR_GOCA>(ctx, st, in_map, out_map, p, lut, n);
       }
     }
-    return launch_ring_alg<uint8_t>(ctx, st, in_map, out_map, p);
+    return launch_ring_alg<uint8_t, true>(ctx, st, in_map, out_map, p);  // uint8 with a threshold image
   }
   if (dtype == SFE_U8 && alg == SFE_CFAR_OS && T >= 1 && T <= 127 && R > 2 * (T + G) && isfinite(tau)) {
     // sliding-histogram OS-CFAR; 256-entry pass table M[v] = smallest cell value with x > tau*v (and the gate)
     std::vector<uint16_t> lut(256);
-    int g = 0;
-    if (p.gate_on) g = (p.gate_d != p.gate_d) ? 256 : (p.gate_d < 0 ? 0 : (p.gate_d >= 255.0 ? 256 : (int)floor(p.gate_d) + 1));
+    const int g = p.gate_on ? u8_above(p.gate_d) : 0;
     for (int v = 0; v < 256; ++v) {
-      const double d = tau * (double)(float)v;
-      const int m = (d != d) ? 256 : (d < 0 ? 0 : (d >= 255.0 ? 256 : (int)floor(d) + 1));
+      const int m = u8_above(tau * (double)(float)v);
       lut[v] = (uint16_t)(m > g ? m : g);
     }
     int rc = ensure(ctx, ctx->scratch[SCR_CFAR_LUT], 65536, st);

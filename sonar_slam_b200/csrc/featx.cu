@@ -426,11 +426,6 @@ __global__ void __launch_bounds__(FI_THREADS)
   }
 }
 
-static bool ctx_force_gather(const sfe_ctx *) {
-  const char *e = getenv("SFE_CART_DENSE");  // development switch: force the dense kernel
-  return e && e[0] == '1';
-}
-
 template <int FPB>
 static int launch_cart(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const uint8_t *mask, const uint32_t *bits, int F, int cap,
                        int32_t *ij, float *xy, int32_t *count) {
@@ -488,7 +483,7 @@ int sfe::cart_points_run(sfe_ctx *ctx, cudaStream_t st, const sfe_maps *m, const
     const size_t pw = (size_t)m->R * wpr, cw = (size_t)(npix + 31) / 32;
     const size_t smem = sizeof(uint32_t) * (pw + cw + (pw + 1) / 2 + 1);
     // (the emission's rank table of Cartesian word pairs reuses the polar plane: it must fit there)
-    if (m->inv_off != nullptr && smem <= (size_t)ctx->max_smem_optin - 2048 && (cw + 1) / 2 <= pw && !ctx_force_gather(ctx)) {
+    if (m->inv_off != nullptr && smem <= (size_t)ctx->max_smem_optin - 2048 && (cw + 1) / 2 <= pw) {
       int per_sm;
       const int rc = ctas_per_sm(ctx, (const void *)cart_scatter_kernel, FXS_THREADS, smem, &per_sm);
       if (rc != SFE_OK) return rc;

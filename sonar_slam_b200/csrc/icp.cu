@@ -55,6 +55,14 @@ __device__ __forceinline__ bool icp_takes(const IcpBox &x, int ns, int nt) {
   return x.ns_lo < ns && ns <= x.ns_hi && x.nt_lo < nt && nt <= x.nt_hi;
 }
 
+// One-pass exact path (per-lane searches with certified matches, no pruning passes): problems of up to
+// ICP_SMALL_MULT source points per thread (and nt <= 4096) take it, and its certificates are ICP_MARGIN_MULT of the
+// point's last step.  Both chosen on the config-4 replay (sources of ~360 points in 128-thread CTAs: a lower limit
+// sends more problems down the slower pruned path); not re-measured on H100.  icp_run hands them to the kernel as
+// IcpBatch fields: folded in as compile-time constants they change icp_kernel's register allocation and spills.
+constexpr int ICP_SMALL_MULT = 5;
+constexpr float ICP_MARGIN_MULT = 6.f;
+
 struct IcpBatch {
   const float *src_pts;
   const int *src_off;
@@ -77,8 +85,8 @@ struct IcpBatch {
   uint16_t *orig_ws;  // [slots][nt_max]
   float2 *nrm_ws;     // [slots][nt_max] point-to-plane only: normal of the target point at every sorted position
   int use_order;      // search passes visit the source points in spatially sorted order (big problems only)
-  float margin_mult;  // certificate size in units of the point's last step (one-pass path)
-  int small_mult;     // problems with ns <= small_mult * blockDim.x (and nt <= 4096) take the one-pass exact path
+  float margin_mult;  // ICP_MARGIN_MULT: certificate size in units of the point's last step (one-pass path)
+  int small_mult;     // ICP_SMALL_MULT: ns <= small_mult * blockDim.x (and nt <= 4096) takes the one-pass path
   int slot_by_smid;   // workspace slot = %smid (one CTA per SM, one CTA per problem) instead of blockIdx.x
   int *next;          // persistent CTAs: work counter (next_work_item), or null: CTA c takes problems c, c + gridDim.x, ...
   const int *list;    // icp_run's classes: this launch's problems, largest first (icp_classify_kernel), or null: 0 .. P-1
@@ -771,22 +779,6 @@ static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool den
   return icp_kernel_of<512, 1, false>(plane, filt);
 }
 
-static void icp_tuning(IcpBatch &b) {
-  // One-pass exact path (per-lane searches with certified matches, no pruning passes) for problems of up to
-  // 5 source points per thread (chosen on the config-4 replay, sources of ~360 points in 128-thread CTAs: a lower
-  // limit sends more problems down the slower pruned path; not re-measured on H100).
-  static const int mult = [] {  // development switch: SFE_ICP_SMALL_MULT
-    const char *e = getenv("SFE_ICP_SMALL_MULT");
-    return e ? atoi(e) : 5;
-  }();
-  b.small_mult = mult;
-  static const float mm = [] {  // development switch: SFE_ICP_MARGIN_MULT
-    const char *e = getenv("SFE_ICP_MARGIN_MULT");
-    return e ? (float)atof(e) : 6.f;
-  }();
-  b.margin_mult = mm;
-}
-
 // The global-source class: sources above what the shared-memory layouts hold (icp_source_limit).  Each persistent CTA
 // keeps its per-source-point arrays in a slice of global workspace; all slices together stay within ICP_SRC_WS_CAP.
 constexpr size_t ICP_SRC_WS_CAP = size_t(512) << 20;
@@ -1321,7 +1313,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.P = pb.P;
   b.box = ICP_BOX_ALL;
   b.cell_scale = 1.0f, b.prm = *prm;
-  icp_tuning(b);
+  b.small_mult = ICP_SMALL_MULT, b.margin_mult = ICP_MARGIN_MULT;
   const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt)};
   if (classes) return icp_run_classes(ctx, st, d, b, class_list, n_classes, ns_max, nt_max, class_of);
   IcpSplit s;

@@ -26,7 +26,7 @@ namespace sfe {
 // (tools/icp_sizes.py): sources after the filters mean 359, max 639 points; window submaps after the 0.5 m thinning
 // (the ICP target) mean 406, max 779.  The class takes every frame of that bag: a second launch that holds only a
 // few frames costs a full problem latency at its tail.  The source cap has no margin over the bag's largest source
-// (639): above 5 points per thread (640 for 128 threads, icp.cu: small_mult) a problem leaves the one-pass path, so a
+// (639): above 5 points per thread (640 for 128 threads, icp.cu: ICP_SMALL_MULT) a problem leaves the one-pass path, so a
 // larger cap would only admit problems that take the slower pruned path.  The target cap keeps 3 % over the bag's
 // largest target (779): at 640 / 800 points a 128-thread CTA needs 27.4 KB of shared memory, which with the 1 KB the
 // driver reserves per CTA lets an H100 SM (228 KB) hold 8 of them (810 is the largest target that does), and the

@@ -167,31 +167,42 @@ def test_large_batch_checksum_properties(gpu_ctx):
     assert np.array_equal(a[idx].cpu().numpy(), want)
 
 
+def _pack_bits(masks):
+    """0/1 masks [F, R, B] as the bit plane sfe_cfar_dev writes: [F, R, ceil(B/32)] words, bit b & 31 of word b >> 5
+    is beam b, the bits past B are 0."""
+    F, R, B = masks.shape
+    padded = np.zeros((F, R, (B + 31) // 32 * 32), np.uint8)
+    padded[..., :B] = masks
+    return np.packbits(padded, axis=-1, bitorder="little").view("<u4")
+
+
 @pytest.mark.parametrize("shape", [(3, 512, 512), (2, 512, 528), (2, 100, 256), (1, 77, 1024), (2, 333, 48),
                                    (1, 51, 16), (2, 512, 1040)])
-@pytest.mark.parametrize("gate", [16, 65, 127])
-def test_u8_gated_four_beam_kernel(gpu_ctx, shape, gate, monkeypatch):
-    """cfar_u8_gate4_kernel (4 beams per thread, detections decided in a rare branch) against the table kernel
-    it replaces and against the oracle: speckle frames (few candidates), bright frames (every row takes the
-    branch), strips that end inside a 512-beam block, images shorter than the window."""
-    rng = np.random.default_rng(shape[1] * 7 + shape[2] + gate)
+@pytest.mark.parametrize("gate", [None, 14, 15, 16, 65, 127, 128])
+def test_u8_gated_four_beam_kernel(gpu_ctx, shape, gate):
+    """The uint8 streaming kernels against the oracle, each reached through cfar_run's own choice: the gated
+    4-beams-per-thread kernel (cfar_u8_gate4_kernel, detections decided in a rare branch) when the pass table's
+    least entry g_min lies in [16, 128], else the table kernel.  A zero window sum has entry 1 for any finite tau, so
+    g_min = max(1, floor(gate) + 1): gates 15 .. 127 take the gate kernel; no gate, 14 and 128 the table kernel.
+    Speckle frames (few candidates), bright frames (every row takes the branch), strips that end inside a 512-beam
+    block, images shorter than the window; masks and bit planes, alone and together."""
+    g_min = 1 if gate is None else max(1, int(np.floor(gate)) + 1)
+    kernel = "gate4" if 16 <= g_min <= 128 else "table"
+    rng = np.random.default_rng(shape[1] * 7 + shape[2] + (gate or 0))
     speckle = np.clip(np.rint(rng.rayleigh(18.0, shape)), 0, 255).astype(np.uint8)
     bright = rng.integers(0, 256, shape).astype(np.uint8)
     for imgs in (speckle, bright):
         dev = torch.from_numpy(imgs).cuda()
         for alg in ("CA", "SOCA", "GOCA"):
-            monkeypatch.setenv("SFE_CFAR_U8_KERNEL", "gate4")
             a = ops.cfar(dev, alg, 20, 5, TAU[alg], gate=gate, want_mask=True, want_bits=True)
             b = ops.cfar(dev, alg, 20, 5, TAU[alg], gate=gate, want_mask=False, want_bits=True)
             c = ops.cfar(dev, alg, 20, 5, TAU[alg], gate=gate, want_mask=True)
-            monkeypatch.setenv("SFE_CFAR_U8_KERNEL", "lut")
-            ref = ops.cfar(dev, alg, 20, 5, TAU[alg], gate=gate, want_mask=True, want_bits=True)
             want, _ = _oracle_batch(alg, imgs, 20, 5, 0, TAU[alg], gate=gate)
-            assert np.array_equal(ref["mask"].cpu().numpy(), want), (alg, "table kernel")
-            assert np.array_equal(a["mask"].cpu().numpy(), want), (alg, shape, gate)
-            assert np.array_equal(c["mask"].cpu().numpy(), want), (alg, shape, gate)
-            assert torch.equal(a["bits"], ref["bits"]) and torch.equal(b["bits"], ref["bits"]), (alg, shape, gate)
-            assert np.array_equal(_unpack_bits(b["bits"], shape[2]), want)
+            tag = (kernel, alg, shape, gate)
+            assert np.array_equal(a["mask"].cpu().numpy(), want), tag
+            assert np.array_equal(c["mask"].cpu().numpy(), want), tag
+            assert np.array_equal(a["bits"].cpu().numpy().view(np.uint32), _pack_bits(want)), tag
+            assert np.array_equal(b["bits"].cpu().numpy().view(np.uint32), _pack_bits(want)), tag
 
 
 def test_float_images_with_nan_and_inf(gpu_ctx):

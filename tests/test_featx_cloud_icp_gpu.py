@@ -56,23 +56,46 @@ def test_cart_points_batches_random_masks_vs_cv2(gpu_ctx):
     assert np.array_equal(small["ij"][1].cpu().numpy(), out["ij"][1, :10].cpu().numpy())
 
 
-def test_cart_points_dense_and_detection_driven_kernels_agree(gpu_ctx, monkeypatch):
-    geo = _geo("uniform")
-    maps = _maps(gpu_ctx, geo, 512, 512)
-    imgs = torch.from_numpy(synth.make_frames(range(40, 46))).cuda()
-    det = ops.cfar(imgs, "SOCA", 20, 5, TAU_SOCA, gate=65, want_bits=True)
-    a = ops.cart_points(maps, bits=det["bits"], capacity=6000)
-    monkeypatch.setenv("SFE_CART_DENSE", "1")
-    b = ops.cart_points(maps, mask=det["mask"], capacity=6000)
-    monkeypatch.delenv("SFE_CART_DENSE")
-    assert torch.equal(a["count"], b["count"]) and int(a["count"].min()) > 100
-    for f in range(6):
-        k = int(a["count"][f])
-        assert torch.equal(a["ij"][f, :k], b["ij"][f, :k]) and torch.equal(a["xy"][f, :k], b["xy"][f, :k])
+def _odd_geo():
+    return featx_ref.Geometry(0.1, 200, np.round(np.linspace(-3000, 3500, 96)).astype(np.int16))
+
+
+def _bits(masks):
+    """0/1 masks [F, R, B] as a CFAR bit plane: int32 [F, R, ceil(B/32)], bit b & 31 of word b >> 5 is beam b."""
+    F, R, B = masks.shape
+    padded = np.zeros((F, R, (B + 31) // 32 * 32), np.uint8)
+    padded[..., :B] = masks
+    return torch.from_numpy(np.packbits(padded, axis=-1, bitorder="little").view("<i4")).cuda()
+
+
+def test_cart_points_dense_and_detection_driven_kernels_agree(gpu_ctx):
+    """Each Cartesian-points kernel against the oracle, from masks and from bit planes, on a geometry cart_points_run
+    sends it to.  The detection-driven scatter kernel needs the rank table of Cartesian word pairs to fit in the polar
+    plane, (cw + 1) / 2 <= pw: the uniform 512 x 512 frame does; the 200 x 96 frame, whose Cartesian image is twice
+    as wide as its beams are many, takes the dense kernel."""
+    speckle = synth.make_frames(range(40, 46))
+    det = ops.cfar(torch.from_numpy(speckle).cuda(), "SOCA", 20, 5, TAU_SOCA, gate=65)["mask"].cpu().numpy()
+    rng = np.random.default_rng(1)
+    for geo, masks, scatter in ((_geo("uniform"), det, True),
+                                (_odd_geo(), (rng.random((5, 200, 96)) < 0.1).astype(np.uint8), False)):
+        F, R, B = masks.shape
+        pw, cw = R * ((B + 31) // 32), (geo.rows * geo.cols + 31) // 32  # polar / Cartesian bit-plane words
+        assert ((cw + 1) // 2 <= pw) == scatter, (pw, cw)
+        maps = _maps(gpu_ctx, geo, R, B)
+        wants = [featx_ref.cart_points(m, geo) for m in masks]
+        assert min(len(w[0]) for w in wants) > 100
+        cap = max(len(w[0]) for w in wants)
+        for kw in (dict(mask=torch.from_numpy(masks).cuda()), dict(bits=_bits(masks))):
+            out = ops.cart_points(maps, capacity=cap, **kw)
+            for f, (locs, pts) in enumerate(wants):
+                k = int(out["count"][f])
+                assert k == len(locs), (scatter, list(kw), f)
+                assert np.array_equal(out["ij"][f, :k].cpu().numpy(), locs), (scatter, list(kw), f)
+                assert np.array_equal(out["xy"][f, :k].cpu().numpy(), pts.astype(np.float32)), (scatter, list(kw), f)
 
 
 def test_cart_points_odd_geometry(gpu_ctx):
-    geo = featx_ref.Geometry(0.1, 200, np.round(np.linspace(-3000, 3500, 96)).astype(np.int16))
+    geo = _odd_geo()
     maps = _maps(gpu_ctx, geo, 200, 96)
     rng = np.random.default_rng(1)
     masks = (rng.random((5, 200, 96)) < 0.1).astype(np.uint8)

@@ -8,9 +8,6 @@ it is meant to reach: 128 / 256 / 512-thread CTAs, <512, 2> and <512, 1>, the sp
 table at the in-CTA limit, one CTA per problem with the workspace slot taken from the SM id, the one-pass certified
 search and the pruned three-pass search."""
 import itertools
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -431,55 +428,6 @@ def test_degenerate_targets(gpu_ctx, kind):
             res = _icp(prm).compute_batch(src, tgt, gs)
             for k, g in enumerate(gs):
                 _assert_equal(res, k, src, tgt, g, oprm, (kind, n))
-
-
-# ------------------------------------------------------------------ development switches
-SWITCH_CALLS = (0, 1, 4, 6, 7)  # of _size_calls: every thread count, both paths, both 512 register budgets
-
-
-def _switch_batch():
-    """The batch a child process runs with a development switch set: results of fixed-20 and shipped checkers."""
-    calls = _size_calls()
-    out = {}
-    for c in SWITCH_CALLS:
-        pairs = _build(calls[c][1], 1, 100 * c)
-        for chk, kw in CHECKERS.items():
-            prm, _ = _params(**kw)
-            for j, r in enumerate(run_pairs(pairs, prm)):
-                for key in ("T", "iterations", "inliers", "status"):
-                    out[f"{c}_{chk}_{j}_{key}"] = np.asarray(r[key])
-    return out
-
-
-def _child_main(path):
-    np.savez(path, **_switch_batch())
-
-
-@pytest.mark.parametrize("var,value", [("SFE_ICP_SMALL_MULT", "0"), ("SFE_ICP_SMALL_MULT", "1000"),
-                                       ("SFE_ICP_MARGIN_MULT", "0.5"), ("SFE_ICP_MARGIN_MULT", "50")])
-def test_development_switches_do_not_change_results(gpu_ctx, tmp_path, var, value):
-    here = os.path.dirname(os.path.abspath(__file__))
-    repo = os.path.dirname(here)
-    out = tmp_path / "child.npz"
-    code = (f"import sys; sys.path[:0] = [{repo!r}, {here!r}]; import test_icp_dispatch_gpu as t; "
-            f"t._child_main({str(out)!r})")
-    env = dict(os.environ, **{var: value})
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=repo, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    child = dict(np.load(out))
-    mine = _switch_batch()
-    assert sorted(child) == sorted(mine)
-    for key in mine:
-        assert np.array_equal(child[key].view(np.uint8), mine[key].view(np.uint8)), key
-    # and the parent's results are the oracle's
-    calls = _size_calls()
-    for c in SWITCH_CALLS:
-        pairs = _build(calls[c][1], 1, 100 * c)
-        for chk, kw in CHECKERS.items():
-            _, oprm = _params(**kw)
-            for j, (s, t, gs) in enumerate(pairs):
-                res = {key: mine[f"{c}_{chk}_{j}_{key}"] for key in ("T", "iterations", "inliers", "status")}
-                _assert_equal(res, 0, s, t, gs[0], oprm, (var, value, c, chk, j))
 
 
 # ------------------------------------------------------------------ the user's route, and what it must refuse
