@@ -33,7 +33,8 @@ extern "C" {
                                  sfe_downsample_cta_limit, dim = 3 in sfe_downsample_dev / _host, sfe_icp_dim_dev,
                                  sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit,
                                  SFE_ICP_DATA_OCTREE and SFE_ICP_DATA_VOXEL (new sfe_icp_data_filter kinds; both structs
-                                 keep their sizes), sfe_ctx_set_grid_sms, sfe_ctx_occupancy */
+                                 keep their sizes), sfe_ctx_set_grid_sms, sfe_ctx_occupancy, sfe_icp_robust with
+                                 sfe_icp_set_robust and sfe_frontend_set_icp_robust */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -433,6 +434,32 @@ SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int di
  * positive, counts in range; SFE_ERR_ARG leaves the setting as it was. */
 SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);
 
+/* libpointmatcher's RobustOutlierFilter with scaleEstimator none / fixed (scale 1) and point2point residuals: a soft
+ * M-estimator weight for every matched pair, from its squared distance e2 (the value MaxDist compares) and k = tuning,
+ * k2 = k * k, all float32 with IEEE-rounded division and sqrt and nothing contracted:
+ *   SFE_ICP_ROBUST_CAUCHY  1 / (1 + e2 / k2)              SFE_ICP_ROBUST_WELSCH  (float)exp((double)(-(e2 / k2)))
+ *   SFE_ICP_ROBUST_SC      e2 >= k ? 4k2 / (k + e2)^2 : 1  SFE_ICP_ROBUST_GM      k2 / (k + e2)^2
+ *   SFE_ICP_ROBUST_TUKEY   e2 >= k2 ? 0 : (1 - e2 / k2)^2  SFE_ICP_ROBUST_HUBER   e2 >= k2 ? k / sqrt(e2) : 1
+ *   SFE_ICP_ROBUST_L1      1 / sqrt(e2)
+ * and 0 where e2 >= approximation (+inf: no cut-off).  A pair's weight is the product with the 0 / 1 weights of the
+ * other outlier filters (MaxDist, Trimmed, MinDist, Median): the robust weight where they keep the pair, else 0 -- NaN
+ * for an L1 weight of inf (e2 == 0).  Pairs of non-zero weight are kept (inliers); the point-to-point minimiser takes
+ * weighted means (sum w p) * (1 / sum w) and the cross-covariance sum (w (r - mean_r)) (p - mean_p)^T, the
+ * point-to-plane one A = sum (w F) F^T and b = -sum (w F) ((q - r).n); every sum sequential in point order
+ * (oracle/robust_ref.c).  2-D clouds only, float32 sums only (flags bit 1 is SFE_ERR_UNSUPPORTED with a robust filter).
+ * The point-to-plane minimiser keeps its sum scratch apart from the distances, 2.5 KB more shared memory per CTA. */
+enum { SFE_ICP_ROBUST_CAUCHY = 1, SFE_ICP_ROBUST_WELSCH = 2, SFE_ICP_ROBUST_SC = 3, SFE_ICP_ROBUST_GM = 4,
+       SFE_ICP_ROBUST_TUKEY = 5, SFE_ICP_ROBUST_HUBER = 6, SFE_ICP_ROBUST_L1 = 7 };
+typedef struct {
+  int fct;             /* SFE_ICP_ROBUST_* */
+  float tuning;        /* k: finite and positive */
+  float approximation; /* weight 0 where e2 >= approximation; not NaN; +inf: no cut-off */
+} sfe_icp_robust;
+/* The RobustOutlierFilter later sfe_icp_dev / _host / _batch_host / sfe_icp_source_limit and sfe_frontend_icp_dev
+ * calls on ctx apply (copied; NULL: none, the default).  Checked here: fct known, tuning finite and positive,
+ * approximation not NaN; SFE_ERR_ARG leaves the setting as it was.  dim 3 calls with it set are SFE_ERR_UNSUPPORTED. */
+SFE_API int sfe_icp_set_robust(sfe_ctx *ctx, const sfe_icp_robust *robust);
+
 /* ------------------------------------------------------------------ robust covariance of ICP samples (row N1)
  * SLAM.compute_icp_with_cov, slam.py:365-371: MinCovDet(store_precision=False, support_fraction=0.8).fit(samples),
  * batched over n_problems candidates.  The algorithm is scikit-learn 1.9's (sklearn/covariance/_robust_covariance.py:
@@ -565,6 +592,9 @@ SFE_API int sfe_frontend_set_scan_match(sfe_frontend *fe, int enable);
  * default).  The reading filters see each frame's cloud, the reference filters its window submap; the min_points test
  * still counts the clouds before the filters (slam.py checks them before ICP runs). */
 SFE_API int sfe_frontend_set_icp_filters(sfe_frontend *fe, const sfe_icp_filters *filters);
+/* The RobustOutlierFilter (sfe_icp_robust) of this front end's scan match, from the next run call on (copied; NULL:
+ * none, the default); checked as by sfe_icp_set_robust. */
+SFE_API int sfe_frontend_set_icp_robust(sfe_frontend *fe, const sfe_icp_robust *robust);
 /* Several sonar geometries in one front end: a bag whose range setting changes (num_ranges, range_resolution, beam
  * count) is fed as one sequence, and the first frames after a change are matched against the keyframes before it, as
  * the reference's window of metric keyframe clouds does (slam.py:632-633).

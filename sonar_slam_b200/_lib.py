@@ -155,6 +155,8 @@ _EXTRA_SIGNATURES = {
     "sfe_icp_cta_limit": [c_void_p, c_int, c_int, c_void_p],
     "sfe_icp_source_limit": [c_void_p, c_void_p, c_int, c_void_p],
     "sfe_frontend_set_icp_filters": [c_void_p, c_void_p],
+    "sfe_icp_set_robust": [c_void_p, c_void_p],
+    "sfe_frontend_set_icp_robust": [c_void_p, c_void_p],
     "sfe_mincovdet_dev": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_mincovdet_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_double, c_double, c_int,
@@ -241,13 +243,29 @@ class IcpFilters(ctypes.Structure):
         return [(arr[k].kind, arr[k].dim, arr[k].dist) for k in range(n)]
 
 
+# SFE_ICP_ROBUST_*: RobustOutlierFilter robustFct codes
+ROBUST_FCT = {"cauchy": 1, "welsch": 2, "sc": 3, "gm": 4, "tukey": 5, "huber": 6, "L1": 7}
+
+
+class IcpRobust(ctypes.Structure):
+    """sfe_icp_robust (include/sonarfe.h): libpointmatcher's RobustOutlierFilter with scaleEstimator none / fixed --
+    fct a ROBUST_FCT name or code, tuning k (finite, > 0), approximation (weight 0 where the squared distance is at
+    least this; +inf: no cut-off)."""
+    _fields_ = [("fct", c_int), ("tuning", c_float), ("approximation", c_float)]
+
+    def __init__(self, fct="cauchy", tuning=1.0, approximation=float("inf")):
+        super().__init__(ROBUST_FCT[fct] if isinstance(fct, str) else int(fct), float(tuning), float(approximation))
+
+
 class IcpConfig(IcpParams):
     """IcpParams as an ICP YAML configures it (bruce_slam.pcl.parse_icp_yaml): the same structure, passed by reference
-    where IcpParams is, plus `.filters` -- the IcpFilters of the modules IcpParams does not carry, or None."""
+    where IcpParams is, plus `.filters` -- the IcpFilters of the modules IcpParams does not carry, or None -- and
+    `.robust` -- the IcpRobust of a RobustOutlierFilter, or None."""
 
-    def __init__(self, *args, filters=None, **kwargs):
+    def __init__(self, *args, filters=None, robust=None, **kwargs):
         super().__init__(*args, **kwargs)
         self.filters = filters
+        self.robust = robust
 
 
 def icp_filters_of(params, filters=None):
@@ -259,6 +277,18 @@ def set_icp_filters(ctx, filters):
     """sfe_icp_set_filters on ctx (None: no filter), so a call never inherits an earlier call's filters."""
     check(ctx.lib.sfe_icp_set_filters(ctx.handle, ctypes.byref(filters) if filters is not None else None),
           "sfe_icp_set_filters")
+
+
+def icp_robust_of(params, robust=None):
+    """The RobustOutlierFilter a call with these ICP parameters runs: `robust` when given, else params.robust
+    (IcpConfig)."""
+    return robust if robust is not None else getattr(params, "robust", None)
+
+
+def set_icp_robust(ctx, robust):
+    """sfe_icp_set_robust on ctx (None: no robust filter), so a call never inherits an earlier call's setting."""
+    check(ctx.lib.sfe_icp_set_robust(ctx.handle, ctypes.byref(robust) if robust is not None else None),
+          "sfe_icp_set_robust")
 
 
 FrontendParams._fields_ = [

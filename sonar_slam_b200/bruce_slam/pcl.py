@@ -148,8 +148,8 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
 _SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are implemented, plus its commented-out "
               "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference, the Max/MinDist data "
               "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, the "
-              "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, and the MinDist / MedianDist "
-              "outlier filters")
+              "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, the MinDist / MedianDist "
+              "outlier filters and one RobustOutlierFilter with scaleEstimator none or fixed")
 _DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
 
 
@@ -214,12 +214,45 @@ def _voxel_filter(p):
 
 
 _RESAMPLERS = {_OCTREE: _octree_filter, _VOXEL: _voxel_filter}
+_ROBUST = "RobustOutlierFilter"
+
+
+def _robust_filter(p):
+    """RobustOutlierFilter {robustFct, tuning, approximation, scaleEstimator, nbIterationForScale, distanceType} ->
+    _lib.IcpRobust.  Upstream defaults robustFct cauchy, tuning 1, approximation inf, distanceType point2point.  With
+    scaleEstimator none or fixed the scale is 1 and the tuning is k itself; nbIterationForScale is then moot."""
+    fct = str(p.get("robustFct", "cauchy"))
+    if fct == "student":
+        raise NotImplementedError(f"ICP yaml: {_ROBUST} robustFct student is not implemented ({_SUPPORTED})")
+    if fct not in _lib.ROBUST_FCT:
+        raise ValueError(f"ICP yaml: {_ROBUST} robustFct {fct!r} ({', '.join(_lib.ROBUST_FCT)})")
+    if "scaleEstimator" not in p:
+        raise NotImplementedError(f"ICP yaml: {_ROBUST} without scaleEstimator is not implemented: the default "
+                                  "estimator cannot be checked against upstream; give scaleEstimator none or fixed")
+    scale = str(p["scaleEstimator"])
+    if scale in ("mad", "berg"):
+        raise NotImplementedError(f"ICP yaml: {_ROBUST} scaleEstimator {scale} is not implemented (none and fixed are)")
+    if scale not in ("none", "fixed"):
+        raise ValueError(f"ICP yaml: {_ROBUST} scaleEstimator {scale!r} (mad, berg, none or fixed)")
+    dist = str(p.get("distanceType", "point2point"))
+    if dist == "point2plane":
+        raise NotImplementedError(f"ICP yaml: {_ROBUST} distanceType point2plane is not implemented (point2point is)")
+    if dist != "point2point":
+        raise ValueError(f"ICP yaml: {_ROBUST} distanceType {dist!r} (point2point or point2plane)")
+    k = float(p.get("tuning", 1.0))
+    if not math.isfinite(k) or k <= 0:
+        raise ValueError(f"ICP yaml: {_ROBUST} tuning {k} must be finite and positive")
+    approx = float(p.get("approximation", float("inf")))
+    if math.isnan(approx):
+        raise ValueError(f"ICP yaml: {_ROBUST} approximation is NaN")
+    return _lib.IcpRobust(fct, k, approx)
 
 
 def parse_icp_yaml(text):
     """libpointmatcher ICP YAML (the subset described by _SUPPORTED) -> _lib.IcpConfig: the IcpParams the shipped modules
     set, with `.filters` = the _lib.IcpFilters of the distance, octree and voxel-grid data filters, in their listed
-    order, and the MinDist / MedianDist outlier filters (None when the YAML has none of them)."""
+    order, and the MinDist / MedianDist outlier filters (None when the YAML has none of them), and `.robust` = the
+    _lib.IcpRobust of its RobustOutlierFilter (None without one)."""
     import yaml
     cfg = yaml.safe_load(text) or {}
 
@@ -240,7 +273,7 @@ def parse_icp_yaml(text):
         chain.append((name,) + f)
 
     prm = _lib.IcpConfig(outlier_max_dist=-1.0, trim_ratio=-1.0, max_iterations=40, smooth_length=0)
-    reading, reference, outlier = [], [], {}
+    reading, reference, outlier, robust = [], [], {}, None
     for node in cfg.get("readingDataPointsFilters") or []:
         name, p = one(node)
         if name not in _DATA_FILTERS and name not in _RESAMPLERS:
@@ -282,6 +315,10 @@ def parse_icp_yaml(text):
             if not math.isfinite(v) or v < 0:
                 raise ValueError(f"ICP yaml: {name} {p} needs a finite, non-negative value")
             outlier[name] = v
+        elif name == _ROBUST:
+            if robust is not None:
+                raise NotImplementedError(f"ICP yaml: a second {_ROBUST} is not implemented ({_SUPPORTED})")
+            robust = _robust_filter(p)
         else:
             raise NotImplementedError(f"ICP yaml: outlier filter {name} ({_SUPPORTED})")
     name, p = one(cfg.get("errorMinimizer", "PointToPointErrorMinimizer"))
@@ -314,6 +351,7 @@ def parse_icp_yaml(text):
         prm.filters = _lib.IcpFilters(min_dist=outlier.get("MinDistOutlierFilter", -1.0),
                                       median_factor=outlier.get("MedianDistOutlierFilter", -1.0),
                                       reading=[f[1:] for f in reading], reference=[f[1:] for f in reference])
+    prm.robust = robust
     return prm
 
 
@@ -358,6 +396,8 @@ class ICP(object):
             if _lib.icp_filters_of(self.params) is not None:
                 raise NotImplementedError("ICP on 3-column clouds: data filters and MinDist / MedianDist outlier filters "
                                           "are not implemented in 3-D")
+            if _lib.icp_robust_of(self.params) is not None:
+                raise NotImplementedError("ICP on 3-column clouds: the RobustOutlierFilter is not implemented in 3-D")
         return dim
 
     @staticmethod
@@ -394,6 +434,7 @@ class ICP(object):
         ctx = _lib.default_context()
         import ctypes
         _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
+        _lib.set_icp_robust(ctx, _lib.icp_robust_of(self.params))
         if dim == 3:
             _lib.check(ctx.lib.sfe_icp_dim_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src), len(src),
                                                 _lib.ptr(tgt), len(tgt), 3, _lib.ptr(g), n, _lib.ptr(T),
@@ -437,6 +478,7 @@ class ICP(object):
         ctx = _lib.default_context()
         import ctypes
         _lib.set_icp_filters(ctx, _lib.icp_filters_of(self.params))
+        _lib.set_icp_robust(ctx, _lib.icp_robust_of(self.params))
         if dim == 3:
             _lib.check(ctx.lib.sfe_icp_batch_dim_host(ctx.handle, ctypes.byref(self.params), _lib.ptr(src),
                                                       _lib.ptr(soff), len(srcs), _lib.ptr(tgt), _lib.ptr(toff),

@@ -504,7 +504,7 @@ int sfe_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pts_de
   return icp_run(ctx, ctx->stream, prm,
                  {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
                   tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev}, nullptr, 0, nullptr,
-                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr, ctx->has_icp_robust ? &ctx->icp_robust : nullptr);
 }
 
 int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters) {
@@ -515,6 +515,17 @@ int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters) {
     ctx->icp_filters = *filters;
   }
   ctx->has_icp_filters = filters != nullptr;
+  return SFE_OK;
+}
+
+int sfe_icp_set_robust(sfe_ctx *ctx, const sfe_icp_robust *robust) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_icp_set_robust: null context");
+  if (robust) {
+    const int rc = icp_robust_check(robust, "sfe_icp_set_robust");
+    if (rc != SFE_OK) return rc;
+    ctx->icp_robust = *robust;
+  }
+  ctx->has_icp_robust = robust != nullptr;
   return SFE_OK;
 }
 
@@ -539,7 +550,8 @@ static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *
   SFE_REQUIRE(ctx && prm, "%s: null context or parameters", name);
   SFE_REQUIRE(dim == 2 || dim == 3, "%s: points must have 2 or 3 columns (got %d)", name, dim);
   const sfe_icp_filters *filt = ctx->has_icp_filters ? &ctx->icp_filters : nullptr;
-  const int rc = icp_params_check(prm, dim, filt, name);  // (before anything is copied)
+  const sfe_icp_robust *robust = ctx->has_icp_robust ? &ctx->icp_robust : nullptr;
+  const int rc = icp_params_check(prm, dim, filt, name, robust);  // (before anything is copied)
   if (rc != SFE_OK) return rc;
   SFE_REQUIRE(n_src_clouds >= 1 && n_tgt_clouds >= 1 && n_problems >= 0, "%s: bad sizes", name);
   if (n_problems == 0) return SFE_OK;
@@ -597,8 +609,8 @@ static int icp_batch_host(sfe_ctx *ctx, const char *name, const sfe_icp_params *
     IcpProblems pb{{d_src, d_soff, nullptr, ns_max}, {d_tgt, d_toff, nullptr, nt_max}, d_ids, d_ids + P, n_problems,
                    d_guess, d_T, d_res, d_res + P, d_res + 2 * P};
     pb.n_tgt_clouds = n_tgt_clouds, pb.n_src_clouds = n_src_clouds;
-    int rc = dim == 3 ? icp3_run(ctx, ctx->stream, prm, pb, filt)
-                      : icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr, filt);
+    int rc = dim == 3 ? icp3_run(ctx, ctx->stream, prm, pb, filt, robust)
+                      : icp_run(ctx, ctx->stream, prm, pb, nullptr, 0, nullptr, filt, robust);
     if (rc != SFE_OK) return rc;
     SFE_CUDA(cudaMemcpyAsync(T_host, d_T, sizeof(float) * TS * P, cudaMemcpyDeviceToHost, ctx->stream));
     SFE_CUDA(cudaMemcpyAsync(iters_host, d_res, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, ctx->stream));
@@ -652,7 +664,7 @@ int sfe_icp_dim_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *src_pt
   return icp3_run(ctx, ctx->stream, prm,
                   {{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, src_id_dev,
                    tgt_id_dev, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev},
-                  ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+                  ctx->has_icp_filters ? &ctx->icp_filters : nullptr, ctx->has_icp_robust ? &ctx->icp_robust : nullptr);
 }
 
 int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit) {
@@ -669,7 +681,8 @@ int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32
   SFE_REQUIRE(ctx && prm && limit, "sfe_icp_source_limit: null pointer");
   SFE_CUDA(cudaSetDevice(ctx->device));
   int n;
-  const int rc = icp_source_limit(ctx, prm, dim, ctx->has_icp_filters ? &ctx->icp_filters : nullptr, &n);
+  const int rc = icp_source_limit(ctx, prm, dim, ctx->has_icp_filters ? &ctx->icp_filters : nullptr, &n,
+                                  ctx->has_icp_robust ? &ctx->icp_robust : nullptr);
   if (rc == SFE_OK) *limit = n;
   return rc;
 }

@@ -77,6 +77,8 @@ struct sfe_ctx {
   int *work = nullptr;  // device [SFE_WORK_COUNTERS]: work counters of the persistent kernels (sfe::next_work_item)
   sfe_icp_filters icp_filters = {};  // sfe_icp_set_filters
   bool has_icp_filters = false;
+  sfe_icp_robust icp_robust = {};  // sfe_icp_set_robust
+  bool has_icp_robust = false;
 };
 
 struct sfe_maps {  // per-geometry polar->Cartesian sampling table (featx.cu)

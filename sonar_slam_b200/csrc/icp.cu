@@ -99,7 +99,7 @@ struct IcpBatch {
   // global-source class (icp_kernel's GSRC instantiations): CTA c keeps its per-source-point arrays at src_ws + c *
   // src_ws_stride in global memory
   unsigned char *src_ws;
-  size_t src_ws_stride;
+  size_t src_ws_stride;  sfe_icp_robust robust;  // the ROBUST kernels only: the RobustOutlierFilter (last, so the other fields keep their offsets)
 };
 
 
@@ -390,6 +390,67 @@ __device__ __forceinline__ float seq_sum9_warp(int n, float *scratch, const Pos 
   return s;
 }
 
+// ROBUST point-to-point: R (<= 8) sequential float32 sums in index order at once, by one warp: lane j parks the R terms
+// of point base + j (term(i, v)) in `scratch` ([R][36] floats, single-buffered), lanes 0..R-1 add their row's 32 values
+// in order.  Lane c (c < R) returns the sum of component c.  All 32 lanes of the warp must call it.
+template <int R, typename F>
+__device__ __forceinline__ float seq_sum_rows_warp(int n, float *scratch, F term) {
+  static_assert(R >= 1 && R <= 8, "seq_sum_rows_warp: one row per lane of the first eight");
+  const int lane = threadIdx.x & 31;
+  float s = 0.f;
+  for (int base = 0; base < n; base += 32) {
+    float v[R];
+    if (base + lane < n) {
+      term(base + lane, v);
+    } else {
+#pragma unroll
+      for (int c = 0; c < R; ++c) v[c] = 0.f;
+    }
+#pragma unroll
+    for (int c = 0; c < R; ++c) scratch[c * 36 + lane] = v[c];
+    __syncwarp();
+    if (lane < R) {
+      const float4 *r = reinterpret_cast<const float4 *>(scratch + lane * 36);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float4 a = r[k];
+        s = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(s, a.x), a.y), a.z), a.w);
+      }
+    }
+    __syncwarp();  // (the next batch rewrites the rows)
+  }
+  return s;
+}
+
+// RobustOutlierFilter weight of a pair of squared distance e2 (oracle/robust_ref.c): k = tuning, k2 = k * k, division
+// and sqrt IEEE-rounded, nothing contracted, welsch's exp in float64 rounded to float32; 0 where e2 >= approximation
+__device__ __forceinline__ float icp_robust_weight(const sfe_icp_robust &r, float e2) {
+  const float k = r.tuning, k2 = __fmul_rn(k, k);
+  float w = 1.f;
+  switch (r.fct) {
+    case SFE_ICP_ROBUST_CAUCHY: w = __fdiv_rn(1.f, __fadd_rn(1.f, __fdiv_rn(e2, k2))); break;
+    case SFE_ICP_ROBUST_WELSCH: w = (float)exp((double)(-__fdiv_rn(e2, k2))); break;
+    case SFE_ICP_ROBUST_SC: {
+      const float t = __fadd_rn(k, e2);
+      w = e2 >= k ? __fdiv_rn(__fmul_rn(4.f, k2), __fmul_rn(t, t)) : 1.f;
+      break;
+    }
+    case SFE_ICP_ROBUST_GM: {
+      const float t = __fadd_rn(k, e2);
+      w = __fdiv_rn(k2, __fmul_rn(t, t));
+      break;
+    }
+    case SFE_ICP_ROBUST_TUKEY: {
+      const float u = __fsub_rn(1.f, __fdiv_rn(e2, k2));
+      w = e2 >= k2 ? 0.f : __fmul_rn(u, u);
+      break;
+    }
+    case SFE_ICP_ROBUST_HUBER: w = e2 >= k2 ? __fdiv_rn(k, __fsqrt_rn(e2)) : 1.f; break;
+    case SFE_ICP_ROBUST_L1: w = __fdiv_rn(1.f, __fsqrt_rn(e2)); break;
+  }
+  return e2 >= r.approximation ? 0.f : w;
+}
+
 #include "icp_kernel_body.cuh"
 
 // Data filters of sfe_icp_filters (MaxDist / MinDistDataPointsFilter): cloud c of a batch (cloud id[c], or c with id
@@ -656,13 +717,24 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
 }
 
 // ---------------------------------------------------------------------------- host side
-int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what) {
-  if (dim == 3 && (prm->minimizer != 0 || (prm->flags & 2) || filt)) {
+int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what,
+                     const sfe_icp_robust *robust) {
+  if (dim == 3 && (prm->minimizer != 0 || (prm->flags & 2) || filt || robust)) {
     set_error("%s: %s is not supported on [x, y, z] clouds by the 3-D scan matcher", what,
               prm->minimizer != 0 ? "the point-to-plane error minimizer"
               : (prm->flags & 2)  ? "float64 accumulation (flags bit 1)"
-                                  : "ICP filters (sfe_icp_set_filters)");
+              : filt              ? "ICP filters (sfe_icp_set_filters)"
+                                  : "the RobustOutlierFilter (sfe_icp_set_robust)");
     return SFE_ERR_UNSUPPORTED;
+  }
+  if (robust && (prm->flags & 2)) {
+    set_error("%s: the RobustOutlierFilter (sfe_icp_set_robust) runs with float32 sums only, not with float64 "
+              "accumulation (flags bit 1)", what);
+    return SFE_ERR_UNSUPPORTED;
+  }
+  if (robust) {
+    const int rc = icp_robust_check(robust, what);
+    if (rc != SFE_OK) return rc;
   }
   SFE_REQUIRE(prm->max_iterations >= 1, "%s: maxIterationCount must be >= 1", what);
   SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "%s: unknown error minimizer %d", what, prm->minimizer);
@@ -678,6 +750,15 @@ int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *
   SFE_REQUIRE(prm->trim_ratio <= 1.0f, "%s: TrimmedDistOutlierFilter ratio %g is above 1", what,
               (double)prm->trim_ratio);
   return filt ? icp_filters_check(filt, what) : SFE_OK;
+}
+
+int icp_robust_check(const sfe_icp_robust *r, const char *what) {
+  SFE_REQUIRE(r->fct >= SFE_ICP_ROBUST_CAUCHY && r->fct <= SFE_ICP_ROBUST_L1, "%s: unknown RobustOutlierFilter robustFct %d",
+              what, r->fct);
+  SFE_REQUIRE(std::isfinite(r->tuning) && r->tuning > 0.f, "%s: RobustOutlierFilter tuning %g (finite and positive)",
+              what, (double)r->tuning);
+  SFE_REQUIRE(!std::isnan(r->approximation), "%s: a NaN RobustOutlierFilter approximation is not supported", what);
+  return SFE_OK;
 }
 
 int icp_filters_check(const sfe_icp_filters *f, const char *what) {
@@ -726,7 +807,7 @@ static int pick_max_cells(int nt_max) {
 // Shared memory of icp_kernel's layout for sources of up to ns_max points (>= 1).  In-CTA class: targets of up to
 // nt_max points (>= 1), 16-bit target positions, after big problems traded cell-table entries (coarser cells) for room;
 // *max_cells receives the table's size.  Map class: 32-bit target positions and no target arrays (*max_cells 0).
-static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, bool map, size_t budget, int *max_cells) {
+static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, bool map, bool robust, size_t budget, int *max_cells) {
   const bool use_order = ns_max > 1024;
   const size_t pos = map ? sizeof(int) : sizeof(uint16_t);  // match[] and prev[]
   auto smem_for = [&](int mc) {
@@ -734,7 +815,7 @@ static size_t icp_cta_smem(int ns_max, int nt_max, bool plane, bool map, size_t 
            (map ? 0 : sizeof(float2) * (size_t)nt_max + sizeof(uint32_t) * (size_t)((mc + 2) / 2 + 1)) + 8 +
            sizeof(float2) * (size_t)ns_max + sizeof(float) * (size_t)ns_max + 2 * pos * (size_t)ns_max +
            (size_t)ns_max + 4 + sizeof(float) * (size_t)ns_max + (use_order ? sizeof(uint16_t) * (size_t)ns_max : 0) +
-           16 + (plane && ns_max < ICP_PLANE_SCRATCH ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
+           16 + (plane && (robust || ns_max < ICP_PLANE_SCRATCH) ? 16 + ICP_PLANE_SCRATCH * sizeof(float) : 0);
   };
   int mc = 0;
   if (!map) {
@@ -756,9 +837,13 @@ static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 153
 // icp_kernel's instantiation for `threads`-thread CTAs with `smem` bytes of layout: (threads, register budget), then
 // the flags.  In-CTA class: 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers;
 // dense (icp_run's classes): 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get
-// them (IcpClass::dense).  Map class: one instantiation per CTA size.  filt: sfe_icp_filters.
+// them (IcpClass::dense).  Map class: one instantiation per CTA size.  filt: sfe_icp_filters; robust: the
+// RobustOutlierFilter (FILT instantiations with ROBUST).
 template <int THREADS, int MINB, bool MAP, bool GSRC = false>
-static const void *icp_kernel_of(bool plane, bool filt) {
+static const void *icp_kernel_of(bool plane, bool filt, bool robust) {
+  if (robust)
+    return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true, GSRC, true>
+                 : (const void *)icp_kernel<THREADS, MINB, false, MAP, true, GSRC, true>;
   if (filt)
     return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true, GSRC>
                  : (const void *)icp_kernel<THREADS, MINB, false, MAP, true, GSRC>;
@@ -766,17 +851,17 @@ static const void *icp_kernel_of(bool plane, bool filt) {
                : (const void *)icp_kernel<THREADS, MINB, false, MAP, false, GSRC>;
 }
 
-static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool map) {
+static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool robust, bool map) {
   if (map) {
-    if (threads == 128) return icp_kernel_of<128, 7, true>(plane, filt);
-    if (threads == 256) return icp_kernel_of<256, 4, true>(plane, filt);
-    return icp_kernel_of<512, 1, true>(plane, filt);
+    if (threads == 128) return icp_kernel_of<128, 7, true>(plane, filt, robust);
+    if (threads == 256) return icp_kernel_of<256, 4, true>(plane, filt, robust);
+    return icp_kernel_of<512, 1, true>(plane, filt, robust);
   }
-  if (threads == 128 && dense) return icp_kernel_of<128, 8, false>(plane, filt);
-  if (threads == 128) return icp_kernel_of<128, 7, false>(plane, filt);
-  if (threads == 256) return icp_kernel_of<256, 4, false>(plane, filt);
-  if (smem <= 110 * 1024) return icp_kernel_of<512, 2, false>(plane, filt);
-  return icp_kernel_of<512, 1, false>(plane, filt);
+  if (threads == 128 && dense) return icp_kernel_of<128, 8, false>(plane, filt, robust);
+  if (threads == 128) return icp_kernel_of<128, 7, false>(plane, filt, robust);
+  if (threads == 256) return icp_kernel_of<256, 4, false>(plane, filt, robust);
+  if (smem <= 110 * 1024) return icp_kernel_of<512, 2, false>(plane, filt, robust);
+  return icp_kernel_of<512, 1, false>(plane, filt, robust);
 }
 
 // The global-source class: sources above what the shared-memory layouts hold (icp_source_limit).  Each persistent CTA
@@ -800,10 +885,11 @@ namespace sfe {
 enum { ICP_CTA = 0, ICP_MAP = 1, ICP_GSRC = 2 };
 
 // One dimension's kernels and layouts: icp_kernel's instantiations for the minimizer and the filters (dim 2), or the
-// icp3_body kernels (dim 3).  filt: sfe_icp_filters (icp_filters_on).
+// icp3_body kernels (dim 3).  filt: sfe_icp_filters (icp_filters_on), or a robust filter; robust: the
+// RobustOutlierFilter.
 struct IcpDim {
   int dim;
-  bool plane, filt;
+  bool plane, filt, robust;
   int threads(int cls, int ns) const { return dim == 3 ? ICP3_THREADS : cls == ICP_GSRC ? ICP_THREADS : icp_threads(ns); }
   // class cls's kernel for `threads`-thread CTAs with `smem` bytes of layout; dense: IcpClass::dense
   const void *kernel(int cls, int threads, size_t smem, bool dense = false) const {
@@ -811,8 +897,8 @@ struct IcpDim {
       return cls == ICP_CTA ? (const void *)icp3_kernel
              : cls == ICP_MAP ? (const void *)icp3_map_kernel
                               : (const void *)icp3_gsrc_kernel;
-    if (cls == ICP_GSRC) return icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt);
-    return icp_kernel_for(threads, smem, plane, dense, filt, cls == ICP_MAP);
+    if (cls == ICP_GSRC) return icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt, robust);
+    return icp_kernel_for(threads, smem, plane, dense, filt, robust, cls == ICP_MAP);
   }
   // shared memory class cls may take next to sources of ns points: the budget of the instantiation that runs the
   // largest of its layouts
@@ -826,7 +912,7 @@ struct IcpDim {
       return dim == 3 ? icp3_gsrc_smem()
                       : ((sizeof(IcpShared) + 15) & ~size_t(15)) + (plane ? ICP_PLANE_SCRATCH * sizeof(float) : 0);
     if (dim == 3) return cls == ICP_MAP ? icp3_map_smem(ns) : icp3_cta_smem(ns, nt, budget, max_cells);
-    return icp_cta_smem(ns, nt, plane, cls == ICP_MAP, budget, max_cells);
+    return icp_cta_smem(ns, nt, plane, cls == ICP_MAP, robust, budget, max_cells);
   }
   size_t slice(int ns) const { return dim == 3 ? icp3_src_slice(ns) : icp_src_slice(ns); }
   const char *what() const { return dim == 3 ? "icp (3-D)" : "icp"; }
@@ -1234,7 +1320,8 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
 // problems: in-CTA, map class (targets above the in-CTA layout's limit, read as map grids from global memory) and
 // global-source class (sources above the shared-memory layouts).
 int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb_in,
-                 const IcpClass *class_list, int n_classes, int *class_of, const sfe_icp_filters *filt) {
+                 const IcpClass *class_list, int n_classes, int *class_of, const sfe_icp_filters *filt,
+                 const sfe_icp_robust *robust) {
   IcpProblems pb = pb_in;
   const int ns_max = pb.src.n_max, nt_max = pb.tgt.n_max;
   SFE_REQUIRE(ctx && prm, "icp: null context or parameters");
@@ -1251,7 +1338,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   const bool classes = n_classes > 0;
   SFE_REQUIRE((ns_max <= 65535 && nt_max <= 65535) || !classes,
               "icp: clouds of more than 65535 points are not supported (got %d, %d)", ns_max, nt_max);
-  int rc = icp_params_check(prm, 2, filt, "icp");
+  int rc = icp_params_check(prm, 2, filt, "icp", robust);
   if (rc != SFE_OK) return rc;
   const int *gate_src = nullptr, *gate_tgt = nullptr;
   if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
@@ -1305,6 +1392,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     b.median_factor = filt->median_factor;
     b.gate_src_cnt = gate_src, b.gate_tgt_cnt = gate_tgt;
   }
+  if (robust) b.robust = *robust;
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;
   b.raw_cnt = pb.raw_cnt, b.raw_cap = pb.raw_cap;
@@ -1314,7 +1402,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.box = ICP_BOX_ALL;
   b.cell_scale = 1.0f, b.prm = *prm;
   b.small_mult = ICP_SMALL_MULT, b.margin_mult = ICP_MARGIN_MULT;
-  const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt)};
+  const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr};
   if (classes) return icp_run_classes(ctx, st, d, b, class_list, n_classes, ns_max, nt_max, class_of);
   IcpSplit s;
   if ((rc = icp_split(ctx, d, ns_max, nt_max, s)) != SFE_OK) return rc;
@@ -1325,19 +1413,20 @@ int sfe::icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit) {
   SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
   SFE_REQUIRE(ns >= 0 && ns <= 65535, "icp: sources of %d points are not supported (0..65535)", ns);
   IcpSplit s;
-  const int rc = icp_split(ctx, {dim, false, false}, ns, 0, s);
+  const int rc = icp_split(ctx, {dim, false, false, false}, ns, 0, s);
   if (rc == SFE_OK) *limit = s.gsrc ? 0 : s.L;  // (a global-source launch: no in-CTA layout holds these sources)
   return rc;
 }
 
 int sfe::icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt,
-                          int *limit) {
+                          int *limit, const sfe_icp_robust *robust) {
   SFE_REQUIRE(ctx && prm && limit, "icp_source_limit: null pointer");
   SFE_REQUIRE(dim == 2 || dim == 3, "icp: points must have 2 or 3 columns (got %d)", dim);
-  int rc = icp_params_check(prm, dim, filt, "icp_source_limit");
+  int rc = icp_params_check(prm, dim, filt, "icp_source_limit", robust);
   if (rc != SFE_OK) return rc;
   IcpSplit s;
-  if ((rc = icp_split(ctx, {dim, prm->minimizer == 1, icp_filters_on(filt)}, 1, 0, s)) == SFE_OK) *limit = s.S;
+  const IcpDim d{dim, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr};
+  if ((rc = icp_split(ctx, d, 1, 0, s)) == SFE_OK) *limit = s.S;
   return rc;
 }
 
@@ -1345,10 +1434,10 @@ int sfe::icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim
 // icp3_map_kernel (targets as map grids from map_build with dim 3, plus their z by grid position) and icp3_gsrc_kernel
 // (sources above the shared-memory layouts) -- as in icp_run.
 int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
-                  const sfe_icp_filters *filt) {
+                  const sfe_icp_filters *filt, const sfe_icp_robust *robust) {
   SFE_REQUIRE(ctx && prm, "icp (3-D): null context or parameters");
   SFE_REQUIRE(pb.P >= 0 && pb.src.n_max >= 0 && pb.tgt.n_max >= 0, "icp (3-D): negative sizes");
-  int rc = icp_params_check(prm, 3, filt, "icp (3-D)");
+  int rc = icp_params_check(prm, 3, filt, "icp (3-D)", robust);
   if (rc != SFE_OK) return rc;
   if (pb.P == 0) return SFE_OK;
   SFE_REQUIRE(pb.src.pts && pb.src.off && pb.tgt.pts && pb.tgt.off && pb.guess && pb.T_out && pb.iters && pb.inliers &&
@@ -1360,7 +1449,7 @@ int sfe::icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, cons
   b.src_id = pb.src_id, b.tgt_id = pb.tgt_id, b.guess = pb.guess;
   b.T_out = pb.T_out, b.iters = pb.iters, b.inliers = pb.inliers, b.status = pb.status;
   b.P = pb.P, b.prm = *prm;
-  const IcpDim d{3, false, false};
+  const IcpDim d{3, false, false, false};
   IcpSplit s;
   if ((rc = icp_split(ctx, d, pb.src.n_max, pb.tgt.n_max, s)) != SFE_OK) return rc;
   return icp_split_run(ctx, st, d, s, b, pb);

@@ -11,10 +11,13 @@
 //          clouds before the data filters;
 //   GSRC:  the global-source class (MAP only) -- sources too large for shared memory: the per-source-point arrays
 //          (reading .. order) sit in the CTA's slice of global workspace (b.src_ws), with 32-bit entries in order[];
-//          shared memory holds IcpShared and, PLANE, seq_sum9_warp's scratch.
+//          shared memory holds IcpShared and, PLANE, seq_sum9_warp's scratch;
+//   ROBUST: (FILT only) the batch runs a RobustOutlierFilter (b.robust): the keep pass (3c) multiplies the 0 / 1 weights
+//          by the robust weight and parks it in dist[], which is dead until the next search; the minimisers' sums
+//          weight their terms by it.  PLANE: seq_sum9_warp's scratch then gets its own 2.5 KB.
 // The body is written in the kernel itself: behind a device-function wrapper the shipped instantiations compiled with
 // larger stack frames.
-template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT, bool GSRC>
+template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT, bool GSRC, bool ROBUST = false>
 __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, const MapArgs mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
@@ -24,6 +27,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
   // block_total's final read (one lane per warp) hold at most 16 warps; the rest of the body loops over blockDim.x.
   static_assert(THREADS % 32 == 0 && THREADS >= 64 && THREADS <= 512, "icp_kernel: 2 to 16 warps per CTA");
   static_assert(MAP || !GSRC, "icp_kernel: the global-source class reads its targets as map grids");
+  static_assert(FILT || !ROBUST, "icp_kernel: the robust filter runs in the FILT instantiations");
   using Pos = std::conditional_t<MAP, int, uint16_t>;   // a target point's sorted position
   using Ord = std::conditional_t<GSRC, int, uint16_t>;  // a source point's index
   constexpr int NONE = MAP ? -1 : 0xffff;                // "no match"
@@ -63,7 +67,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
   // search, which rewrites all of it: launches with room for 640 source points (the front end's small class is
   // exactly that; 2 000 x 20 000 points leave nothing to spare at all) park the scratch there, smaller ones get
   // their own 2.5 KB.  GSRC: always its own, in shared memory.
-  float *pl_scratch = !GSRC && b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
+  float *pl_scratch = !GSRC && !ROBUST && b.ns_max >= ICP_PLANE_SCRATCH ? dist : reinterpret_cast<float *>(smem_raw + off);
   (void)pl_scratch;
 
   const int tid = threadIdx.x, nthr = blockDim.x;
@@ -617,8 +621,24 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
       // 3c. kept pairs.  The candidate match of point i is prev[i] on the one-pass path (its re-search list took
       // match[] meanwhile) and match[i] after the pruning passes; match[i] becomes the candidate or NONE (dropped).
       const Pos *cand = small ? prev : match;
+      // ROBUST: the pair's weight is the product of the 0 / 1 weights and the robust weight (oracle/robust_ref.c): the
+      // robust weight where the others keep the pair, else 0 * w (NaN for w = inf); dist[i] becomes that weight, and
+      // the pair is kept when it is not 0.  A point pruned by pass C (farther than stop_d2 >= 0, so e2 > 0 and w finite)
+      // fails the 0 / 1 filter whose bound set stop_d2, so its weight is 0: the robust filter bounds nothing itself,
+      // and pass C's argument for FILT holds unchanged.
       auto kept = [&](int i) -> int {
         const int m = cand[i];
+        if constexpr (ROBUST) {
+          if (m == NONE) return NONE;
+          bool keep01 = true;
+          if (prm.outlier_max_dist > 0.f) keep01 = keep01 && (dist[i] <= out_d2);
+          if (prm.trim_ratio >= 0.f) keep01 = keep01 && (dist[i] <= limit);
+          if (b.min_d2 >= 0.f) keep01 = keep01 && (dist[i] > b.min_d2);
+          if (b.median_factor >= 0.f) keep01 = keep01 && (dist[i] <= med_limit);
+          const float w = __fmul_rn(keep01 ? 1.f : 0.f, icp_robust_weight(b.robust, dist[i]));
+          dist[i] = w;
+          return w != 0.f ? m : NONE;
+        }
         bool keep = m != NONE;
         if (prm.outlier_max_dist > 0.f) keep = keep && (dist[i] <= out_d2);
         if (prm.trim_ratio >= 0.f) keep = keep && (dist[i] <= limit);
@@ -633,7 +653,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
       // iteration.  (The pruned path's 2 000-point sources keep the weights parallel: measured slower on warp 0.)
       // Float64 mode: every thread takes part in the block_sum reductions.
       int n_keep = 0;
-      float mrx = 0.f, mry = 0.f, mfx = 0.f, mfy = 0.f;
+      float mrx = 0.f, mry = 0.f, mfx = 0.f, mfy = 0.f, sw = 0.f;  // (sw: ROBUST, the sum of the weights)
       double t4[4] = {0, 0, 0, 0};
       float pl[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};  // PLANE: A00 A01 A02 A11 A12 A22, sum F (q-r).n (thread 0)
       if (seq && !small) {  // big problems (long serial sums): every thread forms the weights of its points
@@ -671,6 +691,27 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
             n_keep = __reduce_add_sync(0xffffffffu, cnt);
             __syncwarp();  // (seq_sum9_warp's lanes read other lanes' match[] entries)
           }
+        } else if constexpr (ROBUST) {
+          // the five weighted sums (w, w * step x, w * step y, w * matched reference x, y); dropped pairs add +0
+          int cnt = 0;
+          const float sum = seq_sum_rows_warp<5>(ns, sh.seq_buf, [&](int i, float(&v)[5]) {
+            const int m = small ? kept(i) : match[i];
+            if (small) match[i] = (Pos)m;
+            if (m == NONE) {
+              v[0] = v[1] = v[2] = v[3] = v[4] = 0.f;
+              return;
+            }
+            ++cnt;
+            const float w = dist[i];
+            const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
+            const float2 r = sorted[m];
+            v[0] = w, v[1] = __fmul_rn(w, q.x), v[2] = __fmul_rn(w, q.y), v[3] = __fmul_rn(w, r.x);
+            v[4] = __fmul_rn(w, r.y);
+          });
+          if (small) n_keep = __reduce_add_sync(0xffffffffu, cnt);
+          sw = __shfl_sync(0xffffffffu, sum, 0);
+          mrx = __shfl_sync(0xffffffffu, sum, 1), mry = __shfl_sync(0xffffffffu, sum, 2);
+          mfx = __shfl_sync(0xffffffffu, sum, 3), mfy = __shfl_sync(0xffffffffu, sum, 4);
         } else {
           // the four sums (step x, step y, matched reference x, y); dropped pairs add +0
           int cnt = 0;
@@ -700,6 +741,14 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
               const float2 r = sorted[m];
               const float cr = __fsub_rn(__fmul_rn(q.x, n.y), __fmul_rn(q.y, n.x));
               const float dp = __fadd_rn(__fmul_rn(__fsub_rn(q.x, r.x), n.x), __fmul_rn(__fsub_rn(q.y, r.y), n.y));
+              if constexpr (ROBUST) {  // wF = w * F, then A = sum wF F^T, b = -sum wF ((q - r).n)
+                const float w = dist[i];
+                const float wc = __fmul_rn(w, cr), wx = __fmul_rn(w, n.x), wy = __fmul_rn(w, n.y);
+                v[0] = __fmul_rn(wc, cr), v[1] = __fmul_rn(wc, n.x), v[2] = __fmul_rn(wc, n.y), v[3] = __fmul_rn(wx, n.x);
+                v[4] = __fmul_rn(wx, n.y), v[5] = __fmul_rn(wy, n.y), v[6] = __fmul_rn(wc, dp), v[7] = __fmul_rn(wx, dp);
+                v[8] = __fmul_rn(wy, dp);
+                return;
+              }
               v[0] = __fmul_rn(cr, cr), v[1] = __fmul_rn(cr, n.x), v[2] = __fmul_rn(cr, n.y), v[3] = __fmul_rn(n.x, n.x);
               v[4] = __fmul_rn(n.x, n.y), v[5] = __fmul_rn(n.y, n.y), v[6] = __fmul_rn(cr, dp), v[7] = __fmul_rn(n.x, dp);
               v[8] = __fmul_rn(n.y, dp);
@@ -728,7 +777,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
               for (int k = 0; k < 4; ++k) pl[5 + k] = (float)o4[k];
             }
           } else {
-            const float winv = __fdiv_rn(1.0f, (float)n_keep);
+            const float winv = __fdiv_rn(1.0f, ROBUST ? sw : (float)n_keep);
             mrx = __fmul_rn(mrx, winv), mry = __fmul_rn(mry, winv);
             mfx = __fmul_rn(mfx, winv), mfy = __fmul_rn(mfy, winv);
 
@@ -740,7 +789,8 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
                 const float2 q = apply_T(Ti, reading[i].x, reading[i].y);
                 const float2 r = sorted[m];
                 const float px = __fsub_rn(q.x, mrx), py = __fsub_rn(q.y, mry);
-                const float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
+                float qx = __fsub_rn(r.x, mfx), qy = __fsub_rn(r.y, mfy);
+                if constexpr (ROBUST) qx = __fmul_rn(dist[i], qx), qy = __fmul_rn(dist[i], qy);  // (w r~) p~^T
                 return make_float4(__fmul_rn(qx, px), __fmul_rn(qx, py), __fmul_rn(qy, px), __fmul_rn(qy, py));
               });
 #pragma unroll

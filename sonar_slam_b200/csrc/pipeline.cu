@@ -231,6 +231,8 @@ struct sfe_frontend {
   int scan_match = 1;  // sfe_frontend_set_scan_match
   sfe_icp_filters icp_filters = {};  // sfe_frontend_set_icp_filters
   bool has_icp_filters = false;
+  sfe_icp_robust icp_robust = {};  // sfe_frontend_set_icp_robust
+  bool has_icp_robust = false;
   StageTimer timer;  // optional per-stage timing, on ctx->stream
 };
 
@@ -606,7 +608,8 @@ static int fe_match(sfe_frontend *fe, int f0, int n) {
   pb.guess = fe->guess + 9 * (size_t)f0, pb.T_out = fe->T + 9 * (size_t)f0;
   pb.iters = fe->iters + f0, pb.inliers = fe->inliers + f0, pb.status = fe->status + f0;
   const int rc = icp_run(ctx, st, &p.icp, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, nullptr,
-                         fe->has_icp_filters ? &fe->icp_filters : nullptr);
+                         fe->has_icp_filters ? &fe->icp_filters : nullptr,
+                         fe->has_icp_robust ? &fe->icp_robust : nullptr);
   fe->timer.toc(st);
   return rc;
 }
@@ -787,6 +790,17 @@ int sfe_frontend_set_icp_filters(sfe_frontend *fe, const sfe_icp_filters *filter
     fe->icp_filters = *filters;
   }
   fe->has_icp_filters = filters != nullptr;
+  return SFE_OK;
+}
+
+int sfe_frontend_set_icp_robust(sfe_frontend *fe, const sfe_icp_robust *robust) {
+  SFE_REQUIRE(fe != nullptr, "sfe_frontend_set_icp_robust: null handle");
+  if (robust) {
+    const int rc = icp_robust_check(robust, "sfe_frontend_set_icp_robust");
+    if (rc != SFE_OK) return rc;
+    fe->icp_robust = *robust;
+  }
+  fe->has_icp_robust = robust != nullptr;
   return SFE_OK;
 }
 
@@ -1056,7 +1070,7 @@ int sfe_frontend_icp_dev(sfe_ctx *ctx, const sfe_icp_params *prm, const float *s
   IcpProblems pb{{src_pts_dev, src_off_dev, nullptr, ns_max}, {tgt_pts_dev, tgt_off_dev, nullptr, nt_max}, nullptr,
                  nullptr, n_problems, guess_dev, T_dev, iters_dev, inliers_dev, status_dev};
   return icp_run(ctx, ctx->stream, prm, pb, FE_ICP_CLASSES, FE_ICP_N_CLASSES, class_dev,
-                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr);
+                 ctx->has_icp_filters ? &ctx->icp_filters : nullptr, ctx->has_icp_robust ? &ctx->icp_robust : nullptr);
 }
 
 int sfe_frontend_run_dev(sfe_frontend *fe, const uint8_t *frames_dev, const double *poses_host, int n_frames) {

@@ -76,27 +76,35 @@ constexpr int ICP_MAX_CLASSES = 3;  // classes an icp_run call may list (the cap
 // list.
 // filt (may be null): sfe_icp_filters -- data filters run into scratch once per cloud before the launches (distance
 // filters compacted, octree filters through downsample_run), and the outlier filters in icp_kernel's FILT
-// instantiations; min_points then counts the clouds before the data filters.
+// instantiations; min_points then counts the clouds before the data filters.  robust (may be null): the
+// RobustOutlierFilter, in icp_kernel's ROBUST instantiations (which are FILT ones).
 int icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb, const IcpClass *classes,
-            int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr);
+            int n_classes, int *class_of = nullptr, const sfe_icp_filters *filt = nullptr,
+            const sfe_icp_robust *robust = nullptr);
 // SFE_OK, or SFE_ERR_ARG with a message naming `what`: NaN, unknown kind, dim outside -1 .. 1, counts out of range
 int icp_filters_check(const sfe_icp_filters *f, const char *what);
-// SFE_OK, or an error with a message naming `what`: the settings prm and the filters filt (may be null) that icp_run
-// (dim 2) or icp3_run (dim 3) does not solve.  The 3-D chain refuses point-to-plane, float64 accumulation and filters
+// SFE_OK, or SFE_ERR_ARG with a message naming `what`: unknown robustFct, tuning not finite and positive, NaN
+// approximation
+int icp_robust_check(const sfe_icp_robust *r, const char *what);
+// SFE_OK, or an error with a message naming `what`: the settings prm, the filters filt and the robust filter robust
+// (both may be null) that icp_run (dim 2) or icp3_run (dim 3) does not solve.  The 3-D chain refuses point-to-plane,
+// float64 accumulation, filters and the robust filter; the 2-D one a robust filter with float64 accumulation
 // (SFE_ERR_UNSUPPORTED).
-int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what);
+int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what,
+                     const sfe_icp_robust *robust = nullptr);
 // icp_run on [x, y, z] clouds (icp3.cuh; statement oracle/icp3_ref.c): guess and T_out are [P][16] row-major 4x4,
 // point-to-point with float32 sums only; no counts, classes or filters (icp_params_check).  The same launch split as
 // icp_run without classes: targets above icp_cta_limit(ctx, 3, ns) read map grids, sources above icp_source_limit take
 // the global-source class, with the same results.
 int icp3_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const IcpProblems &pb,
-             const sfe_icp_filters *filt = nullptr);
+             const sfe_icp_filters *filt = nullptr, const sfe_icp_robust *robust = nullptr);
 // *limit = the largest target of `dim` columns that icp_run (dim 2: shipped point-to-point chain, no filters) or
 // icp3_run (dim 3) solves in one CTA next to sources of ns points; larger targets take the map class
 int icp_cta_limit(const sfe_ctx *ctx, int dim, int ns, int *limit);
 // *limit = the largest source of `dim` columns that icp_run / icp3_run solve in their shared-memory layouts next to
-// targets of any size, for the settings prm and filt (may be null); larger sources take the global-source class
-int icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, int *limit);
+// targets of any size, for the settings prm, filt and robust (may be null); larger sources take the global-source class
+int icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, int *limit,
+                     const sfe_icp_robust *robust = nullptr);
 // nearest neighbour in reference cloud p of every point of input cloud p; no counts, in.n_max is not used; references
 // of any size (the map class above one CTA's limit)
 int match_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &ref, const PackedClouds &in, int P, float max_dist,

@@ -171,10 +171,11 @@ def match(ref_pts, ref_off, in_pts, in_off, n_ref_max, max_dist, knn=None, ctx=N
 
 
 def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, src_id=None, tgt_id=None, ctx=None,
-        filters=None):
+        filters=None, robust=None):
     """Batched ICP (include/sonarfe.h: sfe_icp_dev).  guess: [P,3,3] f32 cuda.  Returns dict of cuda tensors.
     filters: _lib.IcpFilters (sfe_icp_set_filters), default params.filters when params is a parsed _lib.IcpConfig;
-    its data filters (distance and octree) run on the device before the iterations.
+    its data filters (distance and octree) run on the device before the iterations.  robust: _lib.IcpRobust, the
+    RobustOutlierFilter (sfe_icp_set_robust), default params.robust likewise; 2-D clouds only.
 
     Targets of any size: problems whose target does not fit one CTA's shared memory next to the sources read it from a
     map grid built once per distinct target (tgt_id) in global memory, with the same results.  Sources of any size:
@@ -182,7 +183,7 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
     global-source class -- their per-point arrays in global memory, every target read from a map grid -- with the same
     results.
     [total,3] points (both clouds) with [P,4,4] guesses: the 3-D point-to-point chain (sfe_icp_dim_dev), which takes no
-    filters, point-to-plane or float64 accumulation."""
+    filters, robust filter, point-to-plane or float64 accumulation."""
     cols = [int(a.shape[1]) if a.dim() == 2 else 0 for a in (src_pts, tgt_pts)]
     dim = 3 if 3 in cols else 2
     if dim == 3 and cols != [3, 3]:
@@ -198,6 +199,7 @@ def icp(src_pts, src_off, tgt_pts, tgt_off, guess, ns_max, nt_max, params=None, 
     inl = torch.empty_like(iters)
     st = torch.empty_like(iters)
     _lib.set_icp_filters(ctx, _lib.icp_filters_of(prm, filters))
+    _lib.set_icp_robust(ctx, _lib.icp_robust_of(prm, robust))
     if dim == 3:
         _lib.check(ctx.lib.sfe_icp_dim_dev(ctx.handle, ctypes.byref(prm), _dp(src_pts), _dp(src_off), _dp(tgt_pts),
                                            _dp(tgt_off), _dp(src_id), _dp(tgt_id), P, 3, int(ns_max), int(nt_max),
@@ -218,13 +220,14 @@ def icp_cta_limit(dim, ns, ctx=None, device=0):
     return int(out[0])
 
 
-def icp_source_limit(dim, params=None, filters=None, ctx=None, device=0):
+def icp_source_limit(dim, params=None, filters=None, ctx=None, device=0, robust=None):
     """The largest source of `dim` columns icp() solves in its shared-memory layouts next to targets of any size, for
-    `params` (default _lib.IcpParams()) and `filters` (as icp() takes them) on this device (sfe_icp_source_limit).
-    Larger sources take the global-source class."""
+    `params` (default _lib.IcpParams()), `filters` and `robust` (as icp() takes them) on this device
+    (sfe_icp_source_limit).  Larger sources take the global-source class."""
     ctx = ctx or context(device)
     prm = params or _lib.IcpParams()
     _lib.set_icp_filters(ctx, _lib.icp_filters_of(prm, filters))
+    _lib.set_icp_robust(ctx, _lib.icp_robust_of(prm, robust))
     out = np.zeros(1, np.int32)
     _lib.check(ctx.lib.sfe_icp_source_limit(ctx.handle, ctypes.byref(prm), int(dim), _lib.ptr(out)),
                "sfe_icp_source_limit")

@@ -17,10 +17,11 @@ from . import _lib, _streams
 
 
 class FrontEnd:
-    def __init__(self, ctx, maps, max_frames, icp_filters=None, **overrides):
+    def __init__(self, ctx, maps, max_frames, icp_filters=None, icp_robust=None, **overrides):
         """overrides: any field of sfe_frontend_params (e.g. tau=..., window=3, cap_points=4096) or
         `icp=_lib.IcpParams(...)`.  icp_filters: _lib.IcpFilters of the scan match (sfe_frontend_set_icp_filters),
-        default icp.filters when `icp` is a parsed _lib.IcpConfig."""
+        default icp.filters when `icp` is a parsed _lib.IcpConfig; icp_robust: its _lib.IcpRobust
+        (sfe_frontend_set_icp_robust), default icp.robust likewise."""
         self.ctx, self.maps, self.lib = ctx, maps, ctx.lib
         p = _lib.FrontendParams()
         self.lib.sfe_frontend_params_default(ctypes.byref(p))
@@ -39,6 +40,9 @@ class FrontEnd:
         filters = _lib.icp_filters_of(overrides.get("icp"), icp_filters)
         if filters is not None:
             _lib.check(self.lib.sfe_frontend_set_icp_filters(h, ctypes.byref(filters)), "sfe_frontend_set_icp_filters")
+        robust = _lib.icp_robust_of(overrides.get("icp"), icp_robust)
+        if robust is not None:
+            _lib.check(self.lib.sfe_frontend_set_icp_robust(h, ctypes.byref(robust)), "sfe_frontend_set_icp_robust")
 
     def add_geometry(self, maps):
         """Register a further sonar geometry (sfe_frontend_add_geometry) and return its id; the creation maps are
