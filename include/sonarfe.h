@@ -34,7 +34,9 @@ extern "C" {
                                  sfe_icp_dim_host, sfe_icp_batch_dim_host, sfe_icp_cta_limit, sfe_icp_source_limit,
                                  SFE_ICP_DATA_OCTREE and SFE_ICP_DATA_VOXEL (new sfe_icp_data_filter kinds; both structs
                                  keep their sizes), sfe_ctx_set_grid_sms, sfe_ctx_occupancy, sfe_icp_robust with
-                                 sfe_icp_set_robust and sfe_frontend_set_icp_robust */
+                                 sfe_icp_set_robust and sfe_frontend_set_icp_robust, SFE_ICP_DATA_SAMPLING_NORMALS (a
+                                 new sfe_icp_data_filter kind; both structs keep their sizes) with
+                                 sfe_icp_sampling_normals_dev */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -289,7 +291,8 @@ typedef struct {
   int normals_knn;        /* point-to-plane only: the reference's normals, as a SurfaceNormalDataPointsFilter{knn}
                              in referenceDataPointsFilters would attach them (libpointmatcher default 5; 3..16):
                              smaller-eigenvalue direction of the covariance of each point's knn nearest reference
-                             points (itself included) */
+                             points (itself included).  With an SFE_ICP_DATA_SAMPLING_NORMALS reference filter (either
+                             minimizer): that filter's knn, the largest box (3..64), and its normals replace these */
 } sfe_icp_params;
 SFE_API void sfe_icp_params_default(sfe_icp_params *p);
 
@@ -374,7 +377,19 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  point order, each divided by (float)count).  A cloud whose numDivX * numDivY does not fit 32 bits
  *                  (or whose bounds are not finite) makes the call SFE_ERR_UNSUPPORTED after the filter stages and
  *                  before any ICP launch (the grid spans the cloud the filter receives, known on the device only;
- *                  the call waits for the stages to check).  A target the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
+ *                  the call waits for the stages to check).
+ *                  SFE_ICP_DATA_SAMPLING_NORMALS {dim, dist}: SamplingSurfaceNormalDataPointsFilter with samplingMethod
+ *                  = dim (1, or 0 for ratio 1) and maxBoxDim = dist (>= 0, +inf allowed); knn = sfe_icp_params.
+ *                  normals_knn (3..64).  Reference side only, and only as its last filter.  The cloud is split into
+ *                  boxes of at most knn points by median cuts (root bounds: the cloud's min and max; a range of more
+ *                  than knn points is cut on the axis of its bounds' larger extent, x on a tie, its first count -
+ *                  count / 2 points in (coordinate, index) order going left, the cut value being the next point's
+ *                  coordinate); a box whose own points span more than maxBoxDim on an axis is dropped; every other box
+ *                  gets the normal of its points in index order (the closed form of the knn normals above, over k
+ *                  points); samplingMethod 1 keeps its lowest-index point moved to the box's float32 centroid, 0 keeps
+ *                  all its points.  Kept points stay in index order, each with its box's normal, which point-to-plane
+ *                  then reads instead of computing normals.
+ *                  A target the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
  *                  SFE_ICP_NO_OUTLIER with a quantile filter (trim_ratio or median_factor) on, else SFE_ICP_NO_POINT.
  *   min_dist       MinDistOutlierFilter minDist (< 0: off): keep pairs with d^2 > minDist^2 (sfe_icp_params.flags
  *                  bit 0: d^2 > minDist, as for MaxDist)
@@ -382,11 +397,13 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  floor(n_finite * 0.5) of the ascending finite squared distances (no finite one: SFE_ICP_NO_OUTLIER)
  * Outlier weights are the product over the chain (with sfe_icp_params' MaxDist and TrimmedDist). */
 enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_DATA_OCTREE = 3, SFE_ICP_DATA_VOXEL = 4,
-       SFE_ICP_MAX_DATA_FILTERS = 4 };
+       SFE_ICP_DATA_SAMPLING_NORMALS = 5, SFE_ICP_MAX_DATA_FILTERS = 4 };
 typedef struct {
-  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST, SFE_ICP_DATA_OCTREE or SFE_ICP_DATA_VOXEL */
-  int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3; voxel: useCentroid, 1 */
-  float dist; /* distance filters: the distance; octree: maxSizeByNode; voxel: vSize */
+  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST, SFE_ICP_DATA_OCTREE, SFE_ICP_DATA_VOXEL or
+                 SFE_ICP_DATA_SAMPLING_NORMALS */
+  int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3; voxel: useCentroid, 1;
+                 sampling normals: samplingMethod, 0 or 1 */
+  float dist; /* distance filters: the distance; octree: maxSizeByNode; voxel: vSize; sampling normals: maxBoxDim */
 } sfe_icp_data_filter;
 typedef struct {
   float min_dist;
@@ -428,6 +445,13 @@ SFE_API int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit);
  * one CTA next to them (sfe_icp_cta_limit).  Settings the chain does not run are reported as by sfe_icp_dim_dev; dim
  * outside 2 .. 3 and null pointers are SFE_ERR_ARG. */
 SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit);
+/* The SFE_ICP_DATA_SAMPLING_NORMALS stage of an ICP call alone, on n_clouds 2-D clouds packed with CSR offsets (device
+ * memory; clouds of up to n_max points): cloud c's kept points, in index order, at out_pts_dev + 2 * c * n_max, their
+ * boxes' normals at the same place of out_nrm_dev, their number in out_count_dev[c].  knn 3..64, method 0 or 1,
+ * max_box >= 0 (+inf allowed).  Clouds of up to 4 096 points take one CTA each, larger ones the grid-wide path. */
+SFE_API int sfe_icp_sampling_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds,
+                                         int n_max, int knn, int method, float max_box, float *out_pts_dev,
+                                         float *out_nrm_dev, int32_t *out_count_dev);
 
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
  * the default).  Checked here: no NaN, kind and dim known, an octree's maxSizeByNode and a voxel filter's vSize finite and

@@ -153,6 +153,8 @@ _EXTRA_SIGNATURES = {
     "sfe_icp_batch_dim_host": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sfe_icp_cta_limit": [c_void_p, c_int, c_int, c_void_p],
+    "sfe_icp_sampling_normals_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                     c_void_p, c_void_p],
     "sfe_icp_source_limit": [c_void_p, c_void_p, c_int, c_void_p],
     "sfe_frontend_set_icp_filters": [c_void_p, c_void_p],
     "sfe_icp_set_robust": [c_void_p, c_void_p],
@@ -210,6 +212,8 @@ class IcpParams(ctypes.Structure):
 MAX_DIST, MIN_DIST = 1, 2  # SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST: the kinds of an IcpDataFilter
 OCTREE = 3                 # SFE_ICP_DATA_OCTREE: OctreeGridDataPointsFilter {dim samplingMethod, dist maxSizeByNode}
 VOXEL = 4                  # SFE_ICP_DATA_VOXEL: VoxelGridDataPointsFilter {dim useCentroid (1), dist vSize}
+SAMPLING_NORMALS = 5       # SFE_ICP_DATA_SAMPLING_NORMALS: SamplingSurfaceNormalDataPointsFilter {dim samplingMethod,
+                           # dist maxBoxDim}; its knn is IcpParams.normals_knn
 MAX_DATA_FILTERS = 4       # SFE_ICP_MAX_DATA_FILTERS per cloud
 
 

@@ -148,7 +148,9 @@ def match_knn(mat_ref, mat_in, knn, max_dist):
 _SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are implemented, plus its commented-out "
               "PointToPlaneErrorMinimizer with a SurfaceNormalDataPointsFilter on the reference, the Max/MinDist data "
               "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, the "
-              "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, the MinDist / MedianDist "
+              "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, the "
+              "SamplingSurfaceNormalDataPointsFilter as the last reference filter (knn 3..64, samplingMethod 1, or 0 "
+              "with ratio 1), the MinDist / MedianDist "
               "outlier filters and one RobustOutlierFilter with scaleEstimator none or fixed")
 _DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
 
@@ -211,6 +213,33 @@ def _voxel_filter(p):
         raise NotImplementedError(f"ICP yaml: {_VOXEL} useCentroid 0 (the voxel centre) is not implemented: its "
                                   "formula cannot be checked against upstream (1, the centroid, is)")
     return _lib.VOXEL, 1, sx
+
+
+_SAMPLING = "SamplingSurfaceNormalDataPointsFilter"
+SAMPLING_KNN_MAX = 64  # the largest box the device's sampling-normals stage takes
+
+
+def _sampling_filter(p):
+    """SamplingSurfaceNormalDataPointsFilter {knn, samplingMethod, ratio, maxBoxDim, keepNormals, ...} -> (knn,
+    (SAMPLING_NORMALS, samplingMethod, maxBoxDim), keepNormals).  Upstream defaults knn 7, samplingMethod 0, ratio 0.5,
+    maxBoxDim inf, keepNormals 1.  averageExistingDescriptors, keepDensities, keepEigenValues and keepEigenVectors have
+    no consumer here and are ignored."""
+    knn = p.get("knn", 7)
+    if isinstance(knn, bool) or int(knn) != knn or not 3 <= int(knn) <= SAMPLING_KNN_MAX:
+        raise NotImplementedError(f"ICP yaml: {_SAMPLING} knn {knn!r} (an integer, 3..{SAMPLING_KNN_MAX})")
+    method = p.get("samplingMethod", 0)
+    if method not in (0, 1) or isinstance(method, bool):
+        raise ValueError(f"ICP yaml: {_SAMPLING} samplingMethod {method!r} (0 random, 1 centroid)")
+    ratio = float(p.get("ratio", 0.5))
+    if not 0.0 < ratio <= 1.0:
+        raise ValueError(f"ICP yaml: {_SAMPLING} ratio {ratio} must lie in (0, 1]")
+    if method == 0 and ratio != 1.0:
+        raise NotImplementedError(f"ICP yaml: {_SAMPLING} samplingMethod 0 with ratio {ratio} (random sampling) is not "
+                                  "implemented: its result depends on a random generator (1, and 0 with ratio 1, are)")
+    box = float(p.get("maxBoxDim", float("inf")))
+    if math.isnan(box) or box < 0:
+        raise ValueError(f"ICP yaml: {_SAMPLING} maxBoxDim {box} must be non-negative")
+    return int(knn), (_lib.SAMPLING_NORMALS, int(method), box), bool(int(p.get("keepNormals", 1)))
 
 
 _RESAMPLERS = {_OCTREE: _octree_filter, _VOXEL: _voxel_filter}
@@ -279,14 +308,24 @@ def parse_icp_yaml(text):
         if name not in _DATA_FILTERS and name not in _RESAMPLERS:
             raise NotImplementedError(f"ICP yaml: reading filter {name} ({_SUPPORTED})")
         add_data_filter(reading, name, p, "reading")
-    have_normals = False
+    have_normals, normal_source = False, None
     for node in cfg.get("referenceDataPointsFilters") or []:
         name, p = one(node)
         if name in _DATA_FILTERS or name in _RESAMPLERS:
-            if have_normals:  # the normals would describe points the filter then removes
-                raise NotImplementedError(f"ICP yaml: {name} after SurfaceNormalDataPointsFilter ({_SUPPORTED}: the "
-                                          "data filters go before it)")
+            if normal_source:  # the normals would describe points the filter then removes
+                raise NotImplementedError(f"ICP yaml: {name} after {normal_source} ({_SUPPORTED}: the data filters go "
+                                          "before it)")
             add_data_filter(reference, name, p, "reference")
+            continue
+        if name in (_SAMPLING, "SurfaceNormalDataPointsFilter") and normal_source:
+            raise NotImplementedError(f"ICP yaml: {name} after {normal_source}: one source of normals per reference "
+                                      f"cloud ({_SUPPORTED})")
+        if name == _SAMPLING:
+            knn, f, keep = _sampling_filter(p)
+            if len(reference) == _lib.MAX_DATA_FILTERS:
+                raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} referenceDataPointsFilters")
+            reference.append((name,) + f)
+            prm.normals_knn, have_normals, normal_source = knn, keep, name
             continue
         # the one other reference filter: point-to-plane needs it, it attaches the "normals" descriptor
         if name != "SurfaceNormalDataPointsFilter" or float(p.get("epsilon", 0)) != 0:
@@ -296,7 +335,7 @@ def parse_icp_yaml(text):
         prm.normals_knn = int(p.get("knn", 5))
         if not 3 <= prm.normals_knn <= 16:
             raise NotImplementedError(f"ICP yaml: SurfaceNormalDataPointsFilter knn {prm.normals_knn} (3..16)")
-        have_normals = True
+        have_normals, normal_source = True, name
     name, p = one(cfg.get("matcher", "KDTreeMatcher"))
     if name != "KDTreeMatcher" or int(p.get("knn", 1)) != 1 or float(p.get("epsilon", 0)) != 0:
         raise NotImplementedError(f"ICP yaml: matcher {name} {p} ({_SUPPORTED})")

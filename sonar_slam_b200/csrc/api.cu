@@ -676,6 +676,31 @@ int sfe_icp_cta_limit(sfe_ctx *ctx, int dim, int ns, int32_t *limit) {
   return rc;
 }
 
+int sfe_icp_sampling_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int n_max,
+                                 int knn, int method, float max_box, float *out_pts_dev, float *out_nrm_dev,
+                                 int32_t *out_count_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_icp_sampling_normals_dev: null context");
+  SFE_REQUIRE(n_clouds >= 0 && n_max >= 0, "sfe_icp_sampling_normals_dev: negative sizes");
+  if (n_clouds == 0) return SFE_OK;
+  SFE_REQUIRE(pts_dev && off_dev && out_pts_dev && out_nrm_dev && out_count_dev,
+              "sfe_icp_sampling_normals_dev: null pointer");
+  sfe_icp_filters f = {-1.f, -1.f, 0, 1, {}, {}};
+  f.reference[0] = {SFE_ICP_DATA_SAMPLING_NORMALS, method, max_box};
+  sfe_icp_params prm;
+  sfe_icp_params_default(&prm);
+  prm.normals_knn = knn;
+  int rc = icp_params_check(&prm, 2, &f, "sfe_icp_sampling_normals_dev");
+  if (rc != SFE_OK) return rc;
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  size_t bytes;
+  if ((rc = sampling_normals_ws(n_clouds, n_max, knn, &bytes)) != SFE_OK) return rc;
+  const size_t off_bytes = (sizeof(int) * (size_t)(n_clouds + 1) + 255) & ~size_t(255);
+  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP_FILTER], off_bytes + bytes, ctx->stream)) != SFE_OK) return rc;
+  char *base = (char *)ctx->scratch[SCR_ICP_FILTER].ptr;
+  return sampling_normals_run(ctx, ctx->stream, {pts_dev, off_dev, nullptr, n_max}, n_clouds, knn, method, max_box,
+                              base + off_bytes, out_pts_dev, (int *)base, out_count_dev, (float2 *)out_nrm_dev);
+}
+
 int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit) {
   SFE_REQUIRE(dim == 2 || dim == 3, "sfe_icp_source_limit: points must have 2 or 3 columns (got %d)", dim);
   SFE_REQUIRE(ctx && prm && limit, "sfe_icp_source_limit: null pointer");

@@ -100,6 +100,7 @@ struct IcpBatch {
   // src_ws_stride in global memory
   unsigned char *src_ws;
   size_t src_ws_stride;  sfe_icp_robust robust;  // the ROBUST kernels only: the RobustOutlierFilter (last, so the other fields keep their offsets)
+  const float2 *given_nrm;  // the GNRM kernels only: the targets' normals, laid out as tgt_pts (after the fields above)
 };
 
 
@@ -717,6 +718,14 @@ __global__ void __launch_bounds__(ICP_THREADS) match_knn_map_kernel(const MatchB
 }
 
 // ---------------------------------------------------------------------------- host side
+constexpr int ICP_SN_KNN_MAX = 64;  // the largest box of a SamplingSurfaceNormalDataPointsFilter
+
+// Whether the reference chain of f (may be null) ends with a SamplingSurfaceNormalDataPointsFilter
+static bool icp_sampling_normals(const sfe_icp_filters *f) {
+  return f && f->n_reference > 0 && f->n_reference <= SFE_ICP_MAX_DATA_FILTERS &&
+         f->reference[f->n_reference - 1].kind == SFE_ICP_DATA_SAMPLING_NORMALS;
+}
+
 int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *filt, const char *what,
                      const sfe_icp_robust *robust) {
   if (dim == 3 && (prm->minimizer != 0 || (prm->flags & 2) || filt || robust)) {
@@ -738,9 +747,15 @@ int icp_params_check(const sfe_icp_params *prm, int dim, const sfe_icp_filters *
   }
   SFE_REQUIRE(prm->max_iterations >= 1, "%s: maxIterationCount must be >= 1", what);
   SFE_REQUIRE(prm->minimizer == 0 || prm->minimizer == 1, "%s: unknown error minimizer %d", what, prm->minimizer);
-  SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
-              "%s: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", what, prm->normals_knn,
-              GRID_KNN_MAX);
+  if (icp_sampling_normals(filt)) {
+    SFE_REQUIRE(prm->normals_knn >= 3 && prm->normals_knn <= ICP_SN_KNN_MAX,
+                "%s: SamplingSurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", what, prm->normals_knn,
+                ICP_SN_KNN_MAX);
+  } else {
+    SFE_REQUIRE(prm->minimizer == 0 || (prm->normals_knn >= 3 && prm->normals_knn <= GRID_KNN_MAX),
+                "%s: SurfaceNormalDataPointsFilter knn %d is not supported (3..%d)", what, prm->normals_knn,
+                GRID_KNN_MAX);
+  }
   SFE_REQUIRE(prm->smooth_length < ICP_HIST, "%s: smoothLength %d is not supported (at most %d)", what,
               prm->smooth_length, ICP_HIST - 1);
   SFE_REQUIRE(!std::isnan(prm->matcher_max_dist) && !std::isnan(prm->outlier_max_dist) &&
@@ -774,8 +789,17 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what) {
     for (int k = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
       const sfe_icp_data_filter &d = side ? f->reference[k] : f->reading[k];
       SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST || d.kind == SFE_ICP_DATA_OCTREE ||
-                      d.kind == SFE_ICP_DATA_VOXEL,
+                      d.kind == SFE_ICP_DATA_VOXEL || d.kind == SFE_ICP_DATA_SAMPLING_NORMALS,
                   "%s: unknown data filter kind %d", what, d.kind);
+      if (d.kind == SFE_ICP_DATA_SAMPLING_NORMALS) {
+        SFE_REQUIRE(side == 1 && k == f->n_reference - 1,
+                    "%s: SamplingSurfaceNormalDataPointsFilter is supported as the last reference filter only", what);
+        SFE_REQUIRE(d.dim == 0 || d.dim == 1,
+                    "%s: SamplingSurfaceNormalDataPointsFilter samplingMethod %d (0 with ratio 1, or 1)", what, d.dim);
+        SFE_REQUIRE(!std::isnan(d.dist) && d.dist >= 0.f,
+                    "%s: SamplingSurfaceNormalDataPointsFilter maxBoxDim %g (non-negative)", what, (double)d.dist);
+        continue;
+      }
       if (d.kind == SFE_ICP_DATA_VOXEL) {
         SFE_REQUIRE(d.dim == 1, "%s: VoxelGridDataPointsFilter useCentroid %d (only 1, the centroid, is supported)",
                     what, d.dim);
@@ -838,9 +862,13 @@ static int icp_threads(int ns_max) { return ns_max <= 640 ? 128 : (ns_max <= 153
 // the flags.  In-CTA class: 512-thread CTAs whose shared memory allows only one per SM get the full 128 registers;
 // dense (icp_run's classes): 128-thread CTAs held to 64 registers, so that layouts small enough for 8 CTAs per SM get
 // them (IcpClass::dense).  Map class: one instantiation per CTA size.  filt: sfe_icp_filters; robust: the
-// RobustOutlierFilter (FILT instantiations with ROBUST).
+// RobustOutlierFilter (FILT instantiations with ROBUST); gnrm: given normals (in-CTA GNRM instantiations).
 template <int THREADS, int MINB, bool MAP, bool GSRC = false>
-static const void *icp_kernel_of(bool plane, bool filt, bool robust) {
+static const void *icp_kernel_of(bool plane, bool filt, bool robust, bool gnrm = false) {
+  if constexpr (!MAP)
+    if (plane && gnrm)
+      return robust ? (const void *)icp_kernel<THREADS, MINB, true, false, true, false, true, true>
+                    : (const void *)icp_kernel<THREADS, MINB, true, false, true, false, false, true>;
   if (robust)
     return plane ? (const void *)icp_kernel<THREADS, MINB, true, MAP, true, GSRC, true>
                  : (const void *)icp_kernel<THREADS, MINB, false, MAP, true, GSRC, true>;
@@ -851,17 +879,18 @@ static const void *icp_kernel_of(bool plane, bool filt, bool robust) {
                : (const void *)icp_kernel<THREADS, MINB, false, MAP, false, GSRC>;
 }
 
-static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool robust, bool map) {
+static const void *icp_kernel_for(int threads, size_t smem, bool plane, bool dense, bool filt, bool robust, bool map,
+                                  bool gnrm) {
   if (map) {
     if (threads == 128) return icp_kernel_of<128, 7, true>(plane, filt, robust);
     if (threads == 256) return icp_kernel_of<256, 4, true>(plane, filt, robust);
     return icp_kernel_of<512, 1, true>(plane, filt, robust);
   }
-  if (threads == 128 && dense) return icp_kernel_of<128, 8, false>(plane, filt, robust);
-  if (threads == 128) return icp_kernel_of<128, 7, false>(plane, filt, robust);
-  if (threads == 256) return icp_kernel_of<256, 4, false>(plane, filt, robust);
-  if (smem <= 110 * 1024) return icp_kernel_of<512, 2, false>(plane, filt, robust);
-  return icp_kernel_of<512, 1, false>(plane, filt, robust);
+  if (threads == 128 && dense) return icp_kernel_of<128, 8, false>(plane, filt, robust, gnrm);
+  if (threads == 128) return icp_kernel_of<128, 7, false>(plane, filt, robust, gnrm);
+  if (threads == 256) return icp_kernel_of<256, 4, false>(plane, filt, robust, gnrm);
+  if (smem <= 110 * 1024) return icp_kernel_of<512, 2, false>(plane, filt, robust, gnrm);
+  return icp_kernel_of<512, 1, false>(plane, filt, robust, gnrm);
 }
 
 // The global-source class: sources above what the shared-memory layouts hold (icp_source_limit).  Each persistent CTA
@@ -886,10 +915,10 @@ enum { ICP_CTA = 0, ICP_MAP = 1, ICP_GSRC = 2 };
 
 // One dimension's kernels and layouts: icp_kernel's instantiations for the minimizer and the filters (dim 2), or the
 // icp3_body kernels (dim 3).  filt: sfe_icp_filters (icp_filters_on), or a robust filter; robust: the
-// RobustOutlierFilter.
+// RobustOutlierFilter; gnrm: point-to-plane reads the normals of a SamplingSurfaceNormalDataPointsFilter.
 struct IcpDim {
   int dim;
-  bool plane, filt, robust;
+  bool plane, filt, robust, gnrm;
   int threads(int cls, int ns) const { return dim == 3 ? ICP3_THREADS : cls == ICP_GSRC ? ICP_THREADS : icp_threads(ns); }
   // class cls's kernel for `threads`-thread CTAs with `smem` bytes of layout; dense: IcpClass::dense
   const void *kernel(int cls, int threads, size_t smem, bool dense = false) const {
@@ -898,7 +927,7 @@ struct IcpDim {
              : cls == ICP_MAP ? (const void *)icp3_map_kernel
                               : (const void *)icp3_gsrc_kernel;
     if (cls == ICP_GSRC) return icp_kernel_of<ICP_THREADS, 1, true, true>(plane, filt, robust);
-    return icp_kernel_for(threads, smem, plane, dense, filt, robust, cls == ICP_MAP);
+    return icp_kernel_for(threads, smem, plane, dense, filt, robust, cls == ICP_MAP, gnrm);
   }
   // shared memory class cls may take next to sources of ns points: the budget of the instantiation that runs the
   // largest of its layouts
@@ -1219,8 +1248,11 @@ static int icp_split_run(sfe_ctx *ctx, cudaStream_t st, const IcpDim &d, const I
   if (s.cta && (rc = icp_enqueue(ctx, st, L[ICP_CTA], base + side, next + ICP_CTA)) != SFE_OK) return rc;
   MapWs w{};
   if (grids) {
-    const int knn = d.plane ? std::min(std::max(b.prm.normals_knn, 1), GRID_KNN_MAX) : 0;
-    rc = map_build(ctx, st, pb.tgt, d.dim, pb.tgt_id, pb.P, grid_limit, slot_cap, true, (b.prm.flags & 2) == 0, knn, w);
+    const float2 *given = nullptr;
+    if constexpr (std::is_same_v<Batch, IcpBatch>) given = d.gnrm ? b.given_nrm : nullptr;
+    const int knn = d.plane && !given ? std::min(std::max(b.prm.normals_knn, 1), GRID_KNN_MAX) : 0;
+    rc = map_build(ctx, st, pb.tgt, d.dim, pb.tgt_id, pb.P, grid_limit, slot_cap, true, (b.prm.flags & 2) == 0, knn, w,
+                   given);
     if (rc != SFE_OK) return rc;
     if constexpr (std::is_same_v<Batch, Icp3Batch>) {
       float *zs = (float *)base, *zm = (float *)(base + z_bytes);
@@ -1252,7 +1284,8 @@ static bool icp_filters_on(const sfe_icp_filters *f) {
 // one voxel_filter_run call likewise; a cloud whose voxel index would overflow sets *vox_overflow.  Two passes over
 // the Carver: the first sizes the block, the second launches.
 static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_filter *f, int n, PackedClouds &c,
-                           const int *&id, int n_clouds, int P, Carver &cv, const int *&gate, int *vox_overflow) {
+                           const int *&id, int n_clouds, int P, Carver &cv, const int *&gate, int *vox_overflow,
+                           int knn = 0, const float2 **nrm_out = nullptr) {
   const int jobs = id && n_clouds > 0 ? n_clouds : P;
   const int n_max = c.n_max > 0 ? c.n_max : 1;
   const size_t pts_bytes = sizeof(float) * 2 * (size_t)jobs * n_max;
@@ -1261,7 +1294,19 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   int *cnt = (int *)cv.take(sizeof(int) * (size_t)jobs);
   int *raw = (int *)cv.take(sizeof(int) * (size_t)jobs);
   bool octree = false;
-  for (int k = 0; k < n; ++k) octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE || f[k].kind == SFE_ICP_DATA_VOXEL;
+  for (int k = 0; k < n; ++k)
+    octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE || f[k].kind == SFE_ICP_DATA_VOXEL ||
+             f[k].kind == SFE_ICP_DATA_SAMPLING_NORMALS;
+  // a sampling-normals stage (the chain's last): the normals it writes, laid out as the points, and its workspace
+  float2 *nrm = nullptr;
+  void *sn_ws = nullptr;
+  if (n > 0 && f[n - 1].kind == SFE_ICP_DATA_SAMPLING_NORMALS) {
+    size_t ws_bytes;
+    const int rc = sampling_normals_ws(jobs, n_max, knn, &ws_bytes);
+    if (rc != SFE_OK) return rc;
+    nrm = (float2 *)cv.take(sizeof(float2) * (size_t)jobs * n_max);
+    sn_ws = cv.take(ws_bytes);
+  }
   // octree and voxel chains: a second set of points and counts the stages alternate with, the down-sample's indices,
   // and the offsets and sizes later compaction passes write (the same offsets; the sizes are not the gate's)
   float *pts2 = nullptr;
@@ -1280,7 +1325,14 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   float *next_pts = pts;
   int *next_cnt = cnt;
   for (int k = 0, first = 1; k < n || first; first = 0) {
-    if (!first && f[k].kind == SFE_ICP_DATA_VOXEL) {
+    if (!first && f[k].kind == SFE_ICP_DATA_SAMPLING_NORMALS) {
+      const int rc = sampling_normals_run(ctx, st, cur, jobs, knn, f[k].dim, f[k].dist, sn_ws, next_pts, off, next_cnt,
+                                          nrm);
+      if (rc != SFE_OK) return rc;
+      icp_keep_too_large_kernel<<<std::min((jobs + 255) / 256, ctx->sm_count), 256, 0, st>>>(cur.cnt, jobs, n_max,
+                                                                                             next_cnt);
+      ++k;
+    } else if (!first && f[k].kind == SFE_ICP_DATA_VOXEL) {
       const int rc = voxel_filter_run(ctx, st, cur, jobs, f[k].dist, next_pts, off, next_cnt, vox_overflow);
       if (rc != SFE_OK) return rc;
       icp_keep_too_large_kernel<<<std::min((jobs + 255) / 256, ctx->sm_count), 256, 0, st>>>(cur.cnt, jobs, n_max,
@@ -1295,7 +1347,10 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
       ++k;
     } else {
       IcpDataFilters df{0, {}};
-      for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE && f[k].kind != SFE_ICP_DATA_VOXEL; ++k) df.f[df.n++] = f[k];
+      for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE && f[k].kind != SFE_ICP_DATA_VOXEL &&
+             f[k].kind != SFE_ICP_DATA_SAMPLING_NORMALS;
+           ++k)
+        df.f[df.n++] = f[k];
       icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
           {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
           first ? raw : raw2);
@@ -1310,6 +1365,7 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   c = cur;
   if (per_problem) id = nullptr;
   gate = raw;
+  if (nrm_out) *nrm_out = nrm;
   return SFE_OK;
 }
 }  // namespace sfe
@@ -1341,6 +1397,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   int rc = icp_params_check(prm, 2, filt, "icp", robust);
   if (rc != SFE_OK) return rc;
   const int *gate_src = nullptr, *gate_tgt = nullptr;
+  const float2 *given_nrm = nullptr;
   if (filt && (filt->n_reading > 0 || filt->n_reference > 0)) {
     bool voxel = false;
     for (int k = 0; k < filt->n_reading; ++k) voxel = voxel || filt->reading[k].kind == SFE_ICP_DATA_VOXEL;
@@ -1360,7 +1417,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
       }
       if (filt->n_reference > 0) {
         rc = icp_filter_side(ctx, st, filt->reference, filt->n_reference, q.tgt, q.tgt_id, q.n_tgt_clouds, q.P, cv,
-                             gate_tgt, vox_overflow);
+                             gate_tgt, vox_overflow, prm->normals_knn, &given_nrm);
         if (rc != SFE_OK) return rc;
         if (q.tgt_id != pb.tgt_id) q.n_tgt_clouds = q.P;  // one compacted target per problem
       }
@@ -1393,6 +1450,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
     b.gate_src_cnt = gate_src, b.gate_tgt_cnt = gate_tgt;
   }
   if (robust) b.robust = *robust;
+  b.given_nrm = prm->minimizer == 1 ? given_nrm : nullptr;
   b.src_pts = pb.src.pts, b.src_off = pb.src.off, b.tgt_pts = pb.tgt.pts, b.tgt_off = pb.tgt.off;
   b.src_cnt = pb.src.cnt, b.tgt_cnt = pb.tgt.cnt, b.min_points = pb.min_points;
   b.raw_cnt = pb.raw_cnt, b.raw_cap = pb.raw_cap;
@@ -1402,7 +1460,7 @@ int sfe::icp_run(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_params *prm, const
   b.box = ICP_BOX_ALL;
   b.cell_scale = 1.0f, b.prm = *prm;
   b.small_mult = ICP_SMALL_MULT, b.margin_mult = ICP_MARGIN_MULT;
-  const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr};
+  const IcpDim d{2, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr, b.given_nrm != nullptr};
   if (classes) return icp_run_classes(ctx, st, d, b, class_list, n_classes, ns_max, nt_max, class_of);
   IcpSplit s;
   if ((rc = icp_split(ctx, d, ns_max, nt_max, s)) != SFE_OK) return rc;
@@ -1425,7 +1483,8 @@ int sfe::icp_source_limit(const sfe_ctx *ctx, const sfe_icp_params *prm, int dim
   int rc = icp_params_check(prm, dim, filt, "icp_source_limit", robust);
   if (rc != SFE_OK) return rc;
   IcpSplit s;
-  const IcpDim d{dim, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr};
+  const IcpDim d{dim, prm->minimizer == 1, icp_filters_on(filt) || robust, robust != nullptr,
+                 prm->minimizer == 1 && icp_sampling_normals(filt)};
   if ((rc = icp_split(ctx, d, 1, 0, s)) == SFE_OK) *limit = s.S;
   return rc;
 }

@@ -14,10 +14,13 @@
 //          shared memory holds IcpShared and, PLANE, seq_sum9_warp's scratch;
 //   ROBUST: (FILT only) the batch runs a RobustOutlierFilter (b.robust): the keep pass (3c) multiplies the 0 / 1 weights
 //          by the robust weight and parks it in dist[], which is dead until the next search; the minimisers' sums
-//          weight their terms by it.  PLANE: seq_sum9_warp's scratch then gets its own 2.5 KB.
+//          weight their terms by it.  PLANE: seq_sum9_warp's scratch then gets its own 2.5 KB;
+//   GNRM:  (PLANE, FILT, in-CTA class only) the target's normals are given (b.given_nrm, laid out as the targets'
+//          points: a SamplingSurfaceNormalDataPointsFilter's) and gathered to the sorted positions instead of computed.
+//          The map classes need no instantiation of their own: map_build gathers them (MapArgs::nrm).
 // The body is written in the kernel itself: behind a device-function wrapper the shipped instantiations compiled with
 // larger stack frames.
-template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT, bool GSRC, bool ROBUST = false>
+template <int THREADS, int MINB, bool PLANE, bool MAP, bool FILT, bool GSRC, bool ROBUST = false, bool GNRM = false>
 __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, const MapArgs mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // layout: [IcpShared][sorted float2 nt_max][cells u32][reading float2 ns_max][dist f32 ns_max][match Pos ns_max]
@@ -28,6 +31,7 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
   static_assert(THREADS % 32 == 0 && THREADS >= 64 && THREADS <= 512, "icp_kernel: 2 to 16 warps per CTA");
   static_assert(MAP || !GSRC, "icp_kernel: the global-source class reads its targets as map grids");
   static_assert(FILT || !ROBUST, "icp_kernel: the robust filter runs in the FILT instantiations");
+  static_assert(!GNRM || (PLANE && FILT && !MAP), "icp_kernel: given normals are point-to-plane, FILT and in-CTA only");
   using Pos = std::conditional_t<MAP, int, uint16_t>;   // a target point's sorted position
   using Ord = std::conditional_t<GSRC, int, uint16_t>;  // a source point's index
   constexpr int NONE = MAP ? -1 : 0xffff;                // "no match"
@@ -220,6 +224,10 @@ __global__ void __launch_bounds__(THREADS, MINB) icp_kernel(const IcpBatch b, co
     float2 *nrm = nullptr;
     if constexpr (PLANE && MAP) {
       nrm = const_cast<float2 *>(mp.nrm);  // computed once per target by map_build
+    } else if constexpr (GNRM) {
+      nrm = b.nrm_ws + (size_t)slot * b.nt_max;
+      const float2 *given = b.given_nrm + b.tgt_off[ti];
+      for (int j = tid; j < nt; j += nthr) nrm[j] = given[orig[j]];
     } else if constexpr (PLANE) {
       nrm = b.nrm_ws + (size_t)slot * b.nt_max;
       const int knn = min(max(prm.normals_knn, 1), GRID_KNN_MAX);

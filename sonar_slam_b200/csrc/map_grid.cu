@@ -154,12 +154,22 @@ __global__ void map_normals_kernel(const unsigned long long *key, const MapArgs 
   nrm[i] = grid_surface_normal(g, i, knn, bd, bi, 1);
 }
 
+// point-to-plane with given normals (SamplingSurfaceNormalDataPointsFilter): the normal of every sorted position
+__global__ void map_given_normals_kernel(const unsigned long long *key, const PackedClouds t, const int *slot_tgt,
+                                         const int *orig, int N, const float2 *given, float2 *nrm) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const unsigned long long k = key[i];
+  if (k == ~0ull) return;
+  nrm[i] = given[t.off[slot_tgt[(int)(k >> 32)]] + orig[i]];
+}
+
 // Builds the map grids of the problems whose target has more than `limit` points.  slot_cap bounds the number of
 // distinct such targets.  Workspace (scratch[SCR_MAP]): 40 bytes per slot point (48 with normals) for slot_cap *
 // nt_max slot points, 4 * (1.5 nt_max + 257) bytes of cell table per slot, 28 bytes per problem, CUB's temporary
 // storage.  knn > 0: normals too.
 int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, const int *tgt_id, int P, int limit,
-              int slot_cap, bool center, bool seq, int knn, MapWs &w) {
+              int slot_cap, bool center, bool seq, int knn, MapWs &w, const float2 *given_nrm) {
   const int nt_max = t.n_max;
   const long long slots = (long long)slot_cap * nt_max;
   SFE_REQUIRE(slots < INT_MAX, "map grids: %d targets of up to %d points exceed %d slot points", slot_cap, nt_max,
@@ -205,7 +215,7 @@ int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, con
     v0 = (int *)cv.take(sizeof(int) * (size_t)N);
     v1 = (int *)cv.take(sizeof(int) * (size_t)N);
     w.pts = (float2 *)cv.take(sizeof(float2) * (size_t)N);
-    w.nrm = knn > 0 ? (float2 *)cv.take(sizeof(float2) * (size_t)N) : nullptr;
+    w.nrm = knn > 0 || given_nrm ? (float2 *)cv.take(sizeof(float2) * (size_t)N) : nullptr;
     w.cstart = (int *)cv.take(sizeof(int) * (size_t)slot_cap * w.cell_cap);
     temp = cv.take(temp_bytes);
     if (pass == 0) {
@@ -241,7 +251,11 @@ int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, con
                                                  w.cstart);
   SFE_CUDA(cudaGetLastError());
   ctx->launches += 9;  // six kernels, the two sorts and the scan counted once each
-  if (knn > 0) {
+  if (given_nrm) {
+    map_given_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), t, w.slot_tgt, w.orig, N, given_nrm, w.nrm);
+    SFE_CUDA(cudaGetLastError());
+    ctx->launches++;
+  } else if (knn > 0) {
     map_normals_kernel<<<nb, MAP_THREADS, 0, st>>>(keys.Current(), w.args(), N, knn, w.nrm);
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;

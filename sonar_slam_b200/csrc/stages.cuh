@@ -53,6 +53,13 @@ int downsample_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_
 // A cloud whose voxel index would not fit 32 bits sets *overflow (device) to 1.  Workspace: scratch[SCR_DS_GRID].
 int voxel_filter_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, float vsize, float *out_pts,
                      int *out_off, int *out_count, int *overflow);
+// SamplingSurfaceNormalDataPointsFilter {knn, samplingMethod `method` (0: every point, 1: one per box), maxBoxDim
+// `max_box`} on every 2-D cloud of `in` (statement oracle/sampling_normal_ref.c; clouds above in.n_max points are not
+// read): the kept points in index order at c * n_max of out_pts, their box's normal at the same place of out_nrm,
+// out_off[c] = c * n_max, out_count[c] their number.  ws: sampling_normals_ws(n_clouds, in.n_max, knn) bytes.
+int sampling_normals_ws(int n_clouds, int n_max, int knn, size_t *bytes);
+int sampling_normals_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int knn, int method,
+                         float max_box, void *ws, float *out_pts, int *out_off, int *out_count, float2 *out_nrm);
 // the largest cloud of `dim` columns (2 or 3) downsample_run's one-CTA kernel lays out in shared memory on this device
 int downsample_cta_limit(const sfe_ctx *ctx, int *limit, int dim);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,
@@ -149,9 +156,10 @@ struct MapWs {  // device pointers into scratch[SCR_MAP]
 // Map grids (map_grid.cu) of the clouds with more than `limit` points among those that P problems name (problem p:
 // cloud tgt_id[p], or p with tgt_id null); slot_cap bounds the number of distinct such clouds.  Points are read from
 // t.pts with a stride of `dim` floats (x, y first).  center: points centred on the cloud's mean (seq: icp_kernel's
-// sequential float32 sum, else a float64 sum); knn > 0: point-to-plane normals too.
+// sequential float32 sum, else a float64 sum); knn > 0: point-to-plane normals too; given_nrm (laid out as t.pts, 2-D):
+// those normals instead, gathered to the sorted positions.
 int map_build(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &t, int dim, const int *tgt_id, int P, int limit,
-              int slot_cap, bool center, bool seq, int knn, MapWs &w);
+              int slot_cap, bool center, bool seq, int knn, MapWs &w, const float2 *given_nrm = nullptr);
 
 // Measurement build (-DSFE_MAP_CLASS_ALL, tools/build_map_class_variant.sh): downsample_run, remove_outlier_run,
 // icp_run and match_run dispatch with a one-CTA limit of 0, so every non-empty cloud takes the large-cloud path and can
