@@ -36,7 +36,9 @@ extern "C" {
                                  keep their sizes), sfe_ctx_set_grid_sms, sfe_ctx_occupancy, sfe_icp_robust with
                                  sfe_icp_set_robust and sfe_frontend_set_icp_robust, SFE_ICP_DATA_SAMPLING_NORMALS (a
                                  new sfe_icp_data_filter kind; both structs keep their sizes) with
-                                 sfe_icp_sampling_normals_dev */
+                                 sfe_icp_sampling_normals_dev, SFE_ICP_DATA_NORMALS and SFE_ICP_DATA_SHADOW (new
+                                 sfe_icp_data_filter kinds, reading side; both structs keep their sizes) with
+                                 sfe_icp_surface_normals_dev */
 
 #if defined(__GNUC__)
 #define SFE_API __attribute__((visibility("default")))
@@ -389,6 +391,16 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  points); samplingMethod 1 keeps its lowest-index point moved to the box's float32 centroid, 0 keeps
  *                  all its points.  Kept points stay in index order, each with its box's normal, which point-to-plane
  *                  then reads instead of computing normals.
+ *                  SFE_ICP_DATA_NORMALS {dim}: SurfaceNormalDataPointsFilter with knn = dim (3..16) on the reading
+ *                  (reading side only, at most once per chain): every point gets the knn normal above, computed on the
+ *                  cloud this filter receives, centred on its mean (sequential float32 sum / n).  The points do not
+ *                  change.  Only distance filters and SFE_ICP_DATA_SHADOW may follow it; each survivor keeps its
+ *                  normal.  The normals are dropped after the reading chain.
+ *                  SFE_ICP_DATA_SHADOW {dist}: ShadowDataPointsFilter with eps = dist (finite, radians; reading side
+ *                  only, after an SFE_ICP_DATA_NORMALS): keeps a point p (as the filter receives it, in the reading's
+ *                  input frame) with normal n iff |n^ . p^| > sinf(eps), where v^ = v / sqrtf(v.v) when v.v > 0, else
+ *                  v, the dot nx * px + ny * py, all float32 and nothing contracted; sinf is the host C library's.
+ *                  It drops points whose surface runs along the line of sight from the sensor at the origin.
  *                  A target the filters empty is SFE_ICP_EMPTY_REF; a source they empty ends as an empty source does:
  *                  SFE_ICP_NO_OUTLIER with a quantile filter (trim_ratio or median_factor) on, else SFE_ICP_NO_POINT.
  *   min_dist       MinDistOutlierFilter minDist (< 0: off): keep pairs with d^2 > minDist^2 (sfe_icp_params.flags
@@ -397,13 +409,15 @@ SFE_API int sfe_icp_batch_host(sfe_ctx *ctx, const sfe_icp_params *prm, const fl
  *                  floor(n_finite * 0.5) of the ascending finite squared distances (no finite one: SFE_ICP_NO_OUTLIER)
  * Outlier weights are the product over the chain (with sfe_icp_params' MaxDist and TrimmedDist). */
 enum { SFE_ICP_DATA_MAX_DIST = 1, SFE_ICP_DATA_MIN_DIST = 2, SFE_ICP_DATA_OCTREE = 3, SFE_ICP_DATA_VOXEL = 4,
-       SFE_ICP_DATA_SAMPLING_NORMALS = 5, SFE_ICP_MAX_DATA_FILTERS = 4 };
+       SFE_ICP_DATA_SAMPLING_NORMALS = 5, SFE_ICP_DATA_NORMALS = 6, SFE_ICP_DATA_SHADOW = 7,
+       SFE_ICP_MAX_DATA_FILTERS = 4 };
 typedef struct {
-  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST, SFE_ICP_DATA_OCTREE, SFE_ICP_DATA_VOXEL or
-                 SFE_ICP_DATA_SAMPLING_NORMALS */
+  int kind;   /* SFE_ICP_DATA_MAX_DIST, SFE_ICP_DATA_MIN_DIST, SFE_ICP_DATA_OCTREE, SFE_ICP_DATA_VOXEL,
+                 SFE_ICP_DATA_SAMPLING_NORMALS, SFE_ICP_DATA_NORMALS or SFE_ICP_DATA_SHADOW */
   int dim;    /* distance filters: -1 radial, 0 x, 1 y; octree: the sampling method, 0, 2 or 3; voxel: useCentroid, 1;
-                 sampling normals: samplingMethod, 0 or 1 */
-  float dist; /* distance filters: the distance; octree: maxSizeByNode; voxel: vSize; sampling normals: maxBoxDim */
+                 sampling normals: samplingMethod, 0 or 1; normals: knn, 3..16; shadow: unused */
+  float dist; /* distance filters: the distance; octree: maxSizeByNode; voxel: vSize; sampling normals: maxBoxDim;
+                 normals: unused; shadow: eps (radians) */
 } sfe_icp_data_filter;
 typedef struct {
   float min_dist;
@@ -452,10 +466,18 @@ SFE_API int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int di
 SFE_API int sfe_icp_sampling_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds,
                                          int n_max, int knn, int method, float max_box, float *out_pts_dev,
                                          float *out_nrm_dev, int32_t *out_count_dev);
+/* The SFE_ICP_DATA_NORMALS stage alone: the knn normal (knn 3..16) of every point of n_clouds 2-D clouds packed with CSR
+ * offsets (device memory; clouds of up to n_max points; larger ones are not read), written in point order to
+ * out_nrm_dev, laid out as the points (cloud c's point i at 2 * (off_dev[c] + i)).  Clouds of up to 4 096 points take
+ * one CTA each with their grid in shared memory; larger ones are sorted into grids in global memory (sfe_icp_dev's map
+ * grid workspace). */
+SFE_API int sfe_icp_surface_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds,
+                                        int n_max, int knn, float *out_nrm_dev);
 
 /* The filters later sfe_icp_dev / _host / _batch_host and sfe_frontend_icp_dev calls on ctx apply (copied; NULL: none,
  * the default).  Checked here: no NaN, kind and dim known, an octree's maxSizeByNode and a voxel filter's vSize finite and
- * positive, counts in range; SFE_ERR_ARG leaves the setting as it was. */
+ * positive, counts in range, SFE_ICP_DATA_NORMALS and SFE_ICP_DATA_SHADOW on the reading only, SHADOW after a NORMALS
+ * with a finite eps, only distance filters and SHADOW after a NORMALS; SFE_ERR_ARG leaves the setting as it was. */
 SFE_API int sfe_icp_set_filters(sfe_ctx *ctx, const sfe_icp_filters *filters);
 
 /* libpointmatcher's RobustOutlierFilter with scaleEstimator none / fixed (scale 1) and point2point residuals: a soft

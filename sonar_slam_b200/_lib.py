@@ -155,6 +155,7 @@ _EXTRA_SIGNATURES = {
     "sfe_icp_cta_limit": [c_void_p, c_int, c_int, c_void_p],
     "sfe_icp_sampling_normals_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                      c_void_p, c_void_p],
+    "sfe_icp_surface_normals_dev": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "sfe_icp_source_limit": [c_void_p, c_void_p, c_int, c_void_p],
     "sfe_frontend_set_icp_filters": [c_void_p, c_void_p],
     "sfe_icp_set_robust": [c_void_p, c_void_p],
@@ -214,6 +215,8 @@ OCTREE = 3                 # SFE_ICP_DATA_OCTREE: OctreeGridDataPointsFilter {di
 VOXEL = 4                  # SFE_ICP_DATA_VOXEL: VoxelGridDataPointsFilter {dim useCentroid (1), dist vSize}
 SAMPLING_NORMALS = 5       # SFE_ICP_DATA_SAMPLING_NORMALS: SamplingSurfaceNormalDataPointsFilter {dim samplingMethod,
                            # dist maxBoxDim}; its knn is IcpParams.normals_knn
+NORMALS = 6                # SFE_ICP_DATA_NORMALS: SurfaceNormalDataPointsFilter on the reading {dim knn (3..16)}
+SHADOW = 7                 # SFE_ICP_DATA_SHADOW: ShadowDataPointsFilter on the reading {dist eps}, after a NORMALS
 MAX_DATA_FILTERS = 4       # SFE_ICP_MAX_DATA_FILTERS per cloud
 
 
@@ -229,7 +232,8 @@ class IcpFilters(ctypes.Structure):
     filters per cloud, run in their order.  reading / reference: sequences of (kind, dim, dist): kind MAX_DIST or
     MIN_DIST with dim -1 (radial), 0 (x) or 1 (y) and the distance; kind OCTREE with dim the samplingMethod (0 first
     point, 2 centroid, 3 medoid) and dist maxSizeByNode (finite, > 0); kind VOXEL with dim 1 (useCentroid) and dist
-    vSize (finite, > 0)."""
+    vSize (finite, > 0); kind SAMPLING_NORMALS (reference, last); on the reading, kind NORMALS with dim the knn (3..16)
+    and kind SHADOW with dist eps (finite), after a NORMALS that only distance filters and SHADOW follow."""
     _fields_ = [("min_dist", c_float), ("median_factor", c_float), ("n_reading", c_int), ("n_reference", c_int),
                 ("reading", IcpDataFilter * MAX_DATA_FILTERS), ("reference", IcpDataFilter * MAX_DATA_FILTERS)]
 

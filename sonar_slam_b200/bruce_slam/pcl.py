@@ -150,7 +150,8 @@ _SUPPORTED = ("the modules of the shipped bruce_slam/config/icp.yaml are impleme
               "filters, the OctreeGridDataPointsFilter with maxSizeByNode and samplingMethod 0, 2 or 3, the "
               "VoxelGridDataPointsFilter with vSizeX == vSizeY and useCentroid 1, the "
               "SamplingSurfaceNormalDataPointsFilter as the last reference filter (knn 3..64, samplingMethod 1, or 0 "
-              "with ratio 1), the MinDist / MedianDist "
+              "with ratio 1), a SurfaceNormalDataPointsFilter on the reading (knn 3..16) followed by distance filters "
+              "and ShadowDataPointsFilter, the MinDist / MedianDist "
               "outlier filters and one RobustOutlierFilter with scaleEstimator none or fixed")
 _DATA_FILTERS = {"MaxDistDataPointsFilter": ("maxDist", _lib.MAX_DIST), "MinDistDataPointsFilter": ("minDist", _lib.MIN_DIST)}
 
@@ -242,6 +243,31 @@ def _sampling_filter(p):
     return int(knn), (_lib.SAMPLING_NORMALS, int(method), box), bool(int(p.get("keepNormals", 1)))
 
 
+_NORMALS = "SurfaceNormalDataPointsFilter"
+_SHADOW = "ShadowDataPointsFilter"
+
+
+def _reading_normals_filter(p):
+    """SurfaceNormalDataPointsFilter {knn, epsilon, keepNormals, ...} on the reading -> (NORMALS, knn, 0.0), or None
+    with keepNormals 0 (nothing reads the normals then).  Upstream defaults knn 5, epsilon 0, keepNormals 1;
+    keepDensities, keepEigenValues, keepEigenVectors and keepMatchedIds have no consumer here and are ignored."""
+    knn = p.get("knn", 5)
+    if isinstance(knn, bool) or int(knn) != knn or not 3 <= int(knn) <= 16:
+        raise NotImplementedError(f"ICP yaml: reading {_NORMALS} knn {knn!r} (an integer, 3..16)")
+    if float(p.get("epsilon", 0)) != 0:
+        raise NotImplementedError(f"ICP yaml: reading {_NORMALS} epsilon {p['epsilon']} (approximate neighbours; 0 is "
+                                  "implemented)")
+    return (_lib.NORMALS, int(knn), 0.0) if int(p.get("keepNormals", 1)) else None
+
+
+def _shadow_filter(p):
+    """ShadowDataPointsFilter {eps} -> (SHADOW, 0, eps); upstream default 0.1 rad."""
+    eps = float(p.get("eps", 0.1))
+    if not math.isfinite(eps):
+        raise ValueError(f"ICP yaml: {_SHADOW} eps {eps} must be finite")
+    return _lib.SHADOW, 0, eps
+
+
 _RESAMPLERS = {_OCTREE: _octree_filter, _VOXEL: _voxel_filter}
 _ROBUST = "RobustOutlierFilter"
 
@@ -303,14 +329,40 @@ def parse_icp_yaml(text):
 
     prm = _lib.IcpConfig(outlier_max_dist=-1.0, trim_ratio=-1.0, max_iterations=40, smooth_length=0)
     reading, reference, outlier, robust = [], [], {}, None
+    reading_normals = False  # a reading SurfaceNormalDataPointsFilter that keeps its normals came before
     for node in cfg.get("readingDataPointsFilters") or []:
         name, p = one(node)
+        if name == _NORMALS:
+            if reading_normals:
+                raise NotImplementedError(f"ICP yaml: a second reading {_NORMALS} ({_SUPPORTED})")
+            f = _reading_normals_filter(p)
+            if f:  # (keepNormals 0: a no-op)
+                if len(reading) == _lib.MAX_DATA_FILTERS:
+                    raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} readingDataPointsFilters")
+                reading.append((name,) + f)
+                reading_normals = True
+            continue
+        if name == _SHADOW:
+            if not reading_normals:
+                # libpointmatcher: InvalidField when the cloud carries no normals descriptor
+                raise ValueError(f"ICP yaml: {_SHADOW} needs the reading's normals (InvalidField: no descriptor "
+                                 f"normals): put a {_NORMALS} with keepNormals 1 before it in readingDataPointsFilters")
+            f = _shadow_filter(p)
+            if len(reading) == _lib.MAX_DATA_FILTERS:
+                raise NotImplementedError(f"ICP yaml: more than {_lib.MAX_DATA_FILTERS} readingDataPointsFilters")
+            reading.append((name,) + f)
+            continue
         if name not in _DATA_FILTERS and name not in _RESAMPLERS:
             raise NotImplementedError(f"ICP yaml: reading filter {name} ({_SUPPORTED})")
+        if name in _RESAMPLERS and reading_normals:  # the normals would need down-sampling with the points
+            raise NotImplementedError(f"ICP yaml: reading filter {name} after {_NORMALS} ({_SUPPORTED}: only the "
+                                      f"distance filters and {_SHADOW} may follow it)")
         add_data_filter(reading, name, p, "reading")
     have_normals, normal_source = False, None
     for node in cfg.get("referenceDataPointsFilters") or []:
         name, p = one(node)
+        if name == _SHADOW:
+            raise NotImplementedError(f"ICP yaml: reference filter {_SHADOW} ({_SUPPORTED}: on the reading only)")
         if name in _DATA_FILTERS or name in _RESAMPLERS:
             if normal_source:  # the normals would describe points the filter then removes
                 raise NotImplementedError(f"ICP yaml: {name} after {normal_source} ({_SUPPORTED}: the data filters go "

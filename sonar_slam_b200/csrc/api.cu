@@ -701,6 +701,22 @@ int sfe_icp_sampling_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32
                               base + off_bytes, out_pts_dev, (int *)base, out_count_dev, (float2 *)out_nrm_dev);
 }
 
+int sfe_icp_surface_normals_dev(sfe_ctx *ctx, const float *pts_dev, const int32_t *off_dev, int n_clouds, int n_max,
+                                int knn, float *out_nrm_dev) {
+  SFE_REQUIRE(ctx != nullptr, "sfe_icp_surface_normals_dev: null context");
+  SFE_REQUIRE(n_clouds >= 0 && n_max >= 0, "sfe_icp_surface_normals_dev: negative sizes");
+  SFE_REQUIRE(knn >= 3 && knn <= GRID_KNN_MAX, "sfe_icp_surface_normals_dev: knn %d (3..%d)", knn, GRID_KNN_MAX);
+  if (n_clouds == 0 || n_max == 0) return SFE_OK;
+  SFE_REQUIRE(pts_dev && off_dev && out_nrm_dev, "sfe_icp_surface_normals_dev: null pointer");
+  SFE_CUDA(cudaSetDevice(ctx->device));
+  size_t bytes;
+  int rc = surface_normals_ws(n_clouds, n_max, &bytes);
+  if (rc != SFE_OK) return rc;
+  if ((rc = ensure(ctx, ctx->scratch[SCR_ICP_FILTER], bytes > 0 ? bytes : 1, ctx->stream)) != SFE_OK) return rc;
+  return surface_normals_run(ctx, ctx->stream, {pts_dev, off_dev, nullptr, n_max}, n_clouds, knn,
+                             ctx->scratch[SCR_ICP_FILTER].ptr, (float2 *)out_nrm_dev);
+}
+
 int sfe_icp_source_limit(sfe_ctx *ctx, const sfe_icp_params *prm, int dim, int32_t *limit) {
   SFE_REQUIRE(dim == 2 || dim == 3, "sfe_icp_source_limit: points must have 2 or 3 columns (got %d)", dim);
   SFE_REQUIRE(ctx && prm && limit, "sfe_icp_source_limit: null pointer");

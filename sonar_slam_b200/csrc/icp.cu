@@ -464,11 +464,35 @@ struct IcpDataFilters {
 };
 constexpr int ICP_DF_THREADS = 256;
 
-__device__ __forceinline__ bool icp_data_keep(const IcpDataFilters &df, float x, float y) {
+// ShadowDataPointsFilter: |n^ . p^| > sin_eps, v^ = v / sqrtf(v.v) when v.v > 0 else v (Eigen's normalized()), every
+// operation rounded on its own (oracle/shadow_ref.c)
+__device__ __forceinline__ bool icp_shadow_keep(float x, float y, float2 n, float sin_eps) {
+  const float nn = __fadd_rn(__fmul_rn(n.x, n.x), __fmul_rn(n.y, n.y));
+  const float pp = __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y));
+  if (nn > 0.f) {
+    const float l = __fsqrt_rn(nn);
+    n.x = __fdiv_rn(n.x, l), n.y = __fdiv_rn(n.y, l);
+  }
+  if (pp > 0.f) {
+    const float l = __fsqrt_rn(pp);
+    x = __fdiv_rn(x, l), y = __fdiv_rn(y, l);
+  }
+  return fabsf(__fadd_rn(__fmul_rn(n.x, x), __fmul_rn(n.y, y))) > sin_eps;
+}
+
+// NRM: the pass after a SurfaceNormalDataPointsFilter -- SFE_ICP_DATA_SHADOW entries (dist = sinf(eps), set on the host)
+// read the point's normal n
+template <bool NRM = false>
+__device__ __forceinline__ bool icp_data_keep(const IcpDataFilters &df, float x, float y, float2 n = {}) {
   bool keep = true;
   for (int k = 0; k < df.n; ++k) {
     const sfe_icp_data_filter &f = df.f[k];
     bool kk;
+    if constexpr (NRM)
+      if (f.kind == SFE_ICP_DATA_SHADOW) {
+        keep = keep && icp_shadow_keep(x, y, n, f.dist);
+        continue;
+      }
     if (f.dim < 0) {  // sqrtf of the unfused float32 x*x + y*y (oracle/icp_filters_ref.c)
       const float r = __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
       kk = f.kind == SFE_ICP_DATA_MAX_DIST ? r < fabsf(f.dist) : r > fabsf(f.dist);
@@ -488,10 +512,12 @@ __global__ void icp_keep_too_large_kernel(const int *in_cnt, int n_clouds, int n
     if (in_cnt[c] > n_max) out_cnt[c] = in_cnt[c];
 }
 
+// NRM: the pass after a SurfaceNormalDataPointsFilter, whose normals in_nrm are laid out as the points (in.off, no id)
+template <bool NRM>
 __global__ void __launch_bounds__(ICP_DF_THREADS) icp_data_filter_kernel(const PackedClouds in, const int *id,
                                                                          int n_clouds, const IcpDataFilters df,
                                                                          float *out_pts, int *out_off, int *out_cnt,
-                                                                         int *out_raw) {
+                                                                         int *out_raw, const float2 *in_nrm) {
   __shared__ int warp_n[ICP_DF_THREADS / 32];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int c = blockIdx.x; c < n_clouds; c += gridDim.x) {
@@ -509,7 +535,11 @@ __global__ void __launch_bounds__(ICP_DF_THREADS) icp_data_filter_kernel(const P
     for (int i0 = 0; i0 < n; i0 += ICP_DF_THREADS) {
       const int i = i0 + tid;
       float x = 0.f, y = 0.f;
-      const bool keep = i < n && (x = src[2 * i], y = src[2 * i + 1], icp_data_keep(df, x, y));
+      bool keep;
+      if constexpr (NRM)
+        keep = i < n && (x = src[2 * i], y = src[2 * i + 1], icp_data_keep<true>(df, x, y, in_nrm[in.off[ci] + i]));
+      else
+        keep = i < n && (x = src[2 * i], y = src[2 * i + 1], icp_data_keep(df, x, y));
       const unsigned m = __ballot_sync(0xffffffffu, keep);
       if (lane == 0) warp_n[warp] = __popc(m);
       __syncthreads();
@@ -786,11 +816,32 @@ int icp_filters_check(const sfe_icp_filters *f, const char *what) {
               "%s: %d reading / %d reference data filters (0..%d each)", what, f->n_reading, f->n_reference,
               SFE_ICP_MAX_DATA_FILTERS);
   for (int side = 0; side < 2; ++side)
-    for (int k = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
+    for (int k = 0, normals = 0; k < (side ? f->n_reference : f->n_reading); ++k) {
       const sfe_icp_data_filter &d = side ? f->reference[k] : f->reading[k];
       SFE_REQUIRE(d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST || d.kind == SFE_ICP_DATA_OCTREE ||
-                      d.kind == SFE_ICP_DATA_VOXEL || d.kind == SFE_ICP_DATA_SAMPLING_NORMALS,
+                      d.kind == SFE_ICP_DATA_VOXEL || d.kind == SFE_ICP_DATA_SAMPLING_NORMALS ||
+                      d.kind == SFE_ICP_DATA_NORMALS || d.kind == SFE_ICP_DATA_SHADOW,
                   "%s: unknown data filter kind %d", what, d.kind);
+      // a reading SurfaceNormalDataPointsFilter: only per-point filters after it (their normals travel with the points)
+      SFE_REQUIRE(!normals || d.kind == SFE_ICP_DATA_MAX_DIST || d.kind == SFE_ICP_DATA_MIN_DIST ||
+                      d.kind == SFE_ICP_DATA_SHADOW,
+                  "%s: data filter kind %d after the reading SurfaceNormalDataPointsFilter (only the distance filters "
+                  "and ShadowDataPointsFilter may follow it)", what, d.kind);
+      if (d.kind == SFE_ICP_DATA_NORMALS || d.kind == SFE_ICP_DATA_SHADOW) {
+        const char *name = d.kind == SFE_ICP_DATA_NORMALS ? "SurfaceNormalDataPointsFilter (SFE_ICP_DATA_NORMALS)"
+                                                          : "ShadowDataPointsFilter";
+        SFE_REQUIRE(side == 0, "%s: %s is supported on the reading cloud only", what, name);
+        if (d.kind == SFE_ICP_DATA_NORMALS) {
+          SFE_REQUIRE(d.dim >= 3 && d.dim <= GRID_KNN_MAX, "%s: reading SurfaceNormalDataPointsFilter knn %d (3..%d)",
+                      what, d.dim, GRID_KNN_MAX);
+          normals = 1;
+        } else {
+          SFE_REQUIRE(normals, "%s: ShadowDataPointsFilter needs the reading's normals: put a "
+                      "SurfaceNormalDataPointsFilter before it", what);
+          SFE_REQUIRE(std::isfinite(d.dist), "%s: ShadowDataPointsFilter eps %g (finite)", what, (double)d.dist);
+        }
+        continue;
+      }
       if (d.kind == SFE_ICP_DATA_SAMPLING_NORMALS) {
         SFE_REQUIRE(side == 1 && k == f->n_reference - 1,
                     "%s: SamplingSurfaceNormalDataPointsFilter is supported as the last reference filter only", what);
@@ -1296,7 +1347,25 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   bool octree = false;
   for (int k = 0; k < n; ++k)
     octree = octree || f[k].kind == SFE_ICP_DATA_OCTREE || f[k].kind == SFE_ICP_DATA_VOXEL ||
-             f[k].kind == SFE_ICP_DATA_SAMPLING_NORMALS;
+             f[k].kind == SFE_ICP_DATA_SAMPLING_NORMALS || f[k].kind == SFE_ICP_DATA_NORMALS;
+  // a reading SurfaceNormalDataPointsFilter whose normals a ShadowDataPointsFilter reads: the normals, laid out as the
+  // points, and the stage's workspace (a filter with no shadow after it changes nothing and does not run)
+  float2 *pnrm = nullptr;
+  void *pn_ws = nullptr;
+  int pn_at = -1;
+  for (int k = 0; k < n; ++k)
+    if (f[k].kind == SFE_ICP_DATA_NORMALS) pn_at = k;
+  if (pn_at >= 0) {
+    bool shadow = false;
+    for (int k = pn_at + 1; k < n; ++k) shadow = shadow || f[k].kind == SFE_ICP_DATA_SHADOW;
+    if (shadow) {
+      size_t ws_bytes;
+      const int rc = surface_normals_ws(jobs, n_max, &ws_bytes);
+      if (rc != SFE_OK) return rc;
+      pnrm = (float2 *)cv.take(sizeof(float2) * (size_t)jobs * n_max);
+      pn_ws = cv.take(ws_bytes);
+    }
+  }
   // a sampling-normals stage (the chain's last): the normals it writes, laid out as the points, and its workspace
   float2 *nrm = nullptr;
   void *sn_ws = nullptr;
@@ -1325,6 +1394,14 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
   float *next_pts = pts;
   int *next_cnt = cnt;
   for (int k = 0, first = 1; k < n || first; first = 0) {
+    if (!first && f[k].kind == SFE_ICP_DATA_NORMALS) {  // the points stay where they are
+      if (pnrm) {
+        const int rc = surface_normals_run(ctx, st, cur, jobs, f[k].dim, pn_ws, pnrm);
+        if (rc != SFE_OK) return rc;
+      }
+      ++k;
+      continue;
+    }
     if (!first && f[k].kind == SFE_ICP_DATA_SAMPLING_NORMALS) {
       const int rc = sampling_normals_run(ctx, st, cur, jobs, knn, f[k].dim, f[k].dist, sn_ws, next_pts, off, next_cnt,
                                           nrm);
@@ -1347,13 +1424,22 @@ static int icp_filter_side(sfe_ctx *ctx, cudaStream_t st, const sfe_icp_data_fil
       ++k;
     } else {
       IcpDataFilters df{0, {}};
+      const bool nrm = !first && k > pn_at && pn_at >= 0;  // after the reading normals: the per-point filters
       for (; k < n && f[k].kind != SFE_ICP_DATA_OCTREE && f[k].kind != SFE_ICP_DATA_VOXEL &&
-             f[k].kind != SFE_ICP_DATA_SAMPLING_NORMALS;
-           ++k)
+             f[k].kind != SFE_ICP_DATA_SAMPLING_NORMALS && f[k].kind != SFE_ICP_DATA_NORMALS;
+           ++k) {
         df.f[df.n++] = f[k];
-      icp_data_filter_kernel<<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
-          {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
-          first ? raw : raw2);
+        // the threshold as upstream computes it, once on the host: the C library's sinf, not the device's
+        if (f[k].kind == SFE_ICP_DATA_SHADOW) df.f[df.n - 1].dist = std::sin(f[k].dist);
+      }
+      if (nrm && pnrm)
+        icp_data_filter_kernel<true><<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
+            {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
+            first ? raw : raw2, pnrm);
+      else
+        icp_data_filter_kernel<false><<<std::min(jobs, ctx->sm_count * 8), ICP_DF_THREADS, 0, st>>>(
+            {cur.pts, cur.off, cur.cnt, n_max}, cur_id, jobs, df, next_pts, first ? off : off2, next_cnt,
+            first ? raw : raw2, nullptr);
     }
     SFE_CUDA(cudaGetLastError());
     ctx->launches++;

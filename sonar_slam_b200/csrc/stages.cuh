@@ -60,6 +60,13 @@ int voxel_filter_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int 
 int sampling_normals_ws(int n_clouds, int n_max, int knn, size_t *bytes);
 int sampling_normals_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int knn, int method,
                          float max_box, void *ws, float *out_pts, int *out_off, int *out_count, float2 *out_nrm);
+// SurfaceNormalDataPointsFilter {knn 3..16} on every 2-D cloud of `in` (statement oracle/shadow_ref.c; clouds above
+// in.n_max points are not read): the knn normal of point i of cloud c, computed on the cloud centred on its mean, at
+// out_nrm[in.off[c] + i].  Clouds of up to 4 096 points take one CTA each, larger ones map grids (map_build, in
+// scratch[SCR_MAP]).  ws: surface_normals_ws(n_clouds, in.n_max) bytes.
+int surface_normals_ws(int n_clouds, int n_max, size_t *bytes);
+int surface_normals_run(sfe_ctx *ctx, cudaStream_t st, const PackedClouds &in, int n_clouds, int knn, void *ws,
+                        float2 *out_nrm);
 // the largest cloud of `dim` columns (2 or 3) downsample_run's one-CTA kernel lays out in shared memory on this device
 int downsample_cta_limit(const sfe_ctx *ctx, int *limit, int dim);
 // n_split > 0: two launches by cloud size (front end), 0: clouds of any size (one-CTA kernel up to the device's limit,

@@ -234,6 +234,20 @@ def icp_source_limit(dim, params=None, filters=None, ctx=None, device=0, robust=
     return int(out[0])
 
 
+def surface_normals(pts, off, n_max, knn=5, ctx=None):
+    """libpointmatcher's SurfaceNormalDataPointsFilter normals of packed 2-D clouds (include/sonarfe.h:
+    sfe_icp_surface_normals_dev): pts [total,2] f32 cuda, off [n+1] int32 cuda (cloud c: rows off[c] .. off[c+1]),
+    n_max >= every cloud's size (larger clouds are not read and their rows stay zero).  Returns [total,2] f32 cuda:
+    every point's knn normal (3..16; ties to the lower index), in point order, computed on its cloud centred on the
+    cloud's mean -- the reading normals of an ICP call with a SurfaceNormalDataPointsFilter in its reading chain."""
+    ctx = ctx or context(pts.device)
+    pts, off = pts.contiguous(), off.contiguous()
+    out = torch.zeros_like(pts)
+    _lib.check(ctx.lib.sfe_icp_surface_normals_dev(ctx.handle, _dp(pts), _dp(off), off.numel() - 1, int(n_max),
+                                                   int(knn), _dp(out)), "sfe_icp_surface_normals_dev")
+    return out
+
+
 def mincovdet(samples, n, subsets, float32=False, ctx=None):
     """Batched MinCovDet(support_fraction=0.8) fits (include/sonarfe.h: sfe_mincovdet_dev; sonar_slam_b200/mcd.py).
 
